@@ -1,11 +1,13 @@
 #!/usr/bin/env python
-"""Benchmark of the ESAC hot path (esac.forward) on B200s.
+"""Benchmark of the ESAC hot path (esac.forward) on H100s.
 
 Metric (BASELINE.json): pose hypotheses scored per second at 640x480, 256 hypotheses x E experts.
 A step = one batch of IMAGES_PER_STEP synthetic images, each through one esac.forward call (sample -> score -> select ->
 refine), exactly as the reference's callers loop over a test set with batch size 1 (test_esac.py:137-205).
 
   python bench.py [--gpus N] [--steps K] [--warmup W]          this repository's CUDA path
+  python bench.py ... --dump-outputs DIR                       also writes the poses and experts of the last timed step
+                                                               (DIR/poses.npy, DIR/experts.npy) for output-by-output checks
   python bench.py --impl reference ...                         the reference's CPU path on the host cores: oracle/_ref (the
                                                                reference's own esac.cpp compiled against the cv2-backed OpenCV
                                                                stand-in), or the cv2 oracle port where _ref is not built
@@ -38,8 +40,8 @@ sys.path.insert(0, str(ROOT))
 METRIC = "pose hypotheses scored/sec (640x480, 256 hyp x E experts)"
 UNIT = "hypotheses/s"
 E_PER_GPU, HYPS_PER_EXPERT, H, W, SUB = 7, 256, 480, 640, 1
-N_SCENES = 6          # rotating inputs: 6 x 25.8 MB > 126 MB L2, so no forward finds its planes in L2
-IMAGES_PER_STEP = 32  # one step = 32 images: long enough (~45 ms) for the clock sampler to see every step
+N_SCENES = 6          # rotating inputs: 6 x 25.8 MB > 50 MB L2, so no forward finds its planes in L2
+IMAGES_PER_STEP = 32  # one step = 32 images: long enough for the 20 ms clock sampler to see every step
 
 
 def workload_config(n_gpus: int) -> dict:
@@ -61,7 +63,7 @@ def make_inputs(rank: int, n: int = N_SCENES):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -111,7 +113,7 @@ def measured_peak():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s)"
 
 
 # -------------------------------------------------------------------------------------------------
@@ -296,6 +298,7 @@ def main():
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-configs", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the poses and experts the last timed step computed")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -330,7 +333,8 @@ def main():
     h_assign = [torch.from_numpy(s.assign).pin_memory() for s in scenes]
     p_coords = [torch.from_numpy(s.coords) for s in scenes]     # ordinary (pageable) host tensors
     p_assign = [torch.from_numpy(s.assign) for s in scenes]
-    d_out = torch.zeros(4, 4, device=dev)
+    d_outs = torch.zeros(IMAGES_PER_STEP, 4, 4, device=dev)   # one pose per image of a step: the last step's stay readable
+    experts = [-1] * IMAGES_PER_STEP
     h_out = torch.zeros(4, 4).pin_memory()
     p_out = torch.zeros(4, 4)
     # input preparation, not a step: the first transfers out of freshly pinned pages run at a fraction of the steady PCIe rate
@@ -347,12 +351,15 @@ def main():
 
     def forward_once(i, mode: str):
         j = i % N_SCENES
-        co, asg, out = {"device": (d_coords, d_assign, d_out), "pinned": (h_coords, h_assign, h_out),
+        co, asg, out = {"device": (d_coords, d_assign, d_outs[i % IMAGES_PER_STEP]), "pinned": (h_coords, h_assign, h_out),
                         "pageable": (p_coords, p_assign, p_out)}[mode]
         if world == 1:
-            return esac.forward(co[j], asg[j], out, *params)
-        return sharded.forward_sharded(co[j], asg[j], out, params, expert_offset=rank * E_PER_GPU, hyp_offset=rank * M_local,
-                                       M_pad=M_local, device=local_rank)
+            e = esac.forward(co[j], asg[j], out, *params)
+        else:
+            e = sharded.forward_sharded(co[j], asg[j], out, params, expert_offset=rank * E_PER_GPU, hyp_offset=rank * M_local,
+                                        M_pad=M_local, device=local_rank)
+        if mode == "device":
+            experts[i % IMAGES_PER_STEP] = e
 
     def timed(mode: str, steps: int, warmup: int):
         k = 0
@@ -388,6 +395,12 @@ def main():
     sampler.start()
     ms, stages, launches, score_launches, last = timed("device", args.steps, args.warmup)
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        # the timed loop runs whole steps, so slot b holds image b of the last one
+        out_dir = Path(args.dump_outputs)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        np.save(out_dir / "poses.npy", d_outs.cpu().numpy().astype(np.float32))
+        np.save(out_dir / "experts.npy", np.asarray(experts, np.float64))
     ms_e2e, stages_e2e, _, _, _ = timed("pinned", args.steps, args.warmup)
     steps_pg = max(1, args.steps // 4)
     ms_pg, _, _, _, _ = timed("pageable", steps_pg, 1)
@@ -459,24 +472,17 @@ def main():
         alg_bytes = M_local * 12.0 * N  # per scoring launch on this rank
         t_score = stages["ms_score"] * 1e-3
         achieved = alg_bytes / t_score / 1e9 if t_score > 0 else 0.0
-        # the resource that actually binds the kernel: 3 MUFU ops per cell-hypothesis at 16 lanes/clk/SM (profiles/r01_pipes.txt)
+        # the resource that actually binds the kernel: 3 MUFU ops per cell-hypothesis at 16 lanes/clk/SM
         sm_count = ctx.device_info()["sm_count"]
-        mhz = (clocks or {}).get("sm_mhz") or 1965.0
+        mhz = (clocks or {}).get("sm_mhz") or 1980.0
         mufu_peak = sm_count * (16.0 / 3.0) * mhz * 1e6 / N  # hypotheses/s
-        on_chip = {"pipe": "MUFU (rsqrt, ex2, rcp per cell-hypothesis; 16 lanes/clk/SM measured)", "peak_hyps_per_s": mufu_peak,
+        on_chip = {"pipe": "MUFU (rsqrt, ex2, rcp per cell-hypothesis; 16 lanes/clk/SM)", "peak_hyps_per_s": mufu_peak,
                    "achieved_hyps_per_s": M_local / t_score if t_score > 0 else None,
                    "frac": (M_local / t_score) / mufu_peak if t_score > 0 else None}
-        traffic = None
-        tp = ROOT / "profiles" / "score_kernel_traffic.json"
-        if tp.exists():
-            try:
-                traffic = json.loads(tp.read_text()).get("dram_bytes_per_launch")
-            except Exception:
-                traffic = None
         h2d = int(scenes[0].coords.nbytes + scenes[0].assign.nbytes) * IMAGES_PER_STEP
         line = {"metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": ms / args.steps, "ms_per_forward": ms / n_fwd, "higher_is_better": True, "scaling": "weak",
-                "vs_baseline": None, "dtype": "f32 (scoring, f32x2 FFMA2) / f64 (P3P, refinement)", "data": "synthetic",
+                "vs_baseline": None, "dtype": "f32 (scoring) / f64 (P3P, refinement)", "data": "synthetic",
                 "config": workload_config(world), "clocks": clocks,
                 "e2e": {"value": e2e, "unit": UNIT, "ms_per_step": ms_e2e / args.steps, "ms_per_forward": ms_e2e / n_fwd,
                         "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": (132 if world == 1 else 80) * IMAGES_PER_STEP, "host_memory": "pinned"},
@@ -485,7 +491,7 @@ def main():
                 "gpu_launches": int(launches), "gpu_launches_per_forward": launches / n_fwd,
                 "batched_e2e": batched, "backward": bwd,
                 "roofline": {"kernel": "esacb200::score_kernel_tma<8>", "bound": "hbm", "achieved": achieved, "peak": peak,
-                             "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                             "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
                              "algorithmic_bytes_per_launch": alg_bytes, "ms_per_launch": t_score * 1e3,
                              "launches_timed": int(score_launches),
                              "hyps_per_s_kernel_only": M_local / t_score if t_score > 0 else None,
@@ -510,7 +516,7 @@ def main():
             try:
                 from oracle.build import c_score
                 sc = scenes[0]
-                esac.forward(d_coords[0], d_assign[0], d_out, *params)
+                esac.forward(d_coords[0], d_assign[0], d_outs[0], *params)
                 poses = ctx.hypotheses()["poses"]
                 n_c = min(M_local, max(256, 4 * cores))
                 idx_c = np.linspace(0, M_local - 1, n_c).astype(int)

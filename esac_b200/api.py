@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's `esac` extension module on top of libesac_b200.so.
 
 `forward` / `backward` keep the positional signatures of esac_forward / esac_backward
-(/root/reference/code/esac/esac.cpp:64-77, 213-230; bound at esac.cpp:513-516) so
+(code/esac/esac.cpp:64-77, 213-230; bound at esac.cpp:513-516) so
 train_esac.py:151-168 and test_esac.py:192-205 run unchanged with `import esac` resolving to the
 top-level `esac.py` shim of this repository.  Tensors may be CPU tensors (what the reference's
 callers pass) or CUDA tensors (no host round trip), or numpy arrays.

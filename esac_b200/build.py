@@ -1,4 +1,4 @@
-"""Builds libesac_b200.so (hand-written sm_100a CUDA + the C ABI) in-tree with nvcc.
+"""Builds libesac_b200.so (hand-written sm_90a CUDA for the H100 + the C ABI) in-tree with nvcc.
 
 No torch extension machinery: the library has a plain C ABI (include/esac_b200.h) and is loaded
 with ctypes, so the build is four nvcc compiles and one link.
@@ -20,12 +20,12 @@ SOURCES = ["score.cu", "hyp.cu", "refine.cu", "bwd.cu", "gating.cu", "reproj.cu"
 HEADERS = ["esac_internal.h", "esac_geom.cuh", "esac_rng.cuh", "esac_p3p_fast.cuh", "../../include/esac_b200.h",
            "../../include/esac_b200_testhooks.h"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-ccbin", "/usr/bin/g++", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3",
+FLAGS = ["-ccbin", "/usr/bin/g++", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3",
          "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 
 
 def _digest(paths) -> str:
-    """Content hash of the sources (mtimes do not survive the snapshot that carries the tree to the GPU box)."""
+    """Content hash of the sources (mtimes do not survive a copy of the tree)."""
     h = hashlib.sha256(" ".join(FLAGS).encode())
     for p in paths:
         h.update(Path(p).name.encode())

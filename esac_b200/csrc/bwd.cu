@@ -423,7 +423,7 @@ void launch_backward_losses(const BwdArgs& a, cudaStream_t st) {
     bwd_loss_kernel<<<1, 1024, 0, st>>>(a, x);
 }
 
-void launch_backward(const BwdArgs& a, int max_jobs, cudaStream_t st) {
+void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t st) {
     BwdAux x;
     x.hg = (HypGrad*)a.hyp_grad;
     x.red = a.red;
@@ -431,10 +431,10 @@ void launch_backward(const BwdArgs& a, int max_jobs, cudaStream_t st) {
     x.tiles = bwd_tiles(a.P.N);
     bwd_loss_kernel<<<1, 1024, 0, st>>>(a, x);
     long long items = (long long)max_jobs * x.tiles;
-    int grid = (int)(items < 148 * 8 ? items : 148 * 8);
+    int grid = (int)(items < sm_count * 8ll ? items : sm_count * 8ll);
     if (grid < 1) grid = 1;
     bwd_reduce_kernel<<<grid, kBwdThreads, 0, st>>>(a, x);
-    bwd_solve_kernel<<<max_jobs < 592 ? max_jobs : 592, 32, 0, st>>>(a, x);
+    bwd_solve_kernel<<<max_jobs < sm_count * 4 ? max_jobs : sm_count * 4, 32, 0, st>>>(a, x);
     bwd_maxjr_kernel<<<grid, kBwdThreads, 0, st>>>(a, x);
     dim3 ga((a.P.N + kBwdThreads - 1) / kBwdThreads, a.P.E);
     bwd_assemble_kernel<<<ga, kBwdThreads, 0, st>>>(a, x);

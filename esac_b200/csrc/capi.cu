@@ -433,13 +433,12 @@ int pick_group(esacb200_ctx* ctx, const Problem& P, int jobs_hint) {
     if (ctx->refine_group_opt > 0) return ctx->refine_group_opt < ctx->refine_coresident ? ctx->refine_group_opt : ctx->refine_coresident;
     const int words = (P.N + 31) / 32;
     // ~320 cells per CTA, up to every co-resident CTA: with the warp-parallel slot summation the inter-CTA barrier costs less
-    // than the fp64 work it spreads, at every shape measured (profiles/r01m_refine_groups.txt: 60x80 -> 16, 480x640 -> 148)
+    // than the fp64 work it spreads (60x80 -> 16 CTAs, 480x640 -> every co-resident CTA)
     int g = words / 10;
     if (g < 1) g = 1;
     // Jobs are handed out dynamically inside the kernel, so a group may work through several jobs: fewer, larger groups even
     // out the differing job lengths (rounds x LM iterations) -- worth it only while a block's share of the map stays large
-    // against the cost of a group exchange (480x640: 8.5 vs 11.2 ms for 47 jobs; 60x80: 0.79 vs 0.39 ms, so not there;
-    // profiles/r02e_refine_timing.txt)
+    // against the cost of a group exchange (480x640: yes; 60x80: no)
     int waves = jobs_hint >= 8 ? ctx->refine_jobs_per_group : 1;
     int concurrent = jobs_hint > 0 ? (jobs_hint + waves - 1) / waves : 1;
     int cap = ctx->refine_coresident / concurrent;
@@ -1190,7 +1189,7 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
         b.expected_override = ctx->stats.as<double>() + 7;
         ctx->st.kernel_launches += 2;
     }
-    launch_backward(b, M, ctx->stream);
+    launch_backward(b, M, ctx->sm_count, ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 5;
     if (reduce_grads) {

@@ -117,6 +117,16 @@ ESAC_HD void rodrigues_m2v(const double R[9], double r[3]) {
 #define ESAC_ADD(a, b) ((a) + (b))
 #endif
 
+// Two fp32 values side by side (float2), one IEEE round-to-nearest operation per lane.  The _rn intrinsics keep the
+// compiler from contracting a product into a following sum, so every lane rounds exactly where the code says.
+#ifdef __CUDACC__
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
+    return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+#endif
+
 ESAC_HD void transform_point(const double R[9], const double t[3], double X, double Y, double Z,
                              double& x, double& y, double& z) {
     x = ESAC_ADD(ESAC_ADD(ESAC_ADD(ESAC_MUL(R[0], X), ESAC_MUL(R[1], Y)), ESAC_MUL(R[2], Z)), t[0]);

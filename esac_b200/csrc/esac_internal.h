@@ -51,7 +51,7 @@ struct ChunkDesc {
 };
 
 // Folded fp32 pose for the scoring kernel: rows [A_r0 A_r1 A_r2 | b_r] of diag(f,f,1)*R and
-// diag(f,f,1)*(R*c + t); FFMA2 broadcasts a scalar register operand to both f32x2 lanes.
+// diag(f,f,1)*(R*c + t).
 struct PosePk {
     float4 v[3];
 };
@@ -202,7 +202,7 @@ struct BwdArgs {
     Problem P;
     const double* expected_override;  // device scalar: global expected loss (multi-GPU), or null
 };
-void launch_backward(const BwdArgs& a, int max_jobs, cudaStream_t st);
+void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t st);
 // phase split for the multi-GPU path: losses + local expectation only / everything after the loss exchange
 void launch_backward_losses(const BwdArgs& a, cudaStream_t st);
 void launch_add_inplace(float* dst, const float* src, size_t n, cudaStream_t st);

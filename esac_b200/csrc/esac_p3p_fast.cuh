@@ -6,10 +6,9 @@
 // (3-way selects instead), reciprocal / rsqrt approximations, and NO data-dependent branch: every "this try certainly
 // fails" / "this try goes to the exact path" exit of the straightforward formulation is a lane mask that latches the
 // verdict, and the arithmetic simply runs on (garbage in decided lanes is harmless).  That is what lets one thread
-// judge TWO tries at once on the packed f32x2 pipe (Pack2: FFMA2 / FMUL2 / FADD2 carry both tries in one issue slot --
-// the prefilter is issue-bound, profiles/r01n_prefilter_kernel_ncu.txt); Pack1 is the same code on one try (tail
-// kernel, host test hooks).  Every decision that is numerically borderline returns "may pass", i.e. hands the try to
-// the exact fp64 path; the invariant "an accepted try is never rejected here" is what
+// judge TWO tries at once (Pack2: two independent dependency chains side by side in a float2); Pack1 is the same code
+// on one try (tail kernel, host test hooks).  Every decision that is numerically borderline returns "may pass", i.e.
+// hands the try to the exact fp64 path; the invariant "an accepted try is never rejected here" is what
 // tests/test_host_geom.py::test_float_prefilter_never_rejects_an_accepted_try checks, for both packings.
 #pragma once
 #include "esac_geom.cuh"
@@ -48,10 +47,10 @@ ESAC_HD Pack1 operator*(Pack1 x, Pack1 y) { return bc1(x.a * y.a); }
 ESAC_HD Pack1 operator-(Pack1 x) { return bc1(-x.a); }
 ESAC_HD Pack1 fma_(Pack1 x, Pack1 y, Pack1 z) { return bc1(fmaf(x.a, y.a, z.a)); }
 #ifdef __CUDA_ARCH__
-ESAC_HD Pack2 operator+(Pack2 x, Pack2 y) { Pack2 r; r.v = __fadd2_rn(x.v, y.v); return r; }
-ESAC_HD Pack2 operator*(Pack2 x, Pack2 y) { Pack2 r; r.v = __fmul2_rn(x.v, y.v); return r; }
-ESAC_HD Pack2 fma_(Pack2 x, Pack2 y, Pack2 z) { Pack2 r; r.v = __ffma2_rn(x.v, y.v, z.v); return r; }
-ESAC_HD Pack2 operator-(Pack2 x, Pack2 y) { Pack2 r; r.v = __ffma2_rn(make_float2(-1.f, -1.f), y.v, x.v); return r; }  // exact: x - y
+ESAC_HD Pack2 operator+(Pack2 x, Pack2 y) { Pack2 r; r.v = fadd2(x.v, y.v); return r; }
+ESAC_HD Pack2 operator*(Pack2 x, Pack2 y) { Pack2 r; r.v = fmul2(x.v, y.v); return r; }
+ESAC_HD Pack2 fma_(Pack2 x, Pack2 y, Pack2 z) { Pack2 r; r.v = ffma2(x.v, y.v, z.v); return r; }
+ESAC_HD Pack2 operator-(Pack2 x, Pack2 y) { Pack2 r; r.v = ffma2(make_float2(-1.f, -1.f), y.v, x.v); return r; }  // exact: x - y
 #else
 ESAC_HD Pack2 operator+(Pack2 x, Pack2 y) { Pack2 r; r.v = make_float2(x.v.x + y.v.x, x.v.y + y.v.y); return r; }
 ESAC_HD Pack2 operator*(Pack2 x, Pack2 y) { Pack2 r; r.v = make_float2(x.v.x * y.v.x, x.v.y * y.v.y); return r; }
@@ -358,7 +357,7 @@ ESAC_HD bool p3p_may_pass_fast(const float obj[4][3], const float img[4][2], flo
     return p3p_may_pass_pack<Pack1>(o, im, f, ppx, ppy, tau, margin, needle).a;
 }
 
-// two tries on the packed f32x2 pipe: verdicts in pass0 / pass1
+// two tries side by side: verdicts in pass0 / pass1
 ESAC_HD void p3p_may_pass_fast2(const float obj0[4][3], const float img0[4][2], const float obj1[4][3], const float img1[4][2], float f,
                                 float ppx, float ppy, float tau, bool& pass0, bool& pass1, float margin = kPrefilterMargin,
                                 float needle = kPrefilterNeedle) {

@@ -9,7 +9,7 @@
 //   wave r (try window [base_h, base_h + span_r) of every unresolved hypothesis; span_0 = 256, then chosen on the
 //   device from the acceptance rate seen so far, ~1.25 / p, so that ~70% of the remaining hypotheses resolve per
 //   wave and < 2x the necessary tries are evaluated):
-//     prefilter_kernel   two tries per thread on the packed f32x2 pipe, fp32 only, branch-free: discards tries whose
+//     prefilter_kernel   two tries per thread (float2 pairs), fp32 only, branch-free: discards tries whose
 //                        every P3P root misses the 4th point by > 2 tau (>96% on wrong experts); the gathers of a
 //                        CTA's next 256-try item are in flight under the math of the current one; survivors are
 //                        appended to a global list
@@ -22,8 +22,7 @@
 //   emit_kernel          one thread per hypothesis: re-derives the winning (or, when exhausted, the last) try and
 //                        writes pose / cells / try count
 //
-// Keeping the float and double paths in different kernels matters: fused, the kernel ran at 10% issue utilisation,
-// stalled on instruction fetch (profiles/r01b_sample_kernel_ncu.json).
+// Keeping the float and double paths in different kernels matters: fused, the kernel stalls on instruction fetch.
 #include "esac_internal.h"
 #include "esac_p3p_fast.cuh"
 #include "esac_rng.cuh"
@@ -136,7 +135,7 @@ __global__ void sample_init_kernel(const __grid_constant__ SampleArgs a) {
     }
 }
 
-// ---- wave phase 1: fp32 prefilter, TWO tries per thread on the packed f32x2 pipe -----------------------------------
+// ---- wave phase 1: fp32 prefilter, TWO tries per thread (float2 pairs) ---------------------------------------------
 constexpr int kPackTries = 2 * kTryThreads;  // tries per CTA pass: thread i judges tries i and i + 128 of the 256-try chunk
 // One work item of the prefilter: 256 consecutive tries of one hypothesis, two per thread.
 struct PreItem {
@@ -180,14 +179,12 @@ __device__ __forceinline__ void prefilter_issue(const SampleArgs& a, long long i
     }
 }
 
-// ---- wave phase 1: fp32 prefilter, TWO tries per thread on the packed f32x2 pipe, gathers one item ahead ---------------
+// ---- wave phase 1: fp32 prefilter, TWO tries per thread (float2 pairs), gathers one item ahead ----------------------
 // The math of an item (~2700 instructions per thread, branch-free) runs while the 8 random 16-byte gathers of the NEXT item
-// are in flight: with 16-20 warps per SM (the two-try pack needs ~128 registers) nothing else would cover their L2 latency
-// (ncu before: long_scoreboard 1.9 of the 6.2 stall cycles per issued instruction at 47 % issue utilisation).
-// What it did NOT buy (profiles/r02o_prefilter_*.txt): the stage's time.  One 3.67 M-try launch takes 266 us against 277 us for
-// the one-try-per-thread kernel it replaces, although a try now costs 1336 instead of 2024 issue slots: both versions hold 1024
-// tries per SM in flight (64 registers per try) and a try's dependent instruction chain is as long as before, so the issue
-// slots saved turn into idle ones (issue utilisation 70 % -> 50 %).  96 registers (5 CTAs per SM) spill and run slower.
+// are in flight: with 16-20 warps per SM (the two-try pack needs ~128 registers) nothing else would cover their L2 latency.
+// The stage is bound by register capacity x dependency-chain latency: an SM holds 1024 tries in flight (64 registers per
+// try) whatever the packing, and a try's dependent instruction chain is the same.  96 registers
+// (5 CTAs per SM) spill.
 __global__ void __launch_bounds__(kTryThreads, 4) prefilter_kernel(const __grid_constant__ SampleArgs a) {
     TraceScope trace(a.trace, a.trace_slot);
     __shared__ float4 s_obj[2][8][kTryThreads];  // [buffer][try * 4 + point][thread]
@@ -402,7 +399,7 @@ __global__ void __launch_bounds__(64) emit_kernel(const __grid_constant__ Sample
 // instead of leaving the GPU idle.  Lanes are dealt by hypothesis parity, or -- when the coordinate maps are still
 // arriving from the host in two halves (split_e > 0) -- by expert: lane 0 = experts [0, split_e), released by
 // ev_half[0]; lane 1 = the rest, released by ev_half[1], so lane 0 samples while the second half is on the wire.
-// What was tried on top of this and measured slower or equal (profiles/r02h_*.txt, DESIGN.md section 8): 3-4 lanes, one
+// What was tried on top of this and measured slower or equal (DESIGN.md section 8): 3-4 lanes, one
 // prefilter stream + per-lane verdict streams in forced anti-phase, other window policies, a single persistent kernel with
 // work / survivor queues, programmatic dependent launch between the kernels of a lane (the ~4 us gaps close, but the early
 // CTAs of one lane starve the other).  option sample_trace shows who runs when.
@@ -449,7 +446,7 @@ int launch_sample(const float* coords, float4* coords4, const int* assign32, con
         if (bound[g] <= 0) continue;
         sample_init_kernel<<<(bound[g] + 255) / 256, 256, 0, sg>>>(a); ++launches;
         // persistent: every CTA resident (4 x 128 threads x 128 registers fill an SM's register file), ~14 items each in a bulk wave;
-        // 3 CTAs per SM + 64-thread verdict CTAs in the room that leaves was measured slower (profiles/r02o_sample_room_for_verdicts.txt)
+        // 3 CTAs per SM + 64-thread verdict CTAs in the room that leaves was measured slower
         const int grid = sm_count * 4;
         for (int r = 0; r < n_waves; ++r) {
             a.trace_slot = (g * 32 + r) * 2;

@@ -21,8 +21,8 @@
 //   -> every CTA sums its share of the cells (warp shuffle -> shared memory) and publishes 29 block totals in its slot,
 //   raising its own epoch flag with a release store -> the root waits for the flags, sums the slots in a fixed order, maps
 //   the sums to (rvec, tvec), accepts / rejects, solves for the next step.  Gather + broadcast instead of all-to-all: with
-//   148 CTAs polling each other's flags and each re-reading all 148 slots, L2 same-line contention cost 20 of the 39
-//   kilocycles an evaluation took (profiles/r02c_refine_profile.txt).  Jobs are drawn from a counter by the roots.
+//   every CTA polling every other CTA's flag and re-reading every slot, L2 same-line contention grows with the group size
+//   and dominates an evaluation.  Jobs are drawn from a counter by the roots.
 #include <cooperative_groups.h>
 
 #include "esac_internal.h"
@@ -34,7 +34,7 @@ constexpr int kRefWarps = kRefThreads / 32;
 constexpr int kRedN = 28;   // 21 (J^T J upper) + 6 (J^T r) + 1 (cost)
 constexpr int kSlot = 32;   // doubles per CTA slot / per command record
 // A CTA whose share of the map is at most this many 32-cell words keeps its cells in shared memory for the whole job (the
-// coordinates never change between evaluations): 96 words = 3072 cells = 36 KB.  Forward at 480x640 on 148 CTAs: 65 words.
+// coordinates never change between evaluations): 96 words = 3072 cells = 36 KB.  Forward at 480x640 on 132 CTAs: 73 words.
 constexpr int kCacheWords = 96;
 constexpr int kCacheCells = kCacheWords * 32;
 // Inlier compaction: after the pass that selects a round's inliers every CTA lists the inlier cells of its share (16-bit

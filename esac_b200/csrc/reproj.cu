@@ -84,9 +84,8 @@ __device__ __forceinline__ CellOut reproj_cell(float X, float Y, float Z, const 
     return o;
 }
 
-// Two cells at once on the packed f32x2 pipe (FFMA2 / FMUL2: one issue slot, two IEEE fp32 results -- bitwise what
-// reproj_cell computes for each).  Halves the FMA-pipe instruction count, which is what keeps this kernel from being
-// issue-bound below the HBM roofline.
+// Two cells at once as float2 pairs (two IEEE fp32 results per operation -- bitwise what
+// reproj_cell computes for each): two independent dependency chains per thread for the scheduler to interleave.
 struct PairConst {
     float2 m[12];            // world->camera entries, broadcast
     float2 f, cx, cy, cut, half_cut, inv_n;
@@ -97,40 +96,40 @@ __device__ __forceinline__ float2 bc(float v) { return make_float2(v, v); }
 __device__ __forceinline__ float2 neg2(float2 v) { return make_float2(-v.x, -v.y); }
 
 __device__ __forceinline__ PairOut reproj_pair(float2 X, float2 Y, float2 Z, const PairConst& k, float2 tx, float2 ty) {
-    const float2 xc = __ffma2_rn(k.m[0], X, __ffma2_rn(k.m[1], Y, __ffma2_rn(k.m[2], Z, k.m[3])));
-    const float2 yc = __ffma2_rn(k.m[4], X, __ffma2_rn(k.m[5], Y, __ffma2_rn(k.m[6], Z, k.m[7])));
-    const float2 zc = __ffma2_rn(k.m[8], X, __ffma2_rn(k.m[9], Y, __ffma2_rn(k.m[10], Z, k.m[11])));
-    const float2 nu = __ffma2_rn(k.f, xc, __fmul2_rn(k.cx, zc));
-    const float2 nv = __ffma2_rn(k.f, yc, __fmul2_rn(k.cy, zc));
+    const float2 xc = ffma2(k.m[0], X, ffma2(k.m[1], Y, ffma2(k.m[2], Z, k.m[3])));
+    const float2 yc = ffma2(k.m[4], X, ffma2(k.m[5], Y, ffma2(k.m[6], Z, k.m[7])));
+    const float2 zc = ffma2(k.m[8], X, ffma2(k.m[9], Y, ffma2(k.m[10], Z, k.m[11])));
+    const float2 nu = ffma2(k.f, xc, fmul2(k.cx, zc));
+    const float2 nv = ffma2(k.f, yc, fmul2(k.cy, zc));
     const bool open0 = zc.x >= k.min_depth, open1 = zc.y >= k.min_depth;
     const float2 zz = make_float2(open0 ? zc.x : k.min_depth, open1 ? zc.y : k.min_depth);
     const float2 iz = make_float2(rcp_fast(zz.x), rcp_fast(zz.y));
-    const float2 du = __fmul2_rn(__ffma2_rn(neg2(tx), zz, nu), iz);
-    const float2 dv = __fmul2_rn(__ffma2_rn(neg2(ty), zz, nv), iz);
-    const float2 s2 = __ffma2_rn(du, du, __fmul2_rn(dv, dv));
+    const float2 du = fmul2(ffma2(neg2(tx), zz, nu), iz);
+    const float2 dv = fmul2(ffma2(neg2(ty), zz, nv), iz);
+    const float2 s2 = ffma2(du, du, fmul2(dv, dv));
     const float2 r = make_float2(rsqrt_fast(fmaxf(s2.x, kTiny)), rsqrt_fast(fmaxf(s2.y, kTiny)));
-    const float2 err = __fmul2_rn(s2, r);
+    const float2 err = fmul2(s2, r);
     const float2 e = make_float2(fminf(err.x, k.max_err), fminf(err.y, k.max_err));
-    const float2 t = __fmul2_rn(k.cut, e);
+    const float2 t = fmul2(k.cut, e);
     const float2 rt = make_float2(rsqrt_fast(fmaxf(t.x, kTiny)), rsqrt_fast(fmaxf(t.y, kTiny)));
-    const float2 sq = __fmul2_rn(t, rt);                  // sqrt(cut * e)
-    const float2 gs = __fmul2_rn(k.half_cut, rt);         // its derivative
+    const float2 sq = fmul2(t, rt);                  // sqrt(cut * e)
+    const float2 gs = fmul2(k.half_cut, rt);         // its derivative
     const bool l0 = e.x <= k.cut_s, l1 = e.y <= k.cut_s;
     PairOut o;
     o.loss = make_float2(l0 ? e.x : sq.x, l1 ? e.y : sq.y);
     float2 g = make_float2(l0 ? 1.f : gs.x, l1 ? 1.f : gs.y);
-    g = __fmul2_rn(g, k.inv_n);
+    g = fmul2(g, k.inv_n);
     g = make_float2(err.x <= k.max_err ? g.x : 0.f, err.y <= k.max_err ? g.y : 0.f);
-    const float2 gr = __fmul2_rn(g, r);
-    const float2 fiz = __fmul2_rn(k.f, iz);
-    const float2 gxc = __fmul2_rn(__fmul2_rn(gr, du), fiz);
-    const float2 gyc = __fmul2_rn(__fmul2_rn(gr, dv), fiz);
-    const float2 go = __fmul2_rn(neg2(__ffma2_rn(gxc, xc, __fmul2_rn(gyc, yc))), iz);
-    const float2 gsh = __fmul2_rn(__fmul2_rn(gr, __ffma2_rn(du, k.cx, __fmul2_rn(dv, k.cy))), iz);
+    const float2 gr = fmul2(g, r);
+    const float2 fiz = fmul2(k.f, iz);
+    const float2 gxc = fmul2(fmul2(gr, du), fiz);
+    const float2 gyc = fmul2(fmul2(gr, dv), fiz);
+    const float2 go = fmul2(neg2(ffma2(gxc, xc, fmul2(gyc, yc))), iz);
+    const float2 gsh = fmul2(fmul2(gr, ffma2(du, k.cx, fmul2(dv, k.cy))), iz);
     const float2 gzc = make_float2(open0 ? go.x : gsh.x, open1 ? go.y : gsh.y);
-    o.gx = __ffma2_rn(k.m[0], gxc, __ffma2_rn(k.m[4], gyc, __fmul2_rn(k.m[8], gzc)));
-    o.gy = __ffma2_rn(k.m[1], gxc, __ffma2_rn(k.m[5], gyc, __fmul2_rn(k.m[9], gzc)));
-    o.gz = __ffma2_rn(k.m[2], gxc, __ffma2_rn(k.m[6], gyc, __fmul2_rn(k.m[10], gzc)));
+    o.gx = ffma2(k.m[0], gxc, ffma2(k.m[4], gyc, fmul2(k.m[8], gzc)));
+    o.gy = ffma2(k.m[1], gxc, ffma2(k.m[5], gyc, fmul2(k.m[9], gzc)));
+    o.gz = ffma2(k.m[2], gxc, ffma2(k.m[6], gyc, fmul2(k.m[10], gzc)));
     if (!(s2.x == s2.x)) { o.loss.x = 0.f; o.gx.x = o.gy.x = o.gz.x = s2.x; }   // NaN input (see reproj_cell)
     if (!(s2.y == s2.y)) { o.loss.y = 0.f; o.gx.y = o.gy.y = o.gz.y = s2.y; }
     return o;

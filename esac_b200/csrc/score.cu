@@ -7,12 +7,12 @@
 //
 // Layout: hypotheses are grouped by expert (stable by index), cut into chunks of <= kMaxChunk; a work
 // item is (chunk, pixel tile).  A CTA keeps its tile's pixels in registers (re-centred coordinates plus
-// the principal-point offset of each cell, two pixels per f32x2 lane pair) and streams the chunk's
+// the principal-point offset of each cell, two pixels per float2 pair) and streams the chunk's
 // folded poses from shared memory, so each coordinate plane is read from HBM/L2 once per chunk instead
 // of once per hypothesis.  Per pixel-hypothesis: 9 FFMA for R*X+t, then
 //   err = |p| / |z|,  p = (xc + (cx-px) z, yc + (cy-py) z)   ->  err = num * rsqrt(num * z^2)
 //   w   = 1 / (1 + 2^(k1*min(err,maxReproj) + k0))           ==  1 - sigmoid(beta*(err - tau))
-// i.e. 3 MUFU (rsq, ex2, rcp) and ~20 fp32-pipe ops issued as FFMA2/FMUL2/FADD2.
+// i.e. 3 MUFU (rsq, ex2, rcp) and ~20 fp32 ops per cell-hypothesis.
 #include <atomic>
 
 #include "esac_internal.h"
@@ -259,7 +259,7 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
     const float2 one = make_float2(1.f, 1.f), tiny = make_float2(1e-30f, 1e-30f);
     const float mr = P.max_reproj;
 
-    // soft-inlier sum of this thread's PPT cells for hypothesis hl (pose = 3 x LDS.128, scalars broadcast to f32x2)
+    // soft-inlier sum of this thread's PPT cells for hypothesis hl (pose = 3 x LDS.128, scalars broadcast to float2)
     auto one_hyp = [&](int hl) -> float {
         const float4* q = sPose + hl * 3;
         const float4 r0 = q[0], r1 = q[1], r2 = q[2];
@@ -269,23 +269,23 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
         float2 acc = make_float2(0.f, 0.f);
 #pragma unroll
         for (int j = 0; j < NP; ++j) {
-            float2 xc = __ffma2_rn(a00, X[j], __ffma2_rn(a01, Y[j], __ffma2_rn(a02, Z[j], b0)));
-            float2 yc = __ffma2_rn(a10, X[j], __ffma2_rn(a11, Y[j], __ffma2_rn(a12, Z[j], b1)));
-            float2 zc = __ffma2_rn(a20, X[j], __ffma2_rn(a21, Y[j], __ffma2_rn(a22, Z[j], b2)));
-            float2 pu = __ffma2_rn(A[j], zc, xc);
-            float2 pv = __ffma2_rn(B[j], zc, yc);
-            float2 num = __ffma2_rn(pu, pu, __fmul2_rn(pv, pv));
-            float2 m = __ffma2_rn(__fmul2_rn(zc, zc), num, tiny);
+            float2 xc = ffma2(a00, X[j], ffma2(a01, Y[j], ffma2(a02, Z[j], b0)));
+            float2 yc = ffma2(a10, X[j], ffma2(a11, Y[j], ffma2(a12, Z[j], b1)));
+            float2 zc = ffma2(a20, X[j], ffma2(a21, Y[j], ffma2(a22, Z[j], b2)));
+            float2 pu = ffma2(A[j], zc, xc);
+            float2 pv = ffma2(B[j], zc, yc);
+            float2 num = ffma2(pu, pu, fmul2(pv, pv));
+            float2 m = ffma2(fmul2(zc, zc), num, tiny);
             float2 rs = make_float2(mufu_rsq(m.x), mufu_rsq(m.y));
-            float2 err = __fmul2_rn(num, rs);
+            float2 err = fmul2(num, rs);
             err.x = fminf(err.x, mr);
             err.y = fminf(err.y, mr);
-            float2 t = __ffma2_rn(err, k1, k0);
+            float2 t = ffma2(err, k1, k0);
             float2 ex = make_float2(mufu_ex2(t.x), mufu_ex2(t.y));
-            float2 den = __fadd2_rn(ex, one);
+            float2 den = fadd2(ex, one);
             float2 w = make_float2(mufu_rcp(den.x), mufu_rcp(den.y));
-            if (TAIL) acc = __ffma2_rn(w, V[j], acc);
-            else acc = __fadd2_rn(acc, w);
+            if (TAIL) acc = ffma2(w, V[j], acc);
+            else acc = fadd2(acc, w);
         }
         return acc.x + acc.y;
     };

@@ -1,7 +1,7 @@
-/* libesac_b200.so -- C ABI of the B200-native ESAC differentiable-RANSAC hot path.
+/* libesac_b200.so -- C ABI of the CUDA (H100, sm_90a) ESAC differentiable-RANSAC hot path.
  *
  * Drop-in boundary for the reference's `esac` Python extension
- * (/root/reference/code/esac/esac.cpp:513-516: m.def("forward", &esac_forward), m.def("backward",
+ * (code/esac/esac.cpp:513-516: m.def("forward", &esac_forward), m.def("backward",
  * &esac_backward)).  esacb200_forward / esacb200_backward take exactly the arguments of
  * esac_forward (esac.cpp:64-77) / esac_backward (esac.cpp:213-230) with the at::Tensor arguments
  * flattened to pointer + sizes; everything else in this header is additive (context handling,

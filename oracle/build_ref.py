@@ -1,16 +1,18 @@
-"""Builds oracle/_ref/esac_ref*.so: the reference's OWN esac extension, compiled from its unmodified sources where they
-lie under /root/reference/code/esac (esac.cpp, thread_rand.cpp + the four headers they include), against the minimal
-OpenCV stand-in of oracle/ref_shim/ (whose calib3d calls are executed by the real OpenCV inside the cv2 wheel).
+"""Builds oracle/_ref/esac_ref*.so: the reference's OWN esac extension, compiled from its unmodified sources where a
+checkout of vislearn/esac is named by $ESAC_REFERENCE (code/esac: esac.cpp, thread_rand.cpp + the four headers they
+include), against the minimal OpenCV stand-in of oracle/ref_shim/ (whose calib3d calls are executed by the real OpenCV
+inside the cv2 wheel).
 
-TEST INFRASTRUCTURE, NOT PRODUCT CODE.  Nothing from /root/reference is copied into the repository; outputs go to
-oracle/_ref/ only (git-ignored, but shipped to the GPU box with the snapshot).  The reference's own build system
-(code/esac/setup.py) is not run: it needs $CONDA_PREFIX and OpenCV C++ headers / libraries this image lacks.
+TEST INFRASTRUCTURE, NOT PRODUCT CODE.  Nothing from the reference is copied into the repository; outputs go to
+oracle/_ref/ only (git-ignored).  The reference's own build system (code/esac/setup.py) is not run: it needs $CONDA_PREFIX
+and the OpenCV C++ headers / libraries.
 
-    python -m oracle.build_ref [--force]
+    ESAC_REFERENCE=<checkout of vislearn/esac> python -m oracle.build_ref [--force]
 """
 from __future__ import annotations
 
 import hashlib
+import os
 import subprocess
 import sys
 import sysconfig
@@ -20,7 +22,7 @@ from pathlib import Path
 HERE = Path(__file__).resolve().parent
 SHIM = HERE / "ref_shim"
 OUT_DIR = HERE / "_ref"
-REF_SRC = Path("/root/reference/code/esac")
+REF_SRC = Path(os.environ["ESAC_REFERENCE"]) / "code" / "esac" if os.environ.get("ESAC_REFERENCE") else None
 REF_FILES = ["esac.cpp", "thread_rand.cpp", "thread_rand.h", "esac_types.h", "esac_util.h", "esac_loss.h",
              "esac_derivative.h", "stop_watch.h"]
 SHIM_FILES = [SHIM / "opencv2" / "opencv.hpp", SHIM / "shim_cv2.cpp", SHIM / "ref_module.cpp"]
@@ -32,7 +34,7 @@ def lib_path() -> Path:
 
 
 def reference_available() -> bool:
-    return all((REF_SRC / f).exists() for f in REF_FILES)
+    return REF_SRC is not None and all(os.access(REF_SRC / f, os.R_OK) for f in REF_FILES)
 
 
 def _digest() -> str:
@@ -44,8 +46,8 @@ def _digest() -> str:
 
 
 def build_ref(force: bool = False, verbose: bool = False) -> Path | None:
-    """Returns the path of the built module, or None when the reference sources are absent and nothing was prebuilt
-    (the GPU box: /root/reference does not exist there, the prebuilt file travels with the snapshot)."""
+    """Returns the path of the built module, or None when the reference sources are absent (or unreadable) and nothing
+    was built before."""
     lib = lib_path()
     if not reference_available():
         return lib if lib.exists() else None

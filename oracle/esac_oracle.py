@@ -8,22 +8,22 @@ What it is: a line-by-line restatement, in Python on top of the *real* OpenCV
 (``cv2`` 4.13 wheel: ``solvePnP`` P3P / ITERATIVE, ``projectPoints``, ``Rodrigues``), of the
 reference's native extension
 
-    /root/reference/code/esac/esac.cpp          esac_forward  64-190, esac_backward 213-511
-    /root/reference/code/esac/esac_util.h       createSampling 53-70, safeSolvePnP 85-114,
+    code/esac/esac.cpp          esac_forward  64-190, esac_backward 213-511
+    code/esac/esac_util.h       createSampling 53-70, safeSolvePnP 85-114,
                                                 sampleHypotheses 129-225, getHypScores 235-260,
                                                 getReproErrs 274-363, refineHyp 378-454,
                                                 softMax 461-482, entropy 489-497, draw 505-530,
                                                 pose2trans 537-548, trans2pose 555-568, getMax 599-612
-    /root/reference/code/esac/esac_derivative.h dProjectdObj 47-102, dPNP 128-185,
+    code/esac/esac_derivative.h dProjectdObj 47-102, dPNP 128-185,
                                                 dScore 205-324, dSMScore 347-420
-    /root/reference/code/esac/esac_loss.h       calcAngularDistance 45-55, loss 66-83, dLoss 94-210
+    code/esac/esac_loss.h       calcAngularDistance 45-55, loss 66-83, dLoss 94-210
 
 including the float/double mix, the x-outer/y-inner point order, EPS / PROB_THRESH / MAXLOSS,
 the ``> 10`` clamps, the dLoss cut quirk, ``PI`` vs ``CV_PI`` and the ``irand`` off-by-one
 (last row / column never sampled).
 
 PARITY PINNED against the reference's own compiled code: oracle/_ref/esac_ref is the unmodified
-/root/reference/code/esac/{esac.cpp, thread_rand.cpp} + headers, compiled by oracle/build_ref.py against a minimal
+code/esac/{esac.cpp, thread_rand.cpp} + headers, compiled by oracle/build_ref.py against a minimal
 <opencv2/opencv.hpp> stand-in whose solvePnP / projectPoints / Rodrigues / Mat::inv are executed by the real OpenCV of the
 cv2 wheel.  Run single-threaded on its default std::mt19937 stream (reproduced here by ThreadRandStream) it returns the
 same winning expert, a bit-identical pose, the same expected loss (<= 5e-11) and the same gradients (<= 3e-9 relative)

@@ -4,8 +4,8 @@
  * this file's library; the product path (esac_b200/) never does.
  *
  * Restates, without OpenCV, the reference's hot loop #1:
- *   getReproErrs (no-Jacobian path)   /root/reference/code/esac/esac_util.h:274-318,355-362
- *   getHypScores                       /root/reference/code/esac/esac_util.h:235-260
+ *   getReproErrs (no-Jacobian path)   code/esac/esac_util.h:274-318,355-362
+ *   getHypScores                       code/esac/esac_util.h:235-260
  *   the `#pragma omp parallel for` over hypotheses that drives them   esac.cpp:131-140
  * cv::projectPoints (OpenCV, not in the reference tree) is restated from its observable arithmetic
  * (SURVEY.md Appendix A, re-verified against cv2 4.13 by tests/test_oracle_c.py): R = Rodrigues(rvec),

@@ -1,6 +1,6 @@
 /* Minimal stand-in for <opencv2/opencv.hpp> -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  *
- * Purpose: let the UNMODIFIED reference sources (/root/reference/code/esac/esac.cpp, esac_util.h, esac_loss.h,
+ * Purpose: let the UNMODIFIED reference sources (code/esac/esac.cpp, esac_util.h, esac_loss.h,
  * esac_derivative.h, thread_rand.cpp) compile in an image that has no OpenCV C++ headers or libraries, only the `cv2`
  * Python wheel (OpenCV 4.13, statically linked, no exported C++ symbols).  This header declares exactly the slice of
  * the cv:: API those files use.  The arithmetic that matters is NOT restated here:

@@ -1,5 +1,5 @@
 /* Python module `esac_ref`: the reference's two entry points, compiled from the UNMODIFIED sources under
- * /root/reference/code/esac (see oracle/build_ref.py) -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
+ * code/esac (see oracle/build_ref.py) -- TEST INFRASTRUCTURE, NOT PRODUCT CODE.
  *
  * Why not the module esac.cpp:513-516 defines itself: that binding keeps the GIL while esac_forward runs, and the
  * reference's OpenMP worker threads would then wait forever for it inside the cv2-forwarding shim.  This file binds the

@@ -1,5 +1,5 @@
 """Writes tests/golden/ref_*.npz: outputs of the reference's OWN compiled code (oracle/_ref/esac_ref = the unmodified
-/root/reference/code/esac sources on the real OpenCV of the cv2 wheel, see oracle/build_ref.py), run single-threaded on its
+code/esac sources on the real OpenCV of the cv2 wheel, see oracle/build_ref.py), run single-threaded on its
 default std::mt19937 stream (seed 1305).
 
 Each fixture holds the scene (small cases) or the make_scene() arguments that regenerate it (480x640 cases: the tensors
@@ -8,7 +8,7 @@ the reference's results: winning expert, camera pose, expected loss and the grad
 sample of its entries plus per-plane sums (480x640 cases).  tests/test_gpu_ref_golden.py injects the same minimal sets into
 the CUDA path and compares; tests/test_oracle.py checks the oracle against them on the CPU.
 
-Needs /root/reference (this container only).  Run:  python tests/golden/make_ref_golden.py [name ...]
+Needs a checkout of vislearn/esac named by $ESAC_REFERENCE.  Run:  python tests/golden/make_ref_golden.py [name ...]
 """
 import sys
 import time
@@ -96,7 +96,7 @@ def run_reference(R, sc):
 if __name__ == "__main__":
     here = Path(__file__).resolve().parent
     R = load_ref()
-    assert R is not None, "needs /root/reference"
+    assert R is not None, "needs $ESAC_REFERENCE"
     R.set_num_threads(1)
     R.set_native_project(False)
     want = set(sys.argv[1:])

@@ -1,4 +1,4 @@
-"""GPU parity of the forward path against the cv2 oracle (run with `-m gpu` on the B200 box).
+"""GPU parity of the forward path against the cv2 oracle (run with `-m gpu` on an H100).
 
 Tolerances are BASELINE.json's: 1e-4 on soft-inlier scores, 1e-3 deg / 1e-3 cm on the final pose."""
 import numpy as np

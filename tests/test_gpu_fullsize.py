@@ -117,7 +117,7 @@ def test_split_upload_of_host_maps_changes_nothing(api, kw):
 
 def test_refinement_code_paths_agree_at_full_resolution(api):
     """The refinement kernel has three ways to walk a CTA's share of the map: cells + inlier list in shared memory (share <= 96
-    words: the forward's 148-CTA group), inlier list in global scratch (<= 2048 words), and predicated passes over all cells
+    words: a 148-CTA group), inlier list in global scratch (<= 2048 words), and predicated passes over all cells
     (larger shares).  Forcing the group size selects each of them at 480x640; rounds and inlier counts must be identical and the
     poses equal up to the summation order (1e-9)."""
     sc = make_scene(E=1, H=480, W=640, M=6, sub=1, seed=21, outlier_frac=0.4)

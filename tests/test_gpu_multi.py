@@ -128,7 +128,7 @@ def _worker(rank, world, port, q):
     dist.destroy_process_group()
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_two_gpu_sharding_reproduces_single_gpu():
     import torch.multiprocessing as mp
     ctx = mp.get_context("spawn")
@@ -161,7 +161,7 @@ def test_two_gpu_sharding_reproduces_single_gpu():
     assert np.abs(ref["ref_grads"]).max() > 0
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
 def test_one_process_two_devices_full_resolution_and_current_device_kept():
     """One process, contexts on cuda:0 and cuda:1: the scoring kernel's >48 KB shared-memory opt-in is a per-device
     attribute (it used to be set once per process), and no entry point may leave the caller's current device switched."""

@@ -219,7 +219,7 @@ def _ref_fixtures_small():
 
 @pytest.mark.parametrize("path", _ref_fixtures_small(), ids=lambda p: p.stem)
 def test_oracle_reproduces_the_compiled_reference_fixtures(path):
-    """No /root/reference needed: the fixtures were written by oracle/_ref (unmodified esac.cpp on the real OpenCV, single
+    """No reference checkout needed: the fixtures were written by oracle/_ref (unmodified esac.cpp on the real OpenCV, single
     thread, default mt19937 stream); ThreadRandStream replays that stream."""
     from ref_golden_util import params_of
     z = np.load(path)

@@ -1,11 +1,15 @@
 """Pins the oracle to the reference's OWN compiled code.
 
-oracle/_ref/esac_ref is the unmodified /root/reference/code/esac/{esac.cpp,thread_rand.cpp} (+ its headers) compiled
+oracle/_ref/esac_ref is the unmodified code/esac/{esac.cpp,thread_rand.cpp} of vislearn/esac (+ its headers) compiled
 against oracle/ref_shim/opencv2/opencv.hpp, whose solvePnP / projectPoints / Rodrigues / Mat::inv are executed by the real
 OpenCV inside the cv2 wheel (oracle/build_ref.py).  With one OpenMP thread the reference consumes one std::mt19937 stream
 in a fixed order; oracle.esac_oracle.ThreadRandStream reproduces that stream, so both see identical minimal sets and every
-output of esac_forward / esac_backward can be compared.  Skipped where neither /root/reference nor a prebuilt module exists.
+output of esac_forward / esac_backward can be compared.  What the compiled reference returned for the calls below is stored
+in tests/golden/pin/ref_pin.npz (tests/golden/make_ref_pin.py); the two tests of the compiled stand-in itself are skipped
+where oracle/_ref is not built.
 """
+from pathlib import Path
+
 import numpy as np
 import pytest
 
@@ -14,30 +18,36 @@ from oracle import esac_oracle as O
 from oracle.build_ref import load_ref
 
 torch = pytest.importorskip("torch")
+GOLD = Path(__file__).resolve().parent / "golden" / "pin" / "ref_pin.npz"
+
+
+@pytest.fixture(scope="module")
+def gold():
+    return np.load(GOLD)
 
 
 @pytest.fixture(scope="module")
 def ref():
     mod = load_ref()
     if mod is None:
-        pytest.skip("oracle/_ref is not built and /root/reference is absent")
+        pytest.skip("oracle/_ref is not built and $ESAC_REFERENCE names no readable reference checkout")
     mod.set_num_threads(1)
     mod.set_native_project(False)
     return mod
 
 
-def test_thread_rand_stream_is_the_references(ref):
+IRAND_MAX = (79, 59, 639, 479, 2, 3_000_000_000 // 2, 7)
+
+
+def test_thread_rand_stream_is_the_references(gold):
     """thread_rand.cpp:34-43,68-71 on generator 0 == ThreadRandStream (mt19937 + libstdc++ uniform_int_distribution)."""
-    ref.force_init(1305)
     mt = O.ThreadRandStream(1305)
-    for exc_max in (79, 59, 639, 479, 2, 3_000_000_000 // 2, 7):
-        a = [ref.irand(0, exc_max, 0) for _ in range(300)]
+    for exc_max, a in zip(IRAND_MAX, gold["irand_1305"].tolist()):
         b = [mt.irand(0, exc_max) for _ in range(300)]
         assert a == b
         assert max(a) <= exc_max - 1 and min(a) >= 0
-    ref.force_init(77)
     mt = O.ThreadRandStream(77)
-    assert [ref.irand(3, 11, 0) for _ in range(50)] == [mt.irand(3, 11) for _ in range(50)]
+    assert gold["irand_77"].tolist() == [mt.irand(3, 11) for _ in range(50)]
 
 
 CASES = {
@@ -49,58 +59,52 @@ CASES = {
 
 
 @pytest.mark.parametrize("name", list(CASES))
-def test_forward_and_backward_equal_the_compiled_reference(ref, name):
+def test_forward_and_backward_equal_the_compiled_reference(gold, name):
     sc = make_scene(**CASES[name])
-    co, asg = torch.from_numpy(sc.coords), torch.from_numpy(sc.assign)
     # forward: esac.cpp:64-190
-    ref.force_init(1305)
-    out = torch.zeros(4, 4)
-    e_ref = ref.forward(co, asg, out, *sc.params)
     mine = np.zeros((4, 4), np.float32)
     e_or = O.forward(sc.coords, sc.assign, mine, *sc.params, mt=O.ThreadRandStream(1305))
-    assert e_ref == e_or
-    assert np.abs(out.numpy() - mine).max() <= 1e-6  # observed: bit-identical
+    assert int(gold[f"{name}_expert"]) == e_or
+    assert np.abs(gold[f"{name}_pose"] - mine).max() <= 1e-6  # observed: bit-identical
     # backward: esac.cpp:213-511 (accumulates into the caller's tensor: start from a non-zero one)
-    ref.force_init(1305)
-    g_ref = torch.full(sc.coords.shape, 0.25)
-    l_ref = ref.backward(co, g_ref, asg, torch.from_numpy(sc.gt_pose), 1.0, 100.0, 100.0, *sc.params)
+    l_ref, g_ref = float(gold[f"{name}_loss"]), gold[f"{name}_grads"]
     g_or = np.full(sc.coords.shape, 0.25, np.float32)
     l_or = O.backward(sc.coords, g_or, sc.assign, sc.gt_pose, 1.0, 100.0, 100.0, *sc.params, mt=O.ThreadRandStream(1305))
     assert abs(l_ref - l_or) <= 1e-9 * max(1.0, abs(l_ref))
     scale = np.abs(g_or - 0.25).max()
     assert scale > 0
-    assert np.abs(g_ref.numpy() - g_or).max() <= 1e-6 * scale  # observed: <= 3e-9
+    assert np.abs(g_ref - g_or).max() <= 1e-6 * scale  # observed: <= 3e-9
 
 
-def test_loss_cut_and_weights_equal_the_compiled_reference(ref):
+CUT_SCENE = dict(E=2, H=24, W=32, M=24, sub=8, seed=9)
+CUT_CASES = ((1.0, 100.0, 5.0), (0.5, 10.0, 1000.0))
+
+
+def test_loss_cut_and_weights_equal_the_compiled_reference(gold):
     """The cut branch (esac_loss.h:78-80 vs :133-137,202-203 -- the sqrt(cut*loss) / 0.5/sqrt(loss) mismatch) and
     non-default weights, on a scene whose poses are far from a deliberately wrong ground truth."""
-    sc = make_scene(E=2, H=24, W=32, M=24, sub=8, seed=9)
+    sc = make_scene(**CUT_SCENE)
     gt = sc.gt_pose.copy()
     gt[:3, 3] += np.array([3.0, -2.0, 1.0], np.float32)
-    for (w_rot, w_trans, cut) in ((1.0, 100.0, 5.0), (0.5, 10.0, 1000.0)):
-        ref.force_init(1305)
-        g_ref = torch.zeros(sc.coords.shape)
-        l_ref = ref.backward(torch.from_numpy(sc.coords), g_ref, torch.from_numpy(sc.assign), torch.from_numpy(gt), w_rot,
-                             w_trans, cut, *sc.params)
+    for i, (w_rot, w_trans, cut) in enumerate(CUT_CASES):
+        l_ref, g_ref = float(gold[f"cut{i}_loss"]), gold[f"cut{i}_grads"]
         g_or = np.zeros_like(sc.coords)
         l_or = O.backward(sc.coords, g_or, sc.assign, gt, w_rot, w_trans, cut, *sc.params, mt=O.ThreadRandStream(1305))
         assert abs(l_ref - l_or) <= 1e-9 * max(1.0, abs(l_ref))
-        assert np.abs(g_ref.numpy() - g_or).max() <= 1e-6 * max(np.abs(g_or).max(), 1e-30)
+        assert np.abs(g_ref - g_or).max() <= 1e-6 * max(np.abs(g_or).max(), 1e-30)
 
 
-def test_stream_state_persists_across_calls(ref):
+PERSIST_SCENE = dict(E=1, H=24, W=32, M=16, sub=8, seed=11)
+
+
+def test_stream_state_persists_across_calls(gold):
     """thread_rand.cpp:4-5: static generators -- a second call continues the stream; so does the oracle's object."""
-    sc = make_scene(E=1, H=24, W=32, M=16, sub=8, seed=11)
-    co, asg = torch.from_numpy(sc.coords), torch.from_numpy(sc.assign)
-    ref.force_init(1305)
+    sc = make_scene(**PERSIST_SCENE)
     mt = O.ThreadRandStream(1305)
-    for _ in range(2):
-        out = torch.zeros(4, 4)
-        ref.forward(co, asg, out, *sc.params)
+    for out in gold["persist_poses"]:
         mine = np.zeros((4, 4), np.float32)
         O.forward(sc.coords, sc.assign, mine, *sc.params, mt=mt)
-        assert np.abs(out.numpy() - mine).max() <= 1e-6
+        assert np.abs(out - mine).max() <= 1e-6
 
 
 def test_native_projection_of_the_shim_is_bit_identical(ref):

@@ -1,5 +1,5 @@
-"""Two esac.backward calls at the bench shape (GPU only) -- the target of the ncu launch list in profiles/ (per-kernel
-durations of the backward's stages)."""
+"""Two esac.backward calls at the bench shape (GPU only) -- the target of a profiler's launch list (per-kernel durations
+of the backward's stages)."""
 import sys
 sys.path.insert(0, str(__import__('pathlib').Path(__file__).resolve().parents[1]))
 import torch

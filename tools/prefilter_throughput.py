@@ -1,6 +1,6 @@
 """Pure prefilter throughput: ONE wave with a 2048-try window for every hypothesis (3.67 M tries in one launch per lane)."""
 import sys
-sys.path.insert(0, "/root/repo")
+sys.path.insert(0, str(__import__('pathlib').Path(__file__).resolve().parents[1]))
 import numpy as np, torch
 import esac_b200.api as api
 from esac_b200.synth import make_scene

@@ -274,8 +274,11 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
             float2 zc = ffma2(a20, X[j], ffma2(a21, Y[j], ffma2(a22, Z[j], b2)));
             float2 pu = ffma2(A[j], zc, xc);
             float2 pv = ffma2(B[j], zc, yc);
-            float2 num = ffma2(pu, pu, fmul2(pv, pv));
-            float2 m = ffma2(fmul2(zc, zc), num, tiny);
+            // num >= 1e-30 (the 1e-30 vanishes in the rounding of any |p|^2 above 1e-22): a cell on the pixel's ray still gets
+            // err ~ 0, while zc == 0 gives m = 0 -> rsq = +inf -> err = +inf -> maxReproj, also for a cell AT the camera centre
+            // (p = 0), which a 1e-30 added to m instead would score as a perfect inlier.  No extra instruction.
+            float2 num = ffma2(pu, pu, ffma2(pv, pv, tiny));
+            float2 m = fmul2(fmul2(zc, zc), num);
             float2 rs = make_float2(mufu_rsq(m.x), mufu_rsq(m.y));
             float2 err = fmul2(num, rs);
             err.x = fminf(err.x, mr);

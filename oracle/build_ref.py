@@ -1,13 +1,13 @@
 """Builds oracle/_ref/esac_ref*.so: the reference's OWN esac extension, compiled from its unmodified sources where a
-checkout of vislearn/esac is named by $ESAC_REFERENCE (code/esac: esac.cpp, thread_rand.cpp + the four headers they
-include), against the minimal OpenCV stand-in of oracle/ref_shim/ (whose calib3d calls are executed by the real OpenCV
-inside the cv2 wheel).
+checkout of vislearn/esac is named by $ESAC_REFERENCE or sits beside the repository as `reference` (code/esac: esac.cpp,
+thread_rand.cpp + the four headers they include), against the minimal OpenCV stand-in of oracle/ref_shim/ (whose calib3d
+calls are executed by the real OpenCV inside the cv2 wheel).
 
 TEST INFRASTRUCTURE, NOT PRODUCT CODE.  Nothing from the reference is copied into the repository; outputs go to
 oracle/_ref/ only (git-ignored).  The reference's own build system (code/esac/setup.py) is not run: it needs $CONDA_PREFIX
 and the OpenCV C++ headers / libraries.
 
-    ESAC_REFERENCE=<checkout of vislearn/esac> python -m oracle.build_ref [--force]
+    [ESAC_REFERENCE=<checkout of vislearn/esac>] python -m oracle.build_ref [--force]
 """
 from __future__ import annotations
 
@@ -22,7 +22,21 @@ from pathlib import Path
 HERE = Path(__file__).resolve().parent
 SHIM = HERE / "ref_shim"
 OUT_DIR = HERE / "_ref"
-REF_SRC = Path(os.environ["ESAC_REFERENCE"]) / "code" / "esac" if os.environ.get("ESAC_REFERENCE") else None
+
+
+def _find_reference() -> Path | None:
+    """code/esac of the reference checkout: the one $ESAC_REFERENCE names, else a checkout named `reference` beside this
+    repository or beside one of its enclosing directories (the nearest wins)."""
+    if os.environ.get("ESAC_REFERENCE"):
+        return Path(os.environ["ESAC_REFERENCE"]) / "code" / "esac"
+    for d in HERE.parent.parents:
+        cand = d / "reference" / "code" / "esac"
+        if cand.is_dir():
+            return cand
+    return None
+
+
+REF_SRC = _find_reference()
 REF_FILES = ["esac.cpp", "thread_rand.cpp", "thread_rand.h", "esac_types.h", "esac_util.h", "esac_loss.h",
              "esac_derivative.h", "stop_watch.h"]
 SHIM_FILES = [SHIM / "opencv2" / "opencv.hpp", SHIM / "shim_cv2.cpp", SHIM / "ref_module.cpp"]

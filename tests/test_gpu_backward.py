@@ -20,9 +20,10 @@ def api():
     (2, 3, 30, 40, 48, {}),
     (3, 2, 24, 31, 32, {"shiftX": 2, "shiftY": -3}),
     (4, 2, 30, 40, 32, {"outlier_frac": 0.8}),      # flat hypothesis distribution: many contributing hypotheses
+    (5, 2, 29, 37, 32, {"sub": 3, "shiftX": -1, "shiftY": 2}),   # odd sub-sampling: pixel centre x*3 + 1
 ])
 def test_backward_matches_oracle(api, seed, E, H, W, M, kw):
-    sc = make_scene(E=E, H=H, W=W, M=M, sub=8, seed=seed, **kw)
+    sc = make_scene(E=E, H=H, W=W, M=M, seed=seed, **{"sub": 8, **kw})
     g_ref = np.zeros_like(sc.coords)
     l_ref, bt = O.backward(sc.coords, g_ref, sc.assign, sc.gt_pose, 1.0, 100.0, 100.0, *sc.params, seed=50 + seed, trace=True)
     api.set_seed(50 + seed)
@@ -36,6 +37,81 @@ def test_backward_matches_oracle(api, seed, E, H, W, M, kw):
     assert abs(loss - l_ref) < 1e-6 * max(1.0, abs(l_ref))
     scale = max(np.abs(g_ref).max(), 1e-12)
     assert np.abs(g - g_ref).max() / scale < 1e-3, (np.abs(g - g_ref).max(), scale)
+
+
+# ---- backward under forced refinement walks and scoring shapes --------------------------------------------------------------
+FORCED_ARGS = (1.0, 100.0, 100.0)     # wLossRot, wLossTrans, lossCut
+
+
+@pytest.fixture(scope="module")
+def forced_scene():
+    """E = 3, 48x64, M = 48 with 90 % outliers: a flat hypothesis distribution, so that backward refines many contributing
+    hypotheses (>= 8 refinement jobs), and the cv2 oracle's backward of it, computed once."""
+    sc = make_scene(E=3, H=48, W=64, M=48, sub=8, seed=17, outlier_frac=0.9)
+    g_ref = np.zeros_like(sc.coords)
+    l_ref, bt = O.backward(sc.coords, g_ref, sc.assign, sc.gt_pose, *FORCED_ARGS, *sc.params, seed=57, trace=True)
+    n_ref = int((bt.probs >= O.PROB_THRESH).sum())
+    assert n_ref >= 8
+    return sc, l_ref, g_ref, n_ref
+
+
+def _check_backward(api, forced_scene, options):
+    sc, l_ref, g_ref, n_ref = forced_scene
+    ctx = api.context()
+    try:
+        for k, v in options.items():
+            ctx.set_option(k, v)
+        api.set_seed(57)
+        g = np.zeros_like(sc.coords)
+        loss = api.backward(sc.coords, g, sc.assign, sc.gt_pose, *FORCED_ARGS, *sc.params)
+        st = api.last_stats()
+    finally:
+        for k, v in {"refine_group": 0, "refine_compact": 1, "score_ppt": 0}.items():
+            ctx.set_option(k, v)
+    assert st["n_contrib"] == n_ref, (options, st["n_contrib"], n_ref)
+    assert abs(loss - l_ref) < 1e-6 * max(1.0, abs(l_ref)), (options, loss, l_ref)
+    scale = max(np.abs(g_ref).max(), 1e-12)
+    assert np.abs(g - g_ref).max() / scale < 1e-3, (options, np.abs(g - g_ref).max(), scale)
+    return st
+
+
+@pytest.mark.parametrize("compact", [0, 1])
+@pytest.mark.parametrize("group", [1, 0, 1 << 20], ids=["group1", "auto", "max"])
+def test_backward_matches_oracle_under_every_refinement_walk(api, forced_scene, group, compact):
+    st = _check_backward(api, forced_scene, {"refine_group": group, "refine_compact": compact})
+    if group == 1:
+        assert st["refine_group"] == 1
+
+
+@pytest.mark.parametrize("ppt", [2, 4, 8])
+def test_backward_matches_oracle_under_every_scoring_shape(api, forced_scene, ppt):
+    st = _check_backward(api, forced_scene, {"score_ppt": ppt})
+    assert st["score_ppt"] == ppt
+
+
+def test_backward_gradient_of_a_misaligned_view_is_bitwise_the_aligned_one(api):
+    """Coordinates and outGradients 4 bytes past a 16-byte boundary (scalar scoring loads, unaligned gradient rows): the same
+    loss and the same gradient bits as aligned CUDA tensors."""
+    import torch
+    sc = make_scene(E=3, H=48, W=64, M=48, sub=8, seed=17, outlier_frac=0.9)
+
+    def view(a, offset):
+        buf = torch.zeros(a.size + 4, dtype=torch.float32, device="cuda")
+        v = buf[offset:offset + a.size].view(a.shape)
+        v.copy_(torch.from_numpy(a))
+        return v
+
+    res = []
+    for offset in (0, 1):
+        co, g = view(sc.coords, offset), view(np.zeros_like(sc.coords), offset)
+        assert co.data_ptr() % 16 == 4 * offset and g.data_ptr() % 16 == 4 * offset
+        api.set_seed(57)
+        loss = api.backward(co, g, torch.from_numpy(sc.assign).cuda(), torch.from_numpy(sc.gt_pose).cuda(), *FORCED_ARGS,
+                            *sc.params)
+        res.append((loss, g.cpu().numpy()))
+    assert res[0][0] == res[1][0]
+    assert np.array_equal(res[0][1], res[1][1])
+    assert np.abs(res[0][1]).max() > 0
 
 
 def test_backward_accumulates_in_place(api):

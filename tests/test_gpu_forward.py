@@ -32,9 +32,10 @@ def _oracle_hyps(sc, seed):
 @pytest.mark.parametrize("E,H,W,M,sub,kw", [
     (1, 60, 80, 64, 8, {}),                                  # config 1 shape (DSAC++ mode)
     (3, 30, 40, 48, 8, {"shiftX": 3, "shiftY": -4}),          # shifted sampling grid (training augmentation)
-    (2, 60, 107, 32, 8, {}),                                  # N % 4 != 0 -> scalar load path, ragged tile
+    (2, 60, 107, 32, 8, {}),                                  # N = 6420: N % 4 == 0, vector loads (ppt 2), ragged tile
     (2, 37, 53, 32, 4, {}),                                   # odd sizes
     (2, 24, 32, 40, 8, {"world_offset": 700.0}),              # world-scale coordinates (re-centring path)
+    (2, 61, 107, 32, 8, {}),                                  # N = 6527 odd -> scalar load path, ragged tile
 ])
 def test_scores_match_oracle_for_given_poses(api, E, H, W, M, sub, kw):
     sc = make_scene(E=E, H=H, W=W, M=M, sub=sub, seed=11, **kw)
@@ -85,6 +86,7 @@ def test_sampling_matches_oracle_stream(api, E, H, W, M):
     (3, 7, 60, 80, 256, 8, {}),                       # config 2 at the native shape
     (4, 2, 60, 107, 64, 8, {"shiftX": -2, "shiftY": 4}),
     (5, 2, 45, 60, 64, 8, {"outlier_frac": 0.7}),
+    (6, 2, 41, 53, 64, 3, {"shiftX": 2, "shiftY": -1}),  # odd sub-sampling: pixel centre x*3 + 1
 ])
 def test_forward_matches_oracle(api, seed, E, H, W, M, sub, kw):
     sc = make_scene(E=E, H=H, W=W, M=M, sub=sub, seed=seed, **kw)
@@ -330,3 +332,100 @@ def test_sampling_gives_up_after_max_tries_on_an_empty_plane(api):
         api.set_option("max_tries", 1000000)
     assert hy["tries"].tolist() == [3000] * 8
     assert np.all(hy["poses"] == 0)  # safeSolvePnP's failure state
+
+
+# ---- every refinement walk against the cv2 oracle -------------------------------------------------------------------
+# refine.cu has four ways to walk a CTA's share of `words` = ceil(N / 32) mask words, chosen per launch from the group size G:
+# share <= kCacheWords (96) -> cells cached in shared memory, else read from global memory; and with refine_compact = 1 the
+# LM evaluations walk a per-CTA inlier list (shared memory when cached, global scratch up to kMaxCompactWords = 2048),
+# otherwise predicated passes over all cells.  At 60x80 (150 words) G = 1 is uncached and G >= 2 cached, so every walk runs.
+REFINE_CACHE_WORDS, REFINE_COMPACT_WORDS = 96, 2048
+
+
+def refine_walk(N, group, compact):
+    words = (N + 31) // 32
+    share = (words + group - 1) // group
+    cached = share <= REFINE_CACHE_WORDS
+    if compact and (cached or share <= REFINE_COMPACT_WORDS):
+        return "shared-list" if cached else "global-list"
+    return "cached-all-cells" if cached else "all-cells"
+
+
+def perturbed_truth(sc, rng, M, rot=0.004, trans=0.02):
+    """Ground truth with a small motion in the camera frame: every refinement round moves."""
+    import cv2
+    T = np.linalg.inv(sc.gt_pose.astype(np.float64))
+    poses6 = np.zeros((M, 6))
+    for h in range(M):
+        dR, _ = cv2.Rodrigues(rng.normal(0, rot, 3))
+        poses6[h, :3] = cv2.Rodrigues(dR @ T[:3, :3])[0].ravel()
+        poses6[h, 3:] = dR @ T[:3, 3] + rng.normal(0, trans, 3)
+    return poses6
+
+
+WALK_SCENES = {
+    "60x80-sub8": dict(E=2, H=60, W=80, M=12, sub=8, seed=6),
+    "120x160-sub4": dict(E=2, H=120, W=160, M=14, sub=4, seed=12, noise=0.05, outlier_frac=0.3),
+}
+
+
+@pytest.fixture(scope="module", params=list(WALK_SCENES))
+def walk_scene(request):
+    """A scene, M >= 12 perturbed-truth poses on the ground-truth plane (so that jobs_hint >= 8) and the cv2 oracle's
+    refineHyp of each, computed once."""
+    kw = WALK_SCENES[request.param]
+    sc = make_scene(**kw)
+    M = kw["M"]
+    assign = np.full(M, sc.gt_expert, np.int64)
+    poses6 = perturbed_truth(sc, np.random.default_rng(kw["seed"]), M)
+    K = O.cam_mat(sc.f, sc.ppx, sc.ppy)
+    H, W = sc.coords.shape[2:]
+    sampling = O.create_sampling(W, H, sc.sub, sc.shiftX, sc.shiftY)
+    ref = []
+    for h in range(M):
+        rv, tv = poses6[h, :3].reshape(3, 1), poses6[h, 3:].reshape(3, 1)
+        errs, _ = O.get_repro_errs(sc.coords, rv, tv, sc.gt_expert, sampling, K, sc.max_reproj)
+        r, t, im, rr = O.refine_hyp(sc.coords, errs, sampling, K, sc.gt_expert, sc.tau, O.MAX_REF_STEPS, sc.max_reproj, rv, tv)
+        ref.append((r, t, 0 if im is None else int(im.sum()), rr))
+    return request.param, sc, assign, poses6, ref
+
+
+def test_every_refinement_walk_matches_oracle(api, walk_scene):
+    """refine_group in {1, 2, auto, max} x refine_compact x refine_pretest x refine_jobs_per_group in {1, 3}: rounds and final
+    inlier counts equal the oracle's and the poses are within 1e-3 deg / 1e-5 m of it; across variants rounds and inliers are
+    identical and the poses equal up to the summation order (1e-9)."""
+    import itertools
+    name, sc, assign, poses6, ref = walk_scene
+    N = sc.coords.shape[2] * sc.coords.shape[3]
+    ctx = api.context()
+    first, walks = None, set()
+    try:
+        for grp, compact, pretest, jpg in itertools.product((1, 2, 0, 1 << 20), (0, 1), (0, 1), (1, 3)):
+            ctx.set_option("refine_group", grp)
+            ctx.set_option("refine_compact", compact)
+            ctx.set_option("refine_pretest", pretest)
+            ctx.set_option("refine_jobs_per_group", jpg)
+            got, rounds, inl = api.refine_poses(sc.coords, assign, poses6, sc.shiftX, sc.shiftY, sc.f, sc.ppx, sc.ppy, sc.tau,
+                                                sc.max_reproj, sc.sub)
+            G = api.last_stats()["refine_group"]
+            if grp in (1, 2):
+                assert G == grp
+            walks.add(refine_walk(N, G, compact))
+            tag = (grp, G, compact, pretest, jpg)
+            for h, (r, t, n_in, rr) in enumerate(ref):
+                assert rounds[h] == rr and inl[h] == n_in, (tag, h, rounds[h], rr, inl[h], n_in)
+                Ta, Tb = O.pose2trans(r, t), O.pose2trans(got[h, :3].reshape(3, 1), got[h, 3:].reshape(3, 1))
+                rot, trans = pose_error(Tb, Ta)
+                assert rot < ROT_TOL_DEG and trans < TRANS_TOL_M, (tag, h, rot, trans)
+            if first is None:
+                first = (got, rounds, inl)
+            assert rounds.tolist() == first[1].tolist() and inl.tolist() == first[2].tolist(), tag
+            assert np.abs(got - first[0]).max() < 1e-9, (tag, np.abs(got - first[0]).max())
+    finally:
+        ctx.set_option("refine_group", 0)
+        ctx.set_option("refine_compact", 1)
+        ctx.set_option("refine_pretest", 1)
+        ctx.set_option("refine_jobs_per_group", 3)
+    assert max(r[3] for r in ref) >= 1 and min(r[2] for r in ref) > 4       # every job was refined
+    if name == "60x80-sub8":
+        assert walks == {"shared-list", "global-list", "cached-all-cells", "all-cells"}, walks

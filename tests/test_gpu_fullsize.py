@@ -116,10 +116,11 @@ def test_split_upload_of_host_maps_changes_nothing(api, kw):
 
 
 def test_refinement_code_paths_agree_at_full_resolution(api):
-    """The refinement kernel has three ways to walk a CTA's share of the map: cells + inlier list in shared memory (share <= 96
-    words: a 148-CTA group), inlier list in global scratch (<= 2048 words), and predicated passes over all cells
-    (larger shares).  Forcing the group size selects each of them at 480x640; rounds and inlier counts must be identical and the
-    poses equal up to the summation order (1e-9)."""
+    """The refinement kernel has three ways to walk a CTA's share of the map's 32-cell mask words: cells + inlier list in
+    shared memory (share <= 96 words), inlier list in global scratch (<= 2048 words), and predicated passes over all cells
+    (larger shares, or refine_compact = 0).  Forcing the group size selects each of them at 480x640 (9600 words); the largest
+    group is every co-resident CTA, as last_stats() reports it.  Rounds and inlier counts must be identical and the poses equal
+    up to the summation order (1e-9)."""
     sc = make_scene(E=1, H=480, W=640, M=6, sub=1, seed=21, outlier_frac=0.4)
     import cv2
     rng = np.random.default_rng(21)
@@ -129,16 +130,34 @@ def test_refinement_code_paths_agree_at_full_resolution(api):
         dR, _ = cv2.Rodrigues(rng.normal(0, 0.003, 3))
         poses6[h, :3] = cv2.Rodrigues(dR @ T[:3, :3])[0].ravel()
         poses6[h, 3:] = dR @ T[:3, 3] + rng.normal(0, 0.01, 3)
+    words = (480 * 640 + 31) // 32
+    share = lambda g: -(-words // g)                                 # noqa: E731
     ctx = api.context()
     outs = {}
+
+    def run(grp, compact):
+        ctx.set_option("refine_group", grp)
+        ctx.set_option("refine_compact", compact)
+        res = api.refine_poses(sc.coords, sc.assign, poses6, sc.shiftX, sc.shiftY, sc.f, sc.ppx, sc.ppy, sc.tau, sc.max_reproj, sc.sub)
+        return res, api.last_stats()["refine_group"]
+
     try:
-        for grp in (148, 16, 2):   # 148: 65 words per CTA (shared-memory lists); 16: 600 words (global lists); 2: 4800 words (no lists)
-            ctx.set_option("refine_group", grp)
-            outs[grp] = api.refine_poses(sc.coords, sc.assign, poses6, sc.shiftX, sc.shiftY, sc.f, sc.ppx, sc.ppy, sc.tau, sc.max_reproj, sc.sub)
+        res, g_max = run(1 << 20, 1)
+        assert share(g_max) <= 96, (g_max, share(g_max))            # shared-memory lists need every co-resident CTA
+        outs["shared-list"] = res
+        g_list = -(-words // 1024)                                      # ~1024 words per CTA: global lists
+        g_all = 2                                                       # 4800 words per CTA: no lists
+        assert 96 < share(g_list) <= 2048 and share(g_all) > 2048
+        for walk, grp, compact in (("global-list", g_list, 1), ("all-cells", g_all, 1), ("cached-all-cells", g_max, 0),
+                                   ("all-cells-uncompacted", g_list, 0)):
+            outs[walk], g = run(grp, compact)
+            assert g == grp, (walk, g, grp)
     finally:
         ctx.set_option("refine_group", 0)
-    assert outs[148][1].max() >= 1 and outs[148][2].min() > 1000
-    for grp in (16, 2):
-        assert outs[grp][1].tolist() == outs[148][1].tolist()
-        assert outs[grp][2].tolist() == outs[148][2].tolist()
-        assert np.abs(outs[grp][0] - outs[148][0]).max() < 1e-9
+        ctx.set_option("refine_compact", 1)
+    base = outs["shared-list"]
+    assert base[1].max() >= 1 and base[2].min() > 1000
+    for walk, o in outs.items():
+        assert o[1].tolist() == base[1].tolist(), walk
+        assert o[2].tolist() == base[2].tolist(), walk
+        assert np.abs(o[0] - base[0]).max() < 1e-9, walk

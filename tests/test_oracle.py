@@ -57,6 +57,68 @@ def test_c_restatement_matches_cv2_oracle_scores(kw):
     assert np.abs(got - ref).max() < 1e-10
 
 
+def _score_pin_poses(sc, seed):
+    """Sampled hypotheses (near the truth on the ground-truth plane) followed by arbitrary poses (cells behind the camera,
+    far off the image): every branch of the projection and the clamp."""
+    K = O.cam_mat(sc.f, sc.ppx, sc.ppy)
+    H, W = sc.coords.shape[2:]
+    samp = O.create_sampling(W, H, sc.sub, sc.shiftX, sc.shiftY)
+    hyps = O.sample_hypotheses(sc.coords, sc.assign, samp, K, 10000, sc.tau, seed)
+    p6 = np.array([np.concatenate([h.rvec.ravel(), h.tvec.ravel()]) for h in hyps])
+    rng = np.random.default_rng(seed)
+    k = len(p6) // 3
+    p6[-k:, :3] = rng.normal(0, 0.5, (k, 3))
+    p6[-k:, 3:] = p6[-k:, 3:] + rng.normal(0, 2.0, (k, 3)) * (1.0 + np.abs(p6[-k:, 3:]).max(axis=1, keepdims=True) * 1e-2)
+    return K, samp, p6
+
+
+@pytest.mark.parametrize("kw", [
+    dict(E=2, H=24, W=31, M=12, sub=8, seed=7),
+    dict(E=2, H=21, W=29, M=12, sub=3, seed=8, shiftX=-4, shiftY=-7),           # odd sub-sampling, negative shifts
+    dict(E=3, H=20, W=26, M=15, sub=4, seed=9, shiftX=3, shiftY=-5, world_offset=700.0),
+    dict(E=1, H=16, W=20, M=9, sub=8, seed=10, outdoor=True, unit_scale=1000.0),  # world scale in millimetres
+])
+def test_fp64_score_reference_matches_both_oracles(kw):
+    """oracle/score_fp64.py (the reference the GPU launch-shape tests compare with) against the cv2 oracle and the C
+    restatement: the scores agree to 1e-5, and so does every cell's soft-inlier weight wherever cv2's float32 error is not
+    within float rounding of maxReproj (there the fp64 clamp and the float one may fall on different sides)."""
+    from oracle import score_fp64
+    sc = make_scene(**kw)
+    K, samp, p6 = _score_pin_poses(sc, kw["seed"])
+    ref64, w64 = score_fp64.score(sc.coords, sc.assign, p6, *sc.params)
+    errs = [O.get_repro_errs(sc.coords, p[:3].reshape(3, 1), p[3:].reshape(3, 1), int(sc.assign[i]), samp, K, sc.max_reproj)[0]
+            for i, p in enumerate(p6)]
+    cv = np.array(O.get_hyp_scores(errs, sc.tau, sc.alpha, sc.beta))
+    cs, _ = c_score(sc.coords, sc.assign, p6, *sc.params)
+    assert np.isfinite(cv).all()
+    assert np.abs(ref64 - cv).max() < 1e-5, np.abs(ref64 - cv).max()
+    assert np.abs(ref64 - cs).max() < 1e-5, np.abs(ref64 - cs).max()
+    e32 = np.stack(errs).astype(np.float64)
+    w_cv = score_fp64.soft_inlier_weights(e32, sc.tau, sc.beta)
+    ok = np.isfinite(e32) & (np.abs(e32 - sc.max_reproj) > 1e-3)
+    assert ok.sum() >= 0.2 * ok.size and (e32[ok] < sc.tau).sum() >= 10    # the comparison covers inliers as well as outliers
+    assert np.abs(w64[ok] - w_cv[ok]).max() < 1e-5, np.abs(w64[ok] - w_cv[ok]).max()
+
+
+def test_fp64_score_reference_rules_for_degenerate_cells():
+    """A cell at depth exactly 0 projects with z = 1 (OpenCV's `z ? 1/z : 1`); a non-finite cell counts as maxReproj."""
+    from oracle import score_fp64
+    coords = np.zeros((1, 3, 2, 3), np.float32)
+    coords[0, :, 0, 1] = [0.01, -0.02, 0.0]            # camera frame (identity pose): z = 0 -> projects to pp + f (x, y)
+    coords[0, :, 1, 0] = [np.nan, 0.0, 1.0]
+    coords[0, :, 1, 1] = [0.0, 0.0, -2.0]              # behind the camera, on the optical axis: the principal point
+    coords[0, 2, 0, 0] = coords[0, 2, 0, 2] = coords[0, 2, 1, 2] = 1.0
+    f, ppx, ppy, sub = 100.0, 7.0, 5.0, 3
+    errs = score_fp64.repro_errs(coords, [0], np.zeros((1, 6)), 0, 0, f, ppx, ppy, 100.0, sub)[0]
+    px, py = score_fp64.pixel_centres(2, 3, sub, 0, 0)
+    assert px[0].tolist() == [1, 4, 7] and py[:, 0].tolist() == [1, 4]
+    assert errs[0, 1] == pytest.approx(np.hypot(ppx + f * 0.01 - 4, ppy - f * 0.02 - 1), abs=1e-12)
+    assert errs[1, 0] == 100.0
+    assert errs[1, 1] == pytest.approx(np.hypot(ppx - 4, ppy - 4), abs=1e-12)
+    w = score_fp64.soft_inlier_weights(np.array([-1e9, 10.0, 1e9]), 10.0, 0.5)
+    assert w.tolist() == [1.0, 0.5, 0.0]
+
+
 def test_softmax_entropy_draw():
     p = O.softmax([1.0, 3.0, 3.0, 2.0])
     assert abs(p.sum() - 1) < 1e-15 and O.draw(p) == 1  # first strict maximum

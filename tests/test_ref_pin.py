@@ -30,7 +30,7 @@ def gold():
 def ref():
     mod = load_ref()
     if mod is None:
-        pytest.skip("oracle/_ref is not built and $ESAC_REFERENCE names no readable reference checkout")
+        pytest.skip("oracle/_ref is not built and no readable reference checkout was found (oracle/build_ref.py)")
     mod.set_num_threads(1)
     mod.set_native_project(False)
     return mod

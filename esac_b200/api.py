@@ -78,10 +78,17 @@ def load_library() -> C.CDLL:
     lib.esacb200_backward_batch.argtypes = ([vp, i32, vp, vp, i32, i32, i32, vp, i64, i32, vp, f32, f32, f32, vp, vp] + cam[2:] +
                                              [vp])
     lib.esacb200_backward_batch.restype = i32
+    cams = [vp, vp, vp, vp, vp, f32, f32, f32, f32, i32]  # per-image shiftX, shiftY, f, ppx, ppy; then tau .. subSampling
+    lib.esacb200_forward_batch_cameras.argtypes = [vp, i32, vp, i32, i32, i32, vp, i64, i32, vp] + cams + [vp]
+    lib.esacb200_forward_batch_cameras.restype = i32
+    lib.esacb200_backward_batch_cameras.argtypes = [vp, i32, vp, vp, i32, i32, i32, vp, i64, i32, vp, f32, f32, f32] + cams + [vp]
+    lib.esacb200_backward_batch_cameras.restype = i32
     lib.esacb200_assign_hypotheses.argtypes = [vp, i32, i32, i32, vp, i32, i32, C.c_uint64, vp, vp]
     lib.esacb200_assign_hypotheses.restype = i32
     lib.esacb200_reproj_loss.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp, f32, f32, f32, i32, f32, f32, f32, vp]
     lib.esacb200_reproj_loss.restype = i32
+    lib.esacb200_reproj_loss_cameras.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, f32, f32, f32, vp]
+    lib.esacb200_reproj_loss_cameras.restype = i32
     lib.esacb200_backward_sharded.argtypes = ([vp, vp, vp, i32, i32, i32, vp, i64, i32, vp, f32, f32, f32] + cam +
                                                [EXCHANGE_FN, vp, C.POINTER(f64)])
     lib.esacb200_backward_sharded.restype = i32
@@ -341,6 +348,26 @@ def _assign_arg(t):
     return a.ctypes.data, stride, M, None, a
 
 
+def _is_number(v) -> bool:
+    """A Python / numpy number or a 0-d array or tensor: one value for the whole batch."""
+    return (v.dim() == 0) if _is_torch(v) else np.ndim(v) == 0
+
+
+def _per_image(v, B: int, dtype, what: str) -> np.ndarray:
+    """A batch argument as B contiguous host values of `dtype`: a number is broadcast; a sequence, numpy array or tensor
+    (CPU or CUDA) must hold B values.  float64 values (a DataLoader's focal lengths) round to float32 exactly as ctypes
+    rounds a Python float.  Raises RuntimeError before any context exists, so the check runs without a GPU."""
+    if _is_number(v):
+        v = [int(v) if dtype == np.int32 else float(v)] * B
+    elif _is_torch(v):
+        v = v.detach().cpu().numpy()
+    a = np.ascontiguousarray(np.asarray(v).reshape(-1), dtype=dtype)
+    if a.shape[0] != B:
+        kind = "an int or {} ints" if dtype == np.int32 else "a number or {} numbers"
+        raise RuntimeError(f"{what} must be {kind.format(B)}, got {a.shape[0]} values")
+    return a
+
+
 _CUDA_STREAM_LEGACY = 0x1
 
 
@@ -473,23 +500,37 @@ def forward_batch(sceneCoordinates, hypAssignment, outPoses, shiftX, shiftY, foc
                   inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling) -> list:
     """esac.forward over a batch: sceneCoordinates [B,E,3,H,W] float32, hypAssignment [B,M] int64 (contiguous rows),
     outPoses [B,4,4] float32 written in place.  Returns the winning expert of every image.  One host synchronisation
-    for the whole batch; host tensors (pinned) are copied on a second stream while the previous image computes."""
+    for the whole batch; host tensors (pinned) are copied on a second stream while the previous image computes.
+    shiftX, shiftY, focalLength, ppointX and ppointY are each a number (one camera for the batch) or B values -- a
+    sequence, numpy array or 1-D tensor, e.g. the DataLoader's `focallength` -- giving image b its own shift and camera;
+    image b then computes what esac.forward with those values computes."""
     _check(sceneCoordinates, "Float", 5, "sceneCoordinates")
     _check(hypAssignment, "Long", 2, "hypAssignment")
     _check(outPoses, "Float", 3, "outPoses")
     B, E, C3, H, W = (int(v) for v in sceneCoordinates.shape)
     if C3 != 3 or tuple(outPoses.shape) != (B, 4, 4) or int(hypAssignment.shape[0]) != B:
         raise RuntimeError("shapes must be [B,E,3,H,W], [B,M], [B,4,4]")
+    one_camera = all(_is_number(v) for v in (shiftX, shiftY, focalLength, ppointX, ppointY))
+    if not one_camera:
+        sx, sy = _per_image(shiftX, B, np.int32, "shiftX"), _per_image(shiftY, B, np.int32, "shiftY")
+        fs = _per_image(focalLength, B, np.float32, "focalLength")
+        cx, cy = _per_image(ppointX, B, np.float32, "ppointX"), _per_image(ppointY, B, np.float32, "ppointY")
     co = _Arg(sceneCoordinates)
     op = _Arg(outPoses, writable=True)
     ha = _Arg(hypAssignment)
     M = int(hypAssignment.shape[1])
     ctx = _pick_ctx(co.device, op.device, ha.device)
     experts = (C.c_int * B)()
-    ctx.check(ctx.lib.esacb200_forward_batch(ctx.handle, B, co.ptr, E, H, W, ha.ptr, 1, M, op.ptr, int(shiftX), int(shiftY),
-                                             float(focalLength), float(ppointX), float(ppointY), float(inlierThreshold),
-                                             float(inlierAlpha), float(inlierBeta), float(maxReproj), int(subSampling),
-                                             experts))
+    if one_camera:
+        rc = ctx.lib.esacb200_forward_batch(ctx.handle, B, co.ptr, E, H, W, ha.ptr, 1, M, op.ptr, int(shiftX), int(shiftY),
+                                            float(focalLength), float(ppointX), float(ppointY), float(inlierThreshold),
+                                            float(inlierAlpha), float(inlierBeta), float(maxReproj), int(subSampling), experts)
+    else:
+        rc = ctx.lib.esacb200_forward_batch_cameras(ctx.handle, B, co.ptr, E, H, W, ha.ptr, 1, M, op.ptr, sx.ctypes.data,
+                                                    sy.ctypes.data, fs.ctypes.data, cx.ctypes.data, cy.ctypes.data,
+                                                    float(inlierThreshold), float(inlierAlpha), float(inlierBeta),
+                                                    float(maxReproj), int(subSampling), experts)
+    ctx.check(rc)
     op.finish()
     return [int(e) for e in experts]
 
@@ -498,8 +539,9 @@ def backward_batch(sceneCoordinates, outGradients, hypAssignment, gtPoses, wLoss
                    focalLength, ppointX, ppointY, inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling) -> list:
     """esac.backward over a batch: sceneCoordinates / outGradients [B,E,3,H,W] float32 (gradients accumulated in place),
     hypAssignment [B,M] int64, gtPoses [B,4,4] float32 (camera->world), shiftX / shiftY an int or a sequence of B ints
-    (train_esac.py:125 draws one shift per image).  Returns the expected loss of every image; equal, image by image, to B
-    consecutive esac.backward calls on the same context."""
+    (train_esac.py:125 draws one shift per image), focalLength / ppointX / ppointY a number or B values (one camera per
+    image, as forward_batch).  Returns the expected loss of every image; equal, image by image, to B consecutive
+    esac.backward calls on the same context, each with its image's shift and camera."""
     _check(sceneCoordinates, "Float", 5, "sceneCoordinates")
     _check(outGradients, "Float", 5, "outGradients")
     _check(hypAssignment, "Long", 2, "hypAssignment")
@@ -513,23 +555,21 @@ def backward_batch(sceneCoordinates, outGradients, hypAssignment, gtPoses, wLoss
     ha = _Arg(hypAssignment)
     gt = _Arg(gtPoses)
     M = int(hypAssignment.shape[1])
-
-    def shifts(v):
-        if isinstance(v, (int, float)):
-            v = [int(v)] * B
-        a = np.ascontiguousarray(np.asarray(v, dtype=np.int32).reshape(-1))
-        if a.shape[0] != B:
-            raise RuntimeError(f"shift must be an int or {B} ints")
-        return a
-
-    sx, sy = shifts(shiftX), shifts(shiftY)
+    sx, sy = _per_image(shiftX, B, np.int32, "shiftX"), _per_image(shiftY, B, np.int32, "shiftY")
+    one_camera = all(_is_number(v) for v in (focalLength, ppointX, ppointY))
+    if not one_camera:
+        fs = _per_image(focalLength, B, np.float32, "focalLength")
+        cx, cy = _per_image(ppointX, B, np.float32, "ppointX"), _per_image(ppointY, B, np.float32, "ppointY")
     ctx = _pick_ctx(co.device, og.device, ha.device, gt.device)
     losses = np.zeros(B, np.float64)
-    ctx.check(ctx.lib.esacb200_backward_batch(ctx.handle, B, co.ptr, og.ptr, E, H, W, ha.ptr, 1, M, gt.ptr, float(wLossRot),
-                                              float(wLossTrans), float(lossCut), sx.ctypes.data, sy.ctypes.data,
-                                              float(focalLength), float(ppointX), float(ppointY), float(inlierThreshold),
-                                              float(inlierAlpha), float(inlierBeta), float(maxReproj), int(subSampling),
-                                              losses.ctypes.data))
+    head = (ctx.handle, B, co.ptr, og.ptr, E, H, W, ha.ptr, 1, M, gt.ptr, float(wLossRot), float(wLossTrans), float(lossCut),
+            sx.ctypes.data, sy.ctypes.data)
+    tail = (float(inlierThreshold), float(inlierAlpha), float(inlierBeta), float(maxReproj), int(subSampling), losses.ctypes.data)
+    if one_camera:
+        rc = ctx.lib.esacb200_backward_batch(*head, float(focalLength), float(ppointX), float(ppointY), *tail)
+    else:
+        rc = ctx.lib.esacb200_backward_batch_cameras(*head, fs.ctypes.data, cx.ctypes.data, cy.ctypes.data, *tail)
+    ctx.check(rc)
     og.finish()
     return [float(v) for v in losses]
 
@@ -563,8 +603,9 @@ def reproj_loss(prediction, gtPoses, focalLength, padX, padY, cutLoss, subSampli
     """The robust reprojection loss of ref_expert.py:103-148 and, when outGradients is given, d loss / d prediction in the
     same pass (what `robust_loss.backward()` hands to the expert, ref_expert.py:150).  prediction [B,3,H,W] float32 (the
     reference has B = 1), gtPoses [B,4,4] float32 camera->world, padX / padY an int or B ints (the random shift),
-    outGradients [B,3,H,W] float32 written in place (overwritten) or None.  The principal point defaults to the centre of
-    the sub*W x sub*H image (ref_expert.py:118-119).  Returns the B losses."""
+    outGradients [B,3,H,W] float32 written in place (overwritten) or None.  focalLength, ppointX and ppointY are a number
+    or B values (one camera per image, e.g. the DataLoader's `focallength`); the principal point defaults to the centre
+    of the sub*W x sub*H image (ref_expert.py:118-119).  Returns the B losses."""
     _check(prediction, "Float", 4, "prediction")
     _check(gtPoses, "Float", 3, "gtPoses")
     B, C3, H, W = (int(v) for v in prediction.shape)
@@ -579,22 +620,22 @@ def reproj_loss(prediction, gtPoses, focalLength, padX, padY, cutLoss, subSampli
             raise RuntimeError("outGradients must have the shape of prediction")
         og = _Arg(outGradients, writable=True)
 
-    def shifts(v):
-        if isinstance(v, (int, float)):
-            v = [int(v)] * B
-        a = np.ascontiguousarray(np.asarray(v, dtype=np.int32).reshape(-1))
-        if a.shape[0] != B:
-            raise RuntimeError(f"pad must be an int or {B} ints")
-        return a
-
-    sx, sy = shifts(padX), shifts(padY)
-    ppx = float(W * subSampling / 2 if ppointX is None else ppointX)
-    ppy = float(H * subSampling / 2 if ppointY is None else ppointY)
+    sx, sy = _per_image(padX, B, np.int32, "padX"), _per_image(padY, B, np.int32, "padY")
+    ppx = W * subSampling / 2 if ppointX is None else ppointX
+    ppy = H * subSampling / 2 if ppointY is None else ppointY
+    one_camera = all(_is_number(v) for v in (focalLength, ppx, ppy))
+    if not one_camera:
+        fs = _per_image(focalLength, B, np.float32, "focalLength")
+        cx, cy = _per_image(ppx, B, np.float32, "ppointX"), _per_image(ppy, B, np.float32, "ppointY")
     ctx = _pick_ctx(pr.device, gt.device, og.device if og else None)
     losses = np.zeros(B, np.float64)
-    ctx.check(ctx.lib.esacb200_reproj_loss(ctx.handle, B, pr.ptr, og.ptr if og else None, H, W, gt.ptr, sx.ctypes.data,
-                                           sy.ctypes.data, float(focalLength), ppx, ppy, int(subSampling), float(cutLoss),
-                                           float(maxReproj), float(minDepth), losses.ctypes.data))
+    head = (ctx.handle, B, pr.ptr, og.ptr if og else None, H, W, gt.ptr, sx.ctypes.data, sy.ctypes.data)
+    tail = (int(subSampling), float(cutLoss), float(maxReproj), float(minDepth), losses.ctypes.data)
+    if one_camera:
+        rc = ctx.lib.esacb200_reproj_loss(*head, float(focalLength), float(ppx), float(ppy), *tail)
+    else:
+        rc = ctx.lib.esacb200_reproj_loss_cameras(*head, fs.ctypes.data, cx.ctypes.data, cy.ctypes.data, *tail)
+    ctx.check(rc)
     if og:
         og.finish()
     return [float(v) for v in losses]

@@ -49,6 +49,54 @@ def esac_loss(scene_coordinates, gating_log_probs, hyp_assignment, gt_pose, *par
     return EsacLoss.apply(scene_coordinates, gating_log_probs, hyp_assignment, gt_pose, *params, expert_selection)
 
 
+class EsacLossBatch(torch.autograd.Function):
+    """EsacLoss over a batch of images, on api.backward_batch: forward returns the B expected pose losses, backward hands
+    d loss_b / d scene_coordinates[b] and row b of the gating gradient -- loss_b * histogram(e_hyps[b]), or loss_b at the
+    drawn expert in expert-selection mode -- to autograd, each computed exactly as EsacLoss computes it for one image."""
+
+    @staticmethod
+    def forward(ctx, scene_coordinates, gating_log_probs, hyp_assignment, gt_poses, w_rot, w_trans, loss_cut, shift_x,
+                shift_y, focal_length, ppoint_x, ppoint_y, inlier_threshold, inlier_alpha, inlier_beta, max_reproj,
+                sub_sampling, expert_selection=None):
+        grads = torch.zeros_like(scene_coordinates)
+        losses = api.backward_batch(scene_coordinates.detach(), grads, hyp_assignment, gt_poses, w_rot, w_trans, loss_cut,
+                                    shift_x, shift_y, focal_length, ppoint_x, ppoint_y, inlier_threshold, inlier_alpha,
+                                    inlier_beta, max_reproj, sub_sampling)
+        E = scene_coordinates.shape[1]
+        if expert_selection is None:
+            # [B,1].expand(B,M): a stride-0 row per image, the batched form of expert.expand(M)
+            expert_selection = hyp_assignment.dim() == 2 and hyp_assignment.shape[1] > 1 and hyp_assignment.stride(1) == 0
+        rows = []
+        for b, loss in enumerate(losses):
+            if expert_selection:
+                g = torch.zeros(E)
+                g[int(hyp_assignment[b, 0])] = loss                                      # train_esac.py:171-173
+            else:
+                hist = torch.histc(hyp_assignment[b].float().cpu(), bins=E, min=0, max=E - 1)   # train_esac.py:140
+                g = loss * hist                                                           # train_esac.py:174-176
+            rows.append(g)
+        g_gating = torch.stack(rows).to(gating_log_probs.device).reshape(gating_log_probs.shape)
+        ctx.save_for_backward(grads, g_gating)
+        return scene_coordinates.new_tensor(losses)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        g_coords, g_gating = ctx.saved_tensors
+        B = grad_out.shape[0]
+        return (g_coords * grad_out.reshape((B,) + (1,) * (g_coords.dim() - 1)),
+                g_gating * grad_out.reshape((B,) + (1,) * (g_gating.dim() - 1))) + (None,) * 16
+
+
+def esac_loss_batch(scene_coordinates, gating_log_probs, hyp_assignment, gt_poses, *params, expert_selection=None):
+    """The batched counterpart of esac_loss (one train_esac.py step on B images, each with its own camera):
+    scene_coordinates [B,E,3,H,W], gating_log_probs [B,E], hyp_assignment [B,M], gt_poses [B,4,4]; params the positional
+    tail of api.backward_batch (wLossRot, wLossTrans, lossCut, shiftX, shiftY, focalLength, ppointX, ppointY,
+    inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling), where shifts and camera may be per image.
+    Returns the B expected losses; image b draws the minimal sets of the b-th of B consecutive esac_loss calls.
+    expert_selection as for esac_loss, decided for the whole batch (None: a stride-0 [B,1].expand(B,M) assignment)."""
+    return EsacLossBatch.apply(scene_coordinates, gating_log_probs, hyp_assignment, gt_poses, *params, expert_selection)
+
+
 class ReprojLoss(torch.autograd.Function):
     """ref_expert.py:103-150 as one autograd node: forward = the robust reprojection loss of a batch of predictions
     (mean over the batch of the per-image losses; the reference has one image per step), backward = its gradient, both
@@ -71,5 +119,6 @@ class ReprojLoss(torch.autograd.Function):
 
 def reproj_loss(prediction, gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling=8, ppoint_x=None, ppoint_y=None):
     """Drop-in for the loss block of ref_expert.py: `robust_loss = reproj_loss(prediction, gt_pose, f, padX, padY,
-    opt.cutloss)` followed by `robust_loss.backward()`.  prediction [B,3,H,W] (CUDA), gt_poses [B,4,4] camera->world."""
+    opt.cutloss)` followed by `robust_loss.backward()`.  prediction [B,3,H,W] (CUDA), gt_poses [B,4,4] camera->world.
+    focal_length, pad_x / pad_y and the principal point are a number or B values, so a batch may mix cameras."""
     return ReprojLoss.apply(prediction, gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling, ppoint_x, ppoint_y)

@@ -872,15 +872,18 @@ int esacb200_forward_sharded(esacb200_ctx* ctx, const float* coords, int E, int 
 // esac_forward over a batch of B images of one shape (BASELINE configs[2]: "batch 8 images").  The reference has no such
 // entry: its callers loop over a DataLoader with batch_size=1 (test_esac.py:137).  Images are processed back to back on
 // the compute stream with ONE host synchronisation at the end; host coordinate maps are double-buffered and copied on a
-// second stream so the copy of image b+1 overlaps the kernels of image b.
-int esacb200_forward_batch(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
-                           int64_t assign_stride, int M, float* out_poses, int shiftX, int shiftY, float f, float ppx,
-                           float ppy, float tau, float alpha, float beta, float maxReproj, int sub, int* out_experts) try {
+// second stream so the copy of image b+1 overlaps the kernels of image b.  Image b runs with its own shift and camera:
+// the pipeline of one image reads them from its Problem, so only the loop below sees the arrays.
+int esacb200_forward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
+                                   int64_t assign_stride, int M, float* out_poses, const int* shiftX, const int* shiftY,
+                                   const float* f, const float* ppx, const float* ppy, float tau, float alpha, float beta,
+                                   float maxReproj, int sub, int* out_experts) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     if (!coords || !assign || !out_poses || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
+    if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
     Plan pl;
-    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub);
+    int rc = fill_problem(ctx, pl.P, E, H, W, M, 0, 0, f[0], ppx[0], ppy[0], tau, alpha, beta, maxReproj, sub);
     if (rc) return rc;
     if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small", W, H);
     begin_call(ctx);
@@ -905,6 +908,11 @@ int esacb200_forward_batch(esacb200_ctx* ctx, int B, const float* coords, int E,
         }
         (void)host_assign;
         if (b == 0) mark(ctx, EV_H2D);
+        pl.P.shiftX = shiftX ? shiftX[b] : 0;
+        pl.P.shiftY = shiftY ? shiftY[b] : 0;
+        pl.P.f = f[b];
+        pl.P.ppx = ppx[b];
+        pl.P.ppy = ppy[b];
         rc = plan_and_prep(ctx, pl);
         if (rc) return rc;
         rc = enqueue_forward_core(ctx, pl, ctx->out_batch.as<float>() + (size_t)b * 20);
@@ -932,6 +940,18 @@ int esacb200_forward_batch(esacb200_ctx* ctx, int B, const float* coords, int E,
     ctx->last_backward = false;
     finish_stats(ctx);
     return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+// One camera for the whole batch: broadcast to B entries.
+int esacb200_forward_batch(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
+                           int64_t assign_stride, int M, float* out_poses, int shiftX, int shiftY, float f, float ppx,
+                           float ppy, float tau, float alpha, float beta, float maxReproj, int sub, int* out_experts) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    const size_t n = B > 0 ? (size_t)B : 1;  // B <= 0 is rejected by the call below, with its usual message
+    const std::vector<int> sx(n, shiftX), sy(n, shiftY);
+    const std::vector<float> fs(n, f), cx(n, ppx), cy(n, ppy);
+    return esacb200_forward_batch_cameras(ctx, B, coords, E, H, W, assign, assign_stride, M, out_poses, sx.data(), sy.data(),
+                                          fs.data(), cx.data(), cy.data(), tau, alpha, beta, maxReproj, sub, out_experts);
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
@@ -1301,13 +1321,15 @@ int esacb200_backward_sharded_nccl(esacb200_ctx* ctx, const float* coords, float
 // esac_backward over a batch.  Every image is an independent problem (SURVEY 8e: "images in a batch are fully
 // independent"), so the images are dealt round-robin to a few worker contexts, each driven by its own host thread on its
 // own stream: the small kernels of one image fill the gaps the host synchronisations of another leave.
-int esacb200_backward_batch(esacb200_ctx* ctx, int B, const float* coords, float* grads, int E, int H, int W,
-                            const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wRot,
-                            float wTrans, float cut, const int* shiftX, const int* shiftY, float f, float ppx, float ppy,
-                            float tau, float alpha, float beta, float maxReproj, int sub, double* out_losses) try {
+int esacb200_backward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords, float* grads, int E, int H, int W,
+                                    const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wRot,
+                                    float wTrans, float cut, const int* shiftX, const int* shiftY, const float* f,
+                                    const float* ppx, const float* ppy, float tau, float alpha, float beta, float maxReproj,
+                                    int sub, double* out_losses) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     if (!coords || !grads || !assign || !gt_poses || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
+    if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
     if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
     if (E <= 0 || H <= 0 || W <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d H=%d W=%d M=%d", E, H, W, M);
     const size_t cstride = (size_t)E * 3 * H * W;
@@ -1355,7 +1377,8 @@ int esacb200_backward_batch(esacb200_ctx* ctx, int B, const float* coords, float
             double loss = 0;
             int rc = backward_impl(w, coords + (size_t)b * cstride, grads + (size_t)b * cstride, E, H, W, assign + (size_t)b * arow,
                                    assign_stride, M, gt + (size_t)b * 16, wRot, wTrans, cut, shiftX ? shiftX[b] : 0,
-                                   shiftY ? shiftY[b] : 0, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, nullptr, nullptr, &loss);
+                                   shiftY ? shiftY[b] : 0, f[b], ppx[b], ppy[b], tau, alpha, beta, maxReproj, sub, nullptr, nullptr,
+                                   &loss);
             if (rc) { rcs[wi] = rc; failed_at[wi] = b; return; }
             if (out_losses) out_losses[b] = loss;
             launches[wi] += w->st.kernel_launches;
@@ -1387,6 +1410,18 @@ int esacb200_backward_batch(esacb200_ctx* ctx, int B, const float* coords, float
     ctx->last_M = 0;  // the per-hypothesis buffers live in the workers
     ctx->last_backward = true;
     return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_backward_batch(esacb200_ctx* ctx, int B, const float* coords, float* grads, int E, int H, int W,
+                            const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wRot,
+                            float wTrans, float cut, const int* shiftX, const int* shiftY, float f, float ppx, float ppy,
+                            float tau, float alpha, float beta, float maxReproj, int sub, double* out_losses) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    const size_t n = B > 0 ? (size_t)B : 1;  // B <= 0 is rejected by the call below, with its usual message
+    const std::vector<float> fs(n, f), cx(n, ppx), cy(n, ppy);
+    return esacb200_backward_batch_cameras(ctx, B, coords, grads, E, H, W, assign, assign_stride, M, gt_poses, wRot, wTrans, cut,
+                                           shiftX, shiftY, fs.data(), cx.data(), cy.data(), tau, alpha, beta, maxReproj, sub,
+                                           out_losses);
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
@@ -1424,12 +1459,13 @@ int esacb200_assign_hypotheses(esacb200_ctx* ctx, int B, int E, int M, const flo
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
-int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* grads, int H, int W, const float* gt_poses,
-                         const int* shiftX, const int* shiftY, float f, float ppx, float ppy, int sub, float cut,
-                         float maxReproj, float minDepth, double* out_losses) try {
+int esacb200_reproj_loss_cameras(esacb200_ctx* ctx, int B, const float* coords, float* grads, int H, int W, const float* gt_poses,
+                                 const int* shiftX, const int* shiftY, const float* f, const float* ppx, const float* ppy, int sub,
+                                 float cut, float maxReproj, float minDepth, double* out_losses) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     if (!coords || !gt_poses || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
     if (B <= 0 || H <= 0 || W <= 0 || sub <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d H=%d W=%d sub=%d", B, H, W, sub);
     if ((long long)H * W > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too large", W, H);
     begin_call(ctx);
@@ -1455,7 +1491,7 @@ int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* g
         memcpy(gt.data(), gt_poses, gt.size() * sizeof(float));
     }
     // world->camera rows: inverse of the affine camera->world matrix (torch's .inverse()[0:3,:], ref_expert.py:127)
-    std::vector<float> img((size_t)B * 16, 0.f);
+    std::vector<float> img((size_t)B * kReprojImgFloats, 0.f);
     for (int b = 0; b < B; ++b) {
         const float* T = gt.data() + (size_t)b * 16;
         double A[9], inv[9];
@@ -1466,17 +1502,20 @@ int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* g
         inv[0] = (A[4] * A[8] - A[5] * A[7]) / det; inv[1] = (A[2] * A[7] - A[1] * A[8]) / det; inv[2] = (A[1] * A[5] - A[2] * A[4]) / det;
         inv[3] = (A[5] * A[6] - A[3] * A[8]) / det; inv[4] = (A[0] * A[8] - A[2] * A[6]) / det; inv[5] = (A[2] * A[3] - A[0] * A[5]) / det;
         inv[6] = (A[3] * A[7] - A[4] * A[6]) / det; inv[7] = (A[1] * A[6] - A[0] * A[7]) / det; inv[8] = (A[0] * A[4] - A[1] * A[3]) / det;
-        float* o = img.data() + (size_t)b * 16;
+        float* o = img.data() + (size_t)b * kReprojImgFloats;
         for (int r = 0; r < 3; ++r) {
             for (int c = 0; c < 3; ++c) o[r * 4 + c] = (float)inv[r * 3 + c];
             o[r * 4 + 3] = (float)-(inv[r * 3] * T[3] + inv[r * 3 + 1] * T[7] + inv[r * 3 + 2] * T[11]);
         }
         o[12] = shiftX ? (float)shiftX[b] : 0.f;
         o[13] = shiftY ? (float)shiftY[b] : 0.f;
+        o[14] = f[b];
+        o[15] = ppx[b];
+        o[16] = ppy[b];
     }
     const int bpi = reproj_blocks_per_image(N, B, ctx->sm_count);
-    // scratch layout: [tickets B u32, padded] [img B*16 f32] [losses B f64] [partials B*bpi f64]
-    const size_t off_img = ((size_t)B * 4 + 63) & ~(size_t)63, off_loss = off_img + (size_t)B * 64,
+    // scratch layout: [tickets B u32, padded] [img B*kReprojImgFloats f32] [losses B f64] [partials B*bpi f64]
+    const size_t off_img = ((size_t)B * 4 + 63) & ~(size_t)63, off_loss = off_img + (((size_t)B * kReprojImgFloats * 4 + 63) & ~(size_t)63),
                  off_part = off_loss + (((size_t)B * 8 + 63) & ~(size_t)63);
     CK(ctx->scratch.ensure(off_part + (size_t)B * bpi * 8));
     char* base = (char*)ctx->scratch.p;
@@ -1484,7 +1523,7 @@ int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* g
     CK(cudaMemcpyAsync(base + off_img, img.data(), img.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
     mark(ctx, EV_H2D);
     mark(ctx, EV_FOLD);  // ms_score = the kernel alone
-    launch_reproj(d_coords, d_grads, (const float*)(base + off_img), B, N, W, (float)sub, f, ppx, ppy, cut, maxReproj, minDepth, bpi,
+    launch_reproj(d_coords, d_grads, (const float*)(base + off_img), B, N, W, (float)sub, cut, maxReproj, minDepth, bpi,
                   (double*)(base + off_part), (unsigned*)base, (double*)(base + off_loss), ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 1;
@@ -1497,6 +1536,16 @@ int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* g
     ctx->last_M = 0;
     finish_stats(ctx);
     return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* grads, int H, int W, const float* gt_poses,
+                         const int* shiftX, const int* shiftY, float f, float ppx, float ppy, int sub, float cut,
+                         float maxReproj, float minDepth, double* out_losses) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    const size_t n = B > 0 ? (size_t)B : 1;  // B <= 0 is rejected by the call below, with its usual message
+    const std::vector<float> fs(n, f), cx(n, ppx), cy(n, ppy);
+    return esacb200_reproj_loss_cameras(ctx, B, coords, grads, H, W, gt_poses, shiftX, shiftY, fs.data(), cx.data(), cy.data(), sub,
+                                        cut, maxReproj, minDepth, out_losses);
 } ESAC_ABI_CATCH(ctx)
 
 int esacb200_copy_last_scores(esacb200_ctx* ctx, double* dst, int M) try {

@@ -169,11 +169,12 @@ void launch_assign(const float* weights, int B, int E, int M, int keep_top, int 
 
 // --- reproj.cu ----------------------------------------------------------------------------
 int reproj_blocks_per_image(int N, int B, int sm_count);
-// img: per image 16 floats = world->camera 3x4 (row major), padX, padY, 2 unused.  partial: B * blocks_per_image doubles,
-// tickets: B zeroed counters (left zeroed), losses: B doubles.  grads may be null (loss only).
-void launch_reproj(const float* coords, float* grads, const float* img, int B, int N, int W, float sub, float f, float cx,
-                   float cy, float cut, float max_err, float min_depth, int blocks_per_image, double* partial,
-                   unsigned* tickets, double* losses, cudaStream_t stream);
+// img: per image kReprojImgFloats floats = world->camera 3x4 (row major), padX, padY, f, cx, cy, 3 unused.  partial:
+// B * blocks_per_image doubles, tickets: B zeroed counters (left zeroed), losses: B doubles.  grads may be null (loss only).
+constexpr int kReprojImgFloats = 20;
+void launch_reproj(const float* coords, float* grads, const float* img, int B, int N, int W, float sub, float cut,
+                   float max_err, float min_depth, int blocks_per_image, double* partial, unsigned* tickets, double* losses,
+                   cudaStream_t stream);
 
 // --- bwd.cu -------------------------------------------------------------------------------
 struct BwdArgs {

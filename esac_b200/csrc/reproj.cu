@@ -135,18 +135,17 @@ __device__ __forceinline__ PairOut reproj_pair(float2 X, float2 Y, float2 Z, con
     return o;
 }
 
-// grid = (blocks_per_image, B).  img[b] = 12 matrix entries, padX, padY, 2 unused.
+// grid = (blocks_per_image, B).  img[b] = kReprojImgFloats floats: 12 matrix entries, padX, padY, f, cx, cy, 3 unused.
 template <bool VEC>
 __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const float* __restrict__ coords, float* __restrict__ grads,
-                                                          const float* __restrict__ img, int N, int W, float sub, float f,
-                                                          float cx, float cy, float cut, float max_err, float min_depth,
-                                                          double* __restrict__ partial, unsigned* __restrict__ tickets,
-                                                          double* __restrict__ losses) {
-    __shared__ float m[16];
+                                                          const float* __restrict__ img, int N, int W, float sub, float cut,
+                                                          float max_err, float min_depth, double* __restrict__ partial,
+                                                          unsigned* __restrict__ tickets, double* __restrict__ losses) {
+    __shared__ float m[kReprojImgFloats];
     __shared__ double warp_sum[kThreads / 32];
     __shared__ bool last;
     const int b = blockIdx.y;
-    if (threadIdx.x < 16) m[threadIdx.x] = img[b * 16 + threadIdx.x];
+    if (threadIdx.x < kReprojImgFloats) m[threadIdx.x] = img[b * kReprojImgFloats + threadIdx.x];
     __syncthreads();
     const float* px = coords + (size_t)b * 3 * N;
     const float* py = px + N;
@@ -159,7 +158,8 @@ __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const float* __rest
     if (VEC) {
 #pragma unroll
         for (int i = 0; i < 12; ++i) kc.m[i] = bc(m[i]);
-        kc.f = bc(f); kc.cx = bc(cx); kc.cy = bc(cy); kc.cut = bc(cut); kc.half_cut = bc(0.5f * cut); kc.inv_n = bc(inv_n);
+        kc.f = bc(m[14]); kc.cx = bc(m[15]); kc.cy = bc(m[16]);   // this image's camera
+        kc.cut = bc(cut); kc.half_cut = bc(0.5f * cut); kc.inv_n = bc(inv_n);
         kc.max_err = max_err; kc.min_depth = min_depth; kc.cut_s = cut;
     }
     double acc = 0.;
@@ -214,25 +214,23 @@ __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const float* __rest
             for (int i = 0; i < 4; ++i) {
                 const float tx = fmaf((float)x, sub, half) - padX;
                 const float ty = fmaf((float)y, sub, half) - padY;
-                const CellOut o = reproj_cell(X[i], Y[i], Z[i], m, f, cx, cy, tx, ty, cut, max_err, min_depth, inv_n);
-                if (i < n) four += o.loss;
-                ox[i] = o.gx; oy[i] = o.gy; oz[i] = o.gz;
+                const CellOut o = reproj_cell(X[i], Y[i], Z[i], m, m[14], m[15], m[16], tx, ty, cut, max_err, min_depth, inv_n);
+                if (i < n) {
+                    four += o.loss;
+                    if (gx) {   // stored as computed: no gradient array stays live across the four cells
+                        gx[p0 + i] = o.gx;
+                        gx[N + p0 + i] = o.gy;
+                        gx[2 * (size_t)N + p0 + i] = o.gz;
+                    }
+                }
                 if (++x == W) { x = 0; ++y; }
             }
         }
         acc += (double)four;
-        if (gx) {
-            if (VEC) {
-                __stcs(reinterpret_cast<float4*>(gx + p0), make_float4(ox[0], ox[1], ox[2], ox[3]));
-                __stcs(reinterpret_cast<float4*>(gx + N + p0), make_float4(oy[0], oy[1], oy[2], oy[3]));
-                __stcs(reinterpret_cast<float4*>(gx + 2 * (size_t)N + p0), make_float4(oz[0], oz[1], oz[2], oz[3]));
-            } else {
-                for (int i = 0; i < n; ++i) {
-                    gx[p0 + i] = ox[i];
-                    gx[N + p0 + i] = oy[i];
-                    gx[2 * (size_t)N + p0 + i] = oz[i];
-                }
-            }
+        if (VEC && gx) {
+            __stcs(reinterpret_cast<float4*>(gx + p0), make_float4(ox[0], ox[1], ox[2], ox[3]));
+            __stcs(reinterpret_cast<float4*>(gx + N + p0), make_float4(oy[0], oy[1], oy[2], oy[3]));
+            __stcs(reinterpret_cast<float4*>(gx + 2 * (size_t)N + p0), make_float4(oz[0], oz[1], oz[2], oz[3]));
         }
     }
     // block sum in a fixed order, then the last block of the image adds the partials, again in a fixed order
@@ -279,17 +277,17 @@ int reproj_blocks_per_image(int N, int B, int sm_count) {
     return need < 64 ? need : (need < 256 ? (need + 1) / 2 : (need + 3) / 4);
 }
 
-void launch_reproj(const float* coords, float* grads, const float* img, int B, int N, int W, float sub, float f, float cx,
-                   float cy, float cut, float max_err, float min_depth, int blocks_per_image, double* partial,
-                   unsigned* tickets, double* losses, cudaStream_t stream) {
+void launch_reproj(const float* coords, float* grads, const float* img, int B, int N, int W, float sub, float cut,
+                   float max_err, float min_depth, int blocks_per_image, double* partial, unsigned* tickets, double* losses,
+                   cudaStream_t stream) {
     const dim3 grid(blocks_per_image, B);
     const bool vec = (N % 4 == 0) && W >= 4 && ((uintptr_t)coords % 16 == 0) && (!grads || (uintptr_t)grads % 16 == 0);
     if (vec)
-        reproj_kernel<true><<<grid, kThreads, 0, stream>>>(coords, grads, img, N, W, sub, f, cx, cy, cut, max_err, min_depth,
-                                                           partial, tickets, losses);
+        reproj_kernel<true><<<grid, kThreads, 0, stream>>>(coords, grads, img, N, W, sub, cut, max_err, min_depth, partial,
+                                                           tickets, losses);
     else
-        reproj_kernel<false><<<grid, kThreads, 0, stream>>>(coords, grads, img, N, W, sub, f, cx, cy, cut, max_err, min_depth,
-                                                            partial, tickets, losses);
+        reproj_kernel<false><<<grid, kThreads, 0, stream>>>(coords, grads, img, N, W, sub, cut, max_err, min_depth, partial,
+                                                            tickets, losses);
 }
 
 }  // namespace esacb200

@@ -49,7 +49,7 @@ class Scene:
 
 def make_scene(E=1, H=60, W=80, M=64, sub=8, seed=0, outlier_frac=0.4, noise=0.02, f=525.0,
                outdoor=False, gt_mass=0.6, per_expert=False, shiftX=0, shiftY=0, world_offset=0.0,
-               active_only=True, unit_scale=1.0, alpha=100.0) -> Scene:
+               active_only=True, unit_scale=1.0, alpha=100.0, ppx=None, ppy=None) -> Scene:
     """One synthetic image worth of expert predictions.
 
     per_expert=False: ``assign`` is a multinomial draw of M hypotheses from a gating vector with
@@ -58,10 +58,12 @@ def make_scene(E=1, H=60, W=80, M=64, sub=8, seed=0, outlier_frac=0.4, noise=0.0
     "256 hyp x E experts" wording).  Experts that receive no hypothesis keep all-zero planes when
     ``active_only`` (test_esac.py:157,183-185).  ``unit_scale`` multiplies every length (maps and ground-truth translation:
     metres -> e.g. millimetres) and ``alpha`` sets the score scale; the clamp fixtures use both
-    (tests/golden/make_ref_golden.py)."""
+    (tests/golden/make_ref_golden.py).  ``ppx`` / ``ppy`` place the principal point (default: the image centre); the map
+    is generated through that camera, so a pose estimated with another camera misses the ground truth."""
     rng = np.random.default_rng(1305 + seed)
     img_w, img_h = W * sub, H * sub
-    ppx, ppy = img_w / 2.0, img_h / 2.0
+    ppx = img_w / 2.0 if ppx is None else float(ppx)
+    ppy = img_h / 2.0 if ppy is None else float(ppy)
     box = 50.0 if outdoor else 2.0
     dmin, dmax = (5.0, 80.0) if outdoor else (1.0, 5.0)
     gt_e = int(rng.integers(E))

@@ -146,6 +146,15 @@ int esacb200_forward_batch(esacb200_ctx* ctx, int B, const float* coords, int E,
                            float ppointX, float ppointY, float inlierThreshold, float inlierAlpha, float inlierBeta,
                            float maxReproj, int subSampling, int* out_experts);
 
+/* esacb200_forward_batch with a camera per image (the reference's callers read focallength from every image,
+ * test_esac.py:145-147): image b runs with shiftX[b] / shiftY[b], focal length f[b] and principal point (ppx[b], ppy[b]),
+ * host arrays of B values.  shiftX / shiftY may be NULL (= 0); f, ppx and ppy may not.  Everything else is as for
+ * esacb200_forward_batch, which is this entry with every array holding its scalar. */
+int esacb200_forward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
+                                   int64_t assign_stride, int M, float* out_poses, const int* shiftX, const int* shiftY,
+                                   const float* f, const float* ppx, const float* ppy, float inlierThreshold, float inlierAlpha,
+                                   float inlierBeta, float maxReproj, int subSampling, int* out_experts);
+
 /* esac_backward over B images of one shape (the reference trains with batch_size=1, train_esac.py:96-100, one
  * esac.backward per image): coords / grads float32 [B,E,3,H,W] (grads accumulated in place, as esac.cpp:490-508),
  * assign int64 [B,M] (as in esacb200_forward_batch), gt_poses float32 [B,4,4] (camera->world), shiftX / shiftY int [B]
@@ -158,6 +167,16 @@ int esacb200_backward_batch(esacb200_ctx* ctx, int B, const float* coords, float
                             float wLossTrans, float lossCut, const int* shiftX, const int* shiftY, float focalLength,
                             float ppointX, float ppointY, float inlierThreshold, float inlierAlpha, float inlierBeta,
                             float maxReproj, int subSampling, double* out_losses);
+
+/* esacb200_backward_batch with a camera per image: image b runs with focal length f[b] and principal point
+ * (ppx[b], ppy[b]), host arrays of B values that may not be NULL; shiftX / shiftY as for esacb200_backward_batch (NULL = 0).
+ * Same worker contexts and the same minimal sets per image as esacb200_backward_batch, which is this entry with every
+ * camera array holding its scalar. */
+int esacb200_backward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords, float* grads, int E, int H, int W,
+                                    const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wLossRot,
+                                    float wLossTrans, float lossCut, const int* shiftX, const int* shiftY, const float* f,
+                                    const float* ppx, const float* ppy, float inlierThreshold, float inlierAlpha,
+                                    float inlierBeta, float maxReproj, int subSampling, double* out_losses);
 
 /* Hypothesis assignment on the device, the three host steps the reference's callers run before esac.forward/backward:
  * util.clamp_probs (util.py:38-48; keep_top < 0 = off), torch.multinomial(probs, M, replacement=True)
@@ -178,6 +197,14 @@ int esacb200_assign_hypotheses(esacb200_ctx* ctx, int B, int E, int M, const flo
 int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* grads, int H, int W, const float* gt_poses,
                          const int* shiftX, const int* shiftY, float focalLength, float ppointX, float ppointY,
                          int subSampling, float cutLoss, float maxReproj, float minDepth, double* out_losses);
+
+/* esacb200_reproj_loss with a camera per image: image b is projected with focal length f[b] and principal point
+ * (ppx[b], ppy[b]), host arrays of B values that may not be NULL; shiftX / shiftY as for esacb200_reproj_loss (NULL = 0).
+ * Still one launch for the batch; esacb200_reproj_loss is this entry with every camera array holding its scalar, and the
+ * per-cell arithmetic is the same, so equal cameras give bitwise the same losses and gradients. */
+int esacb200_reproj_loss_cameras(esacb200_ctx* ctx, int B, const float* coords, float* grads, int H, int W, const float* gt_poses,
+                                 const int* shiftX, const int* shiftY, const float* f, const float* ppx, const float* ppy,
+                                 int subSampling, float cutLoss, float maxReproj, float minDepth, double* out_losses);
 
 /* Soft-inlier scores of given poses (getReproErrs + getHypScores, esac_util.h:235-363) without
  * sampling/selection/refinement: poses6 = host double [M][6] (rvec, tvec); out_scores host double [M]. */

@@ -89,6 +89,8 @@ def load_library() -> C.CDLL:
     lib.esacb200_reproj_loss.restype = i32
     lib.esacb200_reproj_loss_cameras.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, f32, f32, f32, vp]
     lib.esacb200_reproj_loss_cameras.restype = i32
+    lib.esacb200_coord_loss.argtypes = [vp, i32, vp, i32, i32, vp, i32, i32, vp, f32, vp, vp]
+    lib.esacb200_coord_loss.restype = i32
     lib.esacb200_backward_sharded.argtypes = ([vp, vp, vp, i32, i32, i32, vp, i64, i32, vp, f32, f32, f32] + cam +
                                                [EXCHANGE_FN, vp, C.POINTER(f64)])
     lib.esacb200_backward_sharded.restype = i32
@@ -639,6 +641,41 @@ def reproj_loss(prediction, gtPoses, focalLength, padX, padY, cutLoss, subSampli
     if og:
         og.finish()
     return [float(v) for v in losses]
+
+
+def coord_loss(prediction, gtCoords, cutLoss=100.0, outGradients=None, return_counts=False):
+    """The robust scene-coordinate loss of init_expert.py:106-130 and, when outGradients is given, d loss / d prediction in
+    the same call (what `robust_loss.backward()` hands to the expert, :132).  prediction [B,3,Hp,Wp] float32 (the reference
+    has B = 1), gtCoords [B,3,Hg,Wg] float32; the two may differ by at most 1 in H and in W and are cropped to the common
+    top-left window (util.assert_size).  Cells whose ground truth is all zero do not count; the loss of an image is the sum
+    over its valid cells divided by their number (NaN if there is none).  outGradients [B,3,Hp,Wp] float32 is overwritten
+    (0 outside the window and on invalid cells) or None for the loss alone.  Returns the B losses, and with return_counts
+    also the B valid-cell counts."""
+    _check(prediction, "Float", 4, "prediction")
+    _check(gtCoords, "Float", 4, "gtCoords")
+    B, C3, Hp, Wp = (int(v) for v in prediction.shape)
+    Bg, Cg, Hg, Wg = (int(v) for v in gtCoords.shape)
+    if C3 != 3 or Cg != 3 or Bg != B:
+        raise RuntimeError(f"shapes must be [B,3,Hp,Wp] and [B,3,Hg,Wg], got {list(prediction.shape)} and {list(gtCoords.shape)}")
+    if abs(Hp - Hg) > 1 or abs(Wp - Wg) > 1:
+        raise RuntimeError(f"tensor size mismatch: prediction {Hp}x{Wp}, ground truth {Hg}x{Wg} (util.assert_size allows 1)")
+    og = None
+    if outGradients is not None:
+        _check(outGradients, "Float", 4, "outGradients")
+        if tuple(outGradients.shape) != tuple(prediction.shape):
+            raise RuntimeError("outGradients must have the shape of prediction")
+        og = _Arg(outGradients, writable=True)
+    pr = _Arg(prediction)
+    gt = _Arg(gtCoords)
+    ctx = _pick_ctx(pr.device, gt.device, og.device if og else None)
+    losses = np.zeros(B, np.float64)
+    counts = np.zeros(B, np.int64)
+    ctx.check(ctx.lib.esacb200_coord_loss(ctx.handle, B, pr.ptr, Hp, Wp, gt.ptr, Hg, Wg, og.ptr if og else None, float(cutLoss),
+                                          losses.ctypes.data, counts.ctypes.data))
+    if og:
+        og.finish()
+    out = [float(v) for v in losses]
+    return (out, [int(v) for v in counts]) if return_counts else out
 
 
 def nccl_unique_id() -> bytes:

@@ -122,3 +122,29 @@ def reproj_loss(prediction, gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_
     opt.cutloss)` followed by `robust_loss.backward()`.  prediction [B,3,H,W] (CUDA), gt_poses [B,4,4] camera->world.
     focal_length, pad_x / pad_y and the principal point are a number or B values, so a batch may mix cameras."""
     return ReprojLoss.apply(prediction, gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling, ppoint_x, ppoint_y)
+
+
+class CoordLoss(torch.autograd.Function):
+    """init_expert.py:106-132 as one autograd node: forward = the robust scene-coordinate loss of a batch of predictions
+    (mean over the batch of the per-image losses; the reference has one image per step), backward = its gradient, both
+    from the fused kernels behind api.coord_loss."""
+
+    @staticmethod
+    def forward(ctx, prediction, gt_coords, cut_loss):
+        grads = torch.empty_like(prediction)
+        losses = api.coord_loss(prediction.detach(), gt_coords, cut_loss, outGradients=grads)
+        ctx.save_for_backward(grads)
+        ctx.batch = len(losses)
+        return prediction.new_tensor(sum(losses) / len(losses))
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        (grads,) = ctx.saved_tensors
+        return (grads * (grad_out / ctx.batch),) + (None,) * 2
+
+
+def coord_loss(prediction, gt_coords, cut_loss=100.0):
+    """Drop-in for the loss block of init_expert.py: `prediction, gt_coords = util.assert_size(...)` through the robust loss
+    (:114-130) become `robust_loss = coord_loss(prediction, gt_coords, opt.cutloss)`, followed by `robust_loss.backward()`.
+    prediction [B,3,Hp,Wp] (CUDA), gt_coords [B,3,Hg,Wg], at most 1 apart in H and W."""
+    return CoordLoss.apply(prediction, gt_coords, cut_loss)

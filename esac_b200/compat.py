@@ -38,11 +38,13 @@ def random_shift(image: torch.Tensor, max_shift):
 class SyntheticRoomDataset(Dataset):
     """Stand-in for RoomDataset: `num_experts` rooms on the reference's 5 m grid (room_dataset.py:177-184), `length`
     images of 640x480 px, each with a ground-truth pose, ground-truth scene coordinates [3,60,80] and the id of the room it
-    was taken in.  Deterministic in (seed, index)."""
+    was taken in.  Deterministic in (seed, index).  gt_valid_frac < 1 zeroes a deterministic share of 1 - gt_valid_frac
+    of the ground-truth cells (cells without ground truth, as in the sparse SfM datasets)."""
 
     def __init__(self, num_experts: int = 4, length: int = 16, hypotheses: int = 256, seed: int = 0, training: bool = True,
-                 image_hw=(480, 640), outlier_frac: float = 0.4, noise: float = 0.02):
+                 image_hw=(480, 640), outlier_frac: float = 0.4, noise: float = 0.02, gt_valid_frac: float = 1.0):
         self.num_experts = num_experts
+        self.gt_valid_frac = gt_valid_frac
         self.length = length
         self.hypotheses = hypotheses
         self.seed = seed
@@ -75,6 +77,11 @@ class SyntheticRoomDataset(Dataset):
         gt_pose = torch.from_numpy(sc.gt_pose.copy())
         if self.training:
             gt_coords = torch.from_numpy(sc.coords[sc.gt_expert].copy())
+            if self.gt_valid_frac < 1.0:
+                # cells without ground truth are all zero (sparse SfM depth, Aachen / Dubrovnik); own stream, so the image
+                # and the kept cells do not change
+                drop = np.random.default_rng(self.seed * 6151 + index).random(gt_coords.shape[1:]) >= self.gt_valid_frac
+                gt_coords[:, torch.from_numpy(drop)] = 0.0
         else:
             gt_coords = 0                                                              # room_dataset.py:209-212
         return index, image, float(sc.f), gt_pose, gt_coords, int(sc.gt_expert)

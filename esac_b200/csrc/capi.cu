@@ -1548,6 +1548,63 @@ int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* g
                                         cut, maxReproj, minDepth, out_losses);
 } ESAC_ABI_CATCH(ctx)
 
+// -------------------------------------------------------------------------------------------------
+int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int Wp, const float* gt, int Hg, int Wg,
+                        float* grads, float cut, double* out_losses, int64_t* out_counts) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (!pred || !gt || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    if (B <= 0 || Hp <= 0 || Wp <= 0 || Hg <= 0 || Wg <= 0)
+        return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d prediction %dx%d ground truth %dx%d", B, Hp, Wp, Hg, Wg);
+    if (abs(Hp - Hg) > 1 || abs(Wp - Wg) > 1)   // util.assert_size tolerates 1 cell
+        return fail(ctx, ESACB200_ERR_ARG, "size mismatch: prediction %dx%d, ground truth %dx%d (at most 1 apart)", Hp, Wp, Hg, Wg);
+    if ((long long)Hp * Wp > (1ll << 30) || (long long)Hg * Wg > (1ll << 30))
+        return fail(ctx, ESACB200_ERR_ARG, "map too large");
+    begin_call(ctx);
+    const size_t pbytes = (size_t)B * 3 * Hp * Wp * sizeof(float), gbytes = (size_t)B * 3 * Hg * Wg * sizeof(float);
+    const bool p_host = !is_device_ptr(pred), q_host = !is_device_ptr(gt), g_host = grads && !is_device_ptr(grads);
+    const float* d_pred = pred;
+    const float* d_gt = gt;
+    float* d_grads = grads;
+    if (p_host) {
+        CK(ctx->coords.ensure(pbytes));
+        CK(cudaMemcpyAsync(ctx->coords.p, pred, pbytes, cudaMemcpyHostToDevice, ctx->stream));
+        d_pred = ctx->coords.as<float>();
+    }
+    if (q_host) {
+        CK(ctx->coords_alt.ensure(gbytes));
+        CK(cudaMemcpyAsync(ctx->coords_alt.p, gt, gbytes, cudaMemcpyHostToDevice, ctx->stream));
+        d_gt = ctx->coords_alt.as<float>();
+    }
+    if (g_host) {
+        CK(ctx->grads.ensure(pbytes));
+        d_grads = ctx->grads.as<float>();
+    }
+    const int bpi = reproj_blocks_per_image(Hp * Wp, B, ctx->sm_count);
+    // scratch layout: [tickets B u32 | counts B u32, padded] [losses B f64] [valid counts B i64] [partials B*bpi*2 f64]
+    const size_t off_loss = ((size_t)B * 8 + 63) & ~(size_t)63, off_cnt = off_loss + (((size_t)B * 8 + 63) & ~(size_t)63),
+                 off_part = off_cnt + (((size_t)B * 8 + 63) & ~(size_t)63);
+    CK(ctx->scratch.ensure(off_part + (size_t)B * bpi * 2 * 8));
+    char* base = (char*)ctx->scratch.p;
+    CK(cudaMemsetAsync(base, 0, off_loss, ctx->stream));
+    mark(ctx, EV_H2D);
+    mark(ctx, EV_FOLD);  // ms_score = the kernels alone
+    ctx->st.kernel_launches += launch_coord_loss(d_pred, d_gt, d_grads, B, Hp, Wp, Hg, Wg, cut, bpi, (unsigned*)base + B,
+                                                 (double*)(base + off_part), (unsigned*)base, (double*)(base + off_loss),
+                                                 (long long*)(base + off_cnt), ctx->stream);
+    CK(cudaGetLastError());
+    mark(ctx, EV_SCORE);
+    if (g_host) CK(cudaMemcpyAsync(grads, d_grads, pbytes, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(out_losses, base + off_loss, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_counts) CK(cudaMemcpyAsync(out_counts, base + off_cnt, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    mark(ctx, EV_END);
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    ctx->last_M = 0;
+    finish_stats(ctx);
+    return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
 int esacb200_copy_last_scores(esacb200_ctx* ctx, double* dst, int M) try {
     if (!ctx || !dst) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);

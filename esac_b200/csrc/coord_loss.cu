@@ -1,0 +1,220 @@
+// Robust scene-coordinate loss of the expert initialisation stage, loss and gradient (init_expert.py:106-135).
+//
+// init_expert.py crops prediction and ground truth to a common size (:114, util.assert_size, util.py:18-36), drops the cells
+// whose ground truth is all zero (:119-121), takes the Euclidean distance per cell, applies the same L1 / square-root robust
+// loss as the refinement stage and divides by the number of valid cells (:123-130); autograd then walks back through it.  Four
+// boolean-mask indexings each synchronise the host.  Here it is two launches and no host round trip:
+//
+//   count pass   valid cells per image (12 B read per window cell: the ground truth)
+//   loss pass    loss and d loss / d prediction (24 B read + 12 B written per cell), scaled by 1 / count
+//
+// i.e. 48 B per cell with the gradient; a loss-only call skips the count pass and counts in the loss pass (24 B per cell).
+// Per cell, with d = pred - gt in fp32 (the subtraction torch does) and everything after it in fp64:
+//   valid  = gt.x != 0 || gt.y != 0 || gt.z != 0        (gt.abs().sum(0) != 0; NaN counts as valid, no flush to zero)
+//   n      = ||d||
+//   loss   = n <= cut ? n : sqrt(cut * n)
+//   grad   = rho'(n) * d / n / count,  rho' = 1 or 0.5 * sqrt(cut / n);  0 at n = 0 (torch's norm backward)
+// A NaN cell counts but falls in neither masked sum (loss 0, gradient NaN); an invalid cell has loss and gradient 0, as do
+// prediction cells outside the common window.  The per-image loss is summed in fp64 in a fixed order (block partials, the
+// image's last block adds them up), so the result does not depend on scheduling.
+#include "esac_internal.h"
+
+namespace esacb200 {
+
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kCellsPerThread = 4;
+
+struct CoordGeom {
+    int Np, Ng;   // plane sizes of the prediction / the ground truth (Hp*Wp, Hg*Wg)
+    int Wp, Wg;   // their row pitches
+    int H, W;     // the common top-left window
+    int N;        // H*W
+};
+
+__device__ __forceinline__ bool gt_valid(float x, float y, float z) { return x != 0.f || y != 0.f || z != 0.f; }
+
+// Window cell of prediction cell p (scalar path); -1 outside the window, else the ground-truth index.
+__device__ __forceinline__ int gt_index(int y, int x, const CoordGeom& g) { return (y < g.H && x < g.W) ? y * g.Wg + x : -1; }
+
+struct CellOut {
+    double loss;
+    float gx, gy, gz;
+};
+
+// One valid cell.  cnt = valid cells of the image (the gradient's normaliser; unused without GRAD).
+template <bool GRAD>
+__device__ __forceinline__ CellOut coord_cell(float px, float py, float pz, float qx, float qy, float qz, float cut, double cnt) {
+    const float dx = px - qx, dy = py - qy, dz = pz - qz;
+    const double s2 = fma((double)dx, (double)dx, fma((double)dy, (double)dy, (double)dz * (double)dz));   // exact products
+    const double n = sqrt(s2);
+    CellOut o;
+    double w = 0.;                                    // rho'(n) / n / count
+    if (n <= (double)cut) {                           // n == cut is in the L1 branch (loss[loss <= cut])
+        o.loss = n;
+        if (GRAD) w = 1.0 / (n * cnt);
+    } else {
+        o.loss = sqrt((double)cut * n);
+        if (GRAD) w = 0.5 * o.loss / (s2 * cnt);      // 0.5 sqrt(cut / n) / n = 0.5 sqrt(cut n) / n^2
+    }
+    if (!(n > 0.)) w = 0.;                            // n = 0: zero gradient
+    o.gx = (float)(w * dx);
+    o.gy = (float)(w * dy);
+    o.gz = (float)(w * dz);
+    if (!(n == n)) {                                  // NaN: in neither masked sum, gradient NaN
+        o.loss = 0.;
+        o.gx = o.gy = o.gz = (float)n;
+    }
+    return o;
+}
+
+// grid = (blocks_per_image, B).  counts[b] += valid cells of image b (zeroed before the launch).
+template <bool VEC>
+__global__ void __launch_bounds__(kThreads) coord_count_kernel(const float* __restrict__ gt, CoordGeom g,
+                                                                unsigned* __restrict__ counts) {
+    const int b = blockIdx.y;
+    const float* qx = gt + (size_t)b * 3 * g.Ng;
+    const float* qy = qx + g.Ng;
+    const float* qz = qy + g.Ng;
+    unsigned cnt = 0;
+    const int per_block = kThreads * kCellsPerThread;
+    for (int base = blockIdx.x * per_block; base < g.Np; base += gridDim.x * per_block) {
+        const int p0 = base + threadIdx.x * kCellsPerThread;
+        if (VEC) {
+            if (p0 >= g.N) continue;   // the window is the first N cells of both planes (equal pitch, N % 4 == 0)
+            const float4 a = __ldcs(reinterpret_cast<const float4*>(qx + p0));
+            const float4 c = __ldcs(reinterpret_cast<const float4*>(qy + p0));
+            const float4 d = __ldcs(reinterpret_cast<const float4*>(qz + p0));
+            cnt += gt_valid(a.x, c.x, d.x) + gt_valid(a.y, c.y, d.y) + gt_valid(a.z, c.z, d.z) + gt_valid(a.w, c.w, d.w);
+        } else {
+            if (p0 >= g.Np) continue;
+            int y = p0 / g.Wp, x = p0 - y * g.Wp;
+            const int n = min(kCellsPerThread, g.Np - p0);
+            for (int i = 0; i < n; ++i) {
+                const int q = gt_index(y, x, g);
+                if (q >= 0) cnt += gt_valid(qx[q], qy[q], qz[q]);
+                if (++x == g.Wp) { x = 0; ++y; }
+            }
+        }
+    }
+    cnt = __reduce_add_sync(0xffffffffu, cnt);
+    if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&counts[b], cnt);
+}
+
+// grid = (blocks_per_image, B) over the prediction's cells.  GRAD: grads [B,3,Hp,Wp] is overwritten, counts[b] from the
+// count pass.  losses[b] = loss of image b, out_counts[b] = its valid cells; partial: B * blocks_per_image * 2 doubles,
+// tickets: B zeroed counters (left zeroed).
+template <bool VEC, bool GRAD>
+__global__ void __launch_bounds__(kThreads) coord_loss_kernel(const float* __restrict__ pred, const float* __restrict__ gt,
+                                                               float* __restrict__ grads, CoordGeom g, float cut,
+                                                               const unsigned* __restrict__ counts, double* __restrict__ partial,
+                                                               unsigned* __restrict__ tickets, double* __restrict__ losses,
+                                                               long long* __restrict__ out_counts) {
+    const int b = blockIdx.y;
+    const float* px = pred + (size_t)b * 3 * g.Np;
+    const float* py = px + g.Np;
+    const float* pz = py + g.Np;
+    const float* qx = gt + (size_t)b * 3 * g.Ng;
+    const float* qy = qx + g.Ng;
+    const float* qz = qy + g.Ng;
+    float* gx = GRAD ? grads + (size_t)b * 3 * g.Np : nullptr;
+    const double cnt = GRAD ? (double)counts[b] : 0.;
+    double acc = 0.;
+    unsigned nvalid = 0;
+    const int per_block = kThreads * kCellsPerThread;
+    for (int base = blockIdx.x * per_block; base < g.Np; base += gridDim.x * per_block) {
+        const int p0 = base + threadIdx.x * kCellsPerThread;
+        if (p0 >= g.Np) continue;
+        if (VEC) {
+            float o[3][4] = {};
+            if (p0 < g.N) {   // all four cells in the window (N % 4 == 0), else all four outside: zero gradient
+                const float4 a = __ldcs(reinterpret_cast<const float4*>(px + p0));
+                const float4 c = __ldcs(reinterpret_cast<const float4*>(py + p0));
+                const float4 d = __ldcs(reinterpret_cast<const float4*>(pz + p0));
+                const float4 e = __ldcs(reinterpret_cast<const float4*>(qx + p0));
+                const float4 f = __ldcs(reinterpret_cast<const float4*>(qy + p0));
+                const float4 h = __ldcs(reinterpret_cast<const float4*>(qz + p0));
+                const float P[3][4] = {{a.x, a.y, a.z, a.w}, {c.x, c.y, c.z, c.w}, {d.x, d.y, d.z, d.w}};
+                const float Q[3][4] = {{e.x, e.y, e.z, e.w}, {f.x, f.y, f.z, f.w}, {h.x, h.y, h.z, h.w}};
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    if (!gt_valid(Q[0][i], Q[1][i], Q[2][i])) continue;
+                    const CellOut r = coord_cell<GRAD>(P[0][i], P[1][i], P[2][i], Q[0][i], Q[1][i], Q[2][i], cut, cnt);
+                    acc += r.loss;
+                    ++nvalid;
+                    o[0][i] = r.gx; o[1][i] = r.gy; o[2][i] = r.gz;
+                }
+            }
+            if (GRAD) {
+                __stcs(reinterpret_cast<float4*>(gx + p0), make_float4(o[0][0], o[0][1], o[0][2], o[0][3]));
+                __stcs(reinterpret_cast<float4*>(gx + g.Np + p0), make_float4(o[1][0], o[1][1], o[1][2], o[1][3]));
+                __stcs(reinterpret_cast<float4*>(gx + 2 * (size_t)g.Np + p0), make_float4(o[2][0], o[2][1], o[2][2], o[2][3]));
+            }
+        } else {
+            int y = p0 / g.Wp, x = p0 - y * g.Wp;
+            const int n = min(kCellsPerThread, g.Np - p0);
+            for (int i = 0; i < n; ++i) {
+                const int q = gt_index(y, x, g);
+                float rx = 0.f, ry = 0.f, rz = 0.f;
+                if (q >= 0) {
+                    const float ex = qx[q], ey = qy[q], ez = qz[q];
+                    if (gt_valid(ex, ey, ez)) {
+                        const CellOut r = coord_cell<GRAD>(px[p0 + i], py[p0 + i], pz[p0 + i], ex, ey, ez, cut, cnt);
+                        acc += r.loss;
+                        ++nvalid;
+                        rx = r.gx; ry = r.gy; rz = r.gz;
+                    }
+                }
+                if (GRAD) {
+                    gx[p0 + i] = rx;
+                    gx[g.Np + p0 + i] = ry;
+                    gx[2 * (size_t)g.Np + p0 + i] = rz;
+                }
+                if (++x == g.Wp) { x = 0; ++y; }
+            }
+        }
+    }
+    double total[2] = {acc, (double)nvalid};
+    if (block_image_sum<kThreads>(total, partial, tickets)) {
+        losses[b] = total[0] / total[1];   // no valid cell: 0 / 0 = NaN, as in torch
+        out_counts[b] = (long long)total[1];
+    }
+}
+
+}  // namespace
+
+int launch_coord_loss(const float* pred, const float* gt, float* grads, int B, int Hp, int Wp, int Hg, int Wg, float cut,
+                      int blocks_per_image, unsigned* counts, double* partial, unsigned* tickets, double* losses,
+                      long long* out_counts, cudaStream_t stream) {
+    CoordGeom g;
+    g.Np = Hp * Wp; g.Ng = Hg * Wg; g.Wp = Wp; g.Wg = Wg;
+    g.H = Hp < Hg ? Hp : Hg;
+    g.W = Wp < Wg ? Wp : Wg;
+    g.N = g.H * g.W;
+    // 128-bit path: equal row pitch (the window is then the first N cells of every plane), every plane 16-byte aligned
+    const bool vec = Wp == Wg && g.N % 4 == 0 && g.Np % 4 == 0 && g.Ng % 4 == 0 && (uintptr_t)pred % 16 == 0 &&
+                     (uintptr_t)gt % 16 == 0 && (!grads || (uintptr_t)grads % 16 == 0);
+    const dim3 grid(blocks_per_image, B);
+    int launches = 1;
+    if (grads) {
+        if (vec) coord_count_kernel<true><<<grid, kThreads, 0, stream>>>(gt, g, counts);
+        else coord_count_kernel<false><<<grid, kThreads, 0, stream>>>(gt, g, counts);
+        ++launches;
+        if (vec)
+            coord_loss_kernel<true, true><<<grid, kThreads, 0, stream>>>(pred, gt, grads, g, cut, counts, partial, tickets,
+                                                                         losses, out_counts);
+        else
+            coord_loss_kernel<false, true><<<grid, kThreads, 0, stream>>>(pred, gt, grads, g, cut, counts, partial, tickets,
+                                                                          losses, out_counts);
+    } else if (vec) {
+        coord_loss_kernel<true, false><<<grid, kThreads, 0, stream>>>(pred, gt, nullptr, g, cut, counts, partial, tickets,
+                                                                      losses, out_counts);
+    } else {
+        coord_loss_kernel<false, false><<<grid, kThreads, 0, stream>>>(pred, gt, nullptr, g, cut, counts, partial, tickets,
+                                                                       losses, out_counts);
+    }
+    return launches;
+}
+
+}  // namespace esacb200

@@ -29,6 +29,60 @@ __device__ __forceinline__ double warp_reduce_scatter(const double (&v)[NV]) {
     }
     return w[0];
 }
+
+// Sum of NV doubles per thread over a block of THREADS threads in a fixed order: a butterfly within each warp, then the
+// warp totals in warp order.  The totals are valid in thread 0.  Every thread of the block calls it.
+template <int THREADS, int NV>
+__device__ __forceinline__ void block_sum_fixed(double (&v)[NV]) {
+    __shared__ double warp_sum[NV][THREADS / 32];
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) v[i] += __shfl_xor_sync(0xffffffffu, v[i], o);
+    }
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int i = 0; i < NV; ++i) warp_sum[i][threadIdx.x >> 5] = v[i];
+    }
+    __syncthreads();
+#pragma unroll
+    for (int i = 0; i < NV; ++i) {
+        double s = 0.;
+        if (threadIdx.x == 0)
+            for (int w = 0; w < THREADS / 32; ++w) s += warp_sum[i][w];
+        v[i] = s;
+    }
+}
+
+// Per-image sum over the blocks of a (blocks_per_image, B) grid, deterministic: every block sums its threads' NV values
+// (block_sum_fixed) and stores the totals in partial[b][blockIdx.x][NV]; the image's last block to take a ticket adds the
+// partials in block order.  Returns true in thread 0 of that block, with the image totals in v; tickets[b] (zero before
+// the launch) is left zero for the next one.
+template <int THREADS, int NV>
+__device__ __forceinline__ bool block_image_sum(double (&v)[NV], double* __restrict__ partial, unsigned* __restrict__ tickets) {
+    __shared__ bool last;
+    const int b = blockIdx.y;
+    block_sum_fixed<THREADS, NV>(v);
+    if (threadIdx.x == 0) {
+#pragma unroll
+        for (int i = 0; i < NV; ++i) partial[((size_t)b * gridDim.x + blockIdx.x) * NV + i] = v[i];
+        __threadfence();
+        last = atomicAdd(&tickets[b], 1u) == gridDim.x - 1;
+    }
+    __syncthreads();
+    if (!last) return false;
+    __threadfence();
+#pragma unroll
+    for (int i = 0; i < NV; ++i) v[i] = 0.;
+    for (unsigned k = threadIdx.x; k < gridDim.x; k += THREADS) {
+#pragma unroll
+        for (int i = 0; i < NV; ++i) v[i] += __ldcg(&partial[((size_t)b * gridDim.x + k) * NV + i]);
+    }
+    block_sum_fixed<THREADS, NV>(v);
+    if (threadIdx.x == 0) tickets[b] = 0;  // ready for the next launch
+    return threadIdx.x == 0;
+}
 #endif
 
 // Per-call problem description (esac.cpp:64-77 arguments + tensor sizes).
@@ -175,6 +229,16 @@ constexpr int kReprojImgFloats = 20;
 void launch_reproj(const float* coords, float* grads, const float* img, int B, int N, int W, float sub, float cut,
                    float max_err, float min_depth, int blocks_per_image, double* partial, unsigned* tickets, double* losses,
                    cudaStream_t stream);
+
+// --- coord_loss.cu ------------------------------------------------------------------------
+// Both passes run on a (blocks_per_image, B) grid of 256-thread blocks, 4 cells per thread, as the reprojection loss:
+// blocks_per_image = reproj_blocks_per_image(Hp * Wp, ...), a pure function of the size that fixes the summation order.
+// pred [B,3,Hp,Wp], gt [B,3,Hg,Wg] (|Hp-Hg|, |Wp-Wg| <= 1, checked by the caller), grads [B,3,Hp,Wp] overwritten or null
+// (loss only).  counts: B zeroed counters (gradient only), partial: B * blocks_per_image * 2 doubles, tickets: B zeroed
+// counters (left zeroed), losses: B doubles, out_counts: B valid-cell counts.  Returns the number of kernels launched.
+int launch_coord_loss(const float* pred, const float* gt, float* grads, int B, int Hp, int Wp, int Hg, int Wg, float cut,
+                      int blocks_per_image, unsigned* counts, double* partial, unsigned* tickets, double* losses,
+                      long long* out_counts, cudaStream_t stream);
 
 // --- bwd.cu -------------------------------------------------------------------------------
 struct BwdArgs {

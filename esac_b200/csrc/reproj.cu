@@ -142,8 +142,6 @@ __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const float* __rest
                                                           float max_err, float min_depth, double* __restrict__ partial,
                                                           unsigned* __restrict__ tickets, double* __restrict__ losses) {
     __shared__ float m[kReprojImgFloats];
-    __shared__ double warp_sum[kThreads / 32];
-    __shared__ bool last;
     const int b = blockIdx.y;
     if (threadIdx.x < kReprojImgFloats) m[threadIdx.x] = img[b * kReprojImgFloats + threadIdx.x];
     __syncthreads();
@@ -234,34 +232,8 @@ __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const float* __rest
         }
     }
     // block sum in a fixed order, then the last block of the image adds the partials, again in a fixed order
-    auto block_sum = [&](double v) -> double {  // result valid in thread 0
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        __syncthreads();
-        if ((threadIdx.x & 31) == 0) warp_sum[threadIdx.x >> 5] = v;
-        __syncthreads();
-        double s = 0.;
-        if (threadIdx.x == 0)
-            for (int w = 0; w < kThreads / 32; ++w) s += warp_sum[w];
-        return s;
-    };
-    const double mine = block_sum(acc);
-    if (threadIdx.x == 0) {
-        partial[(size_t)b * gridDim.x + blockIdx.x] = mine;
-        __threadfence();
-        last = atomicAdd(&tickets[b], 1u) == gridDim.x - 1;
-    }
-    __syncthreads();
-    if (last) {
-        __threadfence();
-        double v = 0.;
-        for (unsigned k = threadIdx.x; k < gridDim.x; k += kThreads) v += __ldcg(&partial[(size_t)b * gridDim.x + k]);
-        const double s = block_sum(v);
-        if (threadIdx.x == 0) {
-            losses[b] = s / (double)N;
-            tickets[b] = 0;  // ready for the next launch
-        }
-    }
+    double total[1] = {acc};
+    if (block_image_sum<kThreads>(total, partial, tickets)) losses[b] = total[0] / (double)N;
 }
 
 }  // namespace

@@ -206,6 +206,18 @@ int esacb200_reproj_loss_cameras(esacb200_ctx* ctx, int B, const float* coords, 
                                  const int* shiftX, const int* shiftY, const float* f, const float* ppx, const float* ppy,
                                  int subSampling, float cutLoss, float maxReproj, float minDepth, double* out_losses);
 
+/* Robust scene-coordinate loss of the expert initialisation stage and its gradient (init_expert.py:106-135, where it is
+ * ten elementwise torch ops, four boolean-mask indexings + autograd): pred float32 [B,3,Hp,Wp] (one expert's prediction
+ * per image; the reference has B = 1), gt float32 [B,3,Hg,Wg] ground-truth scene coordinates.  The two may differ by at most
+ * 1 in H and in W; both are cropped to the top-left min(Hp,Hg) x min(Wp,Wg) window (util.assert_size, util.py:18-36).  A
+ * cell is valid iff one of its ground-truth components is nonzero (NaN included); n = ||pred - gt||, per-cell loss n for
+ * n <= cutLoss, sqrt(cutLoss * n) above; the image's loss is the sum over valid cells divided by their number (NaN when
+ * there is none).  grads float32 [B,3,Hp,Wp] or NULL (loss only) = d loss_b / d pred (overwritten, not accumulated; 0 outside
+ * the window, on invalid cells and at n = 0, NaN on NaN cells).  out_losses host double [B]; out_counts host int64 [B] valid
+ * cells per image, or NULL.  pred / gt / grads host or device pointers; one host synchronisation, at the end. */
+int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int Wp, const float* gt, int Hg, int Wg,
+                        float* grads, float cutLoss, double* out_losses, int64_t* out_counts);
+
 /* Soft-inlier scores of given poses (getReproErrs + getHypScores, esac_util.h:235-363) without
  * sampling/selection/refinement: poses6 = host double [M][6] (rvec, tvec); out_scores host double [M]. */
 int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,

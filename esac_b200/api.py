@@ -91,6 +91,15 @@ def load_library() -> C.CDLL:
     lib.esacb200_reproj_loss_cameras.restype = i32
     lib.esacb200_coord_loss.argtypes = [vp, i32, vp, i32, i32, vp, i32, i32, vp, f32, vp, vp]
     lib.esacb200_coord_loss.restype = i32
+    # ragged batches: host arrays of B pointers and of B heights / widths
+    lib.esacb200_forward_ragged.argtypes = [vp, i32, vp, vp, vp, i32, vp, i64, i32, vp] + cams + [vp]
+    lib.esacb200_forward_ragged.restype = i32
+    lib.esacb200_backward_ragged.argtypes = [vp, i32, vp, vp, vp, vp, i32, vp, i64, i32, vp, f32, f32, f32] + cams + [vp]
+    lib.esacb200_backward_ragged.restype = i32
+    lib.esacb200_reproj_loss_ragged.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, i32, f32, f32, f32, vp]
+    lib.esacb200_reproj_loss_ragged.restype = i32
+    lib.esacb200_coord_loss_ragged.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, f32, vp, vp]
+    lib.esacb200_coord_loss_ragged.restype = i32
     lib.esacb200_backward_sharded.argtypes = ([vp, vp, vp, i32, i32, i32, vp, i64, i32, vp, f32, f32, f32] + cam +
                                                [EXCHANGE_FN, vp, C.POINTER(f64)])
     lib.esacb200_backward_sharded.restype = i32
@@ -370,6 +379,46 @@ def _per_image(v, B: int, dtype, what: str) -> np.ndarray:
     return a
 
 
+def _is_list(t) -> bool:
+    """A ragged batch: a list or tuple of per-image tensors / arrays (each with its own H x W)."""
+    return isinstance(t, (list, tuple))
+
+
+def _check_list(ts, rank: int, what: str, B: int | None = None) -> list:
+    """Checks a ragged argument (float32 elements of `rank` dims, all CPU / numpy or all CUDA, B of them) and returns the
+    element shapes.  Raises RuntimeError before any context exists."""
+    if not _is_list(ts):
+        raise RuntimeError(f"{what} must be a list or tuple of tensors, as the other image arguments")
+    if len(ts) == 0:
+        raise RuntimeError(f"{what} is an empty list")
+    if B is not None and len(ts) != B:
+        raise RuntimeError(f"{what} holds {len(ts)} tensors for {B} images")
+    for b, t in enumerate(ts):
+        _check(t, "Float", rank, f"{what}[{b}]")
+    if len({bool(_is_torch(t) and t.is_cuda) for t in ts}) > 1:
+        raise RuntimeError(f"{what} mixes CPU and CUDA tensors")
+    return [tuple(int(v) for v in t.shape) for t in ts]
+
+
+def _check_maps(shapes, what: str) -> int:
+    """[E,3,H,W] elements with one E, each large enough to draw 4 distinct cells (esac.cpp:110-113); returns E."""
+    E = shapes[0][0]
+    for b, s in enumerate(shapes):
+        if s[1] != 3 or s[0] != E:
+            raise RuntimeError(f"{what}[{b}] must be [E,3,H,W] with the E of image 0 ({E}), got {list(s)}")
+        if (s[3] - 1) * (s[2] - 1) < 4:
+            raise RuntimeError(f"{what}[{b}]: map {s[3]}x{s[2]} too small to draw 4 distinct cells")
+    return E
+
+
+def _ptr_array(args) -> C.Array:
+    return (C.c_void_p * len(args))(*[a.ptr for a in args])
+
+
+def _dims(shapes, axis: int) -> np.ndarray:
+    return np.ascontiguousarray([s[axis] for s in shapes], np.int32)
+
+
 _CUDA_STREAM_LEGACY = 0x1
 
 
@@ -505,7 +554,12 @@ def forward_batch(sceneCoordinates, hypAssignment, outPoses, shiftX, shiftY, foc
     for the whole batch; host tensors (pinned) are copied on a second stream while the previous image computes.
     shiftX, shiftY, focalLength, ppointX and ppointY are each a number (one camera for the batch) or B values -- a
     sequence, numpy array or 1-D tensor, e.g. the DataLoader's `focallength` -- giving image b its own shift and camera;
-    image b then computes what esac.forward with those values computes."""
+    image b then computes what esac.forward with those values computes.
+    sceneCoordinates may also be a list or tuple of B [E,3,H_b,W_b] tensors (CPU, CUDA or numpy), each image with its own
+    map size (a ragged batch); image b then computes what esac.forward on that tensor computes."""
+    if _is_list(sceneCoordinates):
+        return _forward_ragged(sceneCoordinates, hypAssignment, outPoses, shiftX, shiftY, focalLength, ppointX, ppointY,
+                               inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling)
     _check(sceneCoordinates, "Float", 5, "sceneCoordinates")
     _check(hypAssignment, "Long", 2, "hypAssignment")
     _check(outPoses, "Float", 3, "outPoses")
@@ -537,13 +591,46 @@ def forward_batch(sceneCoordinates, hypAssignment, outPoses, shiftX, shiftY, foc
     return [int(e) for e in experts]
 
 
+def _forward_ragged(sceneCoordinates, hypAssignment, outPoses, shiftX, shiftY, focalLength, ppointX, ppointY,
+                    inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling) -> list:
+    shapes = _check_list(sceneCoordinates, 4, "sceneCoordinates")
+    B = len(shapes)
+    E = _check_maps(shapes, "sceneCoordinates")
+    _check(hypAssignment, "Long", 2, "hypAssignment")
+    _check(outPoses, "Float", 3, "outPoses")
+    if tuple(outPoses.shape) != (B, 4, 4) or int(hypAssignment.shape[0]) != B:
+        raise RuntimeError(f"a list of {B} maps needs hypAssignment [{B},M] and outPoses [{B},4,4]")
+    sx, sy = _per_image(shiftX, B, np.int32, "shiftX"), _per_image(shiftY, B, np.int32, "shiftY")
+    fs = _per_image(focalLength, B, np.float32, "focalLength")
+    cx, cy = _per_image(ppointX, B, np.float32, "ppointX"), _per_image(ppointY, B, np.float32, "ppointY")
+    co = [_Arg(t) for t in sceneCoordinates]
+    op = _Arg(outPoses, writable=True)
+    ha = _Arg(hypAssignment)
+    M = int(hypAssignment.shape[1])
+    ctx = _pick_ctx(*(a.device for a in co), op.device, ha.device)
+    experts = (C.c_int * B)()
+    hs, ws = _dims(shapes, 2), _dims(shapes, 3)
+    ctx.check(ctx.lib.esacb200_forward_ragged(ctx.handle, B, _ptr_array(co), hs.ctypes.data, ws.ctypes.data, E, ha.ptr, 1, M, op.ptr,
+                                              sx.ctypes.data, sy.ctypes.data, fs.ctypes.data, cx.ctypes.data, cy.ctypes.data,
+                                              float(inlierThreshold), float(inlierAlpha), float(inlierBeta), float(maxReproj),
+                                              int(subSampling), experts))
+    op.finish()
+    return [int(e) for e in experts]
+
+
 def backward_batch(sceneCoordinates, outGradients, hypAssignment, gtPoses, wLossRot, wLossTrans, lossCut, shiftX, shiftY,
                    focalLength, ppointX, ppointY, inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling) -> list:
     """esac.backward over a batch: sceneCoordinates / outGradients [B,E,3,H,W] float32 (gradients accumulated in place),
     hypAssignment [B,M] int64, gtPoses [B,4,4] float32 (camera->world), shiftX / shiftY an int or a sequence of B ints
     (train_esac.py:125 draws one shift per image), focalLength / ppointX / ppointY a number or B values (one camera per
     image, as forward_batch).  Returns the expected loss of every image; equal, image by image, to B consecutive
-    esac.backward calls on the same context, each with its image's shift and camera."""
+    esac.backward calls on the same context, each with its image's shift and camera.
+    sceneCoordinates and outGradients may also be lists or tuples of B [E,3,H_b,W_b] tensors (a ragged batch, as for
+    forward_batch); outGradients[b] has the shape of sceneCoordinates[b]."""
+    if _is_list(sceneCoordinates) or _is_list(outGradients):
+        return _backward_ragged(sceneCoordinates, outGradients, hypAssignment, gtPoses, wLossRot, wLossTrans, lossCut, shiftX,
+                                shiftY, focalLength, ppointX, ppointY, inlierThreshold, inlierAlpha, inlierBeta, maxReproj,
+                                subSampling)
     _check(sceneCoordinates, "Float", 5, "sceneCoordinates")
     _check(outGradients, "Float", 5, "outGradients")
     _check(hypAssignment, "Long", 2, "hypAssignment")
@@ -573,6 +660,40 @@ def backward_batch(sceneCoordinates, outGradients, hypAssignment, gtPoses, wLoss
         rc = ctx.lib.esacb200_backward_batch_cameras(*head, fs.ctypes.data, cx.ctypes.data, cy.ctypes.data, *tail)
     ctx.check(rc)
     og.finish()
+    return [float(v) for v in losses]
+
+
+def _backward_ragged(sceneCoordinates, outGradients, hypAssignment, gtPoses, wLossRot, wLossTrans, lossCut, shiftX, shiftY,
+                     focalLength, ppointX, ppointY, inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling) -> list:
+    shapes = _check_list(sceneCoordinates, 4, "sceneCoordinates")
+    B = len(shapes)
+    E = _check_maps(shapes, "sceneCoordinates")
+    gshapes = _check_list(outGradients, 4, "outGradients", B)
+    for b in range(B):
+        if gshapes[b] != shapes[b]:
+            raise RuntimeError(f"outGradients[{b}] is {list(gshapes[b])}, sceneCoordinates[{b}] is {list(shapes[b])}")
+    _check(hypAssignment, "Long", 2, "hypAssignment")
+    _check(gtPoses, "Float", 3, "gtPoses")
+    if tuple(gtPoses.shape) != (B, 4, 4) or int(hypAssignment.shape[0]) != B:
+        raise RuntimeError(f"a list of {B} maps needs hypAssignment [{B},M] and gtPoses [{B},4,4]")
+    sx, sy = _per_image(shiftX, B, np.int32, "shiftX"), _per_image(shiftY, B, np.int32, "shiftY")
+    fs = _per_image(focalLength, B, np.float32, "focalLength")
+    cx, cy = _per_image(ppointX, B, np.float32, "ppointX"), _per_image(ppointY, B, np.float32, "ppointY")
+    co = [_Arg(t) for t in sceneCoordinates]
+    og = [_Arg(t, writable=True) for t in outGradients]
+    ha = _Arg(hypAssignment)
+    gt = _Arg(gtPoses)
+    M = int(hypAssignment.shape[1])
+    ctx = _pick_ctx(*(a.device for a in co + og), ha.device, gt.device)
+    losses = np.zeros(B, np.float64)
+    hs, ws = _dims(shapes, 2), _dims(shapes, 3)
+    ctx.check(ctx.lib.esacb200_backward_ragged(ctx.handle, B, _ptr_array(co), _ptr_array(og), hs.ctypes.data, ws.ctypes.data, E,
+                                               ha.ptr, 1, M, gt.ptr, float(wLossRot), float(wLossTrans), float(lossCut),
+                                               sx.ctypes.data, sy.ctypes.data, fs.ctypes.data, cx.ctypes.data, cy.ctypes.data,
+                                               float(inlierThreshold), float(inlierAlpha), float(inlierBeta), float(maxReproj),
+                                               int(subSampling), losses.ctypes.data))
+    for a in og:
+        a.finish()
     return [float(v) for v in losses]
 
 
@@ -607,7 +728,12 @@ def reproj_loss(prediction, gtPoses, focalLength, padX, padY, cutLoss, subSampli
     reference has B = 1), gtPoses [B,4,4] float32 camera->world, padX / padY an int or B ints (the random shift),
     outGradients [B,3,H,W] float32 written in place (overwritten) or None.  focalLength, ppointX and ppointY are a number
     or B values (one camera per image, e.g. the DataLoader's `focallength`); the principal point defaults to the centre
-    of the sub*W x sub*H image (ref_expert.py:118-119).  Returns the B losses."""
+    of the sub*W x sub*H image (ref_expert.py:118-119).  Returns the B losses.
+    prediction (and outGradients) may also be lists or tuples of B [3,H_b,W_b] tensors (a ragged batch); the default
+    principal point is then each image's own centre, and image b gives bitwise the loss and gradient of a call on it alone."""
+    if _is_list(prediction) or _is_list(outGradients):
+        return _reproj_loss_ragged(prediction, gtPoses, focalLength, padX, padY, cutLoss, subSampling, ppointX, ppointY,
+                                   outGradients, maxReproj, minDepth)
     _check(prediction, "Float", 4, "prediction")
     _check(gtPoses, "Float", 3, "gtPoses")
     B, C3, H, W = (int(v) for v in prediction.shape)
@@ -643,6 +769,43 @@ def reproj_loss(prediction, gtPoses, focalLength, padX, padY, cutLoss, subSampli
     return [float(v) for v in losses]
 
 
+def _reproj_loss_ragged(prediction, gtPoses, focalLength, padX, padY, cutLoss, subSampling, ppointX, ppointY, outGradients,
+                        maxReproj, minDepth):
+    shapes = _check_list(prediction, 3, "prediction")
+    B = len(shapes)
+    for b, s in enumerate(shapes):
+        if s[0] != 3:
+            raise RuntimeError(f"prediction[{b}] must be [3,H,W], got {list(s)}")
+    _check(gtPoses, "Float", 3, "gtPoses")
+    if tuple(gtPoses.shape) != (B, 4, 4):
+        raise RuntimeError(f"a list of {B} predictions needs gtPoses [{B},4,4]")
+    og = None
+    if outGradients is not None:
+        gshapes = _check_list(outGradients, 3, "outGradients", B)
+        for b in range(B):
+            if gshapes[b] != shapes[b]:
+                raise RuntimeError(f"outGradients[{b}] is {list(gshapes[b])}, prediction[{b}] is {list(shapes[b])}")
+        og = [_Arg(t, writable=True) for t in outGradients]
+    sx, sy = _per_image(padX, B, np.int32, "padX"), _per_image(padY, B, np.int32, "padY")
+    fs = _per_image(focalLength, B, np.float32, "focalLength")
+    # the default principal point is the centre of each image's own sub*W x sub*H frame
+    ppx = [s[2] * subSampling / 2 for s in shapes] if ppointX is None else ppointX
+    ppy = [s[1] * subSampling / 2 for s in shapes] if ppointY is None else ppointY
+    cx, cy = _per_image(ppx, B, np.float32, "ppointX"), _per_image(ppy, B, np.float32, "ppointY")
+    pr = [_Arg(t) for t in prediction]
+    gt = _Arg(gtPoses)
+    ctx = _pick_ctx(*(a.device for a in pr + (og or [])), gt.device)
+    losses = np.zeros(B, np.float64)
+    hs, ws = _dims(shapes, 1), _dims(shapes, 2)
+    ctx.check(ctx.lib.esacb200_reproj_loss_ragged(ctx.handle, B, _ptr_array(pr), _ptr_array(og) if og else None, hs.ctypes.data,
+                                                  ws.ctypes.data, gt.ptr, sx.ctypes.data, sy.ctypes.data, fs.ctypes.data,
+                                                  cx.ctypes.data, cy.ctypes.data, int(subSampling), float(cutLoss),
+                                                  float(maxReproj), float(minDepth), losses.ctypes.data))
+    for a in og or []:
+        a.finish()
+    return [float(v) for v in losses]
+
+
 def coord_loss(prediction, gtCoords, cutLoss=100.0, outGradients=None, return_counts=False):
     """The robust scene-coordinate loss of init_expert.py:106-130 and, when outGradients is given, d loss / d prediction in
     the same call (what `robust_loss.backward()` hands to the expert, :132).  prediction [B,3,Hp,Wp] float32 (the reference
@@ -650,7 +813,11 @@ def coord_loss(prediction, gtCoords, cutLoss=100.0, outGradients=None, return_co
     top-left window (util.assert_size).  Cells whose ground truth is all zero do not count; the loss of an image is the sum
     over its valid cells divided by their number (NaN if there is none).  outGradients [B,3,Hp,Wp] float32 is overwritten
     (0 outside the window and on invalid cells) or None for the loss alone.  Returns the B losses, and with return_counts
-    also the B valid-cell counts."""
+    also the B valid-cell counts.
+    prediction, gtCoords (and outGradients) may also all be lists or tuples of B [3,H_b,W_b] tensors (a ragged batch), each
+    pair at most 1 apart; image b gives bitwise the loss and gradient of a call on it alone."""
+    if _is_list(prediction) or _is_list(gtCoords) or _is_list(outGradients):
+        return _coord_loss_ragged(prediction, gtCoords, cutLoss, outGradients, return_counts)
     _check(prediction, "Float", 4, "prediction")
     _check(gtCoords, "Float", 4, "gtCoords")
     B, C3, Hp, Wp = (int(v) for v in prediction.shape)
@@ -674,6 +841,39 @@ def coord_loss(prediction, gtCoords, cutLoss=100.0, outGradients=None, return_co
                                           losses.ctypes.data, counts.ctypes.data))
     if og:
         og.finish()
+    out = [float(v) for v in losses]
+    return (out, [int(v) for v in counts]) if return_counts else out
+
+
+def _coord_loss_ragged(prediction, gtCoords, cutLoss, outGradients, return_counts):
+    shapes = _check_list(prediction, 3, "prediction")
+    B = len(shapes)
+    gshapes = _check_list(gtCoords, 3, "gtCoords", B)
+    for b in range(B):
+        (c, hp, wp), (cg, hg, wg) = shapes[b], gshapes[b]
+        if c != 3 or cg != 3:
+            raise RuntimeError(f"prediction[{b}] / gtCoords[{b}] must be [3,H,W], got {list(shapes[b])} and {list(gshapes[b])}")
+        if abs(hp - hg) > 1 or abs(wp - wg) > 1:
+            raise RuntimeError(f"image {b}: tensor size mismatch: prediction {hp}x{wp}, ground truth {hg}x{wg} "
+                               "(util.assert_size allows 1)")
+    og = None
+    if outGradients is not None:
+        oshapes = _check_list(outGradients, 3, "outGradients", B)
+        for b in range(B):
+            if oshapes[b] != shapes[b]:
+                raise RuntimeError(f"outGradients[{b}] is {list(oshapes[b])}, prediction[{b}] is {list(shapes[b])}")
+        og = [_Arg(t, writable=True) for t in outGradients]
+    pr = [_Arg(t) for t in prediction]
+    gt = [_Arg(t) for t in gtCoords]
+    ctx = _pick_ctx(*(a.device for a in pr + gt + (og or [])))
+    losses = np.zeros(B, np.float64)
+    counts = np.zeros(B, np.int64)
+    hp, wp, hg, wg = _dims(shapes, 1), _dims(shapes, 2), _dims(gshapes, 1), _dims(gshapes, 2)
+    ctx.check(ctx.lib.esacb200_coord_loss_ragged(ctx.handle, B, _ptr_array(pr), hp.ctypes.data, wp.ctypes.data, _ptr_array(gt),
+                                                 hg.ctypes.data, wg.ctypes.data, _ptr_array(og) if og else None, float(cutLoss),
+                                                 losses.ctypes.data, counts.ctypes.data))
+    for a in og or []:
+        a.finish()
     out = [float(v) for v in losses]
     return (out, [int(v) for v in counts]) if return_counts else out
 

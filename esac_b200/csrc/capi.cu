@@ -10,8 +10,10 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <exception>
 #include <new>
+#include <string>
 #include <vector>
 #include <thread>
 #include <chrono>
@@ -278,8 +280,8 @@ int upload_inputs(esacb200_ctx* ctx, Plan& pl, const float* coords, const int64_
     return 0;
 }
 
-// Scoring launch shape, workspace, prep kernel.
-int plan_and_prep(esacb200_ctx* ctx, Plan& pl) {
+// Scoring launch shape (no device work).
+void plan_launch(esacb200_ctx* ctx, Plan& pl) {
     const Problem& P = pl.P;
     // scoring launch shape
     int ppt = 8, hc = 64;
@@ -301,7 +303,12 @@ int plan_and_prep(esacb200_ctx* ctx, Plan& pl) {
     pl.grid = (int)(it < 2ll * ctx->sm_count ? it : 2ll * ctx->sm_count);
     const int need_align = ppt >= 4 ? 4 : 2;
     pl.vec_ok = (P.N % need_align == 0) && (((uintptr_t)pl.d_coords) % (need_align * 4) == 0);
+}
 
+// Scoring launch shape, workspace, prep kernel.
+int plan_and_prep(esacb200_ctx* ctx, Plan& pl) {
+    const Problem& P = pl.P;
+    plan_launch(ctx, pl);
     CK(ctx->assign32.ensure((size_t)P.M * 4));
     CK(ctx->counts.ensure((size_t)P.E * 4));
     CK(ctx->offsets.ensure((size_t)(P.E + 1) * 4));
@@ -322,7 +329,7 @@ int plan_and_prep(esacb200_ctx* ctx, Plan& pl) {
     CK(ctx->contrib.ensure((size_t)P.M * 4));
     CK(ctx->out17.ensure(32 * 4));
     int* sc = ctx->scalars.as<int>();
-    launch_prep(pl.d_coords, pl.d_assign, pl.assign_stride, P, hc, ctx->assign32.as<int>(), ctx->counts.as<int>(),
+    launch_prep(pl.d_coords, pl.d_assign, pl.assign_stride, P, pl.hc, ctx->assign32.as<int>(), ctx->counts.as<int>(),
                 ctx->offsets.as<int>(), ctx->perm.as<int>(), ctx->slot_of.as<int>(), ctx->chunks.as<ChunkDesc>(),
                 sc + S_NCHUNKS, sc + S_WORK, ctx->centres.as<float>(), sc + S_FLAGS, pl.split_e ? 1 : 3, ctx->stream);
     ctx->st.kernel_launches += 1;
@@ -337,19 +344,39 @@ int stage_inputs(esacb200_ctx* ctx, Plan& pl, const float* coords, const int64_t
     return plan_and_prep(ctx, pl);
 }
 
-int run_sample(esacb200_ctx* ctx, const Plan& pl, uint64_t seed) {
+constexpr int kSampleCap = 1 << 19;     // survivors per lane
+constexpr int kSampleCapAcc = 1 << 15;  // staged accepts per lane
+
+// Lanes of the sampling stage and its workspace: ints (smp_int) and survivor / staging bytes (smp_surv).
+struct SampleSizes {
+    int G, Mg;
+    size_t per_group_ints, int_bytes, per_group_bytes, surv_bytes;
+};
+SampleSizes sample_sizes(const esacb200_ctx* ctx, const Plan& pl) {
     const Problem& P = pl.P;
-    const int cap = 1 << 19;       // per group
-    const int cap_acc = 1 << 15;
+    SampleSizes z;
     // two lanes pay once a wave's kernels are long enough to overlap (full-resolution maps, or very many hypotheses)
     int G = pl.split_e ? 2 : ((ctx->sample_groups > 1 && ctx->aux_stream && P.M >= 64 && (P.N >= 65536 || P.M >= 1024)) ? ctx->sample_groups : 1);
     if (G > 2 && (!ctx->aux_more[0] || !ctx->aux_more[1] || P.M < 512)) G = 2;
-    const int Mg = pl.split_e ? P.M : (P.M + G - 1) / G;  // capacity of a lane's work list
+    z.G = G;
+    z.Mg = pl.split_e ? P.M : (P.M + G - 1) / G;  // capacity of a lane's work list
     // ints: [best: 2M] [base: M] [ovf: M] then per group [list: 2*Mg] [counters: 8]
-    const size_t per_group_ints = (size_t)2 * Mg + 8;
-    CK(ctx->smp_int.ensure(((size_t)P.M * 4 + G * per_group_ints) * 4 + 8));
-    const size_t per_group_bytes = (size_t)cap * sizeof(int2) + (size_t)cap_acc * sizeof(Accepted);
-    CK(ctx->smp_surv.ensure(G * per_group_bytes));
+    z.per_group_ints = (size_t)2 * z.Mg + 8;
+    z.int_bytes = ((size_t)P.M * 4 + G * z.per_group_ints) * 4 + 8;
+    z.per_group_bytes = (size_t)kSampleCap * sizeof(int2) + (size_t)kSampleCapAcc * sizeof(Accepted);
+    z.surv_bytes = G * z.per_group_bytes;
+    return z;
+}
+
+int run_sample(esacb200_ctx* ctx, const Plan& pl, uint64_t seed) {
+    const Problem& P = pl.P;
+    const int cap = kSampleCap;
+    const int cap_acc = kSampleCapAcc;
+    const SampleSizes z = sample_sizes(ctx, pl);
+    const int G = z.G, Mg = z.Mg;
+    const size_t per_group_ints = z.per_group_ints, per_group_bytes = z.per_group_bytes;
+    CK(ctx->smp_int.ensure(z.int_bytes));
+    CK(ctx->smp_surv.ensure(z.surv_bytes));
     SampleState st[4];
     int* b = ctx->smp_int.as<int>() + 2 * (size_t)P.M;
     for (int g = 0; g < G; ++g) {
@@ -449,20 +476,43 @@ int pick_group(esacb200_ctx* ctx, const Problem& P, int jobs_hint) {
 }
 
 // Refinement of `n_jobs` (host count, or device scalar when d_njobs != null) hypotheses listed in d_jobs.
-int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, const int* d_jobs, const int* d_njobs,
-               int n_jobs_host, int max_jobs, int group) {
-    const Problem& P = pl.P;
+// Groups of the refinement kernel and its workspace (bytes; clist = 0 when the kernel does not use it).
+struct RefineSizes {
+    int n_groups, cache;
+    size_t masks, rounds, scratch, n_flags, barrier, clist;
+};
+RefineSizes refine_sizes(const esacb200_ctx* ctx, const Problem& P, int max_jobs, int group) {
+    RefineSizes z;
     const int words = (P.N + 31) / 32;
     int n_groups = ctx->refine_coresident / group;
     if (n_groups > max_jobs) n_groups = max_jobs;
     if (n_groups < 1) n_groups = 1;
-    CK(ctx->masks.ensure((size_t)max_jobs * 2 * words * 4));
-    CK(ctx->rounds.ensure((size_t)max_jobs * 2 * 4));
-    CK(ctx->scratch.ensure(refine_scratch_doubles(n_groups, group) * 8));
+    z.n_groups = n_groups;
+    z.masks = (size_t)max_jobs * 2 * words * 4;
+    z.rounds = (size_t)max_jobs * 2 * 4;
+    z.scratch = refine_scratch_doubles(n_groups, group) * 8;
+    z.n_flags = refine_flag_words(n_groups, group);
+    z.barrier = (z.n_flags + 4) * 4;
+    const int wpc = (words + group - 1) / group;
+    z.cache = wpc <= refine_cache_words() ? 1 : 0;
+    z.clist = (ctx->refine_compact && !z.cache && wpc <= refine_max_compact_words())
+                  ? (size_t)n_groups * words * 32 * sizeof(unsigned short) : 0;
+    return z;
+}
+
+int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, const int* d_jobs, const int* d_njobs,
+               int n_jobs_host, int max_jobs, int group) {
+    const Problem& P = pl.P;
+    const int words = (P.N + 31) / 32;
+    const RefineSizes z = refine_sizes(ctx, P, max_jobs, group);
+    const int n_groups = z.n_groups;
+    CK(ctx->masks.ensure(z.masks));
+    CK(ctx->rounds.ensure(z.rounds));
+    CK(ctx->scratch.ensure(z.scratch));
     if (group > 1) CK(cudaMemsetAsync(ctx->scratch.p, 0, refine_scratch_doubles(n_groups, group) * 8, ctx->stream));  // LL elements: no stale sequence numbers
-    const size_t n_flags = refine_flag_words(n_groups, group);
-    CK(ctx->barrier.ensure((n_flags + 4) * 4));
-    CK(cudaMemsetAsync(ctx->barrier.p, 0, (n_flags + 4) * 4, ctx->stream));
+    const size_t n_flags = z.n_flags;
+    CK(ctx->barrier.ensure(z.barrier));
+    CK(cudaMemsetAsync(ctx->barrier.p, 0, z.barrier, ctx->stream));
     RefineArgs a;
     a.coords = pl.d_coords;
     a.centres = ctx->centres.as<float>();
@@ -479,13 +529,12 @@ int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, con
     a.barrier = ctx->barrier.as<unsigned int>();
     a.job_counter = (int*)(ctx->barrier.as<unsigned int>() + n_flags);
     a.group = group;
-    const int wpc = (words + group - 1) / group;
-    a.cache = wpc <= refine_cache_words() ? 1 : 0;
+    a.cache = z.cache;
     a.compact = ctx->refine_compact;
     a.pretest = ctx->refine_pretest;
     a.clist = nullptr;
-    if (a.compact && !a.cache && wpc <= refine_max_compact_words()) {
-        CK(ctx->clist.ensure((size_t)n_groups * words * 32 * sizeof(unsigned short)));
+    if (z.clist) {
+        CK(ctx->clist.ensure(z.clist));
         a.clist = ctx->clist.as<unsigned short>();
     }
     a.prof = nullptr;
@@ -526,6 +575,133 @@ int enqueue_forward_core(esacb200_ctx* ctx, const Plan& pl, float* d_out17) {
     launch_finish_forward(ctx->poses_ref.as<Pose>(), sc + S_WINNER, ctx->assign32.as<int>(), sc + S_FLAGS, d_out17, ctx->stream);
     ctx->st.kernel_launches += 1;
     return 0;
+}
+
+// Sizes every workspace buffer of the forward pipeline (upload, plan_and_prep, sampling, refinement) for the largest of a
+// batch's images before the first one is enqueued: DevBuf::ensure growing mid-batch frees the old buffer, and cudaFree
+// synchronises the device, which would serialise the copy stream's overlap with the previous image.
+int reserve_forward_batch(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool host_coords) {
+    size_t part = 0, cbytes = 0, c4 = 0, sint = 0, ssurv = 0, masks = 0, rounds = 0, scratch = 0, barrier = 0, clist = 0;
+    auto mx = [](size_t& a, size_t b) { if (b > a) a = b; };
+    int M = 0, E = 0;
+    for (Plan pl : plans) {
+        plan_launch(ctx, pl);
+        const Problem& P = pl.P;
+        M = P.M; E = P.E;
+        mx(part, (size_t)P.M * pl.T * 4);
+        mx(cbytes, (size_t)P.E * 3 * P.N * sizeof(float));
+        mx(c4, (size_t)P.E * P.N * sizeof(float4));
+        const SampleSizes a = sample_sizes(ctx, pl);
+        mx(sint, a.int_bytes);
+        mx(ssurv, a.surv_bytes);
+        const RefineSizes r = refine_sizes(ctx, P, 1, pick_group(ctx, P, 1));
+        mx(masks, r.masks); mx(rounds, r.rounds); mx(scratch, r.scratch); mx(barrier, r.barrier); mx(clist, r.clist);
+    }
+    if (host_coords) {
+        CK(ctx->coords.ensure(cbytes));
+        CK(ctx->coords_alt.ensure(cbytes));
+    }
+    CK(ctx->assign64.ensure((size_t)M * 8));
+    CK(ctx->assign64_alt.ensure((size_t)M * 8));
+    CK(ctx->assign32.ensure((size_t)M * 4));
+    CK(ctx->counts.ensure((size_t)E * 4));
+    CK(ctx->offsets.ensure((size_t)(E + 1) * 4));
+    CK(ctx->perm.ensure((size_t)M * 4));
+    CK(ctx->slot_of.ensure((size_t)M * 4));
+    CK(ctx->chunks.ensure((size_t)(M + E) * sizeof(ChunkDesc)));
+    CK(ctx->scalars.ensure(S_COUNT * 4));
+    CK(ctx->centres.ensure((size_t)E * 3 * 4));
+    CK(ctx->poses.ensure((size_t)M * sizeof(Pose)));
+    CK(ctx->poses_ref.ensure((size_t)M * sizeof(Pose)));
+    CK(ctx->cells.ensure((size_t)M * 8 * 4));
+    CK(ctx->tries.ensure((size_t)M * 4));
+    CK(ctx->posepk.ensure((size_t)M * sizeof(PosePk)));
+    CK(ctx->part.ensure(part));
+    CK(ctx->scores.ensure((size_t)M * 8));
+    CK(ctx->probs.ensure((size_t)M * 8));
+    CK(ctx->stats.ensure(8 * 8));
+    CK(ctx->contrib.ensure((size_t)M * 4));
+    CK(ctx->out17.ensure(32 * 4));
+    CK(ctx->smp_int.ensure(sint));
+    CK(ctx->smp_surv.ensure(ssurv));
+    CK(ctx->coords4.ensure(c4));
+    CK(ctx->masks.ensure(masks));
+    CK(ctx->rounds.ensure(rounds));
+    CK(ctx->scratch.ensure(scratch));
+    CK(ctx->barrier.ensure(barrier));
+    if (clist) CK(ctx->clist.ensure(clist));
+    return 0;
+}
+
+// All B pointers of one argument on the device, or all on the host (a mix is an error).  None may be null.
+int pointer_kind(esacb200_ctx* ctx, const void* const* p, int B, const char* what, bool& device) {
+    for (int b = 0; b < B; ++b) {
+        if (!p[b]) return fail(ctx, ESACB200_ERR_ARG, "image %d: %s is null", b, what);
+        const bool d = is_device_ptr(p[b]);
+        if (b == 0) device = d;
+        else if (d != device)
+            return fail(ctx, ESACB200_ERR_ARG, "%s mixes host and device pointers (image 0: %s, image %d: %s)", what,
+                        device ? "device" : "host", b, d ? "device" : "host");
+    }
+    return 0;
+}
+
+// Offsets of B host images packed into one device buffer, each at a 16-byte aligned offset (so that an image keeps the
+// 128-bit load path a single-image call would give it).  Returns the total.
+size_t pack_offsets(const std::vector<size_t>& bytes, std::vector<size_t>& off) {
+    size_t total = 0;
+    off.resize(bytes.size());
+    for (size_t b = 0; b < bytes.size(); ++b) {
+        off[b] = total;
+        total += (bytes[b] + 15) & ~(size_t)15;
+    }
+    return total;
+}
+
+// Copies between B host images and their packed device copies; runs of images that lie back to back on both sides go as
+// one copy (a stacked tensor with N % 4 == 0 is a single copy).
+int copy_packed(esacb200_ctx* ctx, char* const* host, const std::vector<size_t>& bytes, const std::vector<size_t>& off, char* dev,
+                bool to_device, cudaStream_t stream) {
+    const size_t B = bytes.size();
+    for (size_t b = 0; b < B;) {
+        size_t e = b + 1, len = bytes[b];
+        while (e < B && host[e] == host[e - 1] + bytes[e - 1] && off[e] == off[e - 1] + bytes[e - 1]) len += bytes[e++];
+        if (to_device) CK(cudaMemcpyAsync(dev + off[b], host[b], len, cudaMemcpyHostToDevice, stream));
+        else CK(cudaMemcpyAsync(host[b], dev + off[b], len, cudaMemcpyDeviceToHost, stream));
+        b = e;
+    }
+    return 0;
+}
+
+// Stages the B images of one argument on the device: device pointers are used as they are; host images are packed into
+// `buf` at 16-byte aligned offsets (and copied there when `upload`).  dev[b] receives image b's device address.
+template <class T>
+int stage_images(esacb200_ctx* ctx, T* const* ptrs, const std::vector<size_t>& bytes, bool device, bool upload, DevBuf& buf,
+                 std::vector<T*>& dev, std::vector<size_t>& off) {
+    const size_t B = bytes.size();
+    dev.resize(B);
+    if (device) {
+        for (size_t b = 0; b < B; ++b) dev[b] = ptrs[b];
+        return 0;
+    }
+    CK(buf.ensure(pack_offsets(bytes, off)));
+    for (size_t b = 0; b < B; ++b) dev[b] = (T*)((char*)buf.p + off[b]);
+    if (upload) return copy_packed(ctx, (char* const*)ptrs, bytes, off, (char*)buf.p, true, ctx->stream);
+    return 0;
+}
+
+// Orders a loss call's per-image records by load path (128-bit first) so that each path is one launch over a contiguous
+// slice of the table; returns the bytes of the table.
+template <class Rec>
+size_t order_by_path(const std::vector<Rec>& recs, const std::vector<char>& vec, std::vector<Rec>& out, int& n_vec, int& max_vec,
+                     int& max_sc) {
+    out.clear();
+    n_vec = max_vec = max_sc = 0;
+    for (size_t i = 0; i < recs.size(); ++i)
+        if (vec[i]) { out.push_back(recs[i]); ++n_vec; if (recs[i].blocks > max_vec) max_vec = recs[i].blocks; }
+    for (size_t i = 0; i < recs.size(); ++i)
+        if (!vec[i]) { out.push_back(recs[i]); if (recs[i].blocks > max_sc) max_sc = recs[i].blocks; }
+    return out.size() * sizeof(Rec);
 }
 
 void begin_call(esacb200_ctx* ctx) {
@@ -869,28 +1045,37 @@ int esacb200_forward_sharded(esacb200_ctx* ctx, const float* coords, int E, int 
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
-// esac_forward over a batch of B images of one shape (BASELINE configs[2]: "batch 8 images").  The reference has no such
-// entry: its callers loop over a DataLoader with batch_size=1 (test_esac.py:137).  Images are processed back to back on
-// the compute stream with ONE host synchronisation at the end; host coordinate maps are double-buffered and copied on a
-// second stream so the copy of image b+1 overlaps the kernels of image b.  Image b runs with its own shift and camera:
-// the pipeline of one image reads them from its Problem, so only the loop below sees the arrays.
-int esacb200_forward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
-                                   int64_t assign_stride, int M, float* out_poses, const int* shiftX, const int* shiftY,
-                                   const float* f, const float* ppx, const float* ppy, float tau, float alpha, float beta,
-                                   float maxReproj, int sub, int* out_experts) try {
+// esac_forward over a batch of B images (BASELINE configs[2]: "batch 8 images").  The reference has no such entry: its
+// callers loop over a DataLoader with batch_size=1 (test_esac.py:137).  Images are processed back to back on the compute
+// stream with ONE host synchronisation at the end; host coordinate maps are double-buffered and copied on a second stream
+// so the copy of image b+1 overlaps the kernels of image b.  Image b runs with its own map size, shift and camera: the
+// pipeline of one image reads them from its Problem, so only the loop below sees the arrays.  The workspace is sized for
+// the largest image before the first one is enqueued.
+int esacb200_forward_ragged(esacb200_ctx* ctx, int B, const float* const* coords, const int* H, const int* W, int E,
+                            const int64_t* assign, int64_t assign_stride, int M, float* out_poses, const int* shiftX,
+                            const int* shiftY, const float* f, const float* ppx, const float* ppy, float tau, float alpha,
+                            float beta, float maxReproj, int sub, int* out_experts) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
-    if (!coords || !assign || !out_poses || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
+    if (!coords || !H || !W || !assign || !out_poses || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
-    Plan pl;
-    int rc = fill_problem(ctx, pl.P, E, H, W, M, 0, 0, f[0], ppx[0], ppy[0], tau, alpha, beta, maxReproj, sub);
+    std::vector<Plan> plans((size_t)B);
+    for (int b = 0; b < B; ++b) {
+        Plan& pl = plans[b];
+        int rc = fill_problem(ctx, pl.P, E, H[b], W[b], M, shiftX ? shiftX[b] : 0, shiftY ? shiftY[b] : 0, f[b], ppx[b], ppy[b], tau,
+                              alpha, beta, maxReproj, sub);
+        if (rc) return fail(ctx, rc, "image %d: %s", b, std::string(ctx->err).c_str());
+        if ((long long)(W[b] - 1) * (H[b] - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too small", b, W[b], H[b]);
+        pl.d_coords = nullptr;
+    }
+    bool dev_coords = false;
+    int rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_coords);
     if (rc) return rc;
-    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small", W, H);
+    const bool host_coords = !dev_coords;
     begin_call(ctx);
     ctx->inj_M = ctx->inj_T = 0;
-    const size_t cstride = (size_t)E * 3 * H * W;
-    const bool host_coords = !is_device_ptr(coords);
-    const bool host_assign = !is_device_ptr(assign);
+    rc = reserve_forward_batch(ctx, plans, host_coords);
+    if (rc) return rc;
     // element stride between the assignments of consecutive images: rows of a [B, M] tensor
     const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
     CK(ctx->out_batch.ensure((size_t)B * 20 * sizeof(float)));
@@ -898,21 +1083,16 @@ int esacb200_forward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords
     DevBuf* ab[2] = {&ctx->assign64, &ctx->assign64_alt};
     for (int b = 0; b < B; ++b) {
         const int buf = b & 1;
+        Plan& pl = plans[b];
         if (host_coords && b >= 2) CK(cudaStreamWaitEvent(ctx->copy_stream, ctx->ev_consumed[buf], 0));
-        rc = upload_inputs(ctx, pl, coords + (size_t)b * cstride, assign + (size_t)b * arow, assign_stride, *cb[buf], *ab[buf],
+        rc = upload_inputs(ctx, pl, coords[b], assign + (size_t)b * arow, assign_stride, *cb[buf], *ab[buf],
                            host_coords ? ctx->copy_stream : ctx->stream);
         if (rc) return rc;
         if (host_coords) {
             CK(cudaEventRecord(ctx->ev_copied[buf], ctx->copy_stream));
             CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_copied[buf], 0));
         }
-        (void)host_assign;
         if (b == 0) mark(ctx, EV_H2D);
-        pl.P.shiftX = shiftX ? shiftX[b] : 0;
-        pl.P.shiftY = shiftY ? shiftY[b] : 0;
-        pl.P.f = f[b];
-        pl.P.ppx = ppx[b];
-        pl.P.ppy = ppy[b];
         rc = plan_and_prep(ctx, pl);
         if (rc) return rc;
         rc = enqueue_forward_core(ctx, pl, ctx->out_batch.as<float>() + (size_t)b * 20);
@@ -940,6 +1120,26 @@ int esacb200_forward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords
     ctx->last_backward = false;
     finish_stats(ctx);
     return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+// B images of one shape: the pointer and size arrays of a [B,E,3,H,W] tensor.
+int esacb200_forward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
+                                   int64_t assign_stride, int M, float* out_poses, const int* shiftX, const int* shiftY,
+                                   const float* f, const float* ppx, const float* ppy, float tau, float alpha, float beta,
+                                   float maxReproj, int sub, int* out_experts) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    if (!coords || !assign || !out_poses || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
+    if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
+    Problem P;
+    int rc = fill_problem(ctx, P, E, H, W, M, 0, 0, f[0], ppx[0], ppy[0], tau, alpha, beta, maxReproj, sub);
+    if (rc) return rc;
+    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small", W, H);
+    const size_t cstride = (size_t)E * 3 * H * W;
+    std::vector<const float*> ptrs((size_t)B);
+    for (int b = 0; b < B; ++b) ptrs[b] = coords + (size_t)b * cstride;
+    const std::vector<int> hs((size_t)B, H), ws((size_t)B, W);
+    return esacb200_forward_ragged(ctx, B, ptrs.data(), hs.data(), ws.data(), E, assign, assign_stride, M, out_poses, shiftX, shiftY,
+                                   f, ppx, ppy, tau, alpha, beta, maxReproj, sub, out_experts);
 } ESAC_ABI_CATCH(ctx)
 
 // One camera for the whole batch: broadcast to B entries.
@@ -1320,19 +1520,31 @@ int esacb200_backward_sharded_nccl(esacb200_ctx* ctx, const float* coords, float
 // -------------------------------------------------------------------------------------------------
 // esac_backward over a batch.  Every image is an independent problem (SURVEY 8e: "images in a batch are fully
 // independent"), so the images are dealt round-robin to a few worker contexts, each driven by its own host thread on its
-// own stream: the small kernels of one image fill the gaps the host synchronisations of another leave.
-int esacb200_backward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords, float* grads, int E, int H, int W,
-                                    const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wRot,
-                                    float wTrans, float cut, const int* shiftX, const int* shiftY, const float* f,
-                                    const float* ppx, const float* ppy, float tau, float alpha, float beta, float maxReproj,
-                                    int sub, double* out_losses) try {
+// own stream: the small kernels of one image fill the gaps the host synchronisations of another leave.  Image b has its own
+// map size; the seeds are fixed per image before the images are dealt, so a worker runs its images largest first and its
+// workspace grows at most once.
+int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H, const int* W,
+                             int E, const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wRot,
+                             float wTrans, float cut, const int* shiftX, const int* shiftY, const float* f, const float* ppx,
+                             const float* ppy, float tau, float alpha, float beta, float maxReproj, int sub,
+                             double* out_losses) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
-    if (!coords || !grads || !assign || !gt_poses || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
+    if (!coords || !grads || !H || !W || !assign || !gt_poses || B <= 0)
+        return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
     if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
-    if (E <= 0 || H <= 0 || W <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d H=%d W=%d M=%d", E, H, W, M);
-    const size_t cstride = (size_t)E * 3 * H * W;
+    if (E <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d M=%d", E, M);
+    for (int b = 0; b < B; ++b) {
+        if (H[b] <= 0 || W[b] <= 0) return fail(ctx, ESACB200_ERR_ARG, "image %d: bad size %dx%d", b, W[b], H[b]);
+        if ((long long)H[b] * W[b] > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too large", b, W[b], H[b]);
+        if ((long long)(W[b] - 1) * (H[b] - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too small", b, W[b], H[b]);
+    }
+    bool dev_c = false, dev_g = false;
+    int rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
+    if (rc) return rc;
+    rc = pointer_kind(ctx, (const void* const*)grads, B, "grads", dev_g);
+    if (rc) return rc;
     const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
     std::vector<float> gt_host;
     const float* gt = gt_poses;
@@ -1372,18 +1584,22 @@ int esacb200_backward_batch_cameras(esacb200_ctx* ctx, int B, const float* coord
         w->score_ppt_opt = ctx->score_ppt_opt;
         w->score_hc_opt = ctx->score_hc_opt;
         w->fixed_seed = 1;
-        for (int b = wi; b < B; b += nw) {
+        // this worker's images (dealt round-robin), largest first: the workspace grows at most once
+        std::vector<int> mine;
+        for (int b = wi; b < B; b += nw) mine.push_back(b);
+        std::stable_sort(mine.begin(), mine.end(), [&](int a, int c) { return (long long)H[a] * W[a] > (long long)H[c] * W[c]; });
+        for (int b : mine) {
             w->seed = seeds[b];
             double loss = 0;
-            int rc = backward_impl(w, coords + (size_t)b * cstride, grads + (size_t)b * cstride, E, H, W, assign + (size_t)b * arow,
+            int rc = backward_impl(w, coords[b], grads[b], E, H[b], W[b], assign + (size_t)b * arow,
                                    assign_stride, M, gt + (size_t)b * 16, wRot, wTrans, cut, shiftX ? shiftX[b] : 0,
                                    shiftY ? shiftY[b] : 0, f[b], ppx[b], ppy[b], tau, alpha, beta, maxReproj, sub, nullptr, nullptr,
                                    &loss);
             if (rc) { rcs[wi] = rc; failed_at[wi] = b; return; }
             if (out_losses) out_losses[b] = loss;
             launches[wi] += w->st.kernel_launches;
+            if (b == B - 1) last[wi] = w->st;
         }
-        last[wi] = w->st;
         } catch (...) {  // an exception escaping a std::thread would terminate the process
             rcs[wi] = ESACB200_ERR_ARG;
             failed_at[wi] = -1;
@@ -1401,7 +1617,7 @@ int esacb200_backward_batch_cameras(esacb200_ctx* ctx, int B, const float* coord
     const double wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     for (int wi = 0; wi < nw; ++wi)
         if (rcs[wi]) return fail(ctx, rcs[wi], "image %d: %s", failed_at[wi], ctx->workers[wi]->err);
-    // statistics of the call: those of the worker that handled the last image, wall time and launches of the whole batch
+    // statistics of the call: those of the last image, wall time and launches of the whole batch
     ctx->st = last[(B - 1) % nw];
     unsigned long long total = 0;
     for (int wi = 0; wi < nw; ++wi) total += launches[wi];
@@ -1410,6 +1626,29 @@ int esacb200_backward_batch_cameras(esacb200_ctx* ctx, int B, const float* coord
     ctx->last_M = 0;  // the per-hypothesis buffers live in the workers
     ctx->last_backward = true;
     return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+// B images of one shape: the pointer and size arrays of [B,E,3,H,W] tensors.
+int esacb200_backward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords, float* grads, int E, int H, int W,
+                                    const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wRot,
+                                    float wTrans, float cut, const int* shiftX, const int* shiftY, const float* f,
+                                    const float* ppx, const float* ppy, float tau, float alpha, float beta, float maxReproj,
+                                    int sub, double* out_losses) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    if (!coords || !grads || !assign || !gt_poses || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
+    if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
+    if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
+    if (E <= 0 || H <= 0 || W <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d H=%d W=%d M=%d", E, H, W, M);
+    const size_t cstride = (size_t)E * 3 * H * W;
+    std::vector<const float*> cp((size_t)B);
+    std::vector<float*> gp((size_t)B);
+    for (int b = 0; b < B; ++b) {
+        cp[b] = coords + (size_t)b * cstride;
+        gp[b] = grads + (size_t)b * cstride;
+    }
+    const std::vector<int> hs((size_t)B, H), ws((size_t)B, W);
+    return esacb200_backward_ragged(ctx, B, cp.data(), gp.data(), hs.data(), ws.data(), E, assign, assign_stride, M, gt_poses, wRot,
+                                    wTrans, cut, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, out_losses);
 } ESAC_ABI_CATCH(ctx)
 
 int esacb200_backward_batch(esacb200_ctx* ctx, int B, const float* coords, float* grads, int E, int H, int W,
@@ -1459,30 +1698,33 @@ int esacb200_assign_hypotheses(esacb200_ctx* ctx, int B, int E, int M, const flo
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
-int esacb200_reproj_loss_cameras(esacb200_ctx* ctx, int B, const float* coords, float* grads, int H, int W, const float* gt_poses,
-                                 const int* shiftX, const int* shiftY, const float* f, const float* ppx, const float* ppy, int sub,
-                                 float cut, float maxReproj, float minDepth, double* out_losses) try {
+// The reprojection loss over B images, each with its own size: one launch per load path (128-bit / scalar, chosen per
+// image as a single-image call would choose it), each image cut into the blocks a single-image call uses.
+int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H,
+                                const int* W, const float* gt_poses, const int* shiftX, const int* shiftY, const float* f,
+                                const float* ppx, const float* ppy, int sub, float cut, float maxReproj, float minDepth,
+                                double* out_losses) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
-    if (!coords || !gt_poses || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    if (!coords || !H || !W || !gt_poses || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
-    if (B <= 0 || H <= 0 || W <= 0 || sub <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d H=%d W=%d sub=%d", B, H, W, sub);
-    if ((long long)H * W > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too large", W, H);
+    if (B <= 0 || sub <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d sub=%d", B, sub);
+    for (int b = 0; b < B; ++b) {
+        if (H[b] <= 0 || W[b] <= 0) return fail(ctx, ESACB200_ERR_ARG, "image %d: bad size %dx%d", b, W[b], H[b]);
+        if ((long long)H[b] * W[b] > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too large", b, W[b], H[b]);
+    }
+    bool c_dev = false, g_dev = false;
+    int rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", c_dev);
+    if (rc) return rc;
+    if (grads && (rc = pointer_kind(ctx, (const void* const*)grads, B, "grads", g_dev))) return rc;
     begin_call(ctx);
-    const int N = H * W;
-    const size_t cbytes = (size_t)B * 3 * N * sizeof(float);
-    const bool c_host = !is_device_ptr(coords), g_host = grads && !is_device_ptr(grads);
-    const float* d_coords = coords;
-    float* d_grads = grads;
-    if (c_host) {
-        CK(ctx->coords.ensure(cbytes));
-        CK(cudaMemcpyAsync(ctx->coords.p, coords, cbytes, cudaMemcpyHostToDevice, ctx->stream));
-        d_coords = ctx->coords.as<float>();
-    }
-    if (g_host) {
-        CK(ctx->grads.ensure(cbytes));
-        d_grads = ctx->grads.as<float>();
-    }
+    std::vector<size_t> bytes((size_t)B), c_off, g_off;
+    for (int b = 0; b < B; ++b) bytes[b] = (size_t)3 * H[b] * W[b] * sizeof(float);
+    std::vector<const float*> d_coords;
+    std::vector<float*> d_grads((size_t)B, nullptr);
+    rc = stage_images(ctx, coords, bytes, c_dev, true, ctx->coords, d_coords, c_off);
+    if (rc) return rc;
+    if (grads && (rc = stage_images(ctx, grads, bytes, g_dev, false, ctx->grads, d_grads, g_off))) return rc;
     std::vector<float> gt((size_t)B * 16);
     if (is_device_ptr(gt_poses)) {
         CK(cudaMemcpyAsync(gt.data(), gt_poses, gt.size() * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
@@ -1513,22 +1755,52 @@ int esacb200_reproj_loss_cameras(esacb200_ctx* ctx, int B, const float* coords, 
         o[15] = ppx[b];
         o[16] = ppy[b];
     }
-    const int bpi = reproj_blocks_per_image(N, B, ctx->sm_count);
-    // scratch layout: [tickets B u32, padded] [img B*kReprojImgFloats f32] [losses B f64] [partials B*bpi f64]
-    const size_t off_img = ((size_t)B * 4 + 63) & ~(size_t)63, off_loss = off_img + (((size_t)B * kReprojImgFloats * 4 + 63) & ~(size_t)63),
-                 off_part = off_loss + (((size_t)B * 8 + 63) & ~(size_t)63);
-    CK(ctx->scratch.ensure(off_part + (size_t)B * bpi * 8));
+    std::vector<ReprojImage> recs((size_t)B);
+    std::vector<char> vec((size_t)B);
+    long long parts = 0;
+    for (int b = 0; b < B; ++b) {
+        ReprojImage& r = recs[b];
+        r.coords = d_coords[b];
+        r.grads = d_grads[b];
+        r.N = H[b] * W[b];
+        r.W = W[b];
+        r.b = b;
+        r.blocks = reproj_blocks_per_image(r.N);
+        r.part0 = parts;
+        parts += r.blocks;
+        vec[b] = reproj_vec_ok(r.coords, r.grads, r.N, r.W);
+    }
+    std::vector<ReprojImage> ordered;
+    int n_vec, max_vec, max_sc;
+    const size_t rec_bytes = order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
+    // scratch layout: [tickets B u32, padded] [img B*kReprojImgFloats f32 | records, padded] [losses B f64] [partials f64]
+    const size_t img_bytes = img.size() * sizeof(float);
+    const size_t off_img = ((size_t)B * 4 + 63) & ~(size_t)63, off_rec = off_img + ((img_bytes + 15) & ~(size_t)15),
+                 off_loss = (off_rec + rec_bytes + 63) & ~(size_t)63, off_part = off_loss + (((size_t)B * 8 + 63) & ~(size_t)63);
+    CK(ctx->scratch.ensure(off_part + (size_t)parts * 8));
     char* base = (char*)ctx->scratch.p;
+    std::vector<char> staging(off_rec - off_img + rec_bytes);
+    memcpy(staging.data(), img.data(), img_bytes);
+    memcpy(staging.data() + (off_rec - off_img), ordered.data(), rec_bytes);
     CK(cudaMemsetAsync(base, 0, off_img, ctx->stream));
-    CK(cudaMemcpyAsync(base + off_img, img.data(), img.size() * sizeof(float), cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(base + off_img, staging.data(), staging.size(), cudaMemcpyHostToDevice, ctx->stream));
     mark(ctx, EV_H2D);
-    mark(ctx, EV_FOLD);  // ms_score = the kernel alone
-    launch_reproj(d_coords, d_grads, (const float*)(base + off_img), B, N, W, (float)sub, cut, maxReproj, minDepth, bpi,
-                  (double*)(base + off_part), (unsigned*)base, (double*)(base + off_loss), ctx->stream);
-    CK(cudaGetLastError());
-    ctx->st.kernel_launches += 1;
+    mark(ctx, EV_FOLD);  // ms_score = the kernels alone
+    const ReprojImage* d_rec = (const ReprojImage*)(base + off_rec);
+    for (int path = 0; path < 2; ++path) {
+        const int n = path == 0 ? n_vec : B - n_vec;
+        if (n == 0) continue;
+        launch_reproj(path == 0, d_rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, (const float*)(base + off_img),
+                      (float)sub, cut, maxReproj, minDepth, (double*)(base + off_part), (unsigned*)base, (double*)(base + off_loss),
+                      ctx->stream);
+        CK(cudaGetLastError());
+        ctx->st.kernel_launches += 1;
+    }
     mark(ctx, EV_SCORE);
-    if (g_host) CK(cudaMemcpyAsync(grads, d_grads, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (grads && !g_dev) {
+        rc = copy_packed(ctx, (char* const*)grads, bytes, g_off, (char*)ctx->grads.p, false, ctx->stream);
+        if (rc) return rc;
+    }
     CK(cudaMemcpyAsync(out_losses, base + off_loss, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1536,6 +1808,27 @@ int esacb200_reproj_loss_cameras(esacb200_ctx* ctx, int B, const float* coords, 
     ctx->last_M = 0;
     finish_stats(ctx);
     return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+// B images of one shape: the pointer and size arrays of a [B,3,H,W] tensor.
+int esacb200_reproj_loss_cameras(esacb200_ctx* ctx, int B, const float* coords, float* grads, int H, int W, const float* gt_poses,
+                                 const int* shiftX, const int* shiftY, const float* f, const float* ppx, const float* ppy, int sub,
+                                 float cut, float maxReproj, float minDepth, double* out_losses) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    if (!coords || !gt_poses || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
+    if (B <= 0 || H <= 0 || W <= 0 || sub <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d H=%d W=%d sub=%d", B, H, W, sub);
+    if ((long long)H * W > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too large", W, H);
+    const size_t n = (size_t)3 * H * W;
+    std::vector<const float*> cp((size_t)B);
+    std::vector<float*> gp((size_t)B);
+    for (int b = 0; b < B; ++b) {
+        cp[b] = coords + (size_t)b * n;
+        gp[b] = grads ? grads + (size_t)b * n : nullptr;
+    }
+    const std::vector<int> hs((size_t)B, H), ws((size_t)B, W);
+    return esacb200_reproj_loss_ragged(ctx, B, cp.data(), grads ? gp.data() : nullptr, hs.data(), ws.data(), gt_poses, shiftX, shiftY,
+                                       f, ppx, ppy, sub, cut, maxReproj, minDepth, out_losses);
 } ESAC_ABI_CATCH(ctx)
 
 int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* grads, int H, int W, const float* gt_poses,
@@ -1549,52 +1842,82 @@ int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* g
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
-int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int Wp, const float* gt, int Hg, int Wg,
-                        float* grads, float cut, double* out_losses, int64_t* out_counts) try {
+// The coordinate loss over B images, each with its own prediction and ground-truth size: one launch per load path and
+// pass, each image cut into the blocks a single-image call uses.
+int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pred, const int* Hp, const int* Wp,
+                               const float* const* gt, const int* Hg, const int* Wg, float* const* grads, float cut,
+                               double* out_losses, int64_t* out_counts) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
-    if (!pred || !gt || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
-    if (B <= 0 || Hp <= 0 || Wp <= 0 || Hg <= 0 || Wg <= 0)
-        return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d prediction %dx%d ground truth %dx%d", B, Hp, Wp, Hg, Wg);
-    if (abs(Hp - Hg) > 1 || abs(Wp - Wg) > 1)   // util.assert_size tolerates 1 cell
-        return fail(ctx, ESACB200_ERR_ARG, "size mismatch: prediction %dx%d, ground truth %dx%d (at most 1 apart)", Hp, Wp, Hg, Wg);
-    if ((long long)Hp * Wp > (1ll << 30) || (long long)Hg * Wg > (1ll << 30))
-        return fail(ctx, ESACB200_ERR_ARG, "map too large");
+    if (!pred || !gt || !Hp || !Wp || !Hg || !Wg || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d", B);
+    for (int b = 0; b < B; ++b) {
+        if (Hp[b] <= 0 || Wp[b] <= 0 || Hg[b] <= 0 || Wg[b] <= 0)
+            return fail(ctx, ESACB200_ERR_ARG, "image %d: bad sizes prediction %dx%d ground truth %dx%d", b, Hp[b], Wp[b], Hg[b], Wg[b]);
+        if (abs(Hp[b] - Hg[b]) > 1 || abs(Wp[b] - Wg[b]) > 1)   // util.assert_size tolerates 1 cell
+            return fail(ctx, ESACB200_ERR_ARG, "image %d: size mismatch: prediction %dx%d, ground truth %dx%d (at most 1 apart)", b,
+                        Hp[b], Wp[b], Hg[b], Wg[b]);
+        if ((long long)Hp[b] * Wp[b] > (1ll << 30) || (long long)Hg[b] * Wg[b] > (1ll << 30))
+            return fail(ctx, ESACB200_ERR_ARG, "image %d: map too large", b);
+    }
+    bool p_dev = false, q_dev = false, g_dev = false;
+    int rc = pointer_kind(ctx, (const void* const*)pred, B, "pred", p_dev);
+    if (rc) return rc;
+    if ((rc = pointer_kind(ctx, (const void* const*)gt, B, "gt", q_dev))) return rc;
+    if (grads && (rc = pointer_kind(ctx, (const void* const*)grads, B, "grads", g_dev))) return rc;
     begin_call(ctx);
-    const size_t pbytes = (size_t)B * 3 * Hp * Wp * sizeof(float), gbytes = (size_t)B * 3 * Hg * Wg * sizeof(float);
-    const bool p_host = !is_device_ptr(pred), q_host = !is_device_ptr(gt), g_host = grads && !is_device_ptr(grads);
-    const float* d_pred = pred;
-    const float* d_gt = gt;
-    float* d_grads = grads;
-    if (p_host) {
-        CK(ctx->coords.ensure(pbytes));
-        CK(cudaMemcpyAsync(ctx->coords.p, pred, pbytes, cudaMemcpyHostToDevice, ctx->stream));
-        d_pred = ctx->coords.as<float>();
+    std::vector<size_t> pbytes((size_t)B), gbytes((size_t)B), p_off, q_off, g_off;
+    for (int b = 0; b < B; ++b) {
+        pbytes[b] = (size_t)3 * Hp[b] * Wp[b] * sizeof(float);
+        gbytes[b] = (size_t)3 * Hg[b] * Wg[b] * sizeof(float);
     }
-    if (q_host) {
-        CK(ctx->coords_alt.ensure(gbytes));
-        CK(cudaMemcpyAsync(ctx->coords_alt.p, gt, gbytes, cudaMemcpyHostToDevice, ctx->stream));
-        d_gt = ctx->coords_alt.as<float>();
+    std::vector<const float*> d_pred, d_gt;
+    std::vector<float*> d_grads((size_t)B, nullptr);
+    if ((rc = stage_images(ctx, pred, pbytes, p_dev, true, ctx->coords, d_pred, p_off))) return rc;
+    if ((rc = stage_images(ctx, gt, gbytes, q_dev, true, ctx->coords_alt, d_gt, q_off))) return rc;
+    if (grads && (rc = stage_images(ctx, grads, pbytes, g_dev, false, ctx->grads, d_grads, g_off))) return rc;
+    std::vector<CoordImage> recs((size_t)B);
+    std::vector<char> vec((size_t)B);
+    long long parts = 0;
+    for (int b = 0; b < B; ++b) {
+        CoordImage& r = recs[b];
+        r.pred = d_pred[b];
+        r.gt = d_gt[b];
+        r.grads = d_grads[b];
+        vec[b] = coord_image(r, Hp[b], Wp[b], Hg[b], Wg[b]);
+        r.b = b;
+        r.part0 = parts;
+        parts += r.blocks;
     }
-    if (g_host) {
-        CK(ctx->grads.ensure(pbytes));
-        d_grads = ctx->grads.as<float>();
-    }
-    const int bpi = reproj_blocks_per_image(Hp * Wp, B, ctx->sm_count);
-    // scratch layout: [tickets B u32 | counts B u32, padded] [losses B f64] [valid counts B i64] [partials B*bpi*2 f64]
-    const size_t off_loss = ((size_t)B * 8 + 63) & ~(size_t)63, off_cnt = off_loss + (((size_t)B * 8 + 63) & ~(size_t)63),
-                 off_part = off_cnt + (((size_t)B * 8 + 63) & ~(size_t)63);
-    CK(ctx->scratch.ensure(off_part + (size_t)B * bpi * 2 * 8));
+    std::vector<CoordImage> ordered;
+    int n_vec, max_vec, max_sc;
+    const size_t rec_bytes = order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
+    // scratch layout: [tickets B u32 | counts B u32, padded] [records] [losses B f64] [valid counts B i64] [partials 2 f64 each]
+    const size_t off_rec = ((size_t)B * 8 + 63) & ~(size_t)63, off_loss = (off_rec + rec_bytes + 63) & ~(size_t)63,
+                 off_cnt = off_loss + (((size_t)B * 8 + 63) & ~(size_t)63), off_part = off_cnt + (((size_t)B * 8 + 63) & ~(size_t)63);
+    CK(ctx->scratch.ensure(off_part + (size_t)parts * 2 * 8));
     char* base = (char*)ctx->scratch.p;
-    CK(cudaMemsetAsync(base, 0, off_loss, ctx->stream));
+    CK(cudaMemsetAsync(base, 0, off_rec, ctx->stream));
+    CK(cudaMemcpyAsync(base + off_rec, ordered.data(), rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
     mark(ctx, EV_H2D);
     mark(ctx, EV_FOLD);  // ms_score = the kernels alone
-    ctx->st.kernel_launches += launch_coord_loss(d_pred, d_gt, d_grads, B, Hp, Wp, Hg, Wg, cut, bpi, (unsigned*)base + B,
-                                                 (double*)(base + off_part), (unsigned*)base, (double*)(base + off_loss),
-                                                 (long long*)(base + off_cnt), ctx->stream);
-    CK(cudaGetLastError());
+    const CoordImage* d_rec = (const CoordImage*)(base + off_rec);
+    for (int path = 0; path < 2; ++path) {
+        const int n = path == 0 ? n_vec : B - n_vec;
+        if (n == 0) continue;
+        for (int pass = grads ? 1 : 2; pass <= 2; ++pass) {
+            launch_coord_loss(path == 0, pass, grads != nullptr, d_rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, cut,
+                              (unsigned*)base + B, (double*)(base + off_part), (unsigned*)base, (double*)(base + off_loss),
+                              (long long*)(base + off_cnt), ctx->stream);
+            CK(cudaGetLastError());
+            ctx->st.kernel_launches += 1;
+        }
+    }
     mark(ctx, EV_SCORE);
-    if (g_host) CK(cudaMemcpyAsync(grads, d_grads, pbytes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (grads && !g_dev) {
+        rc = copy_packed(ctx, (char* const*)grads, pbytes, g_off, (char*)ctx->grads.p, false, ctx->stream);
+        if (rc) return rc;
+    }
     CK(cudaMemcpyAsync(out_losses, base + off_loss, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
     if (out_counts) CK(cudaMemcpyAsync(out_counts, base + off_cnt, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
     mark(ctx, EV_END);
@@ -1603,6 +1926,30 @@ int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int
     ctx->last_M = 0;
     finish_stats(ctx);
     return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+// B images of one shape: the pointer and size arrays of [B,3,Hp,Wp] / [B,3,Hg,Wg] tensors.
+int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int Wp, const float* gt, int Hg, int Wg,
+                        float* grads, float cut, double* out_losses, int64_t* out_counts) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    if (!pred || !gt || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    if (B <= 0 || Hp <= 0 || Wp <= 0 || Hg <= 0 || Wg <= 0)
+        return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d prediction %dx%d ground truth %dx%d", B, Hp, Wp, Hg, Wg);
+    if (abs(Hp - Hg) > 1 || abs(Wp - Wg) > 1)   // util.assert_size tolerates 1 cell
+        return fail(ctx, ESACB200_ERR_ARG, "size mismatch: prediction %dx%d, ground truth %dx%d (at most 1 apart)", Hp, Wp, Hg, Wg);
+    if ((long long)Hp * Wp > (1ll << 30) || (long long)Hg * Wg > (1ll << 30))
+        return fail(ctx, ESACB200_ERR_ARG, "map too large");
+    const size_t np = (size_t)3 * Hp * Wp, ng = (size_t)3 * Hg * Wg;
+    std::vector<const float*> pp((size_t)B), qp((size_t)B);
+    std::vector<float*> gp((size_t)B);
+    for (int b = 0; b < B; ++b) {
+        pp[b] = pred + (size_t)b * np;
+        qp[b] = gt + (size_t)b * ng;
+        gp[b] = grads ? grads + (size_t)b * np : nullptr;
+    }
+    const std::vector<int> hp((size_t)B, Hp), wp((size_t)B, Wp), hg((size_t)B, Hg), wg((size_t)B, Wg);
+    return esacb200_coord_loss_ragged(ctx, B, pp.data(), hp.data(), wp.data(), qp.data(), hg.data(), wg.data(),
+                                      grads ? gp.data() : nullptr, cut, out_losses, out_counts);
 } ESAC_ABI_CATCH(ctx)
 
 int esacb200_copy_last_scores(esacb200_ctx* ctx, double* dst, int M) try {

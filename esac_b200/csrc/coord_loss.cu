@@ -26,17 +26,10 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kCellsPerThread = 4;
 
-struct CoordGeom {
-    int Np, Ng;   // plane sizes of the prediction / the ground truth (Hp*Wp, Hg*Wg)
-    int Wp, Wg;   // their row pitches
-    int H, W;     // the common top-left window
-    int N;        // H*W
-};
-
 __device__ __forceinline__ bool gt_valid(float x, float y, float z) { return x != 0.f || y != 0.f || z != 0.f; }
 
 // Window cell of prediction cell p (scalar path); -1 outside the window, else the ground-truth index.
-__device__ __forceinline__ int gt_index(int y, int x, const CoordGeom& g) { return (y < g.H && x < g.W) ? y * g.Wg + x : -1; }
+__device__ __forceinline__ int gt_index(int y, int x, const CoordImage& g) { return (y < g.H && x < g.W) ? y * g.Wg + x : -1; }
 
 struct CellOut {
     double loss;
@@ -69,17 +62,19 @@ __device__ __forceinline__ CellOut coord_cell(float px, float py, float pz, floa
     return o;
 }
 
-// grid = (blocks_per_image, B).  counts[b] += valid cells of image b (zeroed before the launch).
+// grid = (max blocks, images of this load path): row blockIdx.y is image recs[blockIdx.y], its blocks are blockIdx.x <
+// blocks.  counts[b] += valid cells of image b (zeroed before the launch).
 template <bool VEC>
-__global__ void __launch_bounds__(kThreads) coord_count_kernel(const float* __restrict__ gt, CoordGeom g,
-                                                                unsigned* __restrict__ counts) {
-    const int b = blockIdx.y;
-    const float* qx = gt + (size_t)b * 3 * g.Ng;
+__global__ void __launch_bounds__(kThreads) coord_count_kernel(const CoordImage* __restrict__ recs, unsigned* __restrict__ counts) {
+    const CoordImage g = recs[blockIdx.y];
+    if ((int)blockIdx.x >= g.blocks) return;
+    const int b = g.b;
+    const float* qx = g.gt;
     const float* qy = qx + g.Ng;
     const float* qz = qy + g.Ng;
     unsigned cnt = 0;
     const int per_block = kThreads * kCellsPerThread;
-    for (int base = blockIdx.x * per_block; base < g.Np; base += gridDim.x * per_block) {
+    for (int base = blockIdx.x * per_block; base < g.Np; base += g.blocks * per_block) {
         const int p0 = base + threadIdx.x * kCellsPerThread;
         if (VEC) {
             if (p0 >= g.N) continue;   // the window is the first N cells of both planes (equal pitch, N % 4 == 0)
@@ -102,28 +97,29 @@ __global__ void __launch_bounds__(kThreads) coord_count_kernel(const float* __re
     if ((threadIdx.x & 31) == 0 && cnt) atomicAdd(&counts[b], cnt);
 }
 
-// grid = (blocks_per_image, B) over the prediction's cells.  GRAD: grads [B,3,Hp,Wp] is overwritten, counts[b] from the
-// count pass.  losses[b] = loss of image b, out_counts[b] = its valid cells; partial: B * blocks_per_image * 2 doubles,
-// tickets: B zeroed counters (left zeroed).
+// grid as for the count pass, over the prediction's cells.  GRAD: grads overwritten, counts[b] from the count pass.
+// losses[b] = loss of image b, out_counts[b] = its valid cells; partial: 2 doubles per block, tickets: zeroed counters
+// (left zeroed).
 template <bool VEC, bool GRAD>
-__global__ void __launch_bounds__(kThreads) coord_loss_kernel(const float* __restrict__ pred, const float* __restrict__ gt,
-                                                               float* __restrict__ grads, CoordGeom g, float cut,
+__global__ void __launch_bounds__(kThreads) coord_loss_kernel(const CoordImage* __restrict__ recs, float cut,
                                                                const unsigned* __restrict__ counts, double* __restrict__ partial,
                                                                unsigned* __restrict__ tickets, double* __restrict__ losses,
                                                                long long* __restrict__ out_counts) {
-    const int b = blockIdx.y;
-    const float* px = pred + (size_t)b * 3 * g.Np;
+    const CoordImage g = recs[blockIdx.y];
+    if ((int)blockIdx.x >= g.blocks) return;
+    const int b = g.b;
+    const float* px = g.pred;
     const float* py = px + g.Np;
     const float* pz = py + g.Np;
-    const float* qx = gt + (size_t)b * 3 * g.Ng;
+    const float* qx = g.gt;
     const float* qy = qx + g.Ng;
     const float* qz = qy + g.Ng;
-    float* gx = GRAD ? grads + (size_t)b * 3 * g.Np : nullptr;
+    float* gx = GRAD ? g.grads : nullptr;
     const double cnt = GRAD ? (double)counts[b] : 0.;
     double acc = 0.;
     unsigned nvalid = 0;
     const int per_block = kThreads * kCellsPerThread;
-    for (int base = blockIdx.x * per_block; base < g.Np; base += gridDim.x * per_block) {
+    for (int base = blockIdx.x * per_block; base < g.Np; base += g.blocks * per_block) {
         const int p0 = base + threadIdx.x * kCellsPerThread;
         if (p0 >= g.Np) continue;
         if (VEC) {
@@ -176,7 +172,7 @@ __global__ void __launch_bounds__(kThreads) coord_loss_kernel(const float* __res
         }
     }
     double total[2] = {acc, (double)nvalid};
-    if (block_image_sum<kThreads>(total, partial, tickets)) {
+    if (block_image_sum<kThreads>(total, partial, tickets, b, g.blocks, (size_t)g.part0)) {
         losses[b] = total[0] / total[1];   // no valid cell: 0 / 0 = NaN, as in torch
         out_counts[b] = (long long)total[1];
     }
@@ -184,37 +180,35 @@ __global__ void __launch_bounds__(kThreads) coord_loss_kernel(const float* __res
 
 }  // namespace
 
-int launch_coord_loss(const float* pred, const float* gt, float* grads, int B, int Hp, int Wp, int Hg, int Wg, float cut,
-                      int blocks_per_image, unsigned* counts, double* partial, unsigned* tickets, double* losses,
-                      long long* out_counts, cudaStream_t stream) {
-    CoordGeom g;
-    g.Np = Hp * Wp; g.Ng = Hg * Wg; g.Wp = Wp; g.Wg = Wg;
-    g.H = Hp < Hg ? Hp : Hg;
-    g.W = Wp < Wg ? Wp : Wg;
-    g.N = g.H * g.W;
+bool coord_image(CoordImage& r, int Hp, int Wp, int Hg, int Wg) {
+    r.Np = Hp * Wp; r.Ng = Hg * Wg; r.Wp = Wp; r.Wg = Wg;
+    r.H = Hp < Hg ? Hp : Hg;
+    r.W = Wp < Wg ? Wp : Wg;
+    r.N = r.H * r.W;
+    r.blocks = reproj_blocks_per_image(r.Np);
+    r.pad = 0;
     // 128-bit path: equal row pitch (the window is then the first N cells of every plane), every plane 16-byte aligned
-    const bool vec = Wp == Wg && g.N % 4 == 0 && g.Np % 4 == 0 && g.Ng % 4 == 0 && (uintptr_t)pred % 16 == 0 &&
-                     (uintptr_t)gt % 16 == 0 && (!grads || (uintptr_t)grads % 16 == 0);
-    const dim3 grid(blocks_per_image, B);
-    int launches = 1;
-    if (grads) {
-        if (vec) coord_count_kernel<true><<<grid, kThreads, 0, stream>>>(gt, g, counts);
-        else coord_count_kernel<false><<<grid, kThreads, 0, stream>>>(gt, g, counts);
-        ++launches;
+    return Wp == Wg && r.N % 4 == 0 && r.Np % 4 == 0 && r.Ng % 4 == 0 && (uintptr_t)r.pred % 16 == 0 &&
+           (uintptr_t)r.gt % 16 == 0 && (!r.grads || (uintptr_t)r.grads % 16 == 0);
+}
+
+void launch_coord_loss(bool vec, int pass, bool grad, const CoordImage* recs, int n, int max_blocks, float cut,
+                       unsigned* counts, double* partial, unsigned* tickets, double* losses, long long* out_counts,
+                       cudaStream_t stream) {
+    const dim3 grid(max_blocks, n);
+    if (pass == 1) {
+        if (vec) coord_count_kernel<true><<<grid, kThreads, 0, stream>>>(recs, counts);
+        else coord_count_kernel<false><<<grid, kThreads, 0, stream>>>(recs, counts);
+    } else if (grad) {
         if (vec)
-            coord_loss_kernel<true, true><<<grid, kThreads, 0, stream>>>(pred, gt, grads, g, cut, counts, partial, tickets,
-                                                                         losses, out_counts);
+            coord_loss_kernel<true, true><<<grid, kThreads, 0, stream>>>(recs, cut, counts, partial, tickets, losses, out_counts);
         else
-            coord_loss_kernel<false, true><<<grid, kThreads, 0, stream>>>(pred, gt, grads, g, cut, counts, partial, tickets,
-                                                                          losses, out_counts);
+            coord_loss_kernel<false, true><<<grid, kThreads, 0, stream>>>(recs, cut, counts, partial, tickets, losses, out_counts);
     } else if (vec) {
-        coord_loss_kernel<true, false><<<grid, kThreads, 0, stream>>>(pred, gt, nullptr, g, cut, counts, partial, tickets,
-                                                                      losses, out_counts);
+        coord_loss_kernel<true, false><<<grid, kThreads, 0, stream>>>(recs, cut, counts, partial, tickets, losses, out_counts);
     } else {
-        coord_loss_kernel<false, false><<<grid, kThreads, 0, stream>>>(pred, gt, nullptr, g, cut, counts, partial, tickets,
-                                                                       losses, out_counts);
+        coord_loss_kernel<false, false><<<grid, kThreads, 0, stream>>>(recs, cut, counts, partial, tickets, losses, out_counts);
     }
-    return launches;
 }
 
 }  // namespace esacb200

@@ -55,29 +55,30 @@ __device__ __forceinline__ void block_sum_fixed(double (&v)[NV]) {
     }
 }
 
-// Per-image sum over the blocks of a (blocks_per_image, B) grid, deterministic: every block sums its threads' NV values
-// (block_sum_fixed) and stores the totals in partial[b][blockIdx.x][NV]; the image's last block to take a ticket adds the
-// partials in block order.  Returns true in thread 0 of that block, with the image totals in v; tickets[b] (zero before
-// the launch) is left zero for the next one.
+// Per-image sum over the `blocks` blocks (blockIdx.x = 0 .. blocks-1) of image b, deterministic: every block sums its
+// threads' NV values (block_sum_fixed) and stores the totals in partial[part0 + blockIdx.x][NV]; the image's last block to
+// take a ticket adds the partials in block order.  Returns true in thread 0 of that block, with the image totals in v;
+// tickets[b] (zero before the launch) is left zero for the next one.  The block count and the partial base are the
+// image's own, so images of different sizes share one launch and each sums exactly as it would alone.
 template <int THREADS, int NV>
-__device__ __forceinline__ bool block_image_sum(double (&v)[NV], double* __restrict__ partial, unsigned* __restrict__ tickets) {
+__device__ __forceinline__ bool block_image_sum(double (&v)[NV], double* __restrict__ partial, unsigned* __restrict__ tickets,
+                                                int b, unsigned blocks, size_t part0) {
     __shared__ bool last;
-    const int b = blockIdx.y;
     block_sum_fixed<THREADS, NV>(v);
     if (threadIdx.x == 0) {
 #pragma unroll
-        for (int i = 0; i < NV; ++i) partial[((size_t)b * gridDim.x + blockIdx.x) * NV + i] = v[i];
+        for (int i = 0; i < NV; ++i) partial[(part0 + blockIdx.x) * NV + i] = v[i];
         __threadfence();
-        last = atomicAdd(&tickets[b], 1u) == gridDim.x - 1;
+        last = atomicAdd(&tickets[b], 1u) == blocks - 1;
     }
     __syncthreads();
     if (!last) return false;
     __threadfence();
 #pragma unroll
     for (int i = 0; i < NV; ++i) v[i] = 0.;
-    for (unsigned k = threadIdx.x; k < gridDim.x; k += THREADS) {
+    for (unsigned k = threadIdx.x; k < blocks; k += THREADS) {
 #pragma unroll
-        for (int i = 0; i < NV; ++i) v[i] += __ldcg(&partial[((size_t)b * gridDim.x + k) * NV + i]);
+        for (int i = 0; i < NV; ++i) v[i] += __ldcg(&partial[(part0 + k) * NV + i]);
     }
     block_sum_fixed<THREADS, NV>(v);
     if (threadIdx.x == 0) tickets[b] = 0;  // ready for the next launch
@@ -222,23 +223,54 @@ void launch_assign(const float* weights, int B, int E, int M, int keep_top, int 
                    float* out_hist, int* flags, cudaStream_t stream);
 
 // --- reproj.cu ----------------------------------------------------------------------------
-int reproj_blocks_per_image(int N, int B, int sm_count);
-// img: per image kReprojImgFloats floats = world->camera 3x4 (row major), padX, padY, f, cx, cy, 3 unused.  partial:
-// B * blocks_per_image doubles, tickets: B zeroed counters (left zeroed), losses: B doubles.  grads may be null (loss only).
+// Blocks of one image in the loss kernels of reproj.cu and coord_loss.cu: a pure function of its cell count N, so an image
+// is cut into the same blocks, and summed in the same order, whatever else is in the batch.
+int reproj_blocks_per_image(int N);
+// One image of a reprojection-loss launch.  The image's blocks are blockIdx.x < blocks of grid row blockIdx.y; its block
+// partials are partial[part0 .. part0 + blocks).
+struct ReprojImage {
+    const float* coords;   // [3, H, W]
+    float* grads;          // [3, H, W] overwritten, or null (loss only)
+    int N, W;              // cells, row pitch
+    int b;                 // index in the batch: img record, ticket, loss
+    int blocks;            // reproj_blocks_per_image(N)
+    long long part0;
+};
+// 128-bit loads and stores for this image: N % 4 == 0, W >= 4, 16-byte aligned planes.
+bool reproj_vec_ok(const float* coords, const float* grads, int N, int W);
+// img: per image kReprojImgFloats floats = world->camera 3x4 (row major), padX, padY, f, cx, cy, 3 unused.  recs: n device
+// records, all on the load path `vec`; max_blocks = their largest block count.  tickets: zeroed counters per batch image
+// (left zeroed), losses: a double per batch image.
 constexpr int kReprojImgFloats = 20;
-void launch_reproj(const float* coords, float* grads, const float* img, int B, int N, int W, float sub, float cut,
-                   float max_err, float min_depth, int blocks_per_image, double* partial, unsigned* tickets, double* losses,
-                   cudaStream_t stream);
+void launch_reproj(bool vec, const ReprojImage* recs, int n, int max_blocks, const float* img, float sub, float cut,
+                   float max_err, float min_depth, double* partial, unsigned* tickets, double* losses, cudaStream_t stream);
 
 // --- coord_loss.cu ------------------------------------------------------------------------
-// Both passes run on a (blocks_per_image, B) grid of 256-thread blocks, 4 cells per thread, as the reprojection loss:
-// blocks_per_image = reproj_blocks_per_image(Hp * Wp, ...), a pure function of the size that fixes the summation order.
-// pred [B,3,Hp,Wp], gt [B,3,Hg,Wg] (|Hp-Hg|, |Wp-Wg| <= 1, checked by the caller), grads [B,3,Hp,Wp] overwritten or null
-// (loss only).  counts: B zeroed counters (gradient only), partial: B * blocks_per_image * 2 doubles, tickets: B zeroed
-// counters (left zeroed), losses: B doubles, out_counts: B valid-cell counts.  Returns the number of kernels launched.
-int launch_coord_loss(const float* pred, const float* gt, float* grads, int B, int Hp, int Wp, int Hg, int Wg, float cut,
-                      int blocks_per_image, unsigned* counts, double* partial, unsigned* tickets, double* losses,
-                      long long* out_counts, cudaStream_t stream);
+// One image of a coordinate-loss launch: pred [3,Hp,Wp], gt [3,Hg,Wg] (|Hp-Hg|, |Wp-Wg| <= 1, checked by the caller),
+// grads [3,Hp,Wp] overwritten or null (loss only).  blocks = reproj_blocks_per_image(Np), partials part0 .. part0 + blocks
+// (2 doubles each), as for ReprojImage.
+struct CoordImage {
+    const float* pred;
+    const float* gt;
+    float* grads;
+    int Np, Ng;   // plane sizes of the prediction / the ground truth (Hp*Wp, Hg*Wg)
+    int Wp, Wg;   // their row pitches
+    int H, W;     // the common top-left window
+    int N;        // H*W
+    int b;        // index in the batch: counter, ticket, loss
+    int blocks;
+    int pad;
+    long long part0;
+};
+// Fills the geometry of r from the two sizes and picks the load path: 128-bit when the row pitches are equal (the window is
+// then the first N cells of every plane), N, Np, Ng % 4 == 0 and every plane is 16-byte aligned.
+bool coord_image(CoordImage& r, int Hp, int Wp, int Hg, int Wg);
+// Both passes run on a (max_blocks, n) grid of 256-thread blocks, 4 cells per thread, as the reprojection loss; recs: n
+// device records on load path `vec`.  counts: a zeroed counter per batch image (gradient only), tickets: zeroed counters
+// (left zeroed), losses / out_counts: per batch image.  pass 1 = count pass (gradient only), 2 = loss pass.
+void launch_coord_loss(bool vec, int pass, bool grad, const CoordImage* recs, int n, int max_blocks, float cut,
+                       unsigned* counts, double* partial, unsigned* tickets, double* losses, long long* out_counts,
+                       cudaStream_t stream);
 
 // --- bwd.cu -------------------------------------------------------------------------------
 struct BwdArgs {

@@ -135,21 +135,25 @@ __device__ __forceinline__ PairOut reproj_pair(float2 X, float2 Y, float2 Z, con
     return o;
 }
 
-// grid = (blocks_per_image, B).  img[b] = kReprojImgFloats floats: 12 matrix entries, padX, padY, f, cx, cy, 3 unused.
+// grid = (max blocks, images of this load path).  Row blockIdx.y is image recs[blockIdx.y]; its blocks are blockIdx.x <
+// rec.blocks, the others leave at once.  img[b] = kReprojImgFloats floats: 12 matrix entries, padX, padY, f, cx, cy, 3 unused.
 template <bool VEC>
-__global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const float* __restrict__ coords, float* __restrict__ grads,
-                                                          const float* __restrict__ img, int N, int W, float sub, float cut,
-                                                          float max_err, float min_depth, double* __restrict__ partial,
-                                                          unsigned* __restrict__ tickets, double* __restrict__ losses) {
+__global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const ReprojImage* __restrict__ recs, const float* __restrict__ img,
+                                                          float sub, float cut, float max_err, float min_depth,
+                                                          double* __restrict__ partial, unsigned* __restrict__ tickets,
+                                                          double* __restrict__ losses) {
     __shared__ float m[kReprojImgFloats];
-    const int b = blockIdx.y;
-    if (threadIdx.x < kReprojImgFloats) m[threadIdx.x] = img[b * kReprojImgFloats + threadIdx.x];
+    // The image's geometry sits in shared memory and is re-read where it is used (volatile).  Unlike kernel parameters,
+    // loaded values cannot be rematerialised: held in registers across the loop they would push the scalar path over the
+    // 48 registers of __launch_bounds__(256, 5).
+    __shared__ ReprojImage rec;
+    const volatile ReprojImage& vrec = rec;
+    if ((int)blockIdx.x >= recs[blockIdx.y].blocks) return;
+    if (threadIdx.x == 0) rec = recs[blockIdx.y];
     __syncthreads();
-    const float* px = coords + (size_t)b * 3 * N;
-    const float* py = px + N;
-    const float* pz = py + N;
-    float* gx = grads ? grads + (size_t)b * 3 * N : nullptr;
-    const float inv_n = 1.f / (float)N;
+    if (threadIdx.x < kReprojImgFloats) m[threadIdx.x] = img[rec.b * kReprojImgFloats + threadIdx.x];
+    __syncthreads();
+    const float inv_n = 1.f / (float)rec.N;
     const float half = sub * 0.5f;
     const float padX = m[12], padY = m[13];
     PairConst kc;
@@ -162,26 +166,22 @@ __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const float* __rest
     }
     double acc = 0.;
     const int per_block = kThreads * kCellsPerThread;
-    for (int base = blockIdx.x * per_block; base < N; base += gridDim.x * per_block) {
+    for (int base = blockIdx.x * per_block; base < vrec.N; base += vrec.blocks * per_block) {
+        const int N = vrec.N, W = vrec.W;
         const int p0 = base + threadIdx.x * kCellsPerThread;
         if (p0 >= N) continue;
         float X[4], Y[4], Z[4];
         int n = min(kCellsPerThread, N - p0);
         if (VEC) {
+            const float* px = vrec.coords;
+            const float* py = px + N;
+            const float* pz = py + N;
             const float4 a = __ldcs(reinterpret_cast<const float4*>(px + p0));
             const float4 c = __ldcs(reinterpret_cast<const float4*>(py + p0));
             const float4 d = __ldcs(reinterpret_cast<const float4*>(pz + p0));
             X[0] = a.x; X[1] = a.y; X[2] = a.z; X[3] = a.w;
             Y[0] = c.x; Y[1] = c.y; Y[2] = c.z; Y[3] = c.w;
             Z[0] = d.x; Z[1] = d.y; Z[2] = d.z; Z[3] = d.w;
-        } else {
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-                const bool ok = i < n;
-                X[i] = ok ? px[p0 + i] : 0.f;
-                Y[i] = ok ? py[p0 + i] : 0.f;
-                Z[i] = ok ? pz[p0 + i] : 1.f;
-            }
         }
         int y = p0 / W, x = p0 - y * W;
         float ox[4], oy[4], oz[4];
@@ -210,21 +210,30 @@ __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const float* __rest
         } else {
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
+                // each cell is loaded where it is used: four cells of inputs held at once would not fit the register budget
+                const float* c = vrec.coords;
+                const bool ok = i < n;
+                X[i] = ok ? c[p0 + i] : 0.f;
+                Y[i] = ok ? c[vrec.N + p0 + i] : 0.f;
+                Z[i] = ok ? c[2 * (size_t)vrec.N + p0 + i] : 1.f;
                 const float tx = fmaf((float)x, sub, half) - padX;
                 const float ty = fmaf((float)y, sub, half) - padY;
                 const CellOut o = reproj_cell(X[i], Y[i], Z[i], m, m[14], m[15], m[16], tx, ty, cut, max_err, min_depth, inv_n);
                 if (i < n) {
                     four += o.loss;
-                    if (gx) {   // stored as computed: no gradient array stays live across the four cells
-                        gx[p0 + i] = o.gx;
-                        gx[N + p0 + i] = o.gy;
-                        gx[2 * (size_t)N + p0 + i] = o.gz;
+                    float* g = vrec.grads;
+                    if (g) {   // stored as computed: no gradient array stays live across the four cells
+                        const int Nv = vrec.N;
+                        g[p0 + i] = o.gx;
+                        g[Nv + p0 + i] = o.gy;
+                        g[2 * (size_t)Nv + p0 + i] = o.gz;
                     }
                 }
-                if (++x == W) { x = 0; ++y; }
+                if (++x == vrec.W) { x = 0; ++y; }
             }
         }
         acc += (double)four;
+        float* gx = vrec.grads;
         if (VEC && gx) {
             __stcs(reinterpret_cast<float4*>(gx + p0), make_float4(ox[0], ox[1], ox[2], ox[3]));
             __stcs(reinterpret_cast<float4*>(gx + N + p0), make_float4(oy[0], oy[1], oy[2], oy[3]));
@@ -233,33 +242,33 @@ __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const float* __rest
     }
     // block sum in a fixed order, then the last block of the image adds the partials, again in a fixed order
     double total[1] = {acc};
-    if (block_image_sum<kThreads>(total, partial, tickets)) losses[b] = total[0] / (double)N;
+    if (block_image_sum<kThreads>(total, partial, tickets, vrec.b, vrec.blocks, (size_t)vrec.part0))
+        losses[vrec.b] = total[0] / (double)vrec.N;
 }
 
 }  // namespace
 
-int reproj_blocks_per_image(int N, int B, int sm_count) {
+int reproj_blocks_per_image(int N) {
     // Many short CTAs (each a few KB of traffic) rather than one resident wave: the hardware scheduler then keeps every SM
     // streaming to the end, where a persistent grid of sm_count * k CTAs would finish with a ragged tail.  Two passes per CTA
     // on large maps amortise the per-CTA prologue / reduction; the count is a pure function of N (the fixed summation
     // order depends on it).
-    (void)B; (void)sm_count;
     const int per_block = kThreads * kCellsPerThread;
     const int need = (N + per_block - 1) / per_block;
     return need < 64 ? need : (need < 256 ? (need + 1) / 2 : (need + 3) / 4);
 }
 
-void launch_reproj(const float* coords, float* grads, const float* img, int B, int N, int W, float sub, float cut,
-                   float max_err, float min_depth, int blocks_per_image, double* partial, unsigned* tickets, double* losses,
-                   cudaStream_t stream) {
-    const dim3 grid(blocks_per_image, B);
-    const bool vec = (N % 4 == 0) && W >= 4 && ((uintptr_t)coords % 16 == 0) && (!grads || (uintptr_t)grads % 16 == 0);
+bool reproj_vec_ok(const float* coords, const float* grads, int N, int W) {
+    return (N % 4 == 0) && W >= 4 && ((uintptr_t)coords % 16 == 0) && (!grads || (uintptr_t)grads % 16 == 0);
+}
+
+void launch_reproj(bool vec, const ReprojImage* recs, int n, int max_blocks, const float* img, float sub, float cut,
+                   float max_err, float min_depth, double* partial, unsigned* tickets, double* losses, cudaStream_t stream) {
+    const dim3 grid(max_blocks, n);
     if (vec)
-        reproj_kernel<true><<<grid, kThreads, 0, stream>>>(coords, grads, img, N, W, sub, cut, max_err, min_depth, partial,
-                                                           tickets, losses);
+        reproj_kernel<true><<<grid, kThreads, 0, stream>>>(recs, img, sub, cut, max_err, min_depth, partial, tickets, losses);
     else
-        reproj_kernel<false><<<grid, kThreads, 0, stream>>>(coords, grads, img, N, W, sub, cut, max_err, min_depth, partial,
-                                                            tickets, losses);
+        reproj_kernel<false><<<grid, kThreads, 0, stream>>>(recs, img, sub, cut, max_err, min_depth, partial, tickets, losses);
 }
 
 }  // namespace esacb200

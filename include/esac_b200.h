@@ -218,6 +218,41 @@ int esacb200_reproj_loss_cameras(esacb200_ctx* ctx, int B, const float* coords, 
 int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int Wp, const float* gt, int Hg, int Wg,
                         float* grads, float cutLoss, double* out_losses, int64_t* out_counts);
 
+/* Ragged batches: B images of different sizes (19Scenes, Aachen and Dubrovnik keep each image's aspect ratio).  Each
+ * image-sized argument is a host array of B pointers to contiguous per-image buffers, with host arrays of B heights and
+ * widths.  All pointers of one argument are device pointers or all are host pointers; a mix is an error.  Image b computes
+ * exactly what a single-image call on it computes: the same minimal sets (forward / backward), bitwise the same losses and
+ * gradients (the two losses).  Size errors name the image.  The one-shape entry points above are these with every image
+ * a slice of one tensor, and give bitwise what they gave before.
+ *
+ * esacb200_forward_batch_cameras on maps coords[b] float32 [E,3,H[b],W[b]]; assign, out_poses, the shifts and cameras as
+ * there.  The workspace is sized for the largest image before the first image is enqueued. */
+int esacb200_forward_ragged(esacb200_ctx* ctx, int B, const float* const* coords, const int* H, const int* W, int E,
+                            const int64_t* assign, int64_t assign_stride, int M, float* out_poses, const int* shiftX,
+                            const int* shiftY, const float* f, const float* ppx, const float* ppy, float inlierThreshold,
+                            float inlierAlpha, float inlierBeta, float maxReproj, int subSampling, int* out_experts);
+
+/* esacb200_backward_batch_cameras on maps coords[b] / grads[b] float32 [E,3,H[b],W[b]] (grads accumulated in place).  Each
+ * worker runs its images largest first. */
+int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H, const int* W,
+                             int E, const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wLossRot,
+                             float wLossTrans, float lossCut, const int* shiftX, const int* shiftY, const float* f,
+                             const float* ppx, const float* ppy, float inlierThreshold, float inlierAlpha, float inlierBeta,
+                             float maxReproj, int subSampling, double* out_losses);
+
+/* esacb200_reproj_loss_cameras on predictions coords[b] float32 [3,H[b],W[b]]; grads NULL (loss only) or B pointers
+ * [3,H[b],W[b]] (overwritten). */
+int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H,
+                                const int* W, const float* gt_poses, const int* shiftX, const int* shiftY, const float* f,
+                                const float* ppx, const float* ppy, int subSampling, float cutLoss, float maxReproj,
+                                float minDepth, double* out_losses);
+
+/* esacb200_coord_loss on pred[b] float32 [3,Hp[b],Wp[b]] and gt[b] float32 [3,Hg[b],Wg[b]], each pair at most 1 apart in H
+ * and in W; grads NULL (loss only) or B pointers [3,Hp[b],Wp[b]] (overwritten). */
+int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pred, const int* Hp, const int* Wp,
+                               const float* const* gt, const int* Hg, const int* Wg, float* const* grads, float cutLoss,
+                               double* out_losses, int64_t* out_counts);
+
 /* Soft-inlier scores of given poses (getReproErrs + getHypScores, esac_util.h:235-363) without
  * sampling/selection/refinement: poses6 = host double [M][6] (rvec, tvec); out_scores host double [M]. */
 int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,

@@ -426,10 +426,11 @@ int run_sample(esacb200_ctx* ctx, const Plan& pl, uint64_t seed) {
 int run_score(esacb200_ctx* ctx, const Plan& pl) {
     const Problem& P = pl.P;
     int* sc = ctx->scalars.as<int>();
-    launch_fold(ctx->poses.as<Pose>(), ctx->perm.as<int>(), ctx->assign32.as<int>(), ctx->centres.as<float>(), P,
-                ctx->posepk.as<PosePk>(), ctx->stream);
-    mark(ctx, EV_FOLD);
     ScoreArgs a;
+    score_constants(P, a);
+    launch_fold(ctx->poses.as<Pose>(), ctx->perm.as<int>(), ctx->assign32.as<int>(), ctx->centres.as<float>(), P,
+                a.fold ? a.k1 : 1.f, ctx->posepk.as<PosePk>(), ctx->stream);
+    mark(ctx, EV_FOLD);
     a.coords = pl.d_coords;
     a.centres = ctx->centres.as<float>();
     a.poses = ctx->posepk.as<PosePk>();
@@ -440,9 +441,6 @@ int run_score(esacb200_ctx* ctx, const Plan& pl) {
     a.P = P;
     a.T = pl.T;
     a.hc = pl.hc;
-    const float log2e = 1.4426950408889634f;
-    a.k1 = P.beta * log2e;
-    a.k0 = -P.beta * P.tau * log2e;
     a.vec_ok = pl.vec_ok;
     launch_score(a, pl.ppt, pl.grid, ctx->stream);
     mark(ctx, EV_SCORE);

@@ -122,7 +122,10 @@ struct ScoreArgs {
     Problem P;
     int T;                   // pixel tiles per plane
     int hc;                  // hypotheses per chunk used when building the chunk table
-    float k1, k0;            // beta*log2(e), -beta*tau*log2(e)
+    float k1, k0;            // beta*log2(e), -beta*tau*log2(e) (minus kScorePairShift when fold)
+    float tmax;              // fold: k1*maxReproj + k0, the exponent of a clamped cell
+    float tiny;              // floor of |p|^2: 1e-30, times k1^2 when fold
+    int fold;                // k1 folded into the f rows and pixel offsets, one reciprocal per pair of cells
     int vec_ok;              // planes are 16-byte aligned and N % 4 == 0
 };
 
@@ -133,8 +136,10 @@ void launch_prep(const float* coords, const long long* assign, long long assign_
                  int* assign32, int* counts, int* offsets, int* perm, int* slot_of, ChunkDesc* chunks, int* n_chunks,
                  int* work_counter, float* centres, int* flags, int roles, cudaStream_t st);
 void launch_fold(const Pose* poses, const int* perm, const int* assign32, const float* centres, const Problem& P,
-                 PosePk* out, cudaStream_t st);
+                 float kf, PosePk* out, cudaStream_t st);
 int score_tile_pixels(int ppt);
+// k1, k0, tmax, tiny and fold of the scoring arguments for this problem
+void score_constants(const Problem& P, ScoreArgs& a);
 void launch_score(const ScoreArgs& a, int ppt, int grid, cudaStream_t st);
 // scores[h] = (alpha/W/H) * sum_tiles part ; softmax ; entropy ; argmax ; contributing list
 void launch_select(const float* part, const int* slot_of, const Problem& P, int T, double* scores, double* probs,

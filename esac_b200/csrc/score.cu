@@ -12,7 +12,11 @@
 // of once per hypothesis.  Per pixel-hypothesis: 9 FFMA for R*X+t, then
 //   err = |p| / |z|,  p = (xc + (cx-px) z, yc + (cy-py) z)   ->  err = num * rsqrt(num * z^2)
 //   w   = 1 / (1 + 2^(k1*min(err,maxReproj) + k0))           ==  1 - sigmoid(beta*(err - tau))
-// i.e. 3 MUFU (rsq, ex2, rcp) and ~20 fp32 ops per cell-hypothesis.
+// i.e. 3 MUFU (rsq, ex2, rcp) and ~20 fp32 ops per cell-hypothesis.  With k1 > 0 ("fold", every practical beta) k1 is
+// folded into the rows that carry f and into the pixel offsets, so num * rsqrt(num z^2) is already k1*err, and the two
+// cells of a float2 pair share one reciprocal (score_item): 2.5 MUFU and one FMUL less per cell-hypothesis.
+//   t = min(num rs + k0 - s, k1 maxReproj + k0 - s),  d = 2^-s + 2^t,  w_a + w_b = 2^-s (d_a + d_b) / (d_a d_b)
+// s = kScorePairShift keeps d_a d_b inside fp32 (unscaled, (1 + 2^65)^2 overflows at tau = 10, beta = 0.5, maxReproj = 100).
 #include <atomic>
 
 #include "esac_internal.h"
@@ -20,6 +24,7 @@
 namespace esacb200 {
 
 constexpr int kScoreThreads = 256;
+constexpr int kScorePairShift = 32;
 
 // ---------------------------------------------------------------------------------------------
 // prep
@@ -124,7 +129,7 @@ void launch_prep(const float* coords, const long long* assign, long long assign_
 // fold: (rvec, tvec) fp64 -> fp32 rows of diag(f,f,1) R and diag(f,f,1)(R c + t), slot order
 // ---------------------------------------------------------------------------------------------
 __global__ void fold_kernel(const Pose* __restrict__ poses, const int* __restrict__ perm, const int* __restrict__ assign32,
-                            const float* __restrict__ centres, Problem P, PosePk* __restrict__ out) {
+                            const float* __restrict__ centres, Problem P, float kf, PosePk* __restrict__ out) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= P.M) return;
     int h = perm[s];
@@ -133,7 +138,7 @@ __global__ void fold_kernel(const Pose* __restrict__ poses, const int* __restric
     double R[9];
     rodrigues_v2m(p.r, R, nullptr);
     double c[3] = {(double)centres[e * 3], (double)centres[e * 3 + 1], (double)centres[e * 3 + 2]};
-    double f = (double)P.f;
+    const double f = (double)P.f * (double)kf;  // kf = k1 when the scoring kernel folds it, else 1
     float A[12];
     for (int r = 0; r < 3; ++r) {
         double sc = r < 2 ? f : 1.0;
@@ -149,8 +154,25 @@ __global__ void fold_kernel(const Pose* __restrict__ poses, const int* __restric
 }
 
 void launch_fold(const Pose* poses, const int* perm, const int* assign32, const float* centres, const Problem& P,
-                 PosePk* out, cudaStream_t st) {
-    fold_kernel<<<(P.M + 127) / 128, 128, 0, st>>>(poses, perm, assign32, centres, P, out);
+                 float kf, PosePk* out, cudaStream_t st) {
+    fold_kernel<<<(P.M + 127) / 128, 128, 0, st>>>(poses, perm, assign32, centres, P, kf, out);
+}
+
+void score_constants(const Problem& P, ScoreArgs& a) {
+    const float log2e = 1.4426950408889634f;
+    a.k1 = P.beta * log2e;
+    a.k0 = -P.beta * P.tau * log2e;
+    const float k0s = a.k0 - (float)kScorePairShift;
+    a.tmax = fmaf(P.max_reproj, a.k1, k0s);
+    // Fold only where the clamp keeps every d <= 2^-s + 2^63 (so d_a d_b stays finite) and 1e-30 k1^2 stays a normal float;
+    // everywhere else (beta <= 0, huge beta * maxReproj, non-finite parameters) the per-cell arithmetic is unchanged.
+    a.fold = a.k1 >= 1e-3f && std::isfinite(a.k1) && std::isfinite(k0s) && a.tmax <= 63.f;
+    if (a.fold) {
+        a.k0 = k0s;
+        a.tiny = 1e-30f * a.k1 * a.k1;
+    } else {
+        a.tiny = 1e-30f;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -174,7 +196,7 @@ __device__ __forceinline__ float mufu_rcp(float x) {
 
 // tileX/Y/Z: when non-null, the tile's three coordinate rows already sit in shared memory (staged by TMA bulk copies);
 // otherwise the cells are read from global memory.
-template <int PPT, bool TAIL>
+template <int PPT, bool TAIL, bool FOLD>
 __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc cd, const int tile, const float4* sPose,
                                            float (*sWarp)[kMaxChunk], const float* tileX = nullptr,
                                            const float* tileY = nullptr, const float* tileZ = nullptr) {
@@ -241,6 +263,7 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
             // createSampling (esac_util.h:64-66): integer pixel centre, then ppoint - pixel in float
             aa[i] = P.ppx - (float)(px * P.sub + P.sub / 2 - P.shiftX);
             bb[i] = P.ppy - (float)(py * P.sub + P.sub / 2 - P.shiftY);
+            if (FOLD) { aa[i] = __fmul_rn(aa[i], a.k1); bb[i] = __fmul_rn(bb[i], a.k1); }
             vv[i] = (p < P.N) ? 1.f : 0.f;
             x[i] -= cX; y[i] -= cY; z[i] -= cZ;
         }
@@ -256,8 +279,9 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
         }
     }
     const float2 k1 = make_float2(a.k1, a.k1), k0 = make_float2(a.k0, a.k0);
-    const float2 one = make_float2(1.f, 1.f), tiny = make_float2(1e-30f, 1e-30f);
-    const float mr = P.max_reproj;
+    const float2 one = make_float2(1.f, 1.f), tiny = make_float2(a.tiny, a.tiny);
+    const float mr = FOLD ? a.tmax : P.max_reproj;
+    const float d0 = 1.f / (float)(1ull << kScorePairShift);
 
     // soft-inlier sum of this thread's PPT cells for hypothesis hl (pose = 3 x LDS.128, scalars broadcast to float2)
     auto one_hyp = [&](int hl) -> float {
@@ -266,7 +290,7 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
         const float2 a00 = make_float2(r0.x, r0.x), a01 = make_float2(r0.y, r0.y), a02 = make_float2(r0.z, r0.z), b0 = make_float2(r0.w, r0.w);
         const float2 a10 = make_float2(r1.x, r1.x), a11 = make_float2(r1.y, r1.y), a12 = make_float2(r1.z, r1.z), b1 = make_float2(r1.w, r1.w);
         const float2 a20 = make_float2(r2.x, r2.x), a21 = make_float2(r2.y, r2.y), a22 = make_float2(r2.z, r2.z), b2 = make_float2(r2.w, r2.w);
-        float2 acc = make_float2(0.f, 0.f);
+        float2 acc = make_float2(0.f, 0.f);  // FOLD: pair sums in units of 2^-s in acc.x
 #pragma unroll
         for (int j = 0; j < NP; ++j) {
             float2 xc = ffma2(a00, X[j], ffma2(a01, Y[j], ffma2(a02, Z[j], b0)));
@@ -280,6 +304,21 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
             float2 num = ffma2(pu, pu, ffma2(pv, pv, tiny));
             float2 m = fmul2(fmul2(zc, zc), num);
             float2 rs = make_float2(mufu_rsq(m.x), mufu_rsq(m.y));
+            if (FOLD) {
+                // NaN (and zc == 0 -> rs = +inf) clamps to tmax exactly as err does below
+                const float ta = fminf(__fmaf_rn(num.x, rs.x, k0.x), mr), tb = fminf(__fmaf_rn(num.y, rs.y, k0.x), mr);
+                const float da = __fadd_rn(mufu_ex2(ta), d0);
+                float db = __fadd_rn(mufu_ex2(tb), d0), ds;
+                if (TAIL) {  // valid cells are a prefix of the tile: b masked -> 1/d_a, both masked -> 0
+                    const bool vb = V[j].y != 0.f;
+                    ds = __fmul_rn(vb ? __fadd_rn(da, db) : da, V[j].x);
+                    db = vb ? db : da;
+                } else {
+                    ds = __fadd_rn(da, db);
+                }
+                acc.x = __fmaf_rn(ds, mufu_rcp(__fmul_rn(da, db)), acc.x);
+                continue;
+            }
             float2 err = fmul2(num, rs);
             err.x = fminf(err.x, mr);
             err.y = fminf(err.y, mr);
@@ -290,7 +329,7 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
             if (TAIL) acc = ffma2(w, V[j], acc);
             else acc = fadd2(acc, w);
         }
-        return acc.x + acc.y;
+        return FOLD ? acc.x : acc.x + acc.y;
     };
 
     int hl = 0;
@@ -322,11 +361,12 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
         float s = 0.f;
 #pragma unroll
         for (int w = 0; w < kScoreThreads / 32; ++w) s += sWarp[w][tid];
+        if (FOLD) s *= 1.f / (float)(1ull << kScorePairShift);  // exact
         a.part[(size_t)(cd.slot0 + tid) * a.T + tile] = s;
     }
 }
 
-template <int PPT>
+template <int PPT, bool FOLD>
 __global__ void __launch_bounds__(kScoreThreads, 2) score_kernel(const __grid_constant__ ScoreArgs a) {
     __shared__ float4 sPose[kMaxChunk * 3];
     __shared__ float sWarp[kScoreThreads / 32][kMaxChunk];
@@ -346,8 +386,8 @@ __global__ void __launch_bounds__(kScoreThreads, 2) score_kernel(const __grid_co
         const float4* src = (const float4*)(a.poses + cd.slot0);
         for (int i = tid; i < cd.count * 3; i += kScoreThreads) sPose[i] = src[i];
         __syncthreads();
-        if (ragged && tile == a.T - 1) score_item<PPT, true>(a, cd, tile, sPose, sWarp);
-        else score_item<PPT, false>(a, cd, tile, sPose, sWarp);
+        if (ragged && tile == a.T - 1) score_item<PPT, true, FOLD>(a, cd, tile, sPose, sWarp);
+        else score_item<PPT, false, FOLD>(a, cd, tile, sPose, sWarp);
         __syncthreads();
     }
 }
@@ -379,7 +419,7 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst, const void* src, uint32_
                  : "memory");
 }
 
-template <int PPT>
+template <int PPT, bool FOLD>
 __global__ void __launch_bounds__(kScoreThreads, 2) score_kernel_tma(const __grid_constant__ ScoreArgs a) {
     constexpr int TP = kScoreThreads * PPT;
     extern __shared__ __align__(128) float sTile[];  // [2 stages][3 rows][TP]
@@ -434,8 +474,8 @@ __global__ void __launch_bounds__(kScoreThreads, 2) score_kernel_tma(const __gri
         phase[stage] ^= 1u;
         __syncthreads();
         const float* tx = sTile + (size_t)stage * 3 * TP;
-        if (ragged && tile == a.T - 1) score_item<PPT, true>(a, cd, tile, sPose, sWarp, tx, tx + TP, tx + 2 * TP);
-        else score_item<PPT, false>(a, cd, tile, sPose, sWarp, tx, tx + TP, tx + 2 * TP);
+        if (ragged && tile == a.T - 1) score_item<PPT, true, FOLD>(a, cd, tile, sPose, sWarp, tx, tx + TP, tx + 2 * TP);
+        else score_item<PPT, false, FOLD>(a, cd, tile, sPose, sWarp, tx, tx + TP, tx + 2 * TP);
         __syncthreads();  // everyone is done with this stage, sPose, sWarp and has read sItem[stage ^ 1]'s predecessor
     }
 }
@@ -444,28 +484,34 @@ int score_tile_pixels(int ppt) { return kScoreThreads * ppt; }
 
 constexpr int kMaxDevices = 64;
 
-void launch_score(const ScoreArgs& a, int ppt, int grid, cudaStream_t st) {
+template <bool FOLD>
+void launch_score_t(const ScoreArgs& a, int ppt, int grid, cudaStream_t st) {
     if (a.vec_ok && ppt >= 4) {  // TMA path (bulk copies need 16-byte granularity)
         const size_t smem = (size_t)2 * 3 * kScoreThreads * ppt * sizeof(float);
         // The opt-in above 48 KB of dynamic shared memory is a per-DEVICE function attribute (one process may hold contexts
         // on several GPUs, api.context(device)), and launches may come from several host threads (backward_batch workers).
-        static std::atomic<unsigned char> attr_set[kMaxDevices][2];
+        static std::atomic<unsigned char> attr_set[kMaxDevices][2];  // one table per FOLD instantiation
         int dev = 0;
         cudaGetDevice(&dev);
         const int which = ppt == 8 ? 0 : 1;
         const bool known = dev >= 0 && dev < kMaxDevices;
         if (!known || !attr_set[dev][which].load(std::memory_order_acquire)) {
-            if (ppt == 8) cudaFuncSetAttribute(score_kernel_tma<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            else cudaFuncSetAttribute(score_kernel_tma<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (ppt == 8) cudaFuncSetAttribute(score_kernel_tma<8, FOLD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            else cudaFuncSetAttribute(score_kernel_tma<4, FOLD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (known) attr_set[dev][which].store(1, std::memory_order_release);
         }
-        if (ppt == 8) score_kernel_tma<8><<<grid, kScoreThreads, smem, st>>>(a);
-        else score_kernel_tma<4><<<grid, kScoreThreads, smem, st>>>(a);
+        if (ppt == 8) score_kernel_tma<8, FOLD><<<grid, kScoreThreads, smem, st>>>(a);
+        else score_kernel_tma<4, FOLD><<<grid, kScoreThreads, smem, st>>>(a);
         return;
     }
-    if (ppt == 8) score_kernel<8><<<grid, kScoreThreads, 0, st>>>(a);
-    else if (ppt == 4) score_kernel<4><<<grid, kScoreThreads, 0, st>>>(a);
-    else score_kernel<2><<<grid, kScoreThreads, 0, st>>>(a);
+    if (ppt == 8) score_kernel<8, FOLD><<<grid, kScoreThreads, 0, st>>>(a);
+    else if (ppt == 4) score_kernel<4, FOLD><<<grid, kScoreThreads, 0, st>>>(a);
+    else score_kernel<2, FOLD><<<grid, kScoreThreads, 0, st>>>(a);
+}
+
+void launch_score(const ScoreArgs& a, int ppt, int grid, cudaStream_t st) {
+    if (a.fold) launch_score_t<true>(a, ppt, grid, st);
+    else launch_score_t<false>(a, ppt, grid, st);
 }
 
 // ---------------------------------------------------------------------------------------------

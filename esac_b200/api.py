@@ -116,6 +116,15 @@ def load_library() -> C.CDLL:
     lib.esacb200_device_info.argtypes = [vp, C.POINTER(i32), C.c_char_p, i32]
     lib.esacb200_copy_last_scores.argtypes = [vp, vp, i32]
     lib.esacb200_copy_last_scores.restype = i32
+    # the hypotheses as an autograd node
+    lib.esacb200_hypotheses_tape_bytes.argtypes = [i32, i32, i32, i32]
+    lib.esacb200_hypotheses_tape_bytes.restype = C.c_size_t
+    lib.esacb200_hypotheses_forward.argtypes = [vp, vp, i32, i32, i32, vp, i64, i32] + cam + [vp, C.c_size_t, vp, vp, vp]
+    lib.esacb200_hypotheses_forward.restype = i32
+    lib.esacb200_hypotheses_backward.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp, vp]
+    lib.esacb200_hypotheses_backward.restype = i32
+    lib.esacb200_pose_loss.argtypes = [vp, i32, vp, vp, f32, f32, f32, vp, vp]
+    lib.esacb200_pose_loss.restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
         getattr(lib, "esacb200_" + name).restype = i32
@@ -1012,6 +1021,110 @@ def refine_poses(sceneCoordinates, hypAssignment, poses6, shiftX, shiftY, focalL
                                             float(inlierThreshold), float(maxReproj), int(subSampling),
                                             rounds.ctypes.data, inl.ctypes.data))
     return poses6, rounds, inl
+
+
+# ------------------------------------------------------------------------------------------------
+# the hypotheses as a differentiable function (the layer under autograd.esac_hypotheses)
+# ------------------------------------------------------------------------------------------------
+def hypotheses_tape_bytes(E: int, H: int, W: int, M: int) -> int:
+    """Bytes of the tape a hypotheses forward of M hypotheses on [E,3,H,W] maps leaves for its backward (no device needed)."""
+    return int(load_library().esacb200_hypotheses_tape_bytes(int(E), int(H), int(W), int(M)))
+
+
+def _out_device(a: _Arg):
+    import torch
+    return torch.device("cuda", a.device) if a.is_cuda else torch.device("cpu")
+
+
+def hypotheses_forward(sceneCoordinates, hypAssignment, shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
+                       inlierAlpha, inlierBeta, maxReproj, subSampling):
+    """The hypotheses of an esac.backward call at the same point of the context's call sequence: the same draws, scores and
+    refinements.  Returns torch tensors (scores float64 [M], poses float64 [M,6] = (rvec, tvec), refined where p >=
+    PROB_THRESH and initial elsewhere, contributing bool [M]) on the coordinates' device (CPU for numpy input), and the tape:
+    a CUDA uint8 tensor holding what hypotheses_backward needs.  Runs on torch's current stream."""
+    _check(sceneCoordinates, "Float", 4, "sceneCoordinates")
+    _check(hypAssignment, "Long", 1, "hypAssignment")
+    E, three, H, W = (int(s) for s in sceneCoordinates.shape)
+    if three != 3:
+        raise RuntimeError("sceneCoordinates must be [E, 3, H, W]")
+    if (W - 1) * (H - 1) < 4:
+        raise RuntimeError(f"sceneCoordinates: map {W}x{H} too small to draw 4 distinct cells")
+    if int(hypAssignment.shape[0]) < 1:
+        raise RuntimeError("hypAssignment holds no hypothesis")
+    import torch
+    co = _Arg(sceneCoordinates)
+    aptr, astride, M, adev, _keep = _assign_arg(hypAssignment)
+    ctx = _pick_ctx(co.device, adev)
+    if co.device is None and adev is None:  # the tape is a CUDA tensor: order the call on torch's stream all the same
+        ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
+    dev = _out_device(co)
+    nbytes = hypotheses_tape_bytes(E, H, W, M)
+    tape = torch.empty(nbytes, dtype=torch.uint8, device=torch.device("cuda", ctx.device))
+    scores = torch.empty(M, dtype=torch.float64, device=dev)
+    poses = torch.empty(M, 6, dtype=torch.float64, device=dev)
+    contributing = torch.empty(M, dtype=torch.bool, device=dev)
+    ctx.check(ctx.lib.esacb200_hypotheses_forward(ctx.handle, co.ptr, E, H, W, aptr, astride, M, int(shiftX), int(shiftY),
+                                                  float(focalLength), float(ppointX), float(ppointY), float(inlierThreshold),
+                                                  float(inlierAlpha), float(inlierBeta), float(maxReproj), int(subSampling),
+                                                  tape.data_ptr(), nbytes, scores.data_ptr(), poses.data_ptr(),
+                                                  contributing.data_ptr()))
+    return scores, poses, contributing, tape
+
+
+def hypotheses_backward(tape, sceneCoordinates, outGradients, gradScores=None, gradPoses=None):
+    """Accumulates (+=) into outGradients [E,3,H,W] the gradient of the scene coordinates for upstream gradients gradScores
+    (float64 [M]) and gradPoses (float64 [M,6]) of a hypotheses_forward's outputs; None counts as zero, and entries of
+    hypotheses that do not contribute are ignored.  sceneCoordinates must hold the values the forward saw."""
+    _check(sceneCoordinates, "Float", 4, "sceneCoordinates")
+    _check(outGradients, "Float", 4, "outGradients")
+    shape = tuple(int(s) for s in sceneCoordinates.shape)
+    if shape[1] != 3 or tuple(int(s) for s in outGradients.shape) != shape:
+        raise RuntimeError("sceneCoordinates / outGradients must both be [E, 3, H, W]")
+    M = None
+    if gradScores is not None:
+        _check(gradScores, "Double", 1, "gradScores")
+        M = int(gradScores.shape[0])
+    if gradPoses is not None:
+        _check(gradPoses, "Double", 2, "gradPoses")
+        if int(gradPoses.shape[1]) != 6 or (M is not None and int(gradPoses.shape[0]) != M):
+            raise RuntimeError(f"gradPoses must be [M, 6] with the M of gradScores, got {list(gradPoses.shape)}")
+        M = int(gradPoses.shape[0])
+    if not (_is_torch(tape) and tape.is_cuda and str(tape.dtype) == "torch.uint8" and tape.dim() == 1 and tape.is_contiguous()):
+        raise RuntimeError("tape must be the contiguous CUDA uint8 tensor hypotheses_forward returned")
+    E, _, H, W = shape
+    if M is not None and int(tape.numel()) != hypotheses_tape_bytes(E, H, W, M):
+        raise RuntimeError(f"the tape is not that of a forward of {M} hypotheses on [{E}, 3, {H}, {W}] maps")
+    co = _Arg(sceneCoordinates)
+    gr = _Arg(outGradients, writable=True)
+    gs = _Arg(gradScores) if gradScores is not None else None
+    gp = _Arg(gradPoses) if gradPoses is not None else None
+    ctx = _pick_ctx(co.device, gr.device, tape.device.index, gs.device if gs else None, gp.device if gp else None)
+    ctx.check(ctx.lib.esacb200_hypotheses_backward(ctx.handle, tape.data_ptr(), co.ptr, gr.ptr, E, H, W,
+                                                   gs.ptr if gs else None, gp.ptr if gp else None))
+    gr.finish()
+
+
+def pose_loss(poses, gtPose, wLossRot, wLossTrans, lossCut):
+    """The reference's loss (esac_loss.h) of scene poses float64 [M,6] = (rvec, tvec) against a float32 [4,4] camera->world
+    ground truth, and its dLoss, quirks included, with esac.backward's arithmetic.  Returns torch tensors (losses float64
+    [M], dloss float64 [M,6]) on the poses' device (CPU for numpy input)."""
+    _check(poses, "Double", 2, "poses")
+    _check(gtPose, "Float", 2, "gtPose")
+    if int(poses.shape[1]) != 6 or int(poses.shape[0]) < 1:
+        raise RuntimeError(f"poses must be [M, 6] with M >= 1, got {list(poses.shape)}")
+    if tuple(int(s) for s in gtPose.shape) != (4, 4):
+        raise RuntimeError("gtPose must be [4, 4]")
+    import torch
+    po = _Arg(poses)
+    gt = _Arg(gtPose)
+    ctx = _pick_ctx(po.device, gt.device)
+    M = int(poses.shape[0])
+    dev = _out_device(po)
+    losses = torch.empty(M, dtype=torch.float64, device=dev)
+    dloss = torch.empty(M, 6, dtype=torch.float64, device=dev)
+    ctx.check(ctx.lib.esacb200_pose_loss(ctx.handle, M, po.ptr, gt.ptr, float(wLossRot), float(wLossTrans), float(lossCut),
+                                         losses.data_ptr(), dloss.data_ptr()))
+    return losses, dloss
 
 
 def set_seed(seed: int, device: int | None = None):

@@ -229,3 +229,99 @@ def coord_loss(prediction, gt_coords, cut_loss=100.0):
     if isinstance(prediction, (list, tuple)):
         return CoordLossRagged.apply((gt_coords, cut_loss), *prediction)
     return CoordLoss.apply(prediction, gt_coords, cut_loss)
+
+
+# ------------------------------------------------------------------------------------------------
+# The hypotheses as an autograd node: any pose loss written in torch
+# ------------------------------------------------------------------------------------------------
+class EsacHypotheses(torch.autograd.Function):
+    """Scores and poses of the hypotheses of an esac.backward call, differentiable with respect to the scene coordinates."""
+
+    @staticmethod
+    def forward(ctx, scene_coordinates, hyp_assignment, *params):
+        scores, poses, contributing, tape = api.hypotheses_forward(scene_coordinates.detach(), hyp_assignment, *params)
+        # the coordinates are passed to the backward again; autograd's version counter catches an in-place change
+        ctx.save_for_backward(scene_coordinates, tape)
+        ctx.mark_non_differentiable(contributing)
+        ctx.set_materialize_grads(False)
+        ctx.n_params = len(params)
+        return scores, poses, contributing
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_scores, grad_poses, _grad_contributing):
+        coords, tape = ctx.saved_tensors
+        grads = torch.zeros_like(coords)
+        api.hypotheses_backward(tape, coords, grads, grad_scores, grad_poses)
+        return (grads, None) + (None,) * ctx.n_params
+
+
+def esac_hypotheses(scene_coordinates, hyp_assignment, shift_x, shift_y, focal_length, ppoint_x, ppoint_y,
+                    inlier_threshold, inlier_alpha, inlier_beta, max_reproj, sub_sampling):
+    """The hypotheses of esac.backward as a differentiable function, so that a trainer can write its own pose loss in torch.
+
+    scene_coordinates [E,3,H,W] float32 (CPU or CUDA), hyp_assignment [M] int64; the other arguments are esac.forward's.
+    Returns, on the coordinates' device:
+      scores        float64 [M]    the soft-inlier scores (softmax(scores) are the hypothesis probabilities),
+      poses         float64 [M,6]  scene pose (rvec, tvec) per hypothesis: refined where p >= PROB_THRESH, else initial,
+      contributing  bool [M]       p >= PROB_THRESH.
+    It draws what an esac.backward call at the same point of the context's call sequence would draw, so with the option
+    fixed_seed and the same seed its hypotheses, scores and refined poses are bitwise those of esac.backward.
+
+    The backward gives d L / d scene_coordinates from the gradients of `scores` and `poses` (either may be absent, which
+    counts as zero).  As in the reference, only contributing hypotheses are differentiated: gradients reaching hypotheses
+    with p < PROB_THRESH are ignored, and a refined pose is differentiated through its refinement's linearisation, with the
+    reference's > 10 clamps.  The node is once differentiable.  With
+        L = (softmax(scores) * reference_pose_loss(poses, gt_pose, w_rot, w_trans, cut)).sum()
+    L and its gradient are those of esac.backward / esac_loss."""
+    return EsacHypotheses.apply(scene_coordinates, hyp_assignment, shift_x, shift_y, focal_length, ppoint_x, ppoint_y,
+                                inlier_threshold, inlier_alpha, inlier_beta, max_reproj, sub_sampling)
+
+
+class ReferencePoseLoss(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, poses, gt_pose, w_rot, w_trans, cut):
+        losses, dloss = api.pose_loss(poses.detach(), gt_pose, w_rot, w_trans, cut)
+        ctx.save_for_backward(dloss)
+        return losses
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_losses):
+        (dloss,) = ctx.saved_tensors
+        return grad_losses.to(dloss.device)[:, None] * dloss, None, None, None, None
+
+
+def reference_pose_loss(poses, gt_pose, w_rot, w_trans, cut):
+    """The reference's pose loss (esac_loss.h `loss`) of scene poses [M,6] = (rvec, tvec) float64 against a float32 [4,4]
+    camera->world ground truth: wRot * angle(deg) + wTrans * |t_est - t_gt|, above `cut` sqrt(cut * l), at most 1e7.
+    Its gradient is the reference's dLoss, bug for bug: above the cut it is scaled as the derivative of sqrt(l) (not of
+    sqrt(cut * l)), the angle uses CV_PI where the loss uses 3.1415926, and it is zero on NaN, on errors below 1e-8 and at
+    the 1e7 cap.  Both come from the device functions esac.backward uses.  Returns float64 [M]."""
+    return ReferencePoseLoss.apply(poses, gt_pose, w_rot, w_trans, cut)
+
+
+def _skew(r):
+    z = torch.zeros_like(r[..., 0])
+    return torch.stack([torch.stack([z, -r[..., 2], r[..., 1]], -1),
+                        torch.stack([r[..., 2], z, -r[..., 0]], -1),
+                        torch.stack([-r[..., 1], r[..., 0], z], -1)], -2)
+
+
+def pose_to_transform(poses):
+    """pose2trans (esac_util.h) in differentiable torch: scene poses [M,6] = (rvec, tvec), world->camera, to camera->world
+    transforms [M,4,4] = [R^T | -R^T t].  R = I + a K + b K^2 with K = [r]x, a = sin(th)/th, b = (1 - cos(th))/th^2; below
+    th = 1e-3 a and b are their Taylor series in th^2, so th = 0 has a finite gradient."""
+    r, t = poses[..., :3], poses[..., 3:]
+    th2 = (r * r).sum(-1)
+    small = th2 < 1e-6
+    th2_safe = torch.where(small, torch.ones_like(th2), th2)
+    th = torch.sqrt(th2_safe)
+    a = torch.where(small, 1 - th2 / 6 + th2 * th2 / 120, torch.sin(th) / th)
+    b = torch.where(small, 0.5 - th2 / 24 + th2 * th2 / 720, (1 - torch.cos(th)) / th2_safe)
+    K = _skew(r)
+    eye = torch.eye(3, dtype=poses.dtype, device=poses.device).expand(K.shape)
+    R = eye + a[..., None, None] * K + b[..., None, None] * (K @ K)
+    Rt = R.transpose(-1, -2)
+    bottom = torch.cat([torch.zeros_like(t[..., None, :]), torch.ones_like(t[..., None, :1])], -1)
+    return torch.cat([torch.cat([Rt, -(Rt @ t[..., None])], -1), bottom], -2)

@@ -66,6 +66,19 @@ struct BwdAux {
     int tiles;
 };
 
+// The fields of job j's record that do not depend on the loss: hypothesis h, its expert, whether it was refined and which
+// refinement mask buffer holds its final inliers, initial and refined rotation with their Rodrigues Jacobians, minimal set.
+__device__ __forceinline__ void job_record(const BwdArgs& a, int j, int h, HypGrad& g) {
+    g.h = h;
+    g.expert = a.assign32[h];
+    g.flagI = a.rounds[2 * j] > 0 ? 1 : 0;
+    g.pad = a.rounds[2 * j + 1];
+    rodrigues_v2m(a.init[h].r, g.Ri, g.dRi);
+    rodrigues_v2m(a.ref[h].r, g.Rr, g.dRr);
+    for (int i = 0; i < 3; ++i) { g.ti[i] = a.init[h].t[i]; g.tr[i] = a.ref[h].t[i]; }
+    for (int i = 0; i < 8; ++i) g.cells[i] = a.cells[h * 8 + i];
+}
+
 // ---------------------------------------------------------------------------------------------
 // B1: losses, expectation, score gradients, per-job records
 // ---------------------------------------------------------------------------------------------
@@ -95,17 +108,10 @@ __global__ void __launch_bounds__(1024) bwd_loss_kernel(const __grid_constant__ 
     for (int j = tid; j < nc; j += blockDim.x) {
         const int h = a.contrib[j];
         HypGrad& g = x.hg[j];
-        g.h = h;
-        g.expert = a.assign32[h];
-        g.flagI = a.rounds[2 * j] > 0 ? 1 : 0;
-        g.pad = a.rounds[2 * j + 1];
+        job_record(a, j, h, g);
         g.p = a.probs[h];
         g.g = a.probs[h] * a.losses[h] - a.probs[h] * expected;  // esac_derivative.h:372-374
-        rodrigues_v2m(a.init[h].r, g.Ri, g.dRi);
-        rodrigues_v2m(a.ref[h].r, g.Rr, g.dRr);
-        for (int i = 0; i < 3; ++i) { g.ti[i] = a.init[h].t[i]; g.tr[i] = a.ref[h].t[i]; }
         pose_dloss(a.ref[h], gtp, (double)a.wRot, (double)a.wTrans, (double)a.cut, g.dl);
-        for (int i = 0; i < 8; ++i) g.cells[i] = a.cells[h * 8 + i];
         g.maxjr_bits = 0ull;
         atomicAdd(&x.expert_njobs[g.expert], 1);
     }
@@ -414,22 +420,118 @@ __global__ void __launch_bounds__(kBwdThreads) bwd_assemble_kernel(const __grid_
     if (live) { gr[p] = o0; gr[P.N + p] = o1; gr[2 * (size_t)P.N + p] = o2; }
 }
 
-void launch_backward_losses(const BwdArgs& a, cudaStream_t st) {
-    BwdAux x;
-    x.hg = (HypGrad*)a.hyp_grad;
-    x.red = a.red;
-    x.expert_njobs = (int*)a.job_of;
-    x.tiles = bwd_tiles(a.P.N);
-    bwd_loss_kernel<<<1, 1024, 0, st>>>(a, x);
+// ---------------------------------------------------------------------------------------------
+// Hypotheses node (esacb200_hypotheses_forward / _backward): the forward keeps the per-job records and the final inlier
+// masks in the caller's tape; the backward rebuilds the records with the caller's upstream gradients and runs B2-B5.
+// ---------------------------------------------------------------------------------------------
+size_t tape_records_offset() { return kTapeHeadBytes; }
+size_t tape_masks_offset(int M) { return kTapeHeadBytes + (size_t)M * sizeof(HypGrad); }
+size_t tape_bytes(int M, int N) { return tape_masks_offset(M) + (size_t)M * 2 * ((N + 31) / 32) * 4; }
+
+// Per-job records of the contributing hypotheses, the header (with n_contrib) and a contributing flag per hypothesis.
+__global__ void __launch_bounds__(1024) tape_record_kernel(const __grid_constant__ BwdArgs a, TapeHead head, TapeHead* out_head,
+                                                           HypGrad* recs, unsigned char* contrib_flags) {
+    const int tid = threadIdx.x;
+    const int nc = *a.n_contrib;
+    for (int h = tid; h < a.P.M; h += blockDim.x) contrib_flags[h] = 0;
+    __syncthreads();
+    for (int j = tid; j < nc; j += blockDim.x) {
+        const int h = a.contrib[j];
+        HypGrad& g = recs[j];
+        job_record(a, j, h, g);
+        g.p = 0;
+        g.g = 0;
+        for (int i = 0; i < 6; ++i) g.dl[i] = 0;
+        g.maxjr_bits = 0ull;
+        contrib_flags[h] = 1;
+    }
+    if (tid == 0) {
+        head.n_contrib = nc;
+        *out_head = head;
+    }
 }
 
-void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t st) {
+void launch_tape_records(const BwdArgs& a, const TapeHead& head, void* tape, unsigned char* contrib_flags, cudaStream_t st) {
+    tape_record_kernel<<<1, 1024, 0, st>>>(a, head, (TapeHead*)tape, (HypGrad*)((char*)tape + tape_records_offset()),
+                                           contrib_flags);
+}
+
+// B1 of the hypotheses node: the tape's records with the caller's upstream gradients.  Path I takes dl = dL/d pose_h with
+// multiplier p = 1, path II takes g = dL/d s_h; B2-B5 are then the vector-Jacobian product of (scores, poses).
+__global__ void __launch_bounds__(1024) bwd_upstream_kernel(const __grid_constant__ BwdArgs a, BwdAux x, const HypGrad* recs,
+                                                            const double* d_scores, const double* d_poses6) {
+    const int tid = threadIdx.x;
+    for (int e = tid; e < a.P.E; e += blockDim.x) x.expert_njobs[e] = 0;
+    const int nc = *a.n_contrib;
+    const size_t n8 = (size_t)nc * (sizeof(HypGrad) / 8);
+    for (size_t i = tid; i < n8; i += blockDim.x) ((double*)x.hg)[i] = ((const double*)recs)[i];
+    __syncthreads();
+    for (int j = tid; j < nc; j += blockDim.x) {
+        HypGrad& g = x.hg[j];
+        const int h = g.h;
+        g.p = 1.0;
+        g.g = d_scores[h];
+        for (int i = 0; i < 6; ++i) g.dl[i] = d_poses6[(size_t)h * 6 + i];
+        g.maxjr_bits = 0ull;
+        atomicAdd(&x.expert_njobs[g.expert], 1);
+    }
+}
+
+// The reference's loss and dLoss of M scene poses against one ground truth (esacb200_pose_loss): the device functions of B1.
+struct Gt16 {
+    float v[16];
+};
+__global__ void __launch_bounds__(256) pose_loss_kernel(const Pose* poses, int M, const Gt16 gt, float wRot, float wTrans,
+                                                         float cut, double* losses, double* dloss6) {
+    __shared__ Pose gtp;
+    __shared__ double gtT[16];
+    if (threadIdx.x == 0) gt_trans2pose(gt.v, gtp, gtT);
+    __syncthreads();
+    for (int h = threadIdx.x; h < M; h += blockDim.x) {
+        double T[16];
+        pose2trans(poses[h], T);
+        losses[h] = pose_loss(T, gtT, (double)wRot, (double)wTrans, (double)cut);
+        pose_dloss(poses[h], gtp, (double)wRot, (double)wTrans, (double)cut, dloss6 + (size_t)h * 6);
+    }
+}
+
+void launch_pose_loss(const Pose* poses, int M, const float gt[16], float wRot, float wTrans, float cut, double* losses,
+                      double* dloss6, cudaStream_t st) {
+    Gt16 g;
+    for (int i = 0; i < 16; ++i) g.v[i] = gt[i];
+    pose_loss_kernel<<<1, 256, 0, st>>>(poses, M, g, wRot, wTrans, cut, losses, dloss6);
+}
+
+static BwdAux bwd_aux(const BwdArgs& a) {
     BwdAux x;
     x.hg = (HypGrad*)a.hyp_grad;
     x.red = a.red;
     x.expert_njobs = (int*)a.job_of;  // [E] ints, buffer provided by the caller
     x.tiles = bwd_tiles(a.P.N);
+    return x;
+}
+
+static void launch_backward_tail(const BwdArgs& a, const BwdAux& x, int max_jobs, int sm_count, cudaStream_t st);
+
+void launch_backward_losses(const BwdArgs& a, cudaStream_t st) {
+    bwd_loss_kernel<<<1, 1024, 0, st>>>(a, bwd_aux(a));
+}
+
+void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t st) {
+    const BwdAux x = bwd_aux(a);
     bwd_loss_kernel<<<1, 1024, 0, st>>>(a, x);
+    launch_backward_tail(a, x, max_jobs, sm_count, st);
+}
+
+void launch_backward_upstream(const BwdArgs& a, const void* tape, const double* d_scores, const double* d_poses6, int max_jobs,
+                              int sm_count, cudaStream_t st) {
+    const BwdAux x = bwd_aux(a);
+    bwd_upstream_kernel<<<1, 1024, 0, st>>>(a, x, (const HypGrad*)((const char*)tape + tape_records_offset()), d_scores, d_poses6);
+    launch_backward_tail(a, x, max_jobs, sm_count, st);
+}
+
+// B2-B5: everything after the per-job records, shared by the loss-driven backward and the hypotheses node.
+static void launch_backward_tail(const BwdArgs& a, const BwdAux& x, int max_jobs, int sm_count, cudaStream_t st) {
     long long items = (long long)max_jobs * x.tiles;
     int grid = (int)(items < sm_count * 8ll ? items : sm_count * 8ll);
     if (grid < 1) grid = 1;

@@ -94,7 +94,8 @@ struct esacb200_ctx {
     // workspace
     DevBuf coords, grads, assign64, assign32, counts, offsets, perm, slot_of, chunks, scalars, centres, poses, poses_ref,
         cells, tries, posepk, part, scores, probs, stats, contrib, masks, rounds, scratch, barrier, out17, inject,
-        losses, red, hypgrad, job_of, gt, smp_int, smp_surv, smp_trace, clist, eflags, coords4, coords_alt, assign64_alt, out_batch, prof;
+        losses, red, hypgrad, job_of, gt, smp_int, smp_surv, smp_trace, clist, eflags, coords4, coords_alt, assign64_alt, out_batch, prof,
+        contrib8, upstream;
     float* h_out = nullptr;  // pinned staging: 32 floats
     double* h_dbl = nullptr; // pinned staging: 8 doubles
     int inj_M = 0, inj_T = 0;
@@ -498,13 +499,17 @@ RefineSizes refine_sizes(const esacb200_ctx* ctx, const Problem& P, int max_jobs
     return z;
 }
 
+// masks_out: where the final inlier masks go ([max_jobs][2][words]); null = the context's workspace.
 int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, const int* d_jobs, const int* d_njobs,
-               int n_jobs_host, int max_jobs, int group) {
+               int n_jobs_host, int max_jobs, int group, uint32_t* masks_out = nullptr) {
     const Problem& P = pl.P;
     const int words = (P.N + 31) / 32;
     const RefineSizes z = refine_sizes(ctx, P, max_jobs, group);
     const int n_groups = z.n_groups;
-    CK(ctx->masks.ensure(z.masks));
+    if (!masks_out) {
+        CK(ctx->masks.ensure(z.masks));
+        masks_out = ctx->masks.as<uint32_t>();
+    }
     CK(ctx->rounds.ensure(z.rounds));
     CK(ctx->scratch.ensure(z.scratch));
     if (group > 1) CK(cudaMemsetAsync(ctx->scratch.p, 0, refine_scratch_doubles(n_groups, group) * 8, ctx->stream));  // LL elements: no stale sequence numbers
@@ -520,7 +525,7 @@ int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, con
     a.jobs = d_jobs;
     a.n_jobs = d_njobs;
     a.n_jobs_host = n_jobs_host;
-    a.masks = ctx->masks.as<uint32_t>();
+    a.masks = masks_out;
     a.mask_words = words;
     a.rounds = ctx->rounds.as<int>();
     a.scratch = ctx->scratch.as<double>();
@@ -793,7 +798,8 @@ void esacb200_destroy(esacb200_ctx* ctx) {
                       &ctx->slot_of, &ctx->chunks, &ctx->scalars, &ctx->centres, &ctx->poses, &ctx->poses_ref, &ctx->cells,
                       &ctx->tries, &ctx->posepk, &ctx->part, &ctx->scores, &ctx->probs, &ctx->stats, &ctx->contrib,
                       &ctx->masks, &ctx->rounds, &ctx->scratch, &ctx->barrier, &ctx->out17, &ctx->inject, &ctx->losses,
-                      &ctx->red, &ctx->hypgrad, &ctx->job_of, &ctx->gt, &ctx->smp_int, &ctx->smp_surv, &ctx->smp_trace, &ctx->clist, &ctx->eflags, &ctx->coords4, &ctx->coords_alt, &ctx->assign64_alt, &ctx->out_batch, &ctx->prof, &ctx->gathered, &ctx->grads_work};
+                      &ctx->red, &ctx->hypgrad, &ctx->job_of, &ctx->gt, &ctx->smp_int, &ctx->smp_surv, &ctx->smp_trace, &ctx->clist, &ctx->eflags, &ctx->coords4, &ctx->coords_alt, &ctx->assign64_alt, &ctx->out_batch, &ctx->prof, &ctx->gathered, &ctx->grads_work,
+                      &ctx->contrib8, &ctx->upstream};
     for (DevBuf* b : bufs) b->release();
     for (int i = 0; i < EV_COUNT; ++i)
         if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
@@ -1268,6 +1274,76 @@ static int for_flagged_planes(esacb200_ctx* ctx, int E, size_t plane, float* wor
     return 0;
 }
 
+// The sharded backward's steps inside the hypotheses prefix (none for a single-GPU call).
+struct ShardSteps {
+    esacb200_exchange_fn exchange = nullptr;  // host callback: softmax normalisation over all ranks
+    void* user = nullptr;
+    bool use_nccl = false;      // the same exchange as an all-gather on the device
+    bool reduce_grads = false;  // hypothesis-major sharding: zero the work buffer's slices of the planes some rank updates
+    float* d_work = nullptr;
+    float* d_dst = nullptr;
+};
+
+// The hypotheses of a backward call: stage -> sample -> score -> select [-> exchange 1] -> refHyps = initHyps -> one read-back
+// of n_contrib -> refinement of every contributing hypothesis (final inlier masks into `masks`, or the workspace when null).
+// esac.backward and the hypotheses node both run it, so they draw, score and refine alike.
+static int run_hypotheses(esacb200_ctx* ctx, Plan& pl, const float* coords, const int64_t* assign, int64_t assign_stride,
+                          const ShardSteps& sh, uint32_t* masks) {
+    int rc = stage_inputs(ctx, pl, coords, assign, assign_stride);
+    if (rc) return rc;
+    const Problem& P = pl.P;
+    const int M = P.M, E = P.E;
+    int* sc = ctx->scalars.as<int>();
+    const uint64_t seed = call_seed(ctx);
+    rc = run_sample(ctx, pl, seed);
+    if (rc) return rc;
+    rc = run_score(ctx, pl);
+    if (rc) return rc;
+    if (sh.exchange) {
+        // exchange 1 (SURVEY 8e): softmax normalisation over the hypotheses of ALL ranks
+        CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.as<double>() + 5, 2 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        double v[2] = {ctx->h_dbl[0], ctx->h_dbl[1]};
+        if (sh.exchange(sh.user, 1, v, 2) != 0) return fail(ctx, ESACB200_ERR_ARG, "exchange callback failed (phase 1)");
+        launch_rescale_probs(ctx->scores.as<double>(), P, v[0], v[1], ctx->probs.as<double>(), ctx->contrib.as<int>(),
+                             sc + S_NCONTRIB, ctx->stream);
+        ctx->st.kernel_launches += 1;
+    } else if (sh.use_nccl) {
+        // exchange 1 on the device: all-gather of the (max, sum exp) pairs, merged by the kernel that rebuilds the probabilities
+        CK(ctx->gathered.ensure((size_t)ctx->comm_world * 2 * 8));
+        CKN(nccl_api().AllGather(ctx->stats.as<double>() + 5, ctx->gathered.p, 2, kNcclFloat64, ctx->nccl_comm, ctx->stream));
+        launch_rescale_probs_gathered(ctx->scores.as<double>(), P, ctx->gathered.as<double>(), ctx->comm_world, nullptr,
+                                      ctx->probs.as<double>(), ctx->contrib.as<int>(), sc + S_NCONTRIB, ctx->stream);
+        ctx->st.kernel_launches += 2;
+    }
+    // refHyps = initHyps for everything below PROB_THRESH (esac.cpp:331-334)
+    CK(cudaMemcpyAsync(ctx->poses_ref.p, ctx->poses.p, (size_t)M * sizeof(Pose), cudaMemcpyDeviceToDevice, ctx->stream));
+    // Refining many hypotheses is fp64-throughput bound, so every SM should be busy and no CTA should wait at an inter-CTA
+    // barrier longer than needed: one 4-byte read-back of the number of contributing hypotheses (a ~20 us stall on a
+    // multi-millisecond call) lets the group size be coresident / jobs.
+    CK(cudaMemcpyAsync(ctx->h_out + 28, sc + S_NCONTRIB, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    if (sh.reduce_grads) {  // which planes receive gradient on some rank: rides on the same host synchronisation
+        CK(ctx->eflags.ensure((size_t)E * sizeof(int)));
+        launch_expert_flags(ctx->contrib.as<int>(), sc + S_NCONTRIB, ctx->assign32.as<int>(), E, ctx->eflags.as<int>(), ctx->stream);
+        CKN(nccl_api().AllReduce(ctx->eflags.p, ctx->eflags.p, (size_t)E, kNcclInt32, kNcclMax, ctx->nccl_comm, ctx->stream));
+        CK(cudaMemcpyAsync(ctx->h_flags, ctx->eflags.p, (size_t)E * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        ctx->st.kernel_launches += 2;
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (sh.reduce_grads) {
+        rc = for_flagged_planes(ctx, E, (size_t)3 * P.N, sh.d_work, sh.d_dst, 0);
+        if (rc) return rc;
+    }
+    int n_jobs_now = *(const int*)(ctx->h_out + 28);
+    if (n_jobs_now < 1) n_jobs_now = 1;
+    int group = pick_group(ctx, P, n_jobs_now);
+    rc = run_refine(ctx, pl, ctx->poses.as<Pose>(), ctx->poses_ref.as<Pose>(), ctx->contrib.as<int>(), sc + S_NCONTRIB, 0, M, group,
+                    masks);
+    if (rc) return rc;
+    mark(ctx, EV_REFINE);
+    return 0;
+}
+
 // -------------------------------------------------------------------------------------------------
 static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, int E, int H, int W, const int64_t* assign,
                          int64_t assign_stride, int M, const float* gt_pose, float wRot, float wTrans, float cut, int shiftX,
@@ -1301,55 +1377,16 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
         rc = ensure_host_flags(ctx, E);
         if (rc) return rc;
     }
-    rc = stage_inputs(ctx, pl, coords, assign, assign_stride);
+    ShardSteps sh;
+    sh.exchange = exchange;
+    sh.user = user;
+    sh.use_nccl = use_nccl;
+    sh.reduce_grads = reduce_grads;
+    sh.d_work = d_grads;
+    sh.d_dst = d_dst;
+    rc = run_hypotheses(ctx, pl, coords, assign, assign_stride, sh, nullptr);
     if (rc) return rc;
     int* sc = ctx->scalars.as<int>();
-    const uint64_t seed = call_seed(ctx);
-    rc = run_sample(ctx, pl, seed);
-    if (rc) return rc;
-    rc = run_score(ctx, pl);
-    if (rc) return rc;
-    if (exchange) {
-        // exchange 1 (SURVEY 8e): softmax normalisation over the hypotheses of ALL ranks
-        CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.as<double>() + 5, 2 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        double v[2] = {ctx->h_dbl[0], ctx->h_dbl[1]};
-        if (exchange(user, 1, v, 2) != 0) return fail(ctx, ESACB200_ERR_ARG, "exchange callback failed (phase 1)");
-        launch_rescale_probs(ctx->scores.as<double>(), P, v[0], v[1], ctx->probs.as<double>(), ctx->contrib.as<int>(),
-                             sc + S_NCONTRIB, ctx->stream);
-        ctx->st.kernel_launches += 1;
-    } else if (use_nccl) {
-        // exchange 1 on the device: all-gather of the (max, sum exp) pairs, merged by the kernel that rebuilds the probabilities
-        CK(ctx->gathered.ensure((size_t)ctx->comm_world * 2 * 8));
-        CKN(nccl_api().AllGather(ctx->stats.as<double>() + 5, ctx->gathered.p, 2, kNcclFloat64, ctx->nccl_comm, ctx->stream));
-        launch_rescale_probs_gathered(ctx->scores.as<double>(), P, ctx->gathered.as<double>(), ctx->comm_world, nullptr,
-                                      ctx->probs.as<double>(), ctx->contrib.as<int>(), sc + S_NCONTRIB, ctx->stream);
-        ctx->st.kernel_launches += 2;
-    }
-    // refHyps = initHyps for everything below PROB_THRESH (esac.cpp:331-334)
-    CK(cudaMemcpyAsync(ctx->poses_ref.p, ctx->poses.p, (size_t)M * sizeof(Pose), cudaMemcpyDeviceToDevice, ctx->stream));
-    // Refining many hypotheses is fp64-throughput bound, so every SM should be busy and no CTA should wait at an inter-CTA
-    // barrier longer than needed: one 4-byte read-back of the number of contributing hypotheses (a ~20 us stall on a
-    // multi-millisecond call) lets the group size be coresident / jobs.
-    CK(cudaMemcpyAsync(ctx->h_out + 28, sc + S_NCONTRIB, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    if (reduce_grads) {  // which planes receive gradient on some rank: rides on the same host synchronisation
-        CK(ctx->eflags.ensure((size_t)E * sizeof(int)));
-        launch_expert_flags(ctx->contrib.as<int>(), sc + S_NCONTRIB, ctx->assign32.as<int>(), E, ctx->eflags.as<int>(), ctx->stream);
-        CKN(nccl_api().AllReduce(ctx->eflags.p, ctx->eflags.p, (size_t)E, kNcclInt32, kNcclMax, ctx->nccl_comm, ctx->stream));
-        CK(cudaMemcpyAsync(ctx->h_flags, ctx->eflags.p, (size_t)E * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-        ctx->st.kernel_launches += 2;
-    }
-    CK(cudaStreamSynchronize(ctx->stream));
-    if (reduce_grads) {
-        rc = for_flagged_planes(ctx, E, (size_t)3 * P.N, d_grads, d_dst, 0);
-        if (rc) return rc;
-    }
-    int n_jobs_now = *(const int*)(ctx->h_out + 28);
-    if (n_jobs_now < 1) n_jobs_now = 1;
-    int group = pick_group(ctx, P, n_jobs_now);
-    rc = run_refine(ctx, pl, ctx->poses.as<Pose>(), ctx->poses_ref.as<Pose>(), ctx->contrib.as<int>(), sc + S_NCONTRIB, 0, M, group);
-    if (rc) return rc;
-    mark(ctx, EV_REFINE);
     const int tiles = bwd_tiles(P.N);
     CK(ctx->losses.ensure((size_t)M * 8));
     CK(ctx->red.ensure((size_t)M * tiles * bwd_red_vals() * 8));
@@ -1445,6 +1482,168 @@ int esacb200_backward(esacb200_ctx* ctx, const float* coords, float* grads, int 
                       double* out_loss) try {
     return backward_impl(ctx, coords, grads, E, H, W, assign, assign_stride, M, gt_pose, wRot, wTrans, cut, shiftX, shiftY, f, ppx,
                          ppy, tau, alpha, beta, maxReproj, sub, nullptr, nullptr, out_loss);
+} ESAC_ABI_CATCH(ctx)
+
+// -------------------------------------------------------------------------------------------------
+// The hypotheses as an autograd node: a forward that returns scores, refined poses and contributing flags and keeps what its
+// backward needs in a caller-owned tape, and a backward that maps upstream gradients of (scores, poses) to the coordinates.
+size_t esacb200_hypotheses_tape_bytes(int E, int H, int W, int M) {
+    if (E <= 0 || H <= 0 || W <= 0 || M <= 0 || (long long)H * W > (1ll << 30)) return 0;
+    return tape_bytes(M, H * W);
+}
+
+int esacb200_hypotheses_forward(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
+                                int64_t assign_stride, int M, int shiftX, int shiftY, float f, float ppx, float ppy, float tau,
+                                float alpha, float beta, float maxReproj, int sub, void* tape, size_t tape_bytes_,
+                                double* out_scores, double* out_poses6, uint8_t* out_contrib) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (!coords || !assign || !tape || !out_scores || !out_poses6 || !out_contrib) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    Plan pl;
+    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub);
+    if (rc) return rc;
+    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small to draw 4 distinct cells from [0,W-2]x[0,H-2]", W, H);
+    if (ctx->inj_M && ctx->inj_M != M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are for M=%d, call has M=%d", ctx->inj_M, M);
+    const size_t need = tape_bytes(M, pl.P.N);
+    if (tape_bytes_ < need) return fail(ctx, ESACB200_ERR_ARG, "tape holds %zu bytes, this call needs %zu", tape_bytes_, need);
+    if (!is_device_ptr(tape) || ((uintptr_t)tape & 15)) return fail(ctx, ESACB200_ERR_ARG, "tape must be 16-byte aligned device memory");
+    begin_call(ctx);
+    rc = run_hypotheses(ctx, pl, coords, assign, assign_stride, ShardSteps(), (uint32_t*)((char*)tape + tape_masks_offset(M)));
+    if (rc) return rc;
+    const Problem& P = pl.P;
+    int* sc = ctx->scalars.as<int>();
+    CK(ctx->contrib8.ensure((size_t)M));
+    BwdArgs b;
+    memset(&b, 0, sizeof(b));
+    b.assign32 = ctx->assign32.as<int>();
+    b.init = ctx->poses.as<Pose>();
+    b.ref = ctx->poses_ref.as<Pose>();
+    b.cells = ctx->cells.as<int>();
+    b.contrib = ctx->contrib.as<int>();
+    b.n_contrib = sc + S_NCONTRIB;
+    b.rounds = ctx->rounds.as<int>();
+    b.P = P;
+    TapeHead head;
+    memset(&head, 0, sizeof(head));
+    head.magic = kTapeMagic;
+    head.M = M;
+    head.mask_words = (P.N + 31) / 32;
+    head.P = P;
+    launch_tape_records(b, head, tape, ctx->contrib8.as<unsigned char>(), ctx->stream);
+    CK(cudaGetLastError());
+    ctx->st.kernel_launches += 1;
+    CK(cudaMemcpyAsync(out_scores, ctx->scores.p, (size_t)M * 8, cudaMemcpyDefault, ctx->stream));
+    CK(cudaMemcpyAsync(out_poses6, ctx->poses_ref.p, (size_t)M * sizeof(Pose), cudaMemcpyDefault, ctx->stream));
+    CK(cudaMemcpyAsync(out_contrib, ctx->contrib8.p, (size_t)M, cudaMemcpyDefault, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->h_out + 20, sc, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.p, 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    mark(ctx, EV_END);
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    const int* hs = (const int*)(ctx->h_out + 20);
+    if (hs[S_FLAGS]) return fail(ctx, ESACB200_ERR_ARG, "hypAssignment holds an expert index outside [0, %d)", E);
+    ctx->st.M = M;
+    ctx->st.winner = hs[S_WINNER];
+    ctx->st.n_contrib = hs[S_NCONTRIB];
+    ctx->st.entropy = ctx->h_dbl[0];
+    ctx->last_M = M;
+    ctx->last_backward = false;
+    finish_stats(ctx);
+    ctx->inj_M = ctx->inj_T = 0;
+    return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_hypotheses_backward(esacb200_ctx* ctx, const void* tape, const float* coords, float* grads, int E, int H, int W,
+                                 const double* d_scores, const double* d_poses6) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (!tape || !coords || !grads) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    if (!is_device_ptr(tape) || ((uintptr_t)tape & 15)) return fail(ctx, ESACB200_ERR_ARG, "tape must be 16-byte aligned device memory");
+    // the header: problem and hypothesis count of the forward (ordered after the forward on this stream)
+    TapeHead head;
+    CK(cudaMemcpyAsync(&head, tape, sizeof(head), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (head.magic != kTapeMagic) return fail(ctx, ESACB200_ERR_ARG, "tape holds no hypotheses forward");
+    const Problem P = head.P;
+    if (P.E != E || P.H != H || P.W != W)
+        return fail(ctx, ESACB200_ERR_ARG, "coordinates are [%d,3,%d,%d], the forward saw [%d,3,%d,%d]", E, H, W, P.E, P.H, P.W);
+    const int M = head.M;
+    begin_call(ctx);
+    const size_t cbytes = (size_t)E * 3 * P.N * sizeof(float);
+    const float* d_coords = coords;
+    if (!is_device_ptr(coords)) {
+        CK(ctx->coords.ensure(cbytes));
+        CK(cudaMemcpyAsync(ctx->coords.p, coords, cbytes, cudaMemcpyHostToDevice, ctx->stream));
+        d_coords = ctx->coords.as<float>();
+    }
+    float* d_grads = grads;
+    const bool grads_on_host = !is_device_ptr(grads);
+    if (grads_on_host) {
+        CK(ctx->grads.ensure(cbytes));
+        CK(cudaMemcpyAsync(ctx->grads.p, grads, cbytes, cudaMemcpyHostToDevice, ctx->stream));
+        d_grads = ctx->grads.as<float>();
+    }
+    // upstream gradients: [M] of the scores then [M,6] of the poses; an absent one is zero
+    CK(ctx->upstream.ensure((size_t)M * 7 * 8));
+    double* up = ctx->upstream.as<double>();
+    if (d_scores) CK(cudaMemcpyAsync(up, d_scores, (size_t)M * 8, cudaMemcpyDefault, ctx->stream));
+    else CK(cudaMemsetAsync(up, 0, (size_t)M * 8, ctx->stream));
+    if (d_poses6) CK(cudaMemcpyAsync(up + M, d_poses6, (size_t)M * 6 * 8, cudaMemcpyDefault, ctx->stream));
+    else CK(cudaMemsetAsync(up + M, 0, (size_t)M * 6 * 8, ctx->stream));
+    mark(ctx, EV_REFINE);
+    const int tiles = bwd_tiles(P.N);
+    CK(ctx->red.ensure((size_t)M * tiles * bwd_red_vals() * 8));
+    CK(ctx->hypgrad.ensure((size_t)M * bwd_hypgrad_bytes()));
+    CK(ctx->job_of.ensure((size_t)(M > E ? M : E) * 4));
+    BwdArgs b;
+    memset(&b, 0, sizeof(b));
+    b.coords = d_coords;
+    b.grads = d_grads;
+    b.n_contrib = (const int*)((const char*)tape + offsetof(TapeHead, n_contrib));
+    b.job_of = ctx->job_of.as<int>();
+    b.masks = (const uint32_t*)((const char*)tape + tape_masks_offset(M));
+    b.mask_words = head.mask_words;
+    b.red = ctx->red.as<double>();
+    b.hyp_grad = ctx->hypgrad.p;
+    b.P = P;
+    launch_backward_upstream(b, tape, up, up + M, M, ctx->sm_count, ctx->stream);
+    CK(cudaGetLastError());
+    ctx->st.kernel_launches += 5;
+    mark(ctx, EV_BWD);
+    if (grads_on_host) CK(cudaMemcpyAsync(grads, d_grads, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
+    mark(ctx, EV_END);
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    ctx->st.M = M;
+    ctx->st.n_contrib = head.n_contrib;
+    finish_stats(ctx);
+    return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_pose_loss(esacb200_ctx* ctx, int M, const double* poses6, const float* gt16, float wRot, float wTrans, float cut,
+                       double* out_losses, double* out_dloss6) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (!poses6 || !gt16 || !out_losses || !out_dloss6) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    if (M <= 0) return fail(ctx, ESACB200_ERR_ARG, "no poses (M=%d)", M);
+    begin_call(ctx);
+    float gt[16];
+    CK(cudaMemcpyAsync(gt, gt16, sizeof(gt), cudaMemcpyDefault, ctx->stream));
+    // [M] poses, [M] losses, [M,6] dLoss
+    CK(ctx->upstream.ensure((size_t)M * 13 * 8));
+    double* buf = ctx->upstream.as<double>();
+    CK(cudaMemcpyAsync(buf, poses6, (size_t)M * sizeof(Pose), cudaMemcpyDefault, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    launch_pose_loss((const Pose*)buf, M, gt, wRot, wTrans, cut, buf + 6 * (size_t)M, buf + 7 * (size_t)M, ctx->stream);
+    CK(cudaGetLastError());
+    ctx->st.kernel_launches += 1;
+    CK(cudaMemcpyAsync(out_losses, buf + 6 * (size_t)M, (size_t)M * 8, cudaMemcpyDefault, ctx->stream));
+    CK(cudaMemcpyAsync(out_dloss6, buf + 7 * (size_t)M, (size_t)M * 6 * 8, cudaMemcpyDefault, ctx->stream));
+    mark(ctx, EV_END);
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    finish_stats(ctx);
+    return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 
 int esacb200_backward_sharded(esacb200_ctx* ctx, const float* coords, float* grads, int E, int H, int W, const int64_t* assign,

@@ -313,4 +313,27 @@ size_t bwd_hypgrad_bytes();
 int bwd_red_vals();
 int bwd_tiles(int N);
 
+// State a hypotheses forward leaves for its backward, in one caller-owned device buffer (the tape):
+//   [TapeHead, kTapeHeadBytes] [M per-job records, bwd_hypgrad_bytes() each] [M jobs x 2 x ceil(N/32) words of inlier masks]
+// Job j's final inliers are mask (2j + its refinement buffer), the layout the refinement writes and B2-B5 read.
+struct TapeHead {
+    unsigned magic;
+    int n_contrib;  // written on the device by the forward
+    int M, mask_words;
+    Problem P;
+};
+constexpr unsigned kTapeMagic = 0x45534831u;  // "ESH1"
+constexpr size_t kTapeHeadBytes = 256;
+size_t tape_records_offset();
+size_t tape_masks_offset(int M);
+size_t tape_bytes(int M, int N);
+// records, header and per-hypothesis contributing flags [M] from a (init, ref, cells, rounds, contrib, n_contrib, assign32)
+void launch_tape_records(const BwdArgs& a, const TapeHead& head, void* tape, unsigned char* contrib_flags, cudaStream_t st);
+// the tape's records with dl = d_poses6[h], g = d_scores[h], p = 1 (device arrays of M), then B2-B5 into a.grads
+void launch_backward_upstream(const BwdArgs& a, const void* tape, const double* d_scores, const double* d_poses6, int max_jobs,
+                              int sm_count, cudaStream_t st);
+// loss / dLoss of M scene poses against a camera->world ground truth (one block)
+void launch_pose_loss(const Pose* poses, int M, const float gt[16], float wRot, float wTrans, float cut, double* losses,
+                      double* dloss6, cudaStream_t st);
+
 }  // namespace esacb200

@@ -20,6 +20,7 @@
 #ifndef ESAC_B200_H
 #define ESAC_B200_H
 
+#include <stddef.h>
 #include <stdint.h>
 
 #ifdef __cplusplus
@@ -74,6 +75,37 @@ int esacb200_backward(esacb200_ctx* ctx, const float* coords, float* grads, int 
                       float wLossTrans, float lossCut, int shiftX, int shiftY, float focalLength, float ppointX,
                       float ppointY, float inlierThreshold, float inlierAlpha, float inlierBeta, float maxReproj,
                       int subSampling, double* out_loss);
+
+/* The hypotheses of esac_backward as a differentiable function, for a pose loss of the caller's choice.
+ *
+ * esacb200_hypotheses_forward draws, scores and refines exactly what an esacb200_backward call at the same point of the
+ * context's call sequence would (same seed use), and writes
+ *   out_scores  double [M]    the soft-inlier scores the softmax sees,
+ *   out_poses6  double [M,6]  scene pose (rvec, tvec) per hypothesis: refined where p >= PROB_THRESH, initial elsewhere,
+ *   out_contrib uint8  [M]    1 where p >= PROB_THRESH (the hypotheses the backward differentiates);
+ * host or device pointers.  Everything its backward needs goes to `tape`: 16-byte aligned device memory of at least
+ * esacb200_hypotheses_tape_bytes(E, H, W, M) bytes, owned by the caller and untouched by any other call, so other library
+ * calls may run between a forward and its backward.  Returns 0 for non-positive or oversized arguments.
+ *
+ * esacb200_hypotheses_backward ACCUMULATES (+=) into grads float32 [E,3,H,W] the vector-Jacobian product
+ *   sum_h d_scores[h] * d score_h / d coords + d_poses6[h] . d pose_h / d coords
+ * over the contributing hypotheses (the reference's truncation; pose_h linearised through the refinement, both > 10 clamps
+ * kept).  d_scores double [M] and d_poses6 double [M,6] are host or device pointers; NULL counts as zero.  coords must hold
+ * the values the forward saw (host maps are staged again).  A tape may be used by any number of backwards. */
+size_t esacb200_hypotheses_tape_bytes(int E, int H, int W, int M);
+int esacb200_hypotheses_forward(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
+                                int64_t assign_stride, int M, int shiftX, int shiftY, float focalLength, float ppointX,
+                                float ppointY, float inlierThreshold, float inlierAlpha, float inlierBeta, float maxReproj,
+                                int subSampling, void* tape, size_t tape_bytes, double* out_scores, double* out_poses6,
+                                uint8_t* out_contrib);
+int esacb200_hypotheses_backward(esacb200_ctx* ctx, const void* tape, const float* coords, float* grads, int E, int H, int W,
+                                 const double* d_scores, const double* d_poses6);
+
+/* The reference's pose loss (esac_loss.h loss) and its dLoss, quirks included, of M scene poses (rvec, tvec) double [M,6]
+ * against a float32 [4,4] camera->world ground truth: out_losses double [M], out_dloss6 double [M,6].  Host or device
+ * pointers; the arithmetic is esacb200_backward's. */
+int esacb200_pose_loss(esacb200_ctx* ctx, int M, const double* poses6, const float* gt16, float wLossRot, float wLossTrans,
+                       float lossCut, double* out_losses, double* out_dloss6);
 
 /* ---- additive entry points ------------------------------------------------------------------ */
 /* esac_backward over hypotheses sharded across processes (one per GPU; experts expert-major, so gradient slices are

@@ -1,0 +1,322 @@
+"""The hypotheses node (autograd.esac_hypotheses, api.hypotheses_forward / hypotheses_backward / pose_loss) on the GPU:
+equivalence with esac.backward and the cv2 oracle under the reference loss, the reference loss entry point, the score path
+against a float64 restatement, linearity and masking of the vector-Jacobian product, tape independence, input kinds and
+streams, and the custom-loss training example (run with `-m gpu`)."""
+import numpy as np
+import pytest
+
+from esac_b200.synth import make_scene
+from oracle import esac_oracle as O
+from oracle.score_fp64 import pixel_centres, rodrigues
+
+pytestmark = pytest.mark.gpu
+
+# the scenes of test_backward_matches_oracle, and forced_scene's shape (E = 3, 48x64, M = 48, 90 % outliers)
+SCENES = [
+    (1, 1, 30, 40, 32, {}),
+    (2, 3, 30, 40, 48, {}),
+    (3, 2, 24, 31, 32, {"shiftX": 2, "shiftY": -3}),
+    (4, 2, 30, 40, 32, {"outlier_frac": 0.8}),
+    (5, 2, 29, 37, 32, {"sub": 3, "shiftX": -1, "shiftY": 2}),
+    (17, 3, 48, 64, 48, {"outlier_frac": 0.9}),
+]
+SCENE_IDS = ["s1", "s2", "s3", "s4", "s5", "forced"]
+# (wRot, wTrans, cut, cut active on some contributing hypothesis)
+LOSSES = [(1.0, 100.0, 0.05, True), (1.0, 100.0, 1e6, False), (1.0, 0.0, 1e6, False), (1.0, 0.0, 0.01, True)]
+
+
+def _scene(seed, E, H, W, M, kw):
+    return make_scene(E=E, H=H, W=W, M=M, seed=seed, **{"sub": 8, **kw})
+
+
+@pytest.fixture(scope="module")
+def api():
+    import esac_b200.api as api
+    api.context().set_option("fixed_seed", 1)
+    return api
+
+
+def _node(api, sc, seed, w, coords=None, assign=None):
+    """softmax(scores) . reference_pose_loss through the node: (loss, coordinate gradient, scores, poses, contributing)."""
+    import torch
+    from esac_b200.autograd import esac_hypotheses, reference_pose_loss
+    if coords is None:
+        coords = torch.from_numpy(sc.coords).cuda()
+    coords = coords.detach().requires_grad_(True)
+    if assign is None:
+        assign = torch.from_numpy(sc.assign).cuda()
+    api.set_seed(seed)
+    scores, poses, contrib = esac_hypotheses(coords, assign, *sc.params)
+    losses = reference_pose_loss(poses, torch.from_numpy(sc.gt_pose).to(poses.device), *w)
+    L = (torch.softmax(scores, 0) * losses).sum()
+    L.backward()
+    return L.item(), coords.grad.cpu().numpy(), scores.detach().cpu().numpy(), poses.detach().cpu().numpy(), \
+        contrib.cpu().numpy(), losses.detach().cpu().numpy()
+
+
+@pytest.mark.parametrize("w", LOSSES, ids=["cut_on", "cut_off", "rot_only", "rot_only_cut_on"])
+@pytest.mark.parametrize("seed,E,H,W,M,kw", SCENES, ids=SCENE_IDS)
+def test_reference_loss_through_the_node_is_esac_backward(api, seed, E, H, W, M, kw, w):
+    sc = _scene(seed, E, H, W, M, kw)
+    L, g, scores, poses, contrib, losses = _node(api, sc, 50 + seed, w[:3])
+    api.set_seed(50 + seed)
+    g_ref = np.zeros_like(sc.coords)
+    l_ref = api.backward(sc.coords, g_ref, sc.assign, sc.gt_pose, *w[:3], *sc.params)
+    hy = api.last_hypotheses(losses=True)
+    st = api.last_stats()
+    assert int(contrib.sum()) == st["n_contrib"] and st["n_contrib"] >= 1
+    assert np.array_equal(contrib, hy["probs"] >= O.PROB_THRESH)
+    assert np.array_equal(poses, hy["refined"])
+    assert np.array_equal(scores, hy["scores"])
+    assert np.array_equal(losses, hy["losses"])
+    assert bool((losses[contrib] > w[2]).any()) == w[3]
+    assert abs(L - l_ref) <= 1e-12 * abs(l_ref), (L, l_ref)
+    scale = np.abs(g_ref).max()
+    assert scale > 0
+    assert np.abs(g - g_ref).max() <= 1e-6 * scale, (np.abs(g - g_ref).max(), scale)
+
+
+@pytest.mark.parametrize("seed,E,H,W,M,kw", SCENES[:5], ids=SCENE_IDS[:5])
+def test_reference_loss_through_the_node_meets_the_oracle(api, seed, E, H, W, M, kw):
+    sc = _scene(seed, E, H, W, M, kw)
+    g_ref = np.zeros_like(sc.coords)
+    l_ref = O.backward(sc.coords, g_ref, sc.assign, sc.gt_pose, 1.0, 100.0, 100.0, *sc.params, seed=50 + seed)
+    L, g, *_ = _node(api, sc, 50 + seed, (1.0, 100.0, 100.0))
+    assert abs(L - l_ref) < 1e-6 * max(1.0, abs(l_ref))
+    scale = max(np.abs(g_ref).max(), 1e-12)
+    assert np.abs(g - g_ref).max() / scale < 1e-3, (np.abs(g - g_ref).max(), scale)
+
+
+def test_reference_pose_loss_entry_point_is_the_oracles_loss_and_dloss(api):
+    import torch
+    from esac_b200.autograd import reference_pose_loss
+    sc = make_scene(E=1, H=24, W=32, M=8, seed=21)
+    gt64 = sc.gt_pose.astype(np.float64)
+    gt_r, gt_t = O.trans2pose(gt64)
+    rng = np.random.default_rng(3)
+    rows = []
+    for k in range(40):  # 2 to 60 degrees and 1 cm to 3 m away from the ground truth
+        ax = rng.normal(size=3)
+        dr = ax / np.linalg.norm(ax) * np.radians(rng.uniform(2, 60))
+        rows.append(np.r_[gt_r.ravel() + dr, gt_t.ravel() + rng.normal(size=3) * 10 ** rng.uniform(-2, 0.5)])
+    poses = torch.tensor(np.array(rows), dtype=torch.float64, device="cuda", requires_grad=True)
+    for w_rot, w_trans in ((1.0, 100.0), (1.0, 0.0)):
+        l_ref = np.array([O.loss(O.pose2trans(p[:3], p[3:]), gt64, w_rot, w_trans, 1e9) for p in rows])
+        cut = float(np.float32(np.median(l_ref)))  # half of the poses above the cut; float32, as the loss takes it
+        losses = reference_pose_loss(poses, torch.from_numpy(sc.gt_pose).cuda(), w_rot, w_trans, cut)
+        up = torch.linspace(0.5, 2.0, len(rows), dtype=torch.float64, device="cuda")
+        g, = torch.autograd.grad((losses * up).sum(), poses)
+        lo, g = losses.detach().cpu().numpy(), g.cpu().numpy() / up.cpu().numpy()[:, None]
+        above = 0
+        for i, p in enumerate(rows):
+            T = O.pose2trans(p[:3], p[3:])
+            lr = O.loss(T, gt64, w_rot, w_trans, cut)
+            above += lr > cut
+            dl = O.d_loss(p[:3], p[3:], gt_r, gt_t, w_rot, w_trans, cut).ravel()
+            assert abs(lo[i] - lr) <= 1e-11 * max(1.0, abs(lr)), (i, lo[i], lr)
+            assert np.abs(g[i] - dl).max() <= 1e-9 * max(1.0, np.abs(dl).max()), (i, g[i], dl)
+        assert 0 < above < len(rows)
+
+
+def _score_vjp_fp64(sc, init_poses, upstream):
+    """torch autograd of sum_h upstream[h] * score_h in float64 at the given poses (oracle/score_fp64.py's operation)."""
+    import torch
+    X = torch.tensor(sc.coords.astype(np.float64), requires_grad=True)
+    E, _, H, W = sc.coords.shape
+    px, py = (torch.tensor(a) for a in pixel_centres(H, W, sc.sub, sc.shiftX, sc.shiftY))
+    total = 0
+    for h in np.nonzero(upstream)[0]:
+        R = torch.tensor(rodrigues(init_poses[h, :3])[0])
+        t = torch.tensor(init_poses[h, 3:])
+        cam = torch.einsum("ij,jhw->ihw", R, X[sc.assign[h]]) + t[:, None, None]
+        u = cam[0] / cam[2] * sc.f + sc.ppx
+        v = cam[1] / cam[2] * sc.f + sc.ppy
+        err = torch.clamp(torch.hypot(u - px, v - py), max=sc.max_reproj)
+        w = 1 - torch.sigmoid(sc.beta * (err - sc.tau))
+        total = total + float(upstream[h]) * sc.alpha / (H * W) * w.sum()
+    total.backward()
+    return X.grad.numpy()
+
+
+def test_score_upstream_matches_a_float64_restatement_outside_the_minimal_sets(api):
+    import torch
+    sc = make_scene(E=3, H=48, W=64, M=48, sub=8, seed=17, outlier_frac=0.9)
+    api.set_seed(57)
+    scores, poses, contrib, tape = api.hypotheses_forward(torch.from_numpy(sc.coords).cuda(), sc.assign, *sc.params)
+    hy = api.last_hypotheses()
+    contrib = contrib.cpu().numpy()
+    assert contrib.sum() >= 8
+    assert np.array_equal(poses.cpu().numpy()[~contrib], hy["poses"][~contrib])  # initial poses where nothing is refined
+    up = np.where(contrib, np.random.default_rng(4).normal(size=sc.assign.shape[0]), 0.0)
+    g = torch.zeros(sc.coords.shape, device="cuda")
+    api.hypotheses_backward(tape, torch.from_numpy(sc.coords).cuda(), g, torch.tensor(up, device="cuda"), None)
+    g = g.cpu().numpy()
+    ref = _score_vjp_fp64(sc, hy["poses"], up)
+    keep = np.ones(sc.coords.shape, bool)
+    for h in np.nonzero(contrib)[0]:
+        for x, y in hy["cells"][h]:
+            keep[sc.assign[h], :, y, x] = False
+    scale = np.abs(ref[keep]).max()
+    assert scale > 0
+    assert np.abs(g[keep] - ref[keep]).max() <= 1e-4 * scale, (np.abs(g[keep] - ref[keep]).max(), scale)
+
+
+@pytest.fixture(scope="module")
+def forced(api):
+    """The forced scene's forward: (scene, CUDA coordinates, tape, contributing flags, assignment)."""
+    import torch
+    sc = make_scene(E=3, H=48, W=64, M=48, sub=8, seed=17, outlier_frac=0.9)
+    coords = torch.from_numpy(sc.coords).cuda()
+    api.set_seed(57)
+    _, _, contrib, tape = api.hypotheses_forward(coords, sc.assign, *sc.params)
+    return sc, coords, tape, contrib.cpu().numpy()
+
+
+def _vjp(api, forced, a=None, b=None, start=None):
+    import torch
+    sc, coords, tape, _ = forced
+    g = torch.zeros(sc.coords.shape, device="cuda") if start is None else torch.from_numpy(start.copy()).cuda()
+    api.hypotheses_backward(tape, coords, g, None if b is None else torch.tensor(b, device="cuda"),
+                            None if a is None else torch.tensor(a, device="cuda"))
+    return g.cpu().numpy()
+
+
+def test_vjp_is_linear_and_ignores_non_contributing_hypotheses(api, forced):
+    sc, _, _, contrib = forced
+    M = sc.assign.shape[0]
+    rng = np.random.default_rng(8)
+    a1, a2 = rng.normal(size=(M, 6)) * 1e-2, rng.normal(size=(M, 6)) * 1e-2
+    b1, b2 = rng.normal(size=M), rng.normal(size=M)
+    g1, g2, g12 = _vjp(api, forced, a1, b1), _vjp(api, forced, a2, b2), _vjp(api, forced, a1 + a2, b1 + b2)
+    scale = np.abs(g12).max()
+    assert scale > 0
+    assert np.abs(g12 - (g1 + g2)).max() <= 1e-5 * scale
+    # random upstream on the hypotheses that do not contribute changes nothing
+    a3, b3 = a1.copy(), b1.copy()
+    a3[~contrib] = rng.normal(size=(int((~contrib).sum()), 6)) * 1e3
+    b3[~contrib] = rng.normal(size=int((~contrib).sum())) * 1e3
+    assert np.array_equal(_vjp(api, forced, a3, b3), g1)
+
+
+def test_zero_upstream_adds_exactly_zero(api, forced):
+    sc, _, _, _ = forced
+    M = sc.assign.shape[0]
+    start = np.random.default_rng(9).normal(size=sc.coords.shape).astype(np.float32)
+    assert np.array_equal(_vjp(api, forced, np.zeros((M, 6)), np.zeros(M), start=start), start)
+    assert np.array_equal(_vjp(api, forced, None, None, start=start), start)
+
+
+def test_a_hypothesis_upstream_reaches_only_its_experts_plane(api, forced):
+    sc, _, _, contrib = forced
+    M = sc.assign.shape[0]
+    for h in np.nonzero(contrib)[0][:4]:
+        a, b = np.zeros((M, 6)), np.zeros(M)
+        a[h], b[h] = 1e-2, 1.0
+        g = _vjp(api, forced, a, b)
+        e = sc.assign[h]
+        assert np.abs(g[e]).max() > 0
+        assert not np.any(np.delete(g, e, axis=0))
+
+
+def test_tapes_are_independent_of_later_calls(api):
+    import torch
+    scenes = [make_scene(E=3, H=48, W=64, M=48, sub=8, seed=17, outlier_frac=0.9), make_scene(E=2, H=30, W=40, M=32, seed=4)]
+    rng = np.random.default_rng(12)
+    ups = [(rng.normal(size=(s.assign.shape[0], 6)) * 1e-2, rng.normal(size=s.assign.shape[0])) for s in scenes]
+
+    def fwd(i):
+        s = scenes[i]
+        api.set_seed(60 + i)
+        return api.hypotheses_forward(torch.from_numpy(s.coords).cuda(), s.assign, *s.params)
+
+    def bwd(i, tape):
+        s = scenes[i]
+        g = torch.zeros(s.coords.shape, device="cuda")
+        api.hypotheses_backward(tape, torch.from_numpy(s.coords).cuda(), g, torch.tensor(ups[i][1], device="cuda"),
+                                torch.tensor(ups[i][0], device="cuda"))
+        return g.cpu().numpy()
+
+    alone = []
+    for i in range(2):
+        out = fwd(i)
+        alone.append((out[0].cpu().numpy(), out[1].cpu().numpy(), bwd(i, out[3])))
+    out0, out1 = fwd(0), fwd(1)
+    g1, g0 = bwd(1, out1[3]), bwd(0, out0[3])     # backwards in reverse order, after both forwards
+    assert np.array_equal(g0, alone[0][2]) and np.array_equal(g1, alone[1][2])
+    assert np.array_equal(out0[1].cpu().numpy(), alone[0][1]) and np.array_equal(out1[1].cpu().numpy(), alone[1][1])
+    assert np.abs(g0).max() > 0 and np.abs(g1).max() > 0
+
+
+def test_retain_graph_and_memory(api):
+    import torch
+    from esac_b200.autograd import esac_hypotheses, pose_to_transform
+    sc = make_scene(E=3, H=48, W=64, M=48, sub=8, seed=17, outlier_frac=0.9)
+
+    def step():
+        coords = torch.from_numpy(sc.coords).cuda().requires_grad_(True)
+        api.set_seed(57)
+        scores, poses, contrib = esac_hypotheses(coords, torch.from_numpy(sc.assign).cuda(), *sc.params)
+        gt = torch.from_numpy(sc.gt_pose).cuda().double()
+        T = pose_to_transform(poses)
+        L = (torch.softmax(scores, 0) * (T[:, :3, 3] - gt[:3, 3]).norm(dim=1)).sum()
+        g1, = torch.autograd.grad(L, coords, retain_graph=True)
+        g2, = torch.autograd.grad(L, coords)
+        assert torch.equal(g1, g2) and g1.abs().max() > 0
+
+    step()  # first use of the batched matmul allocates torch's persistent library workspaces
+    torch.cuda.synchronize()
+    base = torch.cuda.memory_allocated()
+    step()
+    torch.cuda.synchronize()
+    assert torch.cuda.memory_allocated() == base
+
+
+def test_cpu_cuda_and_misaligned_inputs_give_the_same_bits_and_calls_follow_the_stream(api):
+    import torch
+    from esac_b200.autograd import esac_hypotheses
+    sc = make_scene(E=3, H=48, W=64, M=48, sub=8, seed=17, outlier_frac=0.9)
+    M = sc.assign.shape[0]
+    rng = np.random.default_rng(13)
+    a, b = torch.tensor(rng.normal(size=(M, 6)) * 1e-2), torch.tensor(rng.normal(size=M))
+
+    def run(coords, assign):
+        coords = coords.detach().requires_grad_(True)
+        api.set_seed(57)
+        scores, poses, contrib = esac_hypotheses(coords, assign, *sc.params)
+        g, = torch.autograd.grad((scores, poses), coords, (b.to(scores.device), a.to(poses.device)))
+        return [x.detach().cpu().numpy() for x in (scores, poses, contrib, g)]
+
+    buf = torch.zeros(sc.coords.size + 1, device="cuda")
+    misaligned = buf[1:].view(sc.coords.shape)
+    misaligned.copy_(torch.from_numpy(sc.coords))
+    assert misaligned.data_ptr() % 16 == 4
+    assign = torch.from_numpy(sc.assign)
+    runs = [run(torch.from_numpy(sc.coords), assign), run(torch.from_numpy(sc.coords).cuda(), assign.cuda()),
+            run(misaligned, assign.cuda())]
+    s = torch.cuda.Stream()
+    with torch.cuda.stream(s):
+        # the coordinates are produced on the side stream right before the call: the node must run after them
+        slow = torch.zeros(sc.coords.shape, device="cuda")
+        for _ in range(50):
+            slow = slow * 1.0001
+        coords = slow * 0 + torch.from_numpy(sc.coords).cuda()
+        runs.append(run(coords, assign.cuda()))
+    s.synchronize()
+    assert np.abs(runs[0][3]).max() > 0
+    for r in runs[1:]:
+        for x, y in zip(r, runs[0]):
+            assert np.array_equal(x, y)
+
+
+def test_custom_loss_example_checks_against_esac_loss():
+    import runpy
+    import sys
+    from pathlib import Path
+    ex = Path(__file__).resolve().parents[1] / "examples" / "custom_loss_step_synthetic.py"
+    argv = sys.argv
+    sys.argv = [str(ex), "--steps", "3", "--check"]
+    try:
+        mod = runpy.run_path(str(ex), run_name="example")
+        assert mod["main"]() == 0
+    finally:
+        sys.argv = argv

@@ -125,6 +125,12 @@ def load_library() -> C.CDLL:
     lib.esacb200_hypotheses_backward.restype = i32
     lib.esacb200_pose_loss.argtypes = [vp, i32, vp, vp, f32, f32, f32, vp, vp]
     lib.esacb200_pose_loss.restype = i32
+    lib.esacb200_pose_loss_batch.argtypes = [vp, i32, i32, vp, vp, f32, f32, f32, vp, vp]
+    lib.esacb200_pose_loss_batch.restype = i32
+    lib.esacb200_hypotheses_forward_ragged.argtypes = [vp, i32, vp, vp, vp, i32, vp, i64, i32] + cams + [vp, vp, vp, vp, vp]
+    lib.esacb200_hypotheses_forward_ragged.restype = i32
+    lib.esacb200_hypotheses_backward_ragged.argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, vp, vp]
+    lib.esacb200_hypotheses_backward_ragged.restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
         getattr(lib, "esacb200_" + name).restype = i32
@@ -1104,26 +1110,148 @@ def hypotheses_backward(tape, sceneCoordinates, outGradients, gradScores=None, g
     gr.finish()
 
 
+class _Maps:
+    """An image-sized argument of the batched hypotheses node: a [B,E,3,H,W] tensor or a list / tuple of B [E,3,H_b,W_b]
+    tensors, as a host array of B pointers with the heights and widths.  Raises RuntimeError before any context exists."""
+
+    def __init__(self, t, what: str, writable: bool = False, B: int | None = None):
+        self.ragged = _is_list(t)
+        if self.ragged:
+            self.shapes = _check_list(t, 4, what, B)
+            self.args = [_Arg(x, writable=writable) for x in t]
+            ptrs = [a.ptr for a in self.args]
+        else:
+            _check(t, "Float", 5, what)
+            n, *s = (int(v) for v in t.shape)
+            if n < 1 or (B is not None and n != B):
+                raise RuntimeError(f"{what} holds {n} images" + (f" for {B}" if B is not None else ""))
+            self.shapes = [tuple(s)] * n
+            self.args = [_Arg(t, writable=writable)]
+            step = 4 * s[0] * s[1] * s[2] * s[3]
+            ptrs = [self.args[0].ptr + b * step for b in range(n)]
+        self.E = _check_maps(self.shapes, what)
+        self.B = len(self.shapes)
+        self.ptrs = (C.c_void_p * self.B)(*ptrs)
+        self.hs, self.ws = _dims(self.shapes, 2), _dims(self.shapes, 3)
+        self.devices = [a.device for a in self.args]
+
+    def finish(self):
+        for a in self.args:
+            a.finish()
+
+
+def _tape_hypotheses(tape, E: int, H: int, W: int, what: str) -> int:
+    """The number of hypotheses a tape of this size holds for [E,3,H,W] maps (tape_bytes is affine in M)."""
+    if not (_is_torch(tape) and tape.is_cuda and str(tape.dtype) == "torch.uint8" and tape.dim() == 1 and tape.is_contiguous()):
+        raise RuntimeError(f"{what} must be a contiguous CUDA uint8 tensor hypotheses_forward_batch returned")
+    one = hypotheses_tape_bytes(E, H, W, 1)
+    per = hypotheses_tape_bytes(E, H, W, 2) - one
+    n = int(tape.numel()) - (one - per)
+    if n < per or n % per:
+        raise RuntimeError(f"{what} is not the tape of a forward on [{E}, 3, {H}, {W}] maps")
+    return n // per
+
+
+def hypotheses_forward_batch(sceneCoordinates, hypAssignment, shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
+                             inlierAlpha, inlierBeta, maxReproj, subSampling):
+    """hypotheses_forward over a batch: image b draws, scores and refines what the b-th of B consecutive hypotheses_forward
+    (or esac.backward) calls would, with its own shift and camera.  sceneCoordinates [B,E,3,H,W] float32 or a list / tuple of
+    B [E,3,H_b,W_b] tensors; hypAssignment int64 [B,M] (a stride-0 [B,1].expand(B,M) included); shiftX, shiftY,
+    focalLength, ppointX, ppointY each a number or B values.  Returns scores float64 [B,M], poses float64 [B,M,6],
+    contributing bool [B,M] on the coordinates' device (CPU for numpy input), and the B tapes: views into one CUDA uint8
+    tensor, each at a 256-byte aligned offset.  The images run on worker streams (option batch_workers) after everything
+    queued on torch's current stream."""
+    maps = _Maps(sceneCoordinates, "sceneCoordinates")
+    B, E = maps.B, maps.E
+    _check(hypAssignment, "Long", 2, "hypAssignment")
+    if int(hypAssignment.shape[0]) != B:
+        raise RuntimeError(f"hypAssignment must be [{B}, M] for {B} images, got {list(hypAssignment.shape)}")
+    M = int(hypAssignment.shape[1])
+    if M < 1:
+        raise RuntimeError("hypAssignment holds no hypothesis")
+    sx, sy = _per_image(shiftX, B, np.int32, "shiftX"), _per_image(shiftY, B, np.int32, "shiftY")
+    fs = _per_image(focalLength, B, np.float32, "focalLength")
+    cx, cy = _per_image(ppointX, B, np.float32, "ppointX"), _per_image(ppointY, B, np.float32, "ppointY")
+    import torch
+    ha = _Arg(hypAssignment)
+    ctx = _pick_ctx(*maps.devices, ha.device)
+    if all(d is None for d in maps.devices) and ha.device is None:  # the tapes are CUDA tensors: follow torch's stream
+        ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
+    dev = _out_device(maps.args[0])
+    sizes = [hypotheses_tape_bytes(E, h, w, M) for h, w in zip(maps.hs, maps.ws)]
+    offsets = np.cumsum([0] + [(n + 255) // 256 * 256 for n in sizes])
+    buf = torch.empty(int(offsets[-1]), dtype=torch.uint8, device=torch.device("cuda", ctx.device))
+    tapes = [buf[int(o):int(o) + n] for o, n in zip(offsets, sizes)]
+    scores = torch.empty(B, M, dtype=torch.float64, device=dev)
+    poses = torch.empty(B, M, 6, dtype=torch.float64, device=dev)
+    contributing = torch.empty(B, M, dtype=torch.bool, device=dev)
+    tape_ptrs = (C.c_void_p * B)(*[t.data_ptr() for t in tapes])
+    tape_sizes = (C.c_size_t * B)(*sizes)
+    ctx.check(ctx.lib.esacb200_hypotheses_forward_ragged(
+        ctx.handle, B, maps.ptrs, maps.hs.ctypes.data, maps.ws.ctypes.data, E, ha.ptr, 1, M, sx.ctypes.data, sy.ctypes.data,
+        fs.ctypes.data, cx.ctypes.data, cy.ctypes.data, float(inlierThreshold), float(inlierAlpha), float(inlierBeta),
+        float(maxReproj), int(subSampling), tape_ptrs, tape_sizes, scores.data_ptr(), poses.data_ptr(), contributing.data_ptr()))
+    return scores, poses, contributing, tapes
+
+
+def hypotheses_backward_batch(tapes, sceneCoordinates, outGradients, gradScores=None, gradPoses=None):
+    """hypotheses_backward over a batch: accumulates (+=) into outGradients[b] what hypotheses_backward on tapes[b] with
+    gradScores[b] / gradPoses[b] would add.  sceneCoordinates / outGradients [B,E,3,H,W] float32 or lists / tuples of B
+    [E,3,H_b,W_b] tensors of the forward's shapes; gradScores float64 [B,M] and gradPoses float64 [B,M,6], None = zero."""
+    maps = _Maps(sceneCoordinates, "sceneCoordinates")
+    B, E = maps.B, maps.E
+    if _is_list(outGradients) != maps.ragged:
+        raise RuntimeError("outGradients must be of sceneCoordinates' kind: one [B,E,3,H,W] tensor or a list of B maps")
+    grads = _Maps(outGradients, "outGradients", writable=True, B=B)
+    if grads.shapes != maps.shapes:
+        raise RuntimeError(f"outGradients are {[list(s) for s in grads.shapes]}, sceneCoordinates {[list(s) for s in maps.shapes]}")
+    if not (_is_list(tapes) and len(tapes) == B):
+        raise RuntimeError(f"tapes must be the list of {B} tapes hypotheses_forward_batch returned")
+    Ms = {_tape_hypotheses(t, E, int(h), int(w), f"tapes[{b}]") for b, (t, h, w) in enumerate(zip(tapes, maps.hs, maps.ws))}
+    if len(Ms) > 1:
+        raise RuntimeError(f"the tapes hold different numbers of hypotheses {sorted(Ms)}")
+    M = Ms.pop()
+    if gradScores is not None:
+        _check(gradScores, "Double", 2, "gradScores")
+        if tuple(int(s) for s in gradScores.shape) != (B, M):
+            raise RuntimeError(f"gradScores must be [{B}, {M}], got {list(gradScores.shape)}")
+    if gradPoses is not None:
+        _check(gradPoses, "Double", 3, "gradPoses")
+        if tuple(int(s) for s in gradPoses.shape) != (B, M, 6):
+            raise RuntimeError(f"gradPoses must be [{B}, {M}, 6], got {list(gradPoses.shape)}")
+    gs = _Arg(gradScores) if gradScores is not None else None
+    gp = _Arg(gradPoses) if gradPoses is not None else None
+    ctx = _pick_ctx(*maps.devices, *grads.devices, *(t.device.index for t in tapes), gs.device if gs else None,
+                    gp.device if gp else None)
+    tape_ptrs = (C.c_void_p * B)(*[t.data_ptr() for t in tapes])
+    ctx.check(ctx.lib.esacb200_hypotheses_backward_ragged(ctx.handle, B, tape_ptrs, maps.ptrs, grads.ptrs, maps.hs.ctypes.data,
+                                                          maps.ws.ctypes.data, E, gs.ptr if gs else None, gp.ptr if gp else None))
+    grads.finish()
+
+
 def pose_loss(poses, gtPose, wLossRot, wLossTrans, lossCut):
     """The reference's loss (esac_loss.h) of scene poses float64 [M,6] = (rvec, tvec) against a float32 [4,4] camera->world
     ground truth, and its dLoss, quirks included, with esac.backward's arithmetic.  Returns torch tensors (losses float64
-    [M], dloss float64 [M,6]) on the poses' device (CPU for numpy input)."""
-    _check(poses, "Double", 2, "poses")
-    _check(gtPose, "Float", 2, "gtPose")
-    if int(poses.shape[1]) != 6 or int(poses.shape[0]) < 1:
-        raise RuntimeError(f"poses must be [M, 6] with M >= 1, got {list(poses.shape)}")
-    if tuple(int(s) for s in gtPose.shape) != (4, 4):
-        raise RuntimeError("gtPose must be [4, 4]")
+    [M], dloss float64 [M,6]) on the poses' device (CPU for numpy input).  A batch, poses [B,M,6] against ground truths
+    [B,4,4], gives losses [B,M] and dloss [B,M,6] in one launch, row b bitwise what [M,6] against gtPose[b] gives."""
+    batch = (poses.dim() if _is_torch(poses) else np.ndim(poses)) == 3
+    _check(poses, "Double", 3 if batch else 2, "poses")
+    _check(gtPose, "Float", 3 if batch else 2, "gtPose")
+    lead = tuple(int(s) for s in poses.shape[:-2]) if batch else ()
+    if int(poses.shape[-1]) != 6 or int(poses.shape[-2]) < 1 or (batch and lead[0] < 1):
+        raise RuntimeError(f"poses must be {'[B, M, 6] with B, M' if batch else '[M, 6] with M'} >= 1, got {list(poses.shape)}")
+    if tuple(int(s) for s in gtPose.shape) != lead + (4, 4):
+        raise RuntimeError(f"gtPose must be [{lead[0]}, 4, 4] for [B, M, 6] poses" if batch else "gtPose must be [4, 4]")
     import torch
     po = _Arg(poses)
     gt = _Arg(gtPose)
     ctx = _pick_ctx(po.device, gt.device)
-    M = int(poses.shape[0])
+    B, M = (lead[0] if batch else 1), int(poses.shape[-2])
     dev = _out_device(po)
-    losses = torch.empty(M, dtype=torch.float64, device=dev)
-    dloss = torch.empty(M, 6, dtype=torch.float64, device=dev)
-    ctx.check(ctx.lib.esacb200_pose_loss(ctx.handle, M, po.ptr, gt.ptr, float(wLossRot), float(wLossTrans), float(lossCut),
-                                         losses.data_ptr(), dloss.data_ptr()))
+    losses = torch.empty(lead + (M,), dtype=torch.float64, device=dev)
+    dloss = torch.empty(lead + (M, 6), dtype=torch.float64, device=dev)
+    ctx.check(ctx.lib.esacb200_pose_loss_batch(ctx.handle, B, M, po.ptr, gt.ptr, float(wLossRot), float(wLossTrans),
+                                               float(lossCut), losses.data_ptr(), dloss.data_ptr()))
     return losses, dloss
 
 

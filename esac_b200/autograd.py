@@ -278,6 +278,69 @@ def esac_hypotheses(scene_coordinates, hyp_assignment, shift_x, shift_y, focal_l
                                 inlier_threshold, inlier_alpha, inlier_beta, max_reproj, sub_sampling)
 
 
+class EsacHypothesesBatch(torch.autograd.Function):
+    """EsacHypotheses over a batch of images of one shape (api.hypotheses_forward_batch on [B,E,3,H,W] maps)."""
+
+    @staticmethod
+    def forward(ctx, scene_coordinates, hyp_assignment, *params):
+        scores, poses, contributing, tapes = api.hypotheses_forward_batch(scene_coordinates.detach(), hyp_assignment, *params)
+        ctx.save_for_backward(scene_coordinates, *tapes)
+        ctx.mark_non_differentiable(contributing)
+        ctx.set_materialize_grads(False)
+        ctx.n_params = len(params)
+        return scores, poses, contributing
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_scores, grad_poses, _grad_contributing):
+        coords, *tapes = ctx.saved_tensors
+        grads = torch.zeros_like(coords)
+        api.hypotheses_backward_batch(tapes, coords, grads, grad_scores, grad_poses)
+        return (grads, None) + (None,) * ctx.n_params
+
+
+class EsacHypothesesRagged(torch.autograd.Function):
+    """EsacHypothesesBatch on a list of B maps [E,3,H_b,W_b].  The maps come last so that autograd sees every one of them;
+    `meta` holds the non-differentiable arguments."""
+
+    @staticmethod
+    def forward(ctx, meta, *scene_coordinates):
+        hyp_assignment, params = meta
+        scores, poses, contributing, tapes = api.hypotheses_forward_batch([c.detach() for c in scene_coordinates],
+                                                                          hyp_assignment, *params)
+        ctx.save_for_backward(*scene_coordinates, *tapes)
+        ctx.mark_non_differentiable(contributing)
+        ctx.set_materialize_grads(False)
+        ctx.B = len(scene_coordinates)
+        return scores, poses, contributing
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_scores, grad_poses, _grad_contributing):
+        saved = ctx.saved_tensors
+        coords, tapes = list(saved[:ctx.B]), list(saved[ctx.B:])
+        grads = [torch.zeros_like(c) for c in coords]
+        api.hypotheses_backward_batch(tapes, coords, grads, grad_scores, grad_poses)
+        return (None,) + tuple(grads)
+
+
+def esac_hypotheses_batch(scene_coordinates, hyp_assignment, shift_x, shift_y, focal_length, ppoint_x, ppoint_y,
+                          inlier_threshold, inlier_alpha, inlier_beta, max_reproj, sub_sampling):
+    """esac_hypotheses over a batch of images, each with its own shift and camera: scene_coordinates [B,E,3,H,W] float32 or
+    a list / tuple of B [E,3,H_b,W_b] tensors of different sizes (every element then receives its own gradient),
+    hyp_assignment [B,M] int64; shift_x, shift_y, focal_length, ppoint_x, ppoint_y a number or B values.  Returns scores
+    float64 [B,M], poses float64 [B,M,6] and contributing bool [B,M]; row b is what the b-th of B consecutive esac_hypotheses
+    calls would return, and the backward gives each image the gradient esac_hypotheses would.  The images run on the worker
+    streams of api.backward_batch.  With
+        L = (softmax(scores, 1) * reference_pose_loss(poses, gt_poses, w_rot, w_trans, cut)).sum(1)
+    L and its gradient are those of esac_loss_batch."""
+    params = (shift_x, shift_y, focal_length, ppoint_x, ppoint_y, inlier_threshold, inlier_alpha, inlier_beta, max_reproj,
+              sub_sampling)
+    if isinstance(scene_coordinates, (list, tuple)):
+        return EsacHypothesesRagged.apply((hyp_assignment, params), *scene_coordinates)
+    return EsacHypothesesBatch.apply(scene_coordinates, hyp_assignment, *params)
+
+
 class ReferencePoseLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, poses, gt_pose, w_rot, w_trans, cut):
@@ -289,7 +352,7 @@ class ReferencePoseLoss(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_losses):
         (dloss,) = ctx.saved_tensors
-        return grad_losses.to(dloss.device)[:, None] * dloss, None, None, None, None
+        return grad_losses.to(dloss.device)[..., None] * dloss, None, None, None, None
 
 
 def reference_pose_loss(poses, gt_pose, w_rot, w_trans, cut):
@@ -297,7 +360,8 @@ def reference_pose_loss(poses, gt_pose, w_rot, w_trans, cut):
     camera->world ground truth: wRot * angle(deg) + wTrans * |t_est - t_gt|, above `cut` sqrt(cut * l), at most 1e7.
     Its gradient is the reference's dLoss, bug for bug: above the cut it is scaled as the derivative of sqrt(l) (not of
     sqrt(cut * l)), the angle uses CV_PI where the loss uses 3.1415926, and it is zero on NaN, on errors below 1e-8 and at
-    the 1e7 cap.  Both come from the device functions esac.backward uses.  Returns float64 [M]."""
+    the 1e7 cap.  Both come from the device functions esac.backward uses.  Returns float64 [M].  Poses [B,M,6] against
+    ground truths [B,4,4] give [B,M] in one launch, row b bitwise what [M,6] against gt_pose[b] gives."""
     return ReferencePoseLoss.apply(poses, gt_pose, w_rot, w_trans, cut)
 
 

@@ -477,29 +477,28 @@ __global__ void __launch_bounds__(1024) bwd_upstream_kernel(const __grid_constan
     }
 }
 
-// The reference's loss and dLoss of M scene poses against one ground truth (esacb200_pose_loss): the device functions of B1.
-struct Gt16 {
-    float v[16];
-};
-__global__ void __launch_bounds__(256) pose_loss_kernel(const Pose* poses, int M, const Gt16 gt, float wRot, float wTrans,
+// The reference's loss and dLoss of B x M scene poses, image b against its own ground truth (esacb200_pose_loss_batch): the
+// device functions of B1.  CTA (x, b) handles poses [256x, 256x + 256) of image b and reads that image's ground truth from
+// device memory, so no host round trip precedes the launch.  256 threads: at 1024 pose_dloss spills.
+__global__ void __launch_bounds__(256) pose_loss_kernel(const Pose* poses, int M, const float* gt16, float wRot, float wTrans,
                                                          float cut, double* losses, double* dloss6) {
     __shared__ Pose gtp;
     __shared__ double gtT[16];
-    if (threadIdx.x == 0) gt_trans2pose(gt.v, gtp, gtT);
+    const int b = blockIdx.y;
+    if (threadIdx.x == 0) gt_trans2pose(gt16 + (size_t)b * 16, gtp, gtT);
     __syncthreads();
-    for (int h = threadIdx.x; h < M; h += blockDim.x) {
-        double T[16];
-        pose2trans(poses[h], T);
-        losses[h] = pose_loss(T, gtT, (double)wRot, (double)wTrans, (double)cut);
-        pose_dloss(poses[h], gtp, (double)wRot, (double)wTrans, (double)cut, dloss6 + (size_t)h * 6);
-    }
+    const int h = blockIdx.x * blockDim.x + threadIdx.x;
+    if (h >= M) return;
+    const size_t i = (size_t)b * M + h;
+    double T[16];
+    pose2trans(poses[i], T);
+    losses[i] = pose_loss(T, gtT, (double)wRot, (double)wTrans, (double)cut);
+    pose_dloss(poses[i], gtp, (double)wRot, (double)wTrans, (double)cut, dloss6 + i * 6);
 }
 
-void launch_pose_loss(const Pose* poses, int M, const float gt[16], float wRot, float wTrans, float cut, double* losses,
+void launch_pose_loss(const Pose* poses, int B, int M, const float* gt16, float wRot, float wTrans, float cut, double* losses,
                       double* dloss6, cudaStream_t st) {
-    Gt16 g;
-    for (int i = 0; i < 16; ++i) g.v[i] = gt[i];
-    pose_loss_kernel<<<1, 256, 0, st>>>(poses, M, g, wRot, wTrans, cut, losses, dloss6);
+    pose_loss_kernel<<<dim3((M + 255) / 256, B), 256, 0, st>>>(poses, M, gt16, wRot, wTrans, cut, losses, dloss6);
 }
 
 static BwdAux bwd_aux(const BwdArgs& a) {

@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <exception>
+#include <functional>
 #include <new>
 #include <string>
 #include <vector>
@@ -1492,10 +1493,10 @@ size_t esacb200_hypotheses_tape_bytes(int E, int H, int W, int M) {
     return tape_bytes(M, H * W);
 }
 
-int esacb200_hypotheses_forward(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
-                                int64_t assign_stride, int M, int shiftX, int shiftY, float f, float ppx, float ppy, float tau,
-                                float alpha, float beta, float maxReproj, int sub, void* tape, size_t tape_bytes_,
-                                double* out_scores, double* out_poses6, uint8_t* out_contrib) try {
+static int hypotheses_forward_impl(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
+                                   int64_t assign_stride, int M, int shiftX, int shiftY, float f, float ppx, float ppy, float tau,
+                                   float alpha, float beta, float maxReproj, int sub, void* tape, size_t tape_bytes_,
+                                   double* out_scores, double* out_poses6, uint8_t* out_contrib) {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     if (!coords || !assign || !tape || !out_scores || !out_poses6 || !out_contrib) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
@@ -1551,10 +1552,19 @@ int esacb200_hypotheses_forward(esacb200_ctx* ctx, const float* coords, int E, i
     finish_stats(ctx);
     ctx->inj_M = ctx->inj_T = 0;
     return ESACB200_OK;
+}
+
+int esacb200_hypotheses_forward(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
+                                int64_t assign_stride, int M, int shiftX, int shiftY, float f, float ppx, float ppy, float tau,
+                                float alpha, float beta, float maxReproj, int sub, void* tape, size_t tape_bytes_,
+                                double* out_scores, double* out_poses6, uint8_t* out_contrib) try {
+    return hypotheses_forward_impl(ctx, coords, E, H, W, assign, assign_stride, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta,
+                                   maxReproj, sub, tape, tape_bytes_, out_scores, out_poses6, out_contrib);
 } ESAC_ABI_CATCH(ctx)
 
-int esacb200_hypotheses_backward(esacb200_ctx* ctx, const void* tape, const float* coords, float* grads, int E, int H, int W,
-                                 const double* d_scores, const double* d_poses6) try {
+// d_scores / d_poses6 are [rows, M] / [rows, M, 6] arrays (M of the tape) of which row `row` is this tape's upstream.
+static int hypotheses_backward_impl(esacb200_ctx* ctx, const void* tape, const float* coords, float* grads, int E, int H, int W,
+                                    const double* d_scores, const double* d_poses6, int row) {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     if (!tape || !coords || !grads) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
@@ -1568,6 +1578,8 @@ int esacb200_hypotheses_backward(esacb200_ctx* ctx, const void* tape, const floa
     if (P.E != E || P.H != H || P.W != W)
         return fail(ctx, ESACB200_ERR_ARG, "coordinates are [%d,3,%d,%d], the forward saw [%d,3,%d,%d]", E, H, W, P.E, P.H, P.W);
     const int M = head.M;
+    if (d_scores) d_scores += (size_t)row * M;
+    if (d_poses6) d_poses6 += (size_t)row * M * 6;
     begin_call(ctx);
     const size_t cbytes = (size_t)E * 3 * P.N * sizeof(float);
     const float* d_coords = coords;
@@ -1618,33 +1630,44 @@ int esacb200_hypotheses_backward(esacb200_ctx* ctx, const void* tape, const floa
     ctx->st.n_contrib = head.n_contrib;
     finish_stats(ctx);
     return ESACB200_OK;
+}
+
+int esacb200_hypotheses_backward(esacb200_ctx* ctx, const void* tape, const float* coords, float* grads, int E, int H, int W,
+                                 const double* d_scores, const double* d_poses6) try {
+    return hypotheses_backward_impl(ctx, tape, coords, grads, E, H, W, d_scores, d_poses6, 0);
 } ESAC_ABI_CATCH(ctx)
 
-int esacb200_pose_loss(esacb200_ctx* ctx, int M, const double* poses6, const float* gt16, float wRot, float wTrans, float cut,
-                       double* out_losses, double* out_dloss6) try {
+int esacb200_pose_loss_batch(esacb200_ctx* ctx, int B, int M, const double* poses6, const float* gt16, float wRot, float wTrans,
+                             float cut, double* out_losses, double* out_dloss6) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     if (!poses6 || !gt16 || !out_losses || !out_dloss6) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
     if (M <= 0) return fail(ctx, ESACB200_ERR_ARG, "no poses (M=%d)", M);
+    if (B <= 0 || B > 65535) return fail(ctx, ESACB200_ERR_ARG, "batch of %d images outside [1, 65535]", B);
     begin_call(ctx);
-    float gt[16];
-    CK(cudaMemcpyAsync(gt, gt16, sizeof(gt), cudaMemcpyDefault, ctx->stream));
-    // [M] poses, [M] losses, [M,6] dLoss
-    CK(ctx->upstream.ensure((size_t)M * 13 * 8));
+    const size_t n = (size_t)B * M;
+    // [B,M] poses, [B,M] losses, [B,M,6] dLoss; the ground truths [B,4,4] in their own buffer
+    CK(ctx->upstream.ensure(n * 13 * 8));
+    CK(ctx->gt.ensure((size_t)B * 16 * sizeof(float)));
     double* buf = ctx->upstream.as<double>();
-    CK(cudaMemcpyAsync(buf, poses6, (size_t)M * sizeof(Pose), cudaMemcpyDefault, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    launch_pose_loss((const Pose*)buf, M, gt, wRot, wTrans, cut, buf + 6 * (size_t)M, buf + 7 * (size_t)M, ctx->stream);
+    CK(cudaMemcpyAsync(buf, poses6, n * sizeof(Pose), cudaMemcpyDefault, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->gt.p, gt16, (size_t)B * 16 * sizeof(float), cudaMemcpyDefault, ctx->stream));
+    launch_pose_loss((const Pose*)buf, B, M, ctx->gt.as<float>(), wRot, wTrans, cut, buf + 6 * n, buf + 7 * n, ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 1;
-    CK(cudaMemcpyAsync(out_losses, buf + 6 * (size_t)M, (size_t)M * 8, cudaMemcpyDefault, ctx->stream));
-    CK(cudaMemcpyAsync(out_dloss6, buf + 7 * (size_t)M, (size_t)M * 6 * 8, cudaMemcpyDefault, ctx->stream));
+    CK(cudaMemcpyAsync(out_losses, buf + 6 * n, n * 8, cudaMemcpyDefault, ctx->stream));
+    CK(cudaMemcpyAsync(out_dloss6, buf + 7 * n, n * 6 * 8, cudaMemcpyDefault, ctx->stream));
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
     finish_stats(ctx);
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
+
+int esacb200_pose_loss(esacb200_ctx* ctx, int M, const double* poses6, const float* gt16, float wRot, float wTrans, float cut,
+                       double* out_losses, double* out_dloss6) {
+    return esacb200_pose_loss_batch(ctx, 1, M, poses6, gt16, wRot, wTrans, cut, out_losses, out_dloss6);
+}
 
 int esacb200_backward_sharded(esacb200_ctx* ctx, const float* coords, float* grads, int E, int H, int W, const int64_t* assign,
                               int64_t assign_stride, int M, const float* gt_pose, float wRot, float wTrans, float cut,
@@ -1715,45 +1738,19 @@ int esacb200_backward_sharded_nccl(esacb200_ctx* ctx, const float* coords, float
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
-// esac_backward over a batch.  Every image is an independent problem (SURVEY 8e: "images in a batch are fully
-// independent"), so the images are dealt round-robin to a few worker contexts, each driven by its own host thread on its
-// own stream: the small kernels of one image fill the gaps the host synchronisations of another leave.  Image b has its own
-// map size; the seeds are fixed per image before the images are dealt, so a worker runs its images largest first and its
-// workspace grows at most once.
-int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H, const int* W,
-                             int E, const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wRot,
-                             float wTrans, float cut, const int* shiftX, const int* shiftY, const float* f, const float* ppx,
-                             const float* ppy, float tau, float alpha, float beta, float maxReproj, int sub,
-                             double* out_losses) try {
-    if (!ctx) return ESACB200_ERR_ARG;
-    DeviceGuard device_guard(ctx->device);
-    if (!coords || !grads || !H || !W || !assign || !gt_poses || B <= 0)
-        return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
-    if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
-    if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
-    if (E <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d M=%d", E, M);
-    for (int b = 0; b < B; ++b) {
-        if (H[b] <= 0 || W[b] <= 0) return fail(ctx, ESACB200_ERR_ARG, "image %d: bad size %dx%d", b, W[b], H[b]);
-        if ((long long)H[b] * W[b] > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too large", b, W[b], H[b]);
-        if ((long long)(W[b] - 1) * (H[b] - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too small", b, W[b], H[b]);
-    }
-    bool dev_c = false, dev_g = false;
-    int rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
-    if (rc) return rc;
-    rc = pointer_kind(ctx, (const void* const*)grads, B, "grads", dev_g);
-    if (rc) return rc;
-    const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
-    std::vector<float> gt_host;
-    const float* gt = gt_poses;
-    if (is_device_ptr(gt_poses)) {
-        gt_host.resize((size_t)B * 16);
-        CK(cudaMemcpyAsync(gt_host.data(), gt_poses, gt_host.size() * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-        gt = gt_host.data();
-    }
-    // everything the caller queued on its stream (the experts' outputs) is visible to the workers after this
+// Batches.  Every image is an independent problem (SURVEY 8e: "images in a batch are fully independent"), so the images
+// are dealt round-robin to a few worker contexts, each driven by its own host thread on its own stream: the small kernels of
+// one image fill the gaps the host synchronisations of another leave.  Image b has its own map size; with `draws` the seeds
+// are fixed per image before the images are dealt (image b draws what the b-th of B consecutive single-image calls would),
+// so a worker runs its images largest first and its workspace grows at most once.  `image(w, b)` runs image b on worker
+// context w.  Everything the caller queued on its stream (the experts' outputs) is visible to the workers.  The statistics
+// of the call are those of the last image, with the wall time and kernel launches of the whole batch.
+static int run_batch(esacb200_ctx* ctx, int B, const int* H, const int* W, bool draws,
+                     const std::function<int(esacb200_ctx*, int)>& image) {
     CK(cudaStreamSynchronize(ctx->stream));
     std::vector<uint64_t> seeds((size_t)B);
-    for (int b = 0; b < B; ++b) seeds[b] = call_seed(ctx);
+    if (draws)
+        for (int b = 0; b < B; ++b) seeds[b] = call_seed(ctx);
     const int nw = ctx->batch_workers < B ? ctx->batch_workers : B;
     while ((int)ctx->workers.size() < nw) {
         esacb200_ctx* w = nullptr;
@@ -1787,13 +1784,8 @@ int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coord
         std::stable_sort(mine.begin(), mine.end(), [&](int a, int c) { return (long long)H[a] * W[a] > (long long)H[c] * W[c]; });
         for (int b : mine) {
             w->seed = seeds[b];
-            double loss = 0;
-            int rc = backward_impl(w, coords[b], grads[b], E, H[b], W[b], assign + (size_t)b * arow,
-                                   assign_stride, M, gt + (size_t)b * 16, wRot, wTrans, cut, shiftX ? shiftX[b] : 0,
-                                   shiftY ? shiftY[b] : 0, f[b], ppx[b], ppy[b], tau, alpha, beta, maxReproj, sub, nullptr, nullptr,
-                                   &loss);
+            int rc = image(w, b);
             if (rc) { rcs[wi] = rc; failed_at[wi] = b; return; }
-            if (out_losses) out_losses[b] = loss;
             launches[wi] += w->st.kernel_launches;
             if (b == B - 1) last[wi] = w->st;
         }
@@ -1814,15 +1806,126 @@ int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coord
     const double wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     for (int wi = 0; wi < nw; ++wi)
         if (rcs[wi]) return fail(ctx, rcs[wi], "image %d: %s", failed_at[wi], ctx->workers[wi]->err);
-    // statistics of the call: those of the last image, wall time and launches of the whole batch
     ctx->st = last[(B - 1) % nw];
     unsigned long long total = 0;
     for (int wi = 0; wi < nw; ++wi) total += launches[wi];
     ctx->st.kernel_launches = total;
     ctx->st.ms_total = (float)wall_ms;
     ctx->last_M = 0;  // the per-hypothesis buffers live in the workers
+    return ESACB200_OK;
+}
+
+// Sizes of a ragged batch: every image positive, addressable and large enough to draw 4 distinct cells from.
+static int check_ragged_sizes(esacb200_ctx* ctx, int B, const int* H, const int* W) {
+    for (int b = 0; b < B; ++b) {
+        if (H[b] <= 0 || W[b] <= 0) return fail(ctx, ESACB200_ERR_ARG, "image %d: bad size %dx%d", b, W[b], H[b]);
+        if ((long long)H[b] * W[b] > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too large", b, W[b], H[b]);
+        if ((long long)(W[b] - 1) * (H[b] - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too small", b, W[b], H[b]);
+    }
+    return 0;
+}
+
+// esac_backward over a batch, on the worker contexts of run_batch.
+int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H, const int* W,
+                             int E, const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wRot,
+                             float wTrans, float cut, const int* shiftX, const int* shiftY, const float* f, const float* ppx,
+                             const float* ppy, float tau, float alpha, float beta, float maxReproj, int sub,
+                             double* out_losses) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (!coords || !grads || !H || !W || !assign || !gt_poses || B <= 0)
+        return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
+    if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
+    if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
+    if (E <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d M=%d", E, M);
+    int rc = check_ragged_sizes(ctx, B, H, W);
+    if (rc) return rc;
+    bool dev_c = false, dev_g = false;
+    rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
+    if (rc) return rc;
+    rc = pointer_kind(ctx, (const void* const*)grads, B, "grads", dev_g);
+    if (rc) return rc;
+    const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
+    std::vector<float> gt_host;
+    const float* gt = gt_poses;
+    if (is_device_ptr(gt_poses)) {  // read back with run_batch's synchronisation
+        gt_host.resize((size_t)B * 16);
+        CK(cudaMemcpyAsync(gt_host.data(), gt_poses, gt_host.size() * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+        gt = gt_host.data();
+    }
+    rc = run_batch(ctx, B, H, W, true, [&](esacb200_ctx* w, int b) {
+        double loss = 0;
+        int rc = backward_impl(w, coords[b], grads[b], E, H[b], W[b], assign + (size_t)b * arow, assign_stride, M,
+                               gt + (size_t)b * 16, wRot, wTrans, cut, shiftX ? shiftX[b] : 0, shiftY ? shiftY[b] : 0, f[b], ppx[b],
+                               ppy[b], tau, alpha, beta, maxReproj, sub, nullptr, nullptr, &loss);
+        if (!rc && out_losses) out_losses[b] = loss;
+        return rc;
+    });
+    if (rc) return rc;
     ctx->last_backward = true;
     return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+// The hypotheses node over a batch, on the worker contexts of run_batch: image b runs the single-image forward / backward
+// with row b of the [B,M] outputs / upstreams.
+int esacb200_hypotheses_forward_ragged(esacb200_ctx* ctx, int B, const float* const* coords, const int* H, const int* W, int E,
+                                       const int64_t* assign, int64_t assign_stride, int M, const int* shiftX, const int* shiftY,
+                                       const float* f, const float* ppx, const float* ppy, float tau, float alpha, float beta,
+                                       float maxReproj, int sub, void* const* tapes, const size_t* tape_bytes_,
+                                       double* out_scores, double* out_poses6, uint8_t* out_contrib) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (!coords || !H || !W || !assign || !tapes || !tape_bytes_ || !out_scores || !out_poses6 || !out_contrib || B <= 0)
+        return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
+    if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
+    if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
+    if (E <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d M=%d", E, M);
+    int rc = check_ragged_sizes(ctx, B, H, W);
+    if (rc) return rc;
+    bool dev_c = false;
+    rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
+    if (rc) return rc;
+    for (int b = 0; b < B; ++b) {
+        if (!tapes[b]) return fail(ctx, ESACB200_ERR_ARG, "image %d: tape is null", b);
+        const size_t need = tape_bytes(M, H[b] * W[b]);
+        if (tape_bytes_[b] < need)
+            return fail(ctx, ESACB200_ERR_ARG, "image %d: tape holds %zu bytes, this call needs %zu", b, tape_bytes_[b], need);
+        if (!is_device_ptr(tapes[b]) || ((uintptr_t)tapes[b] & 15))
+            return fail(ctx, ESACB200_ERR_ARG, "image %d: tape must be 16-byte aligned device memory", b);
+    }
+    const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
+    rc = run_batch(ctx, B, H, W, true, [&](esacb200_ctx* w, int b) {
+        return hypotheses_forward_impl(w, coords[b], E, H[b], W[b], assign + (size_t)b * arow, assign_stride, M,
+                                       shiftX ? shiftX[b] : 0, shiftY ? shiftY[b] : 0, f[b], ppx[b], ppy[b], tau, alpha, beta,
+                                       maxReproj, sub, tapes[b], tape_bytes_[b], out_scores + (size_t)b * M,
+                                       out_poses6 + (size_t)b * M * 6, out_contrib + (size_t)b * M);
+    });
+    if (rc) return rc;
+    ctx->last_backward = false;
+    return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_hypotheses_backward_ragged(esacb200_ctx* ctx, int B, const void* const* tapes, const float* const* coords,
+                                        float* const* grads, const int* H, const int* W, int E, const double* d_scores,
+                                        const double* d_poses6) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (!tapes || !coords || !grads || !H || !W || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
+    if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
+    if (E <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad size E=%d", E);
+    int rc = check_ragged_sizes(ctx, B, H, W);
+    if (rc) return rc;
+    bool dev_c = false, dev_g = false, dev_t = false;
+    rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
+    if (rc) return rc;
+    rc = pointer_kind(ctx, (const void* const*)grads, B, "grads", dev_g);
+    if (rc) return rc;
+    rc = pointer_kind(ctx, tapes, B, "tape", dev_t);
+    if (rc) return rc;
+    rc = run_batch(ctx, B, H, W, false, [&](esacb200_ctx* w, int b) {
+        return hypotheses_backward_impl(w, tapes[b], coords[b], grads[b], E, H[b], W[b], d_scores, d_poses6, b);
+    });
+    return rc ? rc : ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 
 // B images of one shape: the pointer and size arrays of [B,E,3,H,W] tensors.

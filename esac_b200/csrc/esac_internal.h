@@ -332,8 +332,8 @@ void launch_tape_records(const BwdArgs& a, const TapeHead& head, void* tape, uns
 // the tape's records with dl = d_poses6[h], g = d_scores[h], p = 1 (device arrays of M), then B2-B5 into a.grads
 void launch_backward_upstream(const BwdArgs& a, const void* tape, const double* d_scores, const double* d_poses6, int max_jobs,
                               int sm_count, cudaStream_t st);
-// loss / dLoss of M scene poses against a camera->world ground truth (one block)
-void launch_pose_loss(const Pose* poses, int M, const float gt[16], float wRot, float wTrans, float cut, double* losses,
+// loss / dLoss of [B,M] scene poses, image b against camera->world ground truth gt16[b] (device [B,4,4]); outputs [B,M], [B,M,6]
+void launch_pose_loss(const Pose* poses, int B, int M, const float* gt16, float wRot, float wTrans, float cut, double* losses,
                       double* dloss6, cudaStream_t st);
 
 }  // namespace esacb200

@@ -106,6 +106,30 @@ int esacb200_hypotheses_backward(esacb200_ctx* ctx, const void* tape, const floa
  * pointers; the arithmetic is esacb200_backward's. */
 int esacb200_pose_loss(esacb200_ctx* ctx, int M, const double* poses6, const float* gt16, float wLossRot, float wLossTrans,
                        float lossCut, double* out_losses, double* out_dloss6);
+/* esacb200_pose_loss over a batch, in one launch: poses6 double [B,M,6], image b against gt16[b] of float32 [B,4,4];
+ * out_losses double [B,M], out_dloss6 double [B,M,6].  Row b is bitwise what esacb200_pose_loss on it gives, which is this
+ * entry with B = 1.  No host synchronisation before the launch. */
+int esacb200_pose_loss_batch(esacb200_ctx* ctx, int B, int M, const double* poses6, const float* gt16, float wLossRot,
+                             float wLossTrans, float lossCut, double* out_losses, double* out_dloss6);
+
+/* The hypotheses node over a ragged batch: every image-sized argument is a host array of B pointers (all device or all
+ * host), H / W host int [B], shiftX / shiftY host int [B] or NULL (= 0), f / ppx / ppy host float [B].
+ * esacb200_hypotheses_forward_ragged: image b draws, scores and refines what the b-th of B consecutive
+ * esacb200_hypotheses_forward calls (or esacb200_backward calls) on the context would, with its own shift and camera, and
+ * writes row b of out_scores double [B,M], out_poses6 double [B,M,6], out_contrib uint8 [B,M] (host or device).  tapes[b]
+ * is 16-byte aligned device memory of tape_bytes[b] >= esacb200_hypotheses_tape_bytes(E, H[b], W[b], M) bytes.
+ * esacb200_hypotheses_backward_ragged ACCUMULATES into grads[b] float32 [E,3,H[b],W[b]] what esacb200_hypotheses_backward
+ * on tapes[b] with rows b of d_scores double [B,M] / d_poses6 double [B,M,6] (NULL = zero; M of the tapes) would add.
+ * Images are spread over option "batch_workers" internal streams, as for esacb200_backward_batch; errors name the image. */
+int esacb200_hypotheses_forward_ragged(esacb200_ctx* ctx, int B, const float* const* coords, const int* H, const int* W, int E,
+                                       const int64_t* assign, int64_t assign_stride, int M, const int* shiftX, const int* shiftY,
+                                       const float* f, const float* ppx, const float* ppy, float inlierThreshold,
+                                       float inlierAlpha, float inlierBeta, float maxReproj, int subSampling,
+                                       void* const* tapes, const size_t* tape_bytes, double* out_scores, double* out_poses6,
+                                       uint8_t* out_contrib);
+int esacb200_hypotheses_backward_ragged(esacb200_ctx* ctx, int B, const void* const* tapes, const float* const* coords,
+                                        float* const* grads, const int* H, const int* W, int E, const double* d_scores,
+                                        const double* d_poses6);
 
 /* ---- additive entry points ------------------------------------------------------------------ */
 /* esac_backward over hypotheses sharded across processes (one per GPU; experts expert-major, so gradient slices are

@@ -131,6 +131,10 @@ def load_library() -> C.CDLL:
     lib.esacb200_hypotheses_forward_ragged.restype = i32
     lib.esacb200_hypotheses_backward_ragged.argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, vp, vp]
     lib.esacb200_hypotheses_backward_ragged.restype = i32
+    lib.esacb200_forward_async.argtypes = [vp, i32, vp, i32, i32, i32, vp, i64, i32, vp, vp, f32, f32, f32, f32, i32, vp, vp, vp]
+    lib.esacb200_forward_async.restype = i32
+    lib.esacb200_reserve_forward_async.argtypes = [vp, i32, i32, i32, i32, i32, i32]
+    lib.esacb200_reserve_forward_async.restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
         getattr(lib, "esacb200_" + name).restype = i32
@@ -200,6 +204,11 @@ class Context:
 
     # additive API ------------------------------------------------------------------------------
     def set_seed(self, seed: int):
+        """Seeds the draws and resets the call counters.  Once forward_async has run on the context, the reset of its
+        device-side seed is enqueued on torch's current stream, ordered with the calls and graph replays there."""
+        if getattr(self, "async_used", False):
+            import torch
+            self.set_stream(torch.cuda.current_stream(self.device).cuda_stream or _CUDA_STREAM_LEGACY)
         self.check(self.lib.esacb200_set_seed(self.handle, C.c_uint64(seed & ((1 << 64) - 1))))
 
     def set_option(self, key: str, value: float):
@@ -1253,6 +1262,88 @@ def pose_loss(poses, gtPose, wLossRot, wLossTrans, lossCut):
     ctx.check(ctx.lib.esacb200_pose_loss_batch(ctx.handle, B, M, po.ptr, gt.ptr, float(wLossRot), float(wLossTrans),
                                                float(lossCut), losses.data_ptr(), dloss.data_ptr()))
     return losses, dloss
+
+
+def _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras):
+    """Checks the dtypes and shapes of forward_async's inputs (one B) before any context exists; returns (B, E, H, W, M).
+    [E,3,H,W] / [M] / [2] / [3] inputs are one image."""
+    for t, what in ((sceneCoordinates, "sceneCoordinates"), (hypAssignment, "hypAssignment"), (shifts, "shifts"),
+                    (cameras, "cameras")):
+        if not _is_torch(t):
+            raise RuntimeError(f"forward_async takes torch CUDA tensors only ({what} is a {type(t).__name__})")
+    single = sceneCoordinates.dim() == 4
+    _check(sceneCoordinates, "Float", 4 if single else 5, "sceneCoordinates")
+    _check(hypAssignment, "Long", 1 if single else 2, "hypAssignment")
+    _check(shifts, "Int", 1 if single else 2, "shifts")
+    _check(cameras, "Float", 1 if single else 2, "cameras")
+    lead = () if single else (int(sceneCoordinates.shape[0]),)
+    B = lead[0] if lead else 1
+    E, three, H, W = (int(v) for v in sceneCoordinates.shape[-4:])
+    if three != 3:
+        raise RuntimeError("sceneCoordinates must be [B,E,3,H,W] or [E,3,H,W]")
+    if B < 1 or E < 1:
+        raise RuntimeError("sceneCoordinates holds no image or no expert")
+    if (W - 1) * (H - 1) < 4:
+        raise RuntimeError(f"sceneCoordinates: map {W}x{H} too small to draw 4 distinct cells")
+    M = int(hypAssignment.shape[-1])
+    if M < 1:
+        raise RuntimeError("hypAssignment holds no hypothesis")
+    for t, tail, what in ((hypAssignment, (M,), "hypAssignment"), (shifts, (2,), "shifts"), (cameras, (3,), "cameras")):
+        if tuple(int(v) for v in t.shape) != lead + tail:
+            want = ", ".join(str(v) for v in lead + tail)
+            raise RuntimeError(f"{what} must be [{want}] for {B} image(s), got {list(t.shape)}")
+    return B, E, H, W, M
+
+
+def forward_async(sceneCoordinates, hypAssignment, shifts, cameras, inlierThreshold, inlierAlpha, inlierBeta, maxReproj,
+                  subSampling, outPoses, outExperts, outStatus):
+    """esac.forward enqueued on torch's current stream with no host synchronisation, so it can be captured in a CUDA graph
+    (torch.cuda.graph).  CUDA tensors only: sceneCoordinates float32 [B,E,3,H,W], hypAssignment int64 [B,M], shifts int32
+    [B,2] (shiftX, shiftY), cameras float32 [B,3] (focal length, ppointX, ppointY); the results go to outPoses float32
+    [B,4,4] (camera->world), outExperts int64 [B] and outStatus int32 [B] (0 = OK, 1 = an expert index outside [0,E): pose
+    NaN, expert -1).  [E,3,H,W] / [M] / [2] / [3] / [4,4] / [] tensors are one image.  The seed, shift and camera are read
+    on the device when the kernels run: a replayed graph uses what the tensors hold then, and image b of the j-th call
+    after set_seed(s) draws what the (j*B + b)-th esac.forward after set_seed(s) draws.  Call reserve_forward_async with
+    the largest shape before the first capture; once captured, the workspace never grows again."""
+    B, E, H, W, M = _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras)
+    lead = (B,) if sceneCoordinates.dim() == 5 else ()
+    for t, dt, tail, what in ((outPoses, "Float", (4, 4), "outPoses"), (outExperts, "Long", (), "outExperts"),
+                              (outStatus, "Int", (), "outStatus")):
+        if not _is_torch(t):
+            raise RuntimeError(f"forward_async takes torch CUDA tensors only ({what} is a {type(t).__name__})")
+        _check(t, dt, len(lead + tail), what)
+        if tuple(int(v) for v in t.shape) != lead + tail or not t.is_contiguous():
+            raise RuntimeError(f"{what} must be a contiguous {list(lead + tail)} tensor, got {list(t.shape)}")
+    for t, what in ((sceneCoordinates, "sceneCoordinates"), (shifts, "shifts"), (cameras, "cameras")):
+        if not t.is_contiguous():
+            raise RuntimeError(f"{what} must be contiguous (a copy would not be captured with the call)")
+    if lead and B > 1 and hypAssignment.stride(0) != M * hypAssignment.stride(-1):
+        raise RuntimeError("hypAssignment must hold its rows back to back (row stride M times the element stride)")
+    args = {"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment, "shifts": shifts, "cameras": cameras,
+            "outPoses": outPoses, "outExperts": outExperts, "outStatus": outStatus}
+    for what, t in args.items():
+        if not t.is_cuda:
+            raise RuntimeError(f"forward_async takes CUDA tensors only ({what} is on the CPU)")
+    devs = {t.device.index for t in args.values()}
+    if len(devs) > 1:
+        raise RuntimeError(f"esac_b200: tensors live on different CUDA devices {sorted(devs)}")
+    ctx = _pick_ctx(*devs)
+    ctx.async_used = True
+    ctx.check(ctx.lib.esacb200_forward_async(ctx.handle, B, sceneCoordinates.data_ptr(), E, H, W, hypAssignment.data_ptr(),
+                                             int(hypAssignment.stride(-1)), M, shifts.data_ptr(), cameras.data_ptr(),
+                                             float(inlierThreshold), float(inlierAlpha), float(inlierBeta), float(maxReproj),
+                                             int(subSampling), outPoses.data_ptr(), outExperts.data_ptr(), outStatus.data_ptr()))
+
+
+def reserve_forward_async(B: int, E: int, H: int, W: int, M: int, subSampling: int = 8, device: int | None = None):
+    """Sizes forward_async's workspace for this shape; call it before capturing (it allocates)."""
+    if min(int(B), int(E), int(H), int(W), int(M)) < 1:
+        raise RuntimeError(f"reserve_forward_async: sizes must be positive, got B={B} E={E} H={H} W={W} M={M}")
+    ctx = context(device)
+    import torch
+    ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
+    ctx.async_used = True
+    ctx.check(ctx.lib.esacb200_reserve_forward_async(ctx.handle, int(B), int(E), int(H), int(W), int(M), int(subSampling)))
 
 
 def set_seed(seed: int, device: int | None = None):

@@ -111,6 +111,13 @@ struct esacb200_ctx {
     int comm_world = 1, comm_rank = 0;
     DevBuf gathered, grads_work;
     std::vector<esacb200_ctx*> workers;  // lazily created contexts of esacb200_backward_batch (own stream + workspace each)
+    // Stream-ordered forward (esacb200_forward_async): its own context, so that eager calls never touch the buffers a
+    // captured graph holds.  In that context: is_async = true, seed_state = device {base seed, async calls}, and frozen once
+    // a capture has used the workspace (from then on nothing in it is freed or reallocated).
+    esacb200_ctx* async = nullptr;
+    bool is_async = false;
+    bool frozen = false;
+    DevBuf seed_state;
 };
 
 namespace {
@@ -205,6 +212,7 @@ bool is_device_ptr(const void* p) {
 }
 
 void mark(esacb200_ctx* c, int id) {
+    if (c->is_async) return;  // no stage timers for stream-ordered calls: they would need a synchronisation to read
     cudaEventRecord(c->ev[id], c->stream);
     c->ev_used[id] = true;
 }
@@ -229,6 +237,16 @@ struct Plan {
     const long long* d_assign;
     long long assign_stride;
     int split_e = 0;  // > 0: host maps are uploaded in two halves [0, split_e) / [split_e, E) on the copy stream (ev_copied[0/1])
+    const struct AsyncImage* async = nullptr;  // stream-ordered forward: device parameters and the caller's outputs
+};
+
+// One image of a stream-ordered forward: what its kernels read from device memory, and where its results go.
+struct AsyncImage {
+    DevParams dev;
+    float* pose;        // [4,4]
+    long long* expert;
+    int* status;
+    int advance;        // the last image of an execution: advance the async call counter by B
 };
 
 int fill_problem(esacb200_ctx* ctx, Problem& P, int E, int H, int W, int M, int shiftX, int shiftY, float f, float ppx,
@@ -409,7 +427,8 @@ int run_sample(esacb200_ctx* ctx, const Plan& pl, uint64_t seed) {
                                              ctx->sample_prefilter, ctx->hyp_offset, ctx->hyp_stride, ctx->poses.as<Pose>(), ctx->cells.as<int>(),
                                              ctx->tries.as<int>(), lane_streams, ctx->ev_fork, lane_joins,
                                              pl.split_e, ctx->perm.as<int>(), ctx->offsets.as<int>(), ctx->ev_copied,
-                                             ctx->sample_span0, ctx->sample_window, ctx->sample_waves, trace, ctx->sample_tail_boost);
+                                             ctx->sample_span0, ctx->sample_window, ctx->sample_waves, trace, ctx->sample_tail_boost,
+                                             pl.async ? &pl.async->dev : nullptr);
     CK(cudaGetLastError());
     ctx->smp_groups_last = G;
     ctx->smp_Mg_last = Mg;
@@ -431,7 +450,7 @@ int run_score(esacb200_ctx* ctx, const Plan& pl) {
     ScoreArgs a;
     score_constants(P, a);
     launch_fold(ctx->poses.as<Pose>(), ctx->perm.as<int>(), ctx->assign32.as<int>(), ctx->centres.as<float>(), P,
-                a.fold ? a.k1 : 1.f, ctx->posepk.as<PosePk>(), ctx->stream);
+                a.fold ? a.k1 : 1.f, ctx->posepk.as<PosePk>(), ctx->stream, pl.async ? &pl.async->dev : nullptr);
     mark(ctx, EV_FOLD);
     a.coords = pl.d_coords;
     a.centres = ctx->centres.as<float>();
@@ -444,6 +463,7 @@ int run_score(esacb200_ctx* ctx, const Plan& pl) {
     a.T = pl.T;
     a.hc = pl.hc;
     a.vec_ok = pl.vec_ok;
+    if (pl.async) a.dev = pl.async->dev;
     launch_score(a, pl.ppt, pl.grid, ctx->stream);
     mark(ctx, EV_SCORE);
     launch_select(ctx->part.as<float>(), ctx->slot_of.as<int>(), P, pl.T, ctx->scores.as<double>(), ctx->probs.as<double>(),
@@ -549,6 +569,7 @@ int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, con
     }
     a.P = P;
     a.max_ref_steps = ctx->max_ref_steps;
+    if (pl.async) a.dev = pl.async->dev;
     launch_refine(a, n_groups, ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 1;
@@ -564,10 +585,11 @@ uint64_t call_seed(esacb200_ctx* ctx) {
 }
 
 // sample -> score -> select -> refine(winner) -> camera pose + expert id into d_out17 (17 floats + flags at [17]); no sync.
+// A stream-ordered image (pl.async) takes its seed from device memory and writes the caller's arrays instead.
 int enqueue_forward_core(esacb200_ctx* ctx, const Plan& pl, float* d_out17) {
     const Problem& P = pl.P;
     int* sc = ctx->scalars.as<int>();
-    const uint64_t seed = call_seed(ctx);
+    const uint64_t seed = pl.async ? 0 : call_seed(ctx);
     int rc = run_sample(ctx, pl, seed);
     if (rc) return rc;
     rc = run_score(ctx, pl);
@@ -576,7 +598,12 @@ int enqueue_forward_core(esacb200_ctx* ctx, const Plan& pl, float* d_out17) {
     rc = run_refine(ctx, pl, ctx->poses.as<Pose>(), ctx->poses_ref.as<Pose>(), sc + S_WINNER, nullptr, 1, 1, group);
     if (rc) return rc;
     mark(ctx, EV_REFINE);
-    launch_finish_forward(ctx->poses_ref.as<Pose>(), sc + S_WINNER, ctx->assign32.as<int>(), sc + S_FLAGS, d_out17, ctx->stream);
+    if (pl.async)
+        launch_finish_forward_async(ctx->poses_ref.as<Pose>(), sc + S_WINNER, ctx->assign32.as<int>(), sc + S_FLAGS, pl.async->pose,
+                                    pl.async->expert, pl.async->status, ctx->seed_state.as<unsigned long long>(), pl.async->advance,
+                                    ctx->stream);
+    else
+        launch_finish_forward(ctx->poses_ref.as<Pose>(), sc + S_WINNER, ctx->assign32.as<int>(), sc + S_FLAGS, d_out17, ctx->stream);
     ctx->st.kernel_launches += 1;
     return 0;
 }
@@ -584,9 +611,12 @@ int enqueue_forward_core(esacb200_ctx* ctx, const Plan& pl, float* d_out17) {
 // Sizes every workspace buffer of the forward pipeline (upload, plan_and_prep, sampling, refinement) for the largest of a
 // batch's images before the first one is enqueued: DevBuf::ensure growing mid-batch frees the old buffer, and cudaFree
 // synchronises the device, which would serialise the copy stream's overlap with the previous image.
-int reserve_forward_batch(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool host_coords) {
+// `need(buf, bytes)` is called for every buffer; reserve_forward_batch grows them, the stream-ordered forward also checks them.
+template <class Need>
+int forward_workspace(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool host_coords, Need&& need) {
     size_t part = 0, cbytes = 0, c4 = 0, sint = 0, ssurv = 0, masks = 0, rounds = 0, scratch = 0, barrier = 0, clist = 0;
     auto mx = [](size_t& a, size_t b) { if (b > a) a = b; };
+#define NEED(buf, bytes) do { int r__ = need(buf, bytes); if (r__) return r__; } while (0)
     int M = 0, E = 0;
     for (Plan pl : plans) {
         plan_launch(ctx, pl);
@@ -602,39 +632,47 @@ int reserve_forward_batch(esacb200_ctx* ctx, const std::vector<Plan>& plans, boo
         mx(masks, r.masks); mx(rounds, r.rounds); mx(scratch, r.scratch); mx(barrier, r.barrier); mx(clist, r.clist);
     }
     if (host_coords) {
-        CK(ctx->coords.ensure(cbytes));
-        CK(ctx->coords_alt.ensure(cbytes));
+        NEED(ctx->coords, cbytes);
+        NEED(ctx->coords_alt, cbytes);
     }
-    CK(ctx->assign64.ensure((size_t)M * 8));
-    CK(ctx->assign64_alt.ensure((size_t)M * 8));
-    CK(ctx->assign32.ensure((size_t)M * 4));
-    CK(ctx->counts.ensure((size_t)E * 4));
-    CK(ctx->offsets.ensure((size_t)(E + 1) * 4));
-    CK(ctx->perm.ensure((size_t)M * 4));
-    CK(ctx->slot_of.ensure((size_t)M * 4));
-    CK(ctx->chunks.ensure((size_t)(M + E) * sizeof(ChunkDesc)));
-    CK(ctx->scalars.ensure(S_COUNT * 4));
-    CK(ctx->centres.ensure((size_t)E * 3 * 4));
-    CK(ctx->poses.ensure((size_t)M * sizeof(Pose)));
-    CK(ctx->poses_ref.ensure((size_t)M * sizeof(Pose)));
-    CK(ctx->cells.ensure((size_t)M * 8 * 4));
-    CK(ctx->tries.ensure((size_t)M * 4));
-    CK(ctx->posepk.ensure((size_t)M * sizeof(PosePk)));
-    CK(ctx->part.ensure(part));
-    CK(ctx->scores.ensure((size_t)M * 8));
-    CK(ctx->probs.ensure((size_t)M * 8));
-    CK(ctx->stats.ensure(8 * 8));
-    CK(ctx->contrib.ensure((size_t)M * 4));
-    CK(ctx->out17.ensure(32 * 4));
-    CK(ctx->smp_int.ensure(sint));
-    CK(ctx->smp_surv.ensure(ssurv));
-    CK(ctx->coords4.ensure(c4));
-    CK(ctx->masks.ensure(masks));
-    CK(ctx->rounds.ensure(rounds));
-    CK(ctx->scratch.ensure(scratch));
-    CK(ctx->barrier.ensure(barrier));
-    if (clist) CK(ctx->clist.ensure(clist));
+    NEED(ctx->assign64, (size_t)M * 8);
+    NEED(ctx->assign64_alt, (size_t)M * 8);
+    NEED(ctx->assign32, (size_t)M * 4);
+    NEED(ctx->counts, (size_t)E * 4);
+    NEED(ctx->offsets, (size_t)(E + 1) * 4);
+    NEED(ctx->perm, (size_t)M * 4);
+    NEED(ctx->slot_of, (size_t)M * 4);
+    NEED(ctx->chunks, (size_t)(M + E) * sizeof(ChunkDesc));
+    NEED(ctx->scalars, S_COUNT * 4);
+    NEED(ctx->centres, (size_t)E * 3 * 4);
+    NEED(ctx->poses, (size_t)M * sizeof(Pose));
+    NEED(ctx->poses_ref, (size_t)M * sizeof(Pose));
+    NEED(ctx->cells, (size_t)M * 8 * 4);
+    NEED(ctx->tries, (size_t)M * 4);
+    NEED(ctx->posepk, (size_t)M * sizeof(PosePk));
+    NEED(ctx->part, part);
+    NEED(ctx->scores, (size_t)M * 8);
+    NEED(ctx->probs, (size_t)M * 8);
+    NEED(ctx->stats, 8 * 8);
+    NEED(ctx->contrib, (size_t)M * 4);
+    NEED(ctx->out17, 32 * 4);
+    NEED(ctx->smp_int, sint);
+    NEED(ctx->smp_surv, ssurv);
+    NEED(ctx->coords4, c4);
+    NEED(ctx->masks, masks);
+    NEED(ctx->rounds, rounds);
+    NEED(ctx->scratch, scratch);
+    NEED(ctx->barrier, barrier);
+    if (clist) NEED(ctx->clist, clist);
+#undef NEED
     return 0;
+}
+
+int reserve_forward_batch(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool host_coords) {
+    return forward_workspace(ctx, plans, host_coords, [&](DevBuf& b, size_t bytes) -> int {
+        CK(b.ensure(bytes));
+        return 0;
+    });
 }
 
 // All B pointers of one argument on the device, or all on the host (a mix is an error).  None may be null.
@@ -792,6 +830,8 @@ void esacb200_destroy(esacb200_ctx* ctx) {
     if (!ctx) return;
     for (esacb200_ctx* w : ctx->workers) esacb200_destroy(w);
     ctx->workers.clear();
+    if (ctx->async) esacb200_destroy(ctx->async);
+    ctx->async = nullptr;
     DeviceGuard device_guard(ctx->device);
     if (ctx->nccl_comm) { cudaStreamSynchronize(ctx->stream); nccl_api().CommDestroy(ctx->nccl_comm); ctx->nccl_comm = nullptr; }
     cudaStreamSynchronize(ctx->stream);
@@ -800,7 +840,7 @@ void esacb200_destroy(esacb200_ctx* ctx) {
                       &ctx->tries, &ctx->posepk, &ctx->part, &ctx->scores, &ctx->probs, &ctx->stats, &ctx->contrib,
                       &ctx->masks, &ctx->rounds, &ctx->scratch, &ctx->barrier, &ctx->out17, &ctx->inject, &ctx->losses,
                       &ctx->red, &ctx->hypgrad, &ctx->job_of, &ctx->gt, &ctx->smp_int, &ctx->smp_surv, &ctx->smp_trace, &ctx->clist, &ctx->eflags, &ctx->coords4, &ctx->coords_alt, &ctx->assign64_alt, &ctx->out_batch, &ctx->prof, &ctx->gathered, &ctx->grads_work,
-                      &ctx->contrib8, &ctx->upstream};
+                      &ctx->contrib8, &ctx->upstream, &ctx->seed_state};
     for (DevBuf* b : bufs) b->release();
     for (int i = 0; i < EV_COUNT; ++i)
         if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
@@ -835,6 +875,11 @@ int esacb200_set_seed(esacb200_ctx* ctx, uint64_t seed) {
     if (!ctx) return ESACB200_ERR_ARG;
     ctx->seed = seed;
     ctx->calls = 0;
+    if (ctx->async) {  // the stream-ordered forward's seed and call counter, in stream order
+        DeviceGuard device_guard(ctx->device);
+        launch_seed_reset(ctx->async->seed_state.as<unsigned long long>(), seed, ctx->stream);
+        CK(cudaGetLastError());
+    }
     return ESACB200_OK;
 }
 
@@ -1157,6 +1202,151 @@ int esacb200_forward_batch(esacb200_ctx* ctx, int B, const float* coords, int E,
     const std::vector<float> fs(n, f), cx(n, ppx), cy(n, ppy);
     return esacb200_forward_batch_cameras(ctx, B, coords, E, H, W, assign, assign_stride, M, out_poses, sx.data(), sy.data(),
                                           fs.data(), cx.data(), cy.data(), tau, alpha, beta, maxReproj, sub, out_experts);
+} ESAC_ABI_CATCH(ctx)
+
+// -------------------------------------------------------------------------------------------------
+// Stream-ordered forward.  The pipeline is enqueue_forward_core's, run in the context ctx->async with every image's seed,
+// shift and camera read from device memory (AsyncImage), so a CUDA graph that captured the call replays with the values the
+// arrays hold at replay time.  Nothing here synchronises, reads back or queries an event, and a call that a capture records
+// allocates nothing.
+
+// The stream-ordered forward's context, created on first use with ctx's seed (a capture may not create it: that allocates).
+// The options that shape the pipeline are copied from ctx on every call.
+static int async_context(esacb200_ctx* ctx, bool capturing, esacb200_ctx** out) {
+    if (!ctx->async) {
+        if (capturing)
+            return fail(ctx, ESACB200_ERR_ARG, "forward_async: the first call may not be captured; call reserve_forward_async "
+                                               "(esacb200_reserve_forward_async) with the largest shape before capturing");
+        esacb200_ctx* a = nullptr;
+        int rc = esacb200_create(ctx->device, &a);
+        if (rc) return fail(ctx, rc, "cannot create the context of the stream-ordered forward");
+        a->is_async = true;
+        if (a->seed_state.ensure(2 * sizeof(unsigned long long)) != cudaSuccess) {
+            esacb200_destroy(a);
+            cudaGetLastError();
+            return fail(ctx, ESACB200_ERR_CUDA, "cannot allocate the seed state of the stream-ordered forward");
+        }
+        launch_seed_reset(a->seed_state.as<unsigned long long>(), ctx->seed, ctx->stream);
+        ctx->async = a;
+    }
+    esacb200_ctx* a = ctx->async;
+    a->stream = ctx->stream;
+    a->max_tries = ctx->max_tries;
+    a->max_ref_steps = ctx->max_ref_steps;
+    a->fixed_seed = ctx->fixed_seed;
+    a->refine_group_opt = ctx->refine_group_opt;
+    a->refine_jobs_per_group = ctx->refine_jobs_per_group;
+    a->refine_compact = ctx->refine_compact;
+    a->refine_pretest = ctx->refine_pretest;
+    a->sample_prefilter = ctx->sample_prefilter;
+    a->sample_tail_boost = ctx->sample_tail_boost;
+    a->sample_span0 = ctx->sample_span0;
+    a->sample_window = ctx->sample_window;
+    a->sample_waves = ctx->sample_waves;
+    a->sample_groups = ctx->sample_groups;
+    a->hyp_offset = ctx->hyp_offset;
+    a->hyp_stride = ctx->hyp_stride;
+    a->score_ppt_opt = ctx->score_ppt_opt;
+    a->score_hc_opt = ctx->score_hc_opt;
+    *out = a;
+    return 0;
+}
+
+static int stream_capturing(esacb200_ctx* ctx, bool& capturing) {
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    CK(cudaStreamIsCapturing(ctx->stream, &cs));
+    capturing = cs != cudaStreamCaptureStatusNone;
+    return 0;
+}
+
+// Makes the async workspace hold `plans`: grows it when no capture has used it yet, else fails without touching it.
+static int async_workspace(esacb200_ctx* ctx, esacb200_ctx* a, const std::vector<Plan>& plans, bool capturing) {
+    const bool fits = forward_workspace(a, plans, false, [](DevBuf& b, size_t bytes) { return bytes <= b.cap ? 0 : 1; }) == 0;
+    if (fits) return 0;
+    const Problem& P = plans[0].P;
+    if (capturing || a->frozen)
+        return fail(ctx, ESACB200_ERR_ARG,
+                    "forward_async: E=%d H=%d W=%d M=%d needs more workspace than %s, and a graph that holds it may still be "
+                    "replayed; call reserve_forward_async (esacb200_reserve_forward_async) with the largest shape before the "
+                    "first capture", P.E, P.H, P.W, P.M, capturing ? "was reserved before this capture" : "an earlier capture used");
+    int rc = reserve_forward_batch(a, plans, false);
+    if (rc) return fail(ctx, rc, "%s", a->err);
+    return 0;
+}
+
+int esacb200_reserve_forward_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int sub) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "reserve_forward_async: empty batch (B=%d)", B);
+    std::vector<Plan> plans(1);
+    int rc = fill_problem(ctx, plans[0].P, E, H, W, M, 0, 0, 1.f, 0.f, 0.f, 1.f, 1.f, 1.f, 1.f, sub);
+    if (rc) return rc;
+    plans[0].d_coords = nullptr;  // the load path does not change the workspace
+    bool capturing = false;
+    rc = stream_capturing(ctx, capturing);
+    if (rc) return rc;
+    if (capturing) return fail(ctx, ESACB200_ERR_ARG, "reserve_forward_async allocates: call it before the capture");
+    esacb200_ctx* a = nullptr;
+    rc = async_context(ctx, false, &a);
+    if (rc) return rc;
+    return async_workspace(ctx, a, plans, false);
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
+                           int64_t assign_stride, int M, const int32_t* shifts, const float* cameras, float tau, float alpha,
+                           float beta, float maxReproj, int sub, float* out_poses, int64_t* out_experts, int32_t* out_status) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "forward_async: empty batch (B=%d)", B);
+    Problem P;
+    int rc = fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, tau, alpha, beta, maxReproj, sub);
+    if (rc) return rc;
+    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small to draw 4 distinct cells", W, H);
+    const void* ptrs[] = {coords, assign, shifts, cameras, out_poses, out_experts, out_status};
+    const char* names[] = {"coords", "assign", "shifts", "cameras", "out_poses", "out_experts", "out_status"};
+    for (int i = 0; i < 7; ++i) {
+        if (!ptrs[i]) return fail(ctx, ESACB200_ERR_ARG, "forward_async: %s is null", names[i]);
+        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "forward_async takes device pointers only: %s is host memory", names[i]);
+    }
+    bool capturing = false;
+    rc = stream_capturing(ctx, capturing);
+    if (rc) return rc;
+    esacb200_ctx* a = nullptr;
+    rc = async_context(ctx, capturing, &a);
+    if (rc) return rc;
+    // element stride between the assignments of consecutive images: rows of a [B, M] tensor
+    const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
+    const size_t cstride = (size_t)E * 3 * H * W;
+    std::vector<Plan> plans((size_t)B);
+    std::vector<AsyncImage> imgs((size_t)B);
+    for (int b = 0; b < B; ++b) {
+        Plan& pl = plans[b];
+        pl.P = P;
+        pl.d_coords = coords + (size_t)b * cstride;
+        pl.d_assign = (const long long*)assign + b * arow;
+        pl.assign_stride = assign_stride;
+        AsyncImage& im = imgs[b];
+        im.dev.shift = shifts + 2 * (size_t)b;
+        im.dev.cam = cameras + 3 * (size_t)b;
+        im.dev.seed = a->seed_state.as<unsigned long long>();
+        im.dev.index = b;
+        im.dev.fixed_seed = a->fixed_seed;
+        im.pose = out_poses + 16 * (size_t)b;
+        im.expert = (long long*)out_experts + b;
+        im.status = out_status + b;
+        im.advance = b == B - 1 ? B : 0;
+        pl.async = &im;
+    }
+    rc = async_workspace(ctx, a, plans, capturing);
+    if (rc) return rc;
+    if (capturing) a->frozen = true;
+    for (int b = 0; b < B; ++b) {
+        rc = plan_and_prep(a, plans[b]);
+        if (!rc) rc = enqueue_forward_core(a, plans[b], nullptr);
+        if (rc) return fail(ctx, rc, "image %d: %s", b, a->err);
+    }
+    CK(cudaGetLastError());
+    return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------

@@ -94,6 +94,36 @@ struct Problem {
     float tau, alpha, beta, max_reproj;
 };
 
+// Per-image values of a stream-ordered forward (esacb200_forward_async) that the kernels read from device memory instead
+// of from Problem / a seed argument, so that a captured graph replays with the values current at replay time.  The
+// kernels that take one are templates on a flag DEV; with DEV = false they ignore it and read Problem as before.
+struct DevParams {
+    const int* shift = nullptr;                // [2] shiftX, shiftY
+    const float* cam = nullptr;                // [3] f, ppx, ppy
+    const unsigned long long* seed = nullptr;  // [0] base seed, [1] async calls before this execution
+    int index = 0;                             // image b of the execution: its draws are those of call [1] + b
+    int fixed_seed = 0;
+};
+
+#ifdef __CUDACC__
+// The image's shift and camera: from P, or (DEV) from a.dev, where `a` is the kernel's argument struct.
+template <bool DEV, class A> __device__ __forceinline__ int dev_shift_x(const Problem& P, const A& a) {
+    if constexpr (DEV) return __ldg(a.dev.shift); else return P.shiftX;
+}
+template <bool DEV, class A> __device__ __forceinline__ int dev_shift_y(const Problem& P, const A& a) {
+    if constexpr (DEV) return __ldg(a.dev.shift + 1); else return P.shiftY;
+}
+template <bool DEV, class A> __device__ __forceinline__ float dev_f(const Problem& P, const A& a) {
+    if constexpr (DEV) return __ldg(a.dev.cam); else return P.f;
+}
+template <bool DEV, class A> __device__ __forceinline__ float dev_ppx(const Problem& P, const A& a) {
+    if constexpr (DEV) return __ldg(a.dev.cam + 1); else return P.ppx;
+}
+template <bool DEV, class A> __device__ __forceinline__ float dev_ppy(const Problem& P, const A& a) {
+    if constexpr (DEV) return __ldg(a.dev.cam + 2); else return P.ppy;
+}
+#endif
+
 // Hypotheses of one expert are contiguous in "sorted slot" order (stable by hypothesis index);
 // a chunk is <= kMaxChunk consecutive slots of one expert: the unit the scoring kernel pairs with a
 // pixel tile.
@@ -127,6 +157,7 @@ struct ScoreArgs {
     float tiny;              // floor of |p|^2: 1e-30, times k1^2 when fold
     int fold;                // k1 folded into the f rows and pixel offsets, one reciprocal per pair of cells
     int vec_ok;              // planes are 16-byte aligned and N % 4 == 0
+    DevParams dev;           // dev.shift != null: shift and camera from device memory (stream-ordered forward)
 };
 
 // --- score.cu -----------------------------------------------------------------------------
@@ -135,8 +166,9 @@ struct ScoreArgs {
 void launch_prep(const float* coords, const long long* assign, long long assign_stride, const Problem& P, int hc,
                  int* assign32, int* counts, int* offsets, int* perm, int* slot_of, ChunkDesc* chunks, int* n_chunks,
                  int* work_counter, float* centres, int* flags, int roles, cudaStream_t st);
+// dev: non-null -> f from device memory (stream-ordered forward)
 void launch_fold(const Pose* poses, const int* perm, const int* assign32, const float* centres, const Problem& P,
-                 float kf, PosePk* out, cudaStream_t st);
+                 float kf, PosePk* out, cudaStream_t st, const DevParams* dev = nullptr);
 int score_tile_pixels(int ppt);
 // k1, k0, tmax, tiny and fold of the scoring arguments for this problem
 void score_constants(const Problem& P, ScoreArgs& a);
@@ -176,7 +208,7 @@ int launch_sample(const float* coords, float4* coords4, const int* assign32, con
                   int hyp_offset, int hyp_stride, Pose* poses, int* cells, int* tries, const cudaStream_t* lanes,
                   cudaEvent_t ev_fork, const cudaEvent_t* ev_join, int split_e, const int* perm, const int* offsets,
                   const cudaEvent_t* ev_half, int span0, float window, int n_waves,
-                  unsigned long long* trace, float tail_boost);
+                  unsigned long long* trace, float tail_boost, const DevParams* dev = nullptr);
 void launch_trace_init(unsigned long long* trace, int slots, cudaStream_t st);
 
 // --- refine.cu ----------------------------------------------------------------------------
@@ -205,6 +237,7 @@ struct RefineArgs {
     long long* prof;         // diagnostics: 16 cycle counters of block 0 (null = off)
     Problem P;
     int max_ref_steps;
+    DevParams dev;           // dev.shift != null: shift and camera from device memory (stream-ordered forward)
 };
 void launch_refine(const RefineArgs& a, int n_groups, cudaStream_t st);
 int refine_max_coresident_blocks(int sm_count);
@@ -216,6 +249,13 @@ size_t refine_flag_words(int n_groups, int group);
 // out[17] = bad-assignment flag, out[18] = winning hypothesis
 void launch_finish_forward(const Pose* poses, const int* winner, const int* assign32, const int* flags, float* out20,
                            cudaStream_t st);
+
+// Stream-ordered forward: camera->world pose of poses[*winner] (NaN on a bad assignment) into pose16, its expert (-1 on a bad
+// assignment) into *expert, flags[0] into *status; advance != 0 adds it to seed[1] (the last image of an execution).
+void launch_finish_forward_async(const Pose* poses, const int* winner, const int* assign32, const int* flags, float* pose16,
+                                 long long* expert, int* status, unsigned long long* seed, int advance, cudaStream_t st);
+// seed[0] = base, seed[1] = 0, stream-ordered
+void launch_seed_reset(unsigned long long* seed, unsigned long long base, cudaStream_t st);
 
 void launch_pack_forward(const double* scores, const float* out20, int M, int M_pad, int expert_offset, int hyp_offset, int hyp_stride,
                          double* pack, cudaStream_t st);

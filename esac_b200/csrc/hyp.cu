@@ -27,6 +27,8 @@
 #include "esac_p3p_fast.cuh"
 #include "esac_rng.cuh"
 
+#include <type_traits>
+
 namespace esacb200 {
 
 constexpr int kTryThreads = 128;
@@ -56,6 +58,24 @@ struct SampleArgs {
     unsigned long long* trace;  // diagnostics (option sample_trace): [slot][2] first CTA start / last CTA end, globaltimer ns
     int trace_slot;
 };
+// The DEV kernels' arguments: the seed, shift and camera come from device memory (the eager kernels keep SampleArgs as is).
+struct SampleArgsDev : SampleArgs {
+    DevParams dev;
+};
+template <bool DEV>
+using SampleArgsT = std::conditional_t<DEV, SampleArgsDev, SampleArgs>;
+
+// The seed of the draws: the argument, or (DEV) what call_seed gives the (seed[1] + index)-th call after set_seed.
+template <bool DEV>
+__device__ __forceinline__ uint64_t sample_seed(const SampleArgsT<DEV>& a) {
+    if constexpr (DEV) {
+        const uint64_t base = __ldg(a.dev.seed), calls = __ldg(a.dev.seed + 1) + (uint64_t)a.dev.index;
+        if (calls == 0 || a.dev.fixed_seed) return base;
+        return mix64(base + kGold * calls);
+    } else {
+        return a.seed;
+    }
+}
 
 __device__ __forceinline__ unsigned long long gtime() {
     unsigned long long t;
@@ -78,21 +98,22 @@ __device__ __forceinline__ int lane_hyp(const SampleArgs& a, int k) {
     return a.perm ? a.perm[a.offsets[a.e_lo] + k] : a.h_first + k * a.h_step;
 }
 
-__device__ __forceinline__ void load_try(const SampleArgs& a, int h, int t, int cx[4], int cy[4], float obj[4][3], float img[4][2]) {
+template <bool DEV>
+__device__ __forceinline__ void load_try(const SampleArgsT<DEV>& a, int h, int t, int cx[4], int cy[4], float obj[4][3], float img[4][2]) {
     const Problem& P = a.P;
     if (a.injected) {
         const int* c = a.injected + ((size_t)h * a.inj_T + t) * 8;
         for (int j = 0; j < 4; ++j) { cx[j] = c[2 * j]; cy[j] = c[2 * j + 1]; }
     } else {
-        draw_minimal_set(a.seed, (uint32_t)(h * a.hyp_stride + a.hyp_offset), (uint32_t)t, P.W, P.H, cx, cy);
+        draw_minimal_set(sample_seed<DEV>(a), (uint32_t)(h * a.hyp_stride + a.hyp_offset), (uint32_t)t, P.W, P.H, cx, cy);
     }
     const float4* pl = a.coords4 + (size_t)a.assign32[h] * P.N;
     for (int j = 0; j < 4; ++j) {
         const int p = cy[j] * P.W + cx[j];
         const float4 v = __ldg(pl + p);
         obj[j][0] = v.x; obj[j][1] = v.y; obj[j][2] = v.z;
-        img[j][0] = (float)(cx[j] * P.sub + P.sub / 2 - P.shiftX);
-        img[j][1] = (float)(cy[j] * P.sub + P.sub / 2 - P.shiftY);
+        img[j][0] = (float)(cx[j] * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, a));
+        img[j][1] = (float)(cy[j] * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, a));
     }
 }
 
@@ -100,13 +121,20 @@ __device__ __forceinline__ void load_try(const SampleArgs& a, int h, int t, int 
 // point within 1.25 tau + 1 px (measured on the unpolished depths) is rejected before polish / alignment / Rodrigues / gate --
 // that is ~60 % of what survives the float prefilter's 2 tau band.  `solved` and `pose` are then meaningless; emit_kernel,
 // which needs the failure state of an exhausted hypothesis' last try, calls with verdict_only = false.
-__device__ __noinline__ bool exact_try(const SampleArgs& a, int h, int t, Pose& pose, int cx[4], int cy[4], bool& solved,
+template <bool DEV>
+__device__ __noinline__ bool exact_try(const SampleArgsT<DEV>& a, int h, int t, Pose& pose, int cx[4], int cy[4], bool& solved,
                                        bool verdict_only = false) {
     float obj[4][3], img[4][2];
-    load_try(a, h, t, cx, cy, obj, img);
-    const double f = (double)a.P.f, ppx = (double)a.P.ppx, ppy = (double)a.P.ppy;
-    solved = p3p_pose(obj, img, f, ppx, ppy, pose, verdict_only ? 1.25 * (double)a.P.tau + 1. : 0.);
-    return solved && minimal_set_gate(obj, img, pose, f, ppx, ppy, a.P.tau);
+    load_try<DEV>(a, h, t, cx, cy, obj, img);
+    if constexpr (DEV) {
+        const double f = (double)dev_f<DEV>(a.P, a), ppx = (double)dev_ppx<DEV>(a.P, a), ppy = (double)dev_ppy<DEV>(a.P, a);
+        solved = p3p_pose(obj, img, f, ppx, ppy, pose, verdict_only ? 1.25 * (double)a.P.tau + 1. : 0.);
+        return solved && minimal_set_gate(obj, img, pose, f, ppx, ppy, a.P.tau);
+    } else {  // the eager kernels' code as it was: written with the accessors, ptxas schedules its loads differently
+        const double f = (double)a.P.f, ppx = (double)a.P.ppx, ppy = (double)a.P.ppy;
+        solved = p3p_pose(obj, img, f, ppx, ppy, pose, verdict_only ? 1.25 * (double)a.P.tau + 1. : 0.);
+        return solved && minimal_set_gate(obj, img, pose, f, ppx, ppy, a.P.tau);
+    }
 }
 
 // [E,3,N] planes -> [E,N] float4 cells.  The sampling stage gathers 4 random cells per try, millions of times per
@@ -148,7 +176,8 @@ __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
 }
 // Decodes item -> (hypothesis, tries), draws the 2 x 4 cells and starts the 8 gathers of 16 bytes straight into shared
 // memory (cp.async: no registers are held while they are in flight).
-__device__ __forceinline__ void prefilter_issue(const SampleArgs& a, long long item, int cph, int span, float4 (*dst)[kTryThreads], PreItem& it) {
+template <bool DEV>
+__device__ __forceinline__ void prefilter_issue(const SampleArgsT<DEV>& a, long long item, int cph, int span, float4 (*dst)[kTryThreads], PreItem& it) {
     const int u = (int)(item / cph), c = (int)(item - (long long)u * cph);
     it.h = a.st.list[u];
     const int t0 = a.st.base[it.h];
@@ -169,7 +198,7 @@ __device__ __forceinline__ void prefilter_issue(const SampleArgs& a, long long i
             const int* cc = a.injected + ((size_t)it.h * a.inj_T + t) * 8;
             for (int j = 0; j < 4; ++j) { cx[j] = cc[2 * j]; cy[j] = cc[2 * j + 1]; }
         } else {
-            draw_minimal_set(a.seed, (uint32_t)(it.h * a.hyp_stride + a.hyp_offset), (uint32_t)t, P.W, P.H, cx, cy);
+            draw_minimal_set(sample_seed<DEV>(a), (uint32_t)(it.h * a.hyp_stride + a.hyp_offset), (uint32_t)t, P.W, P.H, cx, cy);
         }
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -185,7 +214,8 @@ __device__ __forceinline__ void prefilter_issue(const SampleArgs& a, long long i
 // The stage is bound by register capacity x dependency-chain latency: an SM holds 1024 tries in flight (64 registers per
 // try) whatever the packing, and a try's dependent instruction chain is the same.  96 registers
 // (5 CTAs per SM) spill.
-__global__ void __launch_bounds__(kTryThreads, 4) prefilter_kernel(const __grid_constant__ SampleArgs a) {
+template <bool DEV>
+__global__ void __launch_bounds__(kTryThreads, 4) prefilter_kernel(const __grid_constant__ SampleArgsT<DEV> a) {
     TraceScope trace(a.trace, a.trace_slot);
     __shared__ float4 s_obj[2][8][kTryThreads];  // [buffer][try * 4 + point][thread]
     const int n_unres = a.st.counters[0];
@@ -196,12 +226,12 @@ __global__ void __launch_bounds__(kTryThreads, 4) prefilter_kernel(const __grid_
     const Problem& P = a.P;
     PreItem cur, nxt;
     long long item = blockIdx.x;
-    if (item < n_items) prefilter_issue(a, item, cph, span, s_obj[0], cur);
+    if (item < n_items) prefilter_issue<DEV>(a, item, cph, span, s_obj[0], cur);
     asm volatile("cp.async.commit_group;" ::: "memory");
     int buf = 0;
     for (; item < n_items; item += gridDim.x) {
         const long long ni = item + gridDim.x;
-        if (ni < n_items) prefilter_issue(a, ni, cph, span, s_obj[buf ^ 1], nxt);
+        if (ni < n_items) prefilter_issue<DEV>(a, ni, cph, span, s_obj[buf ^ 1], nxt);
         asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group 1;" ::: "memory");  // everything but the group just committed has landed
         bool pass0 = false, pass1 = false;
@@ -213,12 +243,14 @@ __global__ void __launch_bounds__(kTryThreads, 4) prefilter_kernel(const __grid_
                 obj0[j][0] = v0.x; obj0[j][1] = v0.y; obj0[j][2] = v0.z;
                 obj1[j][0] = v1.x; obj1[j][1] = v1.y; obj1[j][2] = v1.z;
                 const unsigned c0 = cur.cell[j], c1 = cur.cell[4 + j];
-                img0[j][0] = (float)((int)(c0 & 0xffffu) * P.sub + P.sub / 2 - P.shiftX);
-                img0[j][1] = (float)((int)(c0 >> 16) * P.sub + P.sub / 2 - P.shiftY);
-                img1[j][0] = (float)((int)(c1 & 0xffffu) * P.sub + P.sub / 2 - P.shiftX);
-                img1[j][1] = (float)((int)(c1 >> 16) * P.sub + P.sub / 2 - P.shiftY);
+                img0[j][0] = (float)((int)(c0 & 0xffffu) * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, a));
+                img0[j][1] = (float)((int)(c0 >> 16) * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, a));
+                img1[j][0] = (float)((int)(c1 & 0xffffu) * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, a));
+                img1[j][1] = (float)((int)(c1 >> 16) * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, a));
             }
-            if (a.use_prefilter) p3p_may_pass_fast2(obj0, img0, obj1, img1, P.f, P.ppx, P.ppy, P.tau, pass0, pass1);
+            if (a.use_prefilter)
+                p3p_may_pass_fast2(obj0, img0, obj1, img1, dev_f<DEV>(P, a), dev_ppx<DEV>(P, a), dev_ppy<DEV>(P, a), P.tau,
+                                   pass0, pass1);
             else pass0 = pass1 = true;
             pass0 = pass0 && cur.valid0;
             pass1 = pass1 && cur.valid1;
@@ -251,7 +283,8 @@ __global__ void __launch_bounds__(kTryThreads, 4) prefilter_kernel(const __grid_
 __device__ void advance_wave(const SampleState& st, int limit, float window, float tail_boost);
 
 // ---- wave phase 2: exact fp64 verdict on the survivors -------------------------------------------------------
-__global__ void __launch_bounds__(128) exact_kernel(const __grid_constant__ SampleArgs a) {
+template <bool DEV>
+__global__ void __launch_bounds__(128) exact_kernel(const __grid_constant__ SampleArgsT<DEV> a) {
     TraceScope trace(a.trace, a.trace_slot);
     const int n = min(a.st.counters[1], a.st.cap);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
@@ -260,7 +293,7 @@ __global__ void __launch_bounds__(128) exact_kernel(const __grid_constant__ Samp
         Pose pose;
         int cx[4], cy[4];
         bool solved;
-        if (exact_try(a, ht.x, ht.y, pose, cx, cy, solved, true)) {
+        if (exact_try<DEV>(a, ht.x, ht.y, pose, cx, cy, solved, true)) {
             // stage the accepted pose so that emit_kernel does not have to solve it again
             unsigned slot = (unsigned)atomicAdd(&a.st.counters[2], 1);
             if (slot < (unsigned)a.st.cap_acc) {
@@ -333,7 +366,8 @@ __device__ void advance_wave(const SampleState& st, int limit, float window, flo
 }
 
 // ---- tail: CTA per unresolved hypothesis, both phases inside the CTA, up to the try limit --------------------
-__global__ void __launch_bounds__(kTryThreads) tail_kernel(const __grid_constant__ SampleArgs a) {
+template <bool DEV>
+__global__ void __launch_bounds__(kTryThreads) tail_kernel(const __grid_constant__ SampleArgsT<DEV> a) {
     const int n_unres = a.st.counters[0];
     __shared__ int s_list[kTryThreads * 8];
     __shared__ int s_n, s_best;
@@ -349,8 +383,10 @@ __global__ void __launch_bounds__(kTryThreads) tail_kernel(const __grid_constant
             for (int t = base + threadIdx.x; t < base + span; t += kTryThreads) {
                 int cx[4], cy[4];
                 float obj[4][3], img[4][2];
-                load_try(a, h, t, cx, cy, obj, img);
-                if (!a.use_prefilter || p3p_may_pass_fast(obj, img, a.P.f, a.P.ppx, a.P.ppy, a.P.tau)) s_list[atomicAdd(&s_n, 1)] = t;
+                load_try<DEV>(a, h, t, cx, cy, obj, img);
+                if (!a.use_prefilter ||
+                    p3p_may_pass_fast(obj, img, dev_f<DEV>(a.P, a), dev_ppx<DEV>(a.P, a), dev_ppy<DEV>(a.P, a), a.P.tau))
+                    s_list[atomicAdd(&s_n, 1)] = t;
             }
             __syncthreads();
             const int n = s_n;
@@ -358,7 +394,7 @@ __global__ void __launch_bounds__(kTryThreads) tail_kernel(const __grid_constant
                 Pose pose;
                 int cx[4], cy[4];
                 bool solved;
-                if (exact_try(a, h, s_list[i], pose, cx, cy, solved, true)) atomicMin(&s_best, s_list[i]);
+                if (exact_try<DEV>(a, h, s_list[i], pose, cx, cy, solved, true)) atomicMin(&s_best, s_list[i]);
             }
             __syncthreads();
             if (s_best != kNoTry) break;
@@ -370,7 +406,8 @@ __global__ void __launch_bounds__(kTryThreads) tail_kernel(const __grid_constant
 
 
 // ---- emit: pose / cells / try count of every hypothesis ------------------------------------------------------
-__global__ void __launch_bounds__(64) emit_kernel(const __grid_constant__ SampleArgs a, Pose* poses, int* cells, int* tries) {
+template <bool DEV>
+__global__ void __launch_bounds__(64) emit_kernel(const __grid_constant__ SampleArgsT<DEV> a, Pose* poses, int* cells, int* tries) {
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= lane_size(a)) return;
     const int h = lane_hyp(a, k);
@@ -385,7 +422,7 @@ __global__ void __launch_bounds__(64) emit_kernel(const __grid_constant__ Sample
         for (int j = 0; j < 4; ++j) { cx[j] = ac.cells[2 * j]; cy[j] = ac.cells[2 * j + 1]; }
     } else {
         bool solved;
-        exact_try(a, h, t, pose, cx, cy, solved);
+        exact_try<DEV>(a, h, t, pose, cx, cy, solved);
         if (!solved) { for (int c = 0; c < 3; ++c) { pose.r[c] = 0; pose.t[c] = 0; } }  // safeSolvePnP failure state
     }
     poses[h] = pose;
@@ -408,20 +445,21 @@ int launch_sample(const float* coords, float4* coords4, const int* assign32, con
                   int hyp_offset, int hyp_stride, Pose* poses, int* cells, int* tries, const cudaStream_t* lanes,
                   cudaEvent_t ev_fork, const cudaEvent_t* ev_join, int split_e, const int* perm, const int* offsets,
                   const cudaEvent_t* ev_half, int span0, float window, int n_waves,
-                  unsigned long long* trace, float tail_boost) {
+                  unsigned long long* trace, float tail_boost, const DevParams* dev) {
     int launches = 0;
     cudaStream_t stream = lanes[0];
     if (!split_e) { interleave_kernel<<<sm_count * 8, 256, 0, stream>>>(coords, coords4, P.E, P.N); ++launches; }
-    SampleArgs args[4];
+    SampleArgsDev args[4];
     int bound[4];
     for (int g = 0; g < n_lanes; ++g) {
-        SampleArgs& a = args[g];
+        SampleArgsDev& a = args[g];
         a.coords4 = coords4; a.assign32 = assign32; a.P = P; a.seed = seed;
         a.limit = injected ? (max_tries < inj_T ? max_tries : inj_T) : max_tries;
         a.injected = injected; a.inj_T = inj_T; a.st = st[g]; a.use_prefilter = use_prefilter; a.hyp_offset = hyp_offset; a.hyp_stride = hyp_stride > 0 ? hyp_stride : 1;
         a.h_first = g; a.h_step = n_lanes; a.Mg = (P.M - g + n_lanes - 1) / n_lanes;
         a.perm = nullptr; a.offsets = nullptr; a.e_lo = a.e_hi = 0;
         a.span0 = span0; a.window = window; a.trace = trace; a.trace_slot = 0; a.tail_boost = tail_boost;
+        a.dev = dev ? *dev : DevParams{};
         bound[g] = a.Mg;  // host-side bound on the lane size (grid sizing)
         if (split_e) {
             a.perm = perm; a.offsets = offsets;
@@ -436,7 +474,8 @@ int launch_sample(const float* coords, float4* coords4, const int* assign32, con
     }
     for (int g = 0; g < n_lanes; ++g) {
         cudaStream_t sg = lanes[g];
-        SampleArgs& a = args[g];
+        SampleArgsDev& a = args[g];
+        const SampleArgs& ae = a;  // what the eager kernels take
         if (split_e) {
             cudaStreamWaitEvent(sg, ev_half[g], 0);
             const int ne = a.e_hi - a.e_lo;
@@ -444,18 +483,29 @@ int launch_sample(const float* coords, float4* coords4, const int* assign32, con
             ++launches;
         }
         if (bound[g] <= 0) continue;
-        sample_init_kernel<<<(bound[g] + 255) / 256, 256, 0, sg>>>(a); ++launches;
+        sample_init_kernel<<<(bound[g] + 255) / 256, 256, 0, sg>>>(ae); ++launches;
         // persistent: every CTA resident (4 x 128 threads x 128 registers fill an SM's register file), ~14 items each in a bulk wave;
         // 3 CTAs per SM + 64-thread verdict CTAs in the room that leaves was measured slower
         const int grid = sm_count * 4;
         for (int r = 0; r < n_waves; ++r) {
             a.trace_slot = (g * 32 + r) * 2;
-            prefilter_kernel<<<grid, kTryThreads, 0, sg>>>(a); ++launches;
+            if (dev) prefilter_kernel<true><<<grid, kTryThreads, 0, sg>>>(a);
+            else prefilter_kernel<false><<<grid, kTryThreads, 0, sg>>>(ae);
+            ++launches;
             a.trace_slot = (g * 32 + r) * 2 + 1;
-            exact_kernel<<<sm_count * 4, 128, 0, sg>>>(a); ++launches;  // its last CTA also advances the windows
+            if (dev) exact_kernel<true><<<sm_count * 4, 128, 0, sg>>>(a);  // its last CTA also advances the windows
+            else exact_kernel<false><<<sm_count * 4, 128, 0, sg>>>(ae);
+            ++launches;
         }
-        tail_kernel<<<bound[g] < sm_count * 4 ? bound[g] : sm_count * 4, kTryThreads, 0, sg>>>(a); ++launches;
-        emit_kernel<<<(bound[g] + 63) / 64, 64, 0, sg>>>(a, poses, cells, tries); ++launches;
+        const int tail_grid = bound[g] < sm_count * 4 ? bound[g] : sm_count * 4;
+        if (dev) {
+            tail_kernel<true><<<tail_grid, kTryThreads, 0, sg>>>(a);
+            emit_kernel<true><<<(bound[g] + 63) / 64, 64, 0, sg>>>(a, poses, cells, tries);
+        } else {
+            tail_kernel<false><<<tail_grid, kTryThreads, 0, sg>>>(ae);
+            emit_kernel<false><<<(bound[g] + 63) / 64, 64, 0, sg>>>(ae, poses, cells, tries);
+        }
+        launches += 2;
     }
     for (int g = 1; g < n_lanes; ++g) {
         cudaEventRecord(ev_join[g], lanes[g]);

@@ -640,6 +640,7 @@ __device__ __forceinline__ void root_lm_step(RefShared& sh) {
     for (int i = 0; i < 6; ++i) sh.par[i] = sh.prev[i] - dlt[i];
 }
 
+template <bool DEV>
 __global__ void __launch_bounds__(kRefThreads, 1) refine_kernel(const __grid_constant__ RefineArgs a) {
     __shared__ RefShared sh;
     extern __shared__ float cell_cache[];  // [3][kCacheCells] + the inlier list when the block's share fits (a.cache != 0)
@@ -648,7 +649,12 @@ __global__ void __launch_bounds__(kRefThreads, 1) refine_kernel(const __grid_con
     const int grp = blockIdx.x / a.group, cta = blockIdx.x - grp * a.group;
     const bool root = cta == 0;
     const int n_jobs = a.n_jobs ? *a.n_jobs : a.n_jobs_host;
-    const Problem& P = a.P;
+    Problem Pd = a.P;  // DEV: the image's shift and camera from device memory
+    if constexpr (DEV) {
+        Pd.shiftX = dev_shift_x<DEV>(a.P, a); Pd.shiftY = dev_shift_y<DEV>(a.P, a);
+        Pd.f = dev_f<DEV>(a.P, a); Pd.ppx = dev_ppx<DEV>(a.P, a); Pd.ppy = dev_ppy<DEV>(a.P, a);
+    }
+    const Problem& P = DEV ? Pd : a.P;
     const int words = (P.N + 31) / 32;
     const int wpc = (words + a.group - 1) / a.group;
     const int w0 = min(words, cta * wpc), w1 = min(words, w0 + wpc);
@@ -866,10 +872,11 @@ void launch_refine(const RefineArgs& a, int n_groups, cudaStream_t st) {
     dim3 grid(n_groups * a.group), block(kRefThreads);
     const size_t smem = a.cache ? refine_cache_bytes() : 0;
     void* params[] = {(void*)&a};
+    const void* fn = a.dev.shift ? (const void*)refine_kernel<true> : (const void*)refine_kernel<false>;
     // above the 48 KB a kernel gets without asking; the attribute is per device, so it is set on every launch (it is cheap)
-    cudaFuncSetAttribute((const void*)refine_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)refine_cache_bytes());
-    if (a.group > 1) cudaLaunchCooperativeKernel((const void*)refine_kernel, grid, block, params, smem, st);
-    else cudaLaunchKernel((const void*)refine_kernel, grid, block, params, smem, st);
+    cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)refine_cache_bytes());
+    if (a.group > 1) cudaLaunchCooperativeKernel(fn, grid, block, params, smem, st);
+    else cudaLaunchKernel(fn, grid, block, params, smem, st);
 }
 
 int refine_cache_words() { return kCacheWords; }
@@ -881,8 +888,8 @@ size_t refine_flag_words(int n_groups, int group) { return (size_t)n_groups * (g
 
 int refine_max_coresident_blocks(int sm_count) {
     int nb = 0;
-    cudaFuncSetAttribute((const void*)refine_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)refine_cache_bytes());
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, refine_kernel, kRefThreads, refine_cache_bytes()) != cudaSuccess) {
+    cudaFuncSetAttribute((const void*)refine_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)refine_cache_bytes());
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, refine_kernel<false>, kRefThreads, refine_cache_bytes()) != cudaSuccess) {
         cudaGetLastError();
         nb = 1;
     }
@@ -900,6 +907,27 @@ __global__ void finish_forward_kernel(const Pose* poses, const int* winner, cons
         out[17] = (float)flags[0];
         out[18] = (float)w;
     }
+}
+
+// finish_forward_kernel's pose and expert, written to the caller's arrays of a stream-ordered forward; a bad assignment
+// gives a NaN pose, expert -1 and status 1.  The last image of an execution advances the async call counter.
+__global__ void finish_forward_async_kernel(const Pose* poses, const int* winner, const int* assign32, const int* flags,
+                                            float* pose16, long long* expert, int* status, unsigned long long* seed, int advance) {
+    if (threadIdx.x == 0) {
+        const int w = *winner;
+        const int bad = flags[0];
+        double T[16];
+        pose2trans(poses[w], T);
+        for (int i = 0; i < 16; ++i) pose16[i] = bad ? __int_as_float(0x7fffffff) : (float)T[i];
+        *expert = bad ? -1 : (long long)assign32[w];
+        *status = bad;
+        if (advance) seed[1] += (unsigned long long)advance;
+    }
+}
+
+__global__ void seed_reset_kernel(unsigned long long* seed, unsigned long long base) {
+    seed[0] = base;
+    seed[1] = 0;
 }
 
 // Record one shard contributes to the all-gather of the sharded forward (SURVEY 8e), as doubles:
@@ -980,6 +1008,15 @@ __global__ void __launch_bounds__(256) select_gathered_kernel(const double* __re
 
 void launch_select_gathered(const double* gathered, int world, int M_pad, float* out20, cudaStream_t st) {
     select_gathered_kernel<<<1, 256, 0, st>>>(gathered, world, M_pad, out20);
+}
+
+void launch_finish_forward_async(const Pose* poses, const int* winner, const int* assign32, const int* flags, float* pose16,
+                                 long long* expert, int* status, unsigned long long* seed, int advance, cudaStream_t st) {
+    finish_forward_async_kernel<<<1, 32, 0, st>>>(poses, winner, assign32, flags, pose16, expert, status, seed, advance);
+}
+
+void launch_seed_reset(unsigned long long* seed, unsigned long long base, cudaStream_t st) {
+    seed_reset_kernel<<<1, 1, 0, st>>>(seed, base);
 }
 
 void launch_finish_forward(const Pose* poses, const int* winner, const int* assign32, const int* flags, float* out20,

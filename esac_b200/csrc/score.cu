@@ -128,8 +128,9 @@ void launch_prep(const float* coords, const long long* assign, long long assign_
 // ---------------------------------------------------------------------------------------------
 // fold: (rvec, tvec) fp64 -> fp32 rows of diag(f,f,1) R and diag(f,f,1)(R c + t), slot order
 // ---------------------------------------------------------------------------------------------
+template <bool DEV>
 __global__ void fold_kernel(const Pose* __restrict__ poses, const int* __restrict__ perm, const int* __restrict__ assign32,
-                            const float* __restrict__ centres, Problem P, float kf, PosePk* __restrict__ out) {
+                            const float* __restrict__ centres, Problem P, float kf, PosePk* __restrict__ out, DevParams dev) {
     int s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= P.M) return;
     int h = perm[s];
@@ -138,7 +139,9 @@ __global__ void fold_kernel(const Pose* __restrict__ poses, const int* __restric
     double R[9];
     rodrigues_v2m(p.r, R, nullptr);
     double c[3] = {(double)centres[e * 3], (double)centres[e * 3 + 1], (double)centres[e * 3 + 2]};
-    const double f = (double)P.f * (double)kf;  // kf = k1 when the scoring kernel folds it, else 1
+    float focal = P.f;
+    if constexpr (DEV) focal = __ldg(dev.cam);
+    const double f = (double)focal * (double)kf;  // kf = k1 when the scoring kernel folds it, else 1
     float A[12];
     for (int r = 0; r < 3; ++r) {
         double sc = r < 2 ? f : 1.0;
@@ -154,8 +157,9 @@ __global__ void fold_kernel(const Pose* __restrict__ poses, const int* __restric
 }
 
 void launch_fold(const Pose* poses, const int* perm, const int* assign32, const float* centres, const Problem& P,
-                 float kf, PosePk* out, cudaStream_t st) {
-    fold_kernel<<<(P.M + 127) / 128, 128, 0, st>>>(poses, perm, assign32, centres, P, kf, out);
+                 float kf, PosePk* out, cudaStream_t st, const DevParams* dev) {
+    if (dev) fold_kernel<true><<<(P.M + 127) / 128, 128, 0, st>>>(poses, perm, assign32, centres, P, kf, out, *dev);
+    else fold_kernel<false><<<(P.M + 127) / 128, 128, 0, st>>>(poses, perm, assign32, centres, P, kf, out, DevParams{});
 }
 
 void score_constants(const Problem& P, ScoreArgs& a) {
@@ -196,7 +200,7 @@ __device__ __forceinline__ float mufu_rcp(float x) {
 
 // tileX/Y/Z: when non-null, the tile's three coordinate rows already sit in shared memory (staged by TMA bulk copies);
 // otherwise the cells are read from global memory.
-template <int PPT, bool TAIL, bool FOLD>
+template <int PPT, bool TAIL, bool FOLD, bool DEV>
 __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc cd, const int tile, const float4* sPose,
                                            float (*sWarp)[kMaxChunk], const float* tileX = nullptr,
                                            const float* tileY = nullptr, const float* tileZ = nullptr) {
@@ -261,8 +265,8 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
             int p = p0 + i;
             int py = p / P.W, px = p - py * P.W;
             // createSampling (esac_util.h:64-66): integer pixel centre, then ppoint - pixel in float
-            aa[i] = P.ppx - (float)(px * P.sub + P.sub / 2 - P.shiftX);
-            bb[i] = P.ppy - (float)(py * P.sub + P.sub / 2 - P.shiftY);
+            aa[i] = dev_ppx<DEV>(P, a) - (float)(px * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, a));
+            bb[i] = dev_ppy<DEV>(P, a) - (float)(py * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, a));
             if (FOLD) { aa[i] = __fmul_rn(aa[i], a.k1); bb[i] = __fmul_rn(bb[i], a.k1); }
             vv[i] = (p < P.N) ? 1.f : 0.f;
             x[i] -= cX; y[i] -= cY; z[i] -= cZ;
@@ -366,7 +370,7 @@ __device__ __forceinline__ void score_item(const ScoreArgs& a, const ChunkDesc c
     }
 }
 
-template <int PPT, bool FOLD>
+template <int PPT, bool FOLD, bool DEV>
 __global__ void __launch_bounds__(kScoreThreads, 2) score_kernel(const __grid_constant__ ScoreArgs a) {
     __shared__ float4 sPose[kMaxChunk * 3];
     __shared__ float sWarp[kScoreThreads / 32][kMaxChunk];
@@ -386,8 +390,8 @@ __global__ void __launch_bounds__(kScoreThreads, 2) score_kernel(const __grid_co
         const float4* src = (const float4*)(a.poses + cd.slot0);
         for (int i = tid; i < cd.count * 3; i += kScoreThreads) sPose[i] = src[i];
         __syncthreads();
-        if (ragged && tile == a.T - 1) score_item<PPT, true, FOLD>(a, cd, tile, sPose, sWarp);
-        else score_item<PPT, false, FOLD>(a, cd, tile, sPose, sWarp);
+        if (ragged && tile == a.T - 1) score_item<PPT, true, FOLD, DEV>(a, cd, tile, sPose, sWarp);
+        else score_item<PPT, false, FOLD, DEV>(a, cd, tile, sPose, sWarp);
         __syncthreads();
     }
 }
@@ -419,7 +423,7 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst, const void* src, uint32_
                  : "memory");
 }
 
-template <int PPT, bool FOLD>
+template <int PPT, bool FOLD, bool DEV>
 __global__ void __launch_bounds__(kScoreThreads, 2) score_kernel_tma(const __grid_constant__ ScoreArgs a) {
     constexpr int TP = kScoreThreads * PPT;
     extern __shared__ __align__(128) float sTile[];  // [2 stages][3 rows][TP]
@@ -474,8 +478,8 @@ __global__ void __launch_bounds__(kScoreThreads, 2) score_kernel_tma(const __gri
         phase[stage] ^= 1u;
         __syncthreads();
         const float* tx = sTile + (size_t)stage * 3 * TP;
-        if (ragged && tile == a.T - 1) score_item<PPT, true, FOLD>(a, cd, tile, sPose, sWarp, tx, tx + TP, tx + 2 * TP);
-        else score_item<PPT, false, FOLD>(a, cd, tile, sPose, sWarp, tx, tx + TP, tx + 2 * TP);
+        if (ragged && tile == a.T - 1) score_item<PPT, true, FOLD, DEV>(a, cd, tile, sPose, sWarp, tx, tx + TP, tx + 2 * TP);
+        else score_item<PPT, false, FOLD, DEV>(a, cd, tile, sPose, sWarp, tx, tx + TP, tx + 2 * TP);
         __syncthreads();  // everyone is done with this stage, sPose, sWarp and has read sItem[stage ^ 1]'s predecessor
     }
 }
@@ -484,34 +488,35 @@ int score_tile_pixels(int ppt) { return kScoreThreads * ppt; }
 
 constexpr int kMaxDevices = 64;
 
-template <bool FOLD>
+template <bool FOLD, bool DEV>
 void launch_score_t(const ScoreArgs& a, int ppt, int grid, cudaStream_t st) {
     if (a.vec_ok && ppt >= 4) {  // TMA path (bulk copies need 16-byte granularity)
         const size_t smem = (size_t)2 * 3 * kScoreThreads * ppt * sizeof(float);
         // The opt-in above 48 KB of dynamic shared memory is a per-DEVICE function attribute (one process may hold contexts
         // on several GPUs, api.context(device)), and launches may come from several host threads (backward_batch workers).
-        static std::atomic<unsigned char> attr_set[kMaxDevices][2];  // one table per FOLD instantiation
+        static std::atomic<unsigned char> attr_set[kMaxDevices][2];  // one table per FOLD / DEV instantiation
         int dev = 0;
         cudaGetDevice(&dev);
         const int which = ppt == 8 ? 0 : 1;
         const bool known = dev >= 0 && dev < kMaxDevices;
         if (!known || !attr_set[dev][which].load(std::memory_order_acquire)) {
-            if (ppt == 8) cudaFuncSetAttribute(score_kernel_tma<8, FOLD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            else cudaFuncSetAttribute(score_kernel_tma<4, FOLD>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (ppt == 8) cudaFuncSetAttribute(score_kernel_tma<8, FOLD, DEV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            else cudaFuncSetAttribute(score_kernel_tma<4, FOLD, DEV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (known) attr_set[dev][which].store(1, std::memory_order_release);
         }
-        if (ppt == 8) score_kernel_tma<8, FOLD><<<grid, kScoreThreads, smem, st>>>(a);
-        else score_kernel_tma<4, FOLD><<<grid, kScoreThreads, smem, st>>>(a);
+        if (ppt == 8) score_kernel_tma<8, FOLD, DEV><<<grid, kScoreThreads, smem, st>>>(a);
+        else score_kernel_tma<4, FOLD, DEV><<<grid, kScoreThreads, smem, st>>>(a);
         return;
     }
-    if (ppt == 8) score_kernel<8, FOLD><<<grid, kScoreThreads, 0, st>>>(a);
-    else if (ppt == 4) score_kernel<4, FOLD><<<grid, kScoreThreads, 0, st>>>(a);
-    else score_kernel<2, FOLD><<<grid, kScoreThreads, 0, st>>>(a);
+    if (ppt == 8) score_kernel<8, FOLD, DEV><<<grid, kScoreThreads, 0, st>>>(a);
+    else if (ppt == 4) score_kernel<4, FOLD, DEV><<<grid, kScoreThreads, 0, st>>>(a);
+    else score_kernel<2, FOLD, DEV><<<grid, kScoreThreads, 0, st>>>(a);
 }
 
 void launch_score(const ScoreArgs& a, int ppt, int grid, cudaStream_t st) {
-    if (a.fold) launch_score_t<true>(a, ppt, grid, st);
-    else launch_score_t<false>(a, ppt, grid, st);
+    const bool dev = a.dev.shift != nullptr;
+    if (a.fold) dev ? launch_score_t<true, true>(a, ppt, grid, st) : launch_score_t<true, false>(a, ppt, grid, st);
+    else dev ? launch_score_t<false, true>(a, ppt, grid, st) : launch_score_t<false, false>(a, ppt, grid, st);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -211,6 +211,37 @@ int esacb200_forward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords
                                    const float* f, const float* ppx, const float* ppy, float inlierThreshold, float inlierAlpha,
                                    float inlierBeta, float maxReproj, int subSampling, int* out_experts);
 
+/* Stream-ordered esac_forward that a CUDA graph can capture.  DEVICE pointers only (a host pointer is an error, reported
+ * before anything is enqueued): coords float32 [B,E,3,H,W], assign int64 [B,M] (rows contiguous, element stride
+ * assign_stride), shifts int32 [B,2] (shiftX, shiftY), cameras float32 [B,3] (f, ppx, ppy); results out_poses float32
+ * [B,4,4] camera->world, out_experts int64 [B], out_status int32 [B].  Status 0 = OK; 1 = the image's assignment held an
+ * expert index outside [0,E): its pose is NaN and its expert -1, the other images are unaffected.  B = 1 is one image.
+ *
+ * The call enqueues on the context's stream and returns: no host synchronisation, no read-back, no event query, and while
+ * the stream is being captured (cudaStreamBeginCapture, any capture mode) no allocation.  The seed, shift and camera of
+ * every image are read from device memory when the kernels run, so a graph that captured the call replays with the values
+ * the arrays hold at replay time.
+ *
+ * Seeding: the base seed and a call counter live in device memory; an execution reads them and advances the counter by B.
+ * esacb200_set_seed resets both, enqueued on the context's stream (a set_seed after a capture applies from the next
+ * replay).  Image b of the j-th execution after set_seed(s) draws what the (j*B + b)-th esacb200_forward after set_seed(s)
+ * draws, option "fixed_seed" included (its value at enqueue / capture time).  Eager and stream-ordered calls count apart.
+ *
+ * Workspace: the stream-ordered forward has a workspace of its own, apart from the one the eager calls grow, so eager
+ * calls of any shape leave a captured graph's buffers alone.  An uncaptured call grows it as needed; a captured call cannot
+ * (that would allocate), so call esacb200_reserve_forward_async with the largest shape before the first capture.  Once a
+ * capture has used the workspace nothing in it is freed or reallocated again: a later call or reserve that needs more
+ * fails, before enqueuing anything, with a message that names the reserve call.
+ *
+ * The stage timers of esacb200_get_stats are neither recorded nor updated by these calls. */
+int esacb200_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
+                           int64_t assign_stride, int M, const int32_t* shifts, const float* cameras, float inlierThreshold,
+                           float inlierAlpha, float inlierBeta, float maxReproj, int subSampling, float* out_poses,
+                           int64_t* out_experts, int32_t* out_status);
+/* Sizes the stream-ordered forward's workspace for calls of this shape (and creates its state); allocates, so it may not
+ * run while the context's stream is being captured.  B does not change the workspace: the images run one after another. */
+int esacb200_reserve_forward_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int subSampling);
+
 /* esac_backward over B images of one shape (the reference trains with batch_size=1, train_esac.py:96-100, one
  * esac.backward per image): coords / grads float32 [B,E,3,H,W] (grads accumulated in place, as esac.cpp:490-508),
  * assign int64 [B,M] (as in esacb200_forward_batch), gt_poses float32 [B,4,4] (camera->world), shiftX / shiftY int [B]

@@ -13,6 +13,7 @@
 #include <algorithm>
 #include <exception>
 #include <functional>
+#include <map>
 #include <new>
 #include <string>
 #include <vector>
@@ -29,9 +30,16 @@ using namespace esacb200;
 
 namespace {
 
+// A device buffer that owns its memory: freed when the buffer dies (the owner destroys it on its device, after its stream).
 struct DevBuf {
     void* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() {
+        if (p) cudaFree(p);
+    }
     cudaError_t ensure(size_t bytes) {
         if (bytes <= cap) return cudaSuccess;
         if (p) cudaFree(p);
@@ -42,13 +50,31 @@ struct DevBuf {
         if (e == cudaSuccess) cap = want;
         return e;
     }
-    void release() {
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-    }
     template <class T>
     T* as() const { return (T*)p; }
+};
+
+// The tunables of esacb200_set_option.
+struct Options {
+    int max_tries = 1000000;
+    int max_ref_steps = 100;
+    int fixed_seed = 0;
+    int refine_group_opt = 0;
+    int refine_pretest = 1;    // inlier selection: float pretest with a rounding-error bound, exact arithmetic only where in doubt
+    int refine_compact = 1;    // LM evaluations over per-CTA inlier lists instead of predicated passes over all cells
+    int refine_profile = 0;    // 1: block 0 of the refinement kernel records phase cycle counts (esacb200_get_refine_profile)
+    int refine_jobs_per_group = 3;
+    int sample_prefilter = 1;
+    int sample_span0 = 256;       // tries per hypothesis in the first wave (a multiple of the 256-try pass of a prefilter CTA)
+    float sample_window = 1.25f;  // later waves: window / acceptance rate
+    int sample_waves = 6;         // launched unconditionally (empty ones cost ~6 us each); what is left after them goes to tail_kernel
+    float sample_tail_boost = 1.f;  // window factor once <= 64 hypotheses are left in a lane (x2 more for <= 8)
+    int sample_trace = 0;         // 1: prefilter / exact kernels stamp first-CTA-start / last-CTA-end times (esacb200_get_sample_trace)
+    int sample_groups = 2;        // lanes of the sampling stage (third and fourth lane: no gain measured)
+    int upload_split = 1;
+    int hyp_offset = 0, hyp_stride = 1;
+    int score_ppt_opt = 0, score_hc_opt = 0;
+    int batch_workers = 8;
 };
 
 enum { EV_START = 0, EV_H2D, EV_PREP, EV_SAMPLE, EV_FOLD, EV_SCORE, EV_SELECT, EV_REFINE, EV_BWD, EV_END, EV_COUNT };
@@ -62,34 +88,17 @@ struct esacb200_ctx {
     cudaStream_t own_stream = nullptr;
     cudaStream_t copy_stream = nullptr;
     cudaStream_t aux_stream = nullptr;   // second lane of the sampling stage
-    cudaStream_t aux_more[2] = {nullptr, nullptr};  // third and fourth lane (option sample_groups; no gain measured)
+    cudaStream_t aux_more[2] = {nullptr, nullptr};  // third and fourth lane (option sample_groups)
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr, ev_join_more[2] = {nullptr, nullptr};
-    int sample_groups = 2;
-    int upload_split = 1;
     cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_consumed[2] = {nullptr, nullptr};
     cudaStream_t stream = nullptr;
     uint64_t seed = 1305;  // thread_rand.h:103
     uint64_t calls = 0;
-    int max_tries = 1000000;
-    int max_ref_steps = 100;
-    int fixed_seed = 0;
-    int refine_group_opt = 0;
+    Options opt;
     int* h_flags = nullptr;    // pinned: per-expert "receives gradient on some rank" flags (hypothesis-major sharding)
     int h_flags_cap = 0;
-    int refine_pretest = 1;    // inlier selection: float pretest with a rounding-error bound, exact arithmetic only where in doubt
-    int refine_compact = 1;    // LM evaluations over per-CTA inlier lists instead of predicated passes over all cells
-    int refine_profile = 0;    // 1: block 0 of the refinement kernel records phase cycle counts (esacb200_get_refine_profile)
-    int refine_jobs_per_group = 3;
-    int sample_prefilter = 1;
-    int sample_span0 = 256;       // tries per hypothesis in the first wave (a multiple of the 256-try pass of a prefilter CTA)
-    float sample_window = 1.25f;  // later waves: window / acceptance rate
-    int sample_waves = 6;         // launched unconditionally (empty ones cost ~6 us each); what is left after them goes to tail_kernel
-    float sample_tail_boost = 1.f;  // window factor once <= 64 hypotheses are left in a lane (x2 more for <= 8)
-    int sample_trace = 0;         // 1: prefilter / exact kernels stamp first-CTA-start / last-CTA-end times (esacb200_get_sample_trace)
     int smp_groups_last = 0;      // lanes of the last run_sample (diagnostics read-back)
     int smp_Mg_last = 0;
-    int hyp_offset = 0, hyp_stride = 1;
-    int score_ppt_opt = 0, score_hc_opt = 0;
     int refine_coresident = 0;
     char err[512] = {0};
     // workspace
@@ -105,7 +114,6 @@ struct esacb200_ctx {
     esacb200_stats st;
     int last_M = 0;
     bool last_backward = false;
-    int batch_workers = 8;
     // NCCL communicator of the sharded entry points (esacb200_comm_init); the library is resolved at run time with dlopen
     void* nccl_comm = nullptr;
     int comm_world = 1, comm_rank = 0;
@@ -259,19 +267,41 @@ int fill_problem(esacb200_ctx* ctx, Problem& P, int E, int H, int W, int M, int 
     return 0;
 }
 
+// ---- workspace of the forward pipeline --------------------------------------------------------------------------
+// Each stage states the sizes of its buffers in one function that calls `need(buf, bytes)` once per buffer: the stage
+// itself grows them (grow), and forward_workspace sizes or checks them for a whole batch before anything is enqueued.
+#define NEED(buf, bytes) do { int r__ = need(buf, bytes); if (r__) return r__; } while (0)
+
+auto grow(esacb200_ctx* ctx) {
+    return [ctx](DevBuf& b, size_t bytes) -> int {
+        CK(b.ensure(bytes));
+        return 0;
+    };
+}
+
+// Input staging: a host coordinate map goes to `cbuf`, host assignments to `abuf` (null: that input is not staged).
+template <class Need>
+int input_buffers(const Problem& P, DevBuf* cbuf, DevBuf* abuf, Need&& need) {
+    if (cbuf) NEED(*cbuf, (size_t)P.E * 3 * P.N * sizeof(float));
+    if (abuf) NEED(*abuf, (size_t)P.M * 8);
+    return 0;
+}
+
 // Upload (or alias) the inputs.  Host coordinate maps go to `cbuf` on `copy_stream` (pinned memory: asynchronous).
 int upload_inputs(esacb200_ctx* ctx, Plan& pl, const float* coords, const int64_t* assign, int64_t stride, DevBuf& cbuf,
                   DevBuf& abuf, cudaStream_t copy_stream, bool allow_split = false) {
     const Problem& P = pl.P;
     const size_t cbytes = (size_t)P.E * 3 * P.N * sizeof(float);
+    const bool dev_coords = is_device_ptr(coords), dev_assign = is_device_ptr(assign);
+    int rc = input_buffers(P, dev_coords ? nullptr : &cbuf, dev_assign ? nullptr : &abuf, grow(ctx));
+    if (rc) return rc;
     pl.split_e = 0;
-    if (is_device_ptr(coords)) {
+    if (dev_coords) {
         pl.d_coords = coords;
-    } else if (allow_split && P.E >= 2 && cbytes >= (size_t)(4 << 20) && P.M >= 64 && ctx->aux_stream && ctx->sample_groups > 1 &&
-               ctx->upload_split) {
+    } else if (allow_split && P.E >= 2 && cbytes >= (size_t)(4 << 20) && P.M >= 64 && ctx->aux_stream && ctx->opt.sample_groups > 1 &&
+               ctx->opt.upload_split) {
         // Large host maps: two halves on the copy stream, so the first half's experts are sampled while the second half is
         // still on the wire (launch_sample deals its two lanes by expert in this case).
-        CK(cbuf.ensure(cbytes));
         const int es = (P.E + 1) / 2;
         const size_t first = (size_t)es * 3 * P.N * sizeof(float);
         CK(cudaMemcpyAsync(cbuf.p, coords, first, cudaMemcpyHostToDevice, ctx->copy_stream));
@@ -281,17 +311,15 @@ int upload_inputs(esacb200_ctx* ctx, Plan& pl, const float* coords, const int64_
         pl.d_coords = cbuf.as<float>();
         pl.split_e = es;
     } else {
-        CK(cbuf.ensure(cbytes));
         CK(cudaMemcpyAsync(cbuf.p, coords, cbytes, cudaMemcpyHostToDevice, copy_stream));
         pl.d_coords = cbuf.as<float>();
     }
-    if (is_device_ptr(assign)) {
+    if (dev_assign) {
         pl.d_assign = (const long long*)assign;
         pl.assign_stride = stride;
     } else {
         std::vector<long long> tmp((size_t)P.M);
         for (int h = 0; h < P.M; ++h) tmp[h] = (long long)assign[(long long)h * stride];
-        CK(abuf.ensure((size_t)P.M * 8));
         // pageable source: the copy is staged before cudaMemcpyAsync returns, so tmp may die
         CK(cudaMemcpyAsync(abuf.p, tmp.data(), (size_t)P.M * 8, cudaMemcpyHostToDevice, copy_stream));
         pl.d_assign = abuf.as<long long>();
@@ -313,8 +341,9 @@ void plan_launch(esacb200_ctx* ctx, Plan& pl) {
     };
     if (items(8, 64) < want) { ppt = 4; hc = 32; }
     if (ppt == 4 && items(4, 32) < want) { ppt = 2; hc = 16; }
-    if (ctx->score_ppt_opt == 2 || ctx->score_ppt_opt == 4 || ctx->score_ppt_opt == 8) ppt = ctx->score_ppt_opt;
-    if (ctx->score_hc_opt > 0) hc = ctx->score_hc_opt < 64 ? ctx->score_hc_opt : 64;
+    const int ppt_opt = ctx->opt.score_ppt_opt, hc_opt = ctx->opt.score_hc_opt;
+    if (ppt_opt == 2 || ppt_opt == 4 || ppt_opt == 8) ppt = ppt_opt;
+    if (hc_opt > 0) hc = hc_opt < 64 ? hc_opt : 64;
     pl.ppt = ppt;
     pl.hc = hc;
     pl.T = (P.N + score_tile_pixels(ppt) - 1) / score_tile_pixels(ppt);
@@ -325,29 +354,38 @@ void plan_launch(esacb200_ctx* ctx, Plan& pl) {
     pl.vec_ok = (P.N % need_align == 0) && (((uintptr_t)pl.d_coords) % (need_align * 4) == 0);
 }
 
+// Prep, scoring and selection: per-hypothesis state and the scoring partials (pl.T: plan_launch first).
+template <class Need>
+int prep_buffers(esacb200_ctx* ctx, const Plan& pl, Need&& need) {
+    const Problem& P = pl.P;
+    NEED(ctx->assign32, (size_t)P.M * 4);
+    NEED(ctx->counts, (size_t)P.E * 4);
+    NEED(ctx->offsets, (size_t)(P.E + 1) * 4);
+    NEED(ctx->perm, (size_t)P.M * 4);
+    NEED(ctx->slot_of, (size_t)P.M * 4);
+    NEED(ctx->chunks, (size_t)(P.M + P.E) * sizeof(ChunkDesc));
+    NEED(ctx->scalars, S_COUNT * 4);
+    NEED(ctx->centres, (size_t)P.E * 3 * 4);
+    NEED(ctx->poses, (size_t)P.M * sizeof(Pose));
+    NEED(ctx->poses_ref, (size_t)P.M * sizeof(Pose));
+    NEED(ctx->cells, (size_t)P.M * 8 * 4);
+    NEED(ctx->tries, (size_t)P.M * 4);
+    NEED(ctx->posepk, (size_t)P.M * sizeof(PosePk));
+    NEED(ctx->part, (size_t)P.M * pl.T * 4);
+    NEED(ctx->scores, (size_t)P.M * 8);
+    NEED(ctx->probs, (size_t)P.M * 8);
+    NEED(ctx->stats, 8 * 8);
+    NEED(ctx->contrib, (size_t)P.M * 4);
+    NEED(ctx->out17, 32 * 4);
+    return 0;
+}
+
 // Scoring launch shape, workspace, prep kernel.
 int plan_and_prep(esacb200_ctx* ctx, Plan& pl) {
     const Problem& P = pl.P;
     plan_launch(ctx, pl);
-    CK(ctx->assign32.ensure((size_t)P.M * 4));
-    CK(ctx->counts.ensure((size_t)P.E * 4));
-    CK(ctx->offsets.ensure((size_t)(P.E + 1) * 4));
-    CK(ctx->perm.ensure((size_t)P.M * 4));
-    CK(ctx->slot_of.ensure((size_t)P.M * 4));
-    CK(ctx->chunks.ensure((size_t)(P.M + P.E) * sizeof(ChunkDesc)));
-    CK(ctx->scalars.ensure(S_COUNT * 4));
-    CK(ctx->centres.ensure((size_t)P.E * 3 * 4));
-    CK(ctx->poses.ensure((size_t)P.M * sizeof(Pose)));
-    CK(ctx->poses_ref.ensure((size_t)P.M * sizeof(Pose)));
-    CK(ctx->cells.ensure((size_t)P.M * 8 * 4));
-    CK(ctx->tries.ensure((size_t)P.M * 4));
-    CK(ctx->posepk.ensure((size_t)P.M * sizeof(PosePk)));
-    CK(ctx->part.ensure((size_t)P.M * pl.T * 4));
-    CK(ctx->scores.ensure((size_t)P.M * 8));
-    CK(ctx->probs.ensure((size_t)P.M * 8));
-    CK(ctx->stats.ensure(8 * 8));
-    CK(ctx->contrib.ensure((size_t)P.M * 4));
-    CK(ctx->out17.ensure(32 * 4));
+    int rc = prep_buffers(ctx, pl, grow(ctx));
+    if (rc) return rc;
     int* sc = ctx->scalars.as<int>();
     launch_prep(pl.d_coords, pl.d_assign, pl.assign_stride, P, pl.hc, ctx->assign32.as<int>(), ctx->counts.as<int>(),
                 ctx->offsets.as<int>(), ctx->perm.as<int>(), ctx->slot_of.as<int>(), ctx->chunks.as<ChunkDesc>(),
@@ -376,7 +414,8 @@ SampleSizes sample_sizes(const esacb200_ctx* ctx, const Plan& pl) {
     const Problem& P = pl.P;
     SampleSizes z;
     // two lanes pay once a wave's kernels are long enough to overlap (full-resolution maps, or very many hypotheses)
-    int G = pl.split_e ? 2 : ((ctx->sample_groups > 1 && ctx->aux_stream && P.M >= 64 && (P.N >= 65536 || P.M >= 1024)) ? ctx->sample_groups : 1);
+    const int groups = ctx->opt.sample_groups;
+    int G = pl.split_e ? 2 : ((groups > 1 && ctx->aux_stream && P.M >= 64 && (P.N >= 65536 || P.M >= 1024)) ? groups : 1);
     if (G > 2 && (!ctx->aux_more[0] || !ctx->aux_more[1] || P.M < 512)) G = 2;
     z.G = G;
     z.Mg = pl.split_e ? P.M : (P.M + G - 1) / G;  // capacity of a lane's work list
@@ -388,15 +427,26 @@ SampleSizes sample_sizes(const esacb200_ctx* ctx, const Plan& pl) {
     return z;
 }
 
+// Sampling: the lanes' state and the float4 copy of the maps.
+template <class Need>
+int sample_buffers(esacb200_ctx* ctx, const Plan& pl, Need&& need) {
+    const SampleSizes z = sample_sizes(ctx, pl);
+    NEED(ctx->smp_int, z.int_bytes);
+    NEED(ctx->smp_surv, z.surv_bytes);
+    NEED(ctx->coords4, (size_t)pl.P.E * pl.P.N * sizeof(float4));
+    return 0;
+}
+
 int run_sample(esacb200_ctx* ctx, const Plan& pl, uint64_t seed) {
     const Problem& P = pl.P;
+    const Options& o = ctx->opt;
     const int cap = kSampleCap;
     const int cap_acc = kSampleCapAcc;
     const SampleSizes z = sample_sizes(ctx, pl);
     const int G = z.G, Mg = z.Mg;
     const size_t per_group_ints = z.per_group_ints, per_group_bytes = z.per_group_bytes;
-    CK(ctx->smp_int.ensure(z.int_bytes));
-    CK(ctx->smp_surv.ensure(z.surv_bytes));
+    int rc = sample_buffers(ctx, pl, grow(ctx));
+    if (rc) return rc;
     SampleState st[4];
     int* b = ctx->smp_int.as<int>() + 2 * (size_t)P.M;
     for (int g = 0; g < G; ++g) {
@@ -412,9 +462,8 @@ int run_sample(esacb200_ctx* ctx, const Plan& pl, uint64_t seed) {
         st[g].cap_acc = cap_acc;
         st[g].M = Mg;
     }
-    CK(ctx->coords4.ensure((size_t)P.E * P.N * sizeof(float4)));
     unsigned long long* trace = nullptr;
-    if (ctx->sample_trace) {  // 4 lanes x 32 waves x 2 kernels x (start, end)
+    if (o.sample_trace) {  // 4 lanes x 32 waves x 2 kernels x (start, end)
         CK(ctx->smp_trace.ensure(512 * 8));
         CK(cudaMemsetAsync(ctx->smp_trace.p, 0, 512 * 8, ctx->stream));
         trace = ctx->smp_trace.as<unsigned long long>();
@@ -422,12 +471,12 @@ int run_sample(esacb200_ctx* ctx, const Plan& pl, uint64_t seed) {
     }
     const cudaStream_t lane_streams[4] = {ctx->stream, ctx->aux_stream, ctx->aux_more[0], ctx->aux_more[1]};
     const cudaEvent_t lane_joins[4] = {nullptr, ctx->ev_join, ctx->ev_join_more[0], ctx->ev_join_more[1]};
-    ctx->st.kernel_launches += launch_sample(pl.d_coords, ctx->coords4.as<float4>(), ctx->assign32.as<int>(), P, seed, ctx->max_tries,
+    ctx->st.kernel_launches += launch_sample(pl.d_coords, ctx->coords4.as<float4>(), ctx->assign32.as<int>(), P, seed, o.max_tries,
                                              ctx->inj_M ? ctx->inject.as<int>() : nullptr, ctx->inj_T, st, G, ctx->sm_count,
-                                             ctx->sample_prefilter, ctx->hyp_offset, ctx->hyp_stride, ctx->poses.as<Pose>(), ctx->cells.as<int>(),
+                                             o.sample_prefilter, o.hyp_offset, o.hyp_stride, ctx->poses.as<Pose>(), ctx->cells.as<int>(),
                                              ctx->tries.as<int>(), lane_streams, ctx->ev_fork, lane_joins,
                                              pl.split_e, ctx->perm.as<int>(), ctx->offsets.as<int>(), ctx->ev_copied,
-                                             ctx->sample_span0, ctx->sample_window, ctx->sample_waves, trace, ctx->sample_tail_boost,
+                                             o.sample_span0, o.sample_window, o.sample_waves, trace, o.sample_tail_boost,
                                              pl.async ? &pl.async->dev : nullptr);
     CK(cudaGetLastError());
     ctx->smp_groups_last = G;
@@ -477,7 +526,8 @@ int run_score(esacb200_ctx* ctx, const Plan& pl) {
 }
 
 int pick_group(esacb200_ctx* ctx, const Problem& P, int jobs_hint) {
-    if (ctx->refine_group_opt > 0) return ctx->refine_group_opt < ctx->refine_coresident ? ctx->refine_group_opt : ctx->refine_coresident;
+    const int opt = ctx->opt.refine_group_opt;
+    if (opt > 0) return opt < ctx->refine_coresident ? opt : ctx->refine_coresident;
     const int words = (P.N + 31) / 32;
     // ~320 cells per CTA, up to every co-resident CTA: with the warp-parallel slot summation the inter-CTA barrier costs less
     // than the fp64 work it spreads (60x80 -> 16 CTAs, 480x640 -> every co-resident CTA)
@@ -486,7 +536,7 @@ int pick_group(esacb200_ctx* ctx, const Problem& P, int jobs_hint) {
     // Jobs are handed out dynamically inside the kernel, so a group may work through several jobs: fewer, larger groups even
     // out the differing job lengths (rounds x LM iterations) -- worth it only while a block's share of the map stays large
     // against the cost of a group exchange (480x640: yes; 60x80: no)
-    int waves = jobs_hint >= 8 ? ctx->refine_jobs_per_group : 1;
+    int waves = jobs_hint >= 8 ? ctx->opt.refine_jobs_per_group : 1;
     int concurrent = jobs_hint > 0 ? (jobs_hint + waves - 1) / waves : 1;
     int cap = ctx->refine_coresident / concurrent;
     if (waves > 1 && (cap < 1 || P.N / (cap < 1 ? 1 : cap) < 4096)) cap = ctx->refine_coresident / (jobs_hint > 0 ? jobs_hint : 1);
@@ -515,9 +565,21 @@ RefineSizes refine_sizes(const esacb200_ctx* ctx, const Problem& P, int max_jobs
     z.barrier = (z.n_flags + 4) * 4;
     const int wpc = (words + group - 1) / group;
     z.cache = wpc <= refine_cache_words() ? 1 : 0;
-    z.clist = (ctx->refine_compact && !z.cache && wpc <= refine_max_compact_words())
+    z.clist = (ctx->opt.refine_compact && !z.cache && wpc <= refine_max_compact_words())
                   ? (size_t)n_groups * words * 32 * sizeof(unsigned short) : 0;
     return z;
+}
+
+// Refinement (own_masks: the final inlier masks go to the context's workspace).
+template <class Need>
+int refine_buffers(esacb200_ctx* ctx, const Problem& P, int max_jobs, int group, bool own_masks, Need&& need) {
+    const RefineSizes z = refine_sizes(ctx, P, max_jobs, group);
+    if (own_masks) NEED(ctx->masks, z.masks);
+    NEED(ctx->rounds, z.rounds);
+    NEED(ctx->scratch, z.scratch);
+    NEED(ctx->barrier, z.barrier);
+    if (z.clist) NEED(ctx->clist, z.clist);
+    return 0;
 }
 
 // masks_out: where the final inlier masks go ([max_jobs][2][words]); null = the context's workspace.
@@ -527,15 +589,11 @@ int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, con
     const int words = (P.N + 31) / 32;
     const RefineSizes z = refine_sizes(ctx, P, max_jobs, group);
     const int n_groups = z.n_groups;
-    if (!masks_out) {
-        CK(ctx->masks.ensure(z.masks));
-        masks_out = ctx->masks.as<uint32_t>();
-    }
-    CK(ctx->rounds.ensure(z.rounds));
-    CK(ctx->scratch.ensure(z.scratch));
+    int rc = refine_buffers(ctx, P, max_jobs, group, !masks_out, grow(ctx));
+    if (rc) return rc;
+    if (!masks_out) masks_out = ctx->masks.as<uint32_t>();
     if (group > 1) CK(cudaMemsetAsync(ctx->scratch.p, 0, refine_scratch_doubles(n_groups, group) * 8, ctx->stream));  // LL elements: no stale sequence numbers
     const size_t n_flags = z.n_flags;
-    CK(ctx->barrier.ensure(z.barrier));
     CK(cudaMemsetAsync(ctx->barrier.p, 0, z.barrier, ctx->stream));
     RefineArgs a;
     a.coords = pl.d_coords;
@@ -554,21 +612,17 @@ int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, con
     a.job_counter = (int*)(ctx->barrier.as<unsigned int>() + n_flags);
     a.group = group;
     a.cache = z.cache;
-    a.compact = ctx->refine_compact;
-    a.pretest = ctx->refine_pretest;
-    a.clist = nullptr;
-    if (z.clist) {
-        CK(ctx->clist.ensure(z.clist));
-        a.clist = ctx->clist.as<unsigned short>();
-    }
+    a.compact = ctx->opt.refine_compact;
+    a.pretest = ctx->opt.refine_pretest;
+    a.clist = z.clist ? ctx->clist.as<unsigned short>() : nullptr;
     a.prof = nullptr;
-    if (ctx->refine_profile) {
+    if (ctx->opt.refine_profile) {
         CK(ctx->prof.ensure(16 * 8));
         CK(cudaMemsetAsync(ctx->prof.p, 0, 16 * 8, ctx->stream));
         a.prof = ctx->prof.as<long long>();
     }
     a.P = P;
-    a.max_ref_steps = ctx->max_ref_steps;
+    a.max_ref_steps = ctx->opt.max_ref_steps;
     if (pl.async) a.dev = pl.async->dev;
     launch_refine(a, n_groups, ctx->stream);
     CK(cudaGetLastError());
@@ -578,7 +632,7 @@ int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, con
 }
 
 uint64_t call_seed(esacb200_ctx* ctx) {
-    uint64_t s = ctx->fixed_seed ? ctx->seed : mix64(ctx->seed + kGold * ctx->calls);
+    uint64_t s = ctx->opt.fixed_seed ? ctx->seed : mix64(ctx->seed + kGold * ctx->calls);
     if (ctx->calls == 0) s = ctx->seed;
     ++ctx->calls;
     return s;
@@ -611,68 +665,40 @@ int enqueue_forward_core(esacb200_ctx* ctx, const Plan& pl, float* d_out17) {
 // Sizes every workspace buffer of the forward pipeline (upload, plan_and_prep, sampling, refinement) for the largest of a
 // batch's images before the first one is enqueued: DevBuf::ensure growing mid-batch frees the old buffer, and cudaFree
 // synchronises the device, which would serialise the copy stream's overlap with the previous image.
-// `need(buf, bytes)` is called for every buffer; reserve_forward_batch grows them, the stream-ordered forward also checks them.
+// `need(buf, bytes)` is called once per buffer with the largest size any image needs; reserve_forward_batch grows them, the
+// stream-ordered forward also checks them.  (host_coords: the images' maps are staged, double-buffered.)
 template <class Need>
 int forward_workspace(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool host_coords, Need&& need) {
-    size_t part = 0, cbytes = 0, c4 = 0, sint = 0, ssurv = 0, masks = 0, rounds = 0, scratch = 0, barrier = 0, clist = 0;
-    auto mx = [](size_t& a, size_t b) { if (b > a) a = b; };
-#define NEED(buf, bytes) do { int r__ = need(buf, bytes); if (r__) return r__; } while (0)
-    int M = 0, E = 0;
+    std::map<DevBuf*, size_t> most;
+    auto mx = [&](DevBuf& b, size_t bytes) {
+        most[&b] = std::max(most[&b], bytes);
+        return 0;
+    };
     for (Plan pl : plans) {
         plan_launch(ctx, pl);
-        const Problem& P = pl.P;
-        M = P.M; E = P.E;
-        mx(part, (size_t)P.M * pl.T * 4);
-        mx(cbytes, (size_t)P.E * 3 * P.N * sizeof(float));
-        mx(c4, (size_t)P.E * P.N * sizeof(float4));
-        const SampleSizes a = sample_sizes(ctx, pl);
-        mx(sint, a.int_bytes);
-        mx(ssurv, a.surv_bytes);
-        const RefineSizes r = refine_sizes(ctx, P, 1, pick_group(ctx, P, 1));
-        mx(masks, r.masks); mx(rounds, r.rounds); mx(scratch, r.scratch); mx(barrier, r.barrier); mx(clist, r.clist);
+        input_buffers(pl.P, host_coords ? &ctx->coords : nullptr, &ctx->assign64, mx);
+        input_buffers(pl.P, host_coords ? &ctx->coords_alt : nullptr, &ctx->assign64_alt, mx);
+        prep_buffers(ctx, pl, mx);
+        sample_buffers(ctx, pl, mx);
+        refine_buffers(ctx, pl.P, 1, pick_group(ctx, pl.P, 1), true, mx);
     }
-    if (host_coords) {
-        NEED(ctx->coords, cbytes);
-        NEED(ctx->coords_alt, cbytes);
-    }
-    NEED(ctx->assign64, (size_t)M * 8);
-    NEED(ctx->assign64_alt, (size_t)M * 8);
-    NEED(ctx->assign32, (size_t)M * 4);
-    NEED(ctx->counts, (size_t)E * 4);
-    NEED(ctx->offsets, (size_t)(E + 1) * 4);
-    NEED(ctx->perm, (size_t)M * 4);
-    NEED(ctx->slot_of, (size_t)M * 4);
-    NEED(ctx->chunks, (size_t)(M + E) * sizeof(ChunkDesc));
-    NEED(ctx->scalars, S_COUNT * 4);
-    NEED(ctx->centres, (size_t)E * 3 * 4);
-    NEED(ctx->poses, (size_t)M * sizeof(Pose));
-    NEED(ctx->poses_ref, (size_t)M * sizeof(Pose));
-    NEED(ctx->cells, (size_t)M * 8 * 4);
-    NEED(ctx->tries, (size_t)M * 4);
-    NEED(ctx->posepk, (size_t)M * sizeof(PosePk));
-    NEED(ctx->part, part);
-    NEED(ctx->scores, (size_t)M * 8);
-    NEED(ctx->probs, (size_t)M * 8);
-    NEED(ctx->stats, 8 * 8);
-    NEED(ctx->contrib, (size_t)M * 4);
-    NEED(ctx->out17, 32 * 4);
-    NEED(ctx->smp_int, sint);
-    NEED(ctx->smp_surv, ssurv);
-    NEED(ctx->coords4, c4);
-    NEED(ctx->masks, masks);
-    NEED(ctx->rounds, rounds);
-    NEED(ctx->scratch, scratch);
-    NEED(ctx->barrier, barrier);
-    if (clist) NEED(ctx->clist, clist);
-#undef NEED
+    for (auto& m : most) NEED(*m.first, m.second);
     return 0;
 }
 
+// The backward's tail (bwd_reduce .. bwd_assemble); `losses`: esac.backward's own per-hypothesis losses too.
+template <class Need>
+int backward_buffers(esacb200_ctx* ctx, const Problem& P, bool losses, Need&& need) {
+    if (losses) NEED(ctx->losses, (size_t)P.M * 8);
+    NEED(ctx->red, (size_t)P.M * bwd_tiles(P.N) * bwd_red_vals() * 8);
+    NEED(ctx->hypgrad, (size_t)P.M * bwd_hypgrad_bytes());
+    NEED(ctx->job_of, (size_t)(P.M > P.E ? P.M : P.E) * 4);
+    return 0;
+}
+#undef NEED
+
 int reserve_forward_batch(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool host_coords) {
-    return forward_workspace(ctx, plans, host_coords, [&](DevBuf& b, size_t bytes) -> int {
-        CK(b.ensure(bytes));
-        return 0;
-    });
+    return forward_workspace(ctx, plans, host_coords, grow(ctx));
 }
 
 // All B pointers of one argument on the device, or all on the host (a mix is an error).  None may be null.
@@ -835,13 +861,6 @@ void esacb200_destroy(esacb200_ctx* ctx) {
     DeviceGuard device_guard(ctx->device);
     if (ctx->nccl_comm) { cudaStreamSynchronize(ctx->stream); nccl_api().CommDestroy(ctx->nccl_comm); ctx->nccl_comm = nullptr; }
     cudaStreamSynchronize(ctx->stream);
-    DevBuf* bufs[] = {&ctx->coords, &ctx->grads, &ctx->assign64, &ctx->assign32, &ctx->counts, &ctx->offsets, &ctx->perm,
-                      &ctx->slot_of, &ctx->chunks, &ctx->scalars, &ctx->centres, &ctx->poses, &ctx->poses_ref, &ctx->cells,
-                      &ctx->tries, &ctx->posepk, &ctx->part, &ctx->scores, &ctx->probs, &ctx->stats, &ctx->contrib,
-                      &ctx->masks, &ctx->rounds, &ctx->scratch, &ctx->barrier, &ctx->out17, &ctx->inject, &ctx->losses,
-                      &ctx->red, &ctx->hypgrad, &ctx->job_of, &ctx->gt, &ctx->smp_int, &ctx->smp_surv, &ctx->smp_trace, &ctx->clist, &ctx->eflags, &ctx->coords4, &ctx->coords_alt, &ctx->assign64_alt, &ctx->out_batch, &ctx->prof, &ctx->gathered, &ctx->grads_work,
-                      &ctx->contrib8, &ctx->upstream, &ctx->seed_state};
-    for (DevBuf* b : bufs) b->release();
     for (int i = 0; i < EV_COUNT; ++i)
         if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
     if (ctx->h_out) cudaFreeHost(ctx->h_out);
@@ -860,7 +879,7 @@ void esacb200_destroy(esacb200_ctx* ctx) {
         if (ctx->ev_join_more[i]) cudaEventDestroy(ctx->ev_join_more[i]);
     }
     if (ctx->own_stream) cudaStreamDestroy(ctx->own_stream);
-    delete ctx;
+    delete ctx;  // frees the workspace buffers (still on the context's device, after its stream has drained)
 }
 
 const char* esacb200_last_error(const esacb200_ctx* ctx) { return ctx ? ctx->err : "null context"; }
@@ -885,27 +904,28 @@ int esacb200_set_seed(esacb200_ctx* ctx, uint64_t seed) {
 
 int esacb200_set_option(esacb200_ctx* ctx, const char* key, double v) {
     if (!ctx || !key) return ESACB200_ERR_ARG;
-    if (!strcmp(key, "max_tries")) ctx->max_tries = v < 1 ? 1 : (int)v;
-    else if (!strcmp(key, "max_ref_steps")) ctx->max_ref_steps = v < 0 ? 0 : (int)v;
-    else if (!strcmp(key, "fixed_seed")) ctx->fixed_seed = v != 0;
-    else if (!strcmp(key, "refine_group")) ctx->refine_group_opt = (int)v;
-    else if (!strcmp(key, "refine_pretest")) ctx->refine_pretest = v != 0;
-    else if (!strcmp(key, "refine_compact")) ctx->refine_compact = v != 0;
-    else if (!strcmp(key, "refine_profile")) ctx->refine_profile = v != 0;
-    else if (!strcmp(key, "refine_jobs_per_group")) ctx->refine_jobs_per_group = v < 1 ? 1 : (int)v;
-    else if (!strcmp(key, "sample_prefilter")) ctx->sample_prefilter = v != 0;
-    else if (!strcmp(key, "sample_tail_boost")) ctx->sample_tail_boost = v < 1 ? 1.f : (float)v;
-    else if (!strcmp(key, "sample_trace")) ctx->sample_trace = v != 0;
-    else if (!strcmp(key, "sample_span0")) ctx->sample_span0 = v < 256 ? 256 : ((int)v + 255) / 256 * 256;
-    else if (!strcmp(key, "sample_window")) ctx->sample_window = v < 0.05 ? 0.05f : (float)v;
-    else if (!strcmp(key, "sample_waves")) ctx->sample_waves = v < 0 ? 0 : (v > 64 ? 64 : (int)v);
-    else if (!strcmp(key, "upload_split")) ctx->upload_split = v != 0;  // host maps in two halves, sampling under the second copy
-    else if (!strcmp(key, "sample_groups")) ctx->sample_groups = v >= 4 ? 4 : (v >= 2 ? (int)v : 1);  // interleaved lanes, one stream each
-    else if (!strcmp(key, "hyp_offset")) ctx->hyp_offset = (int)v;  // global index of local hypothesis 0 (sharded runs)
-    else if (!strcmp(key, "hyp_stride")) ctx->hyp_stride = v < 1 ? 1 : (int)v;  // ... of local hypothesis h: offset + h * stride
-    else if (!strcmp(key, "score_ppt")) ctx->score_ppt_opt = (int)v;   // 0 = automatic, else 2 / 4 / 8 cells per thread
-    else if (!strcmp(key, "score_hc")) ctx->score_hc_opt = (int)v;     // 0 = automatic, else hypotheses per chunk (<= 64)
-    else if (!strcmp(key, "batch_workers")) ctx->batch_workers = v < 1 ? 1 : (v > 16 ? 16 : (int)v);  // streams of backward_batch
+    Options& o = ctx->opt;
+    if (!strcmp(key, "max_tries")) o.max_tries = v < 1 ? 1 : (int)v;
+    else if (!strcmp(key, "max_ref_steps")) o.max_ref_steps = v < 0 ? 0 : (int)v;
+    else if (!strcmp(key, "fixed_seed")) o.fixed_seed = v != 0;
+    else if (!strcmp(key, "refine_group")) o.refine_group_opt = (int)v;
+    else if (!strcmp(key, "refine_pretest")) o.refine_pretest = v != 0;
+    else if (!strcmp(key, "refine_compact")) o.refine_compact = v != 0;
+    else if (!strcmp(key, "refine_profile")) o.refine_profile = v != 0;
+    else if (!strcmp(key, "refine_jobs_per_group")) o.refine_jobs_per_group = v < 1 ? 1 : (int)v;
+    else if (!strcmp(key, "sample_prefilter")) o.sample_prefilter = v != 0;
+    else if (!strcmp(key, "sample_tail_boost")) o.sample_tail_boost = v < 1 ? 1.f : (float)v;
+    else if (!strcmp(key, "sample_trace")) o.sample_trace = v != 0;
+    else if (!strcmp(key, "sample_span0")) o.sample_span0 = v < 256 ? 256 : ((int)v + 255) / 256 * 256;
+    else if (!strcmp(key, "sample_window")) o.sample_window = v < 0.05 ? 0.05f : (float)v;
+    else if (!strcmp(key, "sample_waves")) o.sample_waves = v < 0 ? 0 : (v > 64 ? 64 : (int)v);
+    else if (!strcmp(key, "upload_split")) o.upload_split = v != 0;  // host maps in two halves, sampling under the second copy
+    else if (!strcmp(key, "sample_groups")) o.sample_groups = v >= 4 ? 4 : (v >= 2 ? (int)v : 1);  // interleaved lanes, one stream each
+    else if (!strcmp(key, "hyp_offset")) o.hyp_offset = (int)v;  // global index of local hypothesis 0 (sharded runs)
+    else if (!strcmp(key, "hyp_stride")) o.hyp_stride = v < 1 ? 1 : (int)v;  // ... of local hypothesis h: offset + h * stride
+    else if (!strcmp(key, "score_ppt")) o.score_ppt_opt = (int)v;   // 0 = automatic, else 2 / 4 / 8 cells per thread
+    else if (!strcmp(key, "score_hc")) o.score_hc_opt = (int)v;     // 0 = automatic, else hypotheses per chunk (<= 64)
+    else if (!strcmp(key, "batch_workers")) o.batch_workers = v < 1 ? 1 : (v > 16 ? 16 : (int)v);  // streams of backward_batch
     else return fail(ctx, ESACB200_ERR_ARG, "unknown option '%s'", key);
     return ESACB200_OK;
 }
@@ -994,7 +1014,7 @@ static int enqueue_forward_record(esacb200_ctx* ctx, const float* coords, int E,
         CK(ctx->scores.ensure(8));
         CK(ctx->out17.ensure(32 * 4));
     }
-    launch_pack_forward(ctx->scores.as<double>(), ctx->out17.as<float>(), M, M_pad, expert_offset, ctx->hyp_offset, ctx->hyp_stride,
+    launch_pack_forward(ctx->scores.as<double>(), ctx->out17.as<float>(), M, M_pad, expert_offset, ctx->opt.hyp_offset, ctx->opt.hyp_stride,
                         pack_out, ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 1;
@@ -1211,7 +1231,7 @@ int esacb200_forward_batch(esacb200_ctx* ctx, int B, const float* coords, int E,
 // allocates nothing.
 
 // The stream-ordered forward's context, created on first use with ctx's seed (a capture may not create it: that allocates).
-// The options that shape the pipeline are copied from ctx on every call.
+// The options are copied from ctx on every call.
 static int async_context(esacb200_ctx* ctx, bool capturing, esacb200_ctx** out) {
     if (!ctx->async) {
         if (capturing)
@@ -1231,23 +1251,10 @@ static int async_context(esacb200_ctx* ctx, bool capturing, esacb200_ctx** out) 
     }
     esacb200_ctx* a = ctx->async;
     a->stream = ctx->stream;
-    a->max_tries = ctx->max_tries;
-    a->max_ref_steps = ctx->max_ref_steps;
-    a->fixed_seed = ctx->fixed_seed;
-    a->refine_group_opt = ctx->refine_group_opt;
-    a->refine_jobs_per_group = ctx->refine_jobs_per_group;
-    a->refine_compact = ctx->refine_compact;
-    a->refine_pretest = ctx->refine_pretest;
-    a->sample_prefilter = ctx->sample_prefilter;
-    a->sample_tail_boost = ctx->sample_tail_boost;
-    a->sample_span0 = ctx->sample_span0;
-    a->sample_window = ctx->sample_window;
-    a->sample_waves = ctx->sample_waves;
-    a->sample_groups = ctx->sample_groups;
-    a->hyp_offset = ctx->hyp_offset;
-    a->hyp_stride = ctx->hyp_stride;
-    a->score_ppt_opt = ctx->score_ppt_opt;
-    a->score_hc_opt = ctx->score_hc_opt;
+    // The two diagnostics stay off here and in the batch workers: they allocate and need a read-back, which a capture cannot
+    // do, and their getters read the caller's context, not the one that ran the kernels.
+    a->opt = ctx->opt;
+    a->opt.refine_profile = a->opt.sample_trace = 0;
     *out = a;
     return 0;
 }
@@ -1330,7 +1337,7 @@ int esacb200_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E,
         im.dev.cam = cameras + 3 * (size_t)b;
         im.dev.seed = a->seed_state.as<unsigned long long>();
         im.dev.index = b;
-        im.dev.fixed_seed = a->fixed_seed;
+        im.dev.fixed_seed = a->opt.fixed_seed;
         im.pose = out_poses + 16 * (size_t)b;
         im.expert = (long long*)out_experts + b;
         im.status = out_status + b;
@@ -1578,11 +1585,8 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
     rc = run_hypotheses(ctx, pl, coords, assign, assign_stride, sh, nullptr);
     if (rc) return rc;
     int* sc = ctx->scalars.as<int>();
-    const int tiles = bwd_tiles(P.N);
-    CK(ctx->losses.ensure((size_t)M * 8));
-    CK(ctx->red.ensure((size_t)M * tiles * bwd_red_vals() * 8));
-    CK(ctx->hypgrad.ensure((size_t)M * bwd_hypgrad_bytes()));
-    CK(ctx->job_of.ensure((size_t)(M > E ? M : E) * 4));
+    rc = backward_buffers(ctx, P, true, grow(ctx));
+    if (rc) return rc;
     BwdArgs b;
     b.coords = pl.d_coords;
     b.grads = d_grads;
@@ -1793,10 +1797,8 @@ static int hypotheses_backward_impl(esacb200_ctx* ctx, const void* tape, const f
     if (d_poses6) CK(cudaMemcpyAsync(up + M, d_poses6, (size_t)M * 6 * 8, cudaMemcpyDefault, ctx->stream));
     else CK(cudaMemsetAsync(up + M, 0, (size_t)M * 6 * 8, ctx->stream));
     mark(ctx, EV_REFINE);
-    const int tiles = bwd_tiles(P.N);
-    CK(ctx->red.ensure((size_t)M * tiles * bwd_red_vals() * 8));
-    CK(ctx->hypgrad.ensure((size_t)M * bwd_hypgrad_bytes()));
-    CK(ctx->job_of.ensure((size_t)(M > E ? M : E) * 4));
+    int rc = backward_buffers(ctx, P, false, grow(ctx));
+    if (rc) return rc;
     BwdArgs b;
     memset(&b, 0, sizeof(b));
     b.coords = d_coords;
@@ -1941,7 +1943,7 @@ static int run_batch(esacb200_ctx* ctx, int B, const int* H, const int* W, bool 
     std::vector<uint64_t> seeds((size_t)B);
     if (draws)
         for (int b = 0; b < B; ++b) seeds[b] = call_seed(ctx);
-    const int nw = ctx->batch_workers < B ? ctx->batch_workers : B;
+    const int nw = ctx->opt.batch_workers < B ? ctx->opt.batch_workers : B;
     while ((int)ctx->workers.size() < nw) {
         esacb200_ctx* w = nullptr;
         int rc = esacb200_create(ctx->device, &w);
@@ -1955,19 +1957,9 @@ static int run_batch(esacb200_ctx* ctx, int B, const int* H, const int* W, bool 
         try {
         esacb200_ctx* w = ctx->workers[wi];
         cudaSetDevice(ctx->device);
-        w->max_tries = ctx->max_tries;
-        w->max_ref_steps = ctx->max_ref_steps;
-        w->refine_group_opt = ctx->refine_group_opt;
-        w->refine_jobs_per_group = ctx->refine_jobs_per_group;
-        w->refine_compact = ctx->refine_compact;
-        w->refine_pretest = ctx->refine_pretest;
-        w->sample_prefilter = ctx->sample_prefilter;
-        w->sample_tail_boost = ctx->sample_tail_boost;
-        w->hyp_offset = ctx->hyp_offset;
-        w->hyp_stride = ctx->hyp_stride;
-        w->score_ppt_opt = ctx->score_ppt_opt;
-        w->score_hc_opt = ctx->score_hc_opt;
-        w->fixed_seed = 1;
+        w->opt = ctx->opt;
+        w->opt.fixed_seed = 1;
+        w->opt.refine_profile = w->opt.sample_trace = 0;  // as in async_context
         // this worker's images (dealt round-robin), largest first: the workspace grows at most once
         std::vector<int> mine;
         for (int b = wi; b < B; b += nw) mine.push_back(b);

@@ -554,22 +554,31 @@ def d_pnp(img, obj, K, eps=np.float32(0.001)):
 
 
 def d_sm_score(coords, assign, sampling, hyps, losses, probs, repro_errs, jacobeans, K, alpha, beta, tau, max_reproj,
-               clamp_thresh=10.0, clamp_log=None):
+               clamp_thresh=10.0, clamp_log=None, g=None, support_log=None):
     """esac_derivative.h:347-420 (dSMScore) + 205-324 (dScore).  Returns list of [N_rowmajor, 3]
-    f64 (index y*W + x) per hypothesis, zeros for hypotheses below PROB_THRESH."""
+    f64 (index y*W + x) per hypothesis, zeros for hypotheses below PROB_THRESH.
+    ``g``: per-hypothesis upstream dL/d score_h in place of the reference's p_h (l_h - sum_j p_j l_j) (``losses`` is then
+    unused); ``support_log``: a list that receives each hypothesis's dPNP support term, (4, 3) f64 per minimal-set cell
+    in ``hyps[h].cells`` order (zeros below PROB_THRESH)."""
     H, W = sampling.shape[:2]
     M = len(hyps)
     probs = np.asarray(probs, np.float64)
-    losses = np.asarray(losses, np.float64)
+    losses = None if losses is None else np.asarray(losses, np.float64)
+    upstream = g
     out = []
     for h in range(M):
         if probs[h] < PROB_THRESH:
             out.append(np.zeros((H * W, 3)))
+            if support_log is not None:
+                support_log.append(np.zeros((4, 3)))
             continue
-        # scoreOutputGradients (esac_derivative.h:372-374), sequential subtraction order
-        g = probs[h] * losses[h]
-        for j in range(M):
-            g -= probs[h] * probs[j] * losses[j]
+        if upstream is not None:
+            g = float(upstream[h])
+        else:
+            # scoreOutputGradients (esac_derivative.h:372-374), sequential subtraction order
+            g = probs[h] * losses[h]
+            for j in range(M):
+                g -= probs[h] * probs[j] * losses[j]
         e = int(assign[h])
         err = repro_errs[h]
         st = (np.float32(beta) * (err - np.float32(tau))).astype(np.float32).astype(np.float64)
@@ -587,6 +596,8 @@ def d_sm_score(coords, assign, sampling, hyps, losses, probs, repro_errs, jacobe
         w = dRe.T.reshape(-1)  # same ordering
         dPdO = d_project_d_obj_batch(pts2, pts3, rot, hyps[h].tvec, K, max_reproj) * w[:, None]
         support = (w[:, None] * jacobeans[h]).sum(axis=0).reshape(1, 6) @ dHdO  # 1x12
+        if support_log is not None:
+            support_log.append(support.reshape(4, 3).copy())
         g_colmajor = dPdO  # [x*H + y, 3]
         for i, (x, y) in enumerate(hyps[h].cells):
             g_colmajor[x * H + y] += support[0, 3 * i:3 * i + 3]
@@ -645,10 +656,82 @@ class BackwardTrace:
     ref: list
     inlier_maps: list
     losses: list
-    grad_I: list
-    grad_II: list
+    grad_I: list                # per hypothesis: dl_h . dHyp_h [N_rowmajor, 3] (None below PROB_THRESH)
+    grad_II: list               # per hypothesis: the score term, dScore plus the dPNP support on the minimal set
     clamped_jr: list = None     # hypotheses whose max|J_R| > 10 zeroed path I (esac.cpp:436-437)
     clamped_dpnp: list = None   # hypotheses whose max|dPNP| > 10 zeroed the minimal-set term (esac_derivative.h:287)
+    support: list = None        # per hypothesis: the dPNP support inside grad_II, (4, 3) in hyps[h].cells order
+    mult: np.ndarray = None     # per hypothesis: the multiplier of grad_I in the assembly (probs, or 1 in hypotheses_vjp)
+
+
+def _refined_hypotheses(coords, assign, sampling, K, tau, alpha, beta, max_reproj, max_tries, seed, injected_cells, mt):
+    """esac.cpp:244-352: the hypotheses, their reprojection errors and jacobeanHyp at the initial pose, scores, softmax, and
+    the refinement of every hypothesis with p >= PROB_THRESH (the others keep their initial pose and no inlier map)."""
+    hyps = sample_hypotheses(coords, assign, sampling, K, max_tries, tau, seed, injected_cells, mt)
+    errs, jacs = [], []
+    for h, hy in enumerate(hyps):
+        e_, j_ = get_repro_errs(coords, hy.rvec, hy.tvec, int(assign[h]), sampling, K, max_reproj, True)
+        errs.append(e_); jacs.append(j_)
+    scores = get_hyp_scores(errs, tau, alpha, beta)
+    probs = softmax(scores)
+    ref, imaps = [], []
+    for h, hy in enumerate(hyps):
+        if probs[h] < PROB_THRESH:
+            ref.append((hy.rvec.copy(), hy.tvec.copy())); imaps.append(None)
+            continue
+        r, t, im, _ = refine_hyp(coords, errs[h], sampling, K, int(assign[h]), tau, MAX_REF_STEPS, max_reproj,
+                                 hy.rvec, hy.tvec)
+        ref.append((r, t)); imaps.append(im)
+    return hyps, errs, jacs, scores, probs, ref, imaps
+
+
+def d_hyp_d_obj(coords, e, sampling, K, rvec, tvec, inlier_map, max_reproj, clamp_thresh=10.0):
+    """esac.cpp:373-449: dHyp = d (refined pose) / d (scene coordinates) of one contributing hypothesis, 6 x 3N with column
+    (y*W + x)*3 + c, through J_R = -pinv(J^T J) J^T over the final inlier set at the refined pose (rvec, tvec).  Returns
+    (dHyp, clamped): J_R is zeroed when max|J_R| > clamp_thresh (esac.cpp:436-437); dHyp is None when the refinement never
+    accepted a round or kept fewer than 4 inliers (the reference then has no points and dHyp stays zero)."""
+    H, W = sampling.shape[:2]
+    if inlier_map is None:
+        return None, False
+    sel = np.argwhere(inlier_map.T > 0)  # rows ordered x-outer, y-inner: (x, y)
+    if len(sel) < 4:
+        return None, False
+    dHyp = np.zeros((6, H * W * 3))
+    xs, ys = sel[:, 0], sel[:, 1]
+    img = sampling[ys, xs].astype(np.float32)
+    obj = np.stack([coords[e, 0, ys, xs], coords[e, 1, ys, xs], coords[e, 2, ys, xs]], 1).astype(np.float32)
+    proj, J = cv2.projectPoints(obj.reshape(-1, 1, 3), rvec, tvec, K, None)
+    proj = proj.reshape(-1, 2).astype(np.float32)
+    J = J[:, 0:6]
+    d = proj - img
+    err = np.maximum(np.sqrt(d[:, 0].astype(np.float64) ** 2 + d[:, 1].astype(np.float64) ** 2), EPS)
+    jr = (1 / err * d[:, 0].astype(np.float64))[:, None] * J[0::2] + \
+         (1 / err * d[:, 1].astype(np.float64))[:, None] * J[1::2]
+    jr[err > max_reproj] = 0.0
+    jtj = jr.T @ jr
+    inv = cv2.invert(jtj, flags=cv2.DECOMP_SVD)[1]
+    JR = -inv @ jr.T  # 6 x n
+    clamped = get_max(JR) > clamp_thresh
+    if clamped:
+        JR = np.zeros_like(JR)
+    rot, _ = cv2.Rodrigues(rvec)
+    dNdO = d_project_d_obj_batch(img, obj, rot, tvec, K, max_reproj)  # n x 3
+    for k in range(len(xs)):
+        di = int(ys[k]) * W * 3 + int(xs[k]) * 3
+        dHyp[:, di:di + 3] = JR[:, k:k + 1] @ dNdO[k:k + 1, :]
+    return dHyp, clamped
+
+
+def assemble(out_grads, assign, probs, mult, grad_I, grad_II):
+    """esac.cpp:491-508: out_grads[e] += mult_h * grad_I[h] + grad_II[h] for every hypothesis with p >= PROB_THRESH,
+    float += double, sequential in h.  out_grads f32 [E,3,H,W] is accumulated in place."""
+    H, W = out_grads.shape[2], out_grads.shape[3]
+    for h in range(len(assign)):
+        if probs[h] < PROB_THRESH:
+            continue
+        e = int(assign[h])
+        tot = (mult[h] * grad_I[h] + grad_II[h]).reshape(H, W, 3).transpose(2, 0, 1)
+        out_grads[e] = (out_grads[e].astype(np.float64) + tot).astype(np.float32)
 
 
 def backward(coords, out_grads, assign, gt_pose, w_rot, w_trans, cut, shiftX, shiftY, f, ppx, ppy, tau, alpha,
@@ -668,21 +751,8 @@ def backward(coords, out_grads, assign, gt_pose, w_rot, w_trans, cut, shiftX, sh
     K = cam_mat(f, ppx, ppy)
     gtT = np.asarray(gt_pose, np.float32).astype(np.float64)
     sampling = create_sampling(W, H, sub, shiftX, shiftY)
-    hyps = sample_hypotheses(coords, assign, sampling, K, max_tries, tau, seed, injected_cells, mt)
-    errs, jacs = [], []
-    for h, hy in enumerate(hyps):
-        e_, j_ = get_repro_errs(coords, hy.rvec, hy.tvec, int(assign[h]), sampling, K, max_reproj, True)
-        errs.append(e_); jacs.append(j_)
-    scores = get_hyp_scores(errs, tau, alpha, beta)
-    probs = softmax(scores)
-    ref, imaps = [], []
-    for h, hy in enumerate(hyps):
-        if probs[h] < PROB_THRESH:
-            ref.append((hy.rvec.copy(), hy.tvec.copy())); imaps.append(None)
-            continue
-        r, t, im, _ = refine_hyp(coords, errs[h], sampling, K, int(assign[h]), tau, MAX_REF_STEPS, max_reproj,
-                                 hy.rvec, hy.tvec)
-        ref.append((r, t)); imaps.append(im)
+    hyps, errs, jacs, scores, probs, ref, imaps = _refined_hypotheses(coords, assign, sampling, K, tau, alpha, beta,
+                                                                      max_reproj, max_tries, seed, injected_cells, mt)
     losses = []
     expected = 0.0
     for h in range(M):
@@ -696,47 +766,62 @@ def backward(coords, out_grads, assign, gt_pose, w_rot, w_trans, cut, shiftX, sh
     for h in range(M):
         if probs[h] < PROB_THRESH:
             continue
-        e = int(assign[h])
-        dHyp = np.zeros((6, N * 3))
-        im = imaps[h]
-        # empty inlierMap (refinement never accepted a round): cols = 0 -> no points -> skip
-        if im is not None:
-            sel = np.argwhere(im.T > 0)  # rows ordered x-outer, y-inner: (x, y)
-            if len(sel) >= 4:
-                xs, ys = sel[:, 0], sel[:, 1]
-                img = sampling[ys, xs].astype(np.float32)
-                obj = np.stack([coords[e, 0, ys, xs], coords[e, 1, ys, xs], coords[e, 2, ys, xs]], 1).astype(np.float32)
-                proj, J = cv2.projectPoints(obj.reshape(-1, 1, 3), ref[h][0], ref[h][1], K, None)
-                proj = proj.reshape(-1, 2).astype(np.float32)
-                J = J[:, 0:6]
-                d = proj - img
-                err = np.maximum(np.sqrt(d[:, 0].astype(np.float64) ** 2 + d[:, 1].astype(np.float64) ** 2), EPS)
-                jr = (1 / err * d[:, 0].astype(np.float64))[:, None] * J[0::2] + \
-                     (1 / err * d[:, 1].astype(np.float64))[:, None] * J[1::2]
-                jr[err > max_reproj] = 0.0
-                jtj = jr.T @ jr
-                inv = cv2.invert(jtj, flags=cv2.DECOMP_SVD)[1]
-                JR = -inv @ jr.T  # 6 x n
-                if get_max(JR) > clamp_thresh:
-                    JR = np.zeros_like(JR)
-                    clamped_jr.append(h)
-                rot, _ = cv2.Rodrigues(ref[h][0])
-                dNdO = d_project_d_obj_batch(img, obj, rot, ref[h][1], K, max_reproj)  # n x 3
-                for k in range(len(xs)):
-                    di = int(ys[k]) * W * 3 + int(xs[k]) * 3
-                    dHyp[:, di:di + 3] = JR[:, k:k + 1] @ dNdO[k:k + 1, :]
+        dHyp, clamped = d_hyp_d_obj(coords, int(assign[h]), sampling, K, ref[h][0], ref[h][1], imaps[h], max_reproj,
+                                    clamp_thresh)
+        if clamped:
+            clamped_jr.append(h)
+        if dHyp is None:  # empty inlierMap (refinement never accepted a round): cols = 0 -> no points -> dHyp stays zero
+            dHyp = np.zeros((6, N * 3))
         dl = d_loss(ref[h][0], ref[h][1], gt_r, gt_t, w_rot, w_trans, cut)
         grad_I[h] = (dl @ dHyp).reshape(N, 3)
     # ---- path II (esac.cpp:472-486) ----------------------------------------------------------
+    support = []
     grad_II = d_sm_score(coords, assign, sampling, hyps, losses, probs, errs, jacs, K, alpha, beta, tau, max_reproj,
-                         clamp_thresh, clamped_dpnp)
+                         clamp_thresh, clamped_dpnp, support_log=support)
     # ---- assembly (esac.cpp:491-508): float += double, sequential over h ----------------------
+    assemble(out_grads, assign, probs, probs, grad_I, grad_II)
+    if trace:
+        return float(expected), BackwardTrace(hyps, scores, probs, ref, imaps, losses, grad_I, grad_II, clamped_jr, clamped_dpnp,
+                                              support, probs)
+    return float(expected)
+
+
+def hypotheses_vjp(coords, assign, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, max_reproj, sub, seed, grad_poses,
+                   grad_scores, injected_cells=None, max_tries=MAX_SAMPLING_TRIES, mt=None, clamp_thresh=10.0):
+    """The vector-Jacobian product of the hypotheses node (esac_b200.api.hypotheses_forward / hypotheses_backward): the
+    hypotheses backward() would draw, score and refine, with the loss replaced by upstream gradients of (scores, poses).
+    grad_poses [M,6] = dL/d (rvec, tvec) of the refined poses, grad_scores [M] = dL/d score_h (None counts as zero); only
+    hypotheses with p >= PROB_THRESH count.  Path I takes dl = grad_poses[h] with multiplier 1, path II takes
+    g = grad_scores[h]; the assembly is backward()'s.  Returns (gradient f32 [E,3,H,W], BackwardTrace with losses None)."""
+    coords = np.asarray(coords)
+    assert coords.dtype == np.float32 and coords.ndim == 4
+    assign = np.asarray(assign)
+    assert assign.dtype == np.int64 and assign.ndim == 1
+    H, W = coords.shape[2], coords.shape[3]
+    N = H * W
+    M = len(assign)
+    grad_poses = np.zeros((M, 6)) if grad_poses is None else np.asarray(grad_poses, np.float64).reshape(M, 6)
+    grad_scores = np.zeros(M) if grad_scores is None else np.asarray(grad_scores, np.float64).reshape(M)
+    K = cam_mat(f, ppx, ppy)
+    sampling = create_sampling(W, H, sub, shiftX, shiftY)
+    hyps, errs, jacs, scores, probs, ref, imaps = _refined_hypotheses(coords, assign, sampling, K, tau, alpha, beta,
+                                                                      max_reproj, max_tries, seed, injected_cells, mt)
+    grad_I = [None] * M
+    clamped_jr, clamped_dpnp = [], []
     for h in range(M):
         if probs[h] < PROB_THRESH:
             continue
-        e = int(assign[h])
-        tot = (probs[h] * grad_I[h] + grad_II[h]).reshape(H, W, 3).transpose(2, 0, 1)
-        out_grads[e] = (out_grads[e].astype(np.float64) + tot).astype(np.float32)
-    if trace:
-        return float(expected), BackwardTrace(hyps, scores, probs, ref, imaps, losses, grad_I, grad_II, clamped_jr, clamped_dpnp)
-    return float(expected)
+        dHyp, clamped = d_hyp_d_obj(coords, int(assign[h]), sampling, K, ref[h][0], ref[h][1], imaps[h], max_reproj,
+                                    clamp_thresh)
+        if clamped:
+            clamped_jr.append(h)
+        if dHyp is None:
+            dHyp = np.zeros((6, N * 3))
+        grad_I[h] = (grad_poses[h].reshape(1, 6) @ dHyp).reshape(N, 3)
+    support = []
+    grad_II = d_sm_score(coords, assign, sampling, hyps, None, probs, errs, jacs, K, alpha, beta, tau, max_reproj,
+                         clamp_thresh, clamped_dpnp, g=grad_scores, support_log=support)
+    out = np.zeros(coords.shape, np.float32)
+    mult = np.ones(M)
+    assemble(out, assign, probs, mult, grad_I, grad_II)
+    return out, BackwardTrace(hyps, scores, probs, ref, imaps, None, grad_I, grad_II, clamped_jr, clamped_dpnp, support, mult)

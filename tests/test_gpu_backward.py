@@ -1,7 +1,13 @@
-"""GPU parity of esac.backward against the cv2 oracle (run with `-m gpu`)."""
+"""GPU parity of esac.backward against the cv2 oracle (run with `-m gpu`).
+
+Gradients are compared class by class (tests/grad_terms.py): minimal-set cells, final inlier cells and the rest of the
+contributing hypotheses' planes, each against its own largest oracle entry, besides the old bar of 1e-3 of the largest entry.
+The bars below are about 10x the worst class measured on an H100 SXM (80 GB, 700 W); the old bar alone let path I be 0.5 to
+7 % wrong on the inlier cells."""
 import numpy as np
 import pytest
 
+import grad_terms as GT
 from esac_b200.synth import make_scene
 from oracle import esac_oracle as O
 
@@ -13,6 +19,12 @@ def api():
     import esac_b200.api as api
     api.context().set_option("fixed_seed", 1)
     return api
+
+
+# class-wise bars of test_backward_matches_oracle: about 10x the worst class over the five scenes measured on an H100 SXM
+# (80 GB, 700 W) -- minimal 2.44e-6 (scene 5), inlier 6.85e-7 (scene 5), rest 7.47e-6 (scene 3)
+BAR_SCENES = {"minimal": 2.5e-5, "inlier": 7e-6, "rest": 7.5e-5}
+BAR_FORCED = GT.FORCED_BARS   # forced scene under every refinement walk and scoring shape
 
 
 @pytest.mark.parametrize("seed,E,H,W,M,kw", [
@@ -35,8 +47,8 @@ def test_backward_matches_oracle(api, seed, E, H, W, M, kw):
     assert st["n_contrib"] == int((bt.probs >= O.PROB_THRESH).sum())
     assert np.abs(hy["losses"] - np.array(bt.losses)).max() < 1e-5 * max(1.0, np.abs(bt.losses).max())
     assert abs(loss - l_ref) < 1e-6 * max(1.0, abs(l_ref))
-    scale = max(np.abs(g_ref).max(), 1e-12)
-    assert np.abs(g - g_ref).max() / scale < 1e-3, (np.abs(g - g_ref).max(), scale)
+    rep = GT.assert_classwise(g, g_ref, GT.cell_classes(sc.coords.shape, sc.assign, bt), BAR_SCENES, f"scene {seed}")
+    print(f"scene {seed}: {GT.fmt(rep)}")
 
 
 # ---- backward under forced refinement walks and scoring shapes --------------------------------------------------------------
@@ -52,11 +64,11 @@ def forced_scene():
     l_ref, bt = O.backward(sc.coords, g_ref, sc.assign, sc.gt_pose, *FORCED_ARGS, *sc.params, seed=57, trace=True)
     n_ref = int((bt.probs >= O.PROB_THRESH).sum())
     assert n_ref >= 8
-    return sc, l_ref, g_ref, n_ref
+    return sc, l_ref, g_ref, n_ref, GT.cell_classes(sc.coords.shape, sc.assign, bt)
 
 
 def _check_backward(api, forced_scene, options):
-    sc, l_ref, g_ref, n_ref = forced_scene
+    sc, l_ref, g_ref, n_ref, classes = forced_scene
     ctx = api.context()
     try:
         for k, v in options.items():
@@ -70,8 +82,8 @@ def _check_backward(api, forced_scene, options):
             ctx.set_option(k, v)
     assert st["n_contrib"] == n_ref, (options, st["n_contrib"], n_ref)
     assert abs(loss - l_ref) < 1e-6 * max(1.0, abs(l_ref)), (options, loss, l_ref)
-    scale = max(np.abs(g_ref).max(), 1e-12)
-    assert np.abs(g - g_ref).max() / scale < 1e-3, (options, np.abs(g - g_ref).max(), scale)
+    rep = GT.assert_classwise(g, g_ref, classes, BAR_FORCED, str(options))
+    print(f"{options}: {GT.fmt(rep)}")
     return st
 
 

@@ -5,6 +5,7 @@ streams, and the custom-loss training example (run with `-m gpu`)."""
 import numpy as np
 import pytest
 
+import grad_terms as GT
 from esac_b200.synth import make_scene
 from oracle import esac_oracle as O
 from oracle.score_fp64 import pixel_centres, rodrigues
@@ -23,6 +24,11 @@ SCENES = [
 SCENE_IDS = ["s1", "s2", "s3", "s4", "s5", "forced"]
 # (wRot, wTrans, cut, cut active on some contributing hypothesis)
 LOSSES = [(1.0, 100.0, 0.05, True), (1.0, 100.0, 1e6, False), (1.0, 0.0, 1e6, False), (1.0, 0.0, 0.01, True)]
+
+
+# class-wise bars of test_reference_loss_through_the_node_meets_the_oracle: about 10x the worst class over the five scenes
+# measured on an H100 SXM (80 GB, 700 W) -- minimal 2.44e-6, inlier 6.85e-7, rest 7.47e-6, the figures of esac.backward
+BAR_SCENES = {"minimal": 2.5e-5, "inlier": 7e-6, "rest": 7.5e-5}
 
 
 def _scene(seed, E, H, W, M, kw):
@@ -80,11 +86,12 @@ def test_reference_loss_through_the_node_is_esac_backward(api, seed, E, H, W, M,
 def test_reference_loss_through_the_node_meets_the_oracle(api, seed, E, H, W, M, kw):
     sc = _scene(seed, E, H, W, M, kw)
     g_ref = np.zeros_like(sc.coords)
-    l_ref = O.backward(sc.coords, g_ref, sc.assign, sc.gt_pose, 1.0, 100.0, 100.0, *sc.params, seed=50 + seed)
+    l_ref, bt = O.backward(sc.coords, g_ref, sc.assign, sc.gt_pose, 1.0, 100.0, 100.0, *sc.params, seed=50 + seed, trace=True)
     L, g, *_ = _node(api, sc, 50 + seed, (1.0, 100.0, 100.0))
     assert abs(L - l_ref) < 1e-6 * max(1.0, abs(l_ref))
-    scale = max(np.abs(g_ref).max(), 1e-12)
-    assert np.abs(g - g_ref).max() / scale < 1e-3, (np.abs(g - g_ref).max(), scale)
+    # class-wise (tests/grad_terms.py)
+    rep = GT.assert_classwise(g, g_ref, GT.cell_classes(sc.coords.shape, sc.assign, bt), BAR_SCENES, f"scene {seed}")
+    print(f"scene {seed}: {GT.fmt(rep)}")
 
 
 def test_reference_pose_loss_entry_point_is_the_oracles_loss_and_dloss(api):

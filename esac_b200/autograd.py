@@ -8,6 +8,8 @@ gradient to autograd -- loss * histogram(e_hyps) in the default mode (train_esac
 expert only (train_esac.py:171-173).  CUDA tensors stay on the device."""
 from __future__ import annotations
 
+import operator
+
 import torch
 
 from . import api
@@ -49,42 +51,13 @@ def esac_loss(scene_coordinates, gating_log_probs, hyp_assignment, gt_pose, *par
     return EsacLoss.apply(scene_coordinates, gating_log_probs, hyp_assignment, gt_pose, *params, expert_selection)
 
 
-class EsacLossBatch(torch.autograd.Function):
-    """EsacLoss over a batch of images, on api.backward_batch: forward returns the B expected pose losses, backward hands
-    d loss_b / d scene_coordinates[b] and row b of the gating gradient -- loss_b * histogram(e_hyps[b]), or loss_b at the
-    drawn expert in expert-selection mode -- to autograd, each computed exactly as EsacLoss computes it for one image."""
-
-    @staticmethod
-    def forward(ctx, scene_coordinates, gating_log_probs, hyp_assignment, gt_poses, w_rot, w_trans, loss_cut, shift_x,
-                shift_y, focal_length, ppoint_x, ppoint_y, inlier_threshold, inlier_alpha, inlier_beta, max_reproj,
-                sub_sampling, expert_selection=None):
-        grads = torch.zeros_like(scene_coordinates)
-        losses = api.backward_batch(scene_coordinates.detach(), grads, hyp_assignment, gt_poses, w_rot, w_trans, loss_cut,
-                                    shift_x, shift_y, focal_length, ppoint_x, ppoint_y, inlier_threshold, inlier_alpha,
-                                    inlier_beta, max_reproj, sub_sampling)
-        E = scene_coordinates.shape[1]
-        if expert_selection is None:
-            # [B,1].expand(B,M): a stride-0 row per image, the batched form of expert.expand(M)
-            expert_selection = hyp_assignment.dim() == 2 and hyp_assignment.shape[1] > 1 and hyp_assignment.stride(1) == 0
-        rows = []
-        for b, loss in enumerate(losses):
-            if expert_selection:
-                g = torch.zeros(E)
-                g[int(hyp_assignment[b, 0])] = loss                                      # train_esac.py:171-173
-            else:
-                hist = torch.histc(hyp_assignment[b].float().cpu(), bins=E, min=0, max=E - 1)   # train_esac.py:140
-                g = loss * hist                                                           # train_esac.py:174-176
-            rows.append(g)
-        g_gating = torch.stack(rows).to(gating_log_probs.device).reshape(gating_log_probs.shape)
-        ctx.save_for_backward(grads, g_gating)
-        return scene_coordinates.new_tensor(losses)
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        g_coords, g_gating = ctx.saved_tensors
-        B = grad_out.shape[0]
-        return (g_coords * grad_out.reshape((B,) + (1,) * (g_coords.dim() - 1)),
-                g_gating * grad_out.reshape((B,) + (1,) * (g_gating.dim() - 1))) + (None,) * 16
+def _as_inputs(images):
+    """The images of a batched node as trailing autograd inputs, so that autograd sees every one of them: the stacked
+    tensor alone, or the B tensors of a list / tuple.  Also returns `form`, which turns such a sequence of tensors (the
+    inputs, or tensors made like them) back into the api's argument: the one tensor, or a list."""
+    if api._is_list(images):
+        return tuple(images), list
+    return (images,), operator.itemgetter(0)
 
 
 def _gating_rows(losses, hyp_assignment, E, expert_selection):
@@ -100,18 +73,22 @@ def _gating_rows(losses, hyp_assignment, E, expert_selection):
     return torch.stack(rows)
 
 
-class EsacLossRagged(torch.autograd.Function):
-    """EsacLossBatch on a list of B maps [E,3,H_b,W_b] of different sizes (api.backward_batch on a list).  The maps come
-    last so that autograd sees every one of them; `meta` holds the non-differentiable arguments."""
+class EsacLossBatch(torch.autograd.Function):
+    """EsacLoss over a batch of images, on api.backward_batch: forward returns the B expected pose losses, backward hands
+    d loss_b / d scene_coordinates[b] and row b of the gating gradient -- loss_b * histogram(e_hyps[b]), or loss_b at the
+    drawn expert in expert-selection mode -- to autograd, each computed exactly as EsacLoss computes it for one image.
+    The maps come last (_as_inputs); `meta` holds the non-differentiable arguments."""
 
     @staticmethod
     def forward(ctx, meta, gating_log_probs, *scene_coordinates):
-        hyp_assignment, gt_poses, params, expert_selection = meta
+        form, hyp_assignment, gt_poses, params, expert_selection = meta
         grads = [torch.zeros_like(c) for c in scene_coordinates]
-        losses = api.backward_batch([c.detach() for c in scene_coordinates], grads, hyp_assignment, gt_poses, *params)
+        losses = api.backward_batch(form([c.detach() for c in scene_coordinates]), form(grads), hyp_assignment, gt_poses,
+                                    *params)
         if expert_selection is None:
+            # [B,1].expand(B,M): a stride-0 row per image, the batched form of expert.expand(M)
             expert_selection = hyp_assignment.dim() == 2 and hyp_assignment.shape[1] > 1 and hyp_assignment.stride(1) == 0
-        E = scene_coordinates[0].shape[0]
+        E = scene_coordinates[0].shape[-4]
         g_gating = _gating_rows(losses, hyp_assignment, E, expert_selection)
         ctx.save_for_backward(g_gating.to(gating_log_probs.device).reshape(gating_log_probs.shape), *grads)
         return scene_coordinates[0].new_tensor(losses)
@@ -120,8 +97,10 @@ class EsacLossRagged(torch.autograd.Function):
     def backward(ctx, grad_out):
         g_gating, *g_coords = ctx.saved_tensors
         B = grad_out.shape[0]
+        # the factor of each input: [B,1,1,1,1] for a stacked gradient [B,E,3,H,W], [1,1,1,1] for image b's [E,3,H,W]
+        w = grad_out.reshape((len(g_coords), -1) + (1,) * (g_coords[0].dim() - 1))
         return ((None, g_gating * grad_out.reshape((B,) + (1,) * (g_gating.dim() - 1))) +
-                tuple(g * grad_out[b] for b, g in enumerate(g_coords)))
+                tuple(g * wb for g, wb in zip(g_coords, w)))
 
 
 def esac_loss_batch(scene_coordinates, gating_log_probs, hyp_assignment, gt_poses, *params, expert_selection=None):
@@ -133,38 +112,20 @@ def esac_loss_batch(scene_coordinates, gating_log_probs, hyp_assignment, gt_pose
     expert_selection as for esac_loss, decided for the whole batch (None: a stride-0 [B,1].expand(B,M) assignment).
     scene_coordinates may also be a list or tuple of B [E,3,H_b,W_b] tensors of different sizes; every element then
     receives its own gradient."""
-    if isinstance(scene_coordinates, (list, tuple)):
-        return EsacLossRagged.apply((hyp_assignment, gt_poses, params, expert_selection), gating_log_probs, *scene_coordinates)
-    return EsacLossBatch.apply(scene_coordinates, gating_log_probs, hyp_assignment, gt_poses, *params, expert_selection)
+    inputs, form = _as_inputs(scene_coordinates)
+    return EsacLossBatch.apply((form, hyp_assignment, gt_poses, params, expert_selection), gating_log_probs, *inputs)
 
 
 class ReprojLoss(torch.autograd.Function):
     """ref_expert.py:103-150 as one autograd node: forward = the robust reprojection loss of a batch of predictions
     (mean over the batch of the per-image losses; the reference has one image per step), backward = its gradient, both
-    from the single fused kernel behind api.reproj_loss."""
-
-    @staticmethod
-    def forward(ctx, prediction, gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling, ppoint_x, ppoint_y):
-        grads = torch.empty_like(prediction)
-        losses = api.reproj_loss(prediction.detach(), gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling, ppoint_x,
-                                 ppoint_y, outGradients=grads)
-        ctx.save_for_backward(grads)
-        ctx.batch = len(losses)
-        return prediction.new_tensor(sum(losses) / len(losses))
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        (grads,) = ctx.saved_tensors
-        return (grads * (grad_out / ctx.batch),) + (None,) * 8
-
-
-class ReprojLossRagged(torch.autograd.Function):
-    """ReprojLoss on a list of B predictions [3,H_b,W_b]: the batch mean of the per-image losses, a gradient per element."""
+    from the single fused kernel behind api.reproj_loss.  The predictions come last (_as_inputs)."""
 
     @staticmethod
     def forward(ctx, meta, *prediction):
+        form, args = meta
         grads = [torch.empty_like(p) for p in prediction]
-        losses = api.reproj_loss([p.detach() for p in prediction], *meta, outGradients=grads)
+        losses = api.reproj_loss(form([p.detach() for p in prediction]), *args, outGradients=form(grads))
         ctx.save_for_backward(*grads)
         ctx.batch = len(losses)
         return prediction[0].new_tensor(sum(losses) / len(losses))
@@ -179,39 +140,21 @@ def reproj_loss(prediction, gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_
     opt.cutloss)` followed by `robust_loss.backward()`.  prediction [B,3,H,W] (CUDA), gt_poses [B,4,4] camera->world.
     focal_length, pad_x / pad_y and the principal point are a number or B values, so a batch may mix cameras.
     prediction may also be a list or tuple of B [3,H_b,W_b] tensors of different sizes."""
-    if isinstance(prediction, (list, tuple)):
-        meta = (gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling, ppoint_x, ppoint_y)
-        return ReprojLossRagged.apply(meta, *prediction)
-    return ReprojLoss.apply(prediction, gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling, ppoint_x, ppoint_y)
+    inputs, form = _as_inputs(prediction)
+    args = (gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling, ppoint_x, ppoint_y)
+    return ReprojLoss.apply((form, args), *inputs)
 
 
 class CoordLoss(torch.autograd.Function):
     """init_expert.py:106-132 as one autograd node: forward = the robust scene-coordinate loss of a batch of predictions
     (mean over the batch of the per-image losses; the reference has one image per step), backward = its gradient, both
-    from the fused kernels behind api.coord_loss."""
-
-    @staticmethod
-    def forward(ctx, prediction, gt_coords, cut_loss):
-        grads = torch.empty_like(prediction)
-        losses = api.coord_loss(prediction.detach(), gt_coords, cut_loss, outGradients=grads)
-        ctx.save_for_backward(grads)
-        ctx.batch = len(losses)
-        return prediction.new_tensor(sum(losses) / len(losses))
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        (grads,) = ctx.saved_tensors
-        return (grads * (grad_out / ctx.batch),) + (None,) * 2
-
-
-class CoordLossRagged(torch.autograd.Function):
-    """CoordLoss on lists of B predictions [3,Hp_b,Wp_b] and ground truths: the batch mean, a gradient per prediction."""
+    from the fused kernels behind api.coord_loss.  The predictions come last (_as_inputs)."""
 
     @staticmethod
     def forward(ctx, meta, *prediction):
-        gt_coords, cut_loss = meta
+        form, gt_coords, cut_loss = meta
         grads = [torch.empty_like(p) for p in prediction]
-        losses = api.coord_loss([p.detach() for p in prediction], gt_coords, cut_loss, outGradients=grads)
+        losses = api.coord_loss(form([p.detach() for p in prediction]), gt_coords, cut_loss, outGradients=form(grads))
         ctx.save_for_backward(*grads)
         ctx.batch = len(losses)
         return prediction[0].new_tensor(sum(losses) / len(losses))
@@ -226,9 +169,8 @@ def coord_loss(prediction, gt_coords, cut_loss=100.0):
     (:114-130) become `robust_loss = coord_loss(prediction, gt_coords, opt.cutloss)`, followed by `robust_loss.backward()`.
     prediction [B,3,Hp,Wp] (CUDA), gt_coords [B,3,Hg,Wg], at most 1 apart in H and W; or both lists or tuples of B
     [3,H_b,W_b] tensors of different sizes."""
-    if isinstance(prediction, (list, tuple)):
-        return CoordLossRagged.apply((gt_coords, cut_loss), *prediction)
-    return CoordLoss.apply(prediction, gt_coords, cut_loss)
+    inputs, form = _as_inputs(prediction)
+    return CoordLoss.apply((form, gt_coords, cut_loss), *inputs)
 
 
 # ------------------------------------------------------------------------------------------------
@@ -279,48 +221,28 @@ def esac_hypotheses(scene_coordinates, hyp_assignment, shift_x, shift_y, focal_l
 
 
 class EsacHypothesesBatch(torch.autograd.Function):
-    """EsacHypotheses over a batch of images of one shape (api.hypotheses_forward_batch on [B,E,3,H,W] maps)."""
-
-    @staticmethod
-    def forward(ctx, scene_coordinates, hyp_assignment, *params):
-        scores, poses, contributing, tapes = api.hypotheses_forward_batch(scene_coordinates.detach(), hyp_assignment, *params)
-        ctx.save_for_backward(scene_coordinates, *tapes)
-        ctx.mark_non_differentiable(contributing)
-        ctx.set_materialize_grads(False)
-        ctx.n_params = len(params)
-        return scores, poses, contributing
-
-    @staticmethod
-    @torch.autograd.function.once_differentiable
-    def backward(ctx, grad_scores, grad_poses, _grad_contributing):
-        coords, *tapes = ctx.saved_tensors
-        grads = torch.zeros_like(coords)
-        api.hypotheses_backward_batch(tapes, coords, grads, grad_scores, grad_poses)
-        return (grads, None) + (None,) * ctx.n_params
-
-
-class EsacHypothesesRagged(torch.autograd.Function):
-    """EsacHypothesesBatch on a list of B maps [E,3,H_b,W_b].  The maps come last so that autograd sees every one of them;
-    `meta` holds the non-differentiable arguments."""
+    """EsacHypotheses over a batch of images (api.hypotheses_forward_batch).  The maps come last (_as_inputs); `meta` holds
+    the non-differentiable arguments."""
 
     @staticmethod
     def forward(ctx, meta, *scene_coordinates):
-        hyp_assignment, params = meta
-        scores, poses, contributing, tapes = api.hypotheses_forward_batch([c.detach() for c in scene_coordinates],
+        form, hyp_assignment, params = meta
+        scores, poses, contributing, tapes = api.hypotheses_forward_batch(form([c.detach() for c in scene_coordinates]),
                                                                           hyp_assignment, *params)
+        # the coordinates are passed to the backward again; autograd's version counter catches an in-place change
         ctx.save_for_backward(*scene_coordinates, *tapes)
         ctx.mark_non_differentiable(contributing)
         ctx.set_materialize_grads(False)
-        ctx.B = len(scene_coordinates)
+        ctx.form, ctx.n = form, len(scene_coordinates)
         return scores, poses, contributing
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_scores, grad_poses, _grad_contributing):
         saved = ctx.saved_tensors
-        coords, tapes = list(saved[:ctx.B]), list(saved[ctx.B:])
+        coords, tapes = saved[:ctx.n], list(saved[ctx.n:])
         grads = [torch.zeros_like(c) for c in coords]
-        api.hypotheses_backward_batch(tapes, coords, grads, grad_scores, grad_poses)
+        api.hypotheses_backward_batch(tapes, ctx.form(coords), ctx.form(grads), grad_scores, grad_poses)
         return (None,) + tuple(grads)
 
 
@@ -336,9 +258,8 @@ def esac_hypotheses_batch(scene_coordinates, hyp_assignment, shift_x, shift_y, f
     L and its gradient are those of esac_loss_batch."""
     params = (shift_x, shift_y, focal_length, ppoint_x, ppoint_y, inlier_threshold, inlier_alpha, inlier_beta, max_reproj,
               sub_sampling)
-    if isinstance(scene_coordinates, (list, tuple)):
-        return EsacHypothesesRagged.apply((hyp_assignment, params), *scene_coordinates)
-    return EsacHypothesesBatch.apply(scene_coordinates, hyp_assignment, *params)
+    inputs, form = _as_inputs(scene_coordinates)
+    return EsacHypothesesBatch.apply((form, hyp_assignment, params), *inputs)
 
 
 class ReferencePoseLoss(torch.autograd.Function):

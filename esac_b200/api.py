@@ -136,6 +136,11 @@ def load_library() -> C.CDLL:
     lib.esacb200_forward_async.restype = i32
     lib.esacb200_reserve_forward_async.argtypes = [vp, i32, i32, i32, i32, i32, i32]
     lib.esacb200_reserve_forward_async.restype = i32
+    lib.esacb200_backward_async.argtypes = [vp, i32, vp, vp, i32, i32, i32, vp, i64, i32, vp, f32, f32, f32, vp, vp, f32, f32,
+                                            f32, f32, i32, vp, vp]
+    lib.esacb200_backward_async.restype = i32
+    lib.esacb200_reserve_backward_async.argtypes = [vp, i32, i32, i32, i32, i32, i32]
+    lib.esacb200_reserve_backward_async.restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
         getattr(lib, "esacb200_" + name).restype = i32
@@ -1097,13 +1102,13 @@ def pose_loss(poses, gtPose, wLossRot, wLossTrans, lossCut):
     return losses, dloss
 
 
-def _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras):
-    """Checks the dtypes and shapes of forward_async's inputs (one B) before any context exists; returns (B, E, H, W, M).
-    [E,3,H,W] / [M] / [2] / [3] inputs are one image."""
+def _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras, call="forward_async"):
+    """Checks the dtypes and shapes of the inputs forward_async and backward_async (`call`) share (one B) before any
+    context exists; returns (B, E, H, W, M).  [E,3,H,W] / [M] / [2] / [3] inputs are one image."""
     for t, what in ((sceneCoordinates, "sceneCoordinates"), (hypAssignment, "hypAssignment"), (shifts, "shifts"),
                     (cameras, "cameras")):
         if not _is_torch(t):
-            raise RuntimeError(f"forward_async takes torch CUDA tensors only ({what} is a {type(t).__name__})")
+            raise RuntimeError(f"{call} takes torch CUDA tensors only ({what} is a {type(t).__name__})")
     single = sceneCoordinates.dim() == 4
     _check(sceneCoordinates, "Float", 4 if single else 5, "sceneCoordinates")
     _check(hypAssignment, "Long", 1 if single else 2, "hypAssignment")
@@ -1128,6 +1133,35 @@ def _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras):
     return B, E, H, W, M
 
 
+def _async_context(call, lead, M, inputs, fixed):
+    """The checks forward_async and backward_async (`call`) share after _async_shapes, in this order: every `fixed`
+    argument (name -> (tensor, dtype, trailing shape)) is a contiguous torch tensor of shape lead + trailing shape; the
+    inputs (name -> tensor, hypAssignment among them) are contiguous, hypAssignment row by row; all are CUDA tensors of one
+    device.  Returns the context, on torch's current stream."""
+    for what, (t, dt, tail) in fixed.items():
+        if not _is_torch(t):
+            raise RuntimeError(f"{call} takes torch CUDA tensors only ({what} is a {type(t).__name__})")
+        _check(t, dt, len(lead + tail), what)
+        if tuple(int(v) for v in t.shape) != lead + tail or not t.is_contiguous():
+            raise RuntimeError(f"{what} must be a contiguous {list(lead + tail)} tensor, got {list(t.shape)}")
+    for what, t in inputs.items():
+        if what != "hypAssignment" and not t.is_contiguous():
+            raise RuntimeError(f"{what} must be contiguous (a copy would not be captured with the call)")
+    hypAssignment = inputs["hypAssignment"]
+    if lead and lead[0] > 1 and hypAssignment.stride(0) != M * hypAssignment.stride(-1):
+        raise RuntimeError("hypAssignment must hold its rows back to back (row stride M times the element stride)")
+    args = dict(inputs, **{what: t for what, (t, _, _) in fixed.items()})
+    for what, t in args.items():
+        if not t.is_cuda:
+            raise RuntimeError(f"{call} takes CUDA tensors only ({what} is on the CPU)")
+    devs = {t.device.index for t in args.values()}
+    if len(devs) > 1:
+        raise RuntimeError(f"esac_b200: tensors live on different CUDA devices {sorted(devs)}")
+    ctx = _pick_ctx(*devs)
+    ctx.async_used = True
+    return ctx
+
+
 def forward_async(sceneCoordinates, hypAssignment, shifts, cameras, inlierThreshold, inlierAlpha, inlierBeta, maxReproj,
                   subSampling, outPoses, outExperts, outStatus):
     """esac.forward enqueued on torch's current stream with no host synchronisation, so it can be captured in a CUDA graph
@@ -1140,28 +1174,10 @@ def forward_async(sceneCoordinates, hypAssignment, shifts, cameras, inlierThresh
     the largest shape before the first capture; once captured, the workspace never grows again."""
     B, E, H, W, M = _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras)
     lead = (B,) if sceneCoordinates.dim() == 5 else ()
-    for t, dt, tail, what in ((outPoses, "Float", (4, 4), "outPoses"), (outExperts, "Long", (), "outExperts"),
-                              (outStatus, "Int", (), "outStatus")):
-        if not _is_torch(t):
-            raise RuntimeError(f"forward_async takes torch CUDA tensors only ({what} is a {type(t).__name__})")
-        _check(t, dt, len(lead + tail), what)
-        if tuple(int(v) for v in t.shape) != lead + tail or not t.is_contiguous():
-            raise RuntimeError(f"{what} must be a contiguous {list(lead + tail)} tensor, got {list(t.shape)}")
-    for t, what in ((sceneCoordinates, "sceneCoordinates"), (shifts, "shifts"), (cameras, "cameras")):
-        if not t.is_contiguous():
-            raise RuntimeError(f"{what} must be contiguous (a copy would not be captured with the call)")
-    if lead and B > 1 and hypAssignment.stride(0) != M * hypAssignment.stride(-1):
-        raise RuntimeError("hypAssignment must hold its rows back to back (row stride M times the element stride)")
-    args = {"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment, "shifts": shifts, "cameras": cameras,
-            "outPoses": outPoses, "outExperts": outExperts, "outStatus": outStatus}
-    for what, t in args.items():
-        if not t.is_cuda:
-            raise RuntimeError(f"forward_async takes CUDA tensors only ({what} is on the CPU)")
-    devs = {t.device.index for t in args.values()}
-    if len(devs) > 1:
-        raise RuntimeError(f"esac_b200: tensors live on different CUDA devices {sorted(devs)}")
-    ctx = _pick_ctx(*devs)
-    ctx.async_used = True
+    ctx = _async_context("forward_async", lead, M, {"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment,
+                                                    "shifts": shifts, "cameras": cameras},
+                         {"outPoses": (outPoses, "Float", (4, 4)), "outExperts": (outExperts, "Long", ()),
+                          "outStatus": (outStatus, "Int", ())})
     ctx.check(ctx.lib.esacb200_forward_async(ctx.handle, B, sceneCoordinates.data_ptr(), E, H, W, hypAssignment.data_ptr(),
                                              int(hypAssignment.stride(-1)), M, shifts.data_ptr(), cameras.data_ptr(),
                                              float(inlierThreshold), float(inlierAlpha), float(inlierBeta), float(maxReproj),
@@ -1177,6 +1193,44 @@ def reserve_forward_async(B: int, E: int, H: int, W: int, M: int, subSampling: i
     ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
     ctx.async_used = True
     ctx.check(ctx.lib.esacb200_reserve_forward_async(ctx.handle, int(B), int(E), int(H), int(W), int(M), int(subSampling)))
+
+
+def backward_async(sceneCoordinates, outGradients, hypAssignment, gtPoses, shifts, cameras, wLossRot, wLossTrans, lossCut,
+                   inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling, outLosses, outStatus):
+    """esac.backward enqueued on torch's current stream with no host synchronisation, so a training step can be captured
+    in a CUDA graph (torch.cuda.graph).  CUDA tensors only: sceneCoordinates float32 [B,E,3,H,W], outGradients float32
+    [B,E,3,H,W] (accumulated, +=, as esac.backward), hypAssignment int64 [B,M], gtPoses float32 [B,4,4] (camera->world),
+    shifts int32 [B,2], cameras float32 [B,3] (focal length, ppointX, ppointY); the results go to outLosses float64 [B]
+    (what esac.backward returns) and outStatus int32 [B] (0 = OK, 1 = an expert index outside [0,E): loss NaN, gradient
+    slice untouched).  [E,3,H,W] / [M] / [4,4] / [2] / [3] / [] tensors are one image.  The seed, ground truth, shift and
+    camera are read on the device when the kernels run.  forward_async and backward_async share one call counter: image b
+    of the j-th call after set_seed(s) draws what the (j*B + b)-th esac.forward / esac.backward after set_seed(s) draws,
+    and the results are bitwise esac.backward's.  Call reserve_backward_async with the largest shape before the first
+    capture; once captured, the workspace never grows again."""
+    B, E, H, W, M = _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras, "backward_async")
+    lead = (B,) if sceneCoordinates.dim() == 5 else ()
+    ctx = _async_context("backward_async", lead, M, {"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment,
+                                                     "shifts": shifts, "cameras": cameras},
+                         {"outGradients": (outGradients, "Float", (E, 3, H, W)), "gtPoses": (gtPoses, "Float", (4, 4)),
+                          "outLosses": (outLosses, "Double", ()), "outStatus": (outStatus, "Int", ())})
+    ctx.check(ctx.lib.esacb200_backward_async(ctx.handle, B, sceneCoordinates.data_ptr(), outGradients.data_ptr(), E, H, W,
+                                              hypAssignment.data_ptr(), int(hypAssignment.stride(-1)), M, gtPoses.data_ptr(),
+                                              float(wLossRot), float(wLossTrans), float(lossCut), shifts.data_ptr(),
+                                              cameras.data_ptr(), float(inlierThreshold), float(inlierAlpha),
+                                              float(inlierBeta), float(maxReproj), int(subSampling), outLosses.data_ptr(),
+                                              outStatus.data_ptr()))
+
+
+def reserve_backward_async(B: int, E: int, H: int, W: int, M: int, subSampling: int = 8, device: int | None = None):
+    """Sizes backward_async's workspace (which forward_async shares) for this shape; call it before capturing (it
+    allocates)."""
+    if min(int(B), int(E), int(H), int(W), int(M)) < 1:
+        raise RuntimeError(f"reserve_backward_async: sizes must be positive, got B={B} E={E} H={H} W={W} M={M}")
+    ctx = context(device)
+    import torch
+    ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
+    ctx.async_used = True
+    ctx.check(ctx.lib.esacb200_reserve_backward_async(ctx.handle, int(B), int(E), int(H), int(W), int(M), int(subSampling)))
 
 
 def set_seed(seed: int, device: int | None = None):

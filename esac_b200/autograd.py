@@ -116,6 +116,70 @@ def esac_loss_batch(scene_coordinates, gating_log_probs, hyp_assignment, gt_pose
     return EsacLossBatch.apply((form, hyp_assignment, gt_poses, params, expert_selection), gating_log_probs, *inputs)
 
 
+def _gating_grad(losses, hyp_assignment, E, expert_selection):
+    """The gating gradient of esac_loss / esac_loss_batch computed on the assignment's device, with no host round trip:
+    losses float64 [B], hyp_assignment int64 [B,M].  Row b is loss_b at the drawn expert (expert selection), or loss_b
+    times the histogram of row b.  Rounded as esac_loss rounds: the float64 loss becomes a float32 first, and the product
+    with the float32 histogram is a float32 product (torch multiplies a float32 tensor by a Python float in float32).
+    Indices outside [0, E) (an image backward_async flags, whose loss is NaN) are counted nowhere."""
+    loss32 = losses.float()[:, None]
+    valid = (hyp_assignment >= 0) & (hyp_assignment < E)
+    index = torch.where(valid, hyp_assignment, torch.zeros_like(hyp_assignment))
+    g = torch.zeros(hyp_assignment.shape[0], E, device=hyp_assignment.device)
+    if expert_selection:
+        return g.scatter_(1, index[:, :1], loss32)                                           # train_esac.py:171-173
+    counts = g.scatter_add_(1, index, valid.float())                                         # train_esac.py:140
+    return loss32 * counts                                                                    # train_esac.py:174-176
+
+
+class EsacLossAsync(torch.autograd.Function):
+    """esac_loss / esac_loss_batch on api.backward_async: no host synchronisation in the forward or the backward, so the
+    node, and loss.backward() through it, can be captured in a CUDA graph.  The forward returns the expected losses as
+    float32, as esac_loss does; `meta` holds the non-differentiable arguments."""
+
+    @staticmethod
+    def forward(ctx, meta, gating_log_probs, scene_coordinates):
+        hyp_assignment, gt_poses, shifts, cameras, params, expert_selection, status = meta
+        grads = torch.zeros_like(scene_coordinates)
+        lead = scene_coordinates.shape[:-4]
+        losses = torch.empty(lead, dtype=torch.float64, device=scene_coordinates.device)
+        if status is None:
+            status = torch.empty(lead, dtype=torch.int32, device=scene_coordinates.device)
+        w_rot, w_trans, loss_cut, tau, alpha, beta, max_reproj, sub = params
+        api.backward_async(scene_coordinates.detach(), grads, hyp_assignment, gt_poses, shifts, cameras, w_rot, w_trans,
+                           loss_cut, tau, alpha, beta, max_reproj, sub, losses, status)
+        E = scene_coordinates.shape[-4]
+        M = hyp_assignment.shape[-1]
+        if expert_selection is None:
+            # a stride-0 `expert.expand(M)` view (one image: the batched form needs its rows back to back)
+            expert_selection = hyp_assignment.dim() == 1 and M > 1 and hyp_assignment.stride(0) == 0
+        g_gating = _gating_grad(losses.reshape(-1), hyp_assignment.reshape(-1, M), E, expert_selection)
+        ctx.save_for_backward(g_gating.reshape(gating_log_probs.shape), grads)
+        return losses.float()
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        g_gating, g_coords = ctx.saved_tensors
+        w = grad_out.reshape(grad_out.shape + (1,) * 4)
+        return None, g_gating * grad_out.reshape(grad_out.shape + (1,) * (g_gating.dim() - grad_out.dim())), g_coords * w
+
+
+def esac_loss_async(scene_coordinates, gating_log_probs, hyp_assignment, gt_poses, shifts, cameras, w_rot, w_trans, loss_cut,
+                    tau, alpha, beta, max_reproj, sub_sampling, expert_selection=None, status=None):
+    """esac_loss (one image: scene_coordinates [E,3,H,W], hyp_assignment [M], gt_poses [4,4], shifts [2], cameras [3]) or
+    esac_loss_batch (scene_coordinates [B,E,3,H,W], gating_log_probs [B,E], hyp_assignment [B,M], gt_poses [B,4,4], shifts
+    [B,2] int32, cameras [B,3] = focal length, ppointX, ppointY) on api.backward_async, for training steps captured in a CUDA
+    graph: CUDA tensors only, the shifts, cameras and ground truth read on the device at replay time.  The losses,
+    coordinate gradients and gating gradients are bitwise those of esac_loss for the same draws; image b of the j-th call
+    draws what the (j*B + b)-th esac_loss call draws.  expert_selection as for esac_loss (None: a stride-0 one-image
+    assignment means expert selection).  status: an int32 CUDA tensor [B] (or [] for one image) that receives
+    backward_async's per-image status (1 = a bad expert index: that loss is NaN, its gradients are NaN or zero); None
+    keeps it internal."""
+    meta = (hyp_assignment, gt_poses, shifts, cameras, (w_rot, w_trans, loss_cut, tau, alpha, beta, max_reproj, sub_sampling),
+            expert_selection, status)
+    return EsacLossAsync.apply(meta, gating_log_probs, scene_coordinates)
+
+
 class ReprojLoss(torch.autograd.Function):
     """ref_expert.py:103-150 as one autograd node: forward = the robust reprojection loss of a batch of predictions
     (mean over the batch of the per-image losses; the reference has one image per step), backward = its gradient, both

@@ -82,13 +82,16 @@ __device__ __forceinline__ void job_record(const BwdArgs& a, int j, int h, HypGr
 // ---------------------------------------------------------------------------------------------
 // B1: losses, expectation, score gradients, per-job records
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(1024) bwd_loss_kernel(const __grid_constant__ BwdArgs a, BwdAux x) {
+// DEV: the ground truth from dv.gt (stream-ordered backward)
+template <bool DEV>
+__global__ void __launch_bounds__(1024) bwd_loss_kernel(const __grid_constant__ BwdArgs a, BwdAux x,
+                                                        const __grid_constant__ BwdDev dv) {
     const Problem& P = a.P;
     __shared__ Pose gtp;
     __shared__ double gtT[16];
     __shared__ double expected;
     const int tid = threadIdx.x;
-    if (tid == 0) gt_trans2pose(a.gt, gtp, gtT);
+    if (tid == 0) gt_trans2pose(DEV ? dv.gt : a.gt, gtp, gtT);
     for (int e = tid; e < P.E; e += blockDim.x) x.expert_njobs[e] = 0;
     __syncthreads();
     for (int h = tid; h < P.M; h += blockDim.x) {
@@ -142,6 +145,7 @@ __device__ __forceinline__ double score_weight(float err_clamped, const Problem&
     return (-st * (1 - st) * (double)P.beta * g) * fac;
 }
 
+template <bool DEV>
 __device__ __forceinline__ void block_reduce_store(double (&v)[kRed], double* dst) {
     __shared__ double sred[kBwdThreads / 32][kRed];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -162,11 +166,14 @@ __device__ __forceinline__ void block_reduce_store(double (&v)[kRed], double* ds
 // ---------------------------------------------------------------------------------------------
 // B2: per (job, tile) partial sums of J^T J (refined pose, final inliers) and sum w * jacobeanHyp (initial pose)
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kBwdThreads) bwd_reduce_kernel(const __grid_constant__ BwdArgs a, BwdAux x) {
+template <bool DEV>
+__global__ void __launch_bounds__(kBwdThreads) bwd_reduce_kernel(const __grid_constant__ BwdArgs a, BwdAux x,
+                                                                 const __grid_constant__ BwdDev dv) {
     const Problem& P = a.P;
     const int nc = *a.n_contrib;
     const int n_items = nc * x.tiles;
-    const double f = (double)P.f, cx = (double)P.ppx, cy = (double)P.ppy, mr = (double)P.max_reproj;
+    const double f = (double)dev_f<DEV>(P, dv), cx = (double)dev_ppx<DEV>(P, dv), cy = (double)dev_ppy<DEV>(P, dv),
+                 mr = (double)P.max_reproj;
     const float facf = P.alpha / (float)P.W / (float)P.H;
     __shared__ HypGrad sg;
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
@@ -183,8 +190,8 @@ __global__ void __launch_bounds__(kBwdThreads) bwd_reduce_kernel(const __grid_co
             const int p = tile * kBwdTile + k * kBwdThreads + threadIdx.x;
             if (p >= P.N) continue;
             const int yy = p / P.W, xx = p - yy * P.W;
-            const float px = (float)(xx * P.sub + P.sub / 2 - P.shiftX);
-            const float py = (float)(yy * P.sub + P.sub / 2 - P.shiftY);
+            const float px = (float)(xx * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, dv));
+            const float py = (float)(yy * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, dv));
             const float X = pl[p], Y = pl[P.N + p], Z = pl[2 * (size_t)P.N + p];
             double row[6];
             if (sg.flagI && ((mask[p >> 5] >> (p & 31)) & 1u)) {
@@ -205,14 +212,16 @@ __global__ void __launch_bounds__(kBwdThreads) bwd_reduce_kernel(const __grid_co
                 for (int i = 0; i < 6; ++i) acc[21 + i] += w * row[i];
             }
         }
-        block_reduce_store(acc, x.red + ((size_t)j * x.tiles + tile) * kRed);
+        block_reduce_store<DEV>(acc, x.red + ((size_t)j * x.tiles + tile) * kRed);
     }
 }
 
 // ---------------------------------------------------------------------------------------------
 // B3: per job small algebra: pinv(J^T J), v, dPNP by central differences (18 P3P solves on 18 lanes), support
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(32) bwd_solve_kernel(const __grid_constant__ BwdArgs a, BwdAux x) {
+template <bool DEV>
+__global__ void __launch_bounds__(32) bwd_solve_kernel(const __grid_constant__ BwdArgs a, BwdAux x,
+                                                       const __grid_constant__ BwdDev dv) {
     const Problem& P = a.P;
     const int nc = *a.n_contrib;
     const int lane = threadIdx.x;
@@ -238,8 +247,8 @@ __global__ void __launch_bounds__(32) bwd_solve_kernel(const __grid_constant__ B
                 const int cxq = g.cells[2 * q], cyq = g.cells[2 * q + 1];
                 const int p = cyq * P.W + cxq;
                 obj[q][0] = pl[p]; obj[q][1] = pl[P.N + p]; obj[q][2] = pl[2 * (size_t)P.N + p];
-                img[q][0] = (float)(cxq * P.sub + P.sub / 2 - P.shiftX);
-                img[q][1] = (float)(cyq * P.sub + P.sub / 2 - P.shiftY);
+                img[q][0] = (float)(cxq * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, dv));
+                img[q][1] = (float)(cyq * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, dv));
             }
             const int col = lane >> 1, dir = lane & 1, pi = col / 3, pj = col % 3;
             const float eps = 0.001f;
@@ -255,7 +264,8 @@ __global__ void __launch_bounds__(32) bwd_solve_kernel(const __grid_constant__ B
             float vbw = vfw - 2 * eps;
             obj[pi][pj] = dir == 0 ? vfw : vbw;
             Pose ps;
-            const bool ok = p3p_pose(obj, img, (double)P.f, (double)P.ppx, (double)P.ppy, ps);
+            const bool ok =
+                p3p_pose(obj, img, (double)dev_f<DEV>(P, dv), (double)dev_ppx<DEV>(P, dv), (double)dev_ppy<DEV>(P, dv), ps);
             okf[lane] = ok ? 1 : 0;
             for (int q = 0; q < 3; ++q) { fb[lane][q] = ps.r[q]; fb[lane][3 + q] = ps.t[q]; }
         }
@@ -308,11 +318,14 @@ __global__ void __launch_bounds__(32) bwd_solve_kernel(const __grid_constant__ B
 // ---------------------------------------------------------------------------------------------
 // B4: max |J_R| = max_cells,k |(pinv(A) J_cell^T)_k|  (esac.cpp:434-437 clamp)
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kBwdThreads) bwd_maxjr_kernel(const __grid_constant__ BwdArgs a, BwdAux x) {
+template <bool DEV>
+__global__ void __launch_bounds__(kBwdThreads) bwd_maxjr_kernel(const __grid_constant__ BwdArgs a, BwdAux x,
+                                                                const __grid_constant__ BwdDev dv) {
     const Problem& P = a.P;
     const int nc = *a.n_contrib;
     const int n_items = nc * x.tiles;
-    const double f = (double)P.f, cx = (double)P.ppx, cy = (double)P.ppy, mr = (double)P.max_reproj;
+    const double f = (double)dev_f<DEV>(P, dv), cx = (double)dev_ppx<DEV>(P, dv), cy = (double)dev_ppy<DEV>(P, dv),
+                 mr = (double)P.max_reproj;
     __shared__ HypGrad sg;
     __shared__ double smax[kBwdThreads / 32];
     for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
@@ -329,8 +342,8 @@ __global__ void __launch_bounds__(kBwdThreads) bwd_maxjr_kernel(const __grid_con
             if (p >= P.N) continue;
             if (!((mask[p >> 5] >> (p & 31)) & 1u)) continue;
             const int yy = p / P.W, xx = p - yy * P.W;
-            const float px = (float)(xx * P.sub + P.sub / 2 - P.shiftX);
-            const float py = (float)(yy * P.sub + P.sub / 2 - P.shiftY);
+            const float px = (float)(xx * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, dv));
+            const float py = (float)(yy * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, dv));
             double row[6];
             if (!jac_row(sg.Rr, sg.tr, sg.dRr, f, cx, cy, pl[p], pl[P.N + p], pl[2 * (size_t)P.N + p], px, py, mr, row)) continue;
 #pragma unroll
@@ -354,70 +367,25 @@ __global__ void __launch_bounds__(kBwdThreads) bwd_maxjr_kernel(const __grid_con
 // ---------------------------------------------------------------------------------------------
 // B5: assembly, one thread per cell, hypotheses of the cell's expert in ascending order
 // ---------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kBwdThreads) bwd_assemble_kernel(const __grid_constant__ BwdArgs a, BwdAux x) {
+template <bool DEV>
+__global__ void __launch_bounds__(kBwdThreads) bwd_assemble_kernel(const __grid_constant__ BwdArgs a, BwdAux x,
+                                                                   const __grid_constant__ BwdDev dv) {
     const Problem& P = a.P;
-    const int e = blockIdx.y;
-    if (x.expert_njobs[e] == 0) return;
-    const int nc = *a.n_contrib;
-    const double f = (double)P.f, cx = (double)P.ppx, cy = (double)P.ppy, mr = (double)P.max_reproj;
-    const float facf = P.alpha / (float)P.W / (float)P.H;
-    const int p = blockIdx.x * kBwdThreads + threadIdx.x;
-    const bool live = p < P.N;
-    const float* pl = a.coords + (size_t)e * 3 * P.N;
-    float* gr = a.grads + (size_t)e * 3 * P.N;
-    float X = 0, Y = 0, Z = 0, px = 0, py = 0;
-    int xx = 0, yy = 0;
-    float o0 = 0, o1 = 0, o2 = 0;
-    if (live) {
-        yy = p / P.W; xx = p - yy * P.W;
-        px = (float)(xx * P.sub + P.sub / 2 - P.shiftX);
-        py = (float)(yy * P.sub + P.sub / 2 - P.shiftY);
-        X = pl[p]; Y = pl[P.N + p]; Z = pl[2 * (size_t)P.N + p];
-        o0 = gr[p]; o1 = gr[P.N + p]; o2 = gr[2 * (size_t)P.N + p];
-    }
-    __shared__ HypGrad sg;
-    for (int j = 0; j < nc; ++j) {
-        if (x.hg[j].expert != e) continue;  // uniform
-        __syncthreads();
-        for (int i = threadIdx.x; i < (int)(sizeof(HypGrad) / 8); i += blockDim.x) ((double*)&sg)[i] = ((const double*)&x.hg[j])[i];
-        __syncthreads();
-        if (!live) continue;
-        double g0, g1, g2;
-        {   // path II: direct influence on the score at the initial pose (esac_derivative.h:303-306)
-            float err = repro_err_f(sg.Ri, sg.ti, f, cx, cy, X, Y, Z, px, py);
-            err = (P.max_reproj < err) ? P.max_reproj : err;
-            const double w = score_weight(err, P, sg.g, (double)facf);
-            double d[3];
-            d_project_d_obj(px, py, X, Y, Z, sg.Ri, sg.ti, f, cx, cy, mr, d);
-            g0 = d[0] * w; g1 = d[1] * w; g2 = d[2] * w;
-#pragma unroll
-            for (int q = 0; q < 4; ++q)
-                if (sg.cells[2 * q] == xx && sg.cells[2 * q + 1] == yy) {
-                    g0 += sg.support[3 * q]; g1 += sg.support[3 * q + 1]; g2 += sg.support[3 * q + 2];
-                }
-        }
-        double h0 = 0, h1 = 0, h2 = 0;
-        if (sg.flagI) {  // path I: through the refined pose (esac.cpp:442-449, 461-462)
-            const uint32_t* mask = a.masks + ((size_t)j * 2 + sg.pad) * a.mask_words;
-            const double maxjr = __longlong_as_double((long long)sg.maxjr_bits);
-            if (((mask[p >> 5] >> (p & 31)) & 1u) && !(maxjr > 10)) {
-                double row[6];
-                double s = 0;
-                if (jac_row(sg.Rr, sg.tr, sg.dRr, f, cx, cy, X, Y, Z, px, py, mr, row)) {
-#pragma unroll
-                    for (int i = 0; i < 6; ++i) s += sg.v[i] * row[i];
-                }
-                double d[3];
-                d_project_d_obj(px, py, X, Y, Z, sg.Rr, sg.tr, f, cx, cy, mr, d);
-                h0 = s * d[0]; h1 = s * d[1]; h2 = s * d[2];
-            }
-        }
-        // outGradients += hypProbs*gradients + dLoss_dScore : float += double (esac.cpp:501-506)
-        o0 = (float)((double)o0 + (sg.p * h0 + g0));
-        o1 = (float)((double)o1 + (sg.p * h1 + g1));
-        o2 = (float)((double)o2 + (sg.p * h2 + g2));
-    }
-    if (live) { gr[p] = o0; gr[P.N + p] = o1; gr[2 * (size_t)P.N + p] = o2; }
+#include "bwd_assemble_body.inc"
+}
+
+// The stream-ordered instantiation: the image's shift and camera from device memory, and an image whose assignment holds a
+// bad expert index (the prep flag) keeps its gradient untouched.  The body is the eager kernel's, text for text: reading the
+// camera any other way in the eager kernel itself would change its code.
+template <>
+__global__ void __launch_bounds__(kBwdThreads) bwd_assemble_kernel<true>(const __grid_constant__ BwdArgs a, BwdAux x,
+                                                                         const __grid_constant__ BwdDev dv) {
+    if (__ldg(dv.flags)) return;
+    Problem Pd = a.P;
+    Pd.shiftX = dev_shift_x<true>(a.P, dv); Pd.shiftY = dev_shift_y<true>(a.P, dv);
+    Pd.f = dev_f<true>(a.P, dv); Pd.ppx = dev_ppx<true>(a.P, dv); Pd.ppy = dev_ppy<true>(a.P, dv);
+    const Problem& P = Pd;
+#include "bwd_assemble_body.inc"
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -510,35 +478,59 @@ static BwdAux bwd_aux(const BwdArgs& a) {
     return x;
 }
 
-static void launch_backward_tail(const BwdArgs& a, const BwdAux& x, int max_jobs, int sm_count, cudaStream_t st);
+template <bool DEV>
+static void launch_backward_tail(const BwdArgs& a, const BwdAux& x, const BwdDev& dv, int max_jobs, int sm_count, cudaStream_t st);
 
 void launch_backward_losses(const BwdArgs& a, cudaStream_t st) {
-    bwd_loss_kernel<<<1, 1024, 0, st>>>(a, bwd_aux(a));
+    bwd_loss_kernel<false><<<1, 1024, 0, st>>>(a, bwd_aux(a), BwdDev());
 }
 
-void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t st) {
+void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t st, const BwdDev* dev) {
     const BwdAux x = bwd_aux(a);
-    bwd_loss_kernel<<<1, 1024, 0, st>>>(a, x);
-    launch_backward_tail(a, x, max_jobs, sm_count, st);
+    if (dev) {
+        bwd_loss_kernel<true><<<1, 1024, 0, st>>>(a, x, *dev);
+        launch_backward_tail<true>(a, x, *dev, max_jobs, sm_count, st);
+    } else {
+        bwd_loss_kernel<false><<<1, 1024, 0, st>>>(a, x, BwdDev());
+        launch_backward_tail<false>(a, x, BwdDev(), max_jobs, sm_count, st);
+    }
 }
 
 void launch_backward_upstream(const BwdArgs& a, const void* tape, const double* d_scores, const double* d_poses6, int max_jobs,
                               int sm_count, cudaStream_t st) {
     const BwdAux x = bwd_aux(a);
     bwd_upstream_kernel<<<1, 1024, 0, st>>>(a, x, (const HypGrad*)((const char*)tape + tape_records_offset()), d_scores, d_poses6);
-    launch_backward_tail(a, x, max_jobs, sm_count, st);
+    launch_backward_tail<false>(a, x, BwdDev(), max_jobs, sm_count, st);
 }
 
 // B2-B5: everything after the per-job records, shared by the loss-driven backward and the hypotheses node.
-static void launch_backward_tail(const BwdArgs& a, const BwdAux& x, int max_jobs, int sm_count, cudaStream_t st) {
+template <bool DEV>
+static void launch_backward_tail(const BwdArgs& a, const BwdAux& x, const BwdDev& dv, int max_jobs, int sm_count, cudaStream_t st) {
     long long items = (long long)max_jobs * x.tiles;
     int grid = (int)(items < sm_count * 8ll ? items : sm_count * 8ll);
     if (grid < 1) grid = 1;
-    bwd_reduce_kernel<<<grid, kBwdThreads, 0, st>>>(a, x);
-    bwd_solve_kernel<<<max_jobs < sm_count * 4 ? max_jobs : sm_count * 4, 32, 0, st>>>(a, x);
-    bwd_maxjr_kernel<<<grid, kBwdThreads, 0, st>>>(a, x);
+    bwd_reduce_kernel<DEV><<<grid, kBwdThreads, 0, st>>>(a, x, dv);
+    bwd_solve_kernel<DEV><<<max_jobs < sm_count * 4 ? max_jobs : sm_count * 4, 32, 0, st>>>(a, x, dv);
+    bwd_maxjr_kernel<DEV><<<grid, kBwdThreads, 0, st>>>(a, x, dv);
     dim3 ga((a.P.N + kBwdThreads - 1) / kBwdThreads, a.P.E);
-    bwd_assemble_kernel<<<ga, kBwdThreads, 0, st>>>(a, x);
+    bwd_assemble_kernel<DEV><<<ga, kBwdThreads, 0, st>>>(a, x, dv);
+}
+
+// esac.backward's return value for a stream-ordered image: the expected loss (NaN on a bad assignment) and the status; the
+// last image of an execution advances the async call counter.
+__global__ void finish_backward_async_kernel(const double* stats, const int* flags, double* loss, int* status,
+                                             unsigned long long* seed, int advance) {
+    if (threadIdx.x == 0) {
+        const int bad = flags[0];
+        *loss = bad ? __longlong_as_double(0x7ff8000000000000ll) : stats[4];
+        *status = bad;
+        if (advance) seed[1] += (unsigned long long)advance;
+    }
+}
+
+void launch_finish_backward_async(const double* stats, const int* flags, double* loss, int* status, unsigned long long* seed,
+                                  int advance, cudaStream_t st) {
+    finish_backward_async_kernel<<<1, 32, 0, st>>>(stats, flags, loss, status, seed, advance);
 }
 
 // dst += src (the rank-summed gradient of a hypothesis-major sharded backward joins the caller's tensor: esac.cpp:501-506 is +=)

@@ -119,9 +119,9 @@ struct esacb200_ctx {
     int comm_world = 1, comm_rank = 0;
     DevBuf gathered, grads_work;
     std::vector<esacb200_ctx*> workers;  // lazily created contexts of esacb200_backward_batch (own stream + workspace each)
-    // Stream-ordered forward (esacb200_forward_async): its own context, so that eager calls never touch the buffers a
-    // captured graph holds.  In that context: is_async = true, seed_state = device {base seed, async calls}, and frozen once
-    // a capture has used the workspace (from then on nothing in it is freed or reallocated).
+    // Stream-ordered forward and backward (esacb200_forward_async / _backward_async): their own context, so that eager calls
+    // never touch the buffers a captured graph holds.  In that context: is_async = true, seed_state = device {base seed,
+    // async calls}, and frozen once a capture has used the workspace (from then on nothing in it is freed or reallocated).
     esacb200_ctx* async = nullptr;
     bool is_async = false;
     bool frozen = false;
@@ -245,14 +245,16 @@ struct Plan {
     const long long* d_assign;
     long long assign_stride;
     int split_e = 0;  // > 0: host maps are uploaded in two halves [0, split_e) / [split_e, E) on the copy stream (ev_copied[0/1])
-    const struct AsyncImage* async = nullptr;  // stream-ordered forward: device parameters and the caller's outputs
+    const struct AsyncImage* async = nullptr;  // stream-ordered call: device parameters and the caller's outputs
 };
 
-// One image of a stream-ordered forward: what its kernels read from device memory, and where its results go.
+// One image of a stream-ordered forward or backward: what its kernels read from device memory, and where its results go.
 struct AsyncImage {
     DevParams dev;
-    float* pose;        // [4,4]
-    long long* expert;
+    float* pose;        // [4,4] (forward)
+    long long* expert;  // (forward)
+    double* loss;       // (backward) esac.backward's return value
+    const float* gt;    // (backward) [4,4] camera->world ground truth
     int* status;
     int advance;        // the last image of an execution: advance the async call counter by B
 };
@@ -525,24 +527,8 @@ int run_score(esacb200_ctx* ctx, const Plan& pl) {
     return 0;
 }
 
-int pick_group(esacb200_ctx* ctx, const Problem& P, int jobs_hint) {
-    const int opt = ctx->opt.refine_group_opt;
-    if (opt > 0) return opt < ctx->refine_coresident ? opt : ctx->refine_coresident;
-    const int words = (P.N + 31) / 32;
-    // ~320 cells per CTA, up to every co-resident CTA: with the warp-parallel slot summation the inter-CTA barrier costs less
-    // than the fp64 work it spreads (60x80 -> 16 CTAs, 480x640 -> every co-resident CTA)
-    int g = words / 10;
-    if (g < 1) g = 1;
-    // Jobs are handed out dynamically inside the kernel, so a group may work through several jobs: fewer, larger groups even
-    // out the differing job lengths (rounds x LM iterations) -- worth it only while a block's share of the map stays large
-    // against the cost of a group exchange (480x640: yes; 60x80: no)
-    int waves = jobs_hint >= 8 ? ctx->opt.refine_jobs_per_group : 1;
-    int concurrent = jobs_hint > 0 ? (jobs_hint + waves - 1) / waves : 1;
-    int cap = ctx->refine_coresident / concurrent;
-    if (waves > 1 && (cap < 1 || P.N / (cap < 1 ? 1 : cap) < 4096)) cap = ctx->refine_coresident / (jobs_hint > 0 ? jobs_hint : 1);
-    if (cap < 1) cap = 1;
-    if (g > cap) g = cap;
-    return g;
+int pick_group(const esacb200_ctx* ctx, const Problem& P, int jobs_hint) {
+    return refine_group_rule(P.N, ctx->refine_coresident, ctx->opt.refine_group_opt, ctx->opt.refine_jobs_per_group, jobs_hint);
 }
 
 // Refinement of `n_jobs` (host count, or device scalar when d_njobs != null) hypotheses listed in d_jobs.
@@ -551,12 +537,29 @@ struct RefineSizes {
     int n_groups, cache;
     size_t masks, rounds, scratch, n_flags, barrier, clist;
 };
+// group 0: picked on the device from the job count (stream-ordered backward).  The sizes are then the largest of every group
+// a count in 1..max_jobs may pick, cache is 1 when any of them caches, and n_groups is the CTA count of the largest launch.
 RefineSizes refine_sizes(const esacb200_ctx* ctx, const Problem& P, int max_jobs, int group) {
     RefineSizes z;
+    if (group == 0) {
+        z = refine_sizes(ctx, P, max_jobs, pick_group(ctx, P, 1));
+        z.n_groups *= pick_group(ctx, P, 1);
+        for (int n = 2, last = pick_group(ctx, P, 1); n <= max_jobs; ++n) {
+            const int g = pick_group(ctx, P, n);
+            if (g == last) continue;
+            last = g;
+            const RefineSizes y = refine_sizes(ctx, P, max_jobs, g);
+            z.n_groups = std::max(z.n_groups, y.n_groups * g);
+            z.cache = std::max(z.cache, y.cache);
+            z.scratch = std::max(z.scratch, y.scratch);
+            z.n_flags = std::max(z.n_flags, y.n_flags);
+            z.barrier = std::max(z.barrier, y.barrier);
+            z.clist = std::max(z.clist, y.clist);
+        }
+        return z;
+    }
     const int words = (P.N + 31) / 32;
-    int n_groups = ctx->refine_coresident / group;
-    if (n_groups > max_jobs) n_groups = max_jobs;
-    if (n_groups < 1) n_groups = 1;
+    const int n_groups = refine_n_groups(ctx->refine_coresident, group, max_jobs);
     z.n_groups = n_groups;
     z.masks = (size_t)max_jobs * 2 * words * 4;
     z.rounds = (size_t)max_jobs * 2 * 4;
@@ -592,7 +595,8 @@ int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, con
     int rc = refine_buffers(ctx, P, max_jobs, group, !masks_out, grow(ctx));
     if (rc) return rc;
     if (!masks_out) masks_out = ctx->masks.as<uint32_t>();
-    if (group > 1) CK(cudaMemsetAsync(ctx->scratch.p, 0, refine_scratch_doubles(n_groups, group) * 8, ctx->stream));  // LL elements: no stale sequence numbers
+    if (group == 0 && !pl.async) return fail(ctx, ESACB200_ERR_ARG, "refinement group picked on the device outside a stream-ordered call");
+    if (group != 1) CK(cudaMemsetAsync(ctx->scratch.p, 0, z.scratch, ctx->stream));  // LL elements: no stale sequence numbers
     const size_t n_flags = z.n_flags;
     CK(cudaMemsetAsync(ctx->barrier.p, 0, z.barrier, ctx->stream));
     RefineArgs a;
@@ -624,6 +628,10 @@ int run_refine(esacb200_ctx* ctx, const Plan& pl, const Pose* in, Pose* out, con
     a.P = P;
     a.max_ref_steps = ctx->opt.max_ref_steps;
     if (pl.async) a.dev = pl.async->dev;
+    a.coresident = ctx->refine_coresident;
+    a.group_opt = ctx->opt.refine_group_opt;
+    a.jobs_per_group = ctx->opt.refine_jobs_per_group;
+    a.max_jobs = max_jobs;
     launch_refine(a, n_groups, ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 1;
@@ -662,13 +670,25 @@ int enqueue_forward_core(esacb200_ctx* ctx, const Plan& pl, float* d_out17) {
     return 0;
 }
 
+// The backward's tail (bwd_reduce .. bwd_assemble); `losses`: esac.backward's own per-hypothesis losses too.
+template <class Need>
+int backward_buffers(esacb200_ctx* ctx, const Problem& P, bool losses, Need&& need) {
+    if (losses) NEED(ctx->losses, (size_t)P.M * 8);
+    NEED(ctx->red, (size_t)P.M * bwd_tiles(P.N) * bwd_red_vals() * 8);
+    NEED(ctx->hypgrad, (size_t)P.M * bwd_hypgrad_bytes());
+    NEED(ctx->job_of, (size_t)(P.M > P.E ? P.M : P.E) * 4);
+    return 0;
+}
+
 // Sizes every workspace buffer of the forward pipeline (upload, plan_and_prep, sampling, refinement) for the largest of a
 // batch's images before the first one is enqueued: DevBuf::ensure growing mid-batch frees the old buffer, and cudaFree
 // synchronises the device, which would serialise the copy stream's overlap with the previous image.
 // `need(buf, bytes)` is called once per buffer with the largest size any image needs; reserve_forward_batch grows them, the
-// stream-ordered forward also checks them.  (host_coords: the images' maps are staged, double-buffered.)
+// stream-ordered forward also checks them.  (host_coords: the images' maps are staged, double-buffered.)  backward: also the
+// stream-ordered backward's buffers -- the refinement of up to M jobs with its group picked on the device (every group a
+// job count may pick) and backward_buffers.
 template <class Need>
-int forward_workspace(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool host_coords, Need&& need) {
+int forward_workspace(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool host_coords, Need&& need, bool backward = false) {
     std::map<DevBuf*, size_t> most;
     auto mx = [&](DevBuf& b, size_t bytes) {
         most[&b] = std::max(most[&b], bytes);
@@ -681,24 +701,19 @@ int forward_workspace(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool ho
         prep_buffers(ctx, pl, mx);
         sample_buffers(ctx, pl, mx);
         refine_buffers(ctx, pl.P, 1, pick_group(ctx, pl.P, 1), true, mx);
+        if (backward) {
+            refine_buffers(ctx, pl.P, pl.P.M, 0, true, mx);
+            backward_buffers(ctx, pl.P, true, mx);
+        }
     }
     for (auto& m : most) NEED(*m.first, m.second);
     return 0;
 }
 
-// The backward's tail (bwd_reduce .. bwd_assemble); `losses`: esac.backward's own per-hypothesis losses too.
-template <class Need>
-int backward_buffers(esacb200_ctx* ctx, const Problem& P, bool losses, Need&& need) {
-    if (losses) NEED(ctx->losses, (size_t)P.M * 8);
-    NEED(ctx->red, (size_t)P.M * bwd_tiles(P.N) * bwd_red_vals() * 8);
-    NEED(ctx->hypgrad, (size_t)P.M * bwd_hypgrad_bytes());
-    NEED(ctx->job_of, (size_t)(P.M > P.E ? P.M : P.E) * 4);
-    return 0;
-}
 #undef NEED
 
-int reserve_forward_batch(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool host_coords) {
-    return forward_workspace(ctx, plans, host_coords, grow(ctx));
+int reserve_forward_batch(esacb200_ctx* ctx, const std::vector<Plan>& plans, bool host_coords, bool backward = false) {
+    return forward_workspace(ctx, plans, host_coords, grow(ctx), backward);
 }
 
 // All B pointers of one argument on the device, or all on the host (a mix is an error).  None may be null.
@@ -894,7 +909,7 @@ int esacb200_set_seed(esacb200_ctx* ctx, uint64_t seed) {
     if (!ctx) return ESACB200_ERR_ARG;
     ctx->seed = seed;
     ctx->calls = 0;
-    if (ctx->async) {  // the stream-ordered forward's seed and call counter, in stream order
+    if (ctx->async) {  // the stream-ordered calls' seed and call counter, in stream order
         DeviceGuard device_guard(ctx->device);
         launch_seed_reset(ctx->async->seed_state.as<unsigned long long>(), seed, ctx->stream);
         CK(cudaGetLastError());
@@ -1230,21 +1245,23 @@ int esacb200_forward_batch(esacb200_ctx* ctx, int B, const float* coords, int E,
 // arrays hold at replay time.  Nothing here synchronises, reads back or queries an event, and a call that a capture records
 // allocates nothing.
 
-// The stream-ordered forward's context, created on first use with ctx's seed (a capture may not create it: that allocates).
+// The context of the stream-ordered forward and backward, created on first use with ctx's seed (a capture may not create
+// it: that allocates).
 // The options are copied from ctx on every call.
-static int async_context(esacb200_ctx* ctx, bool capturing, esacb200_ctx** out) {
+// `what`: the entry point, forward_async or backward_async, named in the messages with its reserve call.
+static int async_context(esacb200_ctx* ctx, bool capturing, const char* what, esacb200_ctx** out) {
     if (!ctx->async) {
         if (capturing)
-            return fail(ctx, ESACB200_ERR_ARG, "forward_async: the first call may not be captured; call reserve_forward_async "
-                                               "(esacb200_reserve_forward_async) with the largest shape before capturing");
+            return fail(ctx, ESACB200_ERR_ARG, "%s: the first call may not be captured; call reserve_%s (esacb200_reserve_%s) "
+                                               "with the largest shape before capturing", what, what, what);
         esacb200_ctx* a = nullptr;
         int rc = esacb200_create(ctx->device, &a);
-        if (rc) return fail(ctx, rc, "cannot create the context of the stream-ordered forward");
+        if (rc) return fail(ctx, rc, "cannot create the context of the stream-ordered calls");
         a->is_async = true;
         if (a->seed_state.ensure(2 * sizeof(unsigned long long)) != cudaSuccess) {
             esacb200_destroy(a);
             cudaGetLastError();
-            return fail(ctx, ESACB200_ERR_CUDA, "cannot allocate the seed state of the stream-ordered forward");
+            return fail(ctx, ESACB200_ERR_CUDA, "cannot allocate the seed state of the stream-ordered calls");
         }
         launch_seed_reset(a->seed_state.as<unsigned long long>(), ctx->seed, ctx->stream);
         ctx->async = a;
@@ -1267,16 +1284,20 @@ static int stream_capturing(esacb200_ctx* ctx, bool& capturing) {
 }
 
 // Makes the async workspace hold `plans`: grows it when no capture has used it yet, else fails without touching it.
-static int async_workspace(esacb200_ctx* ctx, esacb200_ctx* a, const std::vector<Plan>& plans, bool capturing) {
-    const bool fits = forward_workspace(a, plans, false, [](DevBuf& b, size_t bytes) { return bytes <= b.cap ? 0 : 1; }) == 0;
+// backward: the workspace of the stream-ordered backward (forward_workspace's `backward`), else of the forward.
+static int async_workspace(esacb200_ctx* ctx, esacb200_ctx* a, const std::vector<Plan>& plans, bool capturing, bool backward) {
+    const bool fits =
+        forward_workspace(a, plans, false, [](DevBuf& b, size_t bytes) { return bytes <= b.cap ? 0 : 1; }, backward) == 0;
     if (fits) return 0;
     const Problem& P = plans[0].P;
+    const char* what = backward ? "backward_async" : "forward_async";
     if (capturing || a->frozen)
         return fail(ctx, ESACB200_ERR_ARG,
-                    "forward_async: E=%d H=%d W=%d M=%d needs more workspace than %s, and a graph that holds it may still be "
-                    "replayed; call reserve_forward_async (esacb200_reserve_forward_async) with the largest shape before the "
-                    "first capture", P.E, P.H, P.W, P.M, capturing ? "was reserved before this capture" : "an earlier capture used");
-    int rc = reserve_forward_batch(a, plans, false);
+                    "%s: E=%d H=%d W=%d M=%d needs more workspace than %s, and a graph that holds it may still be "
+                    "replayed; call reserve_%s (esacb200_reserve_%s) with the largest shape before the "
+                    "first capture", what, P.E, P.H, P.W, P.M, capturing ? "was reserved before this capture" : "an earlier capture used",
+                    what, what);
+    int rc = reserve_forward_batch(a, plans, false, backward);
     if (rc) return fail(ctx, rc, "%s", a->err);
     return 0;
 }
@@ -1294,9 +1315,9 @@ int esacb200_reserve_forward_async(esacb200_ctx* ctx, int B, int E, int H, int W
     if (rc) return rc;
     if (capturing) return fail(ctx, ESACB200_ERR_ARG, "reserve_forward_async allocates: call it before the capture");
     esacb200_ctx* a = nullptr;
-    rc = async_context(ctx, false, &a);
+    rc = async_context(ctx, false, "forward_async", &a);
     if (rc) return rc;
-    return async_workspace(ctx, a, plans, false);
+    return async_workspace(ctx, a, plans, false, false);
 } ESAC_ABI_CATCH(ctx)
 
 int esacb200_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
@@ -1319,7 +1340,7 @@ int esacb200_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E,
     rc = stream_capturing(ctx, capturing);
     if (rc) return rc;
     esacb200_ctx* a = nullptr;
-    rc = async_context(ctx, capturing, &a);
+    rc = async_context(ctx, capturing, "forward_async", &a);
     if (rc) return rc;
     // element stride between the assignments of consecutive images: rows of a [B, M] tensor
     const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
@@ -1344,7 +1365,7 @@ int esacb200_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E,
         im.advance = b == B - 1 ? B : 0;
         pl.async = &im;
     }
-    rc = async_workspace(ctx, a, plans, capturing);
+    rc = async_workspace(ctx, a, plans, capturing, false);
     if (rc) return rc;
     if (capturing) a->frozen = true;
     for (int b = 0; b < B; ++b) {
@@ -1492,7 +1513,7 @@ static int run_hypotheses(esacb200_ctx* ctx, Plan& pl, const float* coords, cons
     const Problem& P = pl.P;
     const int M = P.M, E = P.E;
     int* sc = ctx->scalars.as<int>();
-    const uint64_t seed = call_seed(ctx);
+    const uint64_t seed = pl.async ? 0 : call_seed(ctx);
     rc = run_sample(ctx, pl, seed);
     if (rc) return rc;
     rc = run_score(ctx, pl);
@@ -1518,28 +1539,62 @@ static int run_hypotheses(esacb200_ctx* ctx, Plan& pl, const float* coords, cons
     CK(cudaMemcpyAsync(ctx->poses_ref.p, ctx->poses.p, (size_t)M * sizeof(Pose), cudaMemcpyDeviceToDevice, ctx->stream));
     // Refining many hypotheses is fp64-throughput bound, so every SM should be busy and no CTA should wait at an inter-CTA
     // barrier longer than needed: one 4-byte read-back of the number of contributing hypotheses (a ~20 us stall on a
-    // multi-millisecond call) lets the group size be coresident / jobs.
-    CK(cudaMemcpyAsync(ctx->h_out + 28, sc + S_NCONTRIB, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    if (sh.reduce_grads) {  // which planes receive gradient on some rank: rides on the same host synchronisation
-        CK(ctx->eflags.ensure((size_t)E * sizeof(int)));
-        launch_expert_flags(ctx->contrib.as<int>(), sc + S_NCONTRIB, ctx->assign32.as<int>(), E, ctx->eflags.as<int>(), ctx->stream);
-        CKN(nccl_api().AllReduce(ctx->eflags.p, ctx->eflags.p, (size_t)E, kNcclInt32, kNcclMax, ctx->nccl_comm, ctx->stream));
-        CK(cudaMemcpyAsync(ctx->h_flags, ctx->eflags.p, (size_t)E * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-        ctx->st.kernel_launches += 2;
+    // multi-millisecond call) lets the group size be coresident / jobs.  A stream-ordered call (pl.async) reads nothing back:
+    // its refinement kernel picks the same group from the same count on the device (group 0).
+    int group = 0;
+    if (!pl.async) {
+        CK(cudaMemcpyAsync(ctx->h_out + 28, sc + S_NCONTRIB, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        if (sh.reduce_grads) {  // which planes receive gradient on some rank: rides on the same host synchronisation
+            CK(ctx->eflags.ensure((size_t)E * sizeof(int)));
+            launch_expert_flags(ctx->contrib.as<int>(), sc + S_NCONTRIB, ctx->assign32.as<int>(), E, ctx->eflags.as<int>(), ctx->stream);
+            CKN(nccl_api().AllReduce(ctx->eflags.p, ctx->eflags.p, (size_t)E, kNcclInt32, kNcclMax, ctx->nccl_comm, ctx->stream));
+            CK(cudaMemcpyAsync(ctx->h_flags, ctx->eflags.p, (size_t)E * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+            ctx->st.kernel_launches += 2;
+        }
+        CK(cudaStreamSynchronize(ctx->stream));
+        if (sh.reduce_grads) {
+            rc = for_flagged_planes(ctx, E, (size_t)3 * P.N, sh.d_work, sh.d_dst, 0);
+            if (rc) return rc;
+        }
+        int n_jobs_now = *(const int*)(ctx->h_out + 28);
+        if (n_jobs_now < 1) n_jobs_now = 1;
+        group = pick_group(ctx, P, n_jobs_now);
     }
-    CK(cudaStreamSynchronize(ctx->stream));
-    if (sh.reduce_grads) {
-        rc = for_flagged_planes(ctx, E, (size_t)3 * P.N, sh.d_work, sh.d_dst, 0);
-        if (rc) return rc;
-    }
-    int n_jobs_now = *(const int*)(ctx->h_out + 28);
-    if (n_jobs_now < 1) n_jobs_now = 1;
-    int group = pick_group(ctx, P, n_jobs_now);
     rc = run_refine(ctx, pl, ctx->poses.as<Pose>(), ctx->poses_ref.as<Pose>(), ctx->contrib.as<int>(), sc + S_NCONTRIB, 0, M, group,
                     masks);
     if (rc) return rc;
     mark(ctx, EV_REFINE);
     return 0;
+}
+
+// The arguments of launch_backward that come from the context's workspace after run_hypotheses.
+static BwdArgs backward_args(esacb200_ctx* ctx, const Plan& pl, float* grads) {
+    const Problem& P = pl.P;
+    int* sc = ctx->scalars.as<int>();
+    BwdArgs b;
+    b.coords = pl.d_coords;
+    b.grads = grads;
+    b.assign32 = ctx->assign32.as<int>();
+    b.perm = ctx->perm.as<int>();
+    b.counts = ctx->counts.as<int>();
+    b.offsets = ctx->offsets.as<int>();
+    b.init = ctx->poses.as<Pose>();
+    b.ref = ctx->poses_ref.as<Pose>();
+    b.cells = ctx->cells.as<int>();
+    b.probs = ctx->probs.as<double>();
+    b.contrib = ctx->contrib.as<int>();
+    b.n_contrib = sc + S_NCONTRIB;
+    b.job_of = ctx->job_of.as<int>();
+    b.masks = ctx->masks.as<uint32_t>();
+    b.mask_words = (P.N + 31) / 32;
+    b.rounds = ctx->rounds.as<int>();
+    b.losses = ctx->losses.as<double>();
+    b.out_loss = ctx->stats.as<double>() + 4;
+    b.red = ctx->red.as<double>();
+    b.hyp_grad = ctx->hypgrad.p;
+    b.P = P;
+    b.expected_override = nullptr;
+    return b;
 }
 
 // -------------------------------------------------------------------------------------------------
@@ -1587,27 +1642,7 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
     int* sc = ctx->scalars.as<int>();
     rc = backward_buffers(ctx, P, true, grow(ctx));
     if (rc) return rc;
-    BwdArgs b;
-    b.coords = pl.d_coords;
-    b.grads = d_grads;
-    b.assign32 = ctx->assign32.as<int>();
-    b.perm = ctx->perm.as<int>();
-    b.counts = ctx->counts.as<int>();
-    b.offsets = ctx->offsets.as<int>();
-    b.init = ctx->poses.as<Pose>();
-    b.ref = ctx->poses_ref.as<Pose>();
-    b.cells = ctx->cells.as<int>();
-    b.probs = ctx->probs.as<double>();
-    b.contrib = ctx->contrib.as<int>();
-    b.n_contrib = sc + S_NCONTRIB;
-    b.job_of = ctx->job_of.as<int>();
-    b.masks = ctx->masks.as<uint32_t>();
-    b.mask_words = (P.N + 31) / 32;
-    b.rounds = ctx->rounds.as<int>();
-    b.losses = ctx->losses.as<double>();
-    b.out_loss = ctx->stats.as<double>() + 4;
-    b.red = ctx->red.as<double>();
-    b.hyp_grad = ctx->hypgrad.p;
+    BwdArgs b = backward_args(ctx, pl, d_grads);
     if (is_device_ptr(gt_pose)) {
         CK(cudaMemcpyAsync(ctx->h_out, gt_pose, 16 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
@@ -1616,8 +1651,6 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
         memcpy(b.gt, gt_pose, 16 * sizeof(float));
     }
     b.wRot = wRot; b.wTrans = wTrans; b.cut = cut;
-    b.P = P;
-    b.expected_override = nullptr;
     double global_loss = 0;
     if (exchange) {
         // exchange 2: the expectation sum_h p_h loss_h runs over the hypotheses of all ranks (esac.cpp:357-362, esac_derivative.h:372-374)
@@ -1677,6 +1710,98 @@ int esacb200_backward(esacb200_ctx* ctx, const float* coords, float* grads, int 
                       double* out_loss) try {
     return backward_impl(ctx, coords, grads, E, H, W, assign, assign_stride, M, gt_pose, wRot, wTrans, cut, shiftX, shiftY, f, ppx,
                          ppy, tau, alpha, beta, maxReproj, sub, nullptr, nullptr, out_loss);
+} ESAC_ABI_CATCH(ctx)
+
+// -------------------------------------------------------------------------------------------------
+// Stream-ordered backward (esacb200_backward_async): esac.backward with the forward_async contract.  It runs in the same
+// context as forward_async (ctx->async) and counts calls with it; the host path is the eager one, with the refinement group
+// picked on the device from the number of contributing hypotheses.
+int esacb200_reserve_backward_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int sub) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "reserve_backward_async: empty batch (B=%d)", B);
+    std::vector<Plan> plans(1);
+    int rc = fill_problem(ctx, plans[0].P, E, H, W, M, 0, 0, 1.f, 0.f, 0.f, 1.f, 1.f, 1.f, 1.f, sub);
+    if (rc) return rc;
+    plans[0].d_coords = nullptr;  // the load path does not change the workspace
+    bool capturing = false;
+    rc = stream_capturing(ctx, capturing);
+    if (rc) return rc;
+    if (capturing) return fail(ctx, ESACB200_ERR_ARG, "reserve_backward_async allocates: call it before the capture");
+    esacb200_ctx* a = nullptr;
+    rc = async_context(ctx, false, "backward_async", &a);
+    if (rc) return rc;
+    return async_workspace(ctx, a, plans, false, true);
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_backward_async(esacb200_ctx* ctx, int B, const float* coords, float* grads, int E, int H, int W,
+                            const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wRot, float wTrans,
+                            float cut, const int32_t* shifts, const float* cameras, float tau, float alpha, float beta,
+                            float maxReproj, int sub, double* out_losses, int32_t* out_status) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "backward_async: empty batch (B=%d)", B);
+    Problem P;
+    int rc = fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, tau, alpha, beta, maxReproj, sub);
+    if (rc) return rc;
+    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small to draw 4 distinct cells", W, H);
+    const void* ptrs[] = {coords, grads, assign, gt_poses, shifts, cameras, out_losses, out_status};
+    const char* names[] = {"coords", "grads", "assign", "gt_poses", "shifts", "cameras", "out_losses", "out_status"};
+    for (int i = 0; i < 8; ++i) {
+        if (!ptrs[i]) return fail(ctx, ESACB200_ERR_ARG, "backward_async: %s is null", names[i]);
+        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "backward_async takes device pointers only: %s is host memory", names[i]);
+    }
+    bool capturing = false;
+    rc = stream_capturing(ctx, capturing);
+    if (rc) return rc;
+    esacb200_ctx* a = nullptr;
+    rc = async_context(ctx, capturing, "backward_async", &a);
+    if (rc) return rc;
+    const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
+    const size_t cstride = (size_t)E * 3 * H * W;
+    std::vector<Plan> plans((size_t)B);
+    std::vector<AsyncImage> imgs((size_t)B);
+    for (int b = 0; b < B; ++b) {
+        Plan& pl = plans[b];
+        pl.P = P;
+        pl.d_coords = coords + (size_t)b * cstride;
+        pl.d_assign = (const long long*)assign + b * arow;
+        pl.assign_stride = assign_stride;
+        AsyncImage& im = imgs[b];
+        im.dev.shift = shifts + 2 * (size_t)b;
+        im.dev.cam = cameras + 3 * (size_t)b;
+        im.dev.seed = a->seed_state.as<unsigned long long>();
+        im.dev.index = b;
+        im.dev.fixed_seed = a->opt.fixed_seed;
+        im.pose = nullptr;
+        im.expert = nullptr;
+        im.loss = out_losses + b;
+        im.gt = gt_poses + 16 * (size_t)b;
+        im.status = out_status + b;
+        im.advance = b == B - 1 ? B : 0;
+        pl.async = &im;
+    }
+    rc = async_workspace(ctx, a, plans, capturing, true);
+    if (rc) return rc;
+    if (capturing) a->frozen = true;
+    for (int b = 0; b < B; ++b) {
+        Plan& pl = plans[b];
+        rc = run_hypotheses(a, pl, pl.d_coords, (const int64_t*)pl.d_assign, assign_stride, ShardSteps(), nullptr);
+        if (!rc) rc = backward_buffers(a, P, true, grow(a));
+        if (rc) return fail(ctx, rc, "image %d: %s", b, a->err);
+        BwdArgs args = backward_args(a, pl, grads + (size_t)b * cstride);
+        args.wRot = wRot; args.wTrans = wTrans; args.cut = cut;
+        BwdDev dv;
+        dv.gt = imgs[b].gt;
+        dv.flags = a->scalars.as<int>() + S_FLAGS;
+        dv.dev = imgs[b].dev;
+        launch_backward(args, M, a->sm_count, a->stream, &dv);
+        launch_finish_backward_async(a->stats.as<double>(), a->scalars.as<int>() + S_FLAGS, imgs[b].loss, imgs[b].status,
+                                     a->seed_state.as<unsigned long long>(), imgs[b].advance, a->stream);
+        a->st.kernel_launches += 6;
+    }
+    CK(cudaGetLastError());
+    return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
@@ -2609,6 +2734,9 @@ void esacb200_host_dprojectdobj(const float pt[2], const float obj[3], const dou
 }
 
 void esacb200_host_pinv6(const double A[36], double out[36]) { pinv_sym6(A, out); }
+int esacb200_host_pick_group(int N, int coresident, int group_opt, int jobs_per_group, int jobs) {
+    return refine_group_rule(N, coresident, group_opt, jobs_per_group, jobs);
+}
 
 void esacb200_host_draw_cells(uint64_t seed, uint32_t h, uint32_t t, int W, int H, int32_t* cells8) {
     int cx[4], cy[4];

@@ -94,9 +94,10 @@ struct Problem {
     float tau, alpha, beta, max_reproj;
 };
 
-// Per-image values of a stream-ordered forward (esacb200_forward_async) that the kernels read from device memory instead
-// of from Problem / a seed argument, so that a captured graph replays with the values current at replay time.  The
-// kernels that take one are templates on a flag DEV; with DEV = false they ignore it and read Problem as before.
+// Per-image values of a stream-ordered forward or backward (esacb200_forward_async / _backward_async) that the kernels read
+// from device memory instead of from Problem / a seed argument, so that a captured graph replays with the values current at
+// replay time.  The kernels that take one are templates on a flag DEV; with DEV = false they ignore it and read Problem as
+// before.
 struct DevParams {
     const int* shift = nullptr;                // [2] shiftX, shiftY
     const float* cam = nullptr;                // [3] f, ppx, ppy
@@ -123,6 +124,35 @@ template <bool DEV, class A> __device__ __forceinline__ float dev_ppy(const Prob
     if constexpr (DEV) return __ldg(a.dev.cam + 2); else return P.ppy;
 }
 #endif
+
+// CTAs per refinement job for `jobs` jobs of an N-cell map (the host's pick_group, and the stream-ordered backward's
+// refinement kernel, which knows the job count only on the device): one rule, so the two pick the same group.
+ESAC_HD int refine_group_rule(int N, int coresident, int group_opt, int jobs_per_group, int jobs) {
+    if (group_opt > 0) return group_opt < coresident ? group_opt : coresident;
+    const int words = (N + 31) / 32;
+    // ~320 cells per CTA, up to every co-resident CTA: with the warp-parallel slot summation the inter-CTA barrier costs less
+    // than the fp64 work it spreads (60x80 -> 16 CTAs, 480x640 -> every co-resident CTA)
+    int g = words / 10;
+    if (g < 1) g = 1;
+    // Jobs are handed out dynamically inside the kernel, so a group may work through several jobs: fewer, larger groups even
+    // out the differing job lengths (rounds x LM iterations) -- worth it only while a block's share of the map stays large
+    // against the cost of a group exchange (480x640: yes; 60x80: no)
+    int waves = jobs >= 8 ? jobs_per_group : 1;
+    int concurrent = jobs > 0 ? (jobs + waves - 1) / waves : 1;
+    int cap = coresident / concurrent;
+    if (waves > 1 && (cap < 1 || N / (cap < 1 ? 1 : cap) < 4096)) cap = coresident / (jobs > 0 ? jobs : 1);
+    if (cap < 1) cap = 1;
+    if (g > cap) g = cap;
+    return g;
+}
+
+// Groups of one refinement launch of `group` CTAs each, for at most max_jobs jobs.
+ESAC_HD int refine_n_groups(int coresident, int group, int max_jobs) {
+    int n_groups = coresident / group;
+    if (n_groups > max_jobs) n_groups = max_jobs;
+    if (n_groups < 1) n_groups = 1;
+    return n_groups;
+}
 
 // Hypotheses of one expert are contiguous in "sorted slot" order (stable by hypothesis index);
 // a chunk is <= kMaxChunk consecutive slots of one expert: the unit the scoring kernel pairs with a
@@ -238,6 +268,10 @@ struct RefineArgs {
     Problem P;
     int max_ref_steps;
     DevParams dev;           // dev.shift != null: shift and camera from device memory (stream-ordered forward)
+    // group == 0 (with dev): refine_group_kernel picks group = refine_group_rule(N, coresident, group_opt, jobs_per_group,
+    // max(1, *n_jobs)) and derives n_groups, cache and clist from it as refine_sizes does; the grid is the largest any group
+    // needs, and clist (when not null) has room for any of them.
+    int coresident = 0, group_opt = 0, jobs_per_group = 0, max_jobs = 0;
 };
 void launch_refine(const RefineArgs& a, int n_groups, cudaStream_t st);
 int refine_max_coresident_blocks(int sm_count);
@@ -344,7 +378,19 @@ struct BwdArgs {
     Problem P;
     const double* expected_override;  // device scalar: global expected loss (multi-GPU), or null
 };
-void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t st);
+// What B1-B5 of the stream-ordered backward (esacb200_backward_async) read from device memory.  The kernels take it as their
+// last argument, so the arguments of the eager instantiations keep their places.
+struct BwdDev {
+    const float* gt = nullptr;   // [4,4] camera->world ground truth (B1), instead of BwdArgs::gt
+    const int* flags = nullptr;  // the prep kernel's bad-assignment flag: B5 leaves the gradient untouched when it is set
+    DevParams dev;               // shift and camera
+};
+// dev: non-null -> the stream-ordered instantiations, which read *dev
+void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t st, const BwdDev* dev = nullptr);
+// Stream-ordered backward: the expected loss stats[4] (NaN on a bad assignment) into *loss, flags[0] into *status; advance != 0
+// adds it to seed[1] (the last image of an execution).
+void launch_finish_backward_async(const double* stats, const int* flags, double* loss, int* status, unsigned long long* seed,
+                                  int advance, cudaStream_t st);
 // phase split for the multi-GPU path: losses + local expectation only / everything after the loss exchange
 void launch_backward_losses(const BwdArgs& a, cudaStream_t st);
 void launch_add_inplace(float* dst, const float* src, size_t n, cudaStream_t st);

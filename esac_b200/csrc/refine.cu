@@ -640,242 +640,48 @@ __device__ __forceinline__ void root_lm_step(RefShared& sh) {
     for (int i = 0; i < 6; ++i) sh.par[i] = sh.prev[i] - dlt[i];
 }
 
+// One refinement launch: n_groups groups of a.group CTAs, jobs handed to the groups (refine_body.inc).
 template <bool DEV>
 __global__ void __launch_bounds__(kRefThreads, 1) refine_kernel(const __grid_constant__ RefineArgs a) {
     __shared__ RefShared sh;
     extern __shared__ float cell_cache[];  // [3][kCacheCells] + the inlier list when the block's share fits (a.cache != 0)
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int n_groups = gridDim.x / a.group;
-    const int grp = blockIdx.x / a.group, cta = blockIdx.x - grp * a.group;
-    const bool root = cta == 0;
-    const int n_jobs = a.n_jobs ? *a.n_jobs : a.n_jobs_host;
-    Problem Pd = a.P;  // DEV: the image's shift and camera from device memory
-    if constexpr (DEV) {
-        Pd.shiftX = dev_shift_x<DEV>(a.P, a); Pd.shiftY = dev_shift_y<DEV>(a.P, a);
-        Pd.f = dev_f<DEV>(a.P, a); Pd.ppx = dev_ppx<DEV>(a.P, a); Pd.ppy = dev_ppy<DEV>(a.P, a);
-    }
-    const Problem& P = DEV ? Pd : a.P;
-    const int words = (P.N + 31) / 32;
-    const int wpc = (words + a.group - 1) / a.group;
-    const int w0 = min(words, cta * wpc), w1 = min(words, w0 + wpc);
-    const bool cached = a.cache != 0;
-    const bool dynamic = n_groups < n_jobs;
-    // inlier list of this CTA's share: behind the cell cache in shared memory, else in the group's global scratch
-    const bool compact = a.compact && (w1 - w0) <= kMaxCompactWords && (cached || a.clist);
-    unsigned short* list = cached ? reinterpret_cast<unsigned short*>(cell_cache + 3 * kCacheCells)
-                                  : (a.clist ? a.clist + (size_t)grp * words * 32 + (size_t)w0 * 32 : nullptr);
-    unsigned seq = 0;  // sequence number of the current command / result exchange (same in every block of the group)
-    int cur_job = -1, cached_expert = -1;
-    const float* pl = nullptr;
-    uint32_t* mbase = nullptr;
-    double cen[3] = {0., 0., 0.};
-    if (a.prof && blockIdx.x == 0 && tid == 0) sh.prof_last = clock64();
-    if (root && tid == 0) { sh.job = -1; sh.finished = 1; }
-    __syncthreads();
-
-    for (;;) {
-        // ================= root, warp 0: produce the next command =================
-        if (root && warp == 0) {
-            if (lane == 0) {
-                bool need_job = sh.finished != 0;
-                while (need_job) {  // draw jobs until one needs work or the list ends
-                    const int job = dynamic ? atomicAdd(a.job_counter, 1) : (sh.job < 0 ? grp : n_jobs);
-                    sh.job = job;
-                    if (job >= n_jobs) break;
-                    const int hh = a.jobs[job];
-                    if (a.max_ref_steps <= 0) {  // nothing to refine: copy through
-                        a.poses_out[hh] = a.poses_in[hh];
-                        a.rounds[job * 2] = 0;
-                        a.rounds[job * 2 + 1] = 0;
-                        continue;
-                    }
-                    const Pose p0 = a.poses_in[hh];
-                    const int ee = a.assign32[hh];
-                    for (int i = 0; i < 3; ++i) { sh.pose[i] = p0.r[i]; sh.pose[3 + i] = p0.t[i]; sh.cen[i] = (double)a.centres[ee * 3 + i]; }
-                    sh.h = hh;
-                    sh.best = 4;
-                    sh.rounds = 0; sh.sel = 0; sh.step = 0;
-                    sh.mode = CMD_FIRST;
-                    sh.finished = 0;
-                    need_job = false;
-                }
-            }
-            __syncwarp();
-            if (sh.job >= n_jobs) {
-                if (lane == 0) sh.cmd[C_CMD] = (double)CMD_EXIT;
-            } else {
-                if (sh.mode == CMD_FIRST) {
-                    // the round's pose: R must be rodrigues_v2m's (the inlier test reproduces getReproErrs bit for bit)
-                    if (lane == 0) {
-                        double R0[9];
-                        rodrigues_v2m(sh.pose, R0, nullptr);
-                        for (int i = 0; i < 9; ++i) sh.cmd[C_R + i] = R0[i];
-                        for (int i = 0; i < 6; ++i) { sh.par[i] = sh.pose[i]; sh.cmd[C_PAR + i] = sh.pose[i]; }
-                        for (int i = 0; i < 3; ++i)
-                            sh.cmd[C_T + i] = R0[i * 3] * sh.cen[0] + R0[i * 3 + 1] * sh.cen[1] + R0[i * 3 + 2] * sh.cen[2] + sh.pose[3 + i];
-                    }
-                } else {
-                    root_rotation_fast(sh, sh.cen, lane);
-                }
-                if (lane == 0) {
-                    sh.cmd[C_CMD] = (double)sh.mode;
-                    sh.cmd[C_JOB] = (double)sh.job;
-                    sh.cmd[C_SEL] = (double)sh.sel;
-                }
-            }
-            __syncwarp();
-        }
-        ++seq;
-        if (a.group > 1) {
-            if (root) {  // every block gets its own copy of the command (all threads of the root write)
-                __syncthreads();
-                uint4* mb = ll_mailboxes(a, grp);
-                for (int i = tid; i < (a.group - 1) * C_COUNT; i += kRefThreads) {
-                    const int c = 1 + i / C_COUNT, e = i - (c - 1) * C_COUNT;
-                    st_ll(mb + ((size_t)c * 2 + (seq & 1)) * kSlot + e, sh.cmd[e], seq);
-                }
-            } else if (tid < C_COUNT) {
-                const uint4* mine = ll_mailboxes(a, grp) + ((size_t)cta * 2 + (seq & 1)) * kSlot + tid;
-                double v;
-                while (!ld_ll(mine, seq, v)) __nanosleep(32);  // (polling flat out slows the root's stores to these very lines)
-                sh.cmd[tid] = v;
-            }
-        }
-        __syncthreads();
-        tick(a, sh, 0);
-        const int cmd = (int)sh.cmd[C_CMD];
-        if (cmd == CMD_EXIT) break;
-        const int job = (int)sh.cmd[C_JOB];
-        const int sel = (int)sh.cmd[C_SEL];
-        if (job != cur_job) {
-            cur_job = job;
-            const int h = a.jobs[job];
-            const int e = a.assign32[h];
-            pl = a.coords + (size_t)e * 3 * P.N;
-            mbase = a.masks + (size_t)job * 2 * a.mask_words;
-            for (int i = 0; i < 3; ++i) cen[i] = (double)a.centres[e * 3 + i];
-            if (cached && cached_expert != e) {
-                for (int i = tid; i < (w1 - w0) * 32; i += kRefThreads) {
-                    const int p = w0 * 32 + i;
-                    const bool ok = p < P.N;
-                    cell_cache[i] = ok ? pl[p] : 0.f;
-                    cell_cache[kCacheCells + i] = ok ? pl[P.N + p] : 0.f;
-                    cell_cache[2 * kCacheCells + i] = ok ? pl[2 * (size_t)P.N + p] : 0.f;
-                }
-                cached_expert = e;
-                __syncthreads();
-            }
-        }
-        // ================= everybody: this block's share of the cells =================
-        uint32_t* mtent = mbase + (size_t)(1 - sel) * a.mask_words;
-        double acc[kRedN + 1];
-        const double* R = sh.cmd + C_R;
-        const double* t = sh.cmd + C_T;
-        const double* t0 = sh.cmd + C_PAR + 3;
-        if (cmd == CMD_FIRST && compact) {
-            // select the round's inliers, list them, then the sums over the list (the first evaluation of the round)
-            if (cached) lm_select<true>(pl, cell_cache, P, R, t0, t, cen, mtent, w0, w1, sh.cnt, a.pretest != 0);
-            else lm_select<false>(pl, cell_cache, P, R, t0, t, cen, mtent, w0, w1, sh.cnt, a.pretest != 0);
-            build_inlier_list(sh, mtent, w0, w1, list);
-            if (cached) lm_accumulate_list<true>(pl, cell_cache, P, R, t, cen, list, sh.n_list, w0, acc);
-            else lm_accumulate_list<false>(pl, cell_cache, P, R, t, cen, list, sh.n_list, w0, acc);
-            if (tid == 0) acc[kRedN] = (double)sh.n_list;
-        } else if (cmd == CMD_FIRST) {
-            if (cached) lm_accumulate<true, true>(pl, cell_cache, P, R, t, cen, mtent, w0, w1, t0, acc, nullptr);
-            else lm_accumulate<true, false>(pl, cell_cache, P, R, t, cen, mtent, w0, w1, t0, acc, nullptr);
-        } else if (compact) {
-            if (cached) lm_accumulate_list<true>(pl, cell_cache, P, R, t, cen, list, sh.n_list, w0, acc);
-            else lm_accumulate_list<false>(pl, cell_cache, P, R, t, cen, list, sh.n_list, w0, acc);
-        } else {
-            if (cached) lm_accumulate<false, true>(pl, cell_cache, P, R, t, cen, mtent, w0, w1, t0, acc, nullptr);
-            else lm_accumulate<false, false>(pl, cell_cache, P, R, t, cen, mtent, w0, w1, t0, acc, nullptr);
-        }
-        tick(a, sh, 1);
-        block_reduce_publish<kRedN + 1>(acc, sh, a, grp, cta, seq);
-        tick(a, sh, 2);
-        if (!root) continue;
-        // ================= root: gather, decide, step =================
-        if (warp == 0) {
-            // dR/dr, T, G of the evaluated parameters, while the other blocks finish their passes
-            root_rotation_jacobian(sh, sh.cen, lane);
-            root_change_of_variables(sh, lane);
-        }
-        if (a.group > 1) root_gather<kRedN + 1>(sh, a, grp, seq);
-        else __syncthreads();
-        if (warp == 0) {
-            root_map_sums(sh, lane);
-            tick(a, sh, 5);
-            if (lane == 0) {
-                if (a.prof && blockIdx.x == 0) a.prof[8] += 1;
-                bool job_done = false;
-                if (cmd == CMD_FIRST) {
-                    const double n_in = sh.tot[kRedN];
-                    if (!(n_in > sh.best)) {
-                        job_done = true;  // converged (esac_util.h:417-418)
-                    } else {
-                        sh.best = n_in;
-                        for (int i = 0; i < kRedN; ++i) sh.cur[i] = sh.cand[i];
-                        sh.prev_cost = sh.cand[27];  // iters == 0: prevErrNorm = ||err(param0)|| (compared squared)
-                        for (int i = 0; i < 6; ++i) sh.prev[i] = sh.par[i];
-                        sh.lamlg = -3;
-                        sh.iters = 0;
-                        root_lm_step(sh);
-                        sh.mode = CMD_EVAL;
-                    }
-                } else {  // CHECK_ERR of CvLevMarq; the evaluation also yields the Jacobian sums reused if the step is kept
-                    const double cost = sh.cand[27];  // errNorm > prevErrNorm  <=>  cost > previous cost (no square roots)
-                    if (cost > sh.prev_cost && ++sh.lamlg <= 16) {
-                        root_lm_step(sh);  // rejected: same normal equations, more damping
-                    } else {
-                        sh.lamlg = sh.lamlg - 1 > -16 ? sh.lamlg - 1 : -16;
-                        double dn = 0, pn = 0;
-                        for (int i = 0; i < 6; ++i) { const double d = sh.par[i] - sh.prev[i]; dn += d * d; pn += sh.prev[i] * sh.prev[i]; }
-                        // norm(param - prevParam) / norm(prevParam) < FLT_EPSILON, squared
-                        const bool done = (++sh.iters >= 20) || (dn < (double)FLT_EPSILON * (double)FLT_EPSILON * pn);
-                        if (!done) {
-                            sh.prev_cost = cost;
-                            for (int i = 0; i < kRedN; ++i) sh.cur[i] = sh.cand[i];
-                            for (int i = 0; i < 6; ++i) sh.prev[i] = sh.par[i];
-                            root_lm_step(sh);
-                        } else {  // the round's solvePnP is over (esac_util.h:426-447)
-                            bool bad = false;
-                            for (int i = 0; i < 6; ++i) bad = bad || !(sh.par[i] == sh.par[i]);
-                            if (bad) {
-                                job_done = true;
-                            } else {
-                                for (int i = 0; i < 6; ++i) sh.pose[i] = sh.par[i];
-                                sh.sel = 1 - sh.sel;
-                                ++sh.rounds;
-                                if (++sh.step >= a.max_ref_steps) job_done = true;
-                                else sh.mode = CMD_FIRST;
-                            }
-                        }
-                    }
-                }
-                if (job_done) {
-                    Pose out;
-                    for (int i = 0; i < 3; ++i) { out.r[i] = sh.pose[i]; out.t[i] = sh.pose[3 + i]; }
-                    a.poses_out[sh.h] = out;
-                    a.rounds[sh.job * 2] = sh.rounds;
-                    a.rounds[sh.job * 2 + 1] = sh.sel;
-                    sh.finished = 1;
-                }
-            }
-            __syncwarp();
-        }
-        tick(a, sh, 6);
-        __syncthreads();
-    }
+#include "refine_body.inc"
 }
 
+// refine_kernel<true> with the group picked on the device (a_in.group == 0, stream-ordered backward): the group follows from
+// the job count *n_jobs by refine_group_rule, and n_groups, cache and clist from the group as refine_sizes derives them on
+// the host.  The grid is the largest any group needs; the CTAs past the chosen group's launch leave at once.  The body is
+// refine_kernel's, text for text: an argument copy in refine_kernel itself would change its code.
+__global__ void __launch_bounds__(kRefThreads, 1) refine_group_kernel(const __grid_constant__ RefineArgs a_in) {
+    constexpr bool DEV = true;
+    __shared__ RefShared sh;
+    extern __shared__ float cell_cache[];
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int nj = a_in.n_jobs ? *a_in.n_jobs : a_in.n_jobs_host;
+    const int g = refine_group_rule(a_in.P.N, a_in.coresident, a_in.group_opt, a_in.jobs_per_group, nj > 1 ? nj : 1);
+    const int n_groups = refine_n_groups(a_in.coresident, g, a_in.max_jobs);
+    if ((int)blockIdx.x >= n_groups * g) return;
+    const int wpc_g = ((a_in.P.N + 31) / 32 + g - 1) / g;
+    RefineArgs ad = a_in;
+    ad.group = g;
+    ad.cache = wpc_g <= kCacheWords ? 1 : 0;
+    if (!a_in.compact || ad.cache || wpc_g > kMaxCompactWords) ad.clist = nullptr;
+    const RefineArgs& a = ad;
+#include "refine_body.inc"
+}
+
+// a.group == 0 (group picked on the device): n_groups is the CTA count of the largest launch any group needs.
 void launch_refine(const RefineArgs& a, int n_groups, cudaStream_t st) {
-    dim3 grid(n_groups * a.group), block(kRefThreads);
+    dim3 grid(a.group ? n_groups * a.group : n_groups), block(kRefThreads);
     const size_t smem = a.cache ? refine_cache_bytes() : 0;
     void* params[] = {(void*)&a};
-    const void* fn = a.dev.shift ? (const void*)refine_kernel<true> : (const void*)refine_kernel<false>;
+    const void* fn = a.group == 0 ? (const void*)refine_group_kernel
+                     : a.dev.shift ? (const void*)refine_kernel<true> : (const void*)refine_kernel<false>;
     // above the 48 KB a kernel gets without asking; the attribute is per device, so it is set on every launch (it is cheap)
     cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)refine_cache_bytes());
-    if (a.group > 1) cudaLaunchCooperativeKernel(fn, grid, block, params, smem, st);
+    if (a.group != 1) cudaLaunchCooperativeKernel(fn, grid, block, params, smem, st);
     else cudaLaunchKernel(fn, grid, block, params, smem, st);
 }
 

@@ -242,6 +242,31 @@ int esacb200_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E,
  * run while the context's stream is being captured.  B does not change the workspace: the images run one after another. */
 int esacb200_reserve_forward_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int subSampling);
 
+/* esac_backward enqueued with esacb200_forward_async's contract, so that a training step can be captured in a CUDA graph:
+ * device pointers only, checked before anything is enqueued.  coords / grads float32 [B,E,3,H,W] (grads ACCUMULATED, +=,
+ * as esacb200_backward), assign int64 [B,M], gt_poses float32 [B,4,4] camera->world, shifts int32 [B,2], cameras float32
+ * [B,3]; results out_losses double [B] (the value esacb200_backward returns) and out_status int32 [B].  Status 1 = the
+ * image's assignment held an expert index outside [0,E): its loss is NaN and its gradient slice is left untouched; the
+ * other images are unaffected.  No host synchronisation, read-back or event query, and no allocation while capturing.
+ *
+ * esacb200_backward reads the number of contributing hypotheses back to size the refinement's CTA groups; here the
+ * refinement kernel picks the same group from the same count on the device, on a grid as large as any count needs, so the
+ * results are bitwise those of esacb200_backward.  The ground truth, shift and camera are read when the kernels run.
+ *
+ * Seeding: the same device-side seed and call counter as esacb200_forward_async (one counter for both): image b of the
+ * j-th stream-ordered execution after set_seed(s) draws what the (j*B + b)-th esacb200_forward / esacb200_backward after
+ * set_seed(s) draws, "fixed_seed" honoured.  Workspace: esacb200_forward_async's, with its rule; it also holds the
+ * backward's buffers once esacb200_reserve_backward_async (or an uncaptured call) has sized them, and a call that needs
+ * more after a capture fails, naming the reserve call. */
+int esacb200_backward_async(esacb200_ctx* ctx, int B, const float* coords, float* grads, int E, int H, int W,
+                            const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wLossRot,
+                            float wLossTrans, float lossCut, const int32_t* shifts, const float* cameras, float inlierThreshold,
+                            float inlierAlpha, float inlierBeta, float maxReproj, int subSampling, double* out_losses,
+                            int32_t* out_status);
+/* Sizes the stream-ordered workspace for esacb200_backward_async (and esacb200_forward_async) calls of this shape; allocates,
+ * so it may not run while the context's stream is being captured. */
+int esacb200_reserve_backward_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int subSampling);
+
 /* esac_backward over B images of one shape (the reference trains with batch_size=1, train_esac.py:96-100, one
  * esac.backward per image): coords / grads float32 [B,E,3,H,W] (grads accumulated in place, as esac.cpp:490-508),
  * assign int64 [B,M] (as in esacb200_forward_batch), gt_poses float32 [B,4,4] (camera->world), shiftX / shiftY int [B]

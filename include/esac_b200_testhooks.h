@@ -46,6 +46,9 @@ void esacb200_host_dprojectdobj(const float pt[2], const float obj[3], const dou
                                 float ppy, float maxReproj, double out3[3]);
 /* Pseudo-inverse of a symmetric 6x6 (cv::Mat::inv(DECOMP_SVD) semantics). */
 void esacb200_host_pinv6(const double A[36], double out[36]);
+/* CTAs per refinement job for `jobs` jobs on an N-cell map with `coresident` co-resident refinement CTAs and the options
+ * refine_group / refine_jobs_per_group: the one rule the host and the stream-ordered backward's refinement kernel both use. */
+int esacb200_host_pick_group(int N, int coresident, int group_opt, int jobs_per_group, int jobs);
 /* Minimal set of try (seed, h, t): cells int[4][2] (x, y). */
 void esacb200_host_draw_cells(uint64_t seed, uint32_t h, uint32_t t, int W, int H, int32_t* cells8);
 

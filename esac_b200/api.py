@@ -260,7 +260,8 @@ class Context:
         return d
 
     def sample_trace(self) -> np.ndarray:
-        """[lane, wave, kernel (0 prefilter, 1 exact), (start, end)] in ns relative to the first stamp; -1 where nothing ran."""
+        """[lane, wave, kernel (0 prefilter, 1 exact), (start, end)] in ns relative to the first stamp; -1 where nothing ran.
+        Waves 32 and later (option sample_waves goes up to 64) run but are not stamped."""
         raw = np.zeros(512, np.uint64)
         self.check(self.lib.esacb200_get_sample_trace(self.handle, raw.ctypes.data))
         t = raw.reshape(4, 32, 2, 2)

@@ -69,7 +69,7 @@ struct Options {
     float sample_window = 1.25f;  // later waves: window / acceptance rate
     int sample_waves = 6;         // launched unconditionally (empty ones cost ~6 us each); what is left after them goes to tail_kernel
     float sample_tail_boost = 1.f;  // window factor once <= 64 hypotheses are left in a lane (x2 more for <= 8)
-    int sample_trace = 0;         // 1: prefilter / exact kernels stamp first-CTA-start / last-CTA-end times (esacb200_get_sample_trace)
+    int sample_trace = 0;         // 1: prefilter / exact kernels of waves 0-31 stamp first-CTA-start / last-CTA-end times (esacb200_get_sample_trace)
     int sample_groups = 2;        // lanes of the sampling stage (third and fourth lane: no gain measured)
     int upload_split = 1;
     int hyp_offset = 0, hyp_stride = 1;

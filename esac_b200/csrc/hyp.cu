@@ -35,6 +35,7 @@ constexpr int kTryThreads = 128;
 constexpr int kNoTry = 0x7fffffff;
 constexpr unsigned long long kNoKey = ~0ull;   // best[h]: (try << 32) | staging slot
 constexpr unsigned kNoSlot = 0xffffffffu;
+constexpr int kTraceWaves = 32;  // waves per lane in the trace buffer (option sample_trace): [4 lanes][32 waves][2 kernels]
 
 struct SampleArgs {
     const float4* coords4;  // [E][N] interleaved (x, y, z, -) copy of the coordinate planes: one 16-byte sector per gathered cell
@@ -488,11 +489,13 @@ int launch_sample(const float* coords, float4* coords4, const int* assign32, con
         // 3 CTAs per SM + 64-thread verdict CTAs in the room that leaves was measured slower
         const int grid = sm_count * 4;
         for (int r = 0; r < n_waves; ++r) {
-            a.trace_slot = (g * 32 + r) * 2;
+            // the trace holds 32 waves per lane: later waves (sample_waves may be up to 64) are not stamped
+            a.trace = r < kTraceWaves ? trace : nullptr;
+            a.trace_slot = (g * kTraceWaves + r) * 2;
             if (dev) prefilter_kernel<true><<<grid, kTryThreads, 0, sg>>>(a);
             else prefilter_kernel<false><<<grid, kTryThreads, 0, sg>>>(ae);
             ++launches;
-            a.trace_slot = (g * 32 + r) * 2 + 1;
+            a.trace_slot = (g * kTraceWaves + r) * 2 + 1;
             if (dev) exact_kernel<true><<<sm_count * 4, 128, 0, sg>>>(a);  // its last CTA also advances the windows
             else exact_kernel<false><<<sm_count * 4, 128, 0, sg>>>(ae);
             ++launches;

@@ -406,7 +406,8 @@ int esacb200_get_refine_profile(esacb200_ctx* ctx, long long* out16);
  * [4] accepted tries staged, [5] lanes.  out8: host long long [8]. */
 int esacb200_get_sample_profile(esacb200_ctx* ctx, long long* out8);
 /* With option "sample_trace" = 1 the prefilter / exact kernels of the sampling waves stamp %globaltimer: out512 (host uint64
- * [4 lanes][32 waves][2 kernels: prefilter, exact][2: first CTA start, last CTA end], ns; start = ~0 where nothing ran). */
+ * [4 lanes][32 waves][2 kernels: prefilter, exact][2: first CTA start, last CTA end], ns; start = ~0 where nothing ran).
+ * Only waves 0-31 of each lane are stamped: with option "sample_waves" above 32 the later waves run but are not traced. */
 int esacb200_get_sample_trace(esacb200_ctx* ctx, unsigned long long* out512);
 
 /* Read back intermediates of the last forward/backward call (any pointer may be NULL):

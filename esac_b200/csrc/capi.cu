@@ -79,6 +79,16 @@ struct Options {
 
 enum { EV_START = 0, EV_H2D, EV_PREP, EV_SAMPLE, EV_FOLD, EV_SCORE, EV_SELECT, EV_REFINE, EV_BWD, EV_END, EV_COUNT };
 
+// What the last call on a context left in its per-hypothesis buffers: the getters read nothing else.  Every call clears it
+// (begin_call, run_batch); only the code that writes those buffers sets it.
+struct LastCall {
+    int M = 0;
+    bool drew = false;         // poses, cells, tries, probs, refined poses and the sampling lanes' counters
+    int lanes = 0, lane_cap = 0;  // of the sampling stage (sample_sizes: G, Mg)
+    bool scored = false;       // scores
+    bool losses = false;       // esac.backward's per-hypothesis losses
+};
+
 }  // namespace
 
 struct esacb200_ctx {
@@ -97,8 +107,6 @@ struct esacb200_ctx {
     Options opt;
     int* h_flags = nullptr;    // pinned: per-expert "receives gradient on some rank" flags (hypothesis-major sharding)
     int h_flags_cap = 0;
-    int smp_groups_last = 0;      // lanes of the last run_sample (diagnostics read-back)
-    int smp_Mg_last = 0;
     int refine_coresident = 0;
     char err[512] = {0};
     // workspace
@@ -112,8 +120,7 @@ struct esacb200_ctx {
     cudaEvent_t ev[EV_COUNT] = {nullptr};
     bool ev_used[EV_COUNT] = {false};
     esacb200_stats st;
-    int last_M = 0;
-    bool last_backward = false;
+    LastCall last;
     // NCCL communicator of the sharded entry points (esacb200_comm_init); the library is resolved at run time with dlopen
     void* nccl_comm = nullptr;
     int comm_world = 1, comm_rank = 0;
@@ -259,10 +266,18 @@ struct AsyncImage {
     int advance;        // the last image of an execution: advance the async call counter by B
 };
 
+// Whether a call draws hypotheses from its problem, and whether it draws the context's injected cells (esacb200_inject_cells)
+// when there are any; a call that draws ignores or clears them otherwise.
+enum Draw { NO_DRAW, DRAWS, DRAWS_INJECTED };
+
 int fill_problem(esacb200_ctx* ctx, Problem& P, int E, int H, int W, int M, int shiftX, int shiftY, float f, float ppx,
-                 float ppy, float tau, float alpha, float beta, float maxReproj, int sub) {
+                 float ppy, float tau, float alpha, float beta, float maxReproj, int sub, Draw draw) {
     if (E <= 0 || H <= 0 || W <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "empty tensor (E=%d H=%d W=%d M=%d)", E, H, W, M);
     if ((long long)H * W > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "coordinate map too large");
+    if (draw != NO_DRAW && (long long)(W - 1) * (H - 1) < 4)
+        return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small to draw 4 distinct cells from [0,W-2]x[0,H-2]", W, H);
+    if (draw == DRAWS_INJECTED && ctx->inj_M && ctx->inj_M != M)
+        return fail(ctx, ESACB200_ERR_ARG, "injected cells are for M=%d, call has M=%d", ctx->inj_M, M);
     P.E = E; P.H = H; P.W = W; P.N = H * W; P.M = M;
     P.shiftX = shiftX; P.shiftY = shiftY; P.sub = sub;
     P.f = f; P.ppx = ppx; P.ppy = ppy; P.tau = tau; P.alpha = alpha; P.beta = beta; P.max_reproj = maxReproj;
@@ -481,8 +496,6 @@ int run_sample(esacb200_ctx* ctx, const Plan& pl, uint64_t seed) {
                                              o.sample_span0, o.sample_window, o.sample_waves, trace, o.sample_tail_boost,
                                              pl.async ? &pl.async->dev : nullptr);
     CK(cudaGetLastError());
-    ctx->smp_groups_last = G;
-    ctx->smp_Mg_last = Mg;
     if (pl.split_e) {
         // both halves have landed (the join orders this stream after lane 1, which waited for the second half): plane centres
         int* sc = ctx->scalars.as<int>();
@@ -789,6 +802,7 @@ size_t order_by_path(const std::vector<Rec>& recs, const std::vector<char>& vec,
 
 void begin_call(esacb200_ctx* ctx) {
     memset(&ctx->st, 0, sizeof(ctx->st));
+    ctx->last = LastCall();
     for (int i = 0; i < EV_COUNT; ++i) ctx->ev_used[i] = false;
     ctx->err[0] = 0;
     mark(ctx, EV_START);
@@ -804,6 +818,44 @@ void finish_stats(esacb200_ctx* ctx) {
     s.ms_refine = span(ctx, EV_SELECT, EV_REFINE);
     s.ms_backward = span(ctx, EV_REFINE, EV_BWD);
     s.ms_total = span(ctx, EV_START, EV_END);
+}
+
+// The last-call record of a call whose (last) problem `pl` was drawn and scored; `losses`: esac.backward's losses too.
+void record_draw(esacb200_ctx* ctx, const Plan& pl, bool losses) {
+    const SampleSizes z = sample_sizes(ctx, pl);
+    LastCall& l = ctx->last;
+    l.M = pl.P.M;
+    l.drew = l.scored = true;
+    l.lanes = z.G;
+    l.lane_cap = z.Mg;
+    l.losses = losses;
+}
+
+// The end of a call that ran prep .. select on the context and synchronises once: after the copies the caller enqueued,
+// read back the scalars and the first `n_stats` statistics doubles, wait, check the expert indices, fill the statistics
+// and the last-call record (`drew`: the call drew `pl`'s hypotheses, and used up any injected cells; `losses`: see
+// record_draw) and take the stage times.
+int finish_call(esacb200_ctx* ctx, const Plan& pl, int n_stats, bool drew, bool losses = false) {
+    CK(cudaMemcpyAsync(ctx->h_out + 20, ctx->scalars.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    if (n_stats) CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.p, n_stats * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    mark(ctx, EV_END);
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    const int* hs = (const int*)(ctx->h_out + 20);
+    if (hs[S_FLAGS]) return fail(ctx, ESACB200_ERR_ARG, "hypAssignment holds an expert index outside [0, %d)", pl.P.E);
+    ctx->st.M = pl.P.M;
+    ctx->st.winner = hs[S_WINNER];
+    ctx->st.n_contrib = hs[S_NCONTRIB];
+    if (n_stats) ctx->st.entropy = ctx->h_dbl[0];
+    if (drew) {
+        record_draw(ctx, pl, losses);
+        ctx->inj_M = ctx->inj_T = 0;
+    } else {
+        ctx->last.M = pl.P.M;
+        ctx->last.scored = true;
+    }
+    finish_stats(ctx);
+    return 0;
 }
 
 
@@ -973,38 +1025,21 @@ int esacb200_forward(esacb200_ctx* ctx, const float* coords, int E, int H, int W
     DeviceGuard device_guard(ctx->device);
     if (!coords || !assign || !out_pose) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
     Plan pl;
-    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub);
+    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS_INJECTED);
     if (rc) return rc;
-    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small to draw 4 distinct cells from [0,W-2]x[0,H-2]", W, H);
-    if (ctx->inj_M && ctx->inj_M != M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are for M=%d, call has M=%d", ctx->inj_M, M);
     begin_call(ctx);
     rc = stage_inputs(ctx, pl, coords, assign, assign_stride, /*allow_split=*/!ctx->inj_M);
     if (rc) return rc;
-    const Problem& P = pl.P;
-    int* sc = ctx->scalars.as<int>();
     rc = enqueue_forward_core(ctx, pl, ctx->out17.as<float>());
     if (rc) return rc;
     CK(cudaMemcpyAsync(ctx->h_out, ctx->out17.p, 17 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_out + 20, sc, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.p, 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaMemcpyAsync(ctx->h_dbl + 4, ctx->rounds.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     if (is_device_ptr(out_pose)) CK(cudaMemcpyAsync(out_pose, ctx->out17.p, 16 * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-    mark(ctx, EV_END);
-    CK(cudaStreamSynchronize(ctx->stream));
-    CK(cudaGetLastError());
-    const int* hs = (const int*)(ctx->h_out + 20);
-    if (hs[S_FLAGS]) return fail(ctx, ESACB200_ERR_ARG, "hypAssignment holds an expert index outside [0, %d)", E);
+    rc = finish_call(ctx, pl, 3, true);
+    if (rc) return rc;
     if (!is_device_ptr(out_pose)) memcpy(out_pose, ctx->h_out, 16 * sizeof(float));
     if (out_expert) *out_expert = (int)ctx->h_out[16];
-    ctx->st.M = M;
-    ctx->st.winner = hs[S_WINNER];
-    ctx->st.n_contrib = hs[S_NCONTRIB];
-    ctx->st.entropy = ctx->h_dbl[0];
     ctx->st.refine_rounds = ((const int*)(ctx->h_dbl + 4))[0];
-    ctx->last_M = M;
-    ctx->last_backward = false;
-    finish_stats(ctx);
-    ctx->inj_M = ctx->inj_T = 0;
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 
@@ -1016,11 +1051,10 @@ static int enqueue_forward_record(esacb200_ctx* ctx, const float* coords, int E,
     if (M_pad < M || M_pad < 1) return fail(ctx, ESACB200_ERR_ARG, "M_pad (%d) must be >= M (%d) and >= 1", M_pad, M);
     begin_call(ctx);
     ctx->inj_M = ctx->inj_T = 0;
+    Plan pl;
     if (M > 0) {
-        Plan pl;
-        int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub);
+        int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS);
         if (rc) return rc;
-        if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small", W, H);
         rc = stage_inputs(ctx, pl, coords, assign, assign_stride);
         if (rc) return rc;
         rc = enqueue_forward_core(ctx, pl, ctx->out17.as<float>());
@@ -1034,8 +1068,7 @@ static int enqueue_forward_record(esacb200_ctx* ctx, const float* coords, int E,
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 1;
     ctx->st.M = M;
-    ctx->last_M = M;
-    ctx->last_backward = false;
+    if (M > 0) record_draw(ctx, pl, false);
     return ESACB200_OK;
 }
 
@@ -1148,9 +1181,8 @@ int esacb200_forward_ragged(esacb200_ctx* ctx, int B, const float* const* coords
     for (int b = 0; b < B; ++b) {
         Plan& pl = plans[b];
         int rc = fill_problem(ctx, pl.P, E, H[b], W[b], M, shiftX ? shiftX[b] : 0, shiftY ? shiftY[b] : 0, f[b], ppx[b], ppy[b], tau,
-                              alpha, beta, maxReproj, sub);
+                              alpha, beta, maxReproj, sub, DRAWS);
         if (rc) return fail(ctx, rc, "image %d: %s", b, std::string(ctx->err).c_str());
-        if ((long long)(W[b] - 1) * (H[b] - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too small", b, W[b], H[b]);
         pl.d_coords = nullptr;
     }
     bool dev_coords = false;
@@ -1201,8 +1233,7 @@ int esacb200_forward_ragged(esacb200_ctx* ctx, int B, const float* const* coords
     }
     ctx->st.M = M;
     ctx->st.winner = (int)host[(size_t)(B - 1) * 20 + 18];
-    ctx->last_M = M;
-    ctx->last_backward = false;
+    record_draw(ctx, plans[B - 1], false);  // the buffers hold the last image's hypotheses
     finish_stats(ctx);
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
@@ -1215,11 +1246,7 @@ int esacb200_forward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords
     if (!ctx) return ESACB200_ERR_ARG;
     if (!coords || !assign || !out_poses || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
-    Problem P;
-    int rc = fill_problem(ctx, P, E, H, W, M, 0, 0, f[0], ppx[0], ppy[0], tau, alpha, beta, maxReproj, sub);
-    if (rc) return rc;
-    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small", W, H);
-    const size_t cstride = (size_t)E * 3 * H * W;
+    const size_t cstride = (size_t)E * 3 * H * W;  // (sizes are checked image by image by the ragged call)
     std::vector<const float*> ptrs((size_t)B);
     for (int b = 0; b < B; ++b) ptrs[b] = coords + (size_t)b * cstride;
     const std::vector<int> hs((size_t)B, H), ws((size_t)B, W);
@@ -1302,22 +1329,84 @@ static int async_workspace(esacb200_ctx* ctx, esacb200_ctx* a, const std::vector
     return 0;
 }
 
-int esacb200_reserve_forward_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int sub) try {
+// reserve_forward_async / reserve_backward_async (`backward`): sizes the async workspace for B images of one shape.
+static int reserve_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int sub, bool backward) {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
-    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "reserve_forward_async: empty batch (B=%d)", B);
+    const char* what = backward ? "backward_async" : "forward_async";
+    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "reserve_%s: empty batch (B=%d)", what, B);
     std::vector<Plan> plans(1);
-    int rc = fill_problem(ctx, plans[0].P, E, H, W, M, 0, 0, 1.f, 0.f, 0.f, 1.f, 1.f, 1.f, 1.f, sub);
+    int rc = fill_problem(ctx, plans[0].P, E, H, W, M, 0, 0, 1.f, 0.f, 0.f, 1.f, 1.f, 1.f, 1.f, sub, NO_DRAW);
     if (rc) return rc;
     plans[0].d_coords = nullptr;  // the load path does not change the workspace
     bool capturing = false;
     rc = stream_capturing(ctx, capturing);
     if (rc) return rc;
-    if (capturing) return fail(ctx, ESACB200_ERR_ARG, "reserve_forward_async allocates: call it before the capture");
+    if (capturing) return fail(ctx, ESACB200_ERR_ARG, "reserve_%s allocates: call it before the capture", what);
     esacb200_ctx* a = nullptr;
-    rc = async_context(ctx, false, "forward_async", &a);
+    rc = async_context(ctx, false, what, &a);
     if (rc) return rc;
-    return async_workspace(ctx, a, plans, false, false);
+    return async_workspace(ctx, a, plans, false, backward);
+}
+
+// A stream-ordered call of B images of one shape: the async context, and per image its Plan and its AsyncImage (whose
+// outputs the entry point fills in).
+struct AsyncCall {
+    esacb200_ctx* a = nullptr;
+    std::vector<Plan> plans;
+    std::vector<AsyncImage> imgs;
+};
+
+// What forward_async and backward_async (`backward`) share: checks the arguments (the n arrays `ptrs`, called `names`, must
+// be device memory), takes the async context, lays out the images and fits the workspace to them.
+static int begin_async(esacb200_ctx* ctx, bool backward, int B, const float* coords, int E, int H, int W, const int64_t* assign,
+                       int64_t assign_stride, int M, const int32_t* shifts, const float* cameras, float tau, float alpha,
+                       float beta, float maxReproj, int sub, int32_t* out_status, int n, const void* const* ptrs,
+                       const char* const* names, AsyncCall& call) {
+    const char* what = backward ? "backward_async" : "forward_async";
+    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "%s: empty batch (B=%d)", what, B);
+    Problem P;
+    int rc = fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, tau, alpha, beta, maxReproj, sub, DRAWS);
+    if (rc) return rc;
+    for (int i = 0; i < n; ++i) {
+        if (!ptrs[i]) return fail(ctx, ESACB200_ERR_ARG, "%s: %s is null", what, names[i]);
+        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "%s takes device pointers only: %s is host memory", what, names[i]);
+    }
+    bool capturing = false;
+    rc = stream_capturing(ctx, capturing);
+    if (rc) return rc;
+    rc = async_context(ctx, capturing, what, &call.a);
+    if (rc) return rc;
+    esacb200_ctx* a = call.a;
+    // element stride between the assignments of consecutive images: rows of a [B, M] tensor
+    const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
+    const size_t cstride = (size_t)E * 3 * H * W;
+    call.plans.resize((size_t)B);
+    call.imgs.resize((size_t)B);
+    for (int b = 0; b < B; ++b) {
+        Plan& pl = call.plans[b];
+        pl.P = P;
+        pl.d_coords = coords + (size_t)b * cstride;
+        pl.d_assign = (const long long*)assign + b * arow;
+        pl.assign_stride = assign_stride;
+        AsyncImage& im = call.imgs[b];
+        im.dev.shift = shifts + 2 * (size_t)b;
+        im.dev.cam = cameras + 3 * (size_t)b;
+        im.dev.seed = a->seed_state.as<unsigned long long>();
+        im.dev.index = b;
+        im.dev.fixed_seed = a->opt.fixed_seed;
+        im.status = out_status + b;
+        im.advance = b == B - 1 ? B : 0;
+        pl.async = &im;
+    }
+    rc = async_workspace(ctx, a, call.plans, capturing, backward);
+    if (rc) return rc;
+    if (capturing) a->frozen = true;
+    return 0;
+}
+
+int esacb200_reserve_forward_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int sub) try {
+    return reserve_async(ctx, B, E, H, W, M, sub, false);
 } ESAC_ABI_CATCH(ctx)
 
 int esacb200_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
@@ -1325,53 +1414,18 @@ int esacb200_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E,
                            float beta, float maxReproj, int sub, float* out_poses, int64_t* out_experts, int32_t* out_status) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
-    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "forward_async: empty batch (B=%d)", B);
-    Problem P;
-    int rc = fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, tau, alpha, beta, maxReproj, sub);
-    if (rc) return rc;
-    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small to draw 4 distinct cells", W, H);
     const void* ptrs[] = {coords, assign, shifts, cameras, out_poses, out_experts, out_status};
     const char* names[] = {"coords", "assign", "shifts", "cameras", "out_poses", "out_experts", "out_status"};
-    for (int i = 0; i < 7; ++i) {
-        if (!ptrs[i]) return fail(ctx, ESACB200_ERR_ARG, "forward_async: %s is null", names[i]);
-        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "forward_async takes device pointers only: %s is host memory", names[i]);
-    }
-    bool capturing = false;
-    rc = stream_capturing(ctx, capturing);
+    AsyncCall call;
+    int rc = begin_async(ctx, false, B, coords, E, H, W, assign, assign_stride, M, shifts, cameras, tau, alpha, beta, maxReproj,
+                         sub, out_status, 7, ptrs, names, call);
     if (rc) return rc;
-    esacb200_ctx* a = nullptr;
-    rc = async_context(ctx, capturing, "forward_async", &a);
-    if (rc) return rc;
-    // element stride between the assignments of consecutive images: rows of a [B, M] tensor
-    const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
-    const size_t cstride = (size_t)E * 3 * H * W;
-    std::vector<Plan> plans((size_t)B);
-    std::vector<AsyncImage> imgs((size_t)B);
     for (int b = 0; b < B; ++b) {
-        Plan& pl = plans[b];
-        pl.P = P;
-        pl.d_coords = coords + (size_t)b * cstride;
-        pl.d_assign = (const long long*)assign + b * arow;
-        pl.assign_stride = assign_stride;
-        AsyncImage& im = imgs[b];
-        im.dev.shift = shifts + 2 * (size_t)b;
-        im.dev.cam = cameras + 3 * (size_t)b;
-        im.dev.seed = a->seed_state.as<unsigned long long>();
-        im.dev.index = b;
-        im.dev.fixed_seed = a->opt.fixed_seed;
-        im.pose = out_poses + 16 * (size_t)b;
-        im.expert = (long long*)out_experts + b;
-        im.status = out_status + b;
-        im.advance = b == B - 1 ? B : 0;
-        pl.async = &im;
-    }
-    rc = async_workspace(ctx, a, plans, capturing, false);
-    if (rc) return rc;
-    if (capturing) a->frozen = true;
-    for (int b = 0; b < B; ++b) {
-        rc = plan_and_prep(a, plans[b]);
-        if (!rc) rc = enqueue_forward_core(a, plans[b], nullptr);
-        if (rc) return fail(ctx, rc, "image %d: %s", b, a->err);
+        call.imgs[b].pose = out_poses + 16 * (size_t)b;
+        call.imgs[b].expert = (long long*)out_experts + b;
+        rc = plan_and_prep(call.a, call.plans[b]);
+        if (!rc) rc = enqueue_forward_core(call.a, call.plans[b], nullptr);
+        if (rc) return fail(ctx, rc, "image %d: %s", b, call.a->err);
     }
     CK(cudaGetLastError());
     return ESACB200_OK;
@@ -1385,7 +1439,7 @@ int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, i
     DeviceGuard device_guard(ctx->device);
     if (!coords || !assign || !poses6 || !out_scores) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
     Plan pl;
-    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub);
+    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, NO_DRAW);
     if (rc) return rc;
     begin_call(ctx);
     rc = stage_inputs(ctx, pl, coords, assign, assign_stride);
@@ -1395,19 +1449,7 @@ int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, i
     rc = run_score(ctx, pl);
     if (rc) return rc;
     CK(cudaMemcpyAsync(out_scores, ctx->scores.p, (size_t)M * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_out + 20, ctx->scalars.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    mark(ctx, EV_END);
-    CK(cudaStreamSynchronize(ctx->stream));
-    CK(cudaGetLastError());
-    const int* hs = (const int*)(ctx->h_out + 20);
-    if (hs[S_FLAGS]) return fail(ctx, ESACB200_ERR_ARG, "hypAssignment holds an expert index outside [0, %d)", E);
-    ctx->st.M = M;
-    ctx->st.winner = hs[S_WINNER];
-    ctx->st.n_contrib = hs[S_NCONTRIB];
-    ctx->last_M = M;
-    ctx->last_backward = false;
-    finish_stats(ctx);
-    return ESACB200_OK;
+    return finish_call(ctx, pl, 0, false);
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
@@ -1418,7 +1460,7 @@ int esacb200_refine_poses(esacb200_ctx* ctx, const float* coords, int E, int H, 
     DeviceGuard device_guard(ctx->device);
     if (!coords || !assign || !poses6) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
     Plan pl;
-    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, 100.f, 0.5f, maxReproj, sub);
+    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, 100.f, 0.5f, maxReproj, sub, NO_DRAW);
     if (rc) return rc;
     begin_call(ctx);
     rc = stage_inputs(ctx, pl, coords, assign, assign_stride);
@@ -1457,7 +1499,6 @@ int esacb200_refine_poses(esacb200_ctx* ctx, const float* coords, int E, int H, 
         }
     }
     ctx->st.M = M;
-    ctx->last_M = M;
     finish_stats(ctx);
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
@@ -1490,6 +1531,17 @@ static int for_flagged_planes(esacb200_ctx* ctx, int E, size_t plane, float* wor
         }
         e = e1;
     }
+    return 0;
+}
+
+// The gradient tensor the kernels accumulate into: `grads` itself on the device, else a copy of the host tensor in the
+// workspace (d_grads != grads: the caller copies it back after the kernels).
+static int stage_grads(esacb200_ctx* ctx, float* grads, size_t bytes, float*& d_grads) {
+    d_grads = grads;
+    if (is_device_ptr(grads)) return 0;
+    CK(ctx->grads.ensure(bytes));
+    CK(cudaMemcpyAsync(ctx->grads.p, grads, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    d_grads = ctx->grads.as<float>();
     return 0;
 }
 
@@ -1607,20 +1659,14 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
     DeviceGuard device_guard(ctx->device);
     if (!coords || !assign || !grads || !gt_pose) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
     Plan pl;
-    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub);
+    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS_INJECTED);
     if (rc) return rc;
-    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small to draw 4 distinct cells from [0,W-2]x[0,H-2]", W, H);
-    if (ctx->inj_M && ctx->inj_M != M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are for M=%d, call has M=%d", ctx->inj_M, M);
     begin_call(ctx);
     const Problem& P = pl.P;
     const size_t cbytes = (size_t)P.E * 3 * P.N * sizeof(float);
-    float* d_grads = grads;
-    const bool grads_on_host = !is_device_ptr(grads);
-    if (grads_on_host) {
-        CK(ctx->grads.ensure(cbytes));
-        CK(cudaMemcpyAsync(ctx->grads.p, grads, cbytes, cudaMemcpyHostToDevice, ctx->stream));
-        d_grads = ctx->grads.as<float>();
-    }
+    float* d_grads = nullptr;
+    rc = stage_grads(ctx, grads, cbytes, d_grads);
+    if (rc) return rc;
     // hypothesis-major sharding: every rank holds all planes and a slice of the hypotheses, so the gradient slices overlap:
     // the local gradient goes to a zeroed work buffer, is summed over the ranks and only then added to the caller's tensor
     float* d_dst = d_grads;
@@ -1639,7 +1685,6 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
     sh.d_dst = d_dst;
     rc = run_hypotheses(ctx, pl, coords, assign, assign_stride, sh, nullptr);
     if (rc) return rc;
-    int* sc = ctx->scalars.as<int>();
     rc = backward_buffers(ctx, P, true, grow(ctx));
     if (rc) return rc;
     BwdArgs b = backward_args(ctx, pl, d_grads);
@@ -1682,25 +1727,12 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
         d_grads = d_dst;
     }
     mark(ctx, EV_BWD);
-    if (grads_on_host) CK(cudaMemcpyAsync(grads, d_grads, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_out + 20, sc, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.p, 8 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    mark(ctx, EV_END);
-    CK(cudaStreamSynchronize(ctx->stream));
-    CK(cudaGetLastError());
-    const int* hs = (const int*)(ctx->h_out + 20);
-    if (hs[S_FLAGS]) return fail(ctx, ESACB200_ERR_ARG, "hypAssignment holds an expert index outside [0, %d)", E);
+    if (d_grads != grads) CK(cudaMemcpyAsync(grads, d_grads, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
+    rc = finish_call(ctx, pl, 8, true, /*losses=*/true);
+    if (rc) return rc;
     if (use_nccl) global_loss = ctx->h_dbl[7];
-    if (out_loss) *out_loss = (exchange || use_nccl) ? global_loss : ctx->h_dbl[4];
-    ctx->st.M = M;
-    ctx->st.winner = hs[S_WINNER];
-    ctx->st.n_contrib = hs[S_NCONTRIB];
-    ctx->st.entropy = ctx->h_dbl[0];
     ctx->st.expected_loss = (exchange || use_nccl) ? global_loss : ctx->h_dbl[4];
-    ctx->last_M = M;
-    ctx->last_backward = true;
-    finish_stats(ctx);
-    ctx->inj_M = ctx->inj_T = 0;
+    if (out_loss) *out_loss = ctx->st.expected_loss;
     return ESACB200_OK;
 }
 
@@ -1717,21 +1749,7 @@ int esacb200_backward(esacb200_ctx* ctx, const float* coords, float* grads, int 
 // context as forward_async (ctx->async) and counts calls with it; the host path is the eager one, with the refinement group
 // picked on the device from the number of contributing hypotheses.
 int esacb200_reserve_backward_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int sub) try {
-    if (!ctx) return ESACB200_ERR_ARG;
-    DeviceGuard device_guard(ctx->device);
-    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "reserve_backward_async: empty batch (B=%d)", B);
-    std::vector<Plan> plans(1);
-    int rc = fill_problem(ctx, plans[0].P, E, H, W, M, 0, 0, 1.f, 0.f, 0.f, 1.f, 1.f, 1.f, 1.f, sub);
-    if (rc) return rc;
-    plans[0].d_coords = nullptr;  // the load path does not change the workspace
-    bool capturing = false;
-    rc = stream_capturing(ctx, capturing);
-    if (rc) return rc;
-    if (capturing) return fail(ctx, ESACB200_ERR_ARG, "reserve_backward_async allocates: call it before the capture");
-    esacb200_ctx* a = nullptr;
-    rc = async_context(ctx, false, "backward_async", &a);
-    if (rc) return rc;
-    return async_workspace(ctx, a, plans, false, true);
+    return reserve_async(ctx, B, E, H, W, M, sub, true);
 } ESAC_ABI_CATCH(ctx)
 
 int esacb200_backward_async(esacb200_ctx* ctx, int B, const float* coords, float* grads, int E, int H, int W,
@@ -1740,64 +1758,31 @@ int esacb200_backward_async(esacb200_ctx* ctx, int B, const float* coords, float
                             float maxReproj, int sub, double* out_losses, int32_t* out_status) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
-    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "backward_async: empty batch (B=%d)", B);
-    Problem P;
-    int rc = fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, tau, alpha, beta, maxReproj, sub);
-    if (rc) return rc;
-    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small to draw 4 distinct cells", W, H);
     const void* ptrs[] = {coords, grads, assign, gt_poses, shifts, cameras, out_losses, out_status};
     const char* names[] = {"coords", "grads", "assign", "gt_poses", "shifts", "cameras", "out_losses", "out_status"};
-    for (int i = 0; i < 8; ++i) {
-        if (!ptrs[i]) return fail(ctx, ESACB200_ERR_ARG, "backward_async: %s is null", names[i]);
-        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "backward_async takes device pointers only: %s is host memory", names[i]);
-    }
-    bool capturing = false;
-    rc = stream_capturing(ctx, capturing);
+    AsyncCall call;
+    int rc = begin_async(ctx, true, B, coords, E, H, W, assign, assign_stride, M, shifts, cameras, tau, alpha, beta, maxReproj,
+                         sub, out_status, 8, ptrs, names, call);
     if (rc) return rc;
-    esacb200_ctx* a = nullptr;
-    rc = async_context(ctx, capturing, "backward_async", &a);
-    if (rc) return rc;
-    const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
+    esacb200_ctx* a = call.a;
     const size_t cstride = (size_t)E * 3 * H * W;
-    std::vector<Plan> plans((size_t)B);
-    std::vector<AsyncImage> imgs((size_t)B);
     for (int b = 0; b < B; ++b) {
-        Plan& pl = plans[b];
-        pl.P = P;
-        pl.d_coords = coords + (size_t)b * cstride;
-        pl.d_assign = (const long long*)assign + b * arow;
-        pl.assign_stride = assign_stride;
-        AsyncImage& im = imgs[b];
-        im.dev.shift = shifts + 2 * (size_t)b;
-        im.dev.cam = cameras + 3 * (size_t)b;
-        im.dev.seed = a->seed_state.as<unsigned long long>();
-        im.dev.index = b;
-        im.dev.fixed_seed = a->opt.fixed_seed;
-        im.pose = nullptr;
-        im.expert = nullptr;
+        Plan& pl = call.plans[b];
+        AsyncImage& im = call.imgs[b];
         im.loss = out_losses + b;
         im.gt = gt_poses + 16 * (size_t)b;
-        im.status = out_status + b;
-        im.advance = b == B - 1 ? B : 0;
-        pl.async = &im;
-    }
-    rc = async_workspace(ctx, a, plans, capturing, true);
-    if (rc) return rc;
-    if (capturing) a->frozen = true;
-    for (int b = 0; b < B; ++b) {
-        Plan& pl = plans[b];
         rc = run_hypotheses(a, pl, pl.d_coords, (const int64_t*)pl.d_assign, assign_stride, ShardSteps(), nullptr);
-        if (!rc) rc = backward_buffers(a, P, true, grow(a));
+        if (!rc) rc = backward_buffers(a, pl.P, true, grow(a));
         if (rc) return fail(ctx, rc, "image %d: %s", b, a->err);
         BwdArgs args = backward_args(a, pl, grads + (size_t)b * cstride);
         args.wRot = wRot; args.wTrans = wTrans; args.cut = cut;
         BwdDev dv;
-        dv.gt = imgs[b].gt;
+        dv.gt = im.gt;
         dv.flags = a->scalars.as<int>() + S_FLAGS;
-        dv.dev = imgs[b].dev;
+        dv.dev = im.dev;
         launch_backward(args, M, a->sm_count, a->stream, &dv);
-        launch_finish_backward_async(a->stats.as<double>(), a->scalars.as<int>() + S_FLAGS, imgs[b].loss, imgs[b].status,
-                                     a->seed_state.as<unsigned long long>(), imgs[b].advance, a->stream);
+        launch_finish_backward_async(a->stats.as<double>(), a->scalars.as<int>() + S_FLAGS, im.loss, im.status,
+                                     a->seed_state.as<unsigned long long>(), im.advance, a->stream);
         a->st.kernel_launches += 6;
     }
     CK(cudaGetLastError());
@@ -1820,10 +1805,8 @@ static int hypotheses_forward_impl(esacb200_ctx* ctx, const float* coords, int E
     DeviceGuard device_guard(ctx->device);
     if (!coords || !assign || !tape || !out_scores || !out_poses6 || !out_contrib) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
     Plan pl;
-    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub);
+    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS_INJECTED);
     if (rc) return rc;
-    if ((long long)(W - 1) * (H - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small to draw 4 distinct cells from [0,W-2]x[0,H-2]", W, H);
-    if (ctx->inj_M && ctx->inj_M != M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are for M=%d, call has M=%d", ctx->inj_M, M);
     const size_t need = tape_bytes(M, pl.P.N);
     if (tape_bytes_ < need) return fail(ctx, ESACB200_ERR_ARG, "tape holds %zu bytes, this call needs %zu", tape_bytes_, need);
     if (!is_device_ptr(tape) || ((uintptr_t)tape & 15)) return fail(ctx, ESACB200_ERR_ARG, "tape must be 16-byte aligned device memory");
@@ -1855,22 +1838,7 @@ static int hypotheses_forward_impl(esacb200_ctx* ctx, const float* coords, int E
     CK(cudaMemcpyAsync(out_scores, ctx->scores.p, (size_t)M * 8, cudaMemcpyDefault, ctx->stream));
     CK(cudaMemcpyAsync(out_poses6, ctx->poses_ref.p, (size_t)M * sizeof(Pose), cudaMemcpyDefault, ctx->stream));
     CK(cudaMemcpyAsync(out_contrib, ctx->contrib8.p, (size_t)M, cudaMemcpyDefault, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_out + 20, sc, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.p, 3 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
-    mark(ctx, EV_END);
-    CK(cudaStreamSynchronize(ctx->stream));
-    CK(cudaGetLastError());
-    const int* hs = (const int*)(ctx->h_out + 20);
-    if (hs[S_FLAGS]) return fail(ctx, ESACB200_ERR_ARG, "hypAssignment holds an expert index outside [0, %d)", E);
-    ctx->st.M = M;
-    ctx->st.winner = hs[S_WINNER];
-    ctx->st.n_contrib = hs[S_NCONTRIB];
-    ctx->st.entropy = ctx->h_dbl[0];
-    ctx->last_M = M;
-    ctx->last_backward = false;
-    finish_stats(ctx);
-    ctx->inj_M = ctx->inj_T = 0;
-    return ESACB200_OK;
+    return finish_call(ctx, pl, 3, true);
 }
 
 int esacb200_hypotheses_forward(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
@@ -1907,13 +1875,9 @@ static int hypotheses_backward_impl(esacb200_ctx* ctx, const void* tape, const f
         CK(cudaMemcpyAsync(ctx->coords.p, coords, cbytes, cudaMemcpyHostToDevice, ctx->stream));
         d_coords = ctx->coords.as<float>();
     }
-    float* d_grads = grads;
-    const bool grads_on_host = !is_device_ptr(grads);
-    if (grads_on_host) {
-        CK(ctx->grads.ensure(cbytes));
-        CK(cudaMemcpyAsync(ctx->grads.p, grads, cbytes, cudaMemcpyHostToDevice, ctx->stream));
-        d_grads = ctx->grads.as<float>();
-    }
+    float* d_grads = nullptr;
+    int rc = stage_grads(ctx, grads, cbytes, d_grads);
+    if (rc) return rc;
     // upstream gradients: [M] of the scores then [M,6] of the poses; an absent one is zero
     CK(ctx->upstream.ensure((size_t)M * 7 * 8));
     double* up = ctx->upstream.as<double>();
@@ -1922,7 +1886,7 @@ static int hypotheses_backward_impl(esacb200_ctx* ctx, const void* tape, const f
     if (d_poses6) CK(cudaMemcpyAsync(up + M, d_poses6, (size_t)M * 6 * 8, cudaMemcpyDefault, ctx->stream));
     else CK(cudaMemsetAsync(up + M, 0, (size_t)M * 6 * 8, ctx->stream));
     mark(ctx, EV_REFINE);
-    int rc = backward_buffers(ctx, P, false, grow(ctx));
+    rc = backward_buffers(ctx, P, false, grow(ctx));
     if (rc) return rc;
     BwdArgs b;
     memset(&b, 0, sizeof(b));
@@ -1939,7 +1903,7 @@ static int hypotheses_backward_impl(esacb200_ctx* ctx, const void* tape, const f
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 5;
     mark(ctx, EV_BWD);
-    if (grads_on_host) CK(cudaMemcpyAsync(grads, d_grads, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
+    if (d_grads != grads) CK(cudaMemcpyAsync(grads, d_grads, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
@@ -2049,7 +2013,6 @@ int esacb200_backward_sharded_nccl(esacb200_ctx* ctx, const float* coords, float
     CK(cudaStreamSynchronize(ctx->stream));
     if (out_loss) *out_loss = ctx->h_dbl[4];
     ctx->st.expected_loss = ctx->h_dbl[4];
-    ctx->last_M = 0;
     finish_stats(ctx);
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
@@ -2064,6 +2027,7 @@ int esacb200_backward_sharded_nccl(esacb200_ctx* ctx, const float* coords, float
 // of the call are those of the last image, with the wall time and kernel launches of the whole batch.
 static int run_batch(esacb200_ctx* ctx, int B, const int* H, const int* W, bool draws,
                      const std::function<int(esacb200_ctx*, int)>& image) {
+    ctx->last = LastCall();  // the per-hypothesis buffers the images write are the workers'
     CK(cudaStreamSynchronize(ctx->stream));
     std::vector<uint64_t> seeds((size_t)B);
     if (draws)
@@ -2118,16 +2082,16 @@ static int run_batch(esacb200_ctx* ctx, int B, const int* H, const int* W, bool 
     for (int wi = 0; wi < nw; ++wi) total += launches[wi];
     ctx->st.kernel_launches = total;
     ctx->st.ms_total = (float)wall_ms;
-    ctx->last_M = 0;  // the per-hypothesis buffers live in the workers
     return ESACB200_OK;
 }
 
-// Sizes of a ragged batch: every image positive, addressable and large enough to draw 4 distinct cells from.
-static int check_ragged_sizes(esacb200_ctx* ctx, int B, const int* H, const int* W) {
+// The sizes of a ragged batch whose images draw M hypotheses each (or, hypotheses_backward_ragged, were drawn from): the
+// checks of fill_problem, image by image, before any image runs.
+static int check_ragged_draws(esacb200_ctx* ctx, int B, int E, const int* H, const int* W, int M) {
     for (int b = 0; b < B; ++b) {
-        if (H[b] <= 0 || W[b] <= 0) return fail(ctx, ESACB200_ERR_ARG, "image %d: bad size %dx%d", b, W[b], H[b]);
-        if ((long long)H[b] * W[b] > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too large", b, W[b], H[b]);
-        if ((long long)(W[b] - 1) * (H[b] - 1) < 4) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too small", b, W[b], H[b]);
+        Problem P;
+        if (fill_problem(ctx, P, E, H[b], W[b], M, 0, 0, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 1, DRAWS))
+            return fail(ctx, ESACB200_ERR_ARG, "image %d: %s", b, std::string(ctx->err).c_str());
     }
     return 0;
 }
@@ -2145,7 +2109,7 @@ int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coord
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
     if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
     if (E <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d M=%d", E, M);
-    int rc = check_ragged_sizes(ctx, B, H, W);
+    int rc = check_ragged_draws(ctx, B, E, H, W, M);
     if (rc) return rc;
     bool dev_c = false, dev_g = false;
     rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
@@ -2168,9 +2132,7 @@ int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coord
         if (!rc && out_losses) out_losses[b] = loss;
         return rc;
     });
-    if (rc) return rc;
-    ctx->last_backward = true;
-    return ESACB200_OK;
+    return rc ? rc : ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 
 // The hypotheses node over a batch, on the worker contexts of run_batch: image b runs the single-image forward / backward
@@ -2187,7 +2149,7 @@ int esacb200_hypotheses_forward_ragged(esacb200_ctx* ctx, int B, const float* co
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
     if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
     if (E <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d M=%d", E, M);
-    int rc = check_ragged_sizes(ctx, B, H, W);
+    int rc = check_ragged_draws(ctx, B, E, H, W, M);
     if (rc) return rc;
     bool dev_c = false;
     rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
@@ -2207,9 +2169,7 @@ int esacb200_hypotheses_forward_ragged(esacb200_ctx* ctx, int B, const float* co
                                        maxReproj, sub, tapes[b], tape_bytes_[b], out_scores + (size_t)b * M,
                                        out_poses6 + (size_t)b * M * 6, out_contrib + (size_t)b * M);
     });
-    if (rc) return rc;
-    ctx->last_backward = false;
-    return ESACB200_OK;
+    return rc ? rc : ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 
 int esacb200_hypotheses_backward_ragged(esacb200_ctx* ctx, int B, const void* const* tapes, const float* const* coords,
@@ -2220,7 +2180,7 @@ int esacb200_hypotheses_backward_ragged(esacb200_ctx* ctx, int B, const void* co
     if (!tapes || !coords || !grads || !H || !W || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
     if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
     if (E <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad size E=%d", E);
-    int rc = check_ragged_sizes(ctx, B, H, W);
+    int rc = check_ragged_draws(ctx, B, E, H, W, 1);
     if (rc) return rc;
     bool dev_c = false, dev_g = false, dev_t = false;
     rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
@@ -2412,7 +2372,6 @@ int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* co
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
-    ctx->last_M = 0;
     finish_stats(ctx);
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
@@ -2530,7 +2489,6 @@ int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pre
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
-    ctx->last_M = 0;
     finish_stats(ctx);
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
@@ -2559,10 +2517,17 @@ int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int
                                       grads ? gp.data() : nullptr, cut, out_losses, out_counts);
 } ESAC_ABI_CATCH(ctx)
 
+// The getters below read only what the last call on the context wrote (LastCall).
+static int last_call_left(esacb200_ctx* ctx, bool wrote, const char* what) {
+    return wrote ? 0 : fail(ctx, ESACB200_ERR_ARG, "the last call on this context left no %s", what);
+}
+
 int esacb200_copy_last_scores(esacb200_ctx* ctx, double* dst, int M) try {
     if (!ctx || !dst) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
-    if (M != ctx->last_M) return fail(ctx, ESACB200_ERR_ARG, "last call had M=%d, asked for %d", ctx->last_M, M);
+    int rc = last_call_left(ctx, ctx->last.scored, "scores");
+    if (rc) return rc;
+    if (M != ctx->last.M) return fail(ctx, ESACB200_ERR_ARG, "last call had M=%d, asked for %d", ctx->last.M, M);
     CK(cudaMemcpyAsync(dst, ctx->scores.p, (size_t)M * 8, cudaMemcpyDefault, ctx->stream));
     if (!is_device_ptr(dst)) CK(cudaStreamSynchronize(ctx->stream));
     return ESACB200_OK;
@@ -2595,8 +2560,9 @@ int esacb200_get_sample_profile(esacb200_ctx* ctx, long long* out8) try {
     if (!ctx || !out8) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     for (int i = 0; i < 8; ++i) out8[i] = 0;
-    const int G = ctx->smp_groups_last, M = ctx->last_M, Mg = ctx->smp_Mg_last;
-    if (G <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "no previous call");
+    int rc = last_call_left(ctx, ctx->last.drew, "sampling profile");
+    if (rc) return rc;
+    const int G = ctx->last.lanes, M = ctx->last.M, Mg = ctx->last.lane_cap;
     CK(cudaStreamSynchronize(ctx->stream));
     const size_t per_group_ints = (size_t)2 * Mg + 8;
     for (int g = 0; g < G; ++g) {
@@ -2617,18 +2583,17 @@ int esacb200_get_hypotheses(esacb200_ctx* ctx, double* poses6, int32_t* cells, i
                             double* probs, double* refined6, double* losses) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
-    const int M = ctx->last_M;
-    if (M <= 0) return fail(ctx, ESACB200_ERR_ARG, "no previous call");
+    int rc = last_call_left(ctx, ctx->last.drew, "hypotheses");
+    if (!rc && losses) rc = last_call_left(ctx, ctx->last.losses, "per-hypothesis losses");
+    if (rc) return rc;
+    const int M = ctx->last.M;
     if (poses6) CK(cudaMemcpy(poses6, ctx->poses.p, (size_t)M * sizeof(Pose), cudaMemcpyDeviceToHost));
     if (cells) CK(cudaMemcpy(cells, ctx->cells.p, (size_t)M * 32, cudaMemcpyDeviceToHost));
     if (tries) CK(cudaMemcpy(tries, ctx->tries.p, (size_t)M * 4, cudaMemcpyDeviceToHost));
     if (scores) CK(cudaMemcpy(scores, ctx->scores.p, (size_t)M * 8, cudaMemcpyDeviceToHost));
     if (probs) CK(cudaMemcpy(probs, ctx->probs.p, (size_t)M * 8, cudaMemcpyDeviceToHost));
     if (refined6) CK(cudaMemcpy(refined6, ctx->poses_ref.p, (size_t)M * sizeof(Pose), cudaMemcpyDeviceToHost));
-    if (losses) {
-        if (!ctx->last_backward) return fail(ctx, ESACB200_ERR_ARG, "losses exist only after backward");
-        CK(cudaMemcpy(losses, ctx->losses.p, (size_t)M * 8, cudaMemcpyDeviceToHost));
-    }
+    if (losses) CK(cudaMemcpy(losses, ctx->losses.p, (size_t)M * 8, cudaMemcpyDeviceToHost));
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 

@@ -403,22 +403,30 @@ int esacb200_get_refine_profile(esacb200_ctx* ctx, long long* out16);
 
 /* Diagnostics of the last call's sampling stage (summed over its lanes): [0] tries that went through the float prefilter,
  * [1] survivors the fp64 path judged, [2] waves that had work (max over lanes), [3] hypotheses left to the tail kernel,
- * [4] accepted tries staged, [5] lanes.  out8: host long long [8]. */
+ * [4] accepted tries staged, [5] lanes.  out8: host long long [8].  Valid after a call that drew hypotheses (those listed
+ * at esacb200_get_hypotheses); after any other call it fails with ESACB200_ERR_ARG. */
 int esacb200_get_sample_profile(esacb200_ctx* ctx, long long* out8);
 /* With option "sample_trace" = 1 the prefilter / exact kernels of the sampling waves stamp %globaltimer: out512 (host uint64
  * [4 lanes][32 waves][2 kernels: prefilter, exact][2: first CTA start, last CTA end], ns; start = ~0 where nothing ran).
  * Only waves 0-31 of each lane are stamped: with option "sample_waves" above 32 the later waves run but are not traced. */
 int esacb200_get_sample_trace(esacb200_ctx* ctx, unsigned long long* out512);
 
-/* Read back intermediates of the last forward/backward call (any pointer may be NULL):
+/* Read back intermediates of the last call (any pointer may be NULL), M = esacb200_get_stats' M:
  * poses6 double [M][6] initial hypotheses, cells int32 [M][4][2], tries int32 [M], scores / probs double [M],
- * refined6 double [M][6] (backward: refined poses; forward: only the winner's row is meaningful),
- * losses double [M] (backward). */
+ * refined6 double [M][6] (backward, hypotheses_forward: refined poses; forward: only the winner's row is meaningful),
+ * losses double [M] (backward).
+ * Valid after a call that drew hypotheses on this context: forward, backward (and backward_sharded[_nccl] with M > 0),
+ * hypotheses_forward, forward_pack / forward_sharded with M > 0, and forward_ragged / forward_batch[_cameras] (the last
+ * image's).  `losses` is valid only after backward and its sharded forms.  After any other call (score_poses, refine_poses,
+ * the loss entry points, hypotheses_backward, the batches that run on worker contexts) it fails with
+ * ESACB200_ERR_ARG and writes nothing. */
 int esacb200_get_hypotheses(esacb200_ctx* ctx, double* poses6, int32_t* cells, int32_t* tries, double* scores,
                             double* probs, double* refined6, double* losses);
 
 /* Copies the last call's scores (double [M]) to `dst` (host or device pointer), stream-ordered on the
- * context's stream; used by the multi-GPU path to feed its all-gather without a host round trip. */
+ * context's stream; used by the multi-GPU path to feed its all-gather without a host round trip.  Valid after the calls
+ * listed at esacb200_get_hypotheses and after score_poses; fails with ESACB200_ERR_ARG after any other call, or when M is
+ * not the last call's. */
 int esacb200_copy_last_scores(esacb200_ctx* ctx, double* dst, int M);
 
 /* Device properties the bench needs without importing a CUDA binding: SM count and name. */

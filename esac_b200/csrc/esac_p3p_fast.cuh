@@ -4,12 +4,12 @@
 // two lines, line-conic intersections), specialised for throughput: one real root of the cubic (any real root is
 // enough whenever the P3P has a real solution), no loops over dynamically sized sets, no dynamically indexed arrays
 // (3-way selects instead), reciprocal / rsqrt approximations, and NO data-dependent branch: every "this try certainly
-// fails" / "this try goes to the exact path" exit of the straightforward formulation is a lane mask that latches the
-// verdict, and the arithmetic simply runs on (garbage in decided lanes is harmless).  That is what lets one thread
-// judge TWO tries at once (Pack2: two independent dependency chains side by side in a float2); Pack1 is the same code
-// on one try (tail kernel, host test hooks).  Every decision that is numerically borderline returns "may pass", i.e.
-// hands the try to the exact fp64 path; the invariant "an accepted try is never rejected here" is what
-// tests/test_host_geom.py::test_float_prefilter_never_rejects_an_accepted_try checks, for both packings.
+// fails" / "this try goes to the exact path" exit of the straightforward formulation is a mask that latches the
+// verdict, and the arithmetic simply runs on (garbage after a decision is harmless), so a warp never diverges on it.
+// The code is written over a value pack (Pack1: one try per thread; a pack of two tries side by side in a float2 paid
+// on Blackwell's packed fp32x2 pipe and was measured slower on the H100, which has none).  Every decision that is
+// numerically borderline returns "may pass", i.e. hands the try to the exact fp64 path; the invariant "an accepted try
+// is never rejected here" is what tests/test_host_geom.py::test_float_prefilter_never_rejects_an_accepted_try checks.
 #pragma once
 #include "esac_geom.cuh"
 
@@ -23,22 +23,12 @@ struct Pack1 {
 struct Mask1 {
     bool a;
 };
-struct Pack2 {
-    float2 v;
-    static constexpr int W = 2;
-};
-struct Mask2 {
-    bool a, b;
-};
 template <typename P> struct MaskOf;
 template <> struct MaskOf<Pack1> { typedef Mask1 type; };
-template <> struct MaskOf<Pack2> { typedef Mask2 type; };
 
 ESAC_HD Pack1 bc1(float x) { Pack1 r; r.a = x; return r; }
-ESAC_HD Pack2 bc2(float x) { Pack2 r; r.v = make_float2(x, x); return r; }
 template <typename P> ESAC_HD P bc(float x);
 template <> ESAC_HD Pack1 bc<Pack1>(float x) { return bc1(x); }
-template <> ESAC_HD Pack2 bc<Pack2>(float x) { return bc2(x); }
 
 // arithmetic
 ESAC_HD Pack1 operator+(Pack1 x, Pack1 y) { return bc1(x.a + y.a); }
@@ -46,23 +36,10 @@ ESAC_HD Pack1 operator-(Pack1 x, Pack1 y) { return bc1(x.a - y.a); }
 ESAC_HD Pack1 operator*(Pack1 x, Pack1 y) { return bc1(x.a * y.a); }
 ESAC_HD Pack1 operator-(Pack1 x) { return bc1(-x.a); }
 ESAC_HD Pack1 fma_(Pack1 x, Pack1 y, Pack1 z) { return bc1(fmaf(x.a, y.a, z.a)); }
-#ifdef __CUDA_ARCH__
-ESAC_HD Pack2 operator+(Pack2 x, Pack2 y) { Pack2 r; r.v = fadd2(x.v, y.v); return r; }
-ESAC_HD Pack2 operator*(Pack2 x, Pack2 y) { Pack2 r; r.v = fmul2(x.v, y.v); return r; }
-ESAC_HD Pack2 fma_(Pack2 x, Pack2 y, Pack2 z) { Pack2 r; r.v = ffma2(x.v, y.v, z.v); return r; }
-ESAC_HD Pack2 operator-(Pack2 x, Pack2 y) { Pack2 r; r.v = ffma2(make_float2(-1.f, -1.f), y.v, x.v); return r; }  // exact: x - y
-#else
-ESAC_HD Pack2 operator+(Pack2 x, Pack2 y) { Pack2 r; r.v = make_float2(x.v.x + y.v.x, x.v.y + y.v.y); return r; }
-ESAC_HD Pack2 operator*(Pack2 x, Pack2 y) { Pack2 r; r.v = make_float2(x.v.x * y.v.x, x.v.y * y.v.y); return r; }
-ESAC_HD Pack2 fma_(Pack2 x, Pack2 y, Pack2 z) { Pack2 r; r.v = make_float2(fmaf(x.v.x, y.v.x, z.v.x), fmaf(x.v.y, y.v.y, z.v.y)); return r; }
-ESAC_HD Pack2 operator-(Pack2 x, Pack2 y) { Pack2 r; r.v = make_float2(x.v.x - y.v.x, x.v.y - y.v.y); return r; }
-#endif
-ESAC_HD Pack2 operator-(Pack2 x) { Pack2 r; r.v = make_float2(-x.v.x, -x.v.y); return r; }
 
 // per-lane scalar functions
-#define ESAC_PACK_UNARY(name, expr)                                                     \
-    ESAC_HD Pack1 name(Pack1 p) { float x = p.a; return bc1(expr); }                    \
-    ESAC_HD Pack2 name(Pack2 p) { Pack2 r; float x = p.v.x; r.v.x = (expr); x = p.v.y; r.v.y = (expr); return r; }
+#define ESAC_PACK_UNARY(name, expr) \
+    ESAC_HD Pack1 name(Pack1 p) { float x = p.a; return bc1(expr); }
 ESAC_PACK_UNARY(abs_, fabsf(x))
 ESAC_PACK_UNARY(rcp_, Num<float>::div_(1.f, x))
 ESAC_PACK_UNARY(sqrt_, Num<float>::sqrt_(x))
@@ -71,13 +48,10 @@ ESAC_PACK_UNARY(cbrt_, cbrtf(x))
 #undef ESAC_PACK_UNARY
 ESAC_HD Pack1 max_(Pack1 x, Pack1 y) { return bc1(fmaxf(x.a, y.a)); }
 ESAC_HD Pack1 min_(Pack1 x, Pack1 y) { return bc1(fminf(x.a, y.a)); }
-ESAC_HD Pack2 max_(Pack2 x, Pack2 y) { Pack2 r; r.v = make_float2(fmaxf(x.v.x, y.v.x), fmaxf(x.v.y, y.v.y)); return r; }
-ESAC_HD Pack2 min_(Pack2 x, Pack2 y) { Pack2 r; r.v = make_float2(fminf(x.v.x, y.v.x), fminf(x.v.y, y.v.y)); return r; }
 
 // comparisons and masks
-#define ESAC_PACK_CMP(name, op)                                                       \
-    ESAC_HD Mask1 name(Pack1 x, Pack1 y) { Mask1 m; m.a = x.a op y.a; return m; }     \
-    ESAC_HD Mask2 name(Pack2 x, Pack2 y) { Mask2 m; m.a = x.v.x op y.v.x; m.b = x.v.y op y.v.y; return m; }
+#define ESAC_PACK_CMP(name, op) \
+    ESAC_HD Mask1 name(Pack1 x, Pack1 y) { Mask1 m; m.a = x.a op y.a; return m; }
 ESAC_PACK_CMP(lt_, <)
 ESAC_PACK_CMP(le_, <=)
 ESAC_PACK_CMP(gt_, >)
@@ -86,20 +60,12 @@ ESAC_PACK_CMP(ge_, >=)
 ESAC_HD Mask1 operator&(Mask1 x, Mask1 y) { Mask1 m; m.a = x.a && y.a; return m; }
 ESAC_HD Mask1 operator|(Mask1 x, Mask1 y) { Mask1 m; m.a = x.a || y.a; return m; }
 ESAC_HD Mask1 operator!(Mask1 x) { Mask1 m; m.a = !x.a; return m; }
-ESAC_HD Mask2 operator&(Mask2 x, Mask2 y) { Mask2 m; m.a = x.a && y.a; m.b = x.b && y.b; return m; }
-ESAC_HD Mask2 operator|(Mask2 x, Mask2 y) { Mask2 m; m.a = x.a || y.a; m.b = x.b || y.b; return m; }
-ESAC_HD Mask2 operator!(Mask2 x) { Mask2 m; m.a = !x.a; m.b = !x.b; return m; }
 ESAC_HD Mask1 mask1(bool v) { Mask1 m; m.a = v; return m; }
-ESAC_HD Mask2 mask2(bool v) { Mask2 m; m.a = v; m.b = v; return m; }
 template <typename M> ESAC_HD M splat(bool v);
 template <> ESAC_HD Mask1 splat<Mask1>(bool v) { return mask1(v); }
-template <> ESAC_HD Mask2 splat<Mask2>(bool v) { return mask2(v); }
 ESAC_HD bool all_(Mask1 m) { return m.a; }
-ESAC_HD bool all_(Mask2 m) { return m.a && m.b; }
 ESAC_HD Pack1 sel(Mask1 m, Pack1 x, Pack1 y) { return bc1(m.a ? x.a : y.a); }
-ESAC_HD Pack2 sel(Mask2 m, Pack2 x, Pack2 y) { Pack2 r; r.v = make_float2(m.a ? x.v.x : y.v.x, m.b ? x.v.y : y.v.y); return r; }
 ESAC_HD Mask1 nan_(Pack1 x) { return mask1(!(x.a == x.a)); }
-ESAC_HD Mask2 nan_(Pack2 x) { Mask2 m; m.a = !(x.v.x == x.v.x); m.b = !(x.v.y == x.v.y); return m; }
 
 // index of the largest of three magnitudes (ties: the first), as two masks: is0, is1 (else 2)
 template <typename P, typename M>
@@ -344,7 +310,7 @@ ESAC_HD typename MaskOf<P>::type p3p_may_pass_pack(const P obj[4][3], const P im
     return verdict;
 }
 
-// one try (tail kernel, host test hooks)
+// one try (prefilter_kernel, tail_kernel, host test hooks)
 ESAC_HD bool p3p_may_pass_fast(const float obj[4][3], const float img[4][2], float f, float ppx, float ppy, float tau,
                                float margin = kPrefilterMargin, float needle = kPrefilterNeedle) {
     Pack1 o[4][3], im[4][2];
@@ -355,22 +321,6 @@ ESAC_HD bool p3p_may_pass_fast(const float obj[4][3], const float img[4][2], flo
         im[i][0] = bc1(img[i][0]); im[i][1] = bc1(img[i][1]);
     }
     return p3p_may_pass_pack<Pack1>(o, im, f, ppx, ppy, tau, margin, needle).a;
-}
-
-// two tries side by side: verdicts in pass0 / pass1
-ESAC_HD void p3p_may_pass_fast2(const float obj0[4][3], const float img0[4][2], const float obj1[4][3], const float img1[4][2], float f,
-                                float ppx, float ppy, float tau, bool& pass0, bool& pass1, float margin = kPrefilterMargin,
-                                float needle = kPrefilterNeedle) {
-    Pack2 o[4][3], im[4][2];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-#pragma unroll
-        for (int c = 0; c < 3; ++c) o[i][c].v = make_float2(obj0[i][c], obj1[i][c]);
-        im[i][0].v = make_float2(img0[i][0], img1[i][0]);
-        im[i][1].v = make_float2(img0[i][1], img1[i][1]);
-    }
-    const Mask2 m = p3p_may_pass_pack<Pack2>(o, im, f, ppx, ppy, tau, margin, needle);
-    pass0 = m.a; pass1 = m.b;
 }
 
 }  // namespace esacb200

@@ -9,9 +9,9 @@
 //   wave r (try window [base_h, base_h + span_r) of every unresolved hypothesis; span_0 = 256, then chosen on the
 //   device from the acceptance rate seen so far, ~1.25 / p, so that ~70% of the remaining hypotheses resolve per
 //   wave and < 2x the necessary tries are evaluated):
-//     prefilter_kernel   two tries per thread (float2 pairs), fp32 only, branch-free: discards tries whose
+//     prefilter_kernel   one try per thread, fp32 only, branch-free: discards tries whose
 //                        every P3P root misses the 4th point by > 2 tau (>96% on wrong experts); the gathers of a
-//                        CTA's next 256-try item are in flight under the math of the current one; survivors are
+//                        CTA's next 128-try item are in flight under the math of the current one; survivors are
 //                        appended to a global list
 //     exact_kernel       one thread per survivor: the fp64 path (p3p_pose + minimal_set_gate) whose verdict is the
 //                        only one that counts (it leaves early when no P3P candidate can pass, and polishes only the
@@ -164,64 +164,56 @@ __global__ void sample_init_kernel(const __grid_constant__ SampleArgs a) {
     }
 }
 
-// ---- wave phase 1: fp32 prefilter, TWO tries per thread (float2 pairs) ---------------------------------------------
-constexpr int kPackTries = 2 * kTryThreads;  // tries per CTA pass: thread i judges tries i and i + 128 of the 256-try chunk
-// One work item of the prefilter: 256 consecutive tries of one hypothesis, two per thread.
+// ---- wave phase 1: fp32 prefilter, one try per thread ----------------------------------------------------------------
+constexpr int kSpanQuantum = 256;  // windows are multiples of this many tries
+// One work item of the prefilter: kTryThreads consecutive tries of one hypothesis, one per thread.
 struct PreItem {
-    int h, ta, tb;          // hypothesis, this thread's two tries
-    bool valid0, valid1;
-    unsigned cell[8];       // (y << 16) | x of the 2 x 4 cells
+    int h, t;               // hypothesis, this thread's try
+    bool valid;
+    unsigned cell[4];       // (y << 16) | x of the 4 cells
 };
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
 }
-// Decodes item -> (hypothesis, tries), draws the 2 x 4 cells and starts the 8 gathers of 16 bytes straight into shared
-// memory (cp.async: no registers are held while they are in flight).
+// Decodes item -> (hypothesis, try), draws the 4 cells and starts the 4 gathers of 16 bytes straight into shared memory
+// (cp.async: no registers are held while they are in flight).
 template <bool DEV>
 __device__ __forceinline__ void prefilter_issue(const SampleArgsT<DEV>& a, long long item, int cph, int span, float4 (*dst)[kTryThreads], PreItem& it) {
     const int u = (int)(item / cph), c = (int)(item - (long long)u * cph);
     it.h = a.st.list[u];
     const int t0 = a.st.base[it.h];
-    const int off0 = c * kPackTries + threadIdx.x, off1 = off0 + kTryThreads;
-    it.valid0 = off0 < span && t0 + off0 < a.limit;
-    it.valid1 = off1 < span && t0 + off1 < a.limit;
-    // an invalid half re-judges try t0 (in range for every listed hypothesis) and is masked out afterwards
-    it.ta = it.valid0 ? t0 + off0 : t0;
-    it.tb = it.valid1 ? t0 + off1 : t0;
-    if (!(it.valid0 || it.valid1)) return;
+    const int off = c * kTryThreads + threadIdx.x;
+    it.t = t0 + off;
+    it.valid = off < span && it.t < a.limit;
+    if (!it.valid) return;
     const Problem& P = a.P;
     const float4* pl = a.coords4 + (size_t)a.assign32[it.h] * P.N;
+    int cx[4], cy[4];
+    if (a.injected) {
+        const int* cc = a.injected + ((size_t)it.h * a.inj_T + it.t) * 8;
+        for (int j = 0; j < 4; ++j) { cx[j] = cc[2 * j]; cy[j] = cc[2 * j + 1]; }
+    } else {
+        draw_minimal_set(sample_seed<DEV>(a), (uint32_t)(it.h * a.hyp_stride + a.hyp_offset), (uint32_t)it.t, P.W, P.H, cx, cy);
+    }
 #pragma unroll
-    for (int k = 0; k < 2; ++k) {
-        const int t = k == 0 ? it.ta : it.tb;
-        int cx[4], cy[4];
-        if (a.injected) {
-            const int* cc = a.injected + ((size_t)it.h * a.inj_T + t) * 8;
-            for (int j = 0; j < 4; ++j) { cx[j] = cc[2 * j]; cy[j] = cc[2 * j + 1]; }
-        } else {
-            draw_minimal_set(sample_seed<DEV>(a), (uint32_t)(it.h * a.hyp_stride + a.hyp_offset), (uint32_t)t, P.W, P.H, cx, cy);
-        }
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            it.cell[k * 4 + j] = ((unsigned)cy[j] << 16) | (unsigned)cx[j];
-            cp_async16(&dst[k * 4 + j][threadIdx.x], pl + (cy[j] * P.W + cx[j]));
-        }
+    for (int j = 0; j < 4; ++j) {
+        it.cell[j] = ((unsigned)cy[j] << 16) | (unsigned)cx[j];
+        cp_async16(&dst[j][threadIdx.x], pl + (cy[j] * P.W + cx[j]));
     }
 }
 
-// ---- wave phase 1: fp32 prefilter, TWO tries per thread (float2 pairs), gathers one item ahead ----------------------
-// The math of an item (~2700 instructions per thread, branch-free) runs while the 8 random 16-byte gathers of the NEXT item
-// are in flight: with 16-20 warps per SM (the two-try pack needs ~128 registers) nothing else would cover their L2 latency.
-// The stage is bound by register capacity x dependency-chain latency: an SM holds 1024 tries in flight (64 registers per
-// try) whatever the packing, and a try's dependent instruction chain is the same.  96 registers
-// (5 CTAs per SM) spill.
+// ---- wave phase 1: fp32 prefilter, one try per thread, gathers one item ahead ----------------------------------------
+// The math of an item (~1350 instructions per thread, branch-free) runs while the 4 random 16-byte gathers of the NEXT item
+// are in flight.  The stage is bound by register capacity x dependency-chain latency.  On the H100, which has no packed
+// fp32x2 pipe, one try per thread beats two (a float2 pair per value, 128 registers, 4 CTAs per SM), and 6 CTAs of 80
+// registers beat 8 CTAs of 64: bench sampling stage 0.575 ms against 0.589 and 0.655 ms (DESIGN.md section 8).
 template <bool DEV>
-__global__ void __launch_bounds__(kTryThreads, 4) prefilter_kernel(const __grid_constant__ SampleArgsT<DEV> a) {
+__global__ void __launch_bounds__(kTryThreads, 6) prefilter_kernel(const __grid_constant__ SampleArgsT<DEV> a) {
     TraceScope trace(a.trace, a.trace_slot);
-    __shared__ float4 s_obj[2][8][kTryThreads];  // [buffer][try * 4 + point][thread]
+    __shared__ float4 s_obj[2][4][kTryThreads];  // [buffer][point][thread]
     const int n_unres = a.st.counters[0];
     const int span = a.st.counters[3];
-    const int cph = (span + kPackTries - 1) / kPackTries;  // chunks per hypothesis
+    const int cph = (span + kTryThreads - 1) / kTryThreads;  // chunks per hypothesis
     const long long n_items = (long long)n_unres * cph;
     const int lane = threadIdx.x & 31, tid = threadIdx.x;
     const Problem& P = a.P;
@@ -235,44 +227,29 @@ __global__ void __launch_bounds__(kTryThreads, 4) prefilter_kernel(const __grid_
         if (ni < n_items) prefilter_issue<DEV>(a, ni, cph, span, s_obj[buf ^ 1], nxt);
         asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group 1;" ::: "memory");  // everything but the group just committed has landed
-        bool pass0 = false, pass1 = false;
-        if (cur.valid0 || cur.valid1) {
-            float obj0[4][3], img0[4][2], obj1[4][3], img1[4][2];
+        bool pass = false;
+        if (cur.valid) {
+            float obj[4][3], img[4][2];
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-                const float4 v0 = s_obj[buf][j][tid], v1 = s_obj[buf][4 + j][tid];
-                obj0[j][0] = v0.x; obj0[j][1] = v0.y; obj0[j][2] = v0.z;
-                obj1[j][0] = v1.x; obj1[j][1] = v1.y; obj1[j][2] = v1.z;
-                const unsigned c0 = cur.cell[j], c1 = cur.cell[4 + j];
-                img0[j][0] = (float)((int)(c0 & 0xffffu) * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, a));
-                img0[j][1] = (float)((int)(c0 >> 16) * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, a));
-                img1[j][0] = (float)((int)(c1 & 0xffffu) * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, a));
-                img1[j][1] = (float)((int)(c1 >> 16) * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, a));
+                const float4 v = s_obj[buf][j][tid];
+                obj[j][0] = v.x; obj[j][1] = v.y; obj[j][2] = v.z;
+                const unsigned c = cur.cell[j];
+                img[j][0] = (float)((int)(c & 0xffffu) * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, a));
+                img[j][1] = (float)((int)(c >> 16) * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, a));
             }
-            if (a.use_prefilter)
-                p3p_may_pass_fast2(obj0, img0, obj1, img1, dev_f<DEV>(P, a), dev_ppx<DEV>(P, a), dev_ppy<DEV>(P, a), P.tau,
-                                   pass0, pass1);
-            else pass0 = pass1 = true;
-            pass0 = pass0 && cur.valid0;
-            pass1 = pass1 && cur.valid1;
+            pass = !a.use_prefilter || p3p_may_pass_fast(obj, img, dev_f<DEV>(P, a), dev_ppx<DEV>(P, a), dev_ppy<DEV>(P, a), P.tau);
         }
-        // warp-aggregated append of the survivors (both halves in one reservation)
-        const unsigned m0 = __ballot_sync(0xffffffffu, pass0), m1 = __ballot_sync(0xffffffffu, pass1);
-        if (m0 | m1) {
-            const int n0 = __popc(m0);
+        // warp-aggregated append of the survivors
+        const unsigned m = __ballot_sync(0xffffffffu, pass);
+        if (m) {
             int basei = 0;
-            if (lane == 0) basei = atomicAdd(&a.st.counters[1], n0 + __popc(m1));
+            if (lane == 0) basei = atomicAdd(&a.st.counters[1], __popc(m));
             basei = __shfl_sync(0xffffffffu, basei, 0);
-            const unsigned lt = (1u << lane) - 1u;
-            if (pass0) {
-                const int idx = basei + __popc(m0 & lt);
-                if (idx < a.st.cap) a.st.surv[idx] = make_int2(cur.h, cur.ta);
-                else atomicMin(&a.st.ovf[cur.h], cur.ta);  // list full: this hypothesis resumes from here in the next wave
-            }
-            if (pass1) {
-                const int idx = basei + n0 + __popc(m1 & lt);
-                if (idx < a.st.cap) a.st.surv[idx] = make_int2(cur.h, cur.tb);
-                else atomicMin(&a.st.ovf[cur.h], cur.tb);
+            if (pass) {
+                const int idx = basei + __popc(m & ((1u << lane) - 1u));
+                if (idx < a.st.cap) a.st.surv[idx] = make_int2(cur.h, cur.t);
+                else atomicMin(&a.st.ovf[cur.h], cur.t);  // list full: this hypothesis resumes from here in the next wave
             }
         }
         cur = nxt;
@@ -354,7 +331,7 @@ __device__ void advance_wave(const SampleState& st, int limit, float window, flo
         const double boost = nn <= 8 ? tail_boost * 2. : (nn <= 64 ? tail_boost : 1.);
         double next_span = (double)window * boost * tried / hits;
         next_span = next_span < 256. ? 256. : (next_span > 65536. ? 65536. : next_span);
-        st.counters[3] = ((int)next_span + kPackTries - 1) / kPackTries * kPackTries;
+        st.counters[3] = ((int)next_span + kSpanQuantum - 1) / kSpanQuantum * kSpanQuantum;
         st.counters[0] = nn;
         st.counters[1] = 0;
         st.counters[4] = 0;  // ticket of the next exact_kernel
@@ -485,9 +462,8 @@ int launch_sample(const float* coords, float4* coords4, const int* assign32, con
         }
         if (bound[g] <= 0) continue;
         sample_init_kernel<<<(bound[g] + 255) / 256, 256, 0, sg>>>(ae); ++launches;
-        // persistent: every CTA resident (4 x 128 threads x 128 registers fill an SM's register file), ~14 items each in a bulk wave;
-        // 3 CTAs per SM + 64-thread verdict CTAs in the room that leaves was measured slower
-        const int grid = sm_count * 4;
+        // persistent: every CTA resident (6 x 128 threads x 80 registers fill an SM's register file), ~19 items each in a bulk wave
+        const int grid = sm_count * 6;
         for (int r = 0; r < n_waves; ++r) {
             // the trace holds 32 waves per lane: later waves (sample_waves may be up to 64) are not stamped
             a.trace = r < kTraceWaves ? trace : nullptr;

@@ -11,6 +11,7 @@ visible, calls raise RuntimeError.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import math
 import os
@@ -421,6 +422,31 @@ def _cameras(B: int, shiftX, shiftY, focalLength, ppointX, ppointY, shift_names=
             _per_image(ppointY, B, np.float32, "ppointY"))
 
 
+def _thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling) -> tuple:
+    """tau, alpha, beta, maxReproj, subSampling as ctypes takes them (the tail of the `cam` / `cams` argtypes)."""
+    return float(inlierThreshold), float(inlierAlpha), float(inlierBeta), float(maxReproj), int(subSampling)
+
+
+def _camera_tail(shiftX, shiftY, focalLength, ppointX, ppointY, *thresholds) -> tuple:
+    """The scalar tail of a single-image call, shiftX .. subSampling, as ctypes takes it (the `cam` argtypes)."""
+    return (int(shiftX), int(shiftY), float(focalLength), float(ppointX), float(ppointY)) + _thresholds(*thresholds)
+
+
+@contextlib.contextmanager
+def _hypothesis_shard(ctx: Context, hyp_offset: int, hyp_stride: int | None = None):
+    """Options hyp_offset (and hyp_stride) on the context for one sharded call, back to 0 (1) when it returns or raises."""
+    options = {"hyp_offset": (hyp_offset, 0)}
+    if hyp_stride is not None:
+        options["hyp_stride"] = (hyp_stride, 1)
+    for key, (value, _) in options.items():
+        ctx.set_option(key, value)
+    try:
+        yield
+    finally:
+        for key, (_, default) in options.items():
+            ctx.set_option(key, default)
+
+
 def _is_list(t) -> bool:
     """A ragged batch: a list or tuple of per-image tensors / arrays (each with its own H x W)."""
     return isinstance(t, (list, tuple))
@@ -544,10 +570,9 @@ def forward(sceneCoordinates, hypAssignment, outPose, shiftX, shiftY, focalLengt
     ctx = _pick_ctx(co.device, op.device, adev)
     E, _, H, W = (int(s) for s in sceneCoordinates.shape)
     expert = C.c_int(-1)
-    ctx.check(ctx.lib.esacb200_forward(ctx.handle, co.ptr, E, H, W, aptr, astride, M, op.ptr, int(shiftX), int(shiftY),
-                                       float(focalLength), float(ppointX), float(ppointY), float(inlierThreshold),
-                                       float(inlierAlpha), float(inlierBeta), float(maxReproj), int(subSampling),
-                                       C.byref(expert)))
+    ctx.check(ctx.lib.esacb200_forward(ctx.handle, co.ptr, E, H, W, aptr, astride, M, op.ptr,
+                                       *_camera_tail(shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold, inlierAlpha,
+                                                     inlierBeta, maxReproj, subSampling), C.byref(expert)))
     op.finish()
     return int(expert.value)
 
@@ -572,9 +597,9 @@ def backward(sceneCoordinates, outGradients, hypAssignment, gtPose, wLossRot, wL
     E, _, H, W = (int(s) for s in sceneCoordinates.shape)
     loss = C.c_double(0.0)
     ctx.check(ctx.lib.esacb200_backward(ctx.handle, co.ptr, gr.ptr, E, H, W, aptr, astride, M, gt.ptr, float(wLossRot),
-                                        float(wLossTrans), float(lossCut), int(shiftX), int(shiftY), float(focalLength),
-                                        float(ppointX), float(ppointY), float(inlierThreshold), float(inlierAlpha),
-                                        float(inlierBeta), float(maxReproj), int(subSampling), C.byref(loss)))
+                                        float(wLossTrans), float(lossCut),
+                                        *_camera_tail(shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
+                                                      inlierAlpha, inlierBeta, maxReproj, subSampling), C.byref(loss)))
     gr.finish()
     return float(loss.value)
 
@@ -608,14 +633,12 @@ def backward_sharded(sceneCoordinates, outGradients, hypAssignment, gtPose, wLos
 
     cb = EXCHANGE_FN(_cb)
     loss = C.c_double(0.0)
-    ctx.set_option("hyp_offset", hyp_offset)
-    try:
+    with _hypothesis_shard(ctx, hyp_offset):
         rc = ctx.lib.esacb200_backward_sharded(ctx.handle, co.ptr, gr.ptr, E, H, W, aptr, astride, M, gt.ptr, float(wLossRot),
-                                               float(wLossTrans), float(lossCut), int(shiftX), int(shiftY), float(focalLength),
-                                               float(ppointX), float(ppointY), float(inlierThreshold), float(inlierAlpha),
-                                               float(inlierBeta), float(maxReproj), int(subSampling), cb, None, C.byref(loss))
-    finally:
-        ctx.set_option("hyp_offset", 0)
+                                               float(wLossTrans), float(lossCut),
+                                               *_camera_tail(shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
+                                                             inlierAlpha, inlierBeta, maxReproj, subSampling),
+                                               cb, None, C.byref(loss))
     if err:
         raise err[0]
     ctx.check(rc)
@@ -649,8 +672,9 @@ def forward_batch(sceneCoordinates, hypAssignment, outPoses, shiftX, shiftY, foc
     ctx = _pick_ctx(*co.devices, op.device, ha.device)
     experts = (C.c_int * B)()
     ctx.check(ctx.lib.esacb200_forward_ragged(ctx.handle, B, co.ptrs, co.hs, co.ws, E, ha.ptr, 1, M, op.ptr,
-                                              *(a.ctypes.data for a in cams), float(inlierThreshold), float(inlierAlpha),
-                                              float(inlierBeta), float(maxReproj), int(subSampling), experts))
+                                              *(a.ctypes.data for a in cams),
+                                              *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling),
+                                              experts))
     op.finish()
     return [int(e) for e in experts]
 
@@ -680,8 +704,9 @@ def backward_batch(sceneCoordinates, outGradients, hypAssignment, gtPoses, wLoss
     losses = np.zeros(B, np.float64)
     ctx.check(ctx.lib.esacb200_backward_ragged(ctx.handle, B, co.ptrs, og.ptrs, co.hs, co.ws, E, ha.ptr, 1, M, gt.ptr,
                                                float(wLossRot), float(wLossTrans), float(lossCut),
-                                               *(a.ctypes.data for a in cams), float(inlierThreshold), float(inlierAlpha),
-                                               float(inlierBeta), float(maxReproj), int(subSampling), losses.ctypes.data))
+                                               *(a.ctypes.data for a in cams),
+                                               *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling),
+                                               losses.ctypes.data))
     og.finish()
     return [float(v) for v in losses]
 
@@ -801,10 +826,8 @@ def forward_pack(sceneCoordinates, hypAssignment, params, expert_offset: int, pa
         raise RuntimeError(f"pack_out must be a contiguous float64 tensor of M_pad + {PACK_TAIL} elements")
     ctx = _pick_ctx(co.device, adev, pack_out.device.index)
     E, _, H, W = (int(v) for v in sceneCoordinates.shape)
-    shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub = params
-    ctx.check(ctx.lib.esacb200_forward_pack(ctx.handle, co.ptr, E, H, W, aptr, astride, M, M_pad, int(shiftX), int(shiftY), float(f),
-                                            float(ppx), float(ppy), float(tau), float(alpha), float(beta), float(maxReproj),
-                                            int(sub), int(expert_offset), pack_out.data_ptr()))
+    ctx.check(ctx.lib.esacb200_forward_pack(ctx.handle, co.ptr, E, H, W, aptr, astride, M, M_pad, *_camera_tail(*params),
+                                            int(expert_offset), pack_out.data_ptr()))
 
 
 def forward_sharded(sceneCoordinates, hypAssignment, outPose, shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
@@ -824,16 +847,11 @@ def forward_sharded(sceneCoordinates, hypAssignment, outPose, shiftX, shiftY, fo
     ctx = _pick_ctx(*devs) if devs else _pick_ctx_host(device)
     E, _, H, W = (int(s) for s in sceneCoordinates.shape)
     expert = C.c_int(-1)
-    ctx.set_option("hyp_offset", hyp_offset)
-    ctx.set_option("hyp_stride", hyp_stride)
-    try:
-        rc = ctx.lib.esacb200_forward_sharded(ctx.handle, co.ptr, E, H, W, aptr, astride, M, M_pad, op.ptr, int(shiftX), int(shiftY),
-                                              float(focalLength), float(ppointX), float(ppointY), float(inlierThreshold),
-                                              float(inlierAlpha), float(inlierBeta), float(maxReproj), int(subSampling),
+    with _hypothesis_shard(ctx, hyp_offset, hyp_stride):
+        rc = ctx.lib.esacb200_forward_sharded(ctx.handle, co.ptr, E, H, W, aptr, astride, M, M_pad, op.ptr,
+                                              *_camera_tail(shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
+                                                            inlierAlpha, inlierBeta, maxReproj, subSampling),
                                               int(expert_offset), C.byref(expert))
-    finally:
-        ctx.set_option("hyp_offset", 0)
-        ctx.set_option("hyp_stride", 1)
     ctx.check(rc)
     op.finish()
     return int(expert.value)
@@ -857,17 +875,12 @@ def backward_sharded_nccl(sceneCoordinates, outGradients, hypAssignment, gtPose,
     ctx = _pick_ctx(*devs) if devs else _pick_ctx_host(device)
     E, _, H, W = (int(s) for s in sceneCoordinates.shape)
     loss = C.c_double(0.0)
-    ctx.set_option("hyp_offset", hyp_offset)
-    ctx.set_option("hyp_stride", hyp_stride)
-    try:
+    with _hypothesis_shard(ctx, hyp_offset, hyp_stride):
         rc = ctx.lib.esacb200_backward_sharded_nccl(ctx.handle, co.ptr, gr.ptr, E, H, W, aptr, astride, M, gt.ptr, float(wLossRot),
-                                                    float(wLossTrans), float(lossCut), int(shiftX), int(shiftY), float(focalLength),
-                                                    float(ppointX), float(ppointY), float(inlierThreshold), float(inlierAlpha),
-                                                    float(inlierBeta), float(maxReproj), int(subSampling), int(bool(reduce_grads)),
-                                                    C.byref(loss))
-    finally:
-        ctx.set_option("hyp_offset", 0)
-        ctx.set_option("hyp_stride", 1)
+                                                    float(wLossTrans), float(lossCut),
+                                                    *_camera_tail(shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
+                                                                  inlierAlpha, inlierBeta, maxReproj, subSampling),
+                                                    int(bool(reduce_grads)), C.byref(loss))
     ctx.check(rc)
     gr.finish()
     return float(loss.value)
@@ -885,10 +898,9 @@ def score_poses(sceneCoordinates, hypAssignment, poses6, shiftX, shiftY, focalLe
     ctx = _pick_ctx(co.device, adev)
     E, _, H, W = (int(s) for s in sceneCoordinates.shape)
     out = np.zeros(M)
-    ctx.check(ctx.lib.esacb200_score_poses(ctx.handle, co.ptr, E, H, W, aptr, astride, M, poses6.ctypes.data, int(shiftX),
-                                           int(shiftY), float(focalLength), float(ppointX), float(ppointY),
-                                           float(inlierThreshold), float(inlierAlpha), float(inlierBeta), float(maxReproj),
-                                           int(subSampling), out.ctypes.data))
+    ctx.check(ctx.lib.esacb200_score_poses(ctx.handle, co.ptr, E, H, W, aptr, astride, M, poses6.ctypes.data,
+                                           *_camera_tail(shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
+                                                         inlierAlpha, inlierBeta, maxReproj, subSampling), out.ctypes.data))
     return out
 
 
@@ -952,9 +964,9 @@ def hypotheses_forward(sceneCoordinates, hypAssignment, shiftX, shiftY, focalLen
     scores = torch.empty(M, dtype=torch.float64, device=dev)
     poses = torch.empty(M, 6, dtype=torch.float64, device=dev)
     contributing = torch.empty(M, dtype=torch.bool, device=dev)
-    ctx.check(ctx.lib.esacb200_hypotheses_forward(ctx.handle, co.ptr, E, H, W, aptr, astride, M, int(shiftX), int(shiftY),
-                                                  float(focalLength), float(ppointX), float(ppointY), float(inlierThreshold),
-                                                  float(inlierAlpha), float(inlierBeta), float(maxReproj), int(subSampling),
+    ctx.check(ctx.lib.esacb200_hypotheses_forward(ctx.handle, co.ptr, E, H, W, aptr, astride, M,
+                                                  *_camera_tail(shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
+                                                                inlierAlpha, inlierBeta, maxReproj, subSampling),
                                                   tape.data_ptr(), nbytes, scores.data_ptr(), poses.data_ptr(),
                                                   contributing.data_ptr()))
     return scores, poses, contributing, tape
@@ -1040,7 +1052,7 @@ def hypotheses_forward_batch(sceneCoordinates, hypAssignment, shiftX, shiftY, fo
     tape_sizes = (C.c_size_t * B)(*sizes)
     ctx.check(ctx.lib.esacb200_hypotheses_forward_ragged(
         ctx.handle, B, maps.ptrs, maps.hs, maps.ws, E, ha.ptr, 1, M, *(a.ctypes.data for a in cams),
-        float(inlierThreshold), float(inlierAlpha), float(inlierBeta), float(maxReproj), int(subSampling), tape_ptrs, tape_sizes,
+        *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling), tape_ptrs, tape_sizes,
         scores.data_ptr(), poses.data_ptr(), contributing.data_ptr()))
     return scores, poses, contributing, tapes
 
@@ -1181,8 +1193,8 @@ def forward_async(sceneCoordinates, hypAssignment, shifts, cameras, inlierThresh
                           "outStatus": (outStatus, "Int", ())})
     ctx.check(ctx.lib.esacb200_forward_async(ctx.handle, B, sceneCoordinates.data_ptr(), E, H, W, hypAssignment.data_ptr(),
                                              int(hypAssignment.stride(-1)), M, shifts.data_ptr(), cameras.data_ptr(),
-                                             float(inlierThreshold), float(inlierAlpha), float(inlierBeta), float(maxReproj),
-                                             int(subSampling), outPoses.data_ptr(), outExperts.data_ptr(), outStatus.data_ptr()))
+                                             *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling),
+                                             outPoses.data_ptr(), outExperts.data_ptr(), outStatus.data_ptr()))
 
 
 def reserve_forward_async(B: int, E: int, H: int, W: int, M: int, subSampling: int = 8, device: int | None = None):
@@ -1217,9 +1229,9 @@ def backward_async(sceneCoordinates, outGradients, hypAssignment, gtPoses, shift
     ctx.check(ctx.lib.esacb200_backward_async(ctx.handle, B, sceneCoordinates.data_ptr(), outGradients.data_ptr(), E, H, W,
                                               hypAssignment.data_ptr(), int(hypAssignment.stride(-1)), M, gtPoses.data_ptr(),
                                               float(wLossRot), float(wLossTrans), float(lossCut), shifts.data_ptr(),
-                                              cameras.data_ptr(), float(inlierThreshold), float(inlierAlpha),
-                                              float(inlierBeta), float(maxReproj), int(subSampling), outLosses.data_ptr(),
-                                              outStatus.data_ptr()))
+                                              cameras.data_ptr(),
+                                              *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling),
+                                              outLosses.data_ptr(), outStatus.data_ptr()))
 
 
 def reserve_backward_async(B: int, E: int, H: int, W: int, M: int, subSampling: int = 8, device: int | None = None):

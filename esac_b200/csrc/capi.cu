@@ -248,7 +248,7 @@ enum { S_NCHUNKS = 0, S_WORK, S_FLAGS, S_WINNER, S_NCONTRIB, S_COUNT = 16 };
 struct Plan {
     Problem P;
     int T, ppt, hc, grid, vec_ok;
-    const float* d_coords;
+    const float* d_coords = nullptr;
     const long long* d_assign;
     long long assign_stride;
     int split_e = 0;  // > 0: host maps are uploaded in two halves [0, split_e) / [split_e, E) on the copy stream (ev_copied[0/1])
@@ -281,6 +281,19 @@ int fill_problem(esacb200_ctx* ctx, Problem& P, int E, int H, int W, int M, int 
     P.E = E; P.H = H; P.W = W; P.N = H * W; P.M = M;
     P.shiftX = shiftX; P.shiftY = shiftY; P.sub = sub;
     P.f = f; P.ppx = ppx; P.ppy = ppy; P.tau = tau; P.alpha = alpha; P.beta = beta; P.max_reproj = maxReproj;
+    return 0;
+}
+
+// The problems of a ragged batch: image b is H[b] x W[b] with entry b of the shift and camera arrays (a null array: 0),
+// checked image by image under an "image b:" prefix before any image runs.
+int fill_problems(esacb200_ctx* ctx, std::vector<Plan>& plans, int B, int E, const int* H, const int* W, int M, const int* shiftX,
+                  const int* shiftY, const float* f, const float* ppx, const float* ppy, float tau, float alpha, float beta,
+                  float maxReproj, int sub, Draw draw) {
+    plans.resize((size_t)B);
+    for (int b = 0; b < B; ++b)
+        if (fill_problem(ctx, plans[b].P, E, H[b], W[b], M, shiftX ? shiftX[b] : 0, shiftY ? shiftY[b] : 0, f ? f[b] : 0.f,
+                         ppx ? ppx[b] : 0.f, ppy ? ppy[b] : 0.f, tau, alpha, beta, maxReproj, sub, draw))
+            return fail(ctx, ESACB200_ERR_ARG, "image %d: %s", b, std::string(ctx->err).c_str());
     return 0;
 }
 
@@ -742,6 +755,22 @@ int pointer_kind(esacb200_ctx* ctx, const void* const* p, int B, const char* wha
     return 0;
 }
 
+// The B image pointers of a stacked [B, ...] tensor whose images lie `stride` elements apart (a null base: B nulls).
+template <class T>
+std::vector<T*> slices(T* base, int B, size_t stride) {
+    std::vector<T*> p((size_t)B, nullptr);
+    for (int b = 0; base && b < B; ++b) p[b] = base + (size_t)b * stride;
+    return p;
+}
+
+// The tape of a hypotheses forward of problem P: at least tape_bytes large, 16-byte aligned device memory.
+int check_tape(esacb200_ctx* ctx, const void* tape, size_t bytes, const Problem& P) {
+    const size_t need = tape_bytes(P.M, P.N);
+    if (bytes < need) return fail(ctx, ESACB200_ERR_ARG, "tape holds %zu bytes, this call needs %zu", bytes, need);
+    if (!is_device_ptr(tape) || ((uintptr_t)tape & 15)) return fail(ctx, ESACB200_ERR_ARG, "tape must be 16-byte aligned device memory");
+    return 0;
+}
+
 // Offsets of B host images packed into one device buffer, each at a 16-byte aligned offset (so that an image keeps the
 // 128-bit load path a single-image call would give it).  Returns the total.
 size_t pack_offsets(const std::vector<size_t>& bytes, std::vector<size_t>& off) {
@@ -1044,18 +1073,21 @@ int esacb200_forward(esacb200_ctx* ctx, const float* coords, int E, int H, int W
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
-// local half of a sharded forward: pipeline + record, no synchronisation (shared by forward_pack and forward_sharded)
-static int enqueue_forward_record(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
-                                  int64_t assign_stride, int M, int M_pad, int shiftX, int shiftY, float f, float ppx, float ppy,
-                                  float tau, float alpha, float beta, float maxReproj, int sub, int expert_offset, double* pack_out) {
+// Local half of a sharded forward: pipeline + record, no synchronisation (shared by forward_pack and forward_sharded).  The
+// call begins (begin_record) before the shard's problem is filled, so bad sizes still clear the stats and the last-call
+// record; M = 0 is a shard without hypotheses, whose problem is neither filled nor read.
+static int begin_record(esacb200_ctx* ctx, int M, int M_pad) {
     if (M_pad < M || M_pad < 1) return fail(ctx, ESACB200_ERR_ARG, "M_pad (%d) must be >= M (%d) and >= 1", M_pad, M);
     begin_call(ctx);
     ctx->inj_M = ctx->inj_T = 0;
-    Plan pl;
+    return 0;
+}
+
+static int enqueue_forward_record(esacb200_ctx* ctx, const Problem& P, const float* coords, const int64_t* assign,
+                                  int64_t assign_stride, int M, int M_pad, int expert_offset, double* pack_out) {
+    Plan pl{P};
     if (M > 0) {
-        int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS);
-        if (rc) return rc;
-        rc = stage_inputs(ctx, pl, coords, assign, assign_stride);
+        int rc = stage_inputs(ctx, pl, coords, assign, assign_stride);
         if (rc) return rc;
         rc = enqueue_forward_core(ctx, pl, ctx->out17.as<float>());
         if (rc) return rc;
@@ -1080,8 +1112,10 @@ int esacb200_forward_pack(esacb200_ctx* ctx, const float* coords, int E, int H, 
     if (!pack_out || (M > 0 && (!coords || !assign))) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
     if ((M > 0 && (!is_device_ptr(coords) || !is_device_ptr(assign))) || !is_device_ptr(pack_out))
         return fail(ctx, ESACB200_ERR_ARG, "forward_pack takes device pointers only");
-    int rc = enqueue_forward_record(ctx, coords, E, H, W, assign, assign_stride, M, M_pad, shiftX, shiftY, f, ppx, ppy, tau, alpha,
-                                    beta, maxReproj, sub, expert_offset, pack_out);
+    Problem P = {};
+    int rc = begin_record(ctx, M, M_pad);
+    if (!rc && M > 0) rc = fill_problem(ctx, P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS);
+    if (!rc) rc = enqueue_forward_record(ctx, P, coords, assign, assign_stride, M, M_pad, expert_offset, pack_out);
     if (rc) return rc;
     mark(ctx, EV_END);
     return ESACB200_OK;   // stage timers of this call are not collected: that would need the synchronisation
@@ -1142,8 +1176,10 @@ int esacb200_forward_sharded(esacb200_ctx* ctx, const float* coords, int E, int 
     const size_t rec = (size_t)M_pad + kPackTail;
     CK(ctx->gathered.ensure((world + 1) * rec * 8));
     double* mine = ctx->gathered.as<double>() + (size_t)world * rec;
-    int rc = enqueue_forward_record(ctx, coords, E, H, W, assign, assign_stride, M, M_pad, shiftX, shiftY, f, ppx, ppy, tau, alpha,
-                                    beta, maxReproj, sub, expert_offset, mine);
+    Problem P = {};
+    int rc = begin_record(ctx, M, M_pad);
+    if (!rc && M > 0) rc = fill_problem(ctx, P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS);
+    if (!rc) rc = enqueue_forward_record(ctx, P, coords, assign, assign_stride, M, M_pad, expert_offset, mine);
     if (rc) return rc;
     CKN(nccl_api().AllGather(mine, ctx->gathered.p, rec, kNcclFloat64, ctx->nccl_comm, ctx->stream));
     launch_select_gathered(ctx->gathered.as<double>(), world, M_pad, ctx->out17.as<float>(), ctx->stream);
@@ -1177,16 +1213,11 @@ int esacb200_forward_ragged(esacb200_ctx* ctx, int B, const float* const* coords
     DeviceGuard device_guard(ctx->device);
     if (!coords || !H || !W || !assign || !out_poses || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
-    std::vector<Plan> plans((size_t)B);
-    for (int b = 0; b < B; ++b) {
-        Plan& pl = plans[b];
-        int rc = fill_problem(ctx, pl.P, E, H[b], W[b], M, shiftX ? shiftX[b] : 0, shiftY ? shiftY[b] : 0, f[b], ppx[b], ppy[b], tau,
-                              alpha, beta, maxReproj, sub, DRAWS);
-        if (rc) return fail(ctx, rc, "image %d: %s", b, std::string(ctx->err).c_str());
-        pl.d_coords = nullptr;
-    }
+    std::vector<Plan> plans;
+    int rc = fill_problems(ctx, plans, B, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS);
+    if (rc) return rc;
     bool dev_coords = false;
-    int rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_coords);
+    rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_coords);
     if (rc) return rc;
     const bool host_coords = !dev_coords;
     begin_call(ctx);
@@ -1246,9 +1277,7 @@ int esacb200_forward_batch_cameras(esacb200_ctx* ctx, int B, const float* coords
     if (!ctx) return ESACB200_ERR_ARG;
     if (!coords || !assign || !out_poses || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
-    const size_t cstride = (size_t)E * 3 * H * W;  // (sizes are checked image by image by the ragged call)
-    std::vector<const float*> ptrs((size_t)B);
-    for (int b = 0; b < B; ++b) ptrs[b] = coords + (size_t)b * cstride;
+    const auto ptrs = slices(coords, B, (size_t)E * 3 * H * W);  // (sizes are checked image by image by the ragged call)
     const std::vector<int> hs((size_t)B, H), ws((size_t)B, W);
     return esacb200_forward_ragged(ctx, B, ptrs.data(), hs.data(), ws.data(), E, assign, assign_stride, M, out_poses, shiftX, shiftY,
                                    f, ppx, ppy, tau, alpha, beta, maxReproj, sub, out_experts);
@@ -1357,30 +1386,25 @@ struct AsyncCall {
     std::vector<AsyncImage> imgs;
 };
 
-// What forward_async and backward_async (`backward`) share: checks the arguments (the n arrays `ptrs`, called `names`, must
-// be device memory), takes the async context, lays out the images and fits the workspace to them.
-static int begin_async(esacb200_ctx* ctx, bool backward, int B, const float* coords, int E, int H, int W, const int64_t* assign,
-                       int64_t assign_stride, int M, const int32_t* shifts, const float* cameras, float tau, float alpha,
-                       float beta, float maxReproj, int sub, int32_t* out_status, int n, const void* const* ptrs,
-                       const char* const* names, AsyncCall& call) {
+// What forward_async and backward_async (`backward`) share for B images of problem P: checks the arguments (the n arrays
+// `ptrs`, called `names`, must be device memory), takes the async context, lays out the images and fits the workspace.
+static int begin_async(esacb200_ctx* ctx, bool backward, int B, const Problem& P, const float* coords, const int64_t* assign,
+                       int64_t assign_stride, const int32_t* shifts, const float* cameras, int32_t* out_status, int n,
+                       const void* const* ptrs, const char* const* names, AsyncCall& call) {
     const char* what = backward ? "backward_async" : "forward_async";
-    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "%s: empty batch (B=%d)", what, B);
-    Problem P;
-    int rc = fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, tau, alpha, beta, maxReproj, sub, DRAWS);
-    if (rc) return rc;
     for (int i = 0; i < n; ++i) {
         if (!ptrs[i]) return fail(ctx, ESACB200_ERR_ARG, "%s: %s is null", what, names[i]);
         if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "%s takes device pointers only: %s is host memory", what, names[i]);
     }
     bool capturing = false;
-    rc = stream_capturing(ctx, capturing);
+    int rc = stream_capturing(ctx, capturing);
     if (rc) return rc;
     rc = async_context(ctx, capturing, what, &call.a);
     if (rc) return rc;
     esacb200_ctx* a = call.a;
     // element stride between the assignments of consecutive images: rows of a [B, M] tensor
-    const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
-    const size_t cstride = (size_t)E * 3 * H * W;
+    const int64_t arow = assign_stride == 0 ? 0 : (int64_t)P.M * assign_stride;
+    const size_t cstride = (size_t)P.E * 3 * P.N;
     call.plans.resize((size_t)B);
     call.imgs.resize((size_t)B);
     for (int b = 0; b < B; ++b) {
@@ -1417,8 +1441,10 @@ int esacb200_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E,
     const void* ptrs[] = {coords, assign, shifts, cameras, out_poses, out_experts, out_status};
     const char* names[] = {"coords", "assign", "shifts", "cameras", "out_poses", "out_experts", "out_status"};
     AsyncCall call;
-    int rc = begin_async(ctx, false, B, coords, E, H, W, assign, assign_stride, M, shifts, cameras, tau, alpha, beta, maxReproj,
-                         sub, out_status, 7, ptrs, names, call);
+    Problem P;
+    int rc = B <= 0 ? fail(ctx, ESACB200_ERR_ARG, "forward_async: empty batch (B=%d)", B)
+                    : fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, tau, alpha, beta, maxReproj, sub, DRAWS);
+    if (!rc) rc = begin_async(ctx, false, B, P, coords, assign, assign_stride, shifts, cameras, out_status, 7, ptrs, names, call);
     if (rc) return rc;
     for (int b = 0; b < B; ++b) {
         call.imgs[b].pose = out_poses + 16 * (size_t)b;
@@ -1650,37 +1676,26 @@ static BwdArgs backward_args(esacb200_ctx* ctx, const Plan& pl, float* grads) {
 }
 
 // -------------------------------------------------------------------------------------------------
-static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, int E, int H, int W, const int64_t* assign,
-                         int64_t assign_stride, int M, const float* gt_pose, float wRot, float wTrans, float cut, int shiftX,
-                         int shiftY, float f, float ppx, float ppy, float tau, float alpha, float beta, float maxReproj, int sub,
-                         esacb200_exchange_fn exchange, void* user, double* out_loss, bool use_nccl = false,
-                         bool reduce_grads = false) {
-    if (!ctx) return ESACB200_ERR_ARG;
-    DeviceGuard device_guard(ctx->device);
-    if (!coords || !assign || !grads || !gt_pose) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
-    Plan pl;
-    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS_INJECTED);
-    if (rc) return rc;
+// esac.backward on one image of problem P (filled and checked by the caller); `sh`: the steps of a sharded call, whose
+// work and destination buffers this fills in.
+static int backward_impl(esacb200_ctx* ctx, const Problem& P, const float* coords, const int64_t* assign, int64_t assign_stride,
+                         float* grads, const float* gt_pose, float wRot, float wTrans, float cut, ShardSteps sh, double* out_loss) {
+    Plan pl{P};
+    const int M = P.M, E = P.E;
     begin_call(ctx);
-    const Problem& P = pl.P;
     const size_t cbytes = (size_t)P.E * 3 * P.N * sizeof(float);
     float* d_grads = nullptr;
-    rc = stage_grads(ctx, grads, cbytes, d_grads);
+    int rc = stage_grads(ctx, grads, cbytes, d_grads);
     if (rc) return rc;
     // hypothesis-major sharding: every rank holds all planes and a slice of the hypotheses, so the gradient slices overlap:
     // the local gradient goes to a zeroed work buffer, is summed over the ranks and only then added to the caller's tensor
     float* d_dst = d_grads;
-    if (reduce_grads) {
+    if (sh.reduce_grads) {
         CK(ctx->grads_work.ensure(cbytes));
         d_grads = ctx->grads_work.as<float>();  // (the slices that will be used are zeroed once they are known, below)
         rc = ensure_host_flags(ctx, E);
         if (rc) return rc;
     }
-    ShardSteps sh;
-    sh.exchange = exchange;
-    sh.user = user;
-    sh.use_nccl = use_nccl;
-    sh.reduce_grads = reduce_grads;
     sh.d_work = d_grads;
     sh.d_dst = d_dst;
     rc = run_hypotheses(ctx, pl, coords, assign, assign_stride, sh, nullptr);
@@ -1697,19 +1712,19 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
     }
     b.wRot = wRot; b.wTrans = wTrans; b.cut = cut;
     double global_loss = 0;
-    if (exchange) {
+    if (sh.exchange) {
         // exchange 2: the expectation sum_h p_h loss_h runs over the hypotheses of all ranks (esac.cpp:357-362, esac_derivative.h:372-374)
         launch_backward_losses(b, ctx->stream);
         CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.as<double>() + 4, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
         double v[1] = {ctx->h_dbl[0]};
-        if (exchange(user, 2, v, 1) != 0) return fail(ctx, ESACB200_ERR_ARG, "exchange callback failed (phase 2)");
+        if (sh.exchange(sh.user, 2, v, 1) != 0) return fail(ctx, ESACB200_ERR_ARG, "exchange callback failed (phase 2)");
         global_loss = v[0];
         ctx->h_dbl[6] = v[0];
         CK(cudaMemcpyAsync(ctx->stats.as<double>() + 7, ctx->h_dbl + 6, sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
         b.expected_override = ctx->stats.as<double>() + 7;
         ctx->st.kernel_launches += 1;
-    } else if (use_nccl) {
+    } else if (sh.use_nccl) {
         // exchange 2 on the device: all-reduce of the partial expectations, no host round trip
         launch_backward_losses(b, ctx->stream);
         CKN(nccl_api().AllReduce(ctx->stats.as<double>() + 4, ctx->stats.as<double>() + 7, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm,
@@ -1720,7 +1735,7 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
     launch_backward(b, M, ctx->sm_count, ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 5;
-    if (reduce_grads) {
+    if (sh.reduce_grads) {
         rc = for_flagged_planes(ctx, E, (size_t)3 * P.N, d_grads, d_dst, 1);
         if (rc) return rc;
         CK(cudaGetLastError());
@@ -1730,8 +1745,8 @@ static int backward_impl(esacb200_ctx* ctx, const float* coords, float* grads, i
     if (d_grads != grads) CK(cudaMemcpyAsync(grads, d_grads, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
     rc = finish_call(ctx, pl, 8, true, /*losses=*/true);
     if (rc) return rc;
-    if (use_nccl) global_loss = ctx->h_dbl[7];
-    ctx->st.expected_loss = (exchange || use_nccl) ? global_loss : ctx->h_dbl[4];
+    if (sh.use_nccl) global_loss = ctx->h_dbl[7];
+    ctx->st.expected_loss = (sh.exchange || sh.use_nccl) ? global_loss : ctx->h_dbl[4];
     if (out_loss) *out_loss = ctx->st.expected_loss;
     return ESACB200_OK;
 }
@@ -1740,8 +1755,12 @@ int esacb200_backward(esacb200_ctx* ctx, const float* coords, float* grads, int 
                       int64_t assign_stride, int M, const float* gt_pose, float wRot, float wTrans, float cut, int shiftX,
                       int shiftY, float f, float ppx, float ppy, float tau, float alpha, float beta, float maxReproj, int sub,
                       double* out_loss) try {
-    return backward_impl(ctx, coords, grads, E, H, W, assign, assign_stride, M, gt_pose, wRot, wTrans, cut, shiftX, shiftY, f, ppx,
-                         ppy, tau, alpha, beta, maxReproj, sub, nullptr, nullptr, out_loss);
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (!coords || !assign || !grads || !gt_pose) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    Problem P;
+    int rc = fill_problem(ctx, P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS_INJECTED);
+    return rc ? rc : backward_impl(ctx, P, coords, assign, assign_stride, grads, gt_pose, wRot, wTrans, cut, ShardSteps(), out_loss);
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
@@ -1761,8 +1780,10 @@ int esacb200_backward_async(esacb200_ctx* ctx, int B, const float* coords, float
     const void* ptrs[] = {coords, grads, assign, gt_poses, shifts, cameras, out_losses, out_status};
     const char* names[] = {"coords", "grads", "assign", "gt_poses", "shifts", "cameras", "out_losses", "out_status"};
     AsyncCall call;
-    int rc = begin_async(ctx, true, B, coords, E, H, W, assign, assign_stride, M, shifts, cameras, tau, alpha, beta, maxReproj,
-                         sub, out_status, 8, ptrs, names, call);
+    Problem P;
+    int rc = B <= 0 ? fail(ctx, ESACB200_ERR_ARG, "backward_async: empty batch (B=%d)", B)
+                    : fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, tau, alpha, beta, maxReproj, sub, DRAWS);
+    if (!rc) rc = begin_async(ctx, true, B, P, coords, assign, assign_stride, shifts, cameras, out_status, 8, ptrs, names, call);
     if (rc) return rc;
     esacb200_ctx* a = call.a;
     const size_t cstride = (size_t)E * 3 * H * W;
@@ -1797,23 +1818,14 @@ size_t esacb200_hypotheses_tape_bytes(int E, int H, int W, int M) {
     return tape_bytes(M, H * W);
 }
 
-static int hypotheses_forward_impl(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
-                                   int64_t assign_stride, int M, int shiftX, int shiftY, float f, float ppx, float ppy, float tau,
-                                   float alpha, float beta, float maxReproj, int sub, void* tape, size_t tape_bytes_,
-                                   double* out_scores, double* out_poses6, uint8_t* out_contrib) {
-    if (!ctx) return ESACB200_ERR_ARG;
-    DeviceGuard device_guard(ctx->device);
-    if (!coords || !assign || !tape || !out_scores || !out_poses6 || !out_contrib) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
-    Plan pl;
-    int rc = fill_problem(ctx, pl.P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS_INJECTED);
-    if (rc) return rc;
-    const size_t need = tape_bytes(M, pl.P.N);
-    if (tape_bytes_ < need) return fail(ctx, ESACB200_ERR_ARG, "tape holds %zu bytes, this call needs %zu", tape_bytes_, need);
-    if (!is_device_ptr(tape) || ((uintptr_t)tape & 15)) return fail(ctx, ESACB200_ERR_ARG, "tape must be 16-byte aligned device memory");
+// The hypotheses forward of problem P (filled and checked by the caller, with the tape: check_tape).
+static int hypotheses_forward_impl(esacb200_ctx* ctx, const Problem& P, const float* coords, const int64_t* assign,
+                                   int64_t assign_stride, void* tape, double* out_scores, double* out_poses6, uint8_t* out_contrib) {
+    Plan pl{P};
+    const int M = P.M;
     begin_call(ctx);
-    rc = run_hypotheses(ctx, pl, coords, assign, assign_stride, ShardSteps(), (uint32_t*)((char*)tape + tape_masks_offset(M)));
+    int rc = run_hypotheses(ctx, pl, coords, assign, assign_stride, ShardSteps(), (uint32_t*)((char*)tape + tape_masks_offset(M)));
     if (rc) return rc;
-    const Problem& P = pl.P;
     int* sc = ctx->scalars.as<int>();
     CK(ctx->contrib8.ensure((size_t)M));
     BwdArgs b;
@@ -1845,8 +1857,13 @@ int esacb200_hypotheses_forward(esacb200_ctx* ctx, const float* coords, int E, i
                                 int64_t assign_stride, int M, int shiftX, int shiftY, float f, float ppx, float ppy, float tau,
                                 float alpha, float beta, float maxReproj, int sub, void* tape, size_t tape_bytes_,
                                 double* out_scores, double* out_poses6, uint8_t* out_contrib) try {
-    return hypotheses_forward_impl(ctx, coords, E, H, W, assign, assign_stride, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta,
-                                   maxReproj, sub, tape, tape_bytes_, out_scores, out_poses6, out_contrib);
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (!coords || !assign || !tape || !out_scores || !out_poses6 || !out_contrib) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    Problem P;
+    int rc = fill_problem(ctx, P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS_INJECTED);
+    if (!rc) rc = check_tape(ctx, tape, tape_bytes_, P);
+    return rc ? rc : hypotheses_forward_impl(ctx, P, coords, assign, assign_stride, tape, out_scores, out_poses6, out_contrib);
 } ESAC_ABI_CATCH(ctx)
 
 // d_scores / d_poses6 are [rows, M] / [rows, M, 6] arrays (M of the tape) of which row `row` is this tape's upstream.
@@ -1955,8 +1972,12 @@ int esacb200_backward_sharded(esacb200_ctx* ctx, const float* coords, float* gra
                               int shiftX, int shiftY, float f, float ppx, float ppy, float tau, float alpha, float beta,
                               float maxReproj, int sub, esacb200_exchange_fn exchange, void* user, double* out_loss) try {
     if (!exchange) return ctx ? fail(ctx, ESACB200_ERR_ARG, "exchange callback is null") : ESACB200_ERR_ARG;
-    return backward_impl(ctx, coords, grads, E, H, W, assign, assign_stride, M, gt_pose, wRot, wTrans, cut, shiftX, shiftY, f, ppx,
-                         ppy, tau, alpha, beta, maxReproj, sub, exchange, user, out_loss);
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (!coords || !assign || !grads || !gt_pose) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+    Problem P;
+    int rc = fill_problem(ctx, P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS_INJECTED);
+    return rc ? rc : backward_impl(ctx, P, coords, assign, assign_stride, grads, gt_pose, wRot, wTrans, cut, {exchange, user}, out_loss);
 } ESAC_ABI_CATCH(ctx)
 
 // esac_backward with the experts / hypotheses sharded over the ranks of the communicator: the two exchanges of the path
@@ -1969,9 +1990,13 @@ int esacb200_backward_sharded_nccl(esacb200_ctx* ctx, const float* coords, float
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     if (!ctx->nccl_comm) return fail(ctx, ESACB200_ERR_ARG, "no communicator: call esacb200_comm_init first");
-    if (M > 0)
-        return backward_impl(ctx, coords, grads, E, H, W, assign, assign_stride, M, gt_pose, wRot, wTrans, cut, shiftX, shiftY, f, ppx,
-                             ppy, tau, alpha, beta, maxReproj, sub, nullptr, nullptr, out_loss, /*use_nccl=*/true, reduce_grads != 0);
+    if (M > 0) {
+        if (!coords || !assign || !grads || !gt_pose) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
+        Problem P;
+        int rc = fill_problem(ctx, P, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS_INJECTED);
+        const ShardSteps sh = {nullptr, nullptr, /*use_nccl=*/true, /*reduce_grads=*/reduce_grads != 0};
+        return rc ? rc : backward_impl(ctx, P, coords, assign, assign_stride, grads, gt_pose, wRot, wTrans, cut, sh, out_loss);
+    }
     // no hypotheses here: neutral contributions to both collectives
     begin_call(ctx);
     CK(ctx->stats.ensure(8 * 8));
@@ -2085,17 +2110,6 @@ static int run_batch(esacb200_ctx* ctx, int B, const int* H, const int* W, bool 
     return ESACB200_OK;
 }
 
-// The sizes of a ragged batch whose images draw M hypotheses each (or, hypotheses_backward_ragged, were drawn from): the
-// checks of fill_problem, image by image, before any image runs.
-static int check_ragged_draws(esacb200_ctx* ctx, int B, int E, const int* H, const int* W, int M) {
-    for (int b = 0; b < B; ++b) {
-        Problem P;
-        if (fill_problem(ctx, P, E, H[b], W[b], M, 0, 0, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 1, DRAWS))
-            return fail(ctx, ESACB200_ERR_ARG, "image %d: %s", b, std::string(ctx->err).c_str());
-    }
-    return 0;
-}
-
 // esac_backward over a batch, on the worker contexts of run_batch.
 int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H, const int* W,
                              int E, const int64_t* assign, int64_t assign_stride, int M, const float* gt_poses, float wRot,
@@ -2109,7 +2123,8 @@ int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coord
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
     if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
     if (E <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d M=%d", E, M);
-    int rc = check_ragged_draws(ctx, B, E, H, W, M);
+    std::vector<Plan> plans;
+    int rc = fill_problems(ctx, plans, B, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS);
     if (rc) return rc;
     bool dev_c = false, dev_g = false;
     rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
@@ -2126,9 +2141,8 @@ int esacb200_backward_ragged(esacb200_ctx* ctx, int B, const float* const* coord
     }
     rc = run_batch(ctx, B, H, W, true, [&](esacb200_ctx* w, int b) {
         double loss = 0;
-        int rc = backward_impl(w, coords[b], grads[b], E, H[b], W[b], assign + (size_t)b * arow, assign_stride, M,
-                               gt + (size_t)b * 16, wRot, wTrans, cut, shiftX ? shiftX[b] : 0, shiftY ? shiftY[b] : 0, f[b], ppx[b],
-                               ppy[b], tau, alpha, beta, maxReproj, sub, nullptr, nullptr, &loss);
+        int rc = backward_impl(w, plans[b].P, coords[b], assign + (size_t)b * arow, assign_stride, grads[b], gt + (size_t)b * 16, wRot,
+                               wTrans, cut, ShardSteps(), &loss);
         if (!rc && out_losses) out_losses[b] = loss;
         return rc;
     });
@@ -2149,25 +2163,21 @@ int esacb200_hypotheses_forward_ragged(esacb200_ctx* ctx, int B, const float* co
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
     if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
     if (E <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d M=%d", E, M);
-    int rc = check_ragged_draws(ctx, B, E, H, W, M);
+    std::vector<Plan> plans;
+    int rc = fill_problems(ctx, plans, B, E, H, W, M, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, DRAWS);
     if (rc) return rc;
     bool dev_c = false;
     rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
     if (rc) return rc;
     for (int b = 0; b < B; ++b) {
         if (!tapes[b]) return fail(ctx, ESACB200_ERR_ARG, "image %d: tape is null", b);
-        const size_t need = tape_bytes(M, H[b] * W[b]);
-        if (tape_bytes_[b] < need)
-            return fail(ctx, ESACB200_ERR_ARG, "image %d: tape holds %zu bytes, this call needs %zu", b, tape_bytes_[b], need);
-        if (!is_device_ptr(tapes[b]) || ((uintptr_t)tapes[b] & 15))
-            return fail(ctx, ESACB200_ERR_ARG, "image %d: tape must be 16-byte aligned device memory", b);
+        if (check_tape(ctx, tapes[b], tape_bytes_[b], plans[b].P))
+            return fail(ctx, ESACB200_ERR_ARG, "image %d: %s", b, std::string(ctx->err).c_str());
     }
     const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
     rc = run_batch(ctx, B, H, W, true, [&](esacb200_ctx* w, int b) {
-        return hypotheses_forward_impl(w, coords[b], E, H[b], W[b], assign + (size_t)b * arow, assign_stride, M,
-                                       shiftX ? shiftX[b] : 0, shiftY ? shiftY[b] : 0, f[b], ppx[b], ppy[b], tau, alpha, beta,
-                                       maxReproj, sub, tapes[b], tape_bytes_[b], out_scores + (size_t)b * M,
-                                       out_poses6 + (size_t)b * M * 6, out_contrib + (size_t)b * M);
+        return hypotheses_forward_impl(w, plans[b].P, coords[b], assign + (size_t)b * arow, assign_stride, tapes[b],
+                                       out_scores + (size_t)b * M, out_poses6 + (size_t)b * M * 6, out_contrib + (size_t)b * M);
     });
     return rc ? rc : ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
@@ -2180,7 +2190,8 @@ int esacb200_hypotheses_backward_ragged(esacb200_ctx* ctx, int B, const void* co
     if (!tapes || !coords || !grads || !H || !W || B <= 0) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument or empty batch");
     if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
     if (E <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad size E=%d", E);
-    int rc = check_ragged_draws(ctx, B, E, H, W, 1);
+    std::vector<Plan> sizes;  // the maps' sizes, checked as those of a forward of one hypothesis (the tapes hold M)
+    int rc = fill_problems(ctx, sizes, B, E, H, W, 1, nullptr, nullptr, nullptr, nullptr, nullptr, 0.f, 0.f, 0.f, 0.f, 1, DRAWS);
     if (rc) return rc;
     bool dev_c = false, dev_g = false, dev_t = false;
     rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", dev_c);
@@ -2207,12 +2218,8 @@ int esacb200_backward_batch_cameras(esacb200_ctx* ctx, int B, const float* coord
     if (ctx->inj_M) return fail(ctx, ESACB200_ERR_ARG, "injected cells are a single-image test hook");
     if (E <= 0 || H <= 0 || W <= 0 || M <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes E=%d H=%d W=%d M=%d", E, H, W, M);
     const size_t cstride = (size_t)E * 3 * H * W;
-    std::vector<const float*> cp((size_t)B);
-    std::vector<float*> gp((size_t)B);
-    for (int b = 0; b < B; ++b) {
-        cp[b] = coords + (size_t)b * cstride;
-        gp[b] = grads + (size_t)b * cstride;
-    }
+    const auto cp = slices(coords, B, cstride);
+    const auto gp = slices(grads, B, cstride);
     const std::vector<int> hs((size_t)B, H), ws((size_t)B, W);
     return esacb200_backward_ragged(ctx, B, cp.data(), gp.data(), hs.data(), ws.data(), E, assign, assign_stride, M, gt_poses, wRot,
                                     wTrans, cut, shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub, out_losses);
@@ -2386,12 +2393,8 @@ int esacb200_reproj_loss_cameras(esacb200_ctx* ctx, int B, const float* coords, 
     if (B <= 0 || H <= 0 || W <= 0 || sub <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d H=%d W=%d sub=%d", B, H, W, sub);
     if ((long long)H * W > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too large", W, H);
     const size_t n = (size_t)3 * H * W;
-    std::vector<const float*> cp((size_t)B);
-    std::vector<float*> gp((size_t)B);
-    for (int b = 0; b < B; ++b) {
-        cp[b] = coords + (size_t)b * n;
-        gp[b] = grads ? grads + (size_t)b * n : nullptr;
-    }
+    const auto cp = slices(coords, B, n);
+    const auto gp = slices(grads, B, n);
     const std::vector<int> hs((size_t)B, H), ws((size_t)B, W);
     return esacb200_reproj_loss_ragged(ctx, B, cp.data(), grads ? gp.data() : nullptr, hs.data(), ws.data(), gt_poses, shiftX, shiftY,
                                        f, ppx, ppy, sub, cut, maxReproj, minDepth, out_losses);
@@ -2504,14 +2507,9 @@ int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int
         return fail(ctx, ESACB200_ERR_ARG, "size mismatch: prediction %dx%d, ground truth %dx%d (at most 1 apart)", Hp, Wp, Hg, Wg);
     if ((long long)Hp * Wp > (1ll << 30) || (long long)Hg * Wg > (1ll << 30))
         return fail(ctx, ESACB200_ERR_ARG, "map too large");
-    const size_t np = (size_t)3 * Hp * Wp, ng = (size_t)3 * Hg * Wg;
-    std::vector<const float*> pp((size_t)B), qp((size_t)B);
-    std::vector<float*> gp((size_t)B);
-    for (int b = 0; b < B; ++b) {
-        pp[b] = pred + (size_t)b * np;
-        qp[b] = gt + (size_t)b * ng;
-        gp[b] = grads ? grads + (size_t)b * np : nullptr;
-    }
+    const size_t np = (size_t)3 * Hp * Wp;
+    const auto pp = slices(pred, B, np), qp = slices(gt, B, (size_t)3 * Hg * Wg);
+    const auto gp = slices(grads, B, np);
     const std::vector<int> hp((size_t)B, Hp), wp((size_t)B, Wp), hg((size_t)B, Hg), wg((size_t)B, Wg);
     return esacb200_coord_loss_ragged(ctx, B, pp.data(), hp.data(), wp.data(), qp.data(), hg.data(), wg.data(),
                                       grads ? gp.data() : nullptr, cut, out_losses, out_counts);

@@ -919,6 +919,14 @@ ESAC_HDN void pose_dloss(const Pose& est, const Pose& gt, double wRot, double wT
         }
     }
     double denom = 3 - tr * tr + 2 * tr;
+    // At a clamped trace (3 or -1) denom is 0 and the reference's coefficient -1/sqrt(0) is -inf.  Its matrix expression
+    // coef * dTrace * dRotDiff * dRod carries that -inf into the 1x9 row before the product with dRod, where infinities
+    // of both signs (or an inf times a zero) make NaN; the NaN check then returns zeros.  coef * s, with the finished
+    // product s, would give +-inf instead (DESIGN.md section 2).
+    if (!(denom > 0)) {
+        for (int i = 0; i < 6; ++i) out[i] = 0;
+        return;
+    }
     double coef = (180 / kPi * -1 / sqrt(denom));
     for (int i = 0; i < 3; ++i) {
         double s = 0;

@@ -49,7 +49,7 @@ class Scene:
 
 def make_scene(E=1, H=60, W=80, M=64, sub=8, seed=0, outlier_frac=0.4, noise=0.02, f=525.0,
                outdoor=False, gt_mass=0.6, per_expert=False, shiftX=0, shiftY=0, world_offset=0.0,
-               active_only=True, unit_scale=1.0, alpha=100.0, ppx=None, ppy=None) -> Scene:
+               active_only=True, unit_scale=1.0, alpha=100.0, ppx=None, ppy=None, rotation=None) -> Scene:
     """One synthetic image worth of expert predictions.
 
     per_expert=False: ``assign`` is a multinomial draw of M hypotheses from a gating vector with
@@ -59,7 +59,10 @@ def make_scene(E=1, H=60, W=80, M=64, sub=8, seed=0, outlier_frac=0.4, noise=0.0
     ``active_only`` (test_esac.py:157,183-185).  ``unit_scale`` multiplies every length (maps and ground-truth translation:
     metres -> e.g. millimetres) and ``alpha`` sets the score scale; the clamp fixtures use both
     (tests/golden/make_ref_golden.py).  ``ppx`` / ``ppy`` place the principal point (default: the image centre); the map
-    is generated through that camera, so a pose estimated with another camera misses the ground truth."""
+    is generated through that camera, so a pose estimated with another camera misses the ground truth.  ``rotation`` sets
+    the ground truth's world->camera rotation, as an rvec (3,) or a rotation matrix (3, 3), in place of the drawn one (a
+    rotation of at most 30 degrees); the drawn rotation still consumes its random numbers, so every other quantity of the
+    scene is what the same arguments without ``rotation`` give."""
     rng = np.random.default_rng(1305 + seed)
     img_w, img_h = W * sub, H * sub
     ppx = img_w / 2.0 if ppx is None else float(ppx)
@@ -73,11 +76,15 @@ def make_scene(E=1, H=60, W=80, M=64, sub=8, seed=0, outlier_frac=0.4, noise=0.0
             centres[e] = rng.uniform(-100, 100, 3) + world_offset
         else:
             centres[e] = np.array([5.0 * (e % 4), 5.0 * ((e // 4) % 4), 0.0]) + world_offset
-    # ground-truth scene pose (world -> camera): rotation <= 30 deg, camera centre in the box
+    # ground-truth scene pose (world -> camera): rotation <= 30 deg unless given, camera centre in the box
     axis = rng.normal(size=3)
     axis /= np.linalg.norm(axis)
     ang = rng.uniform(0, np.pi / 6)
-    R = rodrigues(axis * ang)
+    if rotation is None:
+        R = rodrigues(axis * ang)
+    else:
+        rotation = np.asarray(rotation, np.float64)
+        R = rotation.copy() if rotation.shape == (3, 3) else rodrigues(rotation)
     C = centres[gt_e] + rng.uniform(-box / 2, box / 2, 3)
     t = -R @ C
     T_scene = np.eye(4)

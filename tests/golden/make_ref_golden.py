@@ -23,6 +23,8 @@ from esac_b200.synth import make_scene  # noqa: E402
 from oracle import esac_oracle as O  # noqa: E402
 from oracle.build_ref import load_ref  # noqa: E402
 
+# pi - 1e-4 about (1, 2, 3)/sqrt(14), as plain floats so that the fixture's scene_kw stays a Python literal
+NEAR_PI_RVEC = tuple(float(v) for v in np.array([1.0, 2.0, 3.0]) / np.sqrt(14.0) * (np.pi - 1e-4))
 T_MAX = 8  # candidate sets kept per hypothesis (hypotheses that needed more tries keep their LAST T_MAX)
 N_SAMPLE = 40000
 
@@ -37,6 +39,11 @@ SMALL = {
     "ref_clamp_dpnp_9x12": dict(E=1, H=9, W=12, M=12, sub=8, seed=71, outlier_frac=0.1, noise=0.01, alpha=5.0),
     "ref_clamp_jr_on_12x16": dict(E=2, H=12, W=16, M=12, sub=8, seed=63, outlier_frac=0.3, noise=0.002, unit_scale=7000.0),
     "ref_clamp_jr_off_12x16": dict(E=2, H=12, W=16, M=12, sub=8, seed=63, outlier_frac=0.3, noise=0.002, unit_scale=5000.0),
+    # cameras far from the world axes (make_scene's own rotations stay within 30 degrees): the half turn about x (y down,
+    # looking along world -z) and 1e-4 rad short of a half turn about (1, 2, 3)/sqrt(14), where good hypotheses' rvecs
+    # sit at the sign flip of Rodrigues' vector
+    "ref_flip_x_30x40": dict(E=2, H=30, W=40, M=32, sub=8, seed=1, rotation=(3.141592653589793, 0.0, 0.0)),
+    "ref_near_pi_30x40": dict(E=2, H=30, W=40, M=32, sub=8, seed=1, rotation=NEAR_PI_RVEC),
 }
 LARGE = {
     "ref_mid_4x120x160": dict(E=4, H=120, W=160, M=48, sub=4, seed=45),

@@ -142,6 +142,14 @@ def load_library() -> C.CDLL:
     lib.esacb200_backward_async.restype = i32
     lib.esacb200_reserve_backward_async.argtypes = [vp, i32, i32, i32, i32, i32, i32]
     lib.esacb200_reserve_backward_async.restype = i32
+    lib.esacb200_hypotheses_forward_async.argtypes = [vp, i32, vp, i32, i32, i32, vp, i64, i32, vp, vp, f32, f32, f32, f32, i32,
+                                                      vp, C.c_size_t, vp, vp, vp, vp]
+    lib.esacb200_hypotheses_forward_async.restype = i32
+    lib.esacb200_hypotheses_backward_async.argtypes = [vp, i32, vp, C.c_size_t, vp, vp, i32, i32, i32, i32, vp, vp, vp]
+    lib.esacb200_hypotheses_backward_async.restype = i32
+    lib.esacb200_pose_loss_async.argtypes = [vp, i32, i32, vp, vp, f32, f32, f32, vp, vp]
+    lib.esacb200_pose_loss_async.restype = i32
+    lib.esacb200_reserve_backward_async.restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
         getattr(lib, "esacb200_" + name).restype = i32
@@ -1149,8 +1157,8 @@ def _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras, call="forwar
 def _async_context(call, lead, M, inputs, fixed):
     """The checks forward_async and backward_async (`call`) share after _async_shapes, in this order: every `fixed`
     argument (name -> (tensor, dtype, trailing shape)) is a contiguous torch tensor of shape lead + trailing shape; the
-    inputs (name -> tensor, hypAssignment among them) are contiguous, hypAssignment row by row; all are CUDA tensors of one
-    device.  Returns the context, on torch's current stream."""
+    inputs (name -> tensor, hypAssignment among them if the call takes one) are contiguous, hypAssignment row by row; all
+    are CUDA tensors of one device.  Returns the context, on torch's current stream."""
     for what, (t, dt, tail) in fixed.items():
         if not _is_torch(t):
             raise RuntimeError(f"{call} takes torch CUDA tensors only ({what} is a {type(t).__name__})")
@@ -1160,8 +1168,8 @@ def _async_context(call, lead, M, inputs, fixed):
     for what, t in inputs.items():
         if what != "hypAssignment" and not t.is_contiguous():
             raise RuntimeError(f"{what} must be contiguous (a copy would not be captured with the call)")
-    hypAssignment = inputs["hypAssignment"]
-    if lead and lead[0] > 1 and hypAssignment.stride(0) != M * hypAssignment.stride(-1):
+    hypAssignment = inputs.get("hypAssignment")
+    if hypAssignment is not None and lead and lead[0] > 1 and hypAssignment.stride(0) != M * hypAssignment.stride(-1):
         raise RuntimeError("hypAssignment must hold its rows back to back (row stride M times the element stride)")
     args = dict(inputs, **{what: t for what, (t, _, _) in fixed.items()})
     for what, t in args.items():
@@ -1244,6 +1252,115 @@ def reserve_backward_async(B: int, E: int, H: int, W: int, M: int, subSampling: 
     ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
     ctx.async_used = True
     ctx.check(ctx.lib.esacb200_reserve_backward_async(ctx.handle, int(B), int(E), int(H), int(W), int(M), int(subSampling)))
+
+
+def hypotheses_tape_stride(E: int, H: int, W: int, M: int) -> int:
+    """Bytes between consecutive images' tapes in hypotheses_forward_async: hypotheses_tape_bytes rounded up to 256."""
+    return (hypotheses_tape_bytes(E, H, W, M) + 255) // 256 * 256
+
+
+def _check_tapes(tapes, B, E, H, W, M, call):
+    if not (_is_torch(tapes) and str(tapes.dtype) == "torch.uint8" and tapes.dim() == 1 and tapes.is_contiguous()):
+        raise RuntimeError(f"{call}: tapes must be a contiguous 1-D uint8 torch tensor")
+    need = B * hypotheses_tape_stride(E, H, W, M)
+    if int(tapes.numel()) < need:
+        raise RuntimeError(f"{call}: tapes hold {int(tapes.numel())} bytes, {B} image(s) of [{E}, 3, {H}, {W}] maps with "
+                           f"M={M} need {need} (B * hypotheses_tape_stride)")
+
+
+def hypotheses_forward_async(sceneCoordinates, hypAssignment, shifts, cameras, inlierThreshold, inlierAlpha, inlierBeta,
+                             maxReproj, subSampling, tapes, outScores, outPoses, outContributing, outStatus):
+    """hypotheses_forward enqueued on torch's current stream with no host synchronisation, so that a training step with
+    a pose loss of the caller's own can be captured in a CUDA graph.  CUDA tensors only: sceneCoordinates float32
+    [B,E,3,H,W], hypAssignment int64 [B,M], shifts int32 [B,2], cameras float32 [B,3] (focal length, ppointX, ppointY),
+    read on the device when the kernels run; tapes a uint8 tensor of at least B * hypotheses_tape_stride(E,H,W,M) bytes
+    (image b's tape at b * stride).  Row b of outScores float64 [B,M], outPoses float64 [B,M,6] and outContributing bool
+    [B,M] is what hypotheses_forward returns for the same draws; outStatus int32 [B]: 0 = OK, 1 = an expert index outside
+    [0,E) (scores and poses NaN, nothing contributes).  [E,3,H,W] / [M] / [2] / [3] / [M,6] / [] tensors are one image.
+    Seeding is forward_async's: image b of the j-th call after set_seed(s) draws what the (j*B + b)-th esac.backward or
+    hypotheses_forward after set_seed(s) draws.  The workspace is backward_async's: call reserve_backward_async with the
+    largest shape before the first capture."""
+    call = "hypotheses_forward_async"
+    B, E, H, W, M = _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras, call)
+    lead = (B,) if sceneCoordinates.dim() == 5 else ()
+    if not _is_torch(tapes):
+        raise RuntimeError(f"{call} takes torch CUDA tensors only (tapes is a {type(tapes).__name__})")
+    _check_tapes(tapes, B, E, H, W, M, call)
+    ctx = _async_context(call, lead, M, {"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment,
+                                         "shifts": shifts, "cameras": cameras, "tapes": tapes},
+                         {"outScores": (outScores, "Double", (M,)), "outPoses": (outPoses, "Double", (M, 6)),
+                          "outContributing": (outContributing, "Bool", (M,)), "outStatus": (outStatus, "Int", ())})
+    ctx.check(ctx.lib.esacb200_hypotheses_forward_async(
+        ctx.handle, B, sceneCoordinates.data_ptr(), E, H, W, hypAssignment.data_ptr(), int(hypAssignment.stride(-1)), M,
+        shifts.data_ptr(), cameras.data_ptr(), *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling),
+        tapes.data_ptr(), int(tapes.numel()), outScores.data_ptr(), outPoses.data_ptr(), outContributing.data_ptr(),
+        outStatus.data_ptr()))
+
+
+def hypotheses_backward_async(tapes, sceneCoordinates, outGradients, M, gradScores=None, gradPoses=None, outStatus=None):
+    """hypotheses_backward enqueued on torch's current stream with no host synchronisation: accumulates (+=) into
+    outGradients float32 [B,E,3,H,W] what hypotheses_backward on image b's tape (written by hypotheses_forward_async with
+    M hypotheses) with gradScores[b] float64 [B,M] / gradPoses[b] float64 [B,M,6] adds; None counts as zero.  CUDA
+    tensors only; [E,3,H,W] / [M] / [M,6] / [] tensors are one image.  outStatus int32 [B] (or None): 0 = OK, 1 = the
+    forward's assignment held a bad expert index, 2 = the tape holds no forward of this shape; the gradient slice of a
+    non-zero status is left untouched.  Draws nothing and leaves the call counter alone."""
+    call = "hypotheses_backward_async"
+    for t, what in ((tapes, "tapes"), (sceneCoordinates, "sceneCoordinates"), (outGradients, "outGradients")):
+        if not _is_torch(t):
+            raise RuntimeError(f"{call} takes torch CUDA tensors only ({what} is a {type(t).__name__})")
+    single = sceneCoordinates.dim() == 4
+    _check(sceneCoordinates, "Float", 4 if single else 5, "sceneCoordinates")
+    lead = () if single else (int(sceneCoordinates.shape[0]),)
+    B = lead[0] if lead else 1
+    E, three, H, W = (int(v) for v in sceneCoordinates.shape[-4:])
+    M = int(M)
+    if three != 3 or B < 1 or E < 1 or M < 1:
+        raise RuntimeError(f"{call}: sceneCoordinates must be [B,E,3,H,W] or [E,3,H,W] and M >= 1")
+    fixed = {"outGradients": (outGradients, "Float", (E, 3, H, W))}
+    if gradScores is not None:
+        fixed["gradScores"] = (gradScores, "Double", (M,))
+    if gradPoses is not None:
+        fixed["gradPoses"] = (gradPoses, "Double", (M, 6))
+    if outStatus is not None:
+        fixed["outStatus"] = (outStatus, "Int", ())
+    _check_tapes(tapes, B, E, H, W, M, call)
+    ctx = _async_context(call, lead, M, {"sceneCoordinates": sceneCoordinates, "tapes": tapes}, fixed)
+    if outStatus is None:
+        import torch
+        outStatus = torch.empty(lead, dtype=torch.int32, device=sceneCoordinates.device)
+    ctx.check(ctx.lib.esacb200_hypotheses_backward_async(
+        ctx.handle, B, tapes.data_ptr(), int(tapes.numel()), sceneCoordinates.data_ptr(), outGradients.data_ptr(), E, H, W, M,
+        gradScores.data_ptr() if gradScores is not None else None, gradPoses.data_ptr() if gradPoses is not None else None,
+        outStatus.data_ptr()))
+    return outStatus
+
+
+def pose_loss_async(poses, gtPose, wLossRot, wLossTrans, lossCut, outLosses=None, outDloss=None):
+    """pose_loss launched on torch's current stream on the caller's CUDA tensors, with no staging copy and no host
+    synchronisation: poses float64 [B,M,6] (or [M,6]) against gtPose float32 [B,4,4] (or [4,4]).  Returns (losses [B,M],
+    dloss [B,M,6]), written into outLosses / outDloss when given; row b is bitwise what pose_loss gives."""
+    call = "pose_loss_async"
+    for t, what in ((poses, "poses"), (gtPose, "gtPose")):
+        if not _is_torch(t):
+            raise RuntimeError(f"{call} takes torch CUDA tensors only ({what} is a {type(t).__name__})")
+    batch = poses.dim() == 3
+    _check(poses, "Double", 3 if batch else 2, "poses")
+    lead = (int(poses.shape[0]),) if batch else ()
+    M = int(poses.shape[-2])
+    if int(poses.shape[-1]) != 6 or M < 1 or (batch and lead[0] < 1):
+        raise RuntimeError(f"poses must be {'[B, M, 6]' if batch else '[M, 6]'} with M >= 1, got {list(poses.shape)}")
+    import torch
+    if outLosses is None:
+        outLosses = torch.empty(lead + (M,), dtype=torch.float64, device=poses.device)
+    if outDloss is None:
+        outDloss = torch.empty(lead + (M, 6), dtype=torch.float64, device=poses.device)
+    ctx = _async_context(call, lead, M, {"poses": poses},
+                         {"gtPose": (gtPose, "Float", (4, 4)), "outLosses": (outLosses, "Double", (M,)),
+                          "outDloss": (outDloss, "Double", (M, 6))})
+    B = lead[0] if lead else 1
+    ctx.check(ctx.lib.esacb200_pose_loss_async(ctx.handle, B, M, poses.data_ptr(), gtPose.data_ptr(), float(wLossRot),
+                                               float(wLossTrans), float(lossCut), outLosses.data_ptr(), outDloss.data_ptr()))
+    return outLosses, outDloss
 
 
 def set_seed(seed: int, device: int | None = None):

@@ -326,6 +326,80 @@ def esac_hypotheses_batch(scene_coordinates, hyp_assignment, shift_x, shift_y, f
     return EsacHypothesesBatch.apply((form, hyp_assignment, params), *inputs)
 
 
+class EsacHypothesesAsync(torch.autograd.Function):
+    """EsacHypotheses / EsacHypothesesBatch on api.hypotheses_forward_async / hypotheses_backward_async: no host
+    synchronisation in the forward or the backward, so a training step with a pose loss of the caller's own can be
+    captured in a CUDA graph.  The tapes are allocated by torch in the forward (inside a capture: in the graph's pool) and
+    live on the autograd context.  `meta` holds the non-differentiable arguments."""
+
+    @staticmethod
+    def forward(ctx, meta, scene_coordinates):
+        hyp_assignment, shifts, cameras, params, status = meta
+        lead = tuple(scene_coordinates.shape[:-4])
+        E, _, H, W = (int(v) for v in scene_coordinates.shape[-4:])
+        M = int(hyp_assignment.shape[-1])
+        B = lead[0] if lead else 1
+        dev = scene_coordinates.device
+        tapes = torch.empty(B * api.hypotheses_tape_stride(E, H, W, M), dtype=torch.uint8, device=dev)
+        scores = torch.empty(lead + (M,), dtype=torch.float64, device=dev)
+        poses = torch.empty(lead + (M, 6), dtype=torch.float64, device=dev)
+        contributing = torch.empty(lead + (M,), dtype=torch.bool, device=dev)
+        if status is None:
+            status = torch.empty(lead, dtype=torch.int32, device=dev)
+        api.hypotheses_forward_async(scene_coordinates.detach(), hyp_assignment, shifts, cameras, *params, tapes, scores, poses,
+                                     contributing, status)
+        # the coordinates are passed to the backward again; autograd's version counter catches an in-place change
+        ctx.save_for_backward(scene_coordinates, tapes)
+        ctx.mark_non_differentiable(contributing)
+        ctx.set_materialize_grads(False)
+        ctx.M = M
+        return scores, poses, contributing
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_scores, grad_poses, _grad_contributing):
+        coords, tapes = ctx.saved_tensors
+        grads = torch.zeros_like(coords)
+        api.hypotheses_backward_async(tapes, coords, grads, ctx.M,
+                                      grad_scores.contiguous() if grad_scores is not None else None,
+                                      grad_poses.contiguous() if grad_poses is not None else None)
+        return None, grads
+
+
+def esac_hypotheses_async(scene_coordinates, hyp_assignment, shifts, cameras, tau, alpha, beta, max_reproj, sub, status=None):
+    """esac_hypotheses (one image: scene_coordinates [E,3,H,W], hyp_assignment [M], shifts [2], cameras [3]) or
+    esac_hypotheses_batch on a stacked batch (scene_coordinates [B,E,3,H,W], hyp_assignment [B,M], shifts [B,2] int32,
+    cameras [B,3] = focal length, ppointX, ppointY) on the stream-ordered node, for training steps captured in a CUDA
+    graph: CUDA tensors only, the shifts and cameras read on the device at replay time.  Returns scores float64 [B,M],
+    poses float64 [B,M,6] and contributing bool [B,M] (or [M], [M,6], [M] for one image), bitwise those of esac_hypotheses
+    for the same draws: image b of the j-th call draws what the (j*B + b)-th esac_hypotheses call draws.  Once
+    differentiable; an absent upstream gradient counts as zero.  status: an int32 CUDA tensor [B] (or []) that receives the
+    forward's per-image status (1 = a bad expert index: scores and poses NaN, no gradient); None keeps it internal.  Call
+    api.reserve_backward_async with the largest shape before the first capture."""
+    meta = (hyp_assignment, shifts, cameras, (tau, alpha, beta, max_reproj, sub), status)
+    return EsacHypothesesAsync.apply(meta, scene_coordinates)
+
+
+class ReferencePoseLossAsync(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, poses, gt_pose, w_rot, w_trans, cut):
+        losses, dloss = api.pose_loss_async(poses.detach(), gt_pose, w_rot, w_trans, cut)
+        ctx.save_for_backward(dloss)
+        return losses
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_losses):
+        (dloss,) = ctx.saved_tensors
+        return grad_losses[..., None] * dloss, None, None, None, None
+
+
+def reference_pose_loss_async(poses, gt_pose, w_rot, w_trans, cut):
+    """reference_pose_loss on api.pose_loss_async: CUDA tensors only, no host synchronisation, so it can be captured in a
+    CUDA graph.  poses [M,6] / [B,M,6] float64 against gt_pose [4,4] / [B,4,4] float32; the same values and gradients."""
+    return ReferencePoseLossAsync.apply(poses, gt_pose, w_rot, w_trans, cut)
+
+
 class ReferencePoseLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, poses, gt_pose, w_rot, w_trans, cut):

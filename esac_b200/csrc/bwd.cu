@@ -145,6 +145,25 @@ __device__ __forceinline__ double score_weight(float err_clamped, const Problem&
     return (-st * (1 - st) * (double)P.beta * g) * fac;
 }
 
+// The problem B2-B5 work on: BwdArgs::P, or (DEV) a copy in `local` whose sub, tau, alpha, beta and maxReproj come from
+// dv.prob when it is set (the stream-ordered hypotheses backward: the forward's values in the tape header).
+template <bool DEV>
+__device__ __forceinline__ const Problem& bwd_problem(const BwdArgs& a, const BwdDev& dv, Problem& local) {
+    if constexpr (DEV) {
+        local = a.P;
+        if (dv.prob) {
+            local.sub = __ldg(&dv.prob->sub);
+            local.tau = __ldg(&dv.prob->tau);
+            local.alpha = __ldg(&dv.prob->alpha);
+            local.beta = __ldg(&dv.prob->beta);
+            local.max_reproj = __ldg(&dv.prob->max_reproj);
+        }
+        return local;
+    } else {
+        return a.P;
+    }
+}
+
 template <bool DEV>
 __device__ __forceinline__ void block_reduce_store(double (&v)[kRed], double* dst) {
     __shared__ double sred[kBwdThreads / 32][kRed];
@@ -169,7 +188,8 @@ __device__ __forceinline__ void block_reduce_store(double (&v)[kRed], double* ds
 template <bool DEV>
 __global__ void __launch_bounds__(kBwdThreads) bwd_reduce_kernel(const __grid_constant__ BwdArgs a, BwdAux x,
                                                                  const __grid_constant__ BwdDev dv) {
-    const Problem& P = a.P;
+    Problem Pl;
+    const Problem& P = bwd_problem<DEV>(a, dv, Pl);
     const int nc = *a.n_contrib;
     const int n_items = nc * x.tiles;
     const double f = (double)dev_f<DEV>(P, dv), cx = (double)dev_ppx<DEV>(P, dv), cy = (double)dev_ppy<DEV>(P, dv),
@@ -222,7 +242,8 @@ __global__ void __launch_bounds__(kBwdThreads) bwd_reduce_kernel(const __grid_co
 template <bool DEV>
 __global__ void __launch_bounds__(32) bwd_solve_kernel(const __grid_constant__ BwdArgs a, BwdAux x,
                                                        const __grid_constant__ BwdDev dv) {
-    const Problem& P = a.P;
+    Problem Pl;
+    const Problem& P = bwd_problem<DEV>(a, dv, Pl);
     const int nc = *a.n_contrib;
     const int lane = threadIdx.x;
     __shared__ double tot[kRed];
@@ -321,7 +342,8 @@ __global__ void __launch_bounds__(32) bwd_solve_kernel(const __grid_constant__ B
 template <bool DEV>
 __global__ void __launch_bounds__(kBwdThreads) bwd_maxjr_kernel(const __grid_constant__ BwdArgs a, BwdAux x,
                                                                 const __grid_constant__ BwdDev dv) {
-    const Problem& P = a.P;
+    Problem Pl;
+    const Problem& P = bwd_problem<DEV>(a, dv, Pl);
     const int nc = *a.n_contrib;
     const int n_items = nc * x.tiles;
     const double f = (double)dev_f<DEV>(P, dv), cx = (double)dev_ppx<DEV>(P, dv), cy = (double)dev_ppy<DEV>(P, dv),
@@ -384,6 +406,10 @@ __global__ void __launch_bounds__(kBwdThreads) bwd_assemble_kernel<true>(const _
     Problem Pd = a.P;
     Pd.shiftX = dev_shift_x<true>(a.P, dv); Pd.shiftY = dev_shift_y<true>(a.P, dv);
     Pd.f = dev_f<true>(a.P, dv); Pd.ppx = dev_ppx<true>(a.P, dv); Pd.ppy = dev_ppy<true>(a.P, dv);
+    if (dv.prob) {
+        Pd.sub = __ldg(&dv.prob->sub); Pd.tau = __ldg(&dv.prob->tau); Pd.alpha = __ldg(&dv.prob->alpha);
+        Pd.beta = __ldg(&dv.prob->beta); Pd.max_reproj = __ldg(&dv.prob->max_reproj);
+    }
     const Problem& P = Pd;
 #include "bwd_assemble_body.inc"
 }
@@ -397,10 +423,18 @@ size_t tape_masks_offset(int M) { return kTapeHeadBytes + (size_t)M * sizeof(Hyp
 size_t tape_bytes(int M, int N) { return tape_masks_offset(M) + (size_t)M * 2 * ((N + 31) / 32) * 4; }
 
 // Per-job records of the contributing hypotheses, the header (with n_contrib) and a contributing flag per hypothesis.
+// DEV (stream-ordered forward): the header's shift and camera are those td.dev held when the forward ran, contrib_flags is
+// the caller's row, the kernel also writes the row's scores, poses and status, and the last image of an execution advances
+// the call counter.  An image whose assignment held a bad expert index records no job, gets NaN scores and poses, zero
+// flags and TapeTail::bad = 1.
+template <bool DEV>
 __global__ void __launch_bounds__(1024) tape_record_kernel(const __grid_constant__ BwdArgs a, TapeHead head, TapeHead* out_head,
-                                                           HypGrad* recs, unsigned char* contrib_flags) {
+                                                           HypGrad* recs, unsigned char* contrib_flags,
+                                                           const __grid_constant__ TapeDev td) {
     const int tid = threadIdx.x;
-    const int nc = *a.n_contrib;
+    bool bad = false;
+    if constexpr (DEV) bad = __ldg(td.flags) != 0;
+    const int nc = bad ? 0 : *a.n_contrib;
     for (int h = tid; h < a.P.M; h += blockDim.x) contrib_flags[h] = 0;
     __syncthreads();
     for (int j = tid; j < nc; j += blockDim.x) {
@@ -415,22 +449,76 @@ __global__ void __launch_bounds__(1024) tape_record_kernel(const __grid_constant
     }
     if (tid == 0) {
         head.n_contrib = nc;
+        if constexpr (DEV) {
+            head.P.shiftX = __ldg(td.dev.shift); head.P.shiftY = __ldg(td.dev.shift + 1);
+            head.P.f = __ldg(td.dev.cam); head.P.ppx = __ldg(td.dev.cam + 1); head.P.ppy = __ldg(td.dev.cam + 2);
+        }
         *out_head = head;
+        if constexpr (DEV) {
+            ((TapeTail*)((char*)out_head + kTapeTailOffset))->bad = bad ? 1 : 0;
+            *td.status = bad ? 1 : 0;
+            if (td.advance) td.seed[1] += (unsigned long long)td.advance;
+        }
+    }
+    if constexpr (DEV) {
+        const double nan = __longlong_as_double(0x7ff8000000000000ll);
+        for (int h = tid; h < a.P.M; h += blockDim.x) {
+            td.out_scores[h] = bad ? nan : td.scores[h];
+            const Pose& q = td.poses[h];
+            for (int i = 0; i < 3; ++i) {
+                td.out_poses6[(size_t)h * 6 + i] = bad ? nan : q.r[i];
+                td.out_poses6[(size_t)h * 6 + 3 + i] = bad ? nan : q.t[i];
+            }
+        }
     }
 }
 
 void launch_tape_records(const BwdArgs& a, const TapeHead& head, void* tape, unsigned char* contrib_flags, cudaStream_t st) {
-    tape_record_kernel<<<1, 1024, 0, st>>>(a, head, (TapeHead*)tape, (HypGrad*)((char*)tape + tape_records_offset()),
-                                           contrib_flags);
+    tape_record_kernel<false><<<1, 1024, 0, st>>>(a, head, (TapeHead*)tape, (HypGrad*)((char*)tape + tape_records_offset()),
+                                                  contrib_flags, TapeDev());
 }
+
+void launch_tape_records_async(const BwdArgs& a, const TapeHead& head, void* tape, unsigned char* contrib_flags, const TapeDev& td,
+                               cudaStream_t st) {
+    tape_record_kernel<true><<<1, 1024, 0, st>>>(a, head, (TapeHead*)tape, (HypGrad*)((char*)tape + tape_records_offset()),
+                                                 contrib_flags, td);
+}
+
+// What the DEV form of bwd_upstream_kernel reads and publishes (launch_backward_upstream_async).
+struct UpstreamDev {
+    const TapeHead* head = nullptr;
+    int M = 0;
+    int* count = nullptr;   // the job count B2-B4 read (BwdArgs::n_contrib)
+    int* skip = nullptr;    // B5's flag (BwdDev::flags)
+    int* status = nullptr;
+};
 
 // B1 of the hypotheses node: the tape's records with the caller's upstream gradients.  Path I takes dl = dL/d pose_h with
 // multiplier p = 1, path II takes g = dL/d s_h; B2-B5 are then the vector-Jacobian product of (scores, poses).
+// DEV (stream-ordered backward): the job count comes from the header, checked here against a.P and ud.M; a tape of another
+// problem (status 2) or of a forward with a bad assignment (status 1) runs no job and sets the skip flag.  A null upstream
+// counts as zero.
+template <bool DEV>
 __global__ void __launch_bounds__(1024) bwd_upstream_kernel(const __grid_constant__ BwdArgs a, BwdAux x, const HypGrad* recs,
-                                                            const double* d_scores, const double* d_poses6) {
+                                                            const double* d_scores, const double* d_poses6,
+                                                            const __grid_constant__ UpstreamDev ud) {
     const int tid = threadIdx.x;
     for (int e = tid; e < a.P.E; e += blockDim.x) x.expert_njobs[e] = 0;
-    const int nc = *a.n_contrib;
+    int nc;
+    if constexpr (DEV) {
+        const TapeHead* hd = ud.head;
+        const bool foreign = hd->magic != kTapeMagic || hd->M != ud.M || hd->P.E != a.P.E || hd->P.H != a.P.H ||
+                             hd->P.W != a.P.W || hd->n_contrib < 0 || hd->n_contrib > ud.M;
+        const int status = foreign ? 2 : (((const TapeTail*)((const char*)hd + kTapeTailOffset))->bad ? 1 : 0);
+        nc = status ? 0 : hd->n_contrib;
+        if (tid == 0) {
+            *ud.count = nc;
+            *ud.skip = status != 0;
+            *ud.status = status;
+        }
+    } else {
+        nc = *a.n_contrib;
+    }
     const size_t n8 = (size_t)nc * (sizeof(HypGrad) / 8);
     for (size_t i = tid; i < n8; i += blockDim.x) ((double*)x.hg)[i] = ((const double*)recs)[i];
     __syncthreads();
@@ -438,8 +526,13 @@ __global__ void __launch_bounds__(1024) bwd_upstream_kernel(const __grid_constan
         HypGrad& g = x.hg[j];
         const int h = g.h;
         g.p = 1.0;
-        g.g = d_scores[h];
-        for (int i = 0; i < 6; ++i) g.dl[i] = d_poses6[(size_t)h * 6 + i];
+        if constexpr (DEV) {
+            g.g = d_scores ? d_scores[h] : 0.0;
+            for (int i = 0; i < 6; ++i) g.dl[i] = d_poses6 ? d_poses6[(size_t)h * 6 + i] : 0.0;
+        } else {
+            g.g = d_scores[h];
+            for (int i = 0; i < 6; ++i) g.dl[i] = d_poses6[(size_t)h * 6 + i];
+        }
         g.maxjr_bits = 0ull;
         atomicAdd(&x.expert_njobs[g.expert], 1);
     }
@@ -499,8 +592,23 @@ void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t 
 void launch_backward_upstream(const BwdArgs& a, const void* tape, const double* d_scores, const double* d_poses6, int max_jobs,
                               int sm_count, cudaStream_t st) {
     const BwdAux x = bwd_aux(a);
-    bwd_upstream_kernel<<<1, 1024, 0, st>>>(a, x, (const HypGrad*)((const char*)tape + tape_records_offset()), d_scores, d_poses6);
+    bwd_upstream_kernel<false><<<1, 1024, 0, st>>>(a, x, (const HypGrad*)((const char*)tape + tape_records_offset()), d_scores,
+                                                   d_poses6, UpstreamDev());
     launch_backward_tail<false>(a, x, BwdDev(), max_jobs, sm_count, st);
+}
+
+void launch_backward_upstream_async(const BwdArgs& a, const void* tape, const double* d_scores, const double* d_poses6, int* count,
+                                    int* skip, int* status, const BwdDev& dv, int max_jobs, int sm_count, cudaStream_t st) {
+    const BwdAux x = bwd_aux(a);
+    UpstreamDev ud;
+    ud.head = (const TapeHead*)tape;
+    ud.M = a.P.M;
+    ud.count = count;
+    ud.skip = skip;
+    ud.status = status;
+    bwd_upstream_kernel<true><<<1, 1024, 0, st>>>(a, x, (const HypGrad*)((const char*)tape + tape_records_offset()), d_scores,
+                                                  d_poses6, ud);
+    launch_backward_tail<true>(a, x, dv, max_jobs, sm_count, st);
 }
 
 // B2-B5: everything after the per-job records, shared by the loss-driven backward and the hypotheses node.

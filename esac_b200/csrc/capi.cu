@@ -1340,8 +1340,10 @@ static int stream_capturing(esacb200_ctx* ctx, bool& capturing) {
 }
 
 // Makes the async workspace hold `plans`: grows it when no capture has used it yet, else fails without touching it.
-// backward: the workspace of the stream-ordered backward (forward_workspace's `backward`), else of the forward.
-static int async_workspace(esacb200_ctx* ctx, esacb200_ctx* a, const std::vector<Plan>& plans, bool capturing, bool backward) {
+// backward: the workspace of the stream-ordered backward (forward_workspace's `backward`), else of the forward.  `name`: the
+// entry point named in the message (null: the one of `backward`).
+static int async_workspace(esacb200_ctx* ctx, esacb200_ctx* a, const std::vector<Plan>& plans, bool capturing, bool backward,
+                           const char* name = nullptr) {
     const bool fits =
         forward_workspace(a, plans, false, [](DevBuf& b, size_t bytes) { return bytes <= b.cap ? 0 : 1; }, backward) == 0;
     if (fits) return 0;
@@ -1351,8 +1353,8 @@ static int async_workspace(esacb200_ctx* ctx, esacb200_ctx* a, const std::vector
         return fail(ctx, ESACB200_ERR_ARG,
                     "%s: E=%d H=%d W=%d M=%d needs more workspace than %s, and a graph that holds it may still be "
                     "replayed; call reserve_%s (esacb200_reserve_%s) with the largest shape before the "
-                    "first capture", what, P.E, P.H, P.W, P.M, capturing ? "was reserved before this capture" : "an earlier capture used",
-                    what, what);
+                    "first capture", name ? name : what, P.E, P.H, P.W, P.M,
+                    capturing ? "was reserved before this capture" : "an earlier capture used", what, what);
     int rc = reserve_forward_batch(a, plans, false, backward);
     if (rc) return fail(ctx, rc, "%s", a->err);
     return 0;
@@ -1388,10 +1390,12 @@ struct AsyncCall {
 
 // What forward_async and backward_async (`backward`) share for B images of problem P: checks the arguments (the n arrays
 // `ptrs`, called `names`, must be device memory), takes the async context, lays out the images and fits the workspace.
+// `name`: the entry point named in the messages (null: the one of `backward`); hypotheses_forward_async passes its own and
+// uses the backward's workspace.
 static int begin_async(esacb200_ctx* ctx, bool backward, int B, const Problem& P, const float* coords, const int64_t* assign,
                        int64_t assign_stride, const int32_t* shifts, const float* cameras, int32_t* out_status, int n,
-                       const void* const* ptrs, const char* const* names, AsyncCall& call) {
-    const char* what = backward ? "backward_async" : "forward_async";
+                       const void* const* ptrs, const char* const* names, AsyncCall& call, const char* name = nullptr) {
+    const char* what = name ? name : backward ? "backward_async" : "forward_async";
     for (int i = 0; i < n; ++i) {
         if (!ptrs[i]) return fail(ctx, ESACB200_ERR_ARG, "%s: %s is null", what, names[i]);
         if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "%s takes device pointers only: %s is host memory", what, names[i]);
@@ -1399,7 +1403,7 @@ static int begin_async(esacb200_ctx* ctx, bool backward, int B, const Problem& P
     bool capturing = false;
     int rc = stream_capturing(ctx, capturing);
     if (rc) return rc;
-    rc = async_context(ctx, capturing, what, &call.a);
+    rc = async_context(ctx, capturing, backward ? "backward_async" : "forward_async", &call.a);
     if (rc) return rc;
     esacb200_ctx* a = call.a;
     // element stride between the assignments of consecutive images: rows of a [B, M] tensor
@@ -1423,7 +1427,7 @@ static int begin_async(esacb200_ctx* ctx, bool backward, int B, const Problem& P
         im.advance = b == B - 1 ? B : 0;
         pl.async = &im;
     }
-    rc = async_workspace(ctx, a, call.plans, capturing, backward);
+    rc = async_workspace(ctx, a, call.plans, capturing, backward, what);
     if (rc) return rc;
     if (capturing) a->frozen = true;
     return 0;
@@ -1844,6 +1848,7 @@ static int hypotheses_forward_impl(esacb200_ctx* ctx, const Problem& P, const fl
     head.M = M;
     head.mask_words = (P.N + 31) / 32;
     head.P = P;
+    CK(cudaMemsetAsync((char*)tape + kTapeTailOffset, 0, sizeof(TapeTail), ctx->stream));  // (a bad assignment fails the call)
     launch_tape_records(b, head, tape, ctx->contrib8.as<unsigned char>(), ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 1;
@@ -1966,6 +1971,161 @@ int esacb200_pose_loss(esacb200_ctx* ctx, int M, const double* poses6, const flo
                        double* out_losses, double* out_dloss6) {
     return esacb200_pose_loss_batch(ctx, 1, M, poses6, gt16, wRot, wTrans, cut, out_losses, out_dloss6);
 }
+
+// -------------------------------------------------------------------------------------------------
+// The hypotheses node with the forward_async contract (esacb200_hypotheses_forward_async / _backward_async): the host path is
+// the eager one, in the stream-ordered context, with the refinement group picked on the device; the record kernel writes the
+// header from device-read values and the caller's outputs, and the backward checks the header on the device.  It uses the
+// workspace of backward_async and its rule.
+
+// Bytes between consecutive images' tapes: the tape rounded up to 256 bytes.
+static size_t tape_stride(const Problem& P) { return (tape_bytes(P.M, P.N) + 255) & ~(size_t)255; }
+
+// The tapes argument of B images: 16-byte aligned device memory of at least B strides.
+static int check_tapes(esacb200_ctx* ctx, const char* what, const void* tapes, size_t bytes, int B, const Problem& P) {
+    const size_t need = (size_t)B * tape_stride(P);
+    if (bytes < need)
+        return fail(ctx, ESACB200_ERR_ARG, "%s: tapes hold %zu bytes, %d image(s) of E=%d H=%d W=%d M=%d need %zu", what, bytes, B,
+                    P.E, P.H, P.W, P.M, need);
+    if ((uintptr_t)tapes & 15) return fail(ctx, ESACB200_ERR_ARG, "%s: tapes must be 16-byte aligned", what);
+    return 0;
+}
+
+int esacb200_hypotheses_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
+                                      int64_t assign_stride, int M, const int32_t* shifts, const float* cameras, float tau,
+                                      float alpha, float beta, float maxReproj, int sub, void* tapes, size_t tapes_bytes,
+                                      double* out_scores, double* out_poses6, uint8_t* out_contrib, int32_t* out_status) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    const char* what = "hypotheses_forward_async";
+    const void* ptrs[] = {coords, assign, shifts, cameras, tapes, out_scores, out_poses6, out_contrib, out_status};
+    const char* names[] = {"coords", "assign", "shifts", "cameras", "tapes", "out_scores", "out_poses6", "out_contrib", "out_status"};
+    AsyncCall call;
+    Problem P;
+    int rc = B <= 0 ? fail(ctx, ESACB200_ERR_ARG, "%s: empty batch (B=%d)", what, B)
+                    : fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, tau, alpha, beta, maxReproj, sub, DRAWS);
+    if (!rc) rc = check_tapes(ctx, what, tapes, tapes_bytes, B, P);
+    if (!rc) rc = begin_async(ctx, true, B, P, coords, assign, assign_stride, shifts, cameras, out_status, 9, ptrs, names, call, what);
+    if (rc) return rc;
+    esacb200_ctx* a = call.a;
+    const size_t stride = tape_stride(P);
+    for (int b = 0; b < B; ++b) {
+        Plan& pl = call.plans[b];
+        const AsyncImage& im = call.imgs[b];
+        char* tape = (char*)tapes + (size_t)b * stride;
+        rc = run_hypotheses(a, pl, pl.d_coords, (const int64_t*)pl.d_assign, assign_stride, ShardSteps(),
+                            (uint32_t*)(tape + tape_masks_offset(M)));
+        if (rc) return fail(ctx, rc, "image %d: %s", b, a->err);
+        int* sc = a->scalars.as<int>();
+        BwdArgs args;
+        memset(&args, 0, sizeof(args));
+        args.assign32 = a->assign32.as<int>();
+        args.init = a->poses.as<Pose>();
+        args.ref = a->poses_ref.as<Pose>();
+        args.cells = a->cells.as<int>();
+        args.contrib = a->contrib.as<int>();
+        args.n_contrib = sc + S_NCONTRIB;
+        args.rounds = a->rounds.as<int>();
+        args.P = P;
+        TapeHead head;
+        memset(&head, 0, sizeof(head));
+        head.magic = kTapeMagic;
+        head.M = M;
+        head.mask_words = (P.N + 31) / 32;
+        head.P = P;
+        TapeDev td;
+        td.dev = im.dev;
+        td.flags = sc + S_FLAGS;
+        td.scores = a->scores.as<double>();
+        td.poses = a->poses_ref.as<Pose>();
+        td.out_scores = out_scores + (size_t)b * M;
+        td.out_poses6 = out_poses6 + (size_t)b * M * 6;
+        td.status = im.status;
+        td.seed = a->seed_state.as<unsigned long long>();
+        td.advance = im.advance;
+        launch_tape_records_async(args, head, tape, out_contrib + (size_t)b * M, td, a->stream);
+        a->st.kernel_launches += 1;
+    }
+    CK(cudaGetLastError());
+    return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_hypotheses_backward_async(esacb200_ctx* ctx, int B, const void* tapes, size_t tapes_bytes, const float* coords,
+                                       float* grads, int E, int H, int W, int M, const double* d_scores, const double* d_poses6,
+                                       int32_t* out_status) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    const char* what = "hypotheses_backward_async";
+    if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "%s: empty batch (B=%d)", what, B);
+    const void* ptrs[] = {tapes, coords, grads, out_status, d_scores, d_poses6};
+    const char* names[] = {"tapes", "coords", "grads", "out_status", "d_scores", "d_poses6"};
+    for (int i = 0; i < 6; ++i) {
+        if (!ptrs[i]) {
+            if (i < 4) return fail(ctx, ESACB200_ERR_ARG, "%s: %s is null", what, names[i]);
+            continue;  // an absent upstream is zero
+        }
+        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "%s takes device pointers only: %s is host memory", what, names[i]);
+    }
+    std::vector<Plan> plans(1);
+    Problem& P = plans[0].P;
+    // sub, tau, alpha, beta and maxReproj are the forward's, read from the tape header on the device (BwdDev::prob)
+    int rc = fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 1, NO_DRAW);
+    if (!rc) rc = check_tapes(ctx, what, tapes, tapes_bytes, B, P);
+    if (rc) return rc;
+    plans[0].d_coords = coords;
+    bool capturing = false;
+    rc = stream_capturing(ctx, capturing);
+    esacb200_ctx* a = nullptr;
+    if (!rc) rc = async_context(ctx, capturing, "backward_async", &a);
+    if (!rc) rc = async_workspace(ctx, a, plans, capturing, true, what);
+    if (rc) return rc;
+    if (capturing) a->frozen = true;
+    int* sc = a->scalars.as<int>();
+    const size_t cstride = (size_t)E * 3 * P.N, stride = tape_stride(P);
+    for (int b = 0; b < B; ++b) {
+        const char* tape = (const char*)tapes + (size_t)b * stride;
+        BwdArgs args;
+        memset(&args, 0, sizeof(args));
+        args.coords = coords + (size_t)b * cstride;
+        args.grads = grads + (size_t)b * cstride;
+        args.n_contrib = sc + S_NCONTRIB;
+        args.job_of = a->job_of.as<int>();
+        args.masks = (const uint32_t*)(tape + tape_masks_offset(M));
+        args.mask_words = (P.N + 31) / 32;
+        args.red = a->red.as<double>();
+        args.hyp_grad = a->hypgrad.p;
+        args.P = P;
+        const Problem* hp = (const Problem*)(tape + offsetof(TapeHead, P));
+        BwdDev dv;
+        dv.flags = sc + S_FLAGS;
+        dv.dev.shift = &hp->shiftX;
+        dv.dev.cam = &hp->f;
+        dv.prob = hp;
+        launch_backward_upstream_async(args, tape, d_scores ? d_scores + (size_t)b * M : nullptr,
+                                       d_poses6 ? d_poses6 + (size_t)b * M * 6 : nullptr, sc + S_NCONTRIB, sc + S_FLAGS,
+                                       out_status + b, dv, M, a->sm_count, a->stream);
+        a->st.kernel_launches += 5;
+    }
+    CK(cudaGetLastError());
+    return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_pose_loss_async(esacb200_ctx* ctx, int B, int M, const double* poses6, const float* gt16, float wRot, float wTrans,
+                             float cut, double* out_losses, double* out_dloss6) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    const void* ptrs[] = {poses6, gt16, out_losses, out_dloss6};
+    const char* names[] = {"poses6", "gt16", "out_losses", "out_dloss6"};
+    for (int i = 0; i < 4; ++i) {
+        if (!ptrs[i]) return fail(ctx, ESACB200_ERR_ARG, "pose_loss_async: %s is null", names[i]);
+        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "pose_loss_async takes device pointers only: %s is host memory", names[i]);
+    }
+    if (M <= 0) return fail(ctx, ESACB200_ERR_ARG, "pose_loss_async: no poses (M=%d)", M);
+    if (B <= 0 || B > 65535) return fail(ctx, ESACB200_ERR_ARG, "pose_loss_async: batch of %d images outside [1, 65535]", B);
+    launch_pose_loss((const Pose*)poses6, B, M, gt16, wRot, wTrans, cut, out_losses, out_dloss6, ctx->stream);
+    CK(cudaGetLastError());
+    return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
 
 int esacb200_backward_sharded(esacb200_ctx* ctx, const float* coords, float* grads, int E, int H, int W, const int64_t* assign,
                               int64_t assign_stride, int M, const float* gt_pose, float wRot, float wTrans, float cut,

@@ -384,6 +384,9 @@ struct BwdDev {
     const float* gt = nullptr;   // [4,4] camera->world ground truth (B1), instead of BwdArgs::gt
     const int* flags = nullptr;  // the prep kernel's bad-assignment flag: B5 leaves the gradient untouched when it is set
     DevParams dev;               // shift and camera
+    // The stream-ordered hypotheses backward: the forward's problem in the tape header, whose sub, tau, alpha, beta and
+    // maxReproj B2-B5 use instead of BwdArgs::P's (the call does not take them); null: BwdArgs::P's.
+    const Problem* prob = nullptr;
 };
 // dev: non-null -> the stream-ordered instantiations, which read *dev
 void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t st, const BwdDev* dev = nullptr);
@@ -410,6 +413,13 @@ struct TapeHead {
 };
 constexpr unsigned kTapeMagic = 0x45534831u;  // "ESH1"
 constexpr size_t kTapeHeadBytes = 256;
+// Header fields behind TapeHead (still inside the kTapeHeadBytes): bad = 1 when the forward's assignment held an expert index
+// outside [0, E) (stream-ordered forward; the eager forward fails instead and writes 0).
+struct TapeTail {
+    int bad;
+};
+constexpr size_t kTapeTailOffset = (sizeof(TapeHead) + 15) & ~(size_t)15;
+static_assert(kTapeTailOffset + sizeof(TapeTail) <= kTapeHeadBytes, "the tape header holds TapeHead and TapeTail");
 size_t tape_records_offset();
 size_t tape_masks_offset(int M);
 size_t tape_bytes(int M, int N);
@@ -418,6 +428,30 @@ void launch_tape_records(const BwdArgs& a, const TapeHead& head, void* tape, uns
 // the tape's records with dl = d_poses6[h], g = d_scores[h], p = 1 (device arrays of M), then B2-B5 into a.grads
 void launch_backward_upstream(const BwdArgs& a, const void* tape, const double* d_scores, const double* d_poses6, int max_jobs,
                               int sm_count, cudaStream_t st);
+
+// Stream-ordered hypotheses forward (esacb200_hypotheses_forward_async): what the record kernel reads from and writes to
+// device memory besides the eager kernel's arguments.
+struct TapeDev {
+    DevParams dev;                   // the shift and camera the forward used (written into the header)
+    const int* flags = nullptr;      // the prep kernel's bad-assignment flag
+    const double* scores = nullptr;  // [M] the workspace's scores
+    const Pose* poses = nullptr;     // [M] the workspace's refined poses
+    double* out_scores = nullptr;    // [M] the caller's row (NaN on a bad assignment)
+    double* out_poses6 = nullptr;    // [M,6] the caller's row (NaN on a bad assignment)
+    int* status = nullptr;           // 0 or 1
+    unsigned long long* seed = nullptr;  // the async call counter seed[1], advanced by `advance`
+    int advance = 0;
+};
+// records, header (its shift and camera from td.dev), contributing flags straight into the caller's row, scores, poses and
+// status; on a bad assignment no records, n_contrib = 0 and TapeTail::bad = 1.
+void launch_tape_records_async(const BwdArgs& a, const TapeHead& head, void* tape, unsigned char* contrib_flags, const TapeDev& td,
+                               cudaStream_t st);
+// Stream-ordered hypotheses backward (esacb200_hypotheses_backward_async): checks the tape header on the device against
+// a.P's E, H, W and M, publishes the job count into *count (a.n_contrib must point there) and the skip flag into *skip
+// (dv.flags), writes *status (0, 1 = bad assignment in the forward, 2 = not a tape of this problem), then B2-B5 with
+// dv.dev / dv.prob pointing into the header.  d_scores / d_poses6 null: zero.
+void launch_backward_upstream_async(const BwdArgs& a, const void* tape, const double* d_scores, const double* d_poses6, int* count,
+                                    int* skip, int* status, const BwdDev& dv, int max_jobs, int sm_count, cudaStream_t st);
 // loss / dLoss of [B,M] scene poses, image b against camera->world ground truth gt16[b] (device [B,4,4]); outputs [B,M], [B,M,6]
 void launch_pose_loss(const Pose* poses, int B, int M, const float* gt16, float wRot, float wTrans, float cut, double* losses,
                       double* dloss6, cudaStream_t st);

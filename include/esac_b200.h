@@ -267,6 +267,42 @@ int esacb200_backward_async(esacb200_ctx* ctx, int B, const float* coords, float
  * so it may not run while the context's stream is being captured. */
 int esacb200_reserve_backward_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int subSampling);
 
+/* The hypotheses node (esacb200_hypotheses_forward / _backward) with esacb200_forward_async's contract, so that a training
+ * step with the caller's own pose loss can be captured in a CUDA graph: device pointers only, checked before anything is
+ * enqueued; no host synchronisation, read-back or event query, and no allocation while capturing.
+ *
+ * esacb200_hypotheses_forward_async: coords float32 [B,E,3,H,W], assign int64 [B,M] (rows contiguous, element stride
+ * assign_stride), shifts int32 [B,2], cameras float32 [B,3] (f, ppx, ppy), read on the device when the kernels run.  Row b
+ * of out_scores double [B,M], out_poses6 double [B,M,6] and out_contrib uint8 [B,M] is what esacb200_hypotheses_forward
+ * gives; image b's tape is at tapes + b * stride, stride = esacb200_hypotheses_tape_bytes(E,H,W,M) rounded up to 256 bytes,
+ * and tapes_bytes must be at least B * stride (16-byte aligned).  The header of a tape holds the shift and camera the
+ * forward used.  Seeding: esacb200_forward_async's device-side seed and call counter: image b of the j-th stream-ordered
+ * execution after set_seed(s) draws what the (j*B + b)-th esacb200_backward / esacb200_hypotheses_forward after set_seed(s)
+ * draws, "fixed_seed" honoured.
+ *
+ * esacb200_hypotheses_backward_async ACCUMULATES (+=) into grads float32 [B,E,3,H,W] what esacb200_hypotheses_backward on
+ * image b's tape with rows b of d_scores double [B,M] / d_poses6 double [B,M,6] (NULL = zero) adds.  It draws nothing and
+ * does not advance the call counter.  The forward's shift, camera, sub and thresholds come from the tape header.
+ *
+ * out_status int32 [B]: 0 = OK; 1 = the image's assignment held an expert index outside [0,E) (forward: its scores and
+ * poses are NaN and its contrib 0; backward of such a tape: its gradient slice is left untouched); 2 (backward only) = the
+ * tape holds no forward of this E, H, W, M: the gradient slice is left untouched.  The other images are unaffected.
+ *
+ * Workspace: esacb200_backward_async's, with its rule: call esacb200_reserve_backward_async with the largest shape before
+ * the first capture; after a capture a call that needs more fails before enqueuing anything, naming that call. */
+int esacb200_hypotheses_forward_async(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W, const int64_t* assign,
+                                      int64_t assign_stride, int M, const int32_t* shifts, const float* cameras,
+                                      float inlierThreshold, float inlierAlpha, float inlierBeta, float maxReproj, int subSampling,
+                                      void* tapes, size_t tapes_bytes, double* out_scores, double* out_poses6,
+                                      uint8_t* out_contrib, int32_t* out_status);
+int esacb200_hypotheses_backward_async(esacb200_ctx* ctx, int B, const void* tapes, size_t tapes_bytes, const float* coords,
+                                       float* grads, int E, int H, int W, int M, const double* d_scores, const double* d_poses6,
+                                       int32_t* out_status);
+/* esacb200_pose_loss_batch launched on the caller's device arrays: no staging copy and no synchronisation (poses6 double
+ * [B,M,6], gt16 float32 [B,4,4], out_losses double [B,M], out_dloss6 double [B,M,6]); bitwise the same rows. */
+int esacb200_pose_loss_async(esacb200_ctx* ctx, int B, int M, const double* poses6, const float* gt16, float wLossRot,
+                             float wLossTrans, float lossCut, double* out_losses, double* out_dloss6);
+
 /* esac_backward over B images of one shape (the reference trains with batch_size=1, train_esac.py:96-100, one
  * esac.backward per image): coords / grads float32 [B,E,3,H,W] (grads accumulated in place, as esac.cpp:490-508),
  * assign int64 [B,M] (as in esacb200_forward_batch), gt_poses float32 [B,4,4] (camera->world), shiftX / shiftY int [B]

@@ -8,6 +8,18 @@
 namespace esacb200 {
 
 #ifdef __CUDACC__
+// One stage of warp_reduce_scatter.  O is a template parameter so that every index into w is a constant: with the stage
+// width a loop variable (o >>= 1) the inner loops were not unrolled, and w lived in local memory.
+template <int O>
+__device__ __forceinline__ void reduce_scatter_stage(double* w, int lane) {
+    const bool up = (lane & O) != 0;
+#pragma unroll
+    for (int i = 0; i < O; ++i) {
+        const double keep = up ? w[i + O] : w[i];
+        const double send = up ? w[i] : w[i + O];
+        w[i] = keep + __shfl_xor_sync(0xffffffffu, send, O);
+    }
+}
 // Warp reduce-scatter of NV <= 32 doubles per lane: lane L returns the warp total of value L (0 for L >= NV).
 // A transposing butterfly: 31 double shuffles instead of 5*NV.
 template <int NV>
@@ -17,16 +29,11 @@ __device__ __forceinline__ double warp_reduce_scatter(const double (&v)[NV]) {
     double w[32];
 #pragma unroll
     for (int i = 0; i < 32; ++i) w[i] = i < NV ? v[i] : 0.0;
-#pragma unroll
-    for (int o = 16; o >= 1; o >>= 1) {
-        const bool up = (lane & o) != 0;
-#pragma unroll
-        for (int i = 0; i < o; ++i) {
-            const double keep = up ? w[i + o] : w[i];
-            const double send = up ? w[i] : w[i + o];
-            w[i] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-        }
-    }
+    reduce_scatter_stage<16>(w, lane);
+    reduce_scatter_stage<8>(w, lane);
+    reduce_scatter_stage<4>(w, lane);
+    reduce_scatter_stage<2>(w, lane);
+    reduce_scatter_stage<1>(w, lane);
     return w[0];
 }
 

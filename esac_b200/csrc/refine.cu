@@ -42,6 +42,9 @@ constexpr int kCacheCells = kCacheWords * 32;
 // cells with the outliers' lanes predicated off -- an fp64 instruction costs the same issue slot however many lanes are on.
 // Up to this many 32-cell words per CTA (offsets must fit 16 bits; the popcounts live in shared memory):
 constexpr int kMaxCompactWords = 2048;
+// Back-off of the exchange's polls (the root's gather and every block's mailbox) between two loads of an element that is not
+// there yet.  0, 32 and 64 ns measure the same on the H100 (DESIGN §8).
+constexpr unsigned kPollNs = 32;
 
 size_t refine_cache_bytes();
 enum { CMD_EVAL = 1, CMD_FIRST = 2, CMD_EXIT = 3 };
@@ -60,6 +63,7 @@ struct RefShared {
     double cand[kRedN];  // same at the candidate
     double par[6], prev[6], pose[6], cen[3];
     double Rc[3], dR[27], T[9], G[36], H1[36];
+    double A[36], dlt[6];  // root_lm_step's damped matrix and step: in shared memory, not the root thread's local memory
     double prev_cost, best;
     int lamlg, iters, mode, rounds, sel, step, job, h, finished;
     int n_list;                    // inlier cells of this CTA's share in the current round (compaction)
@@ -158,7 +162,7 @@ __device__ __forceinline__ void root_gather(RefShared& sh, const RefineArgs& a, 
                     if (c < a.group && !ld_ll(res + ((size_t)c * 2 + (seq & 1)) * kSlot + lane, seq, x[k])) missing |= 1u << k;
                 }
                 while (missing) {
-                    __nanosleep(32);  // do not hammer lines their writers are about to store to
+                    __nanosleep(kPollNs);  // do not hammer lines their writers are about to store to
 #pragma unroll
                     for (int k = 0; k < 10; ++k)
                         if (missing >> k & 1u) {
@@ -501,16 +505,17 @@ __device__ __forceinline__ void root_rotation_fast(RefShared& sh, const double* 
     }
     if (lane < 9) {
         const int ra = lane / 3, cb = lane - 3 * ra;
-        const double r3[3] = {rx, ry, rz};
+        // r[i] by selects: an array indexed by the lane would live in local memory
+        auto r3 = [&](int i) { return i == 0 ? rx : (i == 1 ? ry : rz); };
         // [r]x entry (ra, cb): (0,1) = -rz, (0,2) = ry, (1,0) = rz, (1,2) = -rx, (2,0) = -ry, (2,1) = rx
         const int d = cb - ra;
         double rxm = 0.;
         if (d != 0) {
             const int k = 3 - ra - cb;
             const double sgn = (d == 1 || d == -2) ? -1. : 1.;
-            rxm = sgn * r3[k];
+            rxm = sgn * r3(k);
         }
-        sh.cmd[C_R + lane] = (ra == cb ? 1. - B * x : 0.) + B * r3[ra] * r3[cb] + A * rxm;
+        sh.cmd[C_R + lane] = (ra == cb ? 1. - B * x : 0.) + B * r3(ra) * r3(cb) + A * rxm;
     }
     __syncwarp();
     if (lane < 3) {
@@ -534,20 +539,22 @@ __device__ __forceinline__ void root_rotation_jacobian(RefShared& sh, const doub
     double c = 1., sn = 0., it = 0.;
     if (!tiny) { sincos(theta, &sn, &c); it = 1. / theta; }
     const double c1 = 1. - c;
-    const double rr[3] = {rx0 * it, ry0 * it, rz0 * it};
+    const double rr0 = rx0 * it, rr1 = ry0 * it, rr2 = rz0 * it;
+    auto rr = [&](int i) { return i == 0 ? rr0 : (i == 1 ? rr1 : rr2); };  // selects, not a lane-indexed local array
     if (lane < 27) {  // dR[i*9 + e] = d R[e] / d r_i
         const int i = lane / 9, e_ = lane - 9 * i, ra = e_ / 3, cb = e_ - 3 * ra;
         double v;
         if (tiny) {
             v = -eps3(ra, cb, i);
         } else {
-            const double ri = rr[i];
+            const double ri = rr(i);
             const double a0 = -sn * ri, a1 = (sn - 2 * c1 * it) * ri, a2 = c1 * it, a3 = (c - sn * it) * ri, a4 = sn * it;
             const double I_e = ra == cb ? 1. : 0.;
-            const double rrt = rr[ra] * rr[cb];
-            const double drrt = (ra == i ? rr[cb] : 0.) + (cb == i ? rr[ra] : 0.);
+            const double rrt = rr(ra) * rr(cb);
+            const double drrt = (ra == i ? rr(cb) : 0.) + (cb == i ? rr(ra) : 0.);
             double rxm = 0;  // [r]x entry (ra, cb) = -eps(ra, cb, k) r_k
-            for (int k = 0; k < 3; ++k) rxm -= eps3(ra, cb, k) * rr[k];
+#pragma unroll
+            for (int k = 0; k < 3; ++k) rxm -= eps3(ra, cb, k) * rr(k);
             const double drx = -eps3(ra, cb, i);
             v = a0 * I_e + a1 * rrt + a2 * drrt + a3 * rxm + a4 * drx;
         }
@@ -615,7 +622,8 @@ __device__ __forceinline__ void root_map_sums(RefShared& sh, int lane) {
 }
 // step(): param = prevParam - solve(JtJ with diag * (1 + 10^lamlg), JtErr)   (CvLevMarq::step), thread 0 of the root
 __device__ __forceinline__ void root_lm_step(RefShared& sh) {
-    double A[36];
+    double* A = sh.A;  // the fall-backs index A and dlt at run time, which would put register arrays in local memory
+    double* dlt = sh.dlt;
     int k = 0;
 #pragma unroll
     for (int i = 0; i < 6; ++i)
@@ -626,7 +634,6 @@ __device__ __forceinline__ void root_lm_step(RefShared& sh) {
     for (int i = 0; i < 6; ++i) A[i * 6 + i] *= 1. + lambda;
     // solve(JtJN, JtErr, DECOMP_SVD): direct solve when the damped matrix is positive definite (the solution is the same
     // up to rounding, which the iteration is insensitive to), SVD-style pseudo-inverse otherwise
-    double dlt[6];
     if (!solve6_block(A, &sh.cur[21], dlt) && !chol_solve6(A, &sh.cur[21], dlt)) {
         double Ai[36];
         pinv_sym6(A, Ai);

@@ -432,8 +432,9 @@ int esacb200_get_stats(esacb200_ctx* ctx, esacb200_stats* out);
 
 /* Diagnostics: with option "refine_profile" = 1 block 0 of the refinement kernel accumulates clock64() cycles per phase of
  * an LM evaluation of the root block: [0] produce + receive the command (Rodrigues of the new parameters), [1] pass over
- * the cells, [2] block reduction + slot write + change of variables, [3] wait for the group's epoch flags, [4] slot
- * summation, [5] map the sums to (rvec, tvec), [6] accept / reject + LM step; [8] = number of evaluations.
+ * the cells, [2] block reduction + slot write, [7] dR/dr + change of variables (root, before its gather), [3] wait for the
+ * group's results, [4] slot summation, [5] map the sums to (rvec, tvec), [6] accept / reject + LM step; [8] = number of
+ * evaluations.
  * out16: host long long [16]. */
 int esacb200_get_refine_profile(esacb200_ctx* ctx, long long* out16);
 

@@ -5,8 +5,9 @@ import numpy as np, torch
 import esac_b200.api as api
 from esac_b200.synth import make_scene
 
-NAMES = ["produce + receive the command (Rodrigues)", "pass over the cells", "block reduce + publish + change of variables",
-         "wait for the group's epoch flags", "slot summation", "map sums to (rvec,tvec)", "accept/reject + LM step", "(unused)"]
+NAMES = ["produce + receive the command (Rodrigues)", "pass over the cells", "block reduce + publish",
+         "wait for the group's results", "slot summation", "map sums to (rvec,tvec)", "accept/reject + LM step",
+         "root: dR/dr + change of variables"]
 ctx = api.context()
 ctx.set_option("fixed_seed", 1)
 ctx.set_option("refine_profile", 1)

@@ -37,6 +37,9 @@ class Stats(C.Structure):
 
 _lib = None
 PACK_TAIL = 21  # doubles behind the M_pad scores of a shard's record (include/esac_b200.h)
+# Offsets of the tail's fields from its start (M_pad): camera pose of the local winner (16 doubles), its global expert id
+# (-1 on a bad assignment), local winner, the shard's M, hyp_offset, hyp_stride.
+TAIL_POSE, TAIL_EXPERT, TAIL_WINNER, TAIL_M, TAIL_HYP_OFFSET, TAIL_HYP_STRIDE = 0, 16, 17, 18, 19, 20
 EXCHANGE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_int, C.POINTER(C.c_double), C.c_int)
 
 

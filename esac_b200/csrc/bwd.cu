@@ -626,17 +626,17 @@ static void launch_backward_tail(const BwdArgs& a, const BwdAux& x, const BwdDev
 
 // esac.backward's return value for a stream-ordered image: the expected loss (NaN on a bad assignment) and the status; the
 // last image of an execution advances the async call counter.
-__global__ void finish_backward_async_kernel(const double* stats, const int* flags, double* loss, int* status,
+__global__ void finish_backward_async_kernel(const CallStats* stats, const int* flags, double* loss, int* status,
                                              unsigned long long* seed, int advance) {
     if (threadIdx.x == 0) {
         const int bad = flags[0];
-        *loss = bad ? __longlong_as_double(0x7ff8000000000000ll) : stats[4];
+        *loss = bad ? __longlong_as_double(0x7ff8000000000000ll) : stats->local_loss;
         *status = bad;
         if (advance) seed[1] += (unsigned long long)advance;
     }
 }
 
-void launch_finish_backward_async(const double* stats, const int* flags, double* loss, int* status, unsigned long long* seed,
+void launch_finish_backward_async(const CallStats* stats, const int* flags, double* loss, int* status, unsigned long long* seed,
                                   int advance, cudaStream_t st) {
     finish_backward_async_kernel<<<1, 32, 0, st>>>(stats, flags, loss, status, seed, advance);
 }

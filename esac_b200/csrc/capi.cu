@@ -89,6 +89,20 @@ struct LastCall {
     bool losses = false;       // esac.backward's per-hypothesis losses
 };
 
+// The context's pinned host memory: a member for each value a call reads back or uploads through it, so no two uses share
+// bytes.
+struct Pinned {
+    ForwardRecord fwd;   // the forward record (esacb200_forward, forward_sharded)
+    float gt[16];        // a device ground-truth pose (esac.backward)
+    int scalars[8];      // the head of the scalars buffer (finish_call)
+    int n_contrib;       // contributing hypotheses before the refinement (run_hypotheses)
+    int gating_flags;    // the flags of esacb200_assign
+    CallStats stats;     // the call statistics (finish_call; global_loss: backward_sharded_nccl without hypotheses)
+    int rounds[2];       // head of the refinement rounds of esacb200_forward
+    double exchange[3];  // this rank's contributions to the exchanges of a sharded backward, and their results
+    double upload;       // the global expected loss from the exchange callback, on its way to CallStats::global_loss
+};
+
 }  // namespace
 
 struct esacb200_ctx {
@@ -111,11 +125,10 @@ struct esacb200_ctx {
     char err[512] = {0};
     // workspace
     DevBuf coords, grads, assign64, assign32, counts, offsets, perm, slot_of, chunks, scalars, centres, poses, poses_ref,
-        cells, tries, posepk, part, scores, probs, stats, contrib, masks, rounds, scratch, barrier, out17, inject,
+        cells, tries, posepk, part, scores, probs, stats, contrib, masks, rounds, scratch, barrier, fwd_rec, inject,
         losses, red, hypgrad, job_of, gt, smp_int, smp_surv, smp_trace, clist, eflags, coords4, coords_alt, assign64_alt, out_batch, prof,
         contrib8, upstream;
-    float* h_out = nullptr;  // pinned staging: 32 floats
-    double* h_dbl = nullptr; // pinned staging: 8 doubles
+    Pinned* pin = nullptr;
     int inj_M = 0, inj_T = 0;
     cudaEvent_t ev[EV_COUNT] = {nullptr};
     bool ev_used[EV_COUNT] = {false};
@@ -404,9 +417,9 @@ int prep_buffers(esacb200_ctx* ctx, const Plan& pl, Need&& need) {
     NEED(ctx->part, (size_t)P.M * pl.T * 4);
     NEED(ctx->scores, (size_t)P.M * 8);
     NEED(ctx->probs, (size_t)P.M * 8);
-    NEED(ctx->stats, 8 * 8);
+    NEED(ctx->stats, sizeof(CallStats));
     NEED(ctx->contrib, (size_t)P.M * 4);
-    NEED(ctx->out17, 32 * 4);
+    NEED(ctx->fwd_rec, sizeof(ForwardRecord));
     return 0;
 }
 
@@ -449,8 +462,8 @@ SampleSizes sample_sizes(const esacb200_ctx* ctx, const Plan& pl) {
     if (G > 2 && (!ctx->aux_more[0] || !ctx->aux_more[1] || P.M < 512)) G = 2;
     z.G = G;
     z.Mg = pl.split_e ? P.M : (P.M + G - 1) / G;  // capacity of a lane's work list
-    // ints: [best: 2M] [base: M] [ovf: M] then per group [list: 2*Mg] [counters: 8]
-    z.per_group_ints = (size_t)2 * z.Mg + 8;
+    // ints: [best: 2M] [base: M] [ovf: M] then per group [list: 2*Mg] [counters: SC_COUNT]
+    z.per_group_ints = (size_t)2 * z.Mg + SC_COUNT;
     z.int_bytes = ((size_t)P.M * 4 + G * z.per_group_ints) * 4 + 8;
     z.per_group_bytes = (size_t)kSampleCap * sizeof(int2) + (size_t)kSampleCapAcc * sizeof(Accepted);
     z.surv_bytes = G * z.per_group_bytes;
@@ -544,7 +557,7 @@ int run_score(esacb200_ctx* ctx, const Plan& pl) {
     launch_score(a, pl.ppt, pl.grid, ctx->stream);
     mark(ctx, EV_SCORE);
     launch_select(ctx->part.as<float>(), ctx->slot_of.as<int>(), P, pl.T, ctx->scores.as<double>(), ctx->probs.as<double>(),
-                  ctx->stats.as<double>(), sc + S_WINNER, ctx->contrib.as<int>(), sc + S_NCONTRIB, ctx->stream);
+                  ctx->stats.as<CallStats>(), sc + S_WINNER, ctx->contrib.as<int>(), sc + S_NCONTRIB, ctx->stream);
     mark(ctx, EV_SELECT);
     ctx->st.kernel_launches += 3;
     ctx->st.score_launches += 1;
@@ -672,9 +685,9 @@ uint64_t call_seed(esacb200_ctx* ctx) {
     return s;
 }
 
-// sample -> score -> select -> refine(winner) -> camera pose + expert id into d_out17 (17 floats + flags at [17]); no sync.
+// sample -> score -> select -> refine(winner) -> the forward record (rank aside) into d_rec; no sync.
 // A stream-ordered image (pl.async) takes its seed from device memory and writes the caller's arrays instead.
-int enqueue_forward_core(esacb200_ctx* ctx, const Plan& pl, float* d_out17) {
+int enqueue_forward_core(esacb200_ctx* ctx, const Plan& pl, ForwardRecord* d_rec) {
     const Problem& P = pl.P;
     int* sc = ctx->scalars.as<int>();
     const uint64_t seed = pl.async ? 0 : call_seed(ctx);
@@ -691,7 +704,7 @@ int enqueue_forward_core(esacb200_ctx* ctx, const Plan& pl, float* d_out17) {
                                     pl.async->expert, pl.async->status, ctx->seed_state.as<unsigned long long>(), pl.async->advance,
                                     ctx->stream);
     else
-        launch_finish_forward(ctx->poses_ref.as<Pose>(), sc + S_WINNER, ctx->assign32.as<int>(), sc + S_FLAGS, d_out17, ctx->stream);
+        launch_finish_forward(ctx->poses_ref.as<Pose>(), sc + S_WINNER, ctx->assign32.as<int>(), sc + S_FLAGS, d_rec, ctx->stream);
     ctx->st.kernel_launches += 1;
     return 0;
 }
@@ -860,22 +873,25 @@ void record_draw(esacb200_ctx* ctx, const Plan& pl, bool losses) {
     l.losses = losses;
 }
 
+// How much of CallStats a call reads back: nothing, what the select kernel wrote (entropy .. n_contrib) or all of it.
+constexpr size_t kNoStats = 0, kSelectStats = offsetof(CallStats, unused), kAllStats = sizeof(CallStats);
+
 // The end of a call that ran prep .. select on the context and synchronises once: after the copies the caller enqueued,
-// read back the scalars and the first `n_stats` statistics doubles, wait, check the expert indices, fill the statistics
-// and the last-call record (`drew`: the call drew `pl`'s hypotheses, and used up any injected cells; `losses`: see
-// record_draw) and take the stage times.
-int finish_call(esacb200_ctx* ctx, const Plan& pl, int n_stats, bool drew, bool losses = false) {
-    CK(cudaMemcpyAsync(ctx->h_out + 20, ctx->scalars.p, 8 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    if (n_stats) CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.p, n_stats * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+// read back the scalars and the first `stats_bytes` bytes of the statistics, wait, check the expert indices, fill the
+// statistics and the last-call record (`drew`: the call drew `pl`'s hypotheses, and used up any injected cells; `losses`:
+// see record_draw) and take the stage times.
+int finish_call(esacb200_ctx* ctx, const Plan& pl, size_t stats_bytes, bool drew, bool losses = false) {
+    CK(cudaMemcpyAsync(ctx->pin->scalars, ctx->scalars.p, sizeof(ctx->pin->scalars), cudaMemcpyDeviceToHost, ctx->stream));
+    if (stats_bytes) CK(cudaMemcpyAsync(&ctx->pin->stats, ctx->stats.p, stats_bytes, cudaMemcpyDeviceToHost, ctx->stream));
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
-    const int* hs = (const int*)(ctx->h_out + 20);
+    const int* hs = ctx->pin->scalars;
     if (hs[S_FLAGS]) return fail(ctx, ESACB200_ERR_ARG, "hypAssignment holds an expert index outside [0, %d)", pl.P.E);
     ctx->st.M = pl.P.M;
     ctx->st.winner = hs[S_WINNER];
     ctx->st.n_contrib = hs[S_NCONTRIB];
-    if (n_stats) ctx->st.entropy = ctx->h_dbl[0];
+    if (stats_bytes) ctx->st.entropy = ctx->pin->stats.entropy;
     if (drew) {
         record_draw(ctx, pl, losses);
         ctx->inj_M = ctx->inj_T = 0;
@@ -939,8 +955,7 @@ int esacb200_create(int device, esacb200_ctx** out) {
         cudaEventCreateWithFlags(&ctx->ev_consumed[i], cudaEventDisableTiming);
     }
     for (int i = 0; i < EV_COUNT; ++i) cudaEventCreate(&ctx->ev[i]);
-    cudaMallocHost((void**)&ctx->h_out, 32 * sizeof(float));
-    cudaMallocHost((void**)&ctx->h_dbl, 8 * sizeof(double));
+    cudaMallocHost((void**)&ctx->pin, sizeof(Pinned));
     ctx->refine_coresident = refine_max_coresident_blocks(ctx->sm_count);
     if (ctx->refine_coresident < 1) ctx->refine_coresident = 1;
     memset(&ctx->st, 0, sizeof(ctx->st));
@@ -959,9 +974,8 @@ void esacb200_destroy(esacb200_ctx* ctx) {
     cudaStreamSynchronize(ctx->stream);
     for (int i = 0; i < EV_COUNT; ++i)
         if (ctx->ev[i]) cudaEventDestroy(ctx->ev[i]);
-    if (ctx->h_out) cudaFreeHost(ctx->h_out);
+    if (ctx->pin) cudaFreeHost(ctx->pin);
     if (ctx->h_flags) cudaFreeHost(ctx->h_flags);
-    if (ctx->h_dbl) cudaFreeHost(ctx->h_dbl);
     for (int i = 0; i < 2; ++i) {
         if (ctx->ev_copied[i]) cudaEventDestroy(ctx->ev_copied[i]);
         if (ctx->ev_consumed[i]) cudaEventDestroy(ctx->ev_consumed[i]);
@@ -1059,16 +1073,17 @@ int esacb200_forward(esacb200_ctx* ctx, const float* coords, int E, int H, int W
     begin_call(ctx);
     rc = stage_inputs(ctx, pl, coords, assign, assign_stride, /*allow_split=*/!ctx->inj_M);
     if (rc) return rc;
-    rc = enqueue_forward_core(ctx, pl, ctx->out17.as<float>());
+    rc = enqueue_forward_core(ctx, pl, ctx->fwd_rec.as<ForwardRecord>());
     if (rc) return rc;
-    CK(cudaMemcpyAsync(ctx->h_out, ctx->out17.p, 17 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_dbl + 4, ctx->rounds.p, 2 * sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-    if (is_device_ptr(out_pose)) CK(cudaMemcpyAsync(out_pose, ctx->out17.p, 16 * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-    rc = finish_call(ctx, pl, 3, true);
+    Pinned& h = *ctx->pin;
+    CK(cudaMemcpyAsync(&h.fwd, ctx->fwd_rec.p, offsetof(ForwardRecord, bad), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(h.rounds, ctx->rounds.p, sizeof(h.rounds), cudaMemcpyDeviceToHost, ctx->stream));
+    if (is_device_ptr(out_pose)) CK(cudaMemcpyAsync(out_pose, ctx->fwd_rec.p, sizeof(h.fwd.pose), cudaMemcpyDeviceToDevice, ctx->stream));
+    rc = finish_call(ctx, pl, kSelectStats, true);
     if (rc) return rc;
-    if (!is_device_ptr(out_pose)) memcpy(out_pose, ctx->h_out, 16 * sizeof(float));
-    if (out_expert) *out_expert = (int)ctx->h_out[16];
-    ctx->st.refine_rounds = ((const int*)(ctx->h_dbl + 4))[0];
+    if (!is_device_ptr(out_pose)) memcpy(out_pose, h.fwd.pose, sizeof(h.fwd.pose));
+    if (out_expert) *out_expert = (int)h.fwd.expert;
+    ctx->st.refine_rounds = h.rounds[0];
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 
@@ -1089,14 +1104,14 @@ static int enqueue_forward_record(esacb200_ctx* ctx, const Problem& P, const flo
     if (M > 0) {
         int rc = stage_inputs(ctx, pl, coords, assign, assign_stride);
         if (rc) return rc;
-        rc = enqueue_forward_core(ctx, pl, ctx->out17.as<float>());
+        rc = enqueue_forward_core(ctx, pl, ctx->fwd_rec.as<ForwardRecord>());
         if (rc) return rc;
     } else {
         CK(ctx->scores.ensure(8));
-        CK(ctx->out17.ensure(32 * 4));
+        CK(ctx->fwd_rec.ensure(sizeof(ForwardRecord)));
     }
-    launch_pack_forward(ctx->scores.as<double>(), ctx->out17.as<float>(), M, M_pad, expert_offset, ctx->opt.hyp_offset, ctx->opt.hyp_stride,
-                        pack_out, ctx->stream);
+    launch_pack_forward(ctx->scores.as<double>(), ctx->fwd_rec.as<ForwardRecord>(), M, M_pad, expert_offset, ctx->opt.hyp_offset,
+                        ctx->opt.hyp_stride, pack_out, ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 1;
     ctx->st.M = M;
@@ -1182,18 +1197,19 @@ int esacb200_forward_sharded(esacb200_ctx* ctx, const float* coords, int E, int 
     if (!rc) rc = enqueue_forward_record(ctx, P, coords, assign, assign_stride, M, M_pad, expert_offset, mine);
     if (rc) return rc;
     CKN(nccl_api().AllGather(mine, ctx->gathered.p, rec, kNcclFloat64, ctx->nccl_comm, ctx->stream));
-    launch_select_gathered(ctx->gathered.as<double>(), world, M_pad, ctx->out17.as<float>(), ctx->stream);
+    launch_select_gathered(ctx->gathered.as<double>(), world, M_pad, ctx->fwd_rec.as<ForwardRecord>(), ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 2;
-    CK(cudaMemcpyAsync(ctx->h_out, ctx->out17.p, 20 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-    if (is_device_ptr(out_pose)) CK(cudaMemcpyAsync(out_pose, ctx->out17.p, 16 * sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
+    Pinned& h = *ctx->pin;
+    CK(cudaMemcpyAsync(&h.fwd, ctx->fwd_rec.p, sizeof(ForwardRecord), cudaMemcpyDeviceToHost, ctx->stream));
+    if (is_device_ptr(out_pose)) CK(cudaMemcpyAsync(out_pose, ctx->fwd_rec.p, sizeof(h.fwd.pose), cudaMemcpyDeviceToDevice, ctx->stream));
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
-    if (ctx->h_out[17] != 0.f) return fail(ctx, ESACB200_ERR_ARG, "a shard's hypAssignment holds an expert index outside its experts");
-    if (!is_device_ptr(out_pose)) memcpy(out_pose, ctx->h_out, 16 * sizeof(float));
-    if (out_expert) *out_expert = (int)ctx->h_out[16];
-    ctx->st.winner = (int)ctx->h_out[18];
+    if (h.fwd.bad != 0.f) return fail(ctx, ESACB200_ERR_ARG, "a shard's hypAssignment holds an expert index outside its experts");
+    if (!is_device_ptr(out_pose)) memcpy(out_pose, h.fwd.pose, sizeof(h.fwd.pose));
+    if (out_expert) *out_expert = (int)h.fwd.expert;
+    ctx->st.winner = (int)h.fwd.winner;
     finish_stats(ctx);
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
@@ -1226,7 +1242,7 @@ int esacb200_forward_ragged(esacb200_ctx* ctx, int B, const float* const* coords
     if (rc) return rc;
     // element stride between the assignments of consecutive images: rows of a [B, M] tensor
     const int64_t arow = assign_stride == 0 ? 0 : (int64_t)M * assign_stride;
-    CK(ctx->out_batch.ensure((size_t)B * 20 * sizeof(float)));
+    CK(ctx->out_batch.ensure((size_t)B * sizeof(ForwardRecord)));
     DevBuf* cb[2] = {&ctx->coords, &ctx->coords_alt};
     DevBuf* ab[2] = {&ctx->assign64, &ctx->assign64_alt};
     for (int b = 0; b < B; ++b) {
@@ -1243,27 +1259,28 @@ int esacb200_forward_ragged(esacb200_ctx* ctx, int B, const float* const* coords
         if (b == 0) mark(ctx, EV_H2D);
         rc = plan_and_prep(ctx, pl);
         if (rc) return rc;
-        rc = enqueue_forward_core(ctx, pl, ctx->out_batch.as<float>() + (size_t)b * 20);
+        rc = enqueue_forward_core(ctx, pl, ctx->out_batch.as<ForwardRecord>() + b);
         if (rc) return rc;
         if (host_coords) CK(cudaEventRecord(ctx->ev_consumed[buf], ctx->stream));
     }
-    std::vector<float> host((size_t)B * 20);
-    CK(cudaMemcpyAsync(host.data(), ctx->out_batch.p, host.size() * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+    std::vector<ForwardRecord> host((size_t)B);
+    CK(cudaMemcpyAsync(host.data(), ctx->out_batch.p, host.size() * sizeof(ForwardRecord), cudaMemcpyDeviceToHost, ctx->stream));
     const bool dev_out = is_device_ptr(out_poses);
+    const size_t pose_bytes = sizeof(ForwardRecord::pose);
     if (dev_out)
-        CK(cudaMemcpy2DAsync(out_poses, 16 * sizeof(float), ctx->out_batch.p, 20 * sizeof(float), 16 * sizeof(float), B,
-                             cudaMemcpyDeviceToDevice, ctx->stream));
+        CK(cudaMemcpy2DAsync(out_poses, pose_bytes, ctx->out_batch.p, sizeof(ForwardRecord), pose_bytes, B, cudaMemcpyDeviceToDevice,
+                             ctx->stream));
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
     for (int b = 0; b < B; ++b) {
-        const float* o = host.data() + (size_t)b * 20;
-        if (o[17] != 0.f) return fail(ctx, ESACB200_ERR_ARG, "image %d: hypAssignment holds an expert index outside [0, %d)", b, E);
-        if (!dev_out) memcpy(out_poses + (size_t)b * 16, o, 16 * sizeof(float));
-        if (out_experts) out_experts[b] = (int)o[16];
+        const ForwardRecord& o = host[b];
+        if (o.bad != 0.f) return fail(ctx, ESACB200_ERR_ARG, "image %d: hypAssignment holds an expert index outside [0, %d)", b, E);
+        if (!dev_out) memcpy(out_poses + (size_t)b * 16, o.pose, pose_bytes);
+        if (out_experts) out_experts[b] = (int)o.expert;
     }
     ctx->st.M = M;
-    ctx->st.winner = (int)host[(size_t)(B - 1) * 20 + 18];
+    ctx->st.winner = (int)host[B - 1].winner;
     record_draw(ctx, plans[B - 1], false);  // the buffers hold the last image's hypotheses
     finish_stats(ctx);
     return ESACB200_OK;
@@ -1479,7 +1496,7 @@ int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, i
     rc = run_score(ctx, pl);
     if (rc) return rc;
     CK(cudaMemcpyAsync(out_scores, ctx->scores.p, (size_t)M * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    return finish_call(ctx, pl, 0, false);
+    return finish_call(ctx, pl, kNoStats, false);
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
@@ -1602,9 +1619,10 @@ static int run_hypotheses(esacb200_ctx* ctx, Plan& pl, const float* coords, cons
     if (rc) return rc;
     if (sh.exchange) {
         // exchange 1 (SURVEY 8e): softmax normalisation over the hypotheses of ALL ranks
-        CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.as<double>() + 5, 2 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        double* x = ctx->pin->exchange;
+        CK(cudaMemcpyAsync(x, &ctx->stats.as<CallStats>()->max_score, 2 * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        double v[2] = {ctx->h_dbl[0], ctx->h_dbl[1]};
+        double v[2] = {x[0], x[1]};
         if (sh.exchange(sh.user, 1, v, 2) != 0) return fail(ctx, ESACB200_ERR_ARG, "exchange callback failed (phase 1)");
         launch_rescale_probs(ctx->scores.as<double>(), P, v[0], v[1], ctx->probs.as<double>(), ctx->contrib.as<int>(),
                              sc + S_NCONTRIB, ctx->stream);
@@ -1612,7 +1630,7 @@ static int run_hypotheses(esacb200_ctx* ctx, Plan& pl, const float* coords, cons
     } else if (sh.use_nccl) {
         // exchange 1 on the device: all-gather of the (max, sum exp) pairs, merged by the kernel that rebuilds the probabilities
         CK(ctx->gathered.ensure((size_t)ctx->comm_world * 2 * 8));
-        CKN(nccl_api().AllGather(ctx->stats.as<double>() + 5, ctx->gathered.p, 2, kNcclFloat64, ctx->nccl_comm, ctx->stream));
+        CKN(nccl_api().AllGather(&ctx->stats.as<CallStats>()->max_score, ctx->gathered.p, 2, kNcclFloat64, ctx->nccl_comm, ctx->stream));
         launch_rescale_probs_gathered(ctx->scores.as<double>(), P, ctx->gathered.as<double>(), ctx->comm_world, nullptr,
                                       ctx->probs.as<double>(), ctx->contrib.as<int>(), sc + S_NCONTRIB, ctx->stream);
         ctx->st.kernel_launches += 2;
@@ -1625,7 +1643,7 @@ static int run_hypotheses(esacb200_ctx* ctx, Plan& pl, const float* coords, cons
     // its refinement kernel picks the same group from the same count on the device (group 0).
     int group = 0;
     if (!pl.async) {
-        CK(cudaMemcpyAsync(ctx->h_out + 28, sc + S_NCONTRIB, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(&ctx->pin->n_contrib, sc + S_NCONTRIB, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
         if (sh.reduce_grads) {  // which planes receive gradient on some rank: rides on the same host synchronisation
             CK(ctx->eflags.ensure((size_t)E * sizeof(int)));
             launch_expert_flags(ctx->contrib.as<int>(), sc + S_NCONTRIB, ctx->assign32.as<int>(), E, ctx->eflags.as<int>(), ctx->stream);
@@ -1638,7 +1656,7 @@ static int run_hypotheses(esacb200_ctx* ctx, Plan& pl, const float* coords, cons
             rc = for_flagged_planes(ctx, E, (size_t)3 * P.N, sh.d_work, sh.d_dst, 0);
             if (rc) return rc;
         }
-        int n_jobs_now = *(const int*)(ctx->h_out + 28);
+        int n_jobs_now = ctx->pin->n_contrib;
         if (n_jobs_now < 1) n_jobs_now = 1;
         group = pick_group(ctx, P, n_jobs_now);
     }
@@ -1671,7 +1689,7 @@ static BwdArgs backward_args(esacb200_ctx* ctx, const Plan& pl, float* grads) {
     b.mask_words = (P.N + 31) / 32;
     b.rounds = ctx->rounds.as<int>();
     b.losses = ctx->losses.as<double>();
-    b.out_loss = ctx->stats.as<double>() + 4;
+    b.out_loss = &ctx->stats.as<CallStats>()->local_loss;
     b.red = ctx->red.as<double>();
     b.hyp_grad = ctx->hypgrad.p;
     b.P = P;
@@ -1707,10 +1725,12 @@ static int backward_impl(esacb200_ctx* ctx, const Problem& P, const float* coord
     rc = backward_buffers(ctx, P, true, grow(ctx));
     if (rc) return rc;
     BwdArgs b = backward_args(ctx, pl, d_grads);
+    Pinned& h = *ctx->pin;
+    CallStats* d_stats = ctx->stats.as<CallStats>();
     if (is_device_ptr(gt_pose)) {
-        CK(cudaMemcpyAsync(ctx->h_out, gt_pose, 16 * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(h.gt, gt_pose, sizeof(h.gt), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        memcpy(b.gt, ctx->h_out, 16 * sizeof(float));
+        memcpy(b.gt, h.gt, sizeof(h.gt));
     } else {
         memcpy(b.gt, gt_pose, 16 * sizeof(float));
     }
@@ -1719,21 +1739,20 @@ static int backward_impl(esacb200_ctx* ctx, const Problem& P, const float* coord
     if (sh.exchange) {
         // exchange 2: the expectation sum_h p_h loss_h runs over the hypotheses of all ranks (esac.cpp:357-362, esac_derivative.h:372-374)
         launch_backward_losses(b, ctx->stream);
-        CK(cudaMemcpyAsync(ctx->h_dbl, ctx->stats.as<double>() + 4, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(h.exchange, &d_stats->local_loss, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
-        double v[1] = {ctx->h_dbl[0]};
+        double v[1] = {h.exchange[0]};
         if (sh.exchange(sh.user, 2, v, 1) != 0) return fail(ctx, ESACB200_ERR_ARG, "exchange callback failed (phase 2)");
         global_loss = v[0];
-        ctx->h_dbl[6] = v[0];
-        CK(cudaMemcpyAsync(ctx->stats.as<double>() + 7, ctx->h_dbl + 6, sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
-        b.expected_override = ctx->stats.as<double>() + 7;
+        h.upload = v[0];
+        CK(cudaMemcpyAsync(&d_stats->global_loss, &h.upload, sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+        b.expected_override = &d_stats->global_loss;
         ctx->st.kernel_launches += 1;
     } else if (sh.use_nccl) {
         // exchange 2 on the device: all-reduce of the partial expectations, no host round trip
         launch_backward_losses(b, ctx->stream);
-        CKN(nccl_api().AllReduce(ctx->stats.as<double>() + 4, ctx->stats.as<double>() + 7, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm,
-                                 ctx->stream));
-        b.expected_override = ctx->stats.as<double>() + 7;
+        CKN(nccl_api().AllReduce(&d_stats->local_loss, &d_stats->global_loss, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream));
+        b.expected_override = &d_stats->global_loss;
         ctx->st.kernel_launches += 2;
     }
     launch_backward(b, M, ctx->sm_count, ctx->stream);
@@ -1747,10 +1766,10 @@ static int backward_impl(esacb200_ctx* ctx, const Problem& P, const float* coord
     }
     mark(ctx, EV_BWD);
     if (d_grads != grads) CK(cudaMemcpyAsync(grads, d_grads, cbytes, cudaMemcpyDeviceToHost, ctx->stream));
-    rc = finish_call(ctx, pl, 8, true, /*losses=*/true);
+    rc = finish_call(ctx, pl, kAllStats, true, /*losses=*/true);
     if (rc) return rc;
-    if (sh.use_nccl) global_loss = ctx->h_dbl[7];
-    ctx->st.expected_loss = (sh.exchange || sh.use_nccl) ? global_loss : ctx->h_dbl[4];
+    if (sh.use_nccl) global_loss = h.stats.global_loss;
+    ctx->st.expected_loss = (sh.exchange || sh.use_nccl) ? global_loss : h.stats.local_loss;
     if (out_loss) *out_loss = ctx->st.expected_loss;
     return ESACB200_OK;
 }
@@ -1806,7 +1825,7 @@ int esacb200_backward_async(esacb200_ctx* ctx, int B, const float* coords, float
         dv.flags = a->scalars.as<int>() + S_FLAGS;
         dv.dev = im.dev;
         launch_backward(args, M, a->sm_count, a->stream, &dv);
-        launch_finish_backward_async(a->stats.as<double>(), a->scalars.as<int>() + S_FLAGS, im.loss, im.status,
+        launch_finish_backward_async(a->stats.as<CallStats>(), a->scalars.as<int>() + S_FLAGS, im.loss, im.status,
                                      a->seed_state.as<unsigned long long>(), im.advance, a->stream);
         a->st.kernel_launches += 6;
     }
@@ -1822,6 +1841,32 @@ size_t esacb200_hypotheses_tape_bytes(int E, int H, int W, int M) {
     return tape_bytes(M, H * W);
 }
 
+// The tape header of a hypotheses forward of problem P.
+static TapeHead tape_head(const Problem& P) {
+    TapeHead head;
+    memset(&head, 0, sizeof(head));
+    head.magic = kTapeMagic;
+    head.M = P.M;
+    head.mask_words = (P.N + 31) / 32;
+    head.P = P;
+    return head;
+}
+
+// The arguments of the tape's record kernel: the hypotheses of problem P that run_hypotheses left in ctx's workspace.
+static BwdArgs tape_record_args(esacb200_ctx* ctx, const Problem& P) {
+    BwdArgs b;
+    memset(&b, 0, sizeof(b));
+    b.assign32 = ctx->assign32.as<int>();
+    b.init = ctx->poses.as<Pose>();
+    b.ref = ctx->poses_ref.as<Pose>();
+    b.cells = ctx->cells.as<int>();
+    b.contrib = ctx->contrib.as<int>();
+    b.n_contrib = ctx->scalars.as<int>() + S_NCONTRIB;
+    b.rounds = ctx->rounds.as<int>();
+    b.P = P;
+    return b;
+}
+
 // The hypotheses forward of problem P (filled and checked by the caller, with the tape: check_tape).
 static int hypotheses_forward_impl(esacb200_ctx* ctx, const Problem& P, const float* coords, const int64_t* assign,
                                    int64_t assign_stride, void* tape, double* out_scores, double* out_poses6, uint8_t* out_contrib) {
@@ -1830,32 +1875,15 @@ static int hypotheses_forward_impl(esacb200_ctx* ctx, const Problem& P, const fl
     begin_call(ctx);
     int rc = run_hypotheses(ctx, pl, coords, assign, assign_stride, ShardSteps(), (uint32_t*)((char*)tape + tape_masks_offset(M)));
     if (rc) return rc;
-    int* sc = ctx->scalars.as<int>();
     CK(ctx->contrib8.ensure((size_t)M));
-    BwdArgs b;
-    memset(&b, 0, sizeof(b));
-    b.assign32 = ctx->assign32.as<int>();
-    b.init = ctx->poses.as<Pose>();
-    b.ref = ctx->poses_ref.as<Pose>();
-    b.cells = ctx->cells.as<int>();
-    b.contrib = ctx->contrib.as<int>();
-    b.n_contrib = sc + S_NCONTRIB;
-    b.rounds = ctx->rounds.as<int>();
-    b.P = P;
-    TapeHead head;
-    memset(&head, 0, sizeof(head));
-    head.magic = kTapeMagic;
-    head.M = M;
-    head.mask_words = (P.N + 31) / 32;
-    head.P = P;
     CK(cudaMemsetAsync((char*)tape + kTapeTailOffset, 0, sizeof(TapeTail), ctx->stream));  // (a bad assignment fails the call)
-    launch_tape_records(b, head, tape, ctx->contrib8.as<unsigned char>(), ctx->stream);
+    launch_tape_records(tape_record_args(ctx, P), tape_head(P), tape, ctx->contrib8.as<unsigned char>(), ctx->stream);
     CK(cudaGetLastError());
     ctx->st.kernel_launches += 1;
     CK(cudaMemcpyAsync(out_scores, ctx->scores.p, (size_t)M * 8, cudaMemcpyDefault, ctx->stream));
     CK(cudaMemcpyAsync(out_poses6, ctx->poses_ref.p, (size_t)M * sizeof(Pose), cudaMemcpyDefault, ctx->stream));
     CK(cudaMemcpyAsync(out_contrib, ctx->contrib8.p, (size_t)M, cudaMemcpyDefault, ctx->stream));
-    return finish_call(ctx, pl, 3, true);
+    return finish_call(ctx, pl, kSelectStats, true);
 }
 
 int esacb200_hypotheses_forward(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
@@ -2016,26 +2044,9 @@ int esacb200_hypotheses_forward_async(esacb200_ctx* ctx, int B, const float* coo
         rc = run_hypotheses(a, pl, pl.d_coords, (const int64_t*)pl.d_assign, assign_stride, ShardSteps(),
                             (uint32_t*)(tape + tape_masks_offset(M)));
         if (rc) return fail(ctx, rc, "image %d: %s", b, a->err);
-        int* sc = a->scalars.as<int>();
-        BwdArgs args;
-        memset(&args, 0, sizeof(args));
-        args.assign32 = a->assign32.as<int>();
-        args.init = a->poses.as<Pose>();
-        args.ref = a->poses_ref.as<Pose>();
-        args.cells = a->cells.as<int>();
-        args.contrib = a->contrib.as<int>();
-        args.n_contrib = sc + S_NCONTRIB;
-        args.rounds = a->rounds.as<int>();
-        args.P = P;
-        TapeHead head;
-        memset(&head, 0, sizeof(head));
-        head.magic = kTapeMagic;
-        head.M = M;
-        head.mask_words = (P.N + 31) / 32;
-        head.P = P;
         TapeDev td;
         td.dev = im.dev;
-        td.flags = sc + S_FLAGS;
+        td.flags = a->scalars.as<int>() + S_FLAGS;
         td.scores = a->scores.as<double>();
         td.poses = a->poses_ref.as<Pose>();
         td.out_scores = out_scores + (size_t)b * M;
@@ -2043,7 +2054,7 @@ int esacb200_hypotheses_forward_async(esacb200_ctx* ctx, int B, const float* coo
         td.status = im.status;
         td.seed = a->seed_state.as<unsigned long long>();
         td.advance = im.advance;
-        launch_tape_records_async(args, head, tape, out_contrib + (size_t)b * M, td, a->stream);
+        launch_tape_records_async(tape_record_args(a, P), tape_head(P), tape, out_contrib + (size_t)b * M, td, a->stream);
         a->st.kernel_launches += 1;
     }
     CK(cudaGetLastError());
@@ -2159,12 +2170,14 @@ int esacb200_backward_sharded_nccl(esacb200_ctx* ctx, const float* coords, float
     }
     // no hypotheses here: neutral contributions to both collectives
     begin_call(ctx);
-    CK(ctx->stats.ensure(8 * 8));
+    CK(ctx->stats.ensure(sizeof(CallStats)));
     CK(ctx->gathered.ensure((size_t)ctx->comm_world * 2 * 8));
-    ctx->h_dbl[0] = 0.; ctx->h_dbl[1] = -1e300; ctx->h_dbl[2] = 0.;  // stats[4] partial expectation, [5] max score, [6] sum exp
-    CK(cudaMemcpyAsync(ctx->stats.as<double>() + 4, ctx->h_dbl, 3 * sizeof(double), cudaMemcpyHostToDevice, ctx->stream));
+    Pinned& h = *ctx->pin;
+    CallStats* d_stats = ctx->stats.as<CallStats>();
+    h.exchange[0] = 0.; h.exchange[1] = -1e300; h.exchange[2] = 0.;  // local_loss, max_score, sum_exp
+    CK(cudaMemcpyAsync(&d_stats->local_loss, h.exchange, sizeof(h.exchange), cudaMemcpyHostToDevice, ctx->stream));
     // the collectives below come in the order backward_impl issues them on the ranks that do hold hypotheses
-    CKN(nccl_api().AllGather(ctx->stats.as<double>() + 5, ctx->gathered.p, 2, kNcclFloat64, ctx->nccl_comm, ctx->stream));
+    CKN(nccl_api().AllGather(&d_stats->max_score, ctx->gathered.p, 2, kNcclFloat64, ctx->nccl_comm, ctx->stream));
     const size_t n = reduce_grads ? (size_t)E * 3 * H * W : 0;
     float* d_dst = grads;
     if (reduce_grads) {  // zero contribution to the gradient sum, then the sum is added to this rank's tensor like everywhere
@@ -2185,19 +2198,18 @@ int esacb200_backward_sharded_nccl(esacb200_ctx* ctx, const float* coords, float
         rc = for_flagged_planes(ctx, E, (size_t)3 * H * W, ctx->grads_work.as<float>(), d_dst, 0);
         if (rc) return rc;
     }
-    CKN(nccl_api().AllReduce(ctx->stats.as<double>() + 4, ctx->stats.as<double>() + 7, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm,
-                             ctx->stream));
+    CKN(nccl_api().AllReduce(&d_stats->local_loss, &d_stats->global_loss, 1, kNcclFloat64, kNcclSum, ctx->nccl_comm, ctx->stream));
     if (reduce_grads) {
         int rc = for_flagged_planes(ctx, E, (size_t)3 * H * W, ctx->grads_work.as<float>(), d_dst, 1);
         if (rc) return rc;
         if (!is_device_ptr(grads)) CK(cudaMemcpyAsync(grads, ctx->grads.p, n * 4, cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaGetLastError());
     }
-    CK(cudaMemcpyAsync(ctx->h_dbl + 4, ctx->stats.as<double>() + 7, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(&h.stats.global_loss, &d_stats->global_loss, sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
-    if (out_loss) *out_loss = ctx->h_dbl[4];
-    ctx->st.expected_loss = ctx->h_dbl[4];
+    if (out_loss) *out_loss = h.stats.global_loss;
+    ctx->st.expected_loss = h.stats.global_loss;
     finish_stats(ctx);
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
@@ -2423,9 +2435,9 @@ int esacb200_assign_hypotheses(esacb200_ctx* ctx, int B, int E, int M, const flo
     CK(cudaGetLastError());
     if (a_host) CK(cudaMemcpyAsync(out_assign, d_a, ab, cudaMemcpyDeviceToHost, ctx->stream));
     if (h_host) CK(cudaMemcpyAsync(out_hist, d_h, wb, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->h_out + 30, base, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(&ctx->pin->gating_flags, base, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    const int flags = *(const int*)(ctx->h_out + 30);
+    const int flags = ctx->pin->gating_flags;
     if (flags & 1) return fail(ctx, ESACB200_ERR_ARG, "probability tensor contains either inf, nan or element < 0");
     if (flags & 2) return fail(ctx, ESACB200_ERR_ARG, "invalid multinomial distribution (sum of probabilities <= 0)");
     return ESACB200_OK;
@@ -2722,16 +2734,16 @@ int esacb200_get_sample_profile(esacb200_ctx* ctx, long long* out8) try {
     if (rc) return rc;
     const int G = ctx->last.lanes, M = ctx->last.M, Mg = ctx->last.lane_cap;
     CK(cudaStreamSynchronize(ctx->stream));
-    const size_t per_group_ints = (size_t)2 * Mg + 8;
+    const size_t per_group_ints = (size_t)2 * Mg + SC_COUNT;
     for (int g = 0; g < G; ++g) {
-        int c[8];
+        int c[SC_COUNT];
         const int* src = ctx->smp_int.as<int>() + 4 * (size_t)M + g * per_group_ints + 2 * (size_t)Mg;
         CK(cudaMemcpy(c, src, sizeof(c), cudaMemcpyDeviceToHost));
-        out8[0] += (unsigned)c[5];
-        out8[1] += (unsigned)c[6];
-        out8[2] = out8[2] > c[7] ? out8[2] : c[7];
-        out8[3] += c[0];
-        out8[4] += c[2];
+        out8[0] += (unsigned)c[SC_PREFILTERED];
+        out8[1] += (unsigned)c[SC_JUDGED];
+        out8[2] = out8[2] > c[SC_WAVES] ? out8[2] : c[SC_WAVES];
+        out8[3] += c[SC_UNRESOLVED];
+        out8[4] += c[SC_STAGED];
     }
     out8[5] = G;
     return ESACB200_OK;

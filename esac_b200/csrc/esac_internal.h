@@ -1,6 +1,7 @@
 // Internal declarations shared by the translation units of libesac_b200.so.
 #pragma once
 #include <cuda_runtime.h>
+#include <stddef.h>
 #include <stdint.h>
 
 #include "esac_geom.cuh"
@@ -100,6 +101,37 @@ struct Problem {
     float f, ppx, ppy;
     float tau, alpha, beta, max_reproj;
 };
+
+// What a forward hands back to the host, in one device record that one copy reads (finish_forward_kernel; for a sharded
+// forward select_gathered_kernel): the camera->world pose of the winner, its expert, the bad-assignment flag and the
+// winning hypothesis, and for a sharded forward the owning rank.
+struct ForwardRecord {
+    float pose[16];
+    float expert, bad, winner, rank;
+};
+static_assert(sizeof(ForwardRecord) == 20 * sizeof(float), "ForwardRecord is 20 floats");
+
+// Statistics of one call on the device.  The select kernel writes entropy, winner, n_contrib and the local softmax
+// normalisation (max_score, sum_exp); the backward writes the expected loss over this rank's hypotheses (local_loss) and,
+// sharded, over all ranks (global_loss).
+struct CallStats {
+    double entropy, winner, n_contrib, unused;
+    double local_loss, max_score, sum_exp, global_loss;
+};
+static_assert(sizeof(CallStats) == 8 * sizeof(double), "CallStats is 8 doubles");
+static_assert(offsetof(CallStats, sum_exp) == offsetof(CallStats, max_score) + sizeof(double),
+              "(max_score, sum_exp) are all-gathered as two adjacent doubles");
+
+// Tail of the record a shard contributes to the all-gather of a sharded forward, behind its M_pad scores (include/esac_b200.h):
+// the camera pose of the local winner, its global expert id (-1 on a bad assignment), the local winner, the shard's M, and
+// hyp_offset / hyp_stride (local hypothesis k is hypothesis hyp_offset + k * hyp_stride of the unsharded problem).  With
+// M = 0 every field before M is -1.
+struct ShardTail {
+    double pose[16];
+    double expert, winner, M, hyp_offset, hyp_stride;
+};
+constexpr int kPackTail = sizeof(ShardTail) / sizeof(double);  // doubles behind the M_pad scores of a shard's record
+static_assert(kPackTail == 21, "the shard record's tail is the 21 doubles include/esac_b200.h documents");
 
 // Per-image values of a stream-ordered forward or backward (esacb200_forward_async / _backward_async) that the kernels read
 // from device memory instead of from Problem / a seed argument, so that a captured graph replays with the values current at
@@ -211,9 +243,9 @@ int score_tile_pixels(int ppt);
 void score_constants(const Problem& P, ScoreArgs& a);
 void launch_score(const ScoreArgs& a, int ppt, int grid, cudaStream_t st);
 // scores[h] = (alpha/W/H) * sum_tiles part ; softmax ; entropy ; argmax ; contributing list
+// into stats: entropy, winner, n_contrib, max_score, sum_exp
 void launch_select(const float* part, const int* slot_of, const Problem& P, int T, double* scores, double* probs,
-                   double* stats /* [0]=entropy [1]=winner [2]=n_contrib */, int* winner, int* contrib,
-                   int* n_contrib, cudaStream_t st);
+                   CallStats* stats, int* winner, int* contrib, int* n_contrib, cudaStream_t st);
 
 void launch_rescale_probs(const double* scores, const Problem& P, double gmax, double gsum, double* probs, int* contrib,
                           int* n_contrib, cudaStream_t st);
@@ -235,9 +267,21 @@ struct SampleState {
     int* list;      // [2M] unresolved hypotheses (second half: scratch for rebuilding)
     int2* surv;     // [cap] (hypothesis, try) pairs that passed the float prefilter
     int cap;
-    int* counters;  // [0] unresolved, [1] survivors, [2] staged accepts, [3] span of the current wave, [4] ticket,
-                    // diagnostics: [5] tries prefiltered, [6] survivors judged, [7] waves that had work
+    int* counters;  // [SC_COUNT], indexed by SampleCounter
     int M;
+};
+// Slots of SampleState::counters.
+enum SampleCounter {
+    SC_UNRESOLVED = 0,  // hypotheses in the list
+    SC_SURVIVORS,       // (hypothesis, try) pairs the prefilter passed in the current wave
+    SC_STAGED,          // accepted poses staged
+    SC_SPAN,            // tries per hypothesis in the current wave
+    SC_TICKET,          // exact_kernel CTAs done with the current wave
+    // diagnostics (esacb200_get_sample_profile)
+    SC_PREFILTERED,     // tries prefiltered
+    SC_JUDGED,          // survivors judged
+    SC_WAVES,           // waves that had work
+    SC_COUNT
 };
 // Returns the number of kernel launches it enqueued.
 int launch_sample(const float* coords, float4* coords4, const int* assign32, const Problem& P, uint64_t seed, int max_tries,
@@ -286,9 +330,8 @@ int refine_cache_words();
 int refine_max_compact_words();
 size_t refine_scratch_doubles(int n_groups, int group);
 size_t refine_flag_words(int n_groups, int group);
-// camera->world 4x4 float of poses[*winner] packed for one D2H copy: out[0..15], out[16] = expert id,
-// out[17] = bad-assignment flag, out[18] = winning hypothesis
-void launch_finish_forward(const Pose* poses, const int* winner, const int* assign32, const int* flags, float* out20,
+// camera->world 4x4 float of poses[*winner], its expert, flags[0] and the winner into rec (all but rec->rank)
+void launch_finish_forward(const Pose* poses, const int* winner, const int* assign32, const int* flags, ForwardRecord* rec,
                            cudaStream_t st);
 
 // Stream-ordered forward: camera->world pose of poses[*winner] (NaN on a bad assignment) into pose16, its expert (-1 on a bad
@@ -298,10 +341,9 @@ void launch_finish_forward_async(const Pose* poses, const int* winner, const int
 // seed[0] = base, seed[1] = 0, stream-ordered
 void launch_seed_reset(unsigned long long* seed, unsigned long long base, cudaStream_t st);
 
-void launch_pack_forward(const double* scores, const float* out20, int M, int M_pad, int expert_offset, int hyp_offset, int hyp_stride,
-                         double* pack, cudaStream_t st);
-constexpr int kPackTail = 21;  // doubles behind the M_pad scores of a shard's record
-void launch_select_gathered(const double* gathered, int world, int M_pad, float* out20, cudaStream_t st);
+void launch_pack_forward(const double* scores, const ForwardRecord* fwd, int M, int M_pad, int expert_offset, int hyp_offset,
+                         int hyp_stride, double* pack, cudaStream_t st);
+void launch_select_gathered(const double* gathered, int world, int M_pad, ForwardRecord* rec, cudaStream_t st);
 
 // --- gating.cu ----------------------------------------------------------------------------
 int assign_max_experts();
@@ -397,9 +439,9 @@ struct BwdDev {
 };
 // dev: non-null -> the stream-ordered instantiations, which read *dev
 void launch_backward(const BwdArgs& a, int max_jobs, int sm_count, cudaStream_t st, const BwdDev* dev = nullptr);
-// Stream-ordered backward: the expected loss stats[4] (NaN on a bad assignment) into *loss, flags[0] into *status; advance != 0
-// adds it to seed[1] (the last image of an execution).
-void launch_finish_backward_async(const double* stats, const int* flags, double* loss, int* status, unsigned long long* seed,
+// Stream-ordered backward: the expected loss stats->local_loss (NaN on a bad assignment) into *loss, flags[0] into *status;
+// advance != 0 adds it to seed[1] (the last image of an execution).
+void launch_finish_backward_async(const CallStats* stats, const int* flags, double* loss, int* status, unsigned long long* seed,
                                   int advance, cudaStream_t st);
 // phase split for the multi-GPU path: losses + local expectation only / everything after the loss exchange
 void launch_backward_losses(const BwdArgs& a, cudaStream_t st);

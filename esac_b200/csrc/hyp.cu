@@ -158,9 +158,9 @@ __global__ void sample_init_kernel(const __grid_constant__ SampleArgs a) {
         const int h = lane_hyp(a, k);
         st.best[h] = kNoKey; st.base[h] = 0; st.ovf[h] = kNoTry; st.list[k] = h;
     }
-    if (k == 0) {  // unresolved, survivors, staged, span, ticket; diagnostics: tries prefiltered, survivors judged, waves with work
-        st.counters[0] = n; st.counters[1] = 0; st.counters[2] = 0; st.counters[3] = a.span0; st.counters[4] = 0;
-        st.counters[5] = 0; st.counters[6] = 0; st.counters[7] = 0;
+    if (k == 0) {
+        st.counters[SC_UNRESOLVED] = n; st.counters[SC_SURVIVORS] = 0; st.counters[SC_STAGED] = 0; st.counters[SC_SPAN] = a.span0;
+        st.counters[SC_TICKET] = 0; st.counters[SC_PREFILTERED] = 0; st.counters[SC_JUDGED] = 0; st.counters[SC_WAVES] = 0;
     }
 }
 
@@ -211,8 +211,8 @@ template <bool DEV>
 __global__ void __launch_bounds__(kTryThreads, 6) prefilter_kernel(const __grid_constant__ SampleArgsT<DEV> a) {
     TraceScope trace(a.trace, a.trace_slot);
     __shared__ float4 s_obj[2][4][kTryThreads];  // [buffer][point][thread]
-    const int n_unres = a.st.counters[0];
-    const int span = a.st.counters[3];
+    const int n_unres = a.st.counters[SC_UNRESOLVED];
+    const int span = a.st.counters[SC_SPAN];
     const int cph = (span + kTryThreads - 1) / kTryThreads;  // chunks per hypothesis
     const long long n_items = (long long)n_unres * cph;
     const int lane = threadIdx.x & 31, tid = threadIdx.x;
@@ -244,7 +244,7 @@ __global__ void __launch_bounds__(kTryThreads, 6) prefilter_kernel(const __grid_
         const unsigned m = __ballot_sync(0xffffffffu, pass);
         if (m) {
             int basei = 0;
-            if (lane == 0) basei = atomicAdd(&a.st.counters[1], __popc(m));
+            if (lane == 0) basei = atomicAdd(&a.st.counters[SC_SURVIVORS], __popc(m));
             basei = __shfl_sync(0xffffffffu, basei, 0);
             if (pass) {
                 const int idx = basei + __popc(m & ((1u << lane) - 1u));
@@ -264,7 +264,7 @@ __device__ void advance_wave(const SampleState& st, int limit, float window, flo
 template <bool DEV>
 __global__ void __launch_bounds__(128) exact_kernel(const __grid_constant__ SampleArgsT<DEV> a) {
     TraceScope trace(a.trace, a.trace_slot);
-    const int n = min(a.st.counters[1], a.st.cap);
+    const int n = min(a.st.counters[SC_SURVIVORS], a.st.cap);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const int2 ht = a.st.surv[i];
         if (ht.y >= a.st.ovf[ht.x]) continue;  // beyond the point where the list overflowed: redone next wave
@@ -273,7 +273,7 @@ __global__ void __launch_bounds__(128) exact_kernel(const __grid_constant__ Samp
         bool solved;
         if (exact_try<DEV>(a, ht.x, ht.y, pose, cx, cy, solved, true)) {
             // stage the accepted pose so that emit_kernel does not have to solve it again
-            unsigned slot = (unsigned)atomicAdd(&a.st.counters[2], 1);
+            unsigned slot = (unsigned)atomicAdd(&a.st.counters[SC_STAGED], 1);
             if (slot < (unsigned)a.st.cap_acc) {
                 Accepted& ac = a.st.stage[slot];
                 ac.pose = pose;
@@ -288,7 +288,7 @@ __global__ void __launch_bounds__(128) exact_kernel(const __grid_constant__ Samp
     __shared__ int s_last;
     __threadfence();
     __syncthreads();
-    if (threadIdx.x == 0) s_last = atomicAdd(&a.st.counters[4], 1) == (int)gridDim.x - 1;
+    if (threadIdx.x == 0) s_last = atomicAdd(&a.st.counters[SC_TICKET], 1) == (int)gridDim.x - 1;
     __syncthreads();
     if (s_last) {
         __threadfence();
@@ -299,10 +299,10 @@ __global__ void __launch_bounds__(128) exact_kernel(const __grid_constant__ Samp
 // ---- wave phase 3: bookkeeping (run by the last CTA of exact_kernel to finish) -------------------------------------
 __device__ void advance_wave(const SampleState& st, int limit, float window, float tail_boost) {
     __shared__ int s_fill;
-    const int span = st.counters[3];
+    const int span = st.counters[SC_SPAN];
     if (threadIdx.x == 0) s_fill = 0;
     __syncthreads();
-    const int n_unres = st.counters[0];
+    const int n_unres = st.counters[SC_UNRESOLVED];
     // the next list is built in the second half of the buffer, then copied back (single CTA: no races)
     int* next = st.list + st.M;
     for (int u = threadIdx.x; u < n_unres; u += blockDim.x) {
@@ -324,21 +324,21 @@ __device__ void advance_wave(const SampleState& st, int limit, float window, flo
     __syncthreads();
     if (threadIdx.x == 0) {
         // next window: ~1.25 / (acceptance rate per try seen in this wave), a multiple of the CTA size
-        const int n_surv = min(st.counters[1], st.cap);
+        const int n_surv = min(st.counters[SC_SURVIVORS], st.cap);
         const double tried = (double)n_unres * (double)span;
         const double hits = n_unres - nn > 0 ? (double)(n_unres - nn) : 0.5;
         // few hypotheses left: their tries cost next to nothing, a further wave costs a full verdict latency -- ask for more
         const double boost = nn <= 8 ? tail_boost * 2. : (nn <= 64 ? tail_boost : 1.);
         double next_span = (double)window * boost * tried / hits;
         next_span = next_span < 256. ? 256. : (next_span > 65536. ? 65536. : next_span);
-        st.counters[3] = ((int)next_span + kSpanQuantum - 1) / kSpanQuantum * kSpanQuantum;
-        st.counters[0] = nn;
-        st.counters[1] = 0;
-        st.counters[4] = 0;  // ticket of the next exact_kernel
+        st.counters[SC_SPAN] = ((int)next_span + kSpanQuantum - 1) / kSpanQuantum * kSpanQuantum;
+        st.counters[SC_UNRESOLVED] = nn;
+        st.counters[SC_SURVIVORS] = 0;
+        st.counters[SC_TICKET] = 0;  // ticket of the next exact_kernel
         if (n_unres > 0) {
-            st.counters[5] += n_unres * span;
-            st.counters[6] += n_surv;
-            st.counters[7] += 1;
+            st.counters[SC_PREFILTERED] += n_unres * span;
+            st.counters[SC_JUDGED] += n_surv;
+            st.counters[SC_WAVES] += 1;
         }
     }
 }
@@ -346,7 +346,7 @@ __device__ void advance_wave(const SampleState& st, int limit, float window, flo
 // ---- tail: CTA per unresolved hypothesis, both phases inside the CTA, up to the try limit --------------------
 template <bool DEV>
 __global__ void __launch_bounds__(kTryThreads) tail_kernel(const __grid_constant__ SampleArgsT<DEV> a) {
-    const int n_unres = a.st.counters[0];
+    const int n_unres = a.st.counters[SC_UNRESOLVED];
     __shared__ int s_list[kTryThreads * 8];
     __shared__ int s_n, s_best;
     for (int u = blockIdx.x; u < n_unres; u += gridDim.x) {

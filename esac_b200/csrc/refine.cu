@@ -710,15 +710,15 @@ int refine_max_coresident_blocks(int sm_count) {
     return nb * sm_count;
 }
 
-__global__ void finish_forward_kernel(const Pose* poses, const int* winner, const int* assign32, const int* flags, float* out) {
+__global__ void finish_forward_kernel(const Pose* poses, const int* winner, const int* assign32, const int* flags, ForwardRecord* out) {
     if (threadIdx.x == 0) {
         const int w = *winner;
         double T[16];
         pose2trans(poses[w], T);
-        for (int i = 0; i < 16; ++i) out[i] = (float)T[i];
-        out[16] = (float)assign32[w];
-        out[17] = (float)flags[0];
-        out[18] = (float)w;
+        for (int i = 0; i < 16; ++i) out->pose[i] = (float)T[i];
+        out->expert = (float)assign32[w];
+        out->bad = (float)flags[0];
+        out->winner = (float)w;
     }
 }
 
@@ -743,37 +743,39 @@ __global__ void seed_reset_kernel(unsigned long long* seed, unsigned long long b
     seed[1] = 0;
 }
 
-// Record one shard contributes to the all-gather of the sharded forward (SURVEY 8e), as doubles:
-//   [scores (M_pad; entries >= M are -inf: shards may hold different numbers of hypotheses) | camera pose of the local
-//    winner (16) | global expert id, or -1 on a bad assignment | local winner | M | hyp_offset | hyp_stride]
-// (local hypothesis k is hypothesis hyp_offset + k * hyp_stride of the unsharded problem).  M == 0 gives an all -inf record.
-__global__ void pack_forward_kernel(const double* scores, const float* out20, int M, int M_pad, int expert_offset, int hyp_offset,
-                                    int hyp_stride, double* pack) {
+// Index of ShardTail member m among the doubles of the tail.
+#define TAIL_AT(m) ((int)(offsetof(ShardTail, m) / sizeof(double)))
+
+// Record one shard contributes to the all-gather of the sharded forward (SURVEY 8e), as doubles: its scores (M_pad; entries
+// >= M are -inf: shards may hold different numbers of hypotheses), then a ShardTail from the forward record `fwd`.  M == 0
+// gives an all -inf record.  One double per thread.
+__global__ void pack_forward_kernel(const double* scores, const ForwardRecord* fwd, int M, int M_pad, int expert_offset,
+                                    int hyp_offset, int hyp_stride, double* pack) {
     const double ninf = __longlong_as_double(0xfff0000000000000ull);  // -inf
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < M_pad + kPackTail; i += gridDim.x * blockDim.x) {
         double v;
         if (i < M_pad) v = i < M ? scores[i] : ninf;
-        else if (i == M_pad + 18) v = (double)M;
-        else if (i == M_pad + 19) v = (double)hyp_offset;
-        else if (i == M_pad + 20) v = (double)hyp_stride;
+        else if (i == M_pad + TAIL_AT(M)) v = (double)M;
+        else if (i == M_pad + TAIL_AT(hyp_offset)) v = (double)hyp_offset;
+        else if (i == M_pad + TAIL_AT(hyp_stride)) v = (double)hyp_stride;
         else if (M == 0) v = -1.;
-        else if (i < M_pad + 16) v = (double)out20[i - M_pad];
-        else if (i == M_pad + 16) v = out20[17] != 0.f ? -1. : (double)out20[16] + (double)expert_offset;
-        else v = (double)out20[18];
+        else if (i < M_pad + TAIL_AT(expert)) v = (double)fwd->pose[i - M_pad];
+        else if (i == M_pad + TAIL_AT(expert)) v = fwd->bad != 0.f ? -1. : (double)fwd->expert + (double)expert_offset;
+        else v = (double)fwd->winner;
         pack[i] = v;
     }
 }
 
-void launch_pack_forward(const double* scores, const float* out20, int M, int M_pad, int expert_offset, int hyp_offset, int hyp_stride,
-                         double* pack, cudaStream_t st) {
-    pack_forward_kernel<<<(M_pad + kPackTail + 255) / 256, 256, 0, st>>>(scores, out20, M, M_pad, expert_offset, hyp_offset, hyp_stride, pack);
+void launch_pack_forward(const double* scores, const ForwardRecord* fwd, int M, int M_pad, int expert_offset, int hyp_offset,
+                         int hyp_stride, double* pack, cudaStream_t st) {
+    pack_forward_kernel<<<(M_pad + kPackTail + 255) / 256, 256, 0, st>>>(scores, fwd, M, M_pad, expert_offset, hyp_offset, hyp_stride, pack);
 }
 
 // softMax + draw(training = false) over the gathered records of all shards (esac_util.h:461-530): the first strict maximum in
 // the hypothesis order of the UNSHARDED problem (global index = the record's hyp_offset + k * hyp_stride).  One block.
-// out20: [0..15] camera pose of the global winner, [16] its expert, [17] 1 if any shard flagged a bad assignment,
-// [18] global hypothesis index, [19] owning rank.
-__global__ void __launch_bounds__(256) select_gathered_kernel(const double* __restrict__ g, int world, int M_pad, float* out20) {
+// out: the camera pose of the global winner, its expert, 1 if any shard flagged a bad assignment, its global hypothesis index
+// and its owning rank.
+__global__ void __launch_bounds__(256) select_gathered_kernel(const double* __restrict__ g, int world, int M_pad, ForwardRecord* out) {
     __shared__ double sbest[8];
     __shared__ long long sidx[8];
     __shared__ int srank[8];
@@ -788,13 +790,16 @@ __global__ void __launch_bounds__(256) select_gathered_kernel(const double* __re
     for (int i = tid; i < world * M_pad; i += blockDim.x) {
         const int r = i / M_pad, k = i - r * M_pad;
         const double* rr = g + (size_t)r * rec;
-        if (k >= (int)rr[M_pad + 18]) continue;
+        // (indexed rather than through a ShardTail view, which compiles this loop differently)
+        if (k >= (int)rr[M_pad + TAIL_AT(M)]) continue;
         const double v = rr[k];
-        const long long gi = (long long)rr[M_pad + 19] + (long long)k * (long long)rr[M_pad + 20];
+        const long long gi = (long long)rr[M_pad + TAIL_AT(hyp_offset)] + (long long)k * (long long)rr[M_pad + TAIL_AT(hyp_stride)];
         if (v > best || (v == best && gi < bi)) { best = v; bi = gi; br = r; }
     }
-    for (int r = tid; r < world; r += blockDim.x)
-        if (g[(size_t)r * rec + M_pad + 18] > 0. && g[(size_t)r * rec + M_pad + 16] < 0.) atomicExch(&sbad, 1);
+    for (int r = tid; r < world; r += blockDim.x) {
+        const ShardTail& t = *(const ShardTail*)(g + (size_t)r * rec + M_pad);
+        if (t.M > 0. && t.expert < 0.) atomicExch(&sbad, 1);
+    }
     for (int o = 16; o; o >>= 1) {
         const double ob = __shfl_xor_sync(0xffffffffu, best, o);
         const long long oi = __shfl_xor_sync(0xffffffffu, bi, o);
@@ -810,17 +815,19 @@ __global__ void __launch_bounds__(256) select_gathered_kernel(const double* __re
         for (int w = 1; w < 8; ++w)
             if (sbest[w] > b || (sbest[w] == b && sidx[w] < i)) { b = sbest[w]; i = sidx[w]; r = srank[w]; }
         if (i == 0x7fffffffffffffffll) { i = 0; r = 0; }
-        const double* rr = g + (size_t)r * rec + M_pad;
-        for (int k = 0; k < 16; ++k) out20[k] = (float)rr[k];
-        out20[16] = (float)rr[16];
-        out20[17] = (float)sbad;
-        out20[18] = (float)i;
-        out20[19] = (float)r;
+        const ShardTail& t = *(const ShardTail*)(g + (size_t)r * rec + M_pad);
+        for (int k = 0; k < 16; ++k) out->pose[k] = (float)t.pose[k];
+        out->expert = (float)t.expert;
+        out->bad = (float)sbad;
+        out->winner = (float)i;
+        out->rank = (float)r;
     }
 }
 
-void launch_select_gathered(const double* gathered, int world, int M_pad, float* out20, cudaStream_t st) {
-    select_gathered_kernel<<<1, 256, 0, st>>>(gathered, world, M_pad, out20);
+#undef TAIL_AT
+
+void launch_select_gathered(const double* gathered, int world, int M_pad, ForwardRecord* rec, cudaStream_t st) {
+    select_gathered_kernel<<<1, 256, 0, st>>>(gathered, world, M_pad, rec);
 }
 
 void launch_finish_forward_async(const Pose* poses, const int* winner, const int* assign32, const int* flags, float* pose16,
@@ -832,9 +839,9 @@ void launch_seed_reset(unsigned long long* seed, unsigned long long base, cudaSt
     seed_reset_kernel<<<1, 1, 0, st>>>(seed, base);
 }
 
-void launch_finish_forward(const Pose* poses, const int* winner, const int* assign32, const int* flags, float* out20,
+void launch_finish_forward(const Pose* poses, const int* winner, const int* assign32, const int* flags, ForwardRecord* rec,
                            cudaStream_t st) {
-    finish_forward_kernel<<<1, 32, 0, st>>>(poses, winner, assign32, flags, out20);
+    finish_forward_kernel<<<1, 32, 0, st>>>(poses, winner, assign32, flags, rec);
 }
 
 }  // namespace esacb200

@@ -538,7 +538,7 @@ __global__ void __launch_bounds__(256) finish_scores_kernel(const float* __restr
 }
 
 __global__ void __launch_bounds__(1024) select_kernel(const float* __restrict__ part, const int* __restrict__ slot_of,
-                                                      Problem P, int T, double* scores, double* probs, double* stats,
+                                                      Problem P, int T, double* scores, double* probs, CallStats* stats,
                                                       int* winner, int* contrib, int* n_contrib) {
     __shared__ double sred[32];
     __shared__ int sidx[32];
@@ -594,8 +594,8 @@ __global__ void __launch_bounds__(1024) select_kernel(const float* __restrict__ 
         }
         if (i == 0x7fffffff) i = 0;
         *winner = i;
-        stats[0] = en; stats[1] = (double)i;
-        stats[5] = mx; stats[6] = sum;  // local softmax normalisation, for the multi-GPU exchange
+        stats->entropy = en; stats->winner = (double)i;
+        stats->max_score = mx; stats->sum_exp = sum;  // local softmax normalisation, for the multi-GPU exchange
         srun = 0;
     }
     __syncthreads();
@@ -613,11 +613,11 @@ __global__ void __launch_bounds__(1024) select_kernel(const float* __restrict__ 
         if (tid == 0) { int t = 0; for (int w = 0; w < nw; ++w) t += swc[w]; srun += t; }
         __syncthreads();
     }
-    if (tid == 0) { *n_contrib = srun; stats[2] = (double)srun; }
+    if (tid == 0) { *n_contrib = srun; stats->n_contrib = (double)srun; }
 }
 
 void launch_select(const float* part, const int* slot_of, const Problem& P, int T, double* scores, double* probs,
-                   double* stats, int* winner, int* contrib, int* n_contrib, cudaStream_t st) {
+                   CallStats* stats, int* winner, int* contrib, int* n_contrib, cudaStream_t st) {
     finish_scores_kernel<<<(P.M * 32 + 255) / 256, 256, 0, st>>>(part, slot_of, P, T, scores);
     select_kernel<<<1, 1024, 0, st>>>(part, slot_of, P, T, scores, probs, stats, winner, contrib, n_contrib);
 }

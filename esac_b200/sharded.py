@@ -21,6 +21,8 @@ from __future__ import annotations
 
 import numpy as np
 
+from . import api
+
 _NEG_INF = float("-inf")
 _lib_comm: dict = {}   # device index -> (world, rank) of the library communicator
 
@@ -30,7 +32,6 @@ def init_comm(group=None, device: int | None = None):
     ncclUniqueId, torch.distributed carries its 128 bytes to the others, every rank calls ncclCommInitRank."""
     import torch
     import torch.distributed as dist
-    from . import api
     if device is None:
         device = torch.cuda.current_device()
     world, rank = dist.get_world_size(group), dist.get_rank(group)
@@ -43,7 +44,6 @@ def init_comm(group=None, device: int | None = None):
 
 def destroy_comm(device: int | None = None):
     import torch
-    from . import api
     if device is None:
         device = torch.cuda.current_device()
     if device in _lib_comm:
@@ -60,19 +60,17 @@ def max_over_ranks(value: int, group=None, device=None) -> int:
     return max(int(t.item()), 1)
 
 
-PACK_TAIL = 21
-
-
 def pack_local(scores, pose16, expert_global: int, local_winner: int, M_pad: int | None = None, hyp_offset: int = 0,
                hyp_stride: int = 1):
-    """float64 record [M_pad + 21] (see the module docstring) from a local result."""
+    """float64 record [M_pad + api.PACK_TAIL] (see the module docstring) from a local result."""
     import torch
     scores = scores.reshape(-1).to(torch.float64)
     M = int(scores.numel())
     M_pad = M if M_pad is None else int(M_pad)
     pad = torch.full((M_pad - M,), _NEG_INF, dtype=torch.float64, device=scores.device)
     if M == 0:
-        tail = torch.tensor([-1.0] * 18 + [0.0, float(hyp_offset), float(hyp_stride)], dtype=torch.float64, device=scores.device)
+        tail = torch.tensor([-1.0] * api.TAIL_M + [0.0, float(hyp_offset), float(hyp_stride)], dtype=torch.float64,
+                            device=scores.device)
         return torch.cat([pad, tail])
     tail = torch.tensor([float(expert_global), float(local_winner), float(M), float(hyp_offset), float(hyp_stride)],
                         dtype=torch.float64, device=scores.device)
@@ -80,7 +78,7 @@ def pack_local(scores, pose16, expert_global: int, local_winner: int, M_pad: int
 
 
 def select_global(gathered: np.ndarray, M_pad: int):
-    """gathered: [world, M_pad + 21].  Returns (winner slot = rank * M_pad + local index, owning rank, pose 4x4 float32,
+    """gathered: [world, M_pad + api.PACK_TAIL].  Returns (winner slot = rank * M_pad + local index, owning rank, pose 4x4 float32,
     expert id, probabilities of all M_pad * world slots) with softMax / draw(training=false) semantics (esac_util.h:461-530):
     the first strict maximum in the hypothesis order of the unsharded problem; padded slots carry -inf and probability 0."""
     world = gathered.shape[0]
@@ -90,8 +88,10 @@ def select_global(gathered: np.ndarray, M_pad: int):
     probs = sf / sf.sum()
     # global index of every slot: hyp_offset + k * hyp_stride; draw() keeps the first maximum in that order
     k = np.arange(M_pad)[None, :]
-    gidx = (gathered[:, M_pad + 19:M_pad + 20] + k * np.maximum(gathered[:, M_pad + 20:M_pad + 21], 1)).reshape(-1)
-    gidx = np.where(k.repeat(world, 0).reshape(-1) < gathered[:, M_pad + 18].repeat(M_pad), gidx, np.inf)
+    tail = gathered[:, M_pad:]
+    offset, stride = tail[:, api.TAIL_HYP_OFFSET:api.TAIL_HYP_OFFSET + 1], tail[:, api.TAIL_HYP_STRIDE:api.TAIL_HYP_STRIDE + 1]
+    gidx = (offset + k * np.maximum(stride, 1)).reshape(-1)
+    gidx = np.where(k.repeat(world, 0).reshape(-1) < tail[:, api.TAIL_M].repeat(M_pad), gidx, np.inf)
     if probs.max() >= 1e-8:
         cand = np.flatnonzero(probs == probs.max())
         winner = int(cand[np.argmin(gidx[cand])])
@@ -99,8 +99,8 @@ def select_global(gathered: np.ndarray, M_pad: int):
         winner = 0
     rank = winner // M_pad
     assert rank < world
-    pose = gathered[rank, M_pad:M_pad + 16].reshape(4, 4).astype(np.float32)
-    expert = int(gathered[rank, M_pad + 16])
+    pose = tail[rank, api.TAIL_POSE:api.TAIL_EXPERT].reshape(4, 4).astype(np.float32)
+    expert = int(tail[rank, api.TAIL_EXPERT])
     return winner, rank, pose, expert, probs
 
 
@@ -139,7 +139,6 @@ def backward_sharded(coords_local, grads_local, assign_local, gt_pose, w_rot, w_
     `init_comm` was called for this device, else torch.distributed through the exchange callback.
     reduce_grads (library communicator only): hypothesis-major sharding -- every rank passes ALL planes and a slice of the
     hypotheses; the gradients are summed over the ranks (one ncclAllReduce) and added to grads_local on every rank."""
-    from . import api
     dev = _device_of(coords_local)
     if dev is None:
         dev = device
@@ -172,7 +171,6 @@ def forward_sharded(coords_local, assign_local, out_pose, params, expert_offset:
     (computed with one extra all-reduce when not given)."""
     import torch
     import torch.distributed as dist
-    from . import api
 
     M = int(assign_local.shape[0])
     dev = _device_of(coords_local)
@@ -198,7 +196,7 @@ def forward_sharded(coords_local, assign_local, out_pose, params, expert_offset:
         ctx = api.context(tdev.index)
         ctx.set_option("hyp_offset", hyp_offset)
         ctx.set_option("hyp_stride", hyp_stride)
-        buf = torch.empty(M_pad + PACK_TAIL, dtype=torch.float64, device=tdev)
+        buf = torch.empty(M_pad + api.PACK_TAIL, dtype=torch.float64, device=tdev)
         try:
             if M > 0:
                 api.forward_pack(coords_local, assign_local, params, expert_offset, buf, M_pad=M_pad)   # enqueued, no host sync
@@ -216,24 +214,24 @@ def forward_sharded(coords_local, assign_local, out_pose, params, expert_offset:
         else:
             buf = pack_local(torch.empty(0, dtype=torch.float64), None, -1, 0, M_pad, hyp_offset, hyp_stride)
     world = dist.get_world_size(group)
-    rec = M_pad + PACK_TAIL
+    rec = M_pad + api.PACK_TAIL
     gathered = torch.empty(world * rec, dtype=torch.float64, device=buf.device)
     dist.all_gather_into_tensor(gathered, buf, group=group)
     g = gathered.view(world, rec)
     if g.is_cuda:
         # selection on the device: first maximum = draw(training=false) -- in rank-major order, which is the order of the
         # unsharded problem for contiguous shards (this fallback transport does not support hyp_stride > 1 tie-breaking);
-        # ONE 17-value read-back (the only host sync of the step)
+        # ONE read-back of the winner's pose and expert (the only host sync of the step)
         w = torch.argmax(g[:, :M_pad].reshape(-1))
-        tail = g.reshape(-1)[(w // M_pad) * rec + M_pad + torch.arange(17, device=g.device)]
+        tail = g.reshape(-1)[(w // M_pad) * rec + M_pad + torch.arange(api.TAIL_WINNER, device=g.device)]
         if hasattr(out_pose, "is_cuda") and out_pose.is_cuda:
-            out_pose.copy_(tail[:16].reshape(4, 4))
-            expert = int(tail[16].item())
+            out_pose.copy_(tail[api.TAIL_POSE:api.TAIL_EXPERT].reshape(4, 4))
+            expert = int(tail[api.TAIL_EXPERT].item())
             if expert < 0:
                 raise RuntimeError("hypAssignment holds an expert index outside the shard's experts")
             return expert
         small = tail.cpu().numpy()
-        gpose, expert = small[:16].reshape(4, 4).astype(np.float32), int(small[16])
+        gpose, expert = small[api.TAIL_POSE:api.TAIL_EXPERT].reshape(4, 4).astype(np.float32), int(small[api.TAIL_EXPERT])
         if expert < 0:
             raise RuntimeError("hypAssignment holds an expert index outside the shard's experts")
     else:

@@ -152,6 +152,12 @@ def load_library() -> C.CDLL:
     lib.esacb200_hypotheses_backward_async.restype = i32
     lib.esacb200_pose_loss_async.argtypes = [vp, i32, i32, vp, vp, f32, f32, f32, vp, vp]
     lib.esacb200_pose_loss_async.restype = i32
+    lib.esacb200_reproj_loss_async.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, i32, f32, f32, f32, vp, vp]
+    lib.esacb200_reproj_loss_async.restype = i32
+    lib.esacb200_coord_loss_async.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp, f32, vp, vp]
+    lib.esacb200_coord_loss_async.restype = i32
+    lib.esacb200_reserve_loss_async.argtypes = [vp, i32, i32, i32]
+    lib.esacb200_reserve_loss_async.restype = i32
     lib.esacb200_reserve_backward_async.restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
@@ -1364,6 +1370,110 @@ def pose_loss_async(poses, gtPose, wLossRot, wLossTrans, lossCut, outLosses=None
     ctx.check(ctx.lib.esacb200_pose_loss_async(ctx.handle, B, M, poses.data_ptr(), gtPose.data_ptr(), float(wLossRot),
                                                float(wLossTrans), float(lossCut), outLosses.data_ptr(), outDloss.data_ptr()))
     return outLosses, outDloss
+
+
+def _loss_images(t, what: str, call: str, writable: bool = False, like: _Images | None = None) -> _Images:
+    """An image argument of the stream-ordered losses: torch tensors only, each contiguous (a copy would not be captured
+    with the call); then _Images' dtype, rank and shape checks.  Raises before any context exists."""
+    parts = list(enumerate(t)) if _is_list(t) else [(None, t)]
+    for b, x in parts:
+        name = what if b is None else f"{what}[{b}]"
+        if not _is_torch(x):
+            raise RuntimeError(f"{call} takes torch CUDA tensors only ({name} is a {type(x).__name__})")
+    im = _Images(t, 3, what, writable=writable, like=like)
+    for b, x in parts:
+        if not x.is_contiguous():
+            name = what if b is None else f"{what}[{b}]"
+            raise RuntimeError(f"{name} must be contiguous (a copy would not be captured with the call)")
+    return im
+
+
+def _loss_async_context(call: str, images, fixed: dict) -> Context:
+    """The checks the stream-ordered losses share after their image arguments: every `fixed` argument (name -> (tensor,
+    dtype, shape)) is a contiguous torch tensor of that shape; then every tensor is a CUDA tensor of one device.  Returns
+    the context, on torch's current stream."""
+    for what, (t, dt, shape) in fixed.items():
+        if not _is_torch(t):
+            raise RuntimeError(f"{call} takes torch CUDA tensors only ({what} is a {type(t).__name__})")
+        _check(t, dt, len(shape), what)
+        if tuple(int(v) for v in t.shape) != shape or not t.is_contiguous():
+            raise RuntimeError(f"{what} must be a contiguous {list(shape)} tensor, got {list(t.shape)}")
+    tensors = [(im.what, a.orig) for im in images for a in im.args] + [(what, t) for what, (t, _, _) in fixed.items()]
+    for what, t in tensors:
+        if not t.is_cuda:
+            raise RuntimeError(f"{call} takes CUDA tensors only ({what} is on the CPU)")
+    devs = {t.device.index for _, t in tensors}
+    if len(devs) > 1:
+        raise RuntimeError(f"esac_b200: tensors live on different CUDA devices {sorted(devs)}")
+    ctx = _pick_ctx(*devs)
+    ctx.async_used = True
+    return ctx
+
+
+def reproj_loss_async(prediction, gtPoses, shifts, cameras, cutLoss, subSampling, outLosses, outStatus, outGradients=None,
+                      maxReproj=100.0, minDepth=0.1):
+    """reproj_loss enqueued on torch's current stream with no host synchronisation, so that a ref_expert.py step can be
+    captured in a CUDA graph.  CUDA tensors only: prediction float32 [B,3,H,W] or a list / tuple of B [3,H_b,W_b] tensors,
+    gtPoses float32 [B,4,4] camera->world, shifts int32 [B,2] (padX, padY), cameras float32 [B,3] (focal length, ppointX,
+    ppointY), all read on the device when the kernels run (the image pointers and sizes are fixed by a capture).
+    outGradients (the prediction's form and shapes, overwritten) or None; outLosses float64 [B] and outStatus int32 [B]
+    receive, bitwise, reproj_loss's losses and 0, or for an image whose ground-truth rotation is singular or NaN (where
+    reproj_loss raises) a NaN loss, a zero gradient and status 1.  Call reserve_loss_async with the largest batch and map
+    before the first capture."""
+    call = "reproj_loss_async"
+    pr = _loss_images(prediction, "prediction", call)
+    B = pr.B
+    og = None
+    if outGradients is not None:
+        og = _loss_images(outGradients, "outGradients", call, writable=True, like=pr)
+        og.require_shapes_of(pr)
+    ctx = _loss_async_context(call, [pr] + ([og] if og else []),
+                              {"gtPoses": (gtPoses, "Float", (B, 4, 4)), "shifts": (shifts, "Int", (B, 2)),
+                               "cameras": (cameras, "Float", (B, 3)), "outLosses": (outLosses, "Double", (B,)),
+                               "outStatus": (outStatus, "Int", (B,))})
+    ctx.check(ctx.lib.esacb200_reproj_loss_async(ctx.handle, B, pr.ptrs, og.ptrs if og else None, pr.hs, pr.ws,
+                                                 gtPoses.data_ptr(), shifts.data_ptr(), cameras.data_ptr(), int(subSampling),
+                                                 float(cutLoss), float(maxReproj), float(minDepth), outLosses.data_ptr(),
+                                                 outStatus.data_ptr()))
+
+
+def coord_loss_async(prediction, gtCoords, cutLoss, outLosses, outGradients=None, outCounts=None):
+    """coord_loss enqueued on torch's current stream with no host synchronisation, so that an init_expert.py step can be
+    captured in a CUDA graph.  CUDA tensors only: prediction float32 [B,3,Hp,Wp] and gtCoords float32 [B,3,Hg,Wg] (at most
+    1 apart in H and W), or both lists / tuples of B [3,H_b,W_b] tensors; outGradients (the prediction's form and shapes,
+    overwritten) or None.  outLosses float64 [B] and outCounts int64 [B] (or None) receive, bitwise, coord_loss's losses
+    and valid-cell counts.  The maps are read on the device when the kernels run (their pointers and sizes are fixed by a
+    capture).  Call reserve_loss_async with the largest batch and map before the first capture."""
+    call = "coord_loss_async"
+    pr = _loss_images(prediction, "prediction", call)
+    gt = _loss_images(gtCoords, "gtCoords", call, like=pr)
+    for b, ((_, hp, wp), (_, hg, wg)) in enumerate(zip(pr.shapes, gt.shapes)):
+        if abs(hp - hg) > 1 or abs(wp - wg) > 1:
+            raise RuntimeError(f"image {b}: tensor size mismatch: prediction {hp}x{wp}, ground truth {hg}x{wg} "
+                               "(util.assert_size allows 1)")
+    og = None
+    if outGradients is not None:
+        og = _loss_images(outGradients, "outGradients", call, writable=True, like=pr)
+        og.require_shapes_of(pr)
+    fixed = {"outLosses": (outLosses, "Double", (pr.B,))}
+    if outCounts is not None:
+        fixed["outCounts"] = (outCounts, "Long", (pr.B,))
+    ctx = _loss_async_context(call, [pr, gt] + ([og] if og else []), fixed)
+    ctx.check(ctx.lib.esacb200_coord_loss_async(ctx.handle, pr.B, pr.ptrs, pr.hs, pr.ws, gt.ptrs, gt.hs, gt.ws,
+                                                og.ptrs if og else None, float(cutLoss), outLosses.data_ptr(),
+                                                outCounts.data_ptr() if outCounts is not None else None))
+
+
+def reserve_loss_async(B: int, H: int, W: int, device: int | None = None):
+    """Sizes the workspace of reproj_loss_async and coord_loss_async for B images of at most H x W cells (the prediction's);
+    call it before capturing (it allocates)."""
+    if min(int(B), int(H), int(W)) < 1:
+        raise RuntimeError(f"reserve_loss_async: sizes must be positive, got B={B} H={H} W={W}")
+    ctx = context(device)
+    import torch
+    ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
+    ctx.async_used = True
+    ctx.check(ctx.lib.esacb200_reserve_loss_async(ctx.handle, int(B), int(H), int(W)))
 
 
 def set_seed(seed: int, device: int | None = None):

@@ -237,6 +237,84 @@ def coord_loss(prediction, gt_coords, cut_loss=100.0):
     return CoordLoss.apply((form, gt_coords, cut_loss), *inputs)
 
 
+def _batch_mean(losses):
+    """sum(losses) / len(losses) of ReprojLoss / CoordLoss taken on the device: the float64 losses added left to right, then
+    one float64 division (by a tensor: torch multiplies by the reciprocal of a Python divisor), rounded to float32 as
+    new_tensor rounds it.  No host synchronisation."""
+    total = losses[0]
+    for b in range(1, losses.shape[0]):
+        total = total + losses[b]
+    return (total / torch.full((), float(losses.shape[0]), dtype=torch.float64, device=losses.device)).float()
+
+
+class ReprojLossAsync(torch.autograd.Function):
+    """ReprojLoss on api.reproj_loss_async: no host synchronisation in the forward or the backward, so the node, and
+    loss.backward() through it, can be captured in a CUDA graph.  The predictions come last (_as_inputs)."""
+
+    @staticmethod
+    def forward(ctx, meta, *prediction):
+        form, gt_poses, shifts, cameras, cut_loss, sub_sampling, max_reproj, min_depth, status = meta
+        grads = [torch.empty_like(p) for p in prediction]
+        B = len(prediction) if form is list else prediction[0].shape[0]
+        dev = prediction[0].device
+        losses = torch.empty(B, dtype=torch.float64, device=dev)
+        if status is None:
+            status = torch.empty(B, dtype=torch.int32, device=dev)
+        api.reproj_loss_async(form([p.detach() for p in prediction]), gt_poses, shifts, cameras, cut_loss, sub_sampling, losses,
+                              status, outGradients=form(grads), maxReproj=max_reproj, minDepth=min_depth)
+        ctx.save_for_backward(*grads)
+        ctx.batch = B
+        return _batch_mean(losses)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        return (None,) + tuple(g * (grad_out / ctx.batch) for g in ctx.saved_tensors)
+
+
+def reproj_loss_async(prediction, gt_poses, shifts, cameras, cut_loss, sub_sampling=8, max_reproj=100.0, min_depth=0.1,
+                      status=None):
+    """reproj_loss for training steps captured in a CUDA graph (ref_expert.py as one graph): CUDA tensors only, prediction
+    [B,3,H,W] or a list / tuple of B [3,H_b,W_b] tensors, gt_poses float32 [B,4,4] camera->world, shifts int32 [B,2] (padX,
+    padY), cameras float32 [B,3] (focal length, ppointX, ppointY), all read on the device at replay time.  The loss (the
+    batch mean, float32) and the gradients are bitwise those of reproj_loss.  status: an int32 CUDA tensor [B] that receives
+    the per-image status (1 = a singular ground truth: that loss is NaN, its gradient zero); None keeps it internal.  Call
+    api.reserve_loss_async with the largest batch and map before the first capture."""
+    inputs, form = _as_inputs(prediction)
+    meta = (form, gt_poses, shifts, cameras, cut_loss, sub_sampling, max_reproj, min_depth, status)
+    return ReprojLossAsync.apply(meta, *inputs)
+
+
+class CoordLossAsync(torch.autograd.Function):
+    """CoordLoss on api.coord_loss_async: no host synchronisation in the forward or the backward, so the node, and
+    loss.backward() through it, can be captured in a CUDA graph.  The predictions come last (_as_inputs)."""
+
+    @staticmethod
+    def forward(ctx, meta, *prediction):
+        form, gt_coords, cut_loss, counts = meta
+        grads = [torch.empty_like(p) for p in prediction]
+        B = len(prediction) if form is list else prediction[0].shape[0]
+        losses = torch.empty(B, dtype=torch.float64, device=prediction[0].device)
+        api.coord_loss_async(form([p.detach() for p in prediction]), gt_coords, cut_loss, losses, outGradients=form(grads),
+                             outCounts=counts)
+        ctx.save_for_backward(*grads)
+        ctx.batch = B
+        return _batch_mean(losses)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        return (None,) + tuple(g * (grad_out / ctx.batch) for g in ctx.saved_tensors)
+
+
+def coord_loss_async(prediction, gt_coords, cut_loss=100.0, counts=None):
+    """coord_loss for training steps captured in a CUDA graph (init_expert.py as one graph): CUDA tensors only, prediction
+    [B,3,Hp,Wp] and gt_coords [B,3,Hg,Wg], or both lists / tuples of B [3,H_b,W_b] tensors, read on the device at replay
+    time.  The loss (the batch mean, float32) and the gradients are bitwise those of coord_loss.  counts: an int64 CUDA
+    tensor [B] that receives the valid cells per image, or None.  Call api.reserve_loss_async with the largest batch and
+    map before the first capture."""
+    inputs, form = _as_inputs(prediction)
+    return CoordLossAsync.apply((form, gt_coords, cut_loss, counts), *inputs)
+
+
 # ------------------------------------------------------------------------------------------------
 # The hypotheses as an autograd node: any pose loss written in torch
 # ------------------------------------------------------------------------------------------------

@@ -146,6 +146,11 @@ struct esacb200_ctx {
     bool is_async = false;
     bool frozen = false;
     DevBuf seed_state;
+    // The stream-ordered losses' workspace (esacb200_reproj_loss_async / _coord_loss_async), in the async context: apart from
+    // the forward's and the backward's, so that loss graphs and ESAC graphs do not size each other's buffers; loss_frozen
+    // once a capture has used it.
+    DevBuf loss_ws;
+    bool loss_frozen = false;
 };
 
 namespace {
@@ -2480,27 +2485,10 @@ int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* co
     }
     // world->camera rows: inverse of the affine camera->world matrix (torch's .inverse()[0:3,:], ref_expert.py:127)
     std::vector<float> img((size_t)B * kReprojImgFloats, 0.f);
-    for (int b = 0; b < B; ++b) {
-        const float* T = gt.data() + (size_t)b * 16;
-        double A[9], inv[9];
-        for (int r = 0; r < 3; ++r)
-            for (int c = 0; c < 3; ++c) A[r * 3 + c] = T[r * 4 + c];
-        const double det = A[0] * (A[4] * A[8] - A[5] * A[7]) - A[1] * (A[3] * A[8] - A[5] * A[6]) + A[2] * (A[3] * A[7] - A[4] * A[6]);
-        if (det == 0. || !(det == det)) return fail(ctx, ESACB200_ERR_ARG, "image %d: ground-truth pose is singular", b);
-        inv[0] = (A[4] * A[8] - A[5] * A[7]) / det; inv[1] = (A[2] * A[7] - A[1] * A[8]) / det; inv[2] = (A[1] * A[5] - A[2] * A[4]) / det;
-        inv[3] = (A[5] * A[6] - A[3] * A[8]) / det; inv[4] = (A[0] * A[8] - A[2] * A[6]) / det; inv[5] = (A[2] * A[3] - A[0] * A[5]) / det;
-        inv[6] = (A[3] * A[7] - A[4] * A[6]) / det; inv[7] = (A[1] * A[6] - A[0] * A[7]) / det; inv[8] = (A[0] * A[4] - A[1] * A[3]) / det;
-        float* o = img.data() + (size_t)b * kReprojImgFloats;
-        for (int r = 0; r < 3; ++r) {
-            for (int c = 0; c < 3; ++c) o[r * 4 + c] = (float)inv[r * 3 + c];
-            o[r * 4 + 3] = (float)-(inv[r * 3] * T[3] + inv[r * 3 + 1] * T[7] + inv[r * 3 + 2] * T[11]);
-        }
-        o[12] = shiftX ? (float)shiftX[b] : 0.f;
-        o[13] = shiftY ? (float)shiftY[b] : 0.f;
-        o[14] = f[b];
-        o[15] = ppx[b];
-        o[16] = ppy[b];
-    }
+    for (int b = 0; b < B; ++b)
+        if (!reproj_img_row(gt.data() + (size_t)b * 16, shiftX ? shiftX[b] : 0, shiftY ? shiftY[b] : 0, f[b], ppx[b], ppy[b],
+                            img.data() + (size_t)b * kReprojImgFloats))
+            return fail(ctx, ESACB200_ERR_ARG, "image %d: ground-truth pose is singular", b);
     std::vector<ReprojImage> recs((size_t)B);
     std::vector<char> vec((size_t)B);
     long long parts = 0;
@@ -2685,6 +2673,225 @@ int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int
     const std::vector<int> hp((size_t)B, Hp), wp((size_t)B, Wp), hg((size_t)B, Hg), wg((size_t)B, Wg);
     return esacb200_coord_loss_ragged(ctx, B, pp.data(), hp.data(), wp.data(), qp.data(), hg.data(), wg.data(),
                                       grads ? gp.data() : nullptr, cut, out_losses, out_counts);
+} ESAC_ABI_CATCH(ctx)
+
+// -------------------------------------------------------------------------------------------------
+// Stream-ordered losses.  The eager ragged calls' records and launches, run in the context ctx->async on the caller's device
+// arrays: the records reach the workspace as prep-kernel parameters (loss_async.cu), the ground truth, pads and camera are
+// read on the device, and a finish kernel writes the caller's outputs.  Nothing here synchronises, reads back or queries an
+// event, and a call that a capture records allocates nothing.
+
+static size_t align64(size_t n) { return (n + 63) & ~(size_t)63; }
+
+// Byte offsets in the loss workspace of a call of B images whose blocks have `parts` partials.
+//   reprojection: [tickets B u32] [img B x kReprojImgFloats f32] [records] [losses B f64] [bad B i32] [partials f64 each]
+//   coordinates:  [tickets B u32 | counts B u32] [records] [losses B f64] [valid counts B i64] [partials 2 f64 each]
+struct LossLayout {
+    size_t img = 0, rec, loss, flags, part, end;
+};
+static LossLayout reproj_layout(int B, long long parts) {
+    LossLayout L;
+    L.img = align64((size_t)B * 4);
+    L.rec = L.img + align64((size_t)B * kReprojImgFloats * sizeof(float));
+    L.loss = L.rec + align64((size_t)B * sizeof(ReprojImage));
+    L.flags = L.loss + align64((size_t)B * 8);
+    L.part = L.flags + align64((size_t)B * 4);
+    L.end = L.part + (size_t)parts * 8;
+    return L;
+}
+static LossLayout coord_layout(int B, long long parts) {
+    LossLayout L;
+    L.rec = align64((size_t)B * 8);
+    L.loss = L.rec + align64((size_t)B * sizeof(CoordImage));
+    L.flags = L.loss + align64((size_t)B * 8);
+    L.part = L.flags + align64((size_t)B * 8);
+    L.end = L.part + (size_t)parts * 2 * 8;
+    return L;
+}
+
+// Makes the loss workspace hold `bytes`: grows it when no capture has used it yet, else fails without touching it.
+static int loss_workspace(esacb200_ctx* ctx, esacb200_ctx* a, size_t bytes, bool capturing, const char* what) {
+    if (bytes <= a->loss_ws.cap) return 0;
+    if (capturing || a->loss_frozen)
+        return fail(ctx, ESACB200_ERR_ARG,
+                    "%s: this call needs %zu bytes of loss workspace, more than %s, and a graph that holds it may still be "
+                    "replayed; call reserve_loss_async (esacb200_reserve_loss_async) with the largest batch and map before the "
+                    "first capture", what, bytes, capturing ? "was reserved before this capture" : "an earlier capture used");
+    CK(a->loss_ws.ensure(bytes));
+    return 0;
+}
+
+// The n named arguments are device memory (a null one is an error unless `optional` has its bit set).
+static int device_args(esacb200_ctx* ctx, const char* what, int n, const void* const* ptrs, const char* const* names, unsigned optional = 0) {
+    for (int i = 0; i < n; ++i) {
+        if (!ptrs[i]) {
+            if (optional >> i & 1) continue;
+            return fail(ctx, ESACB200_ERR_ARG, "%s: %s is null", what, names[i]);
+        }
+        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "%s takes device pointers only: %s is host memory", what, names[i]);
+    }
+    return 0;
+}
+
+// The B image pointers of one argument are device memory.
+static int device_images(esacb200_ctx* ctx, const char* what, const char* name, const void* const* p, int B) {
+    for (int b = 0; b < B; ++b) {
+        if (!p[b]) return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: %s is null", what, b, name);
+        if (!is_device_ptr(p[b]))
+            return fail(ctx, ESACB200_ERR_ARG, "%s takes device pointers only: image %d: %s is host memory", what, b, name);
+    }
+    return 0;
+}
+
+// The async context of a loss call, and whether the stream is being captured.
+static int begin_loss_async(esacb200_ctx* ctx, esacb200_ctx*& a, bool& capturing) {
+    int rc = stream_capturing(ctx, capturing);
+    if (!rc) rc = async_context(ctx, capturing, "loss_async", &a);
+    return rc;
+}
+
+int esacb200_reserve_loss_async(esacb200_ctx* ctx, int B, int H, int W) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    if (B <= 0 || H <= 0 || W <= 0 || (long long)H * W > (1ll << 30))
+        return fail(ctx, ESACB200_ERR_ARG, "reserve_loss_async: bad sizes B=%d H=%d W=%d", B, H, W);
+    bool capturing = false;
+    int rc = stream_capturing(ctx, capturing);
+    if (rc) return rc;
+    if (capturing) return fail(ctx, ESACB200_ERR_ARG, "reserve_loss_async allocates: call it before the capture");
+    esacb200_ctx* a = nullptr;
+    rc = async_context(ctx, false, "loss_async", &a);
+    if (rc) return rc;
+    const long long parts = (long long)B * reproj_max_blocks(H * W);
+    return loss_workspace(ctx, a, std::max(reproj_layout(B, parts).end, coord_layout(B, parts).end), false, "reserve_loss_async");
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_reproj_loss_async(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H,
+                               const int* W, const float* gt_poses, const int32_t* shifts, const float* cameras, int sub,
+                               float cut, float maxReproj, float minDepth, double* out_losses, int32_t* out_status) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    const char* what = "reproj_loss_async";
+    if (!coords || !H || !W) return fail(ctx, ESACB200_ERR_ARG, "%s: null pointer or size array", what);
+    if (B <= 0 || B > 65535 || sub <= 0) return fail(ctx, ESACB200_ERR_ARG, "%s: bad sizes B=%d sub=%d", what, B, sub);
+    for (int b = 0; b < B; ++b) {
+        if (H[b] <= 0 || W[b] <= 0) return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: bad size %dx%d", what, b, W[b], H[b]);
+        if ((long long)H[b] * W[b] > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: map %dx%d too large", what, b, W[b], H[b]);
+    }
+    const void* ptrs[] = {gt_poses, shifts, cameras, out_losses, out_status};
+    const char* names[] = {"gt_poses", "shifts", "cameras", "out_losses", "out_status"};
+    int rc = device_args(ctx, what, 5, ptrs, names);
+    if (!rc) rc = device_images(ctx, what, "coords", (const void* const*)coords, B);
+    if (!rc && grads) rc = device_images(ctx, what, "grads", (const void* const*)grads, B);
+    if (rc) return rc;
+    esacb200_ctx* a = nullptr;
+    bool capturing = false;
+    if ((rc = begin_loss_async(ctx, a, capturing))) return rc;
+    std::vector<ReprojImage> recs((size_t)B), ordered;
+    std::vector<char> vec((size_t)B);
+    long long parts = 0;
+    for (int b = 0; b < B; ++b) {
+        ReprojImage& r = recs[b];
+        r.coords = coords[b];
+        r.grads = grads ? grads[b] : nullptr;
+        r.N = H[b] * W[b];
+        r.W = W[b];
+        r.b = b;
+        r.blocks = reproj_blocks_per_image(r.N);
+        r.part0 = parts;
+        parts += r.blocks;
+        vec[b] = reproj_vec_ok(r.coords, r.grads, r.N, r.W);
+    }
+    int n_vec, max_vec, max_sc;
+    order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
+    const LossLayout L = reproj_layout(B, parts);
+    if ((rc = loss_workspace(ctx, a, L.end, capturing, what))) return rc;
+    if (capturing) a->loss_frozen = true;
+    char* base = (char*)a->loss_ws.p;
+    ReprojImage* d_rec = (ReprojImage*)(base + L.rec);
+    float* img = (float*)(base + L.img);
+    double* losses = (double*)(base + L.loss);
+    int* bad = (int*)(base + L.flags);
+    CK(cudaMemsetAsync(base, 0, L.img, a->stream));
+    a->st.kernel_launches += launch_reproj_prep(ordered.data(), B, d_rec, gt_poses, shifts, cameras, img, bad, a->stream);
+    for (int path = 0; path < 2; ++path) {
+        const int n = path == 0 ? n_vec : B - n_vec;
+        if (n == 0) continue;
+        launch_reproj(path == 0, d_rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, img, (float)sub, cut, maxReproj,
+                      minDepth, (double*)(base + L.part), (unsigned*)base, losses, a->stream);
+        a->st.kernel_launches += 1;
+    }
+    launch_reproj_finish(d_rec, B, grads != nullptr, losses, bad, out_losses, out_status, a->stream);
+    a->st.kernel_launches += 1;
+    CK(cudaGetLastError());
+    return ESACB200_OK;
+} ESAC_ABI_CATCH(ctx)
+
+int esacb200_coord_loss_async(esacb200_ctx* ctx, int B, const float* const* pred, const int* Hp, const int* Wp,
+                              const float* const* gt, const int* Hg, const int* Wg, float* const* grads, float cut,
+                              double* out_losses, int64_t* out_counts) try {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    const char* what = "coord_loss_async";
+    if (!pred || !gt || !Hp || !Wp || !Hg || !Wg) return fail(ctx, ESACB200_ERR_ARG, "%s: null pointer or size array", what);
+    if (B <= 0 || B > 65535) return fail(ctx, ESACB200_ERR_ARG, "%s: bad sizes B=%d", what, B);
+    for (int b = 0; b < B; ++b) {
+        if (Hp[b] <= 0 || Wp[b] <= 0 || Hg[b] <= 0 || Wg[b] <= 0)
+            return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: bad sizes prediction %dx%d ground truth %dx%d", what, b, Hp[b], Wp[b],
+                        Hg[b], Wg[b]);
+        if (abs(Hp[b] - Hg[b]) > 1 || abs(Wp[b] - Wg[b]) > 1)   // util.assert_size tolerates 1 cell
+            return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: size mismatch: prediction %dx%d, ground truth %dx%d (at most 1 apart)",
+                        what, b, Hp[b], Wp[b], Hg[b], Wg[b]);
+        if ((long long)Hp[b] * Wp[b] > (1ll << 30) || (long long)Hg[b] * Wg[b] > (1ll << 30))
+            return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: map too large", what, b);
+    }
+    const void* ptrs[] = {out_losses, out_counts};
+    const char* names[] = {"out_losses", "out_counts"};
+    int rc = device_args(ctx, what, 2, ptrs, names, 2u);
+    if (!rc) rc = device_images(ctx, what, "pred", (const void* const*)pred, B);
+    if (!rc) rc = device_images(ctx, what, "gt", (const void* const*)gt, B);
+    if (!rc && grads) rc = device_images(ctx, what, "grads", (const void* const*)grads, B);
+    if (rc) return rc;
+    esacb200_ctx* a = nullptr;
+    bool capturing = false;
+    if ((rc = begin_loss_async(ctx, a, capturing))) return rc;
+    std::vector<CoordImage> recs((size_t)B), ordered;
+    std::vector<char> vec((size_t)B);
+    long long parts = 0;
+    for (int b = 0; b < B; ++b) {
+        CoordImage& r = recs[b];
+        r.pred = pred[b];
+        r.gt = gt[b];
+        r.grads = grads ? grads[b] : nullptr;
+        vec[b] = coord_image(r, Hp[b], Wp[b], Hg[b], Wg[b]);
+        r.b = b;
+        r.part0 = parts;
+        parts += r.blocks;
+    }
+    int n_vec, max_vec, max_sc;
+    order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
+    const LossLayout L = coord_layout(B, parts);
+    if ((rc = loss_workspace(ctx, a, L.end, capturing, what))) return rc;
+    if (capturing) a->loss_frozen = true;
+    char* base = (char*)a->loss_ws.p;
+    CoordImage* d_rec = (CoordImage*)(base + L.rec);
+    double* losses = (double*)(base + L.loss);
+    long long* counts = (long long*)(base + L.flags);
+    CK(cudaMemsetAsync(base, 0, L.rec, a->stream));
+    a->st.kernel_launches += launch_coord_prep(ordered.data(), B, d_rec, a->stream);
+    for (int path = 0; path < 2; ++path) {
+        const int n = path == 0 ? n_vec : B - n_vec;
+        if (n == 0) continue;
+        for (int pass = grads ? 1 : 2; pass <= 2; ++pass) {
+            launch_coord_loss(path == 0, pass, grads != nullptr, d_rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, cut,
+                              (unsigned*)base + B, (double*)(base + L.part), (unsigned*)base, losses, counts, a->stream);
+            a->st.kernel_launches += 1;
+        }
+    }
+    launch_coord_finish(B, losses, counts, out_losses, (long long*)out_counts, a->stream);
+    a->st.kernel_launches += 1;
+    CK(cudaGetLastError());
+    return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 
 // The getters below read only what the last call on the context wrote (LastCall).

@@ -373,6 +373,65 @@ constexpr int kReprojImgFloats = 20;
 void launch_reproj(bool vec, const ReprojImage* recs, int n, int max_blocks, const float* img, float sub, float cut,
                    float max_err, float min_depth, double* partial, unsigned* tickets, double* losses, cudaStream_t stream);
 
+// fp64 products and sums rounded once each, on both sides: nvcc would contract a*b - c*d into an FMA, the host compiler
+// (no -march) does not, and the reprojection loss's ground-truth inversion must round alike on the host and the device.
+ESAC_HD double mul_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+ESAC_HD double add_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+ESAC_HD double sub_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dsub_rn(a, b);
+#else
+    return a - b;
+#endif
+}
+ESAC_HD double div_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __ddiv_rn(a, b);
+#else
+    return a / b;
+#endif
+}
+
+// One image's row of the reprojection loss's `img` table (kReprojImgFloats floats): the world->camera 3x4 inverse of the
+// affine camera->world ground truth T [4,4] (torch's .inverse()[0:3,:], ref_expert.py:127; adjugate over determinant),
+// then padX, padY, f, cx, cy.  Returns false, with o untouched, when the rotation block is singular or NaN (det == 0 or
+// det != det).  The eager call runs it on the host, the stream-ordered call on the device: bitwise the same row.
+ESAC_HD bool reproj_img_row(const float* T, int padX, int padY, float f, float cx, float cy, float* o) {
+    double A[9], inv[9];
+    for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) A[r * 3 + c] = T[r * 4 + c];
+    // cofactor (i,j,k,l) = A[i] * A[j] - A[k] * A[l]
+    auto cof = [&](int i, int j, int k, int l) { return sub_rn(mul_rn(A[i], A[j]), mul_rn(A[k], A[l])); };
+    const double det = add_rn(sub_rn(mul_rn(A[0], cof(4, 8, 5, 7)), mul_rn(A[1], cof(3, 8, 5, 6))), mul_rn(A[2], cof(3, 7, 4, 6)));
+    if (det == 0. || !(det == det)) return false;
+    inv[0] = div_rn(cof(4, 8, 5, 7), det); inv[1] = div_rn(cof(2, 7, 1, 8), det); inv[2] = div_rn(cof(1, 5, 2, 4), det);
+    inv[3] = div_rn(cof(5, 6, 3, 8), det); inv[4] = div_rn(cof(0, 8, 2, 6), det); inv[5] = div_rn(cof(2, 3, 0, 5), det);
+    inv[6] = div_rn(cof(3, 7, 4, 6), det); inv[7] = div_rn(cof(1, 6, 0, 7), det); inv[8] = div_rn(cof(0, 4, 1, 3), det);
+    for (int r = 0; r < 3; ++r) {
+        for (int c = 0; c < 3; ++c) o[r * 4 + c] = (float)inv[r * 3 + c];
+        const double t = add_rn(add_rn(mul_rn(inv[r * 3], T[3]), mul_rn(inv[r * 3 + 1], T[7])), mul_rn(inv[r * 3 + 2], T[11]));
+        o[r * 4 + 3] = (float)-t;
+    }
+    o[12] = (float)padX;
+    o[13] = (float)padY;
+    o[14] = f;
+    o[15] = cx;
+    o[16] = cy;
+    return true;
+}
+
 // --- coord_loss.cu ------------------------------------------------------------------------
 // One image of a coordinate-loss launch: pred [3,Hp,Wp], gt [3,Hg,Wg] (|Hp-Hg|, |Wp-Wg| <= 1, checked by the caller),
 // grads [3,Hp,Wp] overwritten or null (loss only).  blocks = reproj_blocks_per_image(Np), partials part0 .. part0 + blocks
@@ -399,6 +458,28 @@ bool coord_image(CoordImage& r, int Hp, int Wp, int Hg, int Wg);
 void launch_coord_loss(bool vec, int pass, bool grad, const CoordImage* recs, int n, int max_blocks, float cut,
                        unsigned* counts, double* partial, unsigned* tickets, double* losses, long long* out_counts,
                        cudaStream_t stream);
+// The largest reproj_blocks_per_image(n) over n <= N (the count is not monotonic in N): the partials that a workspace for
+// maps of at most N cells must hold per image.
+int reproj_max_blocks(int N);
+
+// --- loss_async.cu ------------------------------------------------------------------------
+// Records per prep-kernel launch of the stream-ordered losses: they travel as a kernel parameter, under the 4 KB limit.
+constexpr size_t kLossChunkBytes = 3072;
+template <class Rec> constexpr int loss_chunk() { return (int)(kLossChunkBytes / sizeof(Rec)); }
+// The n host records (ordered by load path) into recs, in chunks; record i's image b gets its row of img from gt16 [B,4,4]
+// camera->world, shifts [B,2] and cameras [B,3] (device), and bad[b] = 1 (and no blocks) when its rotation block is
+// singular or NaN.  Returns the launches.
+int launch_reproj_prep(const ReprojImage* host_recs, int n, ReprojImage* recs, const float* gt16, const int* shifts,
+                       const float* cameras, float* img, int* bad, cudaStream_t st);
+// out_losses[b] = losses[b] (NaN when bad[b]), status[b] = bad[b], and the gradient of a bad image zeroed (grads: the call
+// has gradients).  recs: the B device records.
+void launch_reproj_finish(const ReprojImage* recs, int B, bool grads, const double* losses, const int* bad, double* out_losses,
+                          int* status, cudaStream_t st);
+// The n host records into recs, in chunks.  Returns the launches.
+int launch_coord_prep(const CoordImage* host_recs, int n, CoordImage* recs, cudaStream_t st);
+// out_losses[b] = losses[b], out_counts[b] = counts[b] (out_counts may be null).
+void launch_coord_finish(int B, const double* losses, const long long* counts, double* out_losses, long long* out_counts,
+                         cudaStream_t st);
 
 // --- bwd.cu -------------------------------------------------------------------------------
 struct BwdArgs {

@@ -258,6 +258,19 @@ int reproj_blocks_per_image(int N) {
     return need < 64 ? need : (need < 256 ? (need + 1) / 2 : (need + 3) / 4);
 }
 
+int reproj_max_blocks(int N) {
+    // the count rises with N within each of its three ranges and drops where a range starts: the largest is at N or at the
+    // end of a range below it
+    const int per_block = kThreads * kCellsPerThread;
+    int most = reproj_blocks_per_image(N);
+    for (int need : {63, 255}) {
+        if ((long long)need * per_block >= N) break;
+        const int b = reproj_blocks_per_image(need * per_block);
+        if (b > most) most = b;
+    }
+    return most;
+}
+
 bool reproj_vec_ok(const float* coords, const float* grads, int N, int W) {
     return (N % 4 == 0) && W >= 4 && ((uintptr_t)coords % 16 == 0) && (!grads || (uintptr_t)grads % 16 == 0);
 }

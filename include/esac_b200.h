@@ -401,6 +401,37 @@ int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pre
                                const float* const* gt, const int* Hg, const int* Wg, float* const* grads, float cutLoss,
                                double* out_losses, int64_t* out_counts);
 
+/* The two losses with esacb200_forward_async's contract, so that a step of init_expert.py / ref_expert.py (the expert's
+ * forward, the loss, its backward and the optimiser) can be captured in one CUDA graph.  Ragged form only: host arrays of B
+ * image pointers and sizes, as in the ragged calls above; the pointers and sizes are fixed for a capture, and every image
+ * pointer, like every other pointer argument, must be DEVICE memory (a host pointer is an error, reported before anything
+ * is enqueued).  The call enqueues on the context's stream and returns: no host synchronisation, no read-back, no event
+ * query, and while the stream is being captured no allocation.  What changes from step to step is read from device memory
+ * when the kernels run: the maps, the ground truths, the pads and the cameras.  B <= 65535.
+ *
+ * esacb200_reproj_loss_async: esacb200_reproj_loss_ragged on coords[b] float32 [3,H[b],W[b]], grads NULL (loss only) or B
+ * pointers [3,H[b],W[b]] (overwritten), gt_poses float32 [B,4,4] camera->world, shifts int32 [B,2] (padX, padY), cameras
+ * float32 [B,3] (f, cx, cy).  The ground truth is inverted on the device with the eager call's host arithmetic, so the
+ * losses and gradients are bitwise the eager call's.  out_losses double [B]; out_status int32 [B]: 0 = OK, 1 = the image's
+ * ground-truth rotation block is singular or NaN (where the eager call fails): its loss is NaN, its gradient slice zero, and
+ * the other images are unaffected.
+ *
+ * esacb200_coord_loss_async: esacb200_coord_loss_ragged on device maps, out_losses double [B], out_counts int64 [B] or NULL;
+ * bitwise the eager call's results.  An image without valid cells has a NaN loss, as there; nothing fails on the device.
+ *
+ * Workspace: the two share one buffer of the stream-ordered context, apart from the forward's and the backward's.  An
+ * uncaptured call grows it as needed; a captured call cannot, so call esacb200_reserve_loss_async before the first capture
+ * (B images of at most H x W cells: for the coordinate loss, cells of the prediction).  Once a capture has used it, nothing
+ * in it is freed or reallocated: a later call or reserve that needs more fails, before enqueuing anything, naming the
+ * reserve call.  The first call on a context, of either loss or of esacb200_reserve_loss_async, may not be captured. */
+int esacb200_reproj_loss_async(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H,
+                               const int* W, const float* gt_poses, const int32_t* shifts, const float* cameras, int subSampling,
+                               float cutLoss, float maxReproj, float minDepth, double* out_losses, int32_t* out_status);
+int esacb200_coord_loss_async(esacb200_ctx* ctx, int B, const float* const* pred, const int* Hp, const int* Wp,
+                              const float* const* gt, const int* Hg, const int* Wg, float* const* grads, float cutLoss,
+                              double* out_losses, int64_t* out_counts);
+int esacb200_reserve_loss_async(esacb200_ctx* ctx, int B, int H, int W);
+
 /* Soft-inlier scores of given poses (getReproErrs + getHypScores, esac_util.h:235-363) without
  * sampling/selection/refinement: poses6 = host double [M][6] (rvec, tvec); out_scores host double [M]. */
 int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,

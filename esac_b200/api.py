@@ -1163,33 +1163,54 @@ def _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras, call="forwar
     return B, E, H, W, M
 
 
-def _async_context(call, lead, M, inputs, fixed):
-    """The checks forward_async and backward_async (`call`) share after _async_shapes, in this order: every `fixed`
-    argument (name -> (tensor, dtype, trailing shape)) is a contiguous torch tensor of shape lead + trailing shape; the
-    inputs (name -> tensor, hypAssignment among them if the call takes one) are contiguous, hypAssignment row by row; all
-    are CUDA tensors of one device.  Returns the context, on torch's current stream."""
-    for what, (t, dt, tail) in fixed.items():
+def _async_context(call, fixed, inputs, check_inputs=None):
+    """The checks every stream-ordered call (`call`) makes before it takes a context, in this order: every `fixed`
+    argument (name -> (tensor, dtype, shape)) is a contiguous torch tensor of that shape; check_inputs(), if given; then
+    the inputs ((name, tensor) pairs) and the fixed arguments are CUDA tensors of one device.  Returns the context, on
+    torch's current stream."""
+    for what, (t, dt, shape) in fixed.items():
         if not _is_torch(t):
             raise RuntimeError(f"{call} takes torch CUDA tensors only ({what} is a {type(t).__name__})")
-        _check(t, dt, len(lead + tail), what)
-        if tuple(int(v) for v in t.shape) != lead + tail or not t.is_contiguous():
-            raise RuntimeError(f"{what} must be a contiguous {list(lead + tail)} tensor, got {list(t.shape)}")
-    for what, t in inputs.items():
-        if what != "hypAssignment" and not t.is_contiguous():
-            raise RuntimeError(f"{what} must be contiguous (a copy would not be captured with the call)")
-    hypAssignment = inputs.get("hypAssignment")
-    if hypAssignment is not None and lead and lead[0] > 1 and hypAssignment.stride(0) != M * hypAssignment.stride(-1):
-        raise RuntimeError("hypAssignment must hold its rows back to back (row stride M times the element stride)")
-    args = dict(inputs, **{what: t for what, (t, _, _) in fixed.items()})
-    for what, t in args.items():
+        _check(t, dt, len(shape), what)
+        if tuple(int(v) for v in t.shape) != shape or not t.is_contiguous():
+            raise RuntimeError(f"{what} must be a contiguous {list(shape)} tensor, got {list(t.shape)}")
+    if check_inputs is not None:
+        check_inputs()
+    tensors = list(inputs) + [(what, t) for what, (t, _, _) in fixed.items()]
+    for what, t in tensors:
         if not t.is_cuda:
             raise RuntimeError(f"{call} takes CUDA tensors only ({what} is on the CPU)")
-    devs = {t.device.index for t in args.values()}
+    devs = {t.device.index for _, t in tensors}
     if len(devs) > 1:
         raise RuntimeError(f"esac_b200: tensors live on different CUDA devices {sorted(devs)}")
     ctx = _pick_ctx(*devs)
     ctx.async_used = True
     return ctx
+
+
+def _esac_inputs(inputs: dict, lead, M):
+    """The stream-ordered ESAC calls' inputs (name -> tensor, hypAssignment among them if the call takes one) are
+    contiguous, hypAssignment row by row.  Returns a check for _async_context and the inputs as (name, tensor) pairs."""
+    def check():
+        for what, t in inputs.items():
+            if what != "hypAssignment" and not t.is_contiguous():
+                raise RuntimeError(f"{what} must be contiguous (a copy would not be captured with the call)")
+        hypAssignment = inputs.get("hypAssignment")
+        if hypAssignment is not None and lead and lead[0] > 1 and hypAssignment.stride(0) != M * hypAssignment.stride(-1):
+            raise RuntimeError("hypAssignment must hold its rows back to back (row stride M times the element stride)")
+    return list(inputs.items()), check
+
+
+def _reserve_async(call, device, sizes: dict, *rest):
+    """esacb200_`call` with the sizes (name -> value, all positive) and `rest`, all as ints, on torch's current stream of
+    the device's context."""
+    if min(int(v) for v in sizes.values()) < 1:
+        raise RuntimeError(f"{call}: sizes must be positive, got " + " ".join(f"{k}={v}" for k, v in sizes.items()))
+    ctx = context(device)
+    import torch
+    ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
+    ctx.async_used = True
+    ctx.check(getattr(ctx.lib, "esacb200_" + call)(ctx.handle, *(int(v) for v in (*sizes.values(), *rest))))
 
 
 def forward_async(sceneCoordinates, hypAssignment, shifts, cameras, inlierThreshold, inlierAlpha, inlierBeta, maxReproj,
@@ -1204,10 +1225,10 @@ def forward_async(sceneCoordinates, hypAssignment, shifts, cameras, inlierThresh
     the largest shape before the first capture; once captured, the workspace never grows again."""
     B, E, H, W, M = _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras)
     lead = (B,) if sceneCoordinates.dim() == 5 else ()
-    ctx = _async_context("forward_async", lead, M, {"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment,
-                                                    "shifts": shifts, "cameras": cameras},
-                         {"outPoses": (outPoses, "Float", (4, 4)), "outExperts": (outExperts, "Long", ()),
-                          "outStatus": (outStatus, "Int", ())})
+    ctx = _async_context("forward_async", {"outPoses": (outPoses, "Float", lead + (4, 4)), "outExperts": (outExperts, "Long", lead),
+                                           "outStatus": (outStatus, "Int", lead)},
+                         *_esac_inputs({"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment, "shifts": shifts,
+                                        "cameras": cameras}, lead, M))
     ctx.check(ctx.lib.esacb200_forward_async(ctx.handle, B, sceneCoordinates.data_ptr(), E, H, W, hypAssignment.data_ptr(),
                                              int(hypAssignment.stride(-1)), M, shifts.data_ptr(), cameras.data_ptr(),
                                              *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling),
@@ -1216,13 +1237,7 @@ def forward_async(sceneCoordinates, hypAssignment, shifts, cameras, inlierThresh
 
 def reserve_forward_async(B: int, E: int, H: int, W: int, M: int, subSampling: int = 8, device: int | None = None):
     """Sizes forward_async's workspace for this shape; call it before capturing (it allocates)."""
-    if min(int(B), int(E), int(H), int(W), int(M)) < 1:
-        raise RuntimeError(f"reserve_forward_async: sizes must be positive, got B={B} E={E} H={H} W={W} M={M}")
-    ctx = context(device)
-    import torch
-    ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
-    ctx.async_used = True
-    ctx.check(ctx.lib.esacb200_reserve_forward_async(ctx.handle, int(B), int(E), int(H), int(W), int(M), int(subSampling)))
+    _reserve_async("reserve_forward_async", device, dict(B=B, E=E, H=H, W=W, M=M), subSampling)
 
 
 def backward_async(sceneCoordinates, outGradients, hypAssignment, gtPoses, shifts, cameras, wLossRot, wLossTrans, lossCut,
@@ -1239,10 +1254,11 @@ def backward_async(sceneCoordinates, outGradients, hypAssignment, gtPoses, shift
     capture; once captured, the workspace never grows again."""
     B, E, H, W, M = _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras, "backward_async")
     lead = (B,) if sceneCoordinates.dim() == 5 else ()
-    ctx = _async_context("backward_async", lead, M, {"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment,
-                                                     "shifts": shifts, "cameras": cameras},
-                         {"outGradients": (outGradients, "Float", (E, 3, H, W)), "gtPoses": (gtPoses, "Float", (4, 4)),
-                          "outLosses": (outLosses, "Double", ()), "outStatus": (outStatus, "Int", ())})
+    ctx = _async_context("backward_async", {"outGradients": (outGradients, "Float", lead + (E, 3, H, W)),
+                                            "gtPoses": (gtPoses, "Float", lead + (4, 4)), "outLosses": (outLosses, "Double", lead),
+                                            "outStatus": (outStatus, "Int", lead)},
+                         *_esac_inputs({"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment, "shifts": shifts,
+                                        "cameras": cameras}, lead, M))
     ctx.check(ctx.lib.esacb200_backward_async(ctx.handle, B, sceneCoordinates.data_ptr(), outGradients.data_ptr(), E, H, W,
                                               hypAssignment.data_ptr(), int(hypAssignment.stride(-1)), M, gtPoses.data_ptr(),
                                               float(wLossRot), float(wLossTrans), float(lossCut), shifts.data_ptr(),
@@ -1254,13 +1270,7 @@ def backward_async(sceneCoordinates, outGradients, hypAssignment, gtPoses, shift
 def reserve_backward_async(B: int, E: int, H: int, W: int, M: int, subSampling: int = 8, device: int | None = None):
     """Sizes backward_async's workspace (which forward_async shares) for this shape; call it before capturing (it
     allocates)."""
-    if min(int(B), int(E), int(H), int(W), int(M)) < 1:
-        raise RuntimeError(f"reserve_backward_async: sizes must be positive, got B={B} E={E} H={H} W={W} M={M}")
-    ctx = context(device)
-    import torch
-    ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
-    ctx.async_used = True
-    ctx.check(ctx.lib.esacb200_reserve_backward_async(ctx.handle, int(B), int(E), int(H), int(W), int(M), int(subSampling)))
+    _reserve_async("reserve_backward_async", device, dict(B=B, E=E, H=H, W=W, M=M), subSampling)
 
 
 def hypotheses_tape_stride(E: int, H: int, W: int, M: int) -> int:
@@ -1295,10 +1305,10 @@ def hypotheses_forward_async(sceneCoordinates, hypAssignment, shifts, cameras, i
     if not _is_torch(tapes):
         raise RuntimeError(f"{call} takes torch CUDA tensors only (tapes is a {type(tapes).__name__})")
     _check_tapes(tapes, B, E, H, W, M, call)
-    ctx = _async_context(call, lead, M, {"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment,
-                                         "shifts": shifts, "cameras": cameras, "tapes": tapes},
-                         {"outScores": (outScores, "Double", (M,)), "outPoses": (outPoses, "Double", (M, 6)),
-                          "outContributing": (outContributing, "Bool", (M,)), "outStatus": (outStatus, "Int", ())})
+    ctx = _async_context(call, {"outScores": (outScores, "Double", lead + (M,)), "outPoses": (outPoses, "Double", lead + (M, 6)),
+                                "outContributing": (outContributing, "Bool", lead + (M,)), "outStatus": (outStatus, "Int", lead)},
+                         *_esac_inputs({"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment, "shifts": shifts,
+                                        "cameras": cameras, "tapes": tapes}, lead, M))
     ctx.check(ctx.lib.esacb200_hypotheses_forward_async(
         ctx.handle, B, sceneCoordinates.data_ptr(), E, H, W, hypAssignment.data_ptr(), int(hypAssignment.stride(-1)), M,
         shifts.data_ptr(), cameras.data_ptr(), *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling),
@@ -1325,15 +1335,15 @@ def hypotheses_backward_async(tapes, sceneCoordinates, outGradients, M, gradScor
     M = int(M)
     if three != 3 or B < 1 or E < 1 or M < 1:
         raise RuntimeError(f"{call}: sceneCoordinates must be [B,E,3,H,W] or [E,3,H,W] and M >= 1")
-    fixed = {"outGradients": (outGradients, "Float", (E, 3, H, W))}
+    fixed = {"outGradients": (outGradients, "Float", lead + (E, 3, H, W))}
     if gradScores is not None:
-        fixed["gradScores"] = (gradScores, "Double", (M,))
+        fixed["gradScores"] = (gradScores, "Double", lead + (M,))
     if gradPoses is not None:
-        fixed["gradPoses"] = (gradPoses, "Double", (M, 6))
+        fixed["gradPoses"] = (gradPoses, "Double", lead + (M, 6))
     if outStatus is not None:
-        fixed["outStatus"] = (outStatus, "Int", ())
+        fixed["outStatus"] = (outStatus, "Int", lead)
     _check_tapes(tapes, B, E, H, W, M, call)
-    ctx = _async_context(call, lead, M, {"sceneCoordinates": sceneCoordinates, "tapes": tapes}, fixed)
+    ctx = _async_context(call, fixed, *_esac_inputs({"sceneCoordinates": sceneCoordinates, "tapes": tapes}, lead, M))
     if outStatus is None:
         import torch
         outStatus = torch.empty(lead, dtype=torch.int32, device=sceneCoordinates.device)
@@ -1363,9 +1373,9 @@ def pose_loss_async(poses, gtPose, wLossRot, wLossTrans, lossCut, outLosses=None
         outLosses = torch.empty(lead + (M,), dtype=torch.float64, device=poses.device)
     if outDloss is None:
         outDloss = torch.empty(lead + (M, 6), dtype=torch.float64, device=poses.device)
-    ctx = _async_context(call, lead, M, {"poses": poses},
-                         {"gtPose": (gtPose, "Float", (4, 4)), "outLosses": (outLosses, "Double", (M,)),
-                          "outDloss": (outDloss, "Double", (M, 6))})
+    ctx = _async_context(call, {"gtPose": (gtPose, "Float", lead + (4, 4)), "outLosses": (outLosses, "Double", lead + (M,)),
+                                "outDloss": (outDloss, "Double", lead + (M, 6))},
+                         *_esac_inputs({"poses": poses}, lead, M))
     B = lead[0] if lead else 1
     ctx.check(ctx.lib.esacb200_pose_loss_async(ctx.handle, B, M, poses.data_ptr(), gtPose.data_ptr(), float(wLossRot),
                                                float(wLossTrans), float(lossCut), outLosses.data_ptr(), outDloss.data_ptr()))
@@ -1388,26 +1398,9 @@ def _loss_images(t, what: str, call: str, writable: bool = False, like: _Images 
     return im
 
 
-def _loss_async_context(call: str, images, fixed: dict) -> Context:
-    """The checks the stream-ordered losses share after their image arguments: every `fixed` argument (name -> (tensor,
-    dtype, shape)) is a contiguous torch tensor of that shape; then every tensor is a CUDA tensor of one device.  Returns
-    the context, on torch's current stream."""
-    for what, (t, dt, shape) in fixed.items():
-        if not _is_torch(t):
-            raise RuntimeError(f"{call} takes torch CUDA tensors only ({what} is a {type(t).__name__})")
-        _check(t, dt, len(shape), what)
-        if tuple(int(v) for v in t.shape) != shape or not t.is_contiguous():
-            raise RuntimeError(f"{what} must be a contiguous {list(shape)} tensor, got {list(t.shape)}")
-    tensors = [(im.what, a.orig) for im in images for a in im.args] + [(what, t) for what, (t, _, _) in fixed.items()]
-    for what, t in tensors:
-        if not t.is_cuda:
-            raise RuntimeError(f"{call} takes CUDA tensors only ({what} is on the CPU)")
-    devs = {t.device.index for _, t in tensors}
-    if len(devs) > 1:
-        raise RuntimeError(f"esac_b200: tensors live on different CUDA devices {sorted(devs)}")
-    ctx = _pick_ctx(*devs)
-    ctx.async_used = True
-    return ctx
+def _image_tensors(images):
+    """The (name, tensor) pairs of the stream-ordered losses' image arguments (_loss_images)."""
+    return [(im.what, a.orig) for im in images for a in im.args]
 
 
 def reproj_loss_async(prediction, gtPoses, shifts, cameras, cutLoss, subSampling, outLosses, outStatus, outGradients=None,
@@ -1427,10 +1420,10 @@ def reproj_loss_async(prediction, gtPoses, shifts, cameras, cutLoss, subSampling
     if outGradients is not None:
         og = _loss_images(outGradients, "outGradients", call, writable=True, like=pr)
         og.require_shapes_of(pr)
-    ctx = _loss_async_context(call, [pr] + ([og] if og else []),
-                              {"gtPoses": (gtPoses, "Float", (B, 4, 4)), "shifts": (shifts, "Int", (B, 2)),
-                               "cameras": (cameras, "Float", (B, 3)), "outLosses": (outLosses, "Double", (B,)),
-                               "outStatus": (outStatus, "Int", (B,))})
+    ctx = _async_context(call, {"gtPoses": (gtPoses, "Float", (B, 4, 4)), "shifts": (shifts, "Int", (B, 2)),
+                                "cameras": (cameras, "Float", (B, 3)), "outLosses": (outLosses, "Double", (B,)),
+                                "outStatus": (outStatus, "Int", (B,))},
+                         _image_tensors([pr] + ([og] if og else [])))
     ctx.check(ctx.lib.esacb200_reproj_loss_async(ctx.handle, B, pr.ptrs, og.ptrs if og else None, pr.hs, pr.ws,
                                                  gtPoses.data_ptr(), shifts.data_ptr(), cameras.data_ptr(), int(subSampling),
                                                  float(cutLoss), float(maxReproj), float(minDepth), outLosses.data_ptr(),
@@ -1458,7 +1451,7 @@ def coord_loss_async(prediction, gtCoords, cutLoss, outLosses, outGradients=None
     fixed = {"outLosses": (outLosses, "Double", (pr.B,))}
     if outCounts is not None:
         fixed["outCounts"] = (outCounts, "Long", (pr.B,))
-    ctx = _loss_async_context(call, [pr, gt] + ([og] if og else []), fixed)
+    ctx = _async_context(call, fixed, _image_tensors([pr, gt] + ([og] if og else [])))
     ctx.check(ctx.lib.esacb200_coord_loss_async(ctx.handle, pr.B, pr.ptrs, pr.hs, pr.ws, gt.ptrs, gt.hs, gt.ws,
                                                 og.ptrs if og else None, float(cutLoss), outLosses.data_ptr(),
                                                 outCounts.data_ptr() if outCounts is not None else None))
@@ -1467,13 +1460,7 @@ def coord_loss_async(prediction, gtCoords, cutLoss, outLosses, outGradients=None
 def reserve_loss_async(B: int, H: int, W: int, device: int | None = None):
     """Sizes the workspace of reproj_loss_async and coord_loss_async for B images of at most H x W cells (the prediction's);
     call it before capturing (it allocates)."""
-    if min(int(B), int(H), int(W)) < 1:
-        raise RuntimeError(f"reserve_loss_async: sizes must be positive, got B={B} H={H} W={W}")
-    ctx = context(device)
-    import torch
-    ctx.set_stream(torch.cuda.current_stream(ctx.device).cuda_stream or _CUDA_STREAM_LEGACY)
-    ctx.async_used = True
-    ctx.check(ctx.lib.esacb200_reserve_loss_async(ctx.handle, int(B), int(H), int(W)))
+    _reserve_async("reserve_loss_async", device, dict(B=B, H=H, W=W))
 
 
 def set_seed(seed: int, device: int | None = None):

@@ -180,7 +180,16 @@ def esac_loss_async(scene_coordinates, gating_log_probs, hyp_assignment, gt_pose
     return EsacLossAsync.apply(meta, gating_log_probs, scene_coordinates)
 
 
-class ReprojLoss(torch.autograd.Function):
+class _BatchMeanLoss(torch.autograd.Function):
+    """The backward of the loss nodes below, whose forward returns the mean over a batch of `ctx.batch` images and saves
+    the gradient of each image's loss with respect to the predictions."""
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        return (None,) + tuple(g * (grad_out / ctx.batch) for g in ctx.saved_tensors)
+
+
+class ReprojLoss(_BatchMeanLoss):
     """ref_expert.py:103-150 as one autograd node: forward = the robust reprojection loss of a batch of predictions
     (mean over the batch of the per-image losses; the reference has one image per step), backward = its gradient, both
     from the single fused kernel behind api.reproj_loss.  The predictions come last (_as_inputs)."""
@@ -194,10 +203,6 @@ class ReprojLoss(torch.autograd.Function):
         ctx.batch = len(losses)
         return prediction[0].new_tensor(sum(losses) / len(losses))
 
-    @staticmethod
-    def backward(ctx, grad_out):
-        return (None,) + tuple(g * (grad_out / ctx.batch) for g in ctx.saved_tensors)
-
 
 def reproj_loss(prediction, gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling=8, ppoint_x=None, ppoint_y=None):
     """Drop-in for the loss block of ref_expert.py: `robust_loss = reproj_loss(prediction, gt_pose, f, padX, padY,
@@ -209,7 +214,7 @@ def reproj_loss(prediction, gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_
     return ReprojLoss.apply((form, args), *inputs)
 
 
-class CoordLoss(torch.autograd.Function):
+class CoordLoss(_BatchMeanLoss):
     """init_expert.py:106-132 as one autograd node: forward = the robust scene-coordinate loss of a batch of predictions
     (mean over the batch of the per-image losses; the reference has one image per step), backward = its gradient, both
     from the fused kernels behind api.coord_loss.  The predictions come last (_as_inputs)."""
@@ -222,10 +227,6 @@ class CoordLoss(torch.autograd.Function):
         ctx.save_for_backward(*grads)
         ctx.batch = len(losses)
         return prediction[0].new_tensor(sum(losses) / len(losses))
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        return (None,) + tuple(g * (grad_out / ctx.batch) for g in ctx.saved_tensors)
 
 
 def coord_loss(prediction, gt_coords, cut_loss=100.0):
@@ -247,7 +248,7 @@ def _batch_mean(losses):
     return (total / torch.full((), float(losses.shape[0]), dtype=torch.float64, device=losses.device)).float()
 
 
-class ReprojLossAsync(torch.autograd.Function):
+class ReprojLossAsync(_BatchMeanLoss):
     """ReprojLoss on api.reproj_loss_async: no host synchronisation in the forward or the backward, so the node, and
     loss.backward() through it, can be captured in a CUDA graph.  The predictions come last (_as_inputs)."""
 
@@ -266,10 +267,6 @@ class ReprojLossAsync(torch.autograd.Function):
         ctx.batch = B
         return _batch_mean(losses)
 
-    @staticmethod
-    def backward(ctx, grad_out):
-        return (None,) + tuple(g * (grad_out / ctx.batch) for g in ctx.saved_tensors)
-
 
 def reproj_loss_async(prediction, gt_poses, shifts, cameras, cut_loss, sub_sampling=8, max_reproj=100.0, min_depth=0.1,
                       status=None):
@@ -284,7 +281,7 @@ def reproj_loss_async(prediction, gt_poses, shifts, cameras, cut_loss, sub_sampl
     return ReprojLossAsync.apply(meta, *inputs)
 
 
-class CoordLossAsync(torch.autograd.Function):
+class CoordLossAsync(_BatchMeanLoss):
     """CoordLoss on api.coord_loss_async: no host synchronisation in the forward or the backward, so the node, and
     loss.backward() through it, can be captured in a CUDA graph.  The predictions come last (_as_inputs)."""
 
@@ -299,10 +296,6 @@ class CoordLossAsync(torch.autograd.Function):
         ctx.save_for_backward(*grads)
         ctx.batch = B
         return _batch_mean(losses)
-
-    @staticmethod
-    def backward(ctx, grad_out):
-        return (None,) + tuple(g * (grad_out / ctx.batch) for g in ctx.saved_tensors)
 
 
 def coord_loss_async(prediction, gt_coords, cut_loss=100.0, counts=None):

@@ -1382,6 +1382,15 @@ static int async_workspace(esacb200_ctx* ctx, esacb200_ctx* a, const std::vector
     return 0;
 }
 
+// The async context of reserve_`what`: a reserve call allocates, so it may not run while the stream is being captured.
+static int reserve_context(esacb200_ctx* ctx, const char* what, esacb200_ctx** out) {
+    bool capturing = false;
+    int rc = stream_capturing(ctx, capturing);
+    if (rc) return rc;
+    if (capturing) return fail(ctx, ESACB200_ERR_ARG, "reserve_%s allocates: call it before the capture", what);
+    return async_context(ctx, false, what, out);
+}
+
 // reserve_forward_async / reserve_backward_async (`backward`): sizes the async workspace for B images of one shape.
 static int reserve_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, int sub, bool backward) {
     if (!ctx) return ESACB200_ERR_ARG;
@@ -1392,14 +1401,21 @@ static int reserve_async(esacb200_ctx* ctx, int B, int E, int H, int W, int M, i
     int rc = fill_problem(ctx, plans[0].P, E, H, W, M, 0, 0, 1.f, 0.f, 0.f, 1.f, 1.f, 1.f, 1.f, sub, NO_DRAW);
     if (rc) return rc;
     plans[0].d_coords = nullptr;  // the load path does not change the workspace
-    bool capturing = false;
-    rc = stream_capturing(ctx, capturing);
-    if (rc) return rc;
-    if (capturing) return fail(ctx, ESACB200_ERR_ARG, "reserve_%s allocates: call it before the capture", what);
     esacb200_ctx* a = nullptr;
-    rc = async_context(ctx, false, what, &a);
-    if (rc) return rc;
+    if ((rc = reserve_context(ctx, what, &a))) return rc;
     return async_workspace(ctx, a, plans, false, backward);
+}
+
+// The n named arguments are device memory (a null one is an error unless `optional` has its bit set).
+static int device_args(esacb200_ctx* ctx, const char* what, int n, const void* const* ptrs, const char* const* names, unsigned optional = 0) {
+    for (int i = 0; i < n; ++i) {
+        if (!ptrs[i]) {
+            if (optional >> i & 1) continue;
+            return fail(ctx, ESACB200_ERR_ARG, "%s: %s is null", what, names[i]);
+        }
+        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "%s takes device pointers only: %s is host memory", what, names[i]);
+    }
+    return 0;
 }
 
 // A stream-ordered call of B images of one shape: the async context, and per image its Plan and its AsyncImage (whose
@@ -1418,12 +1434,10 @@ static int begin_async(esacb200_ctx* ctx, bool backward, int B, const Problem& P
                        int64_t assign_stride, const int32_t* shifts, const float* cameras, int32_t* out_status, int n,
                        const void* const* ptrs, const char* const* names, AsyncCall& call, const char* name = nullptr) {
     const char* what = name ? name : backward ? "backward_async" : "forward_async";
-    for (int i = 0; i < n; ++i) {
-        if (!ptrs[i]) return fail(ctx, ESACB200_ERR_ARG, "%s: %s is null", what, names[i]);
-        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "%s takes device pointers only: %s is host memory", what, names[i]);
-    }
+    int rc = device_args(ctx, what, n, ptrs, names);
+    if (rc) return rc;
     bool capturing = false;
-    int rc = stream_capturing(ctx, capturing);
+    rc = stream_capturing(ctx, capturing);
     if (rc) return rc;
     rc = async_context(ctx, capturing, backward ? "backward_async" : "forward_async", &call.a);
     if (rc) return rc;
@@ -2075,17 +2089,12 @@ int esacb200_hypotheses_backward_async(esacb200_ctx* ctx, int B, const void* tap
     if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "%s: empty batch (B=%d)", what, B);
     const void* ptrs[] = {tapes, coords, grads, out_status, d_scores, d_poses6};
     const char* names[] = {"tapes", "coords", "grads", "out_status", "d_scores", "d_poses6"};
-    for (int i = 0; i < 6; ++i) {
-        if (!ptrs[i]) {
-            if (i < 4) return fail(ctx, ESACB200_ERR_ARG, "%s: %s is null", what, names[i]);
-            continue;  // an absent upstream is zero
-        }
-        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "%s takes device pointers only: %s is host memory", what, names[i]);
-    }
+    int rc = device_args(ctx, what, 6, ptrs, names, 0x30u);  // an absent upstream is zero
+    if (rc) return rc;
     std::vector<Plan> plans(1);
     Problem& P = plans[0].P;
     // sub, tau, alpha, beta and maxReproj are the forward's, read from the tape header on the device (BwdDev::prob)
-    int rc = fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 1, NO_DRAW);
+    rc = fill_problem(ctx, P, E, H, W, M, 0, 0, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 1, NO_DRAW);
     if (!rc) rc = check_tapes(ctx, what, tapes, tapes_bytes, B, P);
     if (rc) return rc;
     plans[0].d_coords = coords;
@@ -2132,10 +2141,8 @@ int esacb200_pose_loss_async(esacb200_ctx* ctx, int B, int M, const double* pose
     DeviceGuard device_guard(ctx->device);
     const void* ptrs[] = {poses6, gt16, out_losses, out_dloss6};
     const char* names[] = {"poses6", "gt16", "out_losses", "out_dloss6"};
-    for (int i = 0; i < 4; ++i) {
-        if (!ptrs[i]) return fail(ctx, ESACB200_ERR_ARG, "pose_loss_async: %s is null", names[i]);
-        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "pose_loss_async takes device pointers only: %s is host memory", names[i]);
-    }
+    const int rc = device_args(ctx, "pose_loss_async", 4, ptrs, names);
+    if (rc) return rc;
     if (M <= 0) return fail(ctx, ESACB200_ERR_ARG, "pose_loss_async: no poses (M=%d)", M);
     if (B <= 0 || B > 65535) return fail(ctx, ESACB200_ERR_ARG, "pose_loss_async: batch of %d images outside [1, 65535]", B);
     launch_pose_loss((const Pose*)poses6, B, M, gt16, wRot, wTrans, cut, out_losses, out_dloss6, ctx->stream);
@@ -2449,6 +2456,145 @@ int esacb200_assign_hypotheses(esacb200_ctx* ctx, int B, int E, int M, const flo
 } ESAC_ABI_CATCH(ctx)
 
 // -------------------------------------------------------------------------------------------------
+// The two losses' steps that the eager ragged calls and the stream-ordered calls share: the per-image size checks, the
+// per-image records, the workspace layout and the launches.
+
+static size_t align64(size_t n) { return (n + 63) & ~(size_t)63; }
+
+// Byte offsets in the loss workspace of a call of B images whose blocks have `parts` partials.
+//   reprojection: [tickets B u32] [img B x kReprojImgFloats f32] [records] [losses B f64] [bad B i32] [partials f64 each]
+//   coordinates:  [tickets B u32 | counts B u32] [records] [losses B f64] [valid counts B i64] [partials 2 f64 each]
+// The eager reprojection loss leaves `bad` unused: a singular ground truth fails it before anything is enqueued.
+struct LossLayout {
+    size_t img = 0, rec, loss, flags, part, end;
+};
+static LossLayout reproj_layout(int B, long long parts) {
+    LossLayout L;
+    L.img = align64((size_t)B * 4);
+    L.rec = L.img + align64((size_t)B * kReprojImgFloats * sizeof(float));
+    L.loss = L.rec + align64((size_t)B * sizeof(ReprojImage));
+    L.flags = L.loss + align64((size_t)B * 8);
+    L.part = L.flags + align64((size_t)B * 4);
+    L.end = L.part + (size_t)parts * 8;
+    return L;
+}
+static LossLayout coord_layout(int B, long long parts) {
+    LossLayout L;
+    L.rec = align64((size_t)B * 8);
+    L.loss = L.rec + align64((size_t)B * sizeof(CoordImage));
+    L.flags = L.loss + align64((size_t)B * 8);
+    L.part = L.flags + align64((size_t)B * 8);
+    L.end = L.part + (size_t)parts * 2 * 8;
+    return L;
+}
+
+// The per-image sizes of a reprojection-loss call: positive, at most 2^30 cells.  `what`: the entry point named in front of
+// each message, or null.
+static int reproj_sizes(esacb200_ctx* ctx, const char* what, int B, const int* H, const int* W) {
+    const char* sep = what ? ": " : "";
+    if (!what) what = "";
+    for (int b = 0; b < B; ++b) {
+        if (H[b] <= 0 || W[b] <= 0) return fail(ctx, ESACB200_ERR_ARG, "%s%simage %d: bad size %dx%d", what, sep, b, W[b], H[b]);
+        if ((long long)H[b] * W[b] > (1ll << 30))
+            return fail(ctx, ESACB200_ERR_ARG, "%s%simage %d: map %dx%d too large", what, sep, b, W[b], H[b]);
+    }
+    return 0;
+}
+
+// The records of a reprojection-loss call on the B images at the device addresses coords[b] and grads[b] (grads, or an
+// entry of it, null: no gradient), and per image whether it takes the 128-bit load path.  Returns the blocks' partials.
+static long long reproj_records(int B, const float* const* coords, float* const* grads, const int* H, const int* W,
+                                std::vector<ReprojImage>& recs, std::vector<char>& vec) {
+    recs.resize((size_t)B);
+    vec.resize((size_t)B);
+    long long parts = 0;
+    for (int b = 0; b < B; ++b) {
+        ReprojImage& r = recs[b];
+        r.coords = coords[b];
+        r.grads = grads ? grads[b] : nullptr;
+        r.N = H[b] * W[b];
+        r.W = W[b];
+        r.b = b;
+        r.blocks = reproj_blocks_per_image(r.N);
+        r.part0 = parts;
+        parts += r.blocks;
+        vec[b] = reproj_vec_ok(r.coords, r.grads, r.N, r.W);
+    }
+    return parts;
+}
+
+// The reprojection loss's launches, one per load path, on the workspace at `base` laid out as L, whose records are in
+// order_by_path's order (n_vec on the 128-bit path first).  They run on run's stream and count in its kernel_launches.
+static void reproj_launches(esacb200_ctx* run, char* base, const LossLayout& L, int B, int n_vec, int max_vec, int max_sc,
+                            int sub, float cut, float maxReproj, float minDepth) {
+    const ReprojImage* rec = (const ReprojImage*)(base + L.rec);
+    for (int path = 0; path < 2; ++path) {
+        const int n = path == 0 ? n_vec : B - n_vec;
+        if (n == 0) continue;
+        launch_reproj(path == 0, rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, (const float*)(base + L.img),
+                      (float)sub, cut, maxReproj, minDepth, (double*)(base + L.part), (unsigned*)base, (double*)(base + L.loss),
+                      run->stream);
+        run->st.kernel_launches += 1;
+    }
+}
+
+// The per-image sizes of a coordinate-loss call: positive, prediction and ground truth at most 1 apart, at most 2^30 cells.
+// `what`: the entry point named in front of each message, or null.
+static int coord_sizes(esacb200_ctx* ctx, const char* what, int B, const int* Hp, const int* Wp, const int* Hg, const int* Wg) {
+    const char* sep = what ? ": " : "";
+    if (!what) what = "";
+    for (int b = 0; b < B; ++b) {
+        if (Hp[b] <= 0 || Wp[b] <= 0 || Hg[b] <= 0 || Wg[b] <= 0)
+            return fail(ctx, ESACB200_ERR_ARG, "%s%simage %d: bad sizes prediction %dx%d ground truth %dx%d", what, sep, b, Hp[b],
+                        Wp[b], Hg[b], Wg[b]);
+        if (abs(Hp[b] - Hg[b]) > 1 || abs(Wp[b] - Wg[b]) > 1)   // util.assert_size tolerates 1 cell
+            return fail(ctx, ESACB200_ERR_ARG, "%s%simage %d: size mismatch: prediction %dx%d, ground truth %dx%d (at most 1 apart)",
+                        what, sep, b, Hp[b], Wp[b], Hg[b], Wg[b]);
+        if ((long long)Hp[b] * Wp[b] > (1ll << 30) || (long long)Hg[b] * Wg[b] > (1ll << 30))
+            return fail(ctx, ESACB200_ERR_ARG, "%s%simage %d: map too large", what, sep, b);
+    }
+    return 0;
+}
+
+// The records of a coordinate-loss call on the B images at the device addresses pred[b], gt[b] and grads[b] (grads, or an
+// entry of it, null: no gradient), and per image whether it takes the 128-bit load path.  Returns the blocks' partials.
+static long long coord_records(int B, const float* const* pred, const float* const* gt, float* const* grads, const int* Hp,
+                               const int* Wp, const int* Hg, const int* Wg, std::vector<CoordImage>& recs, std::vector<char>& vec) {
+    recs.resize((size_t)B);
+    vec.resize((size_t)B);
+    long long parts = 0;
+    for (int b = 0; b < B; ++b) {
+        CoordImage& r = recs[b];
+        r.pred = pred[b];
+        r.gt = gt[b];
+        r.grads = grads ? grads[b] : nullptr;
+        vec[b] = coord_image(r, Hp[b], Wp[b], Hg[b], Wg[b]);
+        r.b = b;
+        r.part0 = parts;
+        parts += r.blocks;
+    }
+    return parts;
+}
+
+// The coordinate loss's launches, per load path the count pass (with gradients) and the loss pass, on the workspace at
+// `base` laid out as L, whose records are in order_by_path's order.  They run on run's stream and count in its
+// kernel_launches.
+static void coord_launches(esacb200_ctx* run, char* base, const LossLayout& L, int B, bool grads, int n_vec, int max_vec,
+                           int max_sc, float cut) {
+    const CoordImage* rec = (const CoordImage*)(base + L.rec);
+    for (int path = 0; path < 2; ++path) {
+        const int n = path == 0 ? n_vec : B - n_vec;
+        if (n == 0) continue;
+        for (int pass = grads ? 1 : 2; pass <= 2; ++pass) {
+            launch_coord_loss(path == 0, pass, grads, rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, cut,
+                              (unsigned*)base + B, (double*)(base + L.part), (unsigned*)base, (double*)(base + L.loss),
+                              (long long*)(base + L.flags), run->stream);
+            run->st.kernel_launches += 1;
+        }
+    }
+}
+
+// -------------------------------------------------------------------------------------------------
 // The reprojection loss over B images, each with its own size: one launch per load path (128-bit / scalar, chosen per
 // image as a single-image call would choose it), each image cut into the blocks a single-image call uses.
 int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H,
@@ -2460,13 +2606,10 @@ int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* co
     if (!coords || !H || !W || !gt_poses || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
     if (!f || !ppx || !ppy) return fail(ctx, ESACB200_ERR_ARG, "null camera array");
     if (B <= 0 || sub <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d sub=%d", B, sub);
-    for (int b = 0; b < B; ++b) {
-        if (H[b] <= 0 || W[b] <= 0) return fail(ctx, ESACB200_ERR_ARG, "image %d: bad size %dx%d", b, W[b], H[b]);
-        if ((long long)H[b] * W[b] > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "image %d: map %dx%d too large", b, W[b], H[b]);
-    }
-    bool c_dev = false, g_dev = false;
-    int rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", c_dev);
+    int rc = reproj_sizes(ctx, nullptr, B, H, W);
     if (rc) return rc;
+    bool c_dev = false, g_dev = false;
+    if ((rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", c_dev))) return rc;
     if (grads && (rc = pointer_kind(ctx, (const void* const*)grads, B, "grads", g_dev))) return rc;
     begin_call(ctx);
     std::vector<size_t> bytes((size_t)B), c_off, g_off;
@@ -2489,53 +2632,29 @@ int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* co
         if (!reproj_img_row(gt.data() + (size_t)b * 16, shiftX ? shiftX[b] : 0, shiftY ? shiftY[b] : 0, f[b], ppx[b], ppy[b],
                             img.data() + (size_t)b * kReprojImgFloats))
             return fail(ctx, ESACB200_ERR_ARG, "image %d: ground-truth pose is singular", b);
-    std::vector<ReprojImage> recs((size_t)B);
-    std::vector<char> vec((size_t)B);
-    long long parts = 0;
-    for (int b = 0; b < B; ++b) {
-        ReprojImage& r = recs[b];
-        r.coords = d_coords[b];
-        r.grads = d_grads[b];
-        r.N = H[b] * W[b];
-        r.W = W[b];
-        r.b = b;
-        r.blocks = reproj_blocks_per_image(r.N);
-        r.part0 = parts;
-        parts += r.blocks;
-        vec[b] = reproj_vec_ok(r.coords, r.grads, r.N, r.W);
-    }
-    std::vector<ReprojImage> ordered;
+    std::vector<ReprojImage> recs, ordered;
+    std::vector<char> vec;
+    const long long parts = reproj_records(B, d_coords.data(), d_grads.data(), H, W, recs, vec);
     int n_vec, max_vec, max_sc;
     const size_t rec_bytes = order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
-    // scratch layout: [tickets B u32, padded] [img B*kReprojImgFloats f32 | records, padded] [losses B f64] [partials f64]
-    const size_t img_bytes = img.size() * sizeof(float);
-    const size_t off_img = ((size_t)B * 4 + 63) & ~(size_t)63, off_rec = off_img + ((img_bytes + 15) & ~(size_t)15),
-                 off_loss = (off_rec + rec_bytes + 63) & ~(size_t)63, off_part = off_loss + (((size_t)B * 8 + 63) & ~(size_t)63);
-    CK(ctx->scratch.ensure(off_part + (size_t)parts * 8));
+    const LossLayout L = reproj_layout(B, parts);
+    CK(ctx->scratch.ensure(L.end));
     char* base = (char*)ctx->scratch.p;
-    std::vector<char> staging(off_rec - off_img + rec_bytes);
-    memcpy(staging.data(), img.data(), img_bytes);
-    memcpy(staging.data() + (off_rec - off_img), ordered.data(), rec_bytes);
-    CK(cudaMemsetAsync(base, 0, off_img, ctx->stream));
-    CK(cudaMemcpyAsync(base + off_img, staging.data(), staging.size(), cudaMemcpyHostToDevice, ctx->stream));
+    std::vector<char> staging(L.rec - L.img + rec_bytes);
+    memcpy(staging.data(), img.data(), img.size() * sizeof(float));
+    memcpy(staging.data() + (L.rec - L.img), ordered.data(), rec_bytes);
+    CK(cudaMemsetAsync(base, 0, L.img, ctx->stream));
+    CK(cudaMemcpyAsync(base + L.img, staging.data(), staging.size(), cudaMemcpyHostToDevice, ctx->stream));
     mark(ctx, EV_H2D);
     mark(ctx, EV_FOLD);  // ms_score = the kernels alone
-    const ReprojImage* d_rec = (const ReprojImage*)(base + off_rec);
-    for (int path = 0; path < 2; ++path) {
-        const int n = path == 0 ? n_vec : B - n_vec;
-        if (n == 0) continue;
-        launch_reproj(path == 0, d_rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, (const float*)(base + off_img),
-                      (float)sub, cut, maxReproj, minDepth, (double*)(base + off_part), (unsigned*)base, (double*)(base + off_loss),
-                      ctx->stream);
-        CK(cudaGetLastError());
-        ctx->st.kernel_launches += 1;
-    }
+    reproj_launches(ctx, base, L, B, n_vec, max_vec, max_sc, sub, cut, maxReproj, minDepth);
+    CK(cudaGetLastError());
     mark(ctx, EV_SCORE);
     if (grads && !g_dev) {
         rc = copy_packed(ctx, (char* const*)grads, bytes, g_off, (char*)ctx->grads.p, false, ctx->stream);
         if (rc) return rc;
     }
-    CK(cudaMemcpyAsync(out_losses, base + off_loss, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(out_losses, base + L.loss, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
@@ -2580,18 +2699,10 @@ int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pre
     DeviceGuard device_guard(ctx->device);
     if (!pred || !gt || !Hp || !Wp || !Hg || !Wg || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
     if (B <= 0) return fail(ctx, ESACB200_ERR_ARG, "bad sizes B=%d", B);
-    for (int b = 0; b < B; ++b) {
-        if (Hp[b] <= 0 || Wp[b] <= 0 || Hg[b] <= 0 || Wg[b] <= 0)
-            return fail(ctx, ESACB200_ERR_ARG, "image %d: bad sizes prediction %dx%d ground truth %dx%d", b, Hp[b], Wp[b], Hg[b], Wg[b]);
-        if (abs(Hp[b] - Hg[b]) > 1 || abs(Wp[b] - Wg[b]) > 1)   // util.assert_size tolerates 1 cell
-            return fail(ctx, ESACB200_ERR_ARG, "image %d: size mismatch: prediction %dx%d, ground truth %dx%d (at most 1 apart)", b,
-                        Hp[b], Wp[b], Hg[b], Wg[b]);
-        if ((long long)Hp[b] * Wp[b] > (1ll << 30) || (long long)Hg[b] * Wg[b] > (1ll << 30))
-            return fail(ctx, ESACB200_ERR_ARG, "image %d: map too large", b);
-    }
-    bool p_dev = false, q_dev = false, g_dev = false;
-    int rc = pointer_kind(ctx, (const void* const*)pred, B, "pred", p_dev);
+    int rc = coord_sizes(ctx, nullptr, B, Hp, Wp, Hg, Wg);
     if (rc) return rc;
+    bool p_dev = false, q_dev = false, g_dev = false;
+    if ((rc = pointer_kind(ctx, (const void* const*)pred, B, "pred", p_dev))) return rc;
     if ((rc = pointer_kind(ctx, (const void* const*)gt, B, "gt", q_dev))) return rc;
     if (grads && (rc = pointer_kind(ctx, (const void* const*)grads, B, "grads", g_dev))) return rc;
     begin_call(ctx);
@@ -2605,50 +2716,27 @@ int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pre
     if ((rc = stage_images(ctx, pred, pbytes, p_dev, true, ctx->coords, d_pred, p_off))) return rc;
     if ((rc = stage_images(ctx, gt, gbytes, q_dev, true, ctx->coords_alt, d_gt, q_off))) return rc;
     if (grads && (rc = stage_images(ctx, grads, pbytes, g_dev, false, ctx->grads, d_grads, g_off))) return rc;
-    std::vector<CoordImage> recs((size_t)B);
-    std::vector<char> vec((size_t)B);
-    long long parts = 0;
-    for (int b = 0; b < B; ++b) {
-        CoordImage& r = recs[b];
-        r.pred = d_pred[b];
-        r.gt = d_gt[b];
-        r.grads = d_grads[b];
-        vec[b] = coord_image(r, Hp[b], Wp[b], Hg[b], Wg[b]);
-        r.b = b;
-        r.part0 = parts;
-        parts += r.blocks;
-    }
-    std::vector<CoordImage> ordered;
+    std::vector<CoordImage> recs, ordered;
+    std::vector<char> vec;
+    const long long parts = coord_records(B, d_pred.data(), d_gt.data(), d_grads.data(), Hp, Wp, Hg, Wg, recs, vec);
     int n_vec, max_vec, max_sc;
     const size_t rec_bytes = order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
-    // scratch layout: [tickets B u32 | counts B u32, padded] [records] [losses B f64] [valid counts B i64] [partials 2 f64 each]
-    const size_t off_rec = ((size_t)B * 8 + 63) & ~(size_t)63, off_loss = (off_rec + rec_bytes + 63) & ~(size_t)63,
-                 off_cnt = off_loss + (((size_t)B * 8 + 63) & ~(size_t)63), off_part = off_cnt + (((size_t)B * 8 + 63) & ~(size_t)63);
-    CK(ctx->scratch.ensure(off_part + (size_t)parts * 2 * 8));
+    const LossLayout L = coord_layout(B, parts);
+    CK(ctx->scratch.ensure(L.end));
     char* base = (char*)ctx->scratch.p;
-    CK(cudaMemsetAsync(base, 0, off_rec, ctx->stream));
-    CK(cudaMemcpyAsync(base + off_rec, ordered.data(), rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemsetAsync(base, 0, L.rec, ctx->stream));
+    CK(cudaMemcpyAsync(base + L.rec, ordered.data(), rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
     mark(ctx, EV_H2D);
     mark(ctx, EV_FOLD);  // ms_score = the kernels alone
-    const CoordImage* d_rec = (const CoordImage*)(base + off_rec);
-    for (int path = 0; path < 2; ++path) {
-        const int n = path == 0 ? n_vec : B - n_vec;
-        if (n == 0) continue;
-        for (int pass = grads ? 1 : 2; pass <= 2; ++pass) {
-            launch_coord_loss(path == 0, pass, grads != nullptr, d_rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, cut,
-                              (unsigned*)base + B, (double*)(base + off_part), (unsigned*)base, (double*)(base + off_loss),
-                              (long long*)(base + off_cnt), ctx->stream);
-            CK(cudaGetLastError());
-            ctx->st.kernel_launches += 1;
-        }
-    }
+    coord_launches(ctx, base, L, B, grads != nullptr, n_vec, max_vec, max_sc, cut);
+    CK(cudaGetLastError());
     mark(ctx, EV_SCORE);
     if (grads && !g_dev) {
         rc = copy_packed(ctx, (char* const*)grads, pbytes, g_off, (char*)ctx->grads.p, false, ctx->stream);
         if (rc) return rc;
     }
-    CK(cudaMemcpyAsync(out_losses, base + off_loss, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_counts) CK(cudaMemcpyAsync(out_counts, base + off_cnt, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(out_losses, base + L.loss, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    if (out_counts) CK(cudaMemcpyAsync(out_counts, base + L.flags, (size_t)B * 8, cudaMemcpyDeviceToHost, ctx->stream));
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
@@ -2681,34 +2769,6 @@ int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int
 // read on the device, and a finish kernel writes the caller's outputs.  Nothing here synchronises, reads back or queries an
 // event, and a call that a capture records allocates nothing.
 
-static size_t align64(size_t n) { return (n + 63) & ~(size_t)63; }
-
-// Byte offsets in the loss workspace of a call of B images whose blocks have `parts` partials.
-//   reprojection: [tickets B u32] [img B x kReprojImgFloats f32] [records] [losses B f64] [bad B i32] [partials f64 each]
-//   coordinates:  [tickets B u32 | counts B u32] [records] [losses B f64] [valid counts B i64] [partials 2 f64 each]
-struct LossLayout {
-    size_t img = 0, rec, loss, flags, part, end;
-};
-static LossLayout reproj_layout(int B, long long parts) {
-    LossLayout L;
-    L.img = align64((size_t)B * 4);
-    L.rec = L.img + align64((size_t)B * kReprojImgFloats * sizeof(float));
-    L.loss = L.rec + align64((size_t)B * sizeof(ReprojImage));
-    L.flags = L.loss + align64((size_t)B * 8);
-    L.part = L.flags + align64((size_t)B * 4);
-    L.end = L.part + (size_t)parts * 8;
-    return L;
-}
-static LossLayout coord_layout(int B, long long parts) {
-    LossLayout L;
-    L.rec = align64((size_t)B * 8);
-    L.loss = L.rec + align64((size_t)B * sizeof(CoordImage));
-    L.flags = L.loss + align64((size_t)B * 8);
-    L.part = L.flags + align64((size_t)B * 8);
-    L.end = L.part + (size_t)parts * 2 * 8;
-    return L;
-}
-
 // Makes the loss workspace hold `bytes`: grows it when no capture has used it yet, else fails without touching it.
 static int loss_workspace(esacb200_ctx* ctx, esacb200_ctx* a, size_t bytes, bool capturing, const char* what) {
     if (bytes <= a->loss_ws.cap) return 0;
@@ -2718,18 +2778,6 @@ static int loss_workspace(esacb200_ctx* ctx, esacb200_ctx* a, size_t bytes, bool
                     "replayed; call reserve_loss_async (esacb200_reserve_loss_async) with the largest batch and map before the "
                     "first capture", what, bytes, capturing ? "was reserved before this capture" : "an earlier capture used");
     CK(a->loss_ws.ensure(bytes));
-    return 0;
-}
-
-// The n named arguments are device memory (a null one is an error unless `optional` has its bit set).
-static int device_args(esacb200_ctx* ctx, const char* what, int n, const void* const* ptrs, const char* const* names, unsigned optional = 0) {
-    for (int i = 0; i < n; ++i) {
-        if (!ptrs[i]) {
-            if (optional >> i & 1) continue;
-            return fail(ctx, ESACB200_ERR_ARG, "%s: %s is null", what, names[i]);
-        }
-        if (!is_device_ptr(ptrs[i])) return fail(ctx, ESACB200_ERR_ARG, "%s takes device pointers only: %s is host memory", what, names[i]);
-    }
     return 0;
 }
 
@@ -2755,12 +2803,8 @@ int esacb200_reserve_loss_async(esacb200_ctx* ctx, int B, int H, int W) try {
     DeviceGuard device_guard(ctx->device);
     if (B <= 0 || H <= 0 || W <= 0 || (long long)H * W > (1ll << 30))
         return fail(ctx, ESACB200_ERR_ARG, "reserve_loss_async: bad sizes B=%d H=%d W=%d", B, H, W);
-    bool capturing = false;
-    int rc = stream_capturing(ctx, capturing);
-    if (rc) return rc;
-    if (capturing) return fail(ctx, ESACB200_ERR_ARG, "reserve_loss_async allocates: call it before the capture");
     esacb200_ctx* a = nullptr;
-    rc = async_context(ctx, false, "loss_async", &a);
+    const int rc = reserve_context(ctx, "loss_async", &a);
     if (rc) return rc;
     const long long parts = (long long)B * reproj_max_blocks(H * W);
     return loss_workspace(ctx, a, std::max(reproj_layout(B, parts).end, coord_layout(B, parts).end), false, "reserve_loss_async");
@@ -2774,34 +2818,19 @@ int esacb200_reproj_loss_async(esacb200_ctx* ctx, int B, const float* const* coo
     const char* what = "reproj_loss_async";
     if (!coords || !H || !W) return fail(ctx, ESACB200_ERR_ARG, "%s: null pointer or size array", what);
     if (B <= 0 || B > 65535 || sub <= 0) return fail(ctx, ESACB200_ERR_ARG, "%s: bad sizes B=%d sub=%d", what, B, sub);
-    for (int b = 0; b < B; ++b) {
-        if (H[b] <= 0 || W[b] <= 0) return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: bad size %dx%d", what, b, W[b], H[b]);
-        if ((long long)H[b] * W[b] > (1ll << 30)) return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: map %dx%d too large", what, b, W[b], H[b]);
-    }
     const void* ptrs[] = {gt_poses, shifts, cameras, out_losses, out_status};
     const char* names[] = {"gt_poses", "shifts", "cameras", "out_losses", "out_status"};
-    int rc = device_args(ctx, what, 5, ptrs, names);
+    int rc = reproj_sizes(ctx, what, B, H, W);
+    if (!rc) rc = device_args(ctx, what, 5, ptrs, names);
     if (!rc) rc = device_images(ctx, what, "coords", (const void* const*)coords, B);
     if (!rc && grads) rc = device_images(ctx, what, "grads", (const void* const*)grads, B);
     if (rc) return rc;
     esacb200_ctx* a = nullptr;
     bool capturing = false;
     if ((rc = begin_loss_async(ctx, a, capturing))) return rc;
-    std::vector<ReprojImage> recs((size_t)B), ordered;
-    std::vector<char> vec((size_t)B);
-    long long parts = 0;
-    for (int b = 0; b < B; ++b) {
-        ReprojImage& r = recs[b];
-        r.coords = coords[b];
-        r.grads = grads ? grads[b] : nullptr;
-        r.N = H[b] * W[b];
-        r.W = W[b];
-        r.b = b;
-        r.blocks = reproj_blocks_per_image(r.N);
-        r.part0 = parts;
-        parts += r.blocks;
-        vec[b] = reproj_vec_ok(r.coords, r.grads, r.N, r.W);
-    }
+    std::vector<ReprojImage> recs, ordered;
+    std::vector<char> vec;
+    const long long parts = reproj_records(B, coords, grads, H, W, recs, vec);
     int n_vec, max_vec, max_sc;
     order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
     const LossLayout L = reproj_layout(B, parts);
@@ -2809,18 +2838,12 @@ int esacb200_reproj_loss_async(esacb200_ctx* ctx, int B, const float* const* coo
     if (capturing) a->loss_frozen = true;
     char* base = (char*)a->loss_ws.p;
     ReprojImage* d_rec = (ReprojImage*)(base + L.rec);
-    float* img = (float*)(base + L.img);
     double* losses = (double*)(base + L.loss);
     int* bad = (int*)(base + L.flags);
     CK(cudaMemsetAsync(base, 0, L.img, a->stream));
-    a->st.kernel_launches += launch_reproj_prep(ordered.data(), B, d_rec, gt_poses, shifts, cameras, img, bad, a->stream);
-    for (int path = 0; path < 2; ++path) {
-        const int n = path == 0 ? n_vec : B - n_vec;
-        if (n == 0) continue;
-        launch_reproj(path == 0, d_rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, img, (float)sub, cut, maxReproj,
-                      minDepth, (double*)(base + L.part), (unsigned*)base, losses, a->stream);
-        a->st.kernel_launches += 1;
-    }
+    a->st.kernel_launches +=
+        launch_reproj_prep(ordered.data(), B, d_rec, gt_poses, shifts, cameras, (float*)(base + L.img), bad, a->stream);
+    reproj_launches(a, base, L, B, n_vec, max_vec, max_sc, sub, cut, maxReproj, minDepth);
     launch_reproj_finish(d_rec, B, grads != nullptr, losses, bad, out_losses, out_status, a->stream);
     a->st.kernel_launches += 1;
     CK(cudaGetLastError());
@@ -2835,19 +2858,10 @@ int esacb200_coord_loss_async(esacb200_ctx* ctx, int B, const float* const* pred
     const char* what = "coord_loss_async";
     if (!pred || !gt || !Hp || !Wp || !Hg || !Wg) return fail(ctx, ESACB200_ERR_ARG, "%s: null pointer or size array", what);
     if (B <= 0 || B > 65535) return fail(ctx, ESACB200_ERR_ARG, "%s: bad sizes B=%d", what, B);
-    for (int b = 0; b < B; ++b) {
-        if (Hp[b] <= 0 || Wp[b] <= 0 || Hg[b] <= 0 || Wg[b] <= 0)
-            return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: bad sizes prediction %dx%d ground truth %dx%d", what, b, Hp[b], Wp[b],
-                        Hg[b], Wg[b]);
-        if (abs(Hp[b] - Hg[b]) > 1 || abs(Wp[b] - Wg[b]) > 1)   // util.assert_size tolerates 1 cell
-            return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: size mismatch: prediction %dx%d, ground truth %dx%d (at most 1 apart)",
-                        what, b, Hp[b], Wp[b], Hg[b], Wg[b]);
-        if ((long long)Hp[b] * Wp[b] > (1ll << 30) || (long long)Hg[b] * Wg[b] > (1ll << 30))
-            return fail(ctx, ESACB200_ERR_ARG, "%s: image %d: map too large", what, b);
-    }
     const void* ptrs[] = {out_losses, out_counts};
     const char* names[] = {"out_losses", "out_counts"};
-    int rc = device_args(ctx, what, 2, ptrs, names, 2u);
+    int rc = coord_sizes(ctx, what, B, Hp, Wp, Hg, Wg);
+    if (!rc) rc = device_args(ctx, what, 2, ptrs, names, 2u);
     if (!rc) rc = device_images(ctx, what, "pred", (const void* const*)pred, B);
     if (!rc) rc = device_images(ctx, what, "gt", (const void* const*)gt, B);
     if (!rc && grads) rc = device_images(ctx, what, "grads", (const void* const*)grads, B);
@@ -2855,40 +2869,20 @@ int esacb200_coord_loss_async(esacb200_ctx* ctx, int B, const float* const* pred
     esacb200_ctx* a = nullptr;
     bool capturing = false;
     if ((rc = begin_loss_async(ctx, a, capturing))) return rc;
-    std::vector<CoordImage> recs((size_t)B), ordered;
-    std::vector<char> vec((size_t)B);
-    long long parts = 0;
-    for (int b = 0; b < B; ++b) {
-        CoordImage& r = recs[b];
-        r.pred = pred[b];
-        r.gt = gt[b];
-        r.grads = grads ? grads[b] : nullptr;
-        vec[b] = coord_image(r, Hp[b], Wp[b], Hg[b], Wg[b]);
-        r.b = b;
-        r.part0 = parts;
-        parts += r.blocks;
-    }
+    std::vector<CoordImage> recs, ordered;
+    std::vector<char> vec;
+    const long long parts = coord_records(B, pred, gt, grads, Hp, Wp, Hg, Wg, recs, vec);
     int n_vec, max_vec, max_sc;
     order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
     const LossLayout L = coord_layout(B, parts);
     if ((rc = loss_workspace(ctx, a, L.end, capturing, what))) return rc;
     if (capturing) a->loss_frozen = true;
     char* base = (char*)a->loss_ws.p;
-    CoordImage* d_rec = (CoordImage*)(base + L.rec);
-    double* losses = (double*)(base + L.loss);
-    long long* counts = (long long*)(base + L.flags);
     CK(cudaMemsetAsync(base, 0, L.rec, a->stream));
-    a->st.kernel_launches += launch_coord_prep(ordered.data(), B, d_rec, a->stream);
-    for (int path = 0; path < 2; ++path) {
-        const int n = path == 0 ? n_vec : B - n_vec;
-        if (n == 0) continue;
-        for (int pass = grads ? 1 : 2; pass <= 2; ++pass) {
-            launch_coord_loss(path == 0, pass, grads != nullptr, d_rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, cut,
-                              (unsigned*)base + B, (double*)(base + L.part), (unsigned*)base, losses, counts, a->stream);
-            a->st.kernel_launches += 1;
-        }
-    }
-    launch_coord_finish(B, losses, counts, out_losses, (long long*)out_counts, a->stream);
+    a->st.kernel_launches += launch_coord_prep(ordered.data(), B, (CoordImage*)(base + L.rec), a->stream);
+    coord_launches(a, base, L, B, grads != nullptr, n_vec, max_vec, max_sc, cut);
+    launch_coord_finish(B, (const double*)(base + L.loss), (const long long*)(base + L.flags), out_losses, (long long*)out_counts,
+                        a->stream);
     a->st.kernel_launches += 1;
     CK(cudaGetLastError());
     return ESACB200_OK;

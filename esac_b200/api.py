@@ -14,6 +14,7 @@ from __future__ import annotations
 import contextlib
 import ctypes as C
 import math
+import numbers
 import os
 from pathlib import Path
 
@@ -148,6 +149,15 @@ def load_library() -> C.CDLL:
     lib.esacb200_hypotheses_forward_async.argtypes = [vp, i32, vp, i32, i32, i32, vp, i64, i32, vp, vp, f32, f32, f32, f32, i32,
                                                       vp, C.c_size_t, vp, vp, vp, vp]
     lib.esacb200_hypotheses_forward_async.restype = i32
+    # the hypotheses node with a probability floor of the caller's (min_prob after subSampling)
+    lib.esacb200_hypotheses_forward_floor.argtypes = [vp, vp, i32, i32, i32, vp, i64, i32] + cam + [f64, vp, C.c_size_t, vp, vp, vp]
+    lib.esacb200_hypotheses_forward_floor.restype = i32
+    lib.esacb200_hypotheses_forward_ragged_floor.argtypes = ([vp, i32, vp, vp, vp, i32, vp, i64, i32] + cams +
+                                                             [f64, vp, vp, vp, vp, vp])
+    lib.esacb200_hypotheses_forward_ragged_floor.restype = i32
+    lib.esacb200_hypotheses_forward_async_floor.argtypes = [vp, i32, vp, i32, i32, i32, vp, i64, i32, vp, vp, f32, f32, f32, f32,
+                                                            i32, f64, vp, C.c_size_t, vp, vp, vp, vp]
+    lib.esacb200_hypotheses_forward_async_floor.restype = i32
     lib.esacb200_hypotheses_backward_async.argtypes = [vp, i32, vp, C.c_size_t, vp, vp, i32, i32, i32, i32, vp, vp, vp]
     lib.esacb200_hypotheses_backward_async.restype = i32
     lib.esacb200_pose_loss_async.argtypes = [vp, i32, i32, vp, vp, f32, f32, f32, vp, vp]
@@ -949,17 +959,42 @@ def hypotheses_tape_bytes(E: int, H: int, W: int, M: int) -> int:
     return int(load_library().esacb200_hypotheses_tape_bytes(int(E), int(H), int(W), int(M)))
 
 
+PROB_THRESH = 1e-3  # the reference's probability threshold (ESACB200_PROB_THRESH): the hypotheses node's default floor
+
+
+def _min_prob(minProb, call: str, name: str = "minProb") -> float:
+    """The hypotheses node's probability floor (argument `name` of `call`) as a float in [0, 1], NaN refused; raises
+    RuntimeError before any context exists, so the check runs without a GPU."""
+    if isinstance(minProb, (bool, np.bool_)) or not isinstance(minProb, numbers.Real):
+        raise RuntimeError(f"{call}: {name} must be a number in [0, 1], got a {type(minProb).__name__}")
+    v = float(minProb)
+    if not 0.0 <= v <= 1.0:
+        raise RuntimeError(f"{call}: {name} must lie in [0, 1], got {v}")
+    return v
+
+
+def _floor_entry(lib, name: str, minProb: float):
+    """esacb200_`name` and the floor arguments it takes after subSampling: at the default floor the entry point without
+    one (which is the _floor entry point with ESACB200_PROB_THRESH), else esacb200_`name`_floor with minProb."""
+    if minProb == PROB_THRESH:
+        return getattr(lib, "esacb200_" + name), ()
+    return getattr(lib, f"esacb200_{name}_floor"), (minProb,)
+
+
 def _out_device(a: _Arg):
     import torch
     return torch.device("cuda", a.device) if a.is_cuda else torch.device("cpu")
 
 
 def hypotheses_forward(sceneCoordinates, hypAssignment, shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
-                       inlierAlpha, inlierBeta, maxReproj, subSampling):
+                       inlierAlpha, inlierBeta, maxReproj, subSampling, minProb=PROB_THRESH):
     """The hypotheses of an esac.backward call at the same point of the context's call sequence: the same draws, scores and
     refinements.  Returns torch tensors (scores float64 [M], poses float64 [M,6] = (rvec, tvec), refined where p >=
-    PROB_THRESH and initial elsewhere, contributing bool [M]) on the coordinates' device (CPU for numpy input), and the tape:
-    a CUDA uint8 tensor holding what hypotheses_backward needs.  Runs on torch's current stream."""
+    minProb and initial elsewhere, contributing bool [M] = p >= minProb) on the coordinates' device (CPU for numpy input),
+    and the tape: a CUDA uint8 tensor holding what hypotheses_backward needs.  p is the hypothesis's softmax probability;
+    minProb in [0, 1] (default PROB_THRESH, the reference's truncation; 0 = every hypothesis, also those whose p underflows
+    to 0).  Runs on torch's current stream."""
+    minProb = _min_prob(minProb, "hypotheses_forward")
     _check(sceneCoordinates, "Float", 4, "sceneCoordinates")
     _check(hypAssignment, "Long", 1, "hypAssignment")
     E, three, H, W = (int(s) for s in sceneCoordinates.shape)
@@ -981,18 +1016,18 @@ def hypotheses_forward(sceneCoordinates, hypAssignment, shiftX, shiftY, focalLen
     scores = torch.empty(M, dtype=torch.float64, device=dev)
     poses = torch.empty(M, 6, dtype=torch.float64, device=dev)
     contributing = torch.empty(M, dtype=torch.bool, device=dev)
-    ctx.check(ctx.lib.esacb200_hypotheses_forward(ctx.handle, co.ptr, E, H, W, aptr, astride, M,
-                                                  *_camera_tail(shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
-                                                                inlierAlpha, inlierBeta, maxReproj, subSampling),
-                                                  tape.data_ptr(), nbytes, scores.data_ptr(), poses.data_ptr(),
-                                                  contributing.data_ptr()))
+    fn, floor = _floor_entry(ctx.lib, "hypotheses_forward", minProb)
+    ctx.check(fn(ctx.handle, co.ptr, E, H, W, aptr, astride, M,
+                 *_camera_tail(shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold, inlierAlpha, inlierBeta,
+                               maxReproj, subSampling),
+                 *floor, tape.data_ptr(), nbytes, scores.data_ptr(), poses.data_ptr(), contributing.data_ptr()))
     return scores, poses, contributing, tape
 
 
 def hypotheses_backward(tape, sceneCoordinates, outGradients, gradScores=None, gradPoses=None):
     """Accumulates (+=) into outGradients [E,3,H,W] the gradient of the scene coordinates for upstream gradients gradScores
     (float64 [M]) and gradPoses (float64 [M,6]) of a hypotheses_forward's outputs; None counts as zero, and entries of
-    hypotheses that do not contribute are ignored.  sceneCoordinates must hold the values the forward saw."""
+    hypotheses that do not contribute (p < the forward's minProb) are ignored.  sceneCoordinates must hold the values the forward saw."""
     _check(sceneCoordinates, "Float", 4, "sceneCoordinates")
     _check(outGradients, "Float", 4, "outGradients")
     shape = tuple(int(s) for s in sceneCoordinates.shape)
@@ -1035,14 +1070,15 @@ def _tape_hypotheses(tape, E: int, H: int, W: int, what: str) -> int:
 
 
 def hypotheses_forward_batch(sceneCoordinates, hypAssignment, shiftX, shiftY, focalLength, ppointX, ppointY, inlierThreshold,
-                             inlierAlpha, inlierBeta, maxReproj, subSampling):
+                             inlierAlpha, inlierBeta, maxReproj, subSampling, minProb=PROB_THRESH):
     """hypotheses_forward over a batch: image b draws, scores and refines what the b-th of B consecutive hypotheses_forward
     (or esac.backward) calls would, with its own shift and camera.  sceneCoordinates [B,E,3,H,W] float32 or a list / tuple of
     B [E,3,H_b,W_b] tensors; hypAssignment int64 [B,M] (a stride-0 [B,1].expand(B,M) included); shiftX, shiftY,
     focalLength, ppointX, ppointY each a number or B values.  Returns scores float64 [B,M], poses float64 [B,M,6],
     contributing bool [B,M] on the coordinates' device (CPU for numpy input), and the B tapes: views into one CUDA uint8
-    tensor, each at a 256-byte aligned offset.  The images run on worker streams (option batch_workers) after everything
-    queued on torch's current stream."""
+    tensor, each at a 256-byte aligned offset.  minProb: hypotheses_forward's, one floor for every image.  The images run on
+    worker streams (option batch_workers) after everything queued on torch's current stream."""
+    minProb = _min_prob(minProb, "hypotheses_forward_batch")
     maps = _Images(sceneCoordinates, 4, "sceneCoordinates")
     B, E = maps.B, _check_maps(maps.shapes, "sceneCoordinates")
     _check(hypAssignment, "Long", 2, "hypAssignment")
@@ -1067,9 +1103,10 @@ def hypotheses_forward_batch(sceneCoordinates, hypAssignment, shiftX, shiftY, fo
     contributing = torch.empty(B, M, dtype=torch.bool, device=dev)
     tape_ptrs = (C.c_void_p * B)(*[t.data_ptr() for t in tapes])
     tape_sizes = (C.c_size_t * B)(*sizes)
-    ctx.check(ctx.lib.esacb200_hypotheses_forward_ragged(
+    fn, floor = _floor_entry(ctx.lib, "hypotheses_forward_ragged", minProb)
+    ctx.check(fn(
         ctx.handle, B, maps.ptrs, maps.hs, maps.ws, E, ha.ptr, 1, M, *(a.ctypes.data for a in cams),
-        *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling), tape_ptrs, tape_sizes,
+        *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling), *floor, tape_ptrs, tape_sizes,
         scores.data_ptr(), poses.data_ptr(), contributing.data_ptr()))
     return scores, poses, contributing, tapes
 
@@ -1288,7 +1325,7 @@ def _check_tapes(tapes, B, E, H, W, M, call):
 
 
 def hypotheses_forward_async(sceneCoordinates, hypAssignment, shifts, cameras, inlierThreshold, inlierAlpha, inlierBeta,
-                             maxReproj, subSampling, tapes, outScores, outPoses, outContributing, outStatus):
+                             maxReproj, subSampling, tapes, outScores, outPoses, outContributing, outStatus, minProb=PROB_THRESH):
     """hypotheses_forward enqueued on torch's current stream with no host synchronisation, so that a training step with
     a pose loss of the caller's own can be captured in a CUDA graph.  CUDA tensors only: sceneCoordinates float32
     [B,E,3,H,W], hypAssignment int64 [B,M], shifts int32 [B,2], cameras float32 [B,3] (focal length, ppointX, ppointY),
@@ -1298,8 +1335,10 @@ def hypotheses_forward_async(sceneCoordinates, hypAssignment, shifts, cameras, i
     [0,E) (scores and poses NaN, nothing contributes).  [E,3,H,W] / [M] / [2] / [3] / [M,6] / [] tensors are one image.
     Seeding is forward_async's: image b of the j-th call after set_seed(s) draws what the (j*B + b)-th esac.backward or
     hypotheses_forward after set_seed(s) draws.  The workspace is backward_async's: call reserve_backward_async with the
-    largest shape before the first capture."""
+    largest shape before the first capture.  minProb: hypotheses_forward's; a captured graph keeps the floor it was
+    captured with (a training hyperparameter, not per-image data)."""
     call = "hypotheses_forward_async"
+    minProb = _min_prob(minProb, call)
     B, E, H, W, M = _async_shapes(sceneCoordinates, hypAssignment, shifts, cameras, call)
     lead = (B,) if sceneCoordinates.dim() == 5 else ()
     if not _is_torch(tapes):
@@ -1309,10 +1348,11 @@ def hypotheses_forward_async(sceneCoordinates, hypAssignment, shifts, cameras, i
                                 "outContributing": (outContributing, "Bool", lead + (M,)), "outStatus": (outStatus, "Int", lead)},
                          *_esac_inputs({"sceneCoordinates": sceneCoordinates, "hypAssignment": hypAssignment, "shifts": shifts,
                                         "cameras": cameras, "tapes": tapes}, lead, M))
-    ctx.check(ctx.lib.esacb200_hypotheses_forward_async(
+    fn, floor = _floor_entry(ctx.lib, "hypotheses_forward_async", minProb)
+    ctx.check(fn(
         ctx.handle, B, sceneCoordinates.data_ptr(), E, H, W, hypAssignment.data_ptr(), int(hypAssignment.stride(-1)), M,
         shifts.data_ptr(), cameras.data_ptr(), *_thresholds(inlierThreshold, inlierAlpha, inlierBeta, maxReproj, subSampling),
-        tapes.data_ptr(), int(tapes.numel()), outScores.data_ptr(), outPoses.data_ptr(), outContributing.data_ptr(),
+        *floor, tapes.data_ptr(), int(tapes.numel()), outScores.data_ptr(), outPoses.data_ptr(), outContributing.data_ptr(),
         outStatus.data_ptr()))
 
 

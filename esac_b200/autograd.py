@@ -334,25 +334,30 @@ class EsacHypotheses(torch.autograd.Function):
 
 
 def esac_hypotheses(scene_coordinates, hyp_assignment, shift_x, shift_y, focal_length, ppoint_x, ppoint_y,
-                    inlier_threshold, inlier_alpha, inlier_beta, max_reproj, sub_sampling):
+                    inlier_threshold, inlier_alpha, inlier_beta, max_reproj, sub_sampling, min_prob=api.PROB_THRESH):
     """The hypotheses of esac.backward as a differentiable function, so that a trainer can write its own pose loss in torch.
 
     scene_coordinates [E,3,H,W] float32 (CPU or CUDA), hyp_assignment [M] int64; the other arguments are esac.forward's.
     Returns, on the coordinates' device:
       scores        float64 [M]    the soft-inlier scores (softmax(scores) are the hypothesis probabilities),
-      poses         float64 [M,6]  scene pose (rvec, tvec) per hypothesis: refined where p >= PROB_THRESH, else initial,
-      contributing  bool [M]       p >= PROB_THRESH.
+      poses         float64 [M,6]  scene pose (rvec, tvec) per hypothesis: refined where p >= min_prob, else initial,
+      contributing  bool [M]       p >= min_prob,
+    p being the softmax probability of the hypothesis's score.
     It draws what an esac.backward call at the same point of the context's call sequence would draw, so with the option
     fixed_seed and the same seed its hypotheses, scores and refined poses are bitwise those of esac.backward.
 
     The backward gives d L / d scene_coordinates from the gradients of `scores` and `poses` (either may be absent, which
-    counts as zero).  As in the reference, only contributing hypotheses are differentiated: gradients reaching hypotheses
-    with p < PROB_THRESH are ignored, and a refined pose is differentiated through its refinement's linearisation, with the
-    reference's > 10 clamps.  The node is once differentiable.  With
+    counts as zero).  Only contributing hypotheses are differentiated: gradients reaching hypotheses with p < min_prob are
+    ignored, and a refined pose is differentiated through its refinement's linearisation, with the reference's > 10
+    clamps.  The node is once differentiable.  With the default min_prob = api.PROB_THRESH (the reference's truncation) and
         L = (softmax(scores) * reference_pose_loss(poses, gt_pose, w_rot, w_trans, cut)).sum()
-    L and its gradient are those of esac.backward / esac_loss."""
+    L and its gradient are those of esac.backward / esac_loss.  A loss that weighs hypotheses otherwise (best-of-M
+    min over reference_pose_loss(poses, ...), softmax(scores / T), a term on every pose) needs a lower floor, or the
+    hypotheses below 1e-3 enter it with their initial poses and no gradient: min_prob = 0 refines and differentiates
+    all M, at the cost of refining every hypothesis."""
+    min_prob = api._min_prob(min_prob, "esac_hypotheses", "min_prob")
     return EsacHypotheses.apply(scene_coordinates, hyp_assignment, shift_x, shift_y, focal_length, ppoint_x, ppoint_y,
-                                inlier_threshold, inlier_alpha, inlier_beta, max_reproj, sub_sampling)
+                                inlier_threshold, inlier_alpha, inlier_beta, max_reproj, sub_sampling, min_prob)
 
 
 class EsacHypothesesBatch(torch.autograd.Function):
@@ -382,7 +387,7 @@ class EsacHypothesesBatch(torch.autograd.Function):
 
 
 def esac_hypotheses_batch(scene_coordinates, hyp_assignment, shift_x, shift_y, focal_length, ppoint_x, ppoint_y,
-                          inlier_threshold, inlier_alpha, inlier_beta, max_reproj, sub_sampling):
+                          inlier_threshold, inlier_alpha, inlier_beta, max_reproj, sub_sampling, min_prob=api.PROB_THRESH):
     """esac_hypotheses over a batch of images, each with its own shift and camera: scene_coordinates [B,E,3,H,W] float32 or
     a list / tuple of B [E,3,H_b,W_b] tensors of different sizes (every element then receives its own gradient),
     hyp_assignment [B,M] int64; shift_x, shift_y, focal_length, ppoint_x, ppoint_y a number or B values.  Returns scores
@@ -390,9 +395,10 @@ def esac_hypotheses_batch(scene_coordinates, hyp_assignment, shift_x, shift_y, f
     calls would return, and the backward gives each image the gradient esac_hypotheses would.  The images run on the worker
     streams of api.backward_batch.  With
         L = (softmax(scores, 1) * reference_pose_loss(poses, gt_poses, w_rot, w_trans, cut)).sum(1)
-    L and its gradient are those of esac_loss_batch."""
+    L and its gradient are those of esac_loss_batch.  min_prob: esac_hypotheses's, one floor for every image."""
+    min_prob = api._min_prob(min_prob, "esac_hypotheses_batch", "min_prob")
     params = (shift_x, shift_y, focal_length, ppoint_x, ppoint_y, inlier_threshold, inlier_alpha, inlier_beta, max_reproj,
-              sub_sampling)
+              sub_sampling, min_prob)
     inputs, form = _as_inputs(scene_coordinates)
     return EsacHypothesesBatch.apply((form, hyp_assignment, params), *inputs)
 
@@ -405,7 +411,7 @@ class EsacHypothesesAsync(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, meta, scene_coordinates):
-        hyp_assignment, shifts, cameras, params, status = meta
+        hyp_assignment, shifts, cameras, params, status, min_prob = meta
         lead = tuple(scene_coordinates.shape[:-4])
         E, _, H, W = (int(v) for v in scene_coordinates.shape[-4:])
         M = int(hyp_assignment.shape[-1])
@@ -418,7 +424,7 @@ class EsacHypothesesAsync(torch.autograd.Function):
         if status is None:
             status = torch.empty(lead, dtype=torch.int32, device=dev)
         api.hypotheses_forward_async(scene_coordinates.detach(), hyp_assignment, shifts, cameras, *params, tapes, scores, poses,
-                                     contributing, status)
+                                     contributing, status, minProb=min_prob)
         # the coordinates are passed to the backward again; autograd's version counter catches an in-place change
         ctx.save_for_backward(scene_coordinates, tapes)
         ctx.mark_non_differentiable(contributing)
@@ -437,7 +443,8 @@ class EsacHypothesesAsync(torch.autograd.Function):
         return None, grads
 
 
-def esac_hypotheses_async(scene_coordinates, hyp_assignment, shifts, cameras, tau, alpha, beta, max_reproj, sub, status=None):
+def esac_hypotheses_async(scene_coordinates, hyp_assignment, shifts, cameras, tau, alpha, beta, max_reproj, sub, status=None,
+                          min_prob=api.PROB_THRESH):
     """esac_hypotheses (one image: scene_coordinates [E,3,H,W], hyp_assignment [M], shifts [2], cameras [3]) or
     esac_hypotheses_batch on a stacked batch (scene_coordinates [B,E,3,H,W], hyp_assignment [B,M], shifts [B,2] int32,
     cameras [B,3] = focal length, ppointX, ppointY) on the stream-ordered node, for training steps captured in a CUDA
@@ -446,8 +453,10 @@ def esac_hypotheses_async(scene_coordinates, hyp_assignment, shifts, cameras, ta
     for the same draws: image b of the j-th call draws what the (j*B + b)-th esac_hypotheses call draws.  Once
     differentiable; an absent upstream gradient counts as zero.  status: an int32 CUDA tensor [B] (or []) that receives the
     forward's per-image status (1 = a bad expert index: scores and poses NaN, no gradient); None keeps it internal.  Call
-    api.reserve_backward_async with the largest shape before the first capture."""
-    meta = (hyp_assignment, shifts, cameras, (tau, alpha, beta, max_reproj, sub), status)
+    api.reserve_backward_async with the largest shape before the first capture.  min_prob: esac_hypotheses's; a captured
+    graph replays with the floor it was captured with."""
+    min_prob = api._min_prob(min_prob, "esac_hypotheses_async", "min_prob")
+    meta = (hyp_assignment, shifts, cameras, (tau, alpha, beta, max_reproj, sub), status, min_prob)
     return EsacHypothesesAsync.apply(meta, scene_coordinates)
 
 

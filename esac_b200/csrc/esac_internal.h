@@ -242,15 +242,16 @@ int score_tile_pixels(int ppt);
 // k1, k0, tmax, tiny and fold of the scoring arguments for this problem
 void score_constants(const Problem& P, ScoreArgs& a);
 void launch_score(const ScoreArgs& a, int ppt, int grid, cudaStream_t st);
-// scores[h] = (alpha/W/H) * sum_tiles part ; softmax ; entropy ; argmax ; contributing list
+// scores[h] = (alpha/W/H) * sum_tiles part ; softmax ; entropy ; argmax ; contributing list (the hypotheses with
+// !(p < min_prob), in ascending order; kProbThresh everywhere but the hypotheses node)
 // into stats: entropy, winner, n_contrib, max_score, sum_exp
 void launch_select(const float* part, const int* slot_of, const Problem& P, int T, double* scores, double* probs,
-                   CallStats* stats, int* winner, int* contrib, int* n_contrib, cudaStream_t st);
+                   CallStats* stats, int* winner, int* contrib, int* n_contrib, double min_prob, cudaStream_t st);
 
 void launch_rescale_probs(const double* scores, const Problem& P, double gmax, double gsum, double* probs, int* contrib,
-                          int* n_contrib, cudaStream_t st);
+                          int* n_contrib, double min_prob, cudaStream_t st);
 void launch_rescale_probs_gathered(const double* scores, const Problem& P, const double* pairs, int world, double* norm_out,
-                                   double* probs, int* contrib, int* n_contrib, cudaStream_t st);
+                                   double* probs, int* contrib, int* n_contrib, double min_prob, cudaStream_t st);
 
 // --- hyp.cu -------------------------------------------------------------------------------
 // Work state of the sampling waves (all device memory, M = hypotheses).
@@ -540,6 +541,7 @@ struct TapeHead {
     int n_contrib;  // written on the device by the forward
     int M, mask_words;
     Problem P;
+    double min_prob;  // the forward's probability floor: its records are the hypotheses with !(p < min_prob)
 };
 constexpr unsigned kTapeMagic = 0x45534831u;  // "ESH1"
 constexpr size_t kTapeHeadBytes = 256;

@@ -83,6 +83,12 @@ int esacb200_backward(esacb200_ctx* ctx, const float* coords, float* grads, int 
  *   out_scores  double [M]    the soft-inlier scores the softmax sees,
  *   out_poses6  double [M,6]  scene pose (rvec, tvec) per hypothesis: refined where p >= PROB_THRESH, initial elsewhere,
  *   out_contrib uint8  [M]    1 where p >= PROB_THRESH (the hypotheses the backward differentiates);
+ * p being the hypothesis's softmax probability.  The _floor variants take that threshold as `min_prob` in [0, 1] (NaN or a
+ * value outside fails with ESACB200_ERR_ARG before anything is enqueued): exactly the hypotheses with !(p < min_prob) are
+ * refined, flagged and differentiated, so min_prob = 0 takes all M, also those whose p underflows to 0.  The entries
+ * without the suffix are the _floor ones with min_prob = ESACB200_PROB_THRESH, the reference's own truncation, which is
+ * right for its loss softmax(scores) . loss and loses the gradient of any hypothesis below it under other losses
+ * (best-of-M, a sharper softmax, a per-hypothesis term).
  * host or device pointers.  Everything its backward needs goes to `tape`: 16-byte aligned device memory of at least
  * esacb200_hypotheses_tape_bytes(E, H, W, M) bytes, owned by the caller and untouched by any other call, so other library
  * calls may run between a forward and its backward.  Returns 0 for non-positive or oversized arguments.
@@ -100,6 +106,13 @@ int esacb200_hypotheses_forward(esacb200_ctx* ctx, const float* coords, int E, i
                                 uint8_t* out_contrib);
 int esacb200_hypotheses_backward(esacb200_ctx* ctx, const void* tape, const float* coords, float* grads, int E, int H, int W,
                                  const double* d_scores, const double* d_poses6);
+/* The reference's probability threshold (esac_derivative.h PROB_THRESH): the default floor of the hypotheses node. */
+#define ESACB200_PROB_THRESH 0.001
+int esacb200_hypotheses_forward_floor(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
+                                      int64_t assign_stride, int M, int shiftX, int shiftY, float focalLength, float ppointX,
+                                      float ppointY, float inlierThreshold, float inlierAlpha, float inlierBeta,
+                                      float maxReproj, int subSampling, double min_prob, void* tape, size_t tape_bytes,
+                                      double* out_scores, double* out_poses6, uint8_t* out_contrib);
 
 /* The reference's pose loss (esac_loss.h loss) and its dLoss, quirks included, of M scene poses (rvec, tvec) double [M,6]
  * against a float32 [4,4] camera->world ground truth: out_losses double [M], out_dloss6 double [M,6].  Host or device
@@ -127,6 +140,12 @@ int esacb200_hypotheses_forward_ragged(esacb200_ctx* ctx, int B, const float* co
                                        float inlierAlpha, float inlierBeta, float maxReproj, int subSampling,
                                        void* const* tapes, const size_t* tape_bytes, double* out_scores, double* out_poses6,
                                        uint8_t* out_contrib);
+int esacb200_hypotheses_forward_ragged_floor(esacb200_ctx* ctx, int B, const float* const* coords, const int* H, const int* W,
+                                             int E, const int64_t* assign, int64_t assign_stride, int M, const int* shiftX,
+                                             const int* shiftY, const float* f, const float* ppx, const float* ppy,
+                                             float inlierThreshold, float inlierAlpha, float inlierBeta, float maxReproj,
+                                             int subSampling, double min_prob, void* const* tapes, const size_t* tape_bytes,
+                                             double* out_scores, double* out_poses6, uint8_t* out_contrib);
 int esacb200_hypotheses_backward_ragged(esacb200_ctx* ctx, int B, const void* const* tapes, const float* const* coords,
                                         float* const* grads, const int* H, const int* W, int E, const double* d_scores,
                                         const double* d_poses6);
@@ -295,6 +314,12 @@ int esacb200_hypotheses_forward_async(esacb200_ctx* ctx, int B, const float* coo
                                       float inlierThreshold, float inlierAlpha, float inlierBeta, float maxReproj, int subSampling,
                                       void* tapes, size_t tapes_bytes, double* out_scores, double* out_poses6,
                                       uint8_t* out_contrib, int32_t* out_status);
+/* The floor is a kernel parameter: a captured graph replays with the min_prob it was captured with. */
+int esacb200_hypotheses_forward_async_floor(esacb200_ctx* ctx, int B, const float* coords, int E, int H, int W,
+                                            const int64_t* assign, int64_t assign_stride, int M, const int32_t* shifts,
+                                            const float* cameras, float inlierThreshold, float inlierAlpha, float inlierBeta,
+                                            float maxReproj, int subSampling, double min_prob, void* tapes, size_t tapes_bytes,
+                                            double* out_scores, double* out_poses6, uint8_t* out_contrib, int32_t* out_status);
 int esacb200_hypotheses_backward_async(esacb200_ctx* ctx, int B, const void* tapes, size_t tapes_bytes, const float* coords,
                                        float* grads, int E, int H, int W, int M, const double* d_scores, const double* d_poses6,
                                        int32_t* out_status);

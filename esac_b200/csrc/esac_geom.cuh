@@ -7,7 +7,7 @@
 //                                                              (replaces cv::solvePnP(SOLVEPNP_P3P); esac_util.h:189-197, esac_derivative.h:153,164)
 //   * small dense helpers: 6x6 Cholesky solve, symmetric Jacobi eigen-decomposition (SVD pseudo-inverse,
 //     esac.cpp:434)
-// Everything is __host__ __device__ so the CPU test-hooks in esac_capi.cu can check the very same
+// Everything is __host__ __device__ so the CPU test-hooks in capi_testhooks.cu can check the very same
 // code against cv2 without a GPU.
 #pragma once
 #include <math.h>

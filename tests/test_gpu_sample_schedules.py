@@ -20,10 +20,10 @@ from oracle import esac_oracle as O
 pytestmark = pytest.mark.gpu
 
 POSE_TOL = 1e-8            # test_gpu_forward.py::test_sampling_matches_oracle_stream
-SAMPLE_CAP = 1 << 19       # capi.cu kSampleCap: survivors per lane and wave
-SAMPLE_CAP_ACC = 1 << 15   # capi.cu kSampleCapAcc: staged accepts per lane and call
+SAMPLE_CAP = 1 << 19       # capi_pipeline.cu kSampleCap: survivors per lane and wave
+SAMPLE_CAP_ACC = 1 << 15   # capi_pipeline.cu kSampleCapAcc: staged accepts per lane and call
 FIXED_SEED = 1             # every call of this module draws from set_seed's seed itself
-# the library's defaults (capi.cu, struct Options) of every option this module sets
+# the library's defaults (capi_internal.h, struct Options) of every option this module sets
 LIBRARY_DEFAULTS = {"max_tries": 1000000, "sample_prefilter": 1, "sample_span0": 256, "sample_window": 1.25,
                     "sample_waves": 6, "sample_tail_boost": 1, "sample_groups": 2, "sample_trace": 0, "upload_split": 1,
                     "hyp_offset": 0, "hyp_stride": 1, "fixed_seed": 0}

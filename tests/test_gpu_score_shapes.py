@@ -1,6 +1,6 @@
 """Every scoring launch shape against the float64 reference (oracle/score_fp64.py), not only the ones the heuristics pick.
 
-plan_and_prep (capi.cu) picks ppt (cells per thread, tile = 256 * ppt cells), hc (hypotheses per chunk) and one of three
+plan_and_prep (capi_pipeline.cu) picks ppt (cells per thread, tile = 256 * ppt cells), hc (hypotheses per chunk) and one of three
 load paths from `vec_ok = N % a == 0 and base % (4 a) == 0`, a = 4 if ppt >= 4 else 2:
   TMA bulk copies when vec_ok and ppt >= 4; vector __ldg when vec_ok and ppt == 2; scalar loads otherwise,
 each with a ragged-tail form when N % tile != 0.  The options score_ppt / score_hc force the shape; the test ids name the
@@ -34,7 +34,7 @@ def api():
 
 
 def load_path(N: int, ptr: int, ppt: int) -> str:
-    """The load path plan_and_prep / launch_score pick (capi.cu, score.cu), plus '-tail' for a ragged last tile."""
+    """The load path plan_and_prep / launch_score pick (capi_pipeline.cu, score.cu), plus '-tail' for a ragged last tile."""
     a = 4 if ppt >= 4 else 2
     vec_ok = N % a == 0 and ptr % (4 * a) == 0
     path = "tma" if vec_ok and ppt >= 4 else ("vec" if vec_ok else "scalar")

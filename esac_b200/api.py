@@ -91,6 +91,18 @@ def load_library() -> C.CDLL:
     lib.esacb200_backward_batch_cameras.restype = i32
     lib.esacb200_assign_hypotheses.argtypes = [vp, i32, i32, i32, vp, i32, i32, C.c_uint64, vp, vp]
     lib.esacb200_assign_hypotheses.restype = i32
+    lib.esacb200_assign_hypotheses_async.argtypes = [vp, i32, i32, i32, vp, i32, i32, vp, vp, vp, vp]
+    lib.esacb200_assign_hypotheses_async.restype = i32
+    lib.esacb200_gate_create.argtypes = [vp, i32, C.POINTER(vp)]
+    lib.esacb200_gate_create.restype = i32
+    lib.esacb200_gate_destroy.argtypes = [vp]
+    lib.esacb200_gate_destroy.restype = None
+    lib.esacb200_gate_arm.argtypes = [vp, vp, vp]
+    lib.esacb200_gate_arm.restype = i32
+    lib.esacb200_gate_mark.argtypes = [vp, i32, i32, vp]
+    lib.esacb200_gate_mark.restype = i32
+    lib.esacb200_gate_finalize.argtypes = [vp, vp]
+    lib.esacb200_gate_finalize.restype = i32
     lib.esacb200_reproj_loss.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp, f32, f32, f32, i32, f32, f32, f32, vp]
     lib.esacb200_reproj_loss.restype = i32
     lib.esacb200_reproj_loss_cameras.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp, vp, vp, vp, i32, f32, f32, f32, vp]
@@ -201,6 +213,8 @@ def load_library() -> C.CDLL:
     lib.esacb200_host_pinv6.restype = None
     lib.esacb200_host_draw_cells.argtypes = [C.c_uint64, C.c_uint32, C.c_uint32, i32, i32, vp]
     lib.esacb200_host_draw_cells.restype = None
+    lib.esacb200_graph_node_types.argtypes = [vp, vp, i32]
+    lib.esacb200_graph_node_types.restype = i32
     _lib = lib
     return lib
 
@@ -760,6 +774,48 @@ def assign_hypotheses(gatingProbs, hypotheses: int, seed: int, maxExperts: int =
     ctx.check(ctx.lib.esacb200_assign_hypotheses(ctx.handle, B, E, M, gp.ptr, int(maxExperts), int(bool(expertSelection)),
                                                  int(seed) & 0xFFFFFFFFFFFFFFFF, ap, hp))
     return assign, hist
+
+
+MAX_EXPERTS = 1024  # experts one assignment CTA holds, and handles one ExpertGate holds (include/esac_b200.h)
+
+
+def assign_hypotheses_async(gatingProbs, hypotheses, seed, outAssign, outHist, outStatus, maxExperts: int = -1,
+                            expertSelection: bool = False):
+    """assign_hypotheses enqueued on torch's current stream with no host synchronisation, so that a CUDA graph can capture
+    the draw.  CUDA tensors only: gatingProbs float32 [B,E] (or [E]), seed int64 [1] (or []), read when the kernel runs --
+    a graph can advance it (seed.add_(1) in the capture) or the caller can write a new one before each replay; the results
+    go to outAssign int64 [B,M] (M = hypotheses), outHist float32 [B,E] or None and outStatus int32 [B] (0; 1 for a row
+    with a negative, NaN or infinite probability; 2 for a row that sums to 0 -- where assign_hypotheses raises; that row's
+    draws are then meaningless).  Given the same seed value it draws bitwise what assign_hypotheses draws."""
+    call = "assign_hypotheses_async"
+    if not _is_torch(gatingProbs):
+        raise RuntimeError(f"{call} takes torch CUDA tensors only (gatingProbs is a {type(gatingProbs).__name__})")
+    if _dtype_name(gatingProbs) != "Float":
+        raise RuntimeError(f"expected scalar type Float but found {_dtype_name(gatingProbs)} (gatingProbs)")
+    if gatingProbs.dim() not in (1, 2):
+        raise RuntimeError(f"gatingProbs must be [B,E] or [E], got {list(gatingProbs.shape)}")
+    lead = tuple(int(v) for v in gatingProbs.shape[:-1])
+    B, E, M = (lead[0] if lead else 1), int(gatingProbs.shape[-1]), int(hypotheses)
+    if B < 1 or E < 1 or M < 1:
+        raise RuntimeError(f"{call}: sizes must be positive, got B={B} E={E} M={M}")
+    if E > MAX_EXPERTS:
+        raise RuntimeError(f"{call}: E={E} exceeds the {MAX_EXPERTS} experts one CTA holds")
+    if not _is_torch(seed) or _dtype_name(seed) != "Long" or int(seed.numel()) != 1:
+        raise RuntimeError(f"seed must be an int64 CUDA tensor of one element, got "
+                           f"{_dtype_name(seed) if _is_torch(seed) else type(seed).__name__}"
+                           f"{list(seed.shape) if _is_torch(seed) else ''}")
+    fixed = {"outAssign": (outAssign, "Long", lead + (M,)), "outStatus": (outStatus, "Int", lead)}
+    if outHist is not None:
+        fixed["outHist"] = (outHist, "Float", lead + (E,))
+
+    def check():
+        if not gatingProbs.is_contiguous():
+            raise RuntimeError("gatingProbs must be contiguous (a copy would not be captured with the call)")
+    ctx = _async_context(call, fixed, [("gatingProbs", gatingProbs), ("seed", seed)], check)
+    ctx.check(ctx.lib.esacb200_assign_hypotheses_async(ctx.handle, B, E, M, gatingProbs.data_ptr(), int(maxExperts),
+                                                       int(bool(expertSelection)), seed.data_ptr(), outAssign.data_ptr(),
+                                                       outHist.data_ptr() if outHist is not None else None,
+                                                       outStatus.data_ptr()))
 
 
 def reproj_loss(prediction, gtPoses, focalLength, padX, padY, cutLoss, subSampling=8, ppointX=None, ppointY=None,

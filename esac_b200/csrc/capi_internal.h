@@ -6,6 +6,7 @@
 //   capi_esac.cu        esac.forward / esac.backward in every form
 //   capi_hypotheses.cu  the hypotheses node and the pose loss
 //   capi_losses.cu      the two expert losses
+//   capi_gate.cu        expert gates and the stream-ordered hypothesis assignment
 //   capi_testhooks.cu   include/esac_b200_testhooks.h
 #pragma once
 #include <cuda_runtime.h>

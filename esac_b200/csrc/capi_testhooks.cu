@@ -4,6 +4,8 @@
 #include "esac_p3p_fast.cuh"
 #include "esac_rng.cuh"
 
+#include <vector>
+
 using namespace esacb200;
 
 extern "C" {
@@ -118,6 +120,26 @@ void esacb200_host_draw_cells(uint64_t seed, uint32_t h, uint32_t t, int W, int 
     int cx[4], cy[4];
     draw_minimal_set(seed, h, t, W, H, cx, cy);
     for (int j = 0; j < 4; ++j) { cells8[2 * j] = cx[j]; cells8[2 * j + 1] = cy[j]; }
+}
+
+int esacb200_graph_node_types(void* graph, int* types, int cap) {
+    typedef int (*GetType)(cudaGraphNode_t, int*);
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPoint("cuGraphNodeGetType", &f, cudaEnableDefault, &q) != cudaSuccess || q != cudaDriverEntryPointSuccess) {
+        cudaGetLastError();
+        return -1;
+    }
+    size_t n = 0;
+    if (cudaGraphGetNodes((cudaGraph_t)graph, nullptr, &n) != cudaSuccess) { cudaGetLastError(); return -1; }
+    std::vector<cudaGraphNode_t> nodes(n);
+    if (n && cudaGraphGetNodes((cudaGraph_t)graph, nodes.data(), &n) != cudaSuccess) { cudaGetLastError(); return -1; }
+    for (size_t i = 0; i < n && (int)i < cap; ++i) {
+        int t = -1;
+        if (((GetType)f)(nodes[i], &t) != 0) return -1;
+        types[i] = t;
+    }
+    return (int)n;
 }
 
 }  // extern "C"

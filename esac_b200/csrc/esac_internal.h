@@ -350,6 +350,37 @@ void launch_select_gathered(const double* gathered, int world, int M_pad, Forwar
 int assign_max_experts();
 void launch_assign(const float* weights, int B, int E, int M, int keep_top, int single, uint64_t seed, int64_t* out_assign,
                    float* out_hist, int* flags, cudaStream_t stream);
+// The stream-ordered assignment: the seed read from d_seed on the device, image b's status (0 / 1 / 2) written to out_status[b].
+void launch_assign_async(const float* weights, int B, int E, int M, int keep_top, int single, const long long* d_seed,
+                         int64_t* out_assign, float* out_hist, int* out_status, cudaStream_t stream);
+
+// --- gate.cu ------------------------------------------------------------------------------
+// An expert gate's device side: the arm kernel sets the gate's conditional handles from a histogram on the device, and the
+// marker kernel, which does nothing, delimits one region in a captured graph.  The host finds both in the graph by their
+// function pointers (gate_arm_fn / gate_mark_fn) and reads their single parameter.
+constexpr int kGateMax = 1024;
+// What finalize leaves for the arm kernel: until `ready`, nothing; then `count` (index, handle) pairs, one per region.
+struct GateTable {
+    unsigned long long ready;
+    unsigned long long count;
+    const unsigned long long* pairs;  // [count][2]: the region's index into counts, its conditional handle
+};
+struct GateArm {
+    unsigned gate;  // the gate's id
+    int n;
+    const float* counts;       // [n]: the regions of index i run where counts[i] > 0
+    const GateTable* table;
+};
+struct GateTag {
+    unsigned gate;  // the gate's id
+    int serial;     // the region's serial number on its gate (a begin and its end share it; -1: an end without a begin)
+    int index;      // the gate's handle the region runs on
+    int begin;      // 1: begin marker, 0: end marker
+};
+const void* gate_arm_fn();
+const void* gate_mark_fn();
+void launch_gate_arm(const GateArm& a, cudaStream_t stream);
+void launch_gate_mark(const GateTag& t, cudaStream_t stream);
 
 // --- reproj.cu ----------------------------------------------------------------------------
 // Blocks of one image in the loss kernels of reproj.cu and coord_loss.cu: a pure function of its cell count N, so an image

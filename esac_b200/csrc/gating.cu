@@ -23,9 +23,15 @@ constexpr int kMaxExperts = 1024;
 // keep_top < 0: no clamping; else all but the keep_top largest weights are zeroed first (ties: the later index wins a place,
 // as a stable ascending sort would leave it nearer the top).  single != 0: one draw per image, repeated M times
 // (the "expertselection" mode, train_esac.py:133-135).
+// DEV = false: the eager call -- the seed is a parameter and `flags` one int the images OR their error bits into.
+// DEV = true: the stream-ordered call -- the seed is read from d_seed when the kernel runs (a graph replays with what the
+// tensor holds then) and `flags` is [B]: image b's status (0, 1 or 2) is written, not OR-ed, so no memset precedes it.
+template <bool DEV>
 __global__ void __launch_bounds__(256) assign_kernel(const float* __restrict__ weights, int E, int M, int keep_top, int single,
-                                                     uint64_t seed, int64_t* __restrict__ out_assign,
-                                                     float* __restrict__ out_hist, int* __restrict__ flags) {
+                                                     uint64_t seed, const long long* __restrict__ d_seed,
+                                                     int64_t* __restrict__ out_assign, float* __restrict__ out_hist,
+                                                     int* __restrict__ flags) {
+    if constexpr (DEV) seed = (uint64_t)*d_seed;
     __shared__ float w[kMaxExperts];
     __shared__ double cdf[kMaxExperts];
     __shared__ int hist[kMaxExperts];
@@ -60,7 +66,8 @@ __global__ void __launch_bounds__(256) assign_kernel(const float* __restrict__ w
             if (v > 0.f) { acc += (double)v; lp = e; }
             cdf[e] = acc;
         }
-        if (bad || lp < 0) atomicOr(flags, bad ? 1 : 2);  // 2: "invalid multinomial distribution (sum of probabilities <= 0)"
+        if constexpr (DEV) flags[b] = bad ? 1 : (lp < 0 ? 2 : 0);
+        else if (bad || lp < 0) atomicOr(flags, bad ? 1 : 2);  // 2: "invalid multinomial distribution (sum of probabilities <= 0)"
         last_pos = lp;
     }
     __syncthreads();
@@ -94,7 +101,12 @@ int assign_max_experts() { return kMaxExperts; }
 
 void launch_assign(const float* weights, int B, int E, int M, int keep_top, int single, uint64_t seed, int64_t* out_assign,
                    float* out_hist, int* flags, cudaStream_t stream) {
-    assign_kernel<<<B, 256, 0, stream>>>(weights, E, M, keep_top, single, seed, out_assign, out_hist, flags);
+    assign_kernel<false><<<B, 256, 0, stream>>>(weights, E, M, keep_top, single, seed, nullptr, out_assign, out_hist, flags);
+}
+
+void launch_assign_async(const float* weights, int B, int E, int M, int keep_top, int single, const long long* d_seed,
+                         int64_t* out_assign, float* out_hist, int* out_status, cudaStream_t stream) {
+    assign_kernel<true><<<B, 256, 0, stream>>>(weights, E, M, keep_top, single, 0, d_seed, out_assign, out_hist, out_status);
 }
 
 }  // namespace esacb200

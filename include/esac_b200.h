@@ -360,6 +360,40 @@ int esacb200_backward_batch_cameras(esacb200_ctx* ctx, int B, const float* coord
 int esacb200_assign_hypotheses(esacb200_ctx* ctx, int B, int E, int M, const float* weights, int keep_top,
                                int single_expert, uint64_t seed, int64_t* out_assign, float* out_hist);
 
+/* esacb200_assign_hypotheses enqueued on the context's stream with no host synchronisation, so a CUDA graph can capture it.
+ * Every pointer is a device pointer: weights float32 [B,E], seed int64 [1] (read when the kernel runs, so a graph can
+ * advance it or the caller can rewrite it between replays), out_assign int64 [B,M], out_hist float32 [B,E] or NULL, and
+ * out_status int32 [B]: 0, or 1 for a row with a negative / non-finite weight, 2 for a row that sums to 0 (the errors of
+ * the eager call; the row's draws are then meaningless).  Given the same seed value it draws exactly what
+ * esacb200_assign_hypotheses draws. */
+int esacb200_assign_hypotheses_async(esacb200_ctx* ctx, int B, int E, int M, const float* weights, int keep_top,
+                                     int single_expert, const int64_t* seed, int64_t* out_assign, float* out_hist,
+                                     int* out_status);
+
+/* ---- expert gates: run a region of a captured CUDA graph only where a count on the device is positive ---------------
+ * A gate has n <= ESACB200_GATE_MAX switches and serves one graph.  While a stream is being captured:
+ *   esacb200_gate_arm   enqueues a kernel that, at every replay of the finalized graph, sets switch i to (counts[i] > 0);
+ *                       counts: device float32 [n], typically a hypothesis histogram.  Once per gate.
+ *   esacb200_gate_mark  enqueues an empty marker kernel that opens (begin != 0) or closes region `index` of the gate.
+ * After the capture ends and before the graph is instantiated, esacb200_gate_finalize rewrites the graph: every region
+ * (begin marker, end marker and the nodes downstream of the begin and upstream of the end) moves into the body of an IF
+ * conditional node on the gate's conditional handle `index`, which takes its place.  The handles are created on the graph
+ * there, with the default value 0 applied at every launch.  Several regions may share an index.  A region must be closed:
+ * work forked from it must join before its end, work it waits on must precede its begin, regions may not nest or overlap,
+ * the gate must be armed upstream of every region, and a region may hold only kernel, memset, device memcpy, empty,
+ * child graph and conditional nodes.  On a violation finalize returns ESACB200_ERR_ARG, names the region and the reason in
+ * esacb200_last_error, and leaves the graph untouched: it then runs every region, and its arm kernel does nothing.
+ * Conditional nodes need a CUDA 12.3 driver: gate_create fails with ESACB200_ERR_CUDA on an older one.  The gate must
+ * outlive the graph's replays (the arm kernel reads the handles from the gate's memory).  A gate's errors are reported on
+ * its context. */
+#define ESACB200_GATE_MAX 1024
+typedef struct esacb200_gate esacb200_gate;
+int esacb200_gate_create(esacb200_ctx* ctx, int n, esacb200_gate** out);
+void esacb200_gate_destroy(esacb200_gate* gate);
+int esacb200_gate_arm(esacb200_gate* gate, const float* counts, void* stream);
+int esacb200_gate_mark(esacb200_gate* gate, int index, int begin, void* stream);
+int esacb200_gate_finalize(esacb200_gate* gate, void* graph);
+
 /* Robust reprojection loss of the expert refinement stage and its gradient, one fused pass (ref_expert.py:103-146, where
  * it is six elementwise torch ops + autograd): coords float32 [B,3,H,W] (one expert's prediction per image; the reference
  * has B = 1), grads float32 [B,3,H,W] or NULL = d loss_b / d coords (overwritten, not accumulated), gt_poses float32

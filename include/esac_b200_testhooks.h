@@ -51,6 +51,9 @@ void esacb200_host_pinv6(const double A[36], double out[36]);
 int esacb200_host_pick_group(int N, int coresident, int group_opt, int jobs_per_group, int jobs);
 /* Minimal set of try (seed, h, t): cells int[4][2] (x, y). */
 void esacb200_host_draw_cells(uint64_t seed, uint32_t h, uint32_t t, int W, int H, int32_t* cells8);
+/* The node types (cudaGraphNodeType values) of a CUDA graph's top level, through the runtime the library uses: writes up
+ * to `cap` of them to `types` and returns the node count, or -1 if the runtime refuses the graph. */
+int esacb200_graph_node_types(void* graph, int* types, int cap);
 
 #ifdef __cplusplus
 }

@@ -19,9 +19,19 @@ namespace {
 
 constexpr int kMaxExperts = 1024;
 
+// Whether weight a at index ia comes before weight b at index ib in the stable ascending order of torch.sort and
+// np.argsort(kind="stable"): NaN above every number (+inf included), equal values and NaNs among themselves by index.
+// A plain a < b would give a NaN rank 0, so keep_top would zero it and draw from the rest where torch keeps it and raises.
+__device__ __forceinline__ bool sorts_before(float a, int ia, float b, int ib) {
+    const bool na = a != a, nb = b != b;
+    if (na || nb) return !na || (nb && ia < ib);
+    return a < b || (a == b && ia < ib);
+}
+
 // weights [B, E] (>= 0, need not sum to 1: multinomial normalises), out_assign [B, M] int64, out_hist [B, E] float.
-// keep_top < 0: no clamping; else all but the keep_top largest weights are zeroed first (ties: the later index wins a place,
-// as a stable ascending sort would leave it nearer the top).  single != 0: one draw per image, repeated M times
+// keep_top < 0: no clamping; else all but the keep_top largest weights are zeroed first, largest in the stable ascending
+// order of sorts_before (ties: the later index wins a place; a NaN is kept before any number, and then flagged below).
+// single != 0: one draw per image, repeated M times
 // (the "expertselection" mode, train_esac.py:133-135).
 // DEV = false: the eager call -- the seed is a parameter and `flags` one int the images OR their error bits into.
 // DEV = true: the stream-ordered call -- the seed is read from d_seed when the kernel runs (a graph replays with what the
@@ -43,11 +53,11 @@ __global__ void __launch_bounds__(256) assign_kernel(const float* __restrict__ w
     }
     __syncthreads();
     if (keep_top >= 0 && keep_top < E) {
-        // rank of entry e in the stable ascending order = #{j: w[j] < w[e]} + #{j < e: w[j] == w[e]}
+        // rank of entry e in the stable ascending order = #{j: (w[j], j) sorts before (w[e], e)}
         for (int e = threadIdx.x; e < E; e += blockDim.x) {
             const float we = w[e];
             int rank = 0;
-            for (int j = 0; j < E; ++j) rank += (w[j] < we) || (w[j] == we && j < e);
+            for (int j = 0; j < E; ++j) rank += sorts_before(w[j], j, we, e);
             if (rank < E - keep_top) cdf[e] = 0.;  // remember the verdict; w is still being read by other threads
             else cdf[e] = 1.;
         }

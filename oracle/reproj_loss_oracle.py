@@ -1,7 +1,7 @@
 """Oracle for the expert-refinement reprojection loss (SURVEY 8f rank 4).  TEST INFRASTRUCTURE ONLY.
 
 A restatement of ref_expert.py:84-89 (target grid) and :103-148 (projection, clamps, robust loss) as one function of
-(prediction, gt_pose, focal length, pad, cut) built from the same torch ops in the same order, so that torch's own
+(prediction, gt_pose, focal length, pad, cut, clamps) built from the same torch ops in the same order, so that torch's own
 autograd provides the reference gradient.  It runs on the CPU in float32 (what the original computes in, on its GPU) or,
 with dtype=torch.float64, as the higher-precision yardstick that the tolerance of the fp32 comparison is judged by.
 
@@ -18,8 +18,9 @@ import torch
 
 def reproj_errors(prediction: torch.Tensor, gt_pose: torch.Tensor, focallength: float, pad_x: float, pad_y: float,
                   subsample: int = 8, image_w: float | None = None, image_h: float | None = None,
-                  dtype=torch.float32) -> torch.Tensor:
-    """Per-cell reprojection error clamped to [0, 100] px, flat [h*w] (ref_expert.py:103-142).
+                  dtype=torch.float32, max_reproj: float = 100.0, min_depth: float = 0.1) -> torch.Tensor:
+    """Per-cell reprojection error clamped to [0, max_reproj] px, flat [h*w] (ref_expert.py:103-142, where
+    max_reproj = 100 and the depth clamp min_depth = 0.1).
     prediction [1 or none,3,h,w] scene coordinates (requires_grad allowed), gt_pose [4,4] camera->world.
     image_w/h: size of the (padded) input image; default sub*w, sub*h -> principal point at the map centre
     (ref_expert.py:118-119)."""
@@ -45,18 +46,19 @@ def reproj_errors(prediction: torch.Tensor, gt_pose: torch.Tensor, focallength: 
     pred = pred[0].view(4, -1)                           # :131
     eye = torch.mm(pose, pred)                           # :132
     px = torch.mm(cam_mat, eye)                          # :135
-    px[2].clamp_(min=0.1)                                # :136
+    px[2].clamp_(min=min_depth)                          # :136
     px = px[0:2] / px[2]                                 # :137
     px = px - grid                                       # :140
     px = px.norm(2, 0)                                   # :141
-    return px.clamp(0, 100)                              # :142
+    return px.clamp(0, max_reproj)                       # :142
 
 
 def reproj_loss(prediction: torch.Tensor, gt_pose: torch.Tensor, focallength: float, pad_x: float, pad_y: float,
                 cutloss: float, subsample: int = 8, image_w: float | None = None, image_h: float | None = None,
-                dtype=torch.float32) -> torch.Tensor:
+                dtype=torch.float32, max_reproj: float = 100.0, min_depth: float = 0.1) -> torch.Tensor:
     """The robust loss of ref_expert.py:144-148 over reproj_errors()."""
-    px = reproj_errors(prediction, gt_pose, focallength, pad_x, pad_y, subsample, image_w, image_h, dtype)
+    px = reproj_errors(prediction, gt_pose, focallength, pad_x, pad_y, subsample, image_w, image_h, dtype, max_reproj,
+                       min_depth)
     loss_l1 = px[px <= cutloss]                          # :144
     loss_sqrt = px[px > cutloss]                         # :145
     loss_sqrt = torch.sqrt(cutloss * loss_sqrt)          # :146
@@ -64,10 +66,11 @@ def reproj_loss(prediction: torch.Tensor, gt_pose: torch.Tensor, focallength: fl
 
 
 def reproj_loss_and_grad(prediction, gt_pose, focallength, pad_x, pad_y, cutloss, subsample=8, image_w=None, image_h=None,
-                         dtype=torch.float32):
+                         dtype=torch.float32, max_reproj=100.0, min_depth=0.1):
     """(loss, d loss / d prediction [3,h,w]) through torch autograd, as `robust_loss.backward()` (ref_expert.py:150)."""
     p = torch.as_tensor(prediction).detach().clone().to(dtype).requires_grad_(True)
-    loss = reproj_loss(p, torch.as_tensor(gt_pose), focallength, pad_x, pad_y, cutloss, subsample, image_w, image_h, dtype)
+    loss = reproj_loss(p, torch.as_tensor(gt_pose), focallength, pad_x, pad_y, cutloss, subsample, image_w, image_h, dtype,
+                       max_reproj, min_depth)
     loss.backward()
     g = p.grad
     return float(loss.detach()), (g[0] if g.dim() == 4 else g)

@@ -204,14 +204,53 @@ class ReprojLoss(_BatchMeanLoss):
         return prediction[0].new_tensor(sum(losses) / len(losses))
 
 
+class _AmpBatchMeanLoss(torch.autograd.Function):
+    """The 16-bit counterparts of the loss nodes above, for predictions of an expert run under torch.autocast (float16 or
+    bfloat16).  Their forward is a loss-only launch that saves the predictions; their backward launches again, with the
+    gradient scale s = grad_out / batch taken on the device as _BatchMeanLoss.backward takes it, so that each gradient is
+    rounded to 16 bits once, after the scale: bitwise the gradient that the float32 node gives p through p.float().  The
+    loss is float32, bitwise the float32 node's on p.float().  Subclasses define `_grads(ctx, prediction, grads, scale)`."""
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        prediction = ctx.saved_tensors
+        grads = [torch.empty_like(p) for p in prediction]
+        ctx._forward_cls._grads(ctx, prediction, grads, grad_out / ctx.batch)
+        return (None,) + tuple(grads)
+
+
+def _amp(prediction) -> bool:
+    """The prediction (a tensor, or the first of a list) is float16 or bfloat16: the loss takes a 16-bit node."""
+    p = prediction[0] if api._is_list(prediction) else prediction
+    return api._is_torch(p) and p.dtype in (torch.float16, torch.bfloat16)
+
+
+class ReprojLossAmp(_AmpBatchMeanLoss):
+    """ReprojLoss on 16-bit predictions (api.reproj_loss_amp)."""
+
+    @staticmethod
+    def forward(ctx, meta, *prediction):
+        form, args = meta
+        losses = api.reproj_loss_amp(form([p.detach() for p in prediction]), *args)
+        ctx.save_for_backward(*prediction)
+        ctx.meta, ctx.batch = meta, len(losses)
+        return torch.tensor(sum(losses) / len(losses), dtype=torch.float32, device=prediction[0].device)
+
+    @staticmethod
+    def _grads(ctx, prediction, grads, scale):
+        form, args = ctx.meta
+        api.reproj_loss_amp(form([p.detach() for p in prediction]), *args, outGradients=form(grads), gradScale=scale)
+
+
 def reproj_loss(prediction, gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling=8, ppoint_x=None, ppoint_y=None):
     """Drop-in for the loss block of ref_expert.py: `robust_loss = reproj_loss(prediction, gt_pose, f, padX, padY,
     opt.cutloss)` followed by `robust_loss.backward()`.  prediction [B,3,H,W] (CUDA), gt_poses [B,4,4] camera->world.
     focal_length, pad_x / pad_y and the principal point are a number or B values, so a batch may mix cameras.
-    prediction may also be a list or tuple of B [3,H_b,W_b] tensors of different sizes."""
+    prediction may also be a list or tuple of B [3,H_b,W_b] tensors of different sizes.  A float16 or bfloat16 prediction
+    (an expert under torch.autocast) takes the 16-bit node: a float32 loss and the 16-bit gradient of p.float()'s route."""
     inputs, form = _as_inputs(prediction)
     args = (gt_poses, focal_length, pad_x, pad_y, cut_loss, sub_sampling, ppoint_x, ppoint_y)
-    return ReprojLoss.apply((form, args), *inputs)
+    return (ReprojLossAmp if _amp(prediction) else ReprojLoss).apply((form, args), *inputs)
 
 
 class CoordLoss(_BatchMeanLoss):
@@ -229,13 +268,32 @@ class CoordLoss(_BatchMeanLoss):
         return prediction[0].new_tensor(sum(losses) / len(losses))
 
 
+class CoordLossAmp(_AmpBatchMeanLoss):
+    """CoordLoss on 16-bit predictions (api.coord_loss_amp)."""
+
+    @staticmethod
+    def forward(ctx, meta, *prediction):
+        form, gt_coords, cut_loss = meta
+        losses = api.coord_loss_amp(form([p.detach() for p in prediction]), gt_coords, cut_loss)
+        ctx.save_for_backward(*prediction)
+        ctx.meta, ctx.batch = meta, len(losses)
+        return torch.tensor(sum(losses) / len(losses), dtype=torch.float32, device=prediction[0].device)
+
+    @staticmethod
+    def _grads(ctx, prediction, grads, scale):
+        form, gt_coords, cut_loss = ctx.meta
+        api.coord_loss_amp(form([p.detach() for p in prediction]), gt_coords, cut_loss, outGradients=form(grads),
+                           gradScale=scale)
+
+
 def coord_loss(prediction, gt_coords, cut_loss=100.0):
     """Drop-in for the loss block of init_expert.py: `prediction, gt_coords = util.assert_size(...)` through the robust loss
     (:114-130) become `robust_loss = coord_loss(prediction, gt_coords, opt.cutloss)`, followed by `robust_loss.backward()`.
     prediction [B,3,Hp,Wp] (CUDA), gt_coords [B,3,Hg,Wg], at most 1 apart in H and W; or both lists or tuples of B
-    [3,H_b,W_b] tensors of different sizes."""
+    [3,H_b,W_b] tensors of different sizes.  A float16 or bfloat16 prediction takes the 16-bit node (as reproj_loss);
+    gt_coords stays float32."""
     inputs, form = _as_inputs(prediction)
-    return CoordLoss.apply((form, gt_coords, cut_loss), *inputs)
+    return (CoordLossAmp if _amp(prediction) else CoordLoss).apply((form, gt_coords, cut_loss), *inputs)
 
 
 def _batch_mean(losses):
@@ -268,6 +326,35 @@ class ReprojLossAsync(_BatchMeanLoss):
         return _batch_mean(losses)
 
 
+class ReprojLossAmpAsync(_AmpBatchMeanLoss):
+    """ReprojLossAsync on 16-bit predictions (api.reproj_loss_amp_async): capturable, as ReprojLossAsync; the backward's
+    scale stays on the device."""
+
+    @staticmethod
+    def forward(ctx, meta, *prediction):
+        form, gt_poses, shifts, cameras, cut_loss, sub_sampling, max_reproj, min_depth, status = meta
+        B = len(prediction) if form is list else prediction[0].shape[0]
+        dev = prediction[0].device
+        losses = torch.empty(B, dtype=torch.float64, device=dev)
+        if status is None:
+            status = torch.empty(B, dtype=torch.int32, device=dev)
+        api.reproj_loss_amp_async(form([p.detach() for p in prediction]), gt_poses, shifts, cameras, cut_loss, sub_sampling,
+                                  losses, status, maxReproj=max_reproj, minDepth=min_depth)
+        ctx.save_for_backward(*prediction)
+        ctx.meta, ctx.batch = meta, B
+        return _batch_mean(losses)
+
+    @staticmethod
+    def _grads(ctx, prediction, grads, scale):
+        form, gt_poses, shifts, cameras, cut_loss, sub_sampling, max_reproj, min_depth, _ = ctx.meta
+        dev = prediction[0].device
+        losses = torch.empty(ctx.batch, dtype=torch.float64, device=dev)
+        status = torch.empty(ctx.batch, dtype=torch.int32, device=dev)
+        api.reproj_loss_amp_async(form([p.detach() for p in prediction]), gt_poses, shifts, cameras, cut_loss, sub_sampling,
+                                  losses, status, outGradients=form(grads), maxReproj=max_reproj, minDepth=min_depth,
+                                  gradScale=scale)
+
+
 def reproj_loss_async(prediction, gt_poses, shifts, cameras, cut_loss, sub_sampling=8, max_reproj=100.0, min_depth=0.1,
                       status=None):
     """reproj_loss for training steps captured in a CUDA graph (ref_expert.py as one graph): CUDA tensors only, prediction
@@ -275,10 +362,11 @@ def reproj_loss_async(prediction, gt_poses, shifts, cameras, cut_loss, sub_sampl
     padY), cameras float32 [B,3] (focal length, ppointX, ppointY), all read on the device at replay time.  The loss (the
     batch mean, float32) and the gradients are bitwise those of reproj_loss.  status: an int32 CUDA tensor [B] that receives
     the per-image status (1 = a singular ground truth: that loss is NaN, its gradient zero); None keeps it internal.  Call
-    api.reserve_loss_async with the largest batch and map before the first capture."""
+    api.reserve_loss_async with the largest batch and map before the first capture.  A float16 or bfloat16 prediction
+    takes the 16-bit node, as in reproj_loss."""
     inputs, form = _as_inputs(prediction)
     meta = (form, gt_poses, shifts, cameras, cut_loss, sub_sampling, max_reproj, min_depth, status)
-    return ReprojLossAsync.apply(meta, *inputs)
+    return (ReprojLossAmpAsync if _amp(prediction) else ReprojLossAsync).apply(meta, *inputs)
 
 
 class CoordLossAsync(_BatchMeanLoss):
@@ -298,14 +386,35 @@ class CoordLossAsync(_BatchMeanLoss):
         return _batch_mean(losses)
 
 
+class CoordLossAmpAsync(_AmpBatchMeanLoss):
+    """CoordLossAsync on 16-bit predictions (api.coord_loss_amp_async): capturable, as CoordLossAsync."""
+
+    @staticmethod
+    def forward(ctx, meta, *prediction):
+        form, gt_coords, cut_loss, counts = meta
+        B = len(prediction) if form is list else prediction[0].shape[0]
+        losses = torch.empty(B, dtype=torch.float64, device=prediction[0].device)
+        api.coord_loss_amp_async(form([p.detach() for p in prediction]), gt_coords, cut_loss, losses, outCounts=counts)
+        ctx.save_for_backward(*prediction)
+        ctx.meta, ctx.batch = meta, B
+        return _batch_mean(losses)
+
+    @staticmethod
+    def _grads(ctx, prediction, grads, scale):
+        form, gt_coords, cut_loss, _ = ctx.meta
+        losses = torch.empty(ctx.batch, dtype=torch.float64, device=prediction[0].device)
+        api.coord_loss_amp_async(form([p.detach() for p in prediction]), gt_coords, cut_loss, losses, outGradients=form(grads),
+                                 gradScale=scale)
+
+
 def coord_loss_async(prediction, gt_coords, cut_loss=100.0, counts=None):
     """coord_loss for training steps captured in a CUDA graph (init_expert.py as one graph): CUDA tensors only, prediction
     [B,3,Hp,Wp] and gt_coords [B,3,Hg,Wg], or both lists / tuples of B [3,H_b,W_b] tensors, read on the device at replay
     time.  The loss (the batch mean, float32) and the gradients are bitwise those of coord_loss.  counts: an int64 CUDA
     tensor [B] that receives the valid cells per image, or None.  Call api.reserve_loss_async with the largest batch and
-    map before the first capture."""
+    map before the first capture.  A float16 or bfloat16 prediction takes the 16-bit node, as in coord_loss."""
     inputs, form = _as_inputs(prediction)
-    return CoordLossAsync.apply((form, gt_coords, cut_loss, counts), *inputs)
+    return (CoordLossAmpAsync if _amp(prediction) else CoordLossAsync).apply((form, gt_coords, cut_loss, counts), *inputs)
 
 
 # ------------------------------------------------------------------------------------------------

@@ -123,8 +123,9 @@ static int reproj_sizes(esacb200_ctx* ctx, const char* what, int B, const int* H
 }
 
 // The records of a reprojection-loss call on the B images at the device addresses coords[b] and grads[b] (grads, or an
-// entry of it, null: no gradient), and per image whether it takes the 128-bit load path.  Returns the blocks' partials.
-static long long reproj_records(int B, const float* const* coords, float* const* grads, const int* H, const int* W,
+// entry of it, null: no gradient) of elements of `esize` bytes, and per image whether it takes the vector load path.
+// Returns the blocks' partials.
+static long long reproj_records(int B, const void* const* coords, void* const* grads, const int* H, const int* W, int esize,
                                 std::vector<ReprojImage>& recs, std::vector<char>& vec) {
     recs.resize((size_t)B);
     vec.resize((size_t)B);
@@ -139,22 +140,23 @@ static long long reproj_records(int B, const float* const* coords, float* const*
         r.blocks = reproj_blocks_per_image(r.N);
         r.part0 = parts;
         parts += r.blocks;
-        vec[b] = reproj_vec_ok(r.coords, r.grads, r.N, r.W);
+        vec[b] = reproj_vec_ok(r.coords, r.grads, r.N, r.W, esize);
     }
     return parts;
 }
 
 // The reprojection loss's launches, one per load path, on the workspace at `base` laid out as L, whose records are in
-// order_by_path's order (n_vec on the 128-bit path first).  They run on run's stream and count in its kernel_launches.
+// order_by_path's order (n_vec on the vector path first), for maps of `dtype` with gradients scaled by grad_scale (or not).
+// They run on run's stream and count in its kernel_launches.
 static void reproj_launches(esacb200_ctx* run, char* base, const LossLayout& L, int B, int n_vec, int max_vec, int max_sc,
-                            int sub, float cut, float maxReproj, float minDepth) {
+                            int sub, float cut, float maxReproj, float minDepth, int dtype, const float* grad_scale) {
     const ReprojImage* rec = (const ReprojImage*)(base + L.rec);
     for (int path = 0; path < 2; ++path) {
         const int n = path == 0 ? n_vec : B - n_vec;
         if (n == 0) continue;
-        launch_reproj(path == 0, rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, (const float*)(base + L.img),
-                      (float)sub, cut, maxReproj, minDepth, (double*)(base + L.part), (unsigned*)base, (double*)(base + L.loss),
-                      run->stream);
+        launch_reproj(path == 0, dtype, rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc,
+                      (const float*)(base + L.img), (float)sub, cut, maxReproj, minDepth, grad_scale, (double*)(base + L.part),
+                      (unsigned*)base, (double*)(base + L.loss), run->stream);
         run->st.kernel_launches += 1;
     }
 }
@@ -178,9 +180,11 @@ static int coord_sizes(esacb200_ctx* ctx, const char* what, int B, const int* Hp
 }
 
 // The records of a coordinate-loss call on the B images at the device addresses pred[b], gt[b] and grads[b] (grads, or an
-// entry of it, null: no gradient), and per image whether it takes the 128-bit load path.  Returns the blocks' partials.
-static long long coord_records(int B, const float* const* pred, const float* const* gt, float* const* grads, const int* Hp,
-                               const int* Wp, const int* Hg, const int* Wg, std::vector<CoordImage>& recs, std::vector<char>& vec) {
+// entry of it, null: no gradient; pred and grads of elements of `esize` bytes), and per image whether it takes the vector
+// load path.  Returns the blocks' partials.
+static long long coord_records(int B, const void* const* pred, const float* const* gt, void* const* grads, const int* Hp,
+                               const int* Wp, const int* Hg, const int* Wg, int esize, std::vector<CoordImage>& recs,
+                               std::vector<char>& vec) {
     recs.resize((size_t)B);
     vec.resize((size_t)B);
     long long parts = 0;
@@ -189,7 +193,7 @@ static long long coord_records(int B, const float* const* pred, const float* con
         r.pred = pred[b];
         r.gt = gt[b];
         r.grads = grads ? grads[b] : nullptr;
-        vec[b] = coord_image(r, Hp[b], Wp[b], Hg[b], Wg[b]);
+        vec[b] = coord_image(r, Hp[b], Wp[b], Hg[b], Wg[b], esize);
         r.b = b;
         r.part0 = parts;
         parts += r.blocks;
@@ -198,30 +202,51 @@ static long long coord_records(int B, const float* const* pred, const float* con
 }
 
 // The coordinate loss's launches, per load path the count pass (with gradients) and the loss pass, on the workspace at
-// `base` laid out as L, whose records are in order_by_path's order.  They run on run's stream and count in its
-// kernel_launches.
+// `base` laid out as L, whose records are in order_by_path's order; dtype and grad_scale as for reproj_launches.  They run
+// on run's stream and count in its kernel_launches.
 static void coord_launches(esacb200_ctx* run, char* base, const LossLayout& L, int B, bool grads, int n_vec, int max_vec,
-                           int max_sc, float cut) {
+                           int max_sc, float cut, int dtype, const float* grad_scale) {
     const CoordImage* rec = (const CoordImage*)(base + L.rec);
     for (int path = 0; path < 2; ++path) {
         const int n = path == 0 ? n_vec : B - n_vec;
         if (n == 0) continue;
         for (int pass = grads ? 1 : 2; pass <= 2; ++pass) {
-            launch_coord_loss(path == 0, pass, grads, rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, cut,
-                              (unsigned*)base + B, (double*)(base + L.part), (unsigned*)base, (double*)(base + L.loss),
-                              (long long*)(base + L.flags), run->stream);
+            launch_coord_loss(path == 0, pass, grads, dtype, rec + (path == 0 ? 0 : n_vec), n, path == 0 ? max_vec : max_sc, cut,
+                              grad_scale, (unsigned*)base + B, (double*)(base + L.part), (unsigned*)base,
+                              (double*)(base + L.loss), (long long*)(base + L.flags), run->stream);
             run->st.kernel_launches += 1;
         }
     }
 }
 
+// The element type of a typed loss call: a known dtype code; grad_scale only with a 16-bit code, and then device memory;
+// 16-bit images (device: whether every image argument is device memory) only in device memory.  esize receives the
+// element's bytes.  `what`: the entry point named in front of each message, or null.
+static int loss_dtype(esacb200_ctx* ctx, const char* what, int dtype, const float* grad_scale, bool device, int& esize) {
+    const char* sep = what ? ": " : "";
+    if (!what) what = "";
+    if (dtype != ESACB200_FLOAT32 && dtype != ESACB200_FLOAT16 && dtype != ESACB200_BFLOAT16)
+        return fail(ctx, ESACB200_ERR_ARG, "%s%sunknown dtype code %d", what, sep, dtype);
+    esize = loss_elem_bytes(dtype);
+    if (dtype == ESACB200_FLOAT32) {
+        if (grad_scale) return fail(ctx, ESACB200_ERR_ARG, "%s%sgrad_scale is for float16 / bfloat16 maps only", what, sep);
+        return 0;
+    }
+    if (!device) return fail(ctx, ESACB200_ERR_ARG, "%s%sfloat16 / bfloat16 maps must be device memory", what, sep);
+    if (grad_scale && !is_device_ptr(grad_scale))
+        return fail(ctx, ESACB200_ERR_ARG, "%s%sgrad_scale must be device memory", what, sep);
+    return 0;
+}
+static_assert(ESACB200_FLOAT32 == kLossF32 && ESACB200_FLOAT16 == kLossF16 && ESACB200_BFLOAT16 == kLossBF16,
+              "the C ABI's dtype codes are the kernels' LossDtype");
+
 // -------------------------------------------------------------------------------------------------
 // The reprojection loss over B images, each with its own size: one launch per load path (128-bit / scalar, chosen per
 // image as a single-image call would choose it), each image cut into the blocks a single-image call uses.
-int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H,
-                                const int* W, const float* gt_poses, const int* shiftX, const int* shiftY, const float* f,
-                                const float* ppx, const float* ppy, int sub, float cut, float maxReproj, float minDepth,
-                                double* out_losses) try {
+int esacb200_reproj_loss_ragged_typed(esacb200_ctx* ctx, int B, int dtype, const void* const* coords, void* const* grads,
+                                      const int* H, const int* W, const float* gt_poses, const int* shiftX, const int* shiftY,
+                                      const float* f, const float* ppx, const float* ppy, int sub, float cut, float maxReproj,
+                                      float minDepth, const float* grad_scale, double* out_losses) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     if (!coords || !H || !W || !gt_poses || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
@@ -232,11 +257,13 @@ int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* co
     bool c_dev = false, g_dev = false;
     if ((rc = pointer_kind(ctx, (const void* const*)coords, B, "coords", c_dev))) return rc;
     if (grads && (rc = pointer_kind(ctx, (const void* const*)grads, B, "grads", g_dev))) return rc;
+    int esize = 0;
+    if ((rc = loss_dtype(ctx, nullptr, dtype, grad_scale, c_dev && (!grads || g_dev), esize))) return rc;
     begin_call(ctx);
     std::vector<size_t> bytes((size_t)B), c_off, g_off;
-    for (int b = 0; b < B; ++b) bytes[b] = (size_t)3 * H[b] * W[b] * sizeof(float);
-    std::vector<const float*> d_coords;
-    std::vector<float*> d_grads((size_t)B, nullptr);
+    for (int b = 0; b < B; ++b) bytes[b] = (size_t)3 * H[b] * W[b] * esize;
+    std::vector<const void*> d_coords;
+    std::vector<void*> d_grads((size_t)B, nullptr);
     rc = stage_images(ctx, coords, bytes, c_dev, true, ctx->coords, d_coords, c_off);
     if (rc) return rc;
     if (grads && (rc = stage_images(ctx, grads, bytes, g_dev, false, ctx->grads, d_grads, g_off))) return rc;
@@ -255,7 +282,7 @@ int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* co
             return fail(ctx, ESACB200_ERR_ARG, "image %d: ground-truth pose is singular", b);
     std::vector<ReprojImage> recs, ordered;
     std::vector<char> vec;
-    const long long parts = reproj_records(B, d_coords.data(), d_grads.data(), H, W, recs, vec);
+    const long long parts = reproj_records(B, d_coords.data(), d_grads.data(), H, W, esize, recs, vec);
     int n_vec, max_vec, max_sc;
     const size_t rec_bytes = order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
     const LossLayout L = reproj_layout(B, parts);
@@ -268,7 +295,7 @@ int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* co
     CK(cudaMemcpyAsync(base + L.img, staging.data(), staging.size(), cudaMemcpyHostToDevice, ctx->stream));
     mark(ctx, EV_H2D);
     mark(ctx, EV_FOLD);  // ms_score = the kernels alone
-    reproj_launches(ctx, base, L, B, n_vec, max_vec, max_sc, sub, cut, maxReproj, minDepth);
+    reproj_launches(ctx, base, L, B, n_vec, max_vec, max_sc, sub, cut, maxReproj, minDepth, dtype, grad_scale);
     CK(cudaGetLastError());
     mark(ctx, EV_SCORE);
     if (grads && !g_dev) {
@@ -282,6 +309,15 @@ int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* co
     finish_stats(ctx);
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
+
+int esacb200_reproj_loss_ragged(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H,
+                                const int* W, const float* gt_poses, const int* shiftX, const int* shiftY, const float* f,
+                                const float* ppx, const float* ppy, int sub, float cut, float maxReproj, float minDepth,
+                                double* out_losses) {
+    return esacb200_reproj_loss_ragged_typed(ctx, B, ESACB200_FLOAT32, (const void* const*)coords, (void* const*)grads, H, W,
+                                             gt_poses, shiftX, shiftY, f, ppx, ppy, sub, cut, maxReproj, minDepth, nullptr,
+                                             out_losses);
+}
 
 // B images of one shape: the pointer and size arrays of a [B,3,H,W] tensor.
 int esacb200_reproj_loss_cameras(esacb200_ctx* ctx, int B, const float* coords, float* grads, int H, int W, const float* gt_poses,
@@ -313,9 +349,9 @@ int esacb200_reproj_loss(esacb200_ctx* ctx, int B, const float* coords, float* g
 // -------------------------------------------------------------------------------------------------
 // The coordinate loss over B images, each with its own prediction and ground-truth size: one launch per load path and
 // pass, each image cut into the blocks a single-image call uses.
-int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pred, const int* Hp, const int* Wp,
-                               const float* const* gt, const int* Hg, const int* Wg, float* const* grads, float cut,
-                               double* out_losses, int64_t* out_counts) try {
+int esacb200_coord_loss_ragged_typed(esacb200_ctx* ctx, int B, int dtype, const void* const* pred, const int* Hp, const int* Wp,
+                                     const float* const* gt, const int* Hg, const int* Wg, void* const* grads, float cut,
+                                     const float* grad_scale, double* out_losses, int64_t* out_counts) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     if (!pred || !gt || !Hp || !Wp || !Hg || !Wg || !out_losses) return fail(ctx, ESACB200_ERR_ARG, "null pointer argument");
@@ -326,20 +362,23 @@ int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pre
     if ((rc = pointer_kind(ctx, (const void* const*)pred, B, "pred", p_dev))) return rc;
     if ((rc = pointer_kind(ctx, (const void* const*)gt, B, "gt", q_dev))) return rc;
     if (grads && (rc = pointer_kind(ctx, (const void* const*)grads, B, "grads", g_dev))) return rc;
+    int esize = 0;
+    if ((rc = loss_dtype(ctx, nullptr, dtype, grad_scale, p_dev && (!grads || g_dev), esize))) return rc;
     begin_call(ctx);
     std::vector<size_t> pbytes((size_t)B), gbytes((size_t)B), p_off, q_off, g_off;
     for (int b = 0; b < B; ++b) {
-        pbytes[b] = (size_t)3 * Hp[b] * Wp[b] * sizeof(float);
+        pbytes[b] = (size_t)3 * Hp[b] * Wp[b] * esize;
         gbytes[b] = (size_t)3 * Hg[b] * Wg[b] * sizeof(float);
     }
-    std::vector<const float*> d_pred, d_gt;
-    std::vector<float*> d_grads((size_t)B, nullptr);
+    std::vector<const void*> d_pred;
+    std::vector<const float*> d_gt;
+    std::vector<void*> d_grads((size_t)B, nullptr);
     if ((rc = stage_images(ctx, pred, pbytes, p_dev, true, ctx->coords, d_pred, p_off))) return rc;
     if ((rc = stage_images(ctx, gt, gbytes, q_dev, true, ctx->coords_alt, d_gt, q_off))) return rc;
     if (grads && (rc = stage_images(ctx, grads, pbytes, g_dev, false, ctx->grads, d_grads, g_off))) return rc;
     std::vector<CoordImage> recs, ordered;
     std::vector<char> vec;
-    const long long parts = coord_records(B, d_pred.data(), d_gt.data(), d_grads.data(), Hp, Wp, Hg, Wg, recs, vec);
+    const long long parts = coord_records(B, d_pred.data(), d_gt.data(), d_grads.data(), Hp, Wp, Hg, Wg, esize, recs, vec);
     int n_vec, max_vec, max_sc;
     const size_t rec_bytes = order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
     const LossLayout L = coord_layout(B, parts);
@@ -349,7 +388,7 @@ int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pre
     CK(cudaMemcpyAsync(base + L.rec, ordered.data(), rec_bytes, cudaMemcpyHostToDevice, ctx->stream));
     mark(ctx, EV_H2D);
     mark(ctx, EV_FOLD);  // ms_score = the kernels alone
-    coord_launches(ctx, base, L, B, grads != nullptr, n_vec, max_vec, max_sc, cut);
+    coord_launches(ctx, base, L, B, grads != nullptr, n_vec, max_vec, max_sc, cut, dtype, grad_scale);
     CK(cudaGetLastError());
     mark(ctx, EV_SCORE);
     if (grads && !g_dev) {
@@ -364,6 +403,13 @@ int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pre
     finish_stats(ctx);
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
+
+int esacb200_coord_loss_ragged(esacb200_ctx* ctx, int B, const float* const* pred, const int* Hp, const int* Wp,
+                               const float* const* gt, const int* Hg, const int* Wg, float* const* grads, float cut,
+                               double* out_losses, int64_t* out_counts) {
+    return esacb200_coord_loss_ragged_typed(ctx, B, ESACB200_FLOAT32, (const void* const*)pred, Hp, Wp, gt, Hg, Wg,
+                                            (void* const*)grads, cut, nullptr, out_losses, out_counts);
+}
 
 // B images of one shape: the pointer and size arrays of [B,3,Hp,Wp] / [B,3,Hg,Wg] tensors.
 int esacb200_coord_loss(esacb200_ctx* ctx, int B, const float* pred, int Hp, int Wp, const float* gt, int Hg, int Wg,
@@ -431,9 +477,10 @@ int esacb200_reserve_loss_async(esacb200_ctx* ctx, int B, int H, int W) try {
     return loss_workspace(ctx, a, std::max(reproj_layout(B, parts).end, coord_layout(B, parts).end), false, "reserve_loss_async");
 } ESAC_ABI_CATCH(ctx)
 
-int esacb200_reproj_loss_async(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H,
-                               const int* W, const float* gt_poses, const int32_t* shifts, const float* cameras, int sub,
-                               float cut, float maxReproj, float minDepth, double* out_losses, int32_t* out_status) try {
+int esacb200_reproj_loss_async_typed(esacb200_ctx* ctx, int B, int dtype, const void* const* coords, void* const* grads,
+                                     const int* H, const int* W, const float* gt_poses, const int32_t* shifts,
+                                     const float* cameras, int sub, float cut, float maxReproj, float minDepth,
+                                     const float* grad_scale, double* out_losses, int32_t* out_status) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     const char* what = "reproj_loss_async";
@@ -445,13 +492,15 @@ int esacb200_reproj_loss_async(esacb200_ctx* ctx, int B, const float* const* coo
     if (!rc) rc = device_args(ctx, what, 5, ptrs, names);
     if (!rc) rc = device_images(ctx, what, "coords", (const void* const*)coords, B);
     if (!rc && grads) rc = device_images(ctx, what, "grads", (const void* const*)grads, B);
+    int esize = 0;
+    if (!rc) rc = loss_dtype(ctx, what, dtype, grad_scale, true, esize);
     if (rc) return rc;
     esacb200_ctx* a = nullptr;
     bool capturing = false;
     if ((rc = begin_loss_async(ctx, a, capturing))) return rc;
     std::vector<ReprojImage> recs, ordered;
     std::vector<char> vec;
-    const long long parts = reproj_records(B, coords, grads, H, W, recs, vec);
+    const long long parts = reproj_records(B, coords, grads, H, W, esize, recs, vec);
     int n_vec, max_vec, max_sc;
     order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
     const LossLayout L = reproj_layout(B, parts);
@@ -464,16 +513,24 @@ int esacb200_reproj_loss_async(esacb200_ctx* ctx, int B, const float* const* coo
     CK(cudaMemsetAsync(base, 0, L.img, a->stream));
     a->st.kernel_launches +=
         launch_reproj_prep(ordered.data(), B, d_rec, gt_poses, shifts, cameras, (float*)(base + L.img), bad, a->stream);
-    reproj_launches(a, base, L, B, n_vec, max_vec, max_sc, sub, cut, maxReproj, minDepth);
-    launch_reproj_finish(d_rec, B, grads != nullptr, losses, bad, out_losses, out_status, a->stream);
+    reproj_launches(a, base, L, B, n_vec, max_vec, max_sc, sub, cut, maxReproj, minDepth, dtype, grad_scale);
+    launch_reproj_finish(d_rec, B, grads != nullptr, dtype, grad_scale, losses, bad, out_losses, out_status, a->stream);
     a->st.kernel_launches += 1;
     CK(cudaGetLastError());
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 
-int esacb200_coord_loss_async(esacb200_ctx* ctx, int B, const float* const* pred, const int* Hp, const int* Wp,
-                              const float* const* gt, const int* Hg, const int* Wg, float* const* grads, float cut,
-                              double* out_losses, int64_t* out_counts) try {
+int esacb200_reproj_loss_async(esacb200_ctx* ctx, int B, const float* const* coords, float* const* grads, const int* H,
+                               const int* W, const float* gt_poses, const int32_t* shifts, const float* cameras, int sub,
+                               float cut, float maxReproj, float minDepth, double* out_losses, int32_t* out_status) {
+    return esacb200_reproj_loss_async_typed(ctx, B, ESACB200_FLOAT32, (const void* const*)coords, (void* const*)grads, H, W,
+                                            gt_poses, shifts, cameras, sub, cut, maxReproj, minDepth, nullptr, out_losses,
+                                            out_status);
+}
+
+int esacb200_coord_loss_async_typed(esacb200_ctx* ctx, int B, int dtype, const void* const* pred, const int* Hp, const int* Wp,
+                                    const float* const* gt, const int* Hg, const int* Wg, void* const* grads, float cut,
+                                    const float* grad_scale, double* out_losses, int64_t* out_counts) try {
     if (!ctx) return ESACB200_ERR_ARG;
     DeviceGuard device_guard(ctx->device);
     const char* what = "coord_loss_async";
@@ -486,13 +543,15 @@ int esacb200_coord_loss_async(esacb200_ctx* ctx, int B, const float* const* pred
     if (!rc) rc = device_images(ctx, what, "pred", (const void* const*)pred, B);
     if (!rc) rc = device_images(ctx, what, "gt", (const void* const*)gt, B);
     if (!rc && grads) rc = device_images(ctx, what, "grads", (const void* const*)grads, B);
+    int esize = 0;
+    if (!rc) rc = loss_dtype(ctx, what, dtype, grad_scale, true, esize);
     if (rc) return rc;
     esacb200_ctx* a = nullptr;
     bool capturing = false;
     if ((rc = begin_loss_async(ctx, a, capturing))) return rc;
     std::vector<CoordImage> recs, ordered;
     std::vector<char> vec;
-    const long long parts = coord_records(B, pred, gt, grads, Hp, Wp, Hg, Wg, recs, vec);
+    const long long parts = coord_records(B, pred, gt, grads, Hp, Wp, Hg, Wg, esize, recs, vec);
     int n_vec, max_vec, max_sc;
     order_by_path(recs, vec, ordered, n_vec, max_vec, max_sc);
     const LossLayout L = coord_layout(B, parts);
@@ -501,12 +560,19 @@ int esacb200_coord_loss_async(esacb200_ctx* ctx, int B, const float* const* pred
     char* base = (char*)a->loss_ws.p;
     CK(cudaMemsetAsync(base, 0, L.rec, a->stream));
     a->st.kernel_launches += launch_coord_prep(ordered.data(), B, (CoordImage*)(base + L.rec), a->stream);
-    coord_launches(a, base, L, B, grads != nullptr, n_vec, max_vec, max_sc, cut);
+    coord_launches(a, base, L, B, grads != nullptr, n_vec, max_vec, max_sc, cut, dtype, grad_scale);
     launch_coord_finish(B, (const double*)(base + L.loss), (const long long*)(base + L.flags), out_losses, (long long*)out_counts,
                         a->stream);
     a->st.kernel_launches += 1;
     CK(cudaGetLastError());
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
+
+int esacb200_coord_loss_async(esacb200_ctx* ctx, int B, const float* const* pred, const int* Hp, const int* Wp,
+                              const float* const* gt, const int* Hg, const int* Wg, float* const* grads, float cut,
+                              double* out_losses, int64_t* out_counts) {
+    return esacb200_coord_loss_async_typed(ctx, B, ESACB200_FLOAT32, (const void* const*)pred, Hp, Wp, gt, Hg, Wg,
+                                           (void* const*)grads, cut, nullptr, out_losses, out_counts);
+}
 
 }  // extern "C"

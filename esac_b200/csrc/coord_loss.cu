@@ -17,6 +17,8 @@
 // A NaN cell counts but falls in neither masked sum (loss 0, gradient NaN); an invalid cell has loss and gradient 0, as do
 // prediction cells outside the common window.  The per-image loss is summed in fp64 in a fixed order (block partials, the
 // image's last block adds them up), so the result does not depend on scheduling.
+#include <type_traits>
+
 #include "esac_internal.h"
 
 namespace esacb200 {
@@ -99,23 +101,26 @@ __global__ void __launch_bounds__(kThreads) coord_count_kernel(const CoordImage*
 
 // grid as for the count pass, over the prediction's cells.  GRAD: grads overwritten, counts[b] from the count pass.
 // losses[b] = loss of image b, out_counts[b] = its valid cells; partial: 2 doubles per block, tickets: zeroed counters
-// (left zeroed).
-template <bool VEC, bool GRAD>
+// (left zeroed).  T: the prediction's and gradient's element type, widened on load; SCALE: every gradient (zeros included)
+// times *grad_scale (loss_scale) after coord_cell's rounding to float, then rounded to T.
+template <class T, bool VEC, bool GRAD, bool SCALE>
 __global__ void __launch_bounds__(kThreads) coord_loss_kernel(const CoordImage* __restrict__ recs, float cut,
+                                                               const float* __restrict__ grad_scale,
                                                                const unsigned* __restrict__ counts, double* __restrict__ partial,
                                                                unsigned* __restrict__ tickets, double* __restrict__ losses,
                                                                long long* __restrict__ out_counts) {
     const CoordImage g = recs[blockIdx.y];
     if ((int)blockIdx.x >= g.blocks) return;
     const int b = g.b;
-    const float* px = g.pred;
-    const float* py = px + g.Np;
-    const float* pz = py + g.Np;
+    const T* px = static_cast<const T*>(g.pred);
+    const T* py = px + g.Np;
+    const T* pz = py + g.Np;
     const float* qx = g.gt;
     const float* qy = qx + g.Ng;
     const float* qz = qy + g.Ng;
-    float* gx = GRAD ? g.grads : nullptr;
+    T* gx = GRAD ? static_cast<T*>(g.grads) : nullptr;
     const double cnt = GRAD ? (double)counts[b] : 0.;
+    const float s = SCALE ? *grad_scale : 1.f;
     double acc = 0.;
     unsigned nvalid = 0;
     const int per_block = kThreads * kCellsPerThread;
@@ -125,9 +130,9 @@ __global__ void __launch_bounds__(kThreads) coord_loss_kernel(const CoordImage* 
         if (VEC) {
             float o[3][4] = {};
             if (p0 < g.N) {   // all four cells in the window (N % 4 == 0), else all four outside: zero gradient
-                const float4 a = __ldcs(reinterpret_cast<const float4*>(px + p0));
-                const float4 c = __ldcs(reinterpret_cast<const float4*>(py + p0));
-                const float4 d = __ldcs(reinterpret_cast<const float4*>(pz + p0));
+                const float4 a = loss_ld4(px + p0);
+                const float4 c = loss_ld4(py + p0);
+                const float4 d = loss_ld4(pz + p0);
                 const float4 e = __ldcs(reinterpret_cast<const float4*>(qx + p0));
                 const float4 f = __ldcs(reinterpret_cast<const float4*>(qy + p0));
                 const float4 h = __ldcs(reinterpret_cast<const float4*>(qz + p0));
@@ -143,9 +148,10 @@ __global__ void __launch_bounds__(kThreads) coord_loss_kernel(const CoordImage* 
                 }
             }
             if (GRAD) {
-                __stcs(reinterpret_cast<float4*>(gx + p0), make_float4(o[0][0], o[0][1], o[0][2], o[0][3]));
-                __stcs(reinterpret_cast<float4*>(gx + g.Np + p0), make_float4(o[1][0], o[1][1], o[1][2], o[1][3]));
-                __stcs(reinterpret_cast<float4*>(gx + 2 * (size_t)g.Np + p0), make_float4(o[2][0], o[2][1], o[2][2], o[2][3]));
+                auto sc = [s](float v) { return loss_scale<SCALE>(v, s); };
+                loss_st4(gx + p0, sc(o[0][0]), sc(o[0][1]), sc(o[0][2]), sc(o[0][3]));
+                loss_st4(gx + g.Np + p0, sc(o[1][0]), sc(o[1][1]), sc(o[1][2]), sc(o[1][3]));
+                loss_st4(gx + 2 * (size_t)g.Np + p0, sc(o[2][0]), sc(o[2][1]), sc(o[2][2]), sc(o[2][3]));
             }
         } else {
             int y = p0 / g.Wp, x = p0 - y * g.Wp;
@@ -156,16 +162,17 @@ __global__ void __launch_bounds__(kThreads) coord_loss_kernel(const CoordImage* 
                 if (q >= 0) {
                     const float ex = qx[q], ey = qy[q], ez = qz[q];
                     if (gt_valid(ex, ey, ez)) {
-                        const CellOut r = coord_cell<GRAD>(px[p0 + i], py[p0 + i], pz[p0 + i], ex, ey, ez, cut, cnt);
+                        const CellOut r = coord_cell<GRAD>(loss_in(px[p0 + i]), loss_in(py[p0 + i]), loss_in(pz[p0 + i]), ex, ey,
+                                                           ez, cut, cnt);
                         acc += r.loss;
                         ++nvalid;
                         rx = r.gx; ry = r.gy; rz = r.gz;
                     }
                 }
                 if (GRAD) {
-                    gx[p0 + i] = rx;
-                    gx[g.Np + p0 + i] = ry;
-                    gx[2 * (size_t)g.Np + p0 + i] = rz;
+                    gx[p0 + i] = loss_out<T>(loss_scale<SCALE>(rx, s));
+                    gx[g.Np + p0 + i] = loss_out<T>(loss_scale<SCALE>(ry, s));
+                    gx[2 * (size_t)g.Np + p0 + i] = loss_out<T>(loss_scale<SCALE>(rz, s));
                 }
                 if (++x == g.Wp) { x = 0; ++y; }
             }
@@ -180,34 +187,54 @@ __global__ void __launch_bounds__(kThreads) coord_loss_kernel(const CoordImage* 
 
 }  // namespace
 
-bool coord_image(CoordImage& r, int Hp, int Wp, int Hg, int Wg) {
+bool coord_image(CoordImage& r, int Hp, int Wp, int Hg, int Wg, int esize) {
     r.Np = Hp * Wp; r.Ng = Hg * Wg; r.Wp = Wp; r.Wg = Wg;
     r.H = Hp < Hg ? Hp : Hg;
     r.W = Wp < Wg ? Wp : Wg;
     r.N = r.H * r.W;
     r.blocks = reproj_blocks_per_image(r.Np);
     r.pad = 0;
-    // 128-bit path: equal row pitch (the window is then the first N cells of every plane), every plane 16-byte aligned
-    return Wp == Wg && r.N % 4 == 0 && r.Np % 4 == 0 && r.Ng % 4 == 0 && (uintptr_t)r.pred % 16 == 0 &&
-           (uintptr_t)r.gt % 16 == 0 && (!r.grads || (uintptr_t)r.grads % 16 == 0);
+    // vector path: equal row pitch (the window is then the first N cells of every plane), every plane aligned for a 4-element
+    // access (16 bytes for float32, 8 for the 16-bit types; the ground truth is float32)
+    const uintptr_t align = 4 * (uintptr_t)esize;
+    return Wp == Wg && r.N % 4 == 0 && r.Np % 4 == 0 && r.Ng % 4 == 0 && (uintptr_t)r.pred % align == 0 &&
+           (uintptr_t)r.gt % 16 == 0 && (!r.grads || (uintptr_t)r.grads % align == 0);
 }
 
-void launch_coord_loss(bool vec, int pass, bool grad, const CoordImage* recs, int n, int max_blocks, float cut,
-                       unsigned* counts, double* partial, unsigned* tickets, double* losses, long long* out_counts,
-                       cudaStream_t stream) {
+// The loss pass of element type T: loss only, or with gradients (scaled when grad_scale is not null).
+template <class T>
+static void launch_coord_pass(bool vec, bool grad, dim3 grid, const CoordImage* recs, float cut, const float* grad_scale,
+                              unsigned* counts, double* partial, unsigned* tickets, double* losses, long long* out_counts,
+                              cudaStream_t stream) {
+#define ESAC_COORD_LOSS(V, G, S) \
+    coord_loss_kernel<T, V, G, S><<<grid, kThreads, 0, stream>>>(recs, cut, grad_scale, counts, partial, tickets, losses, out_counts)
+    if (!grad) {
+        if (vec) ESAC_COORD_LOSS(true, false, false);
+        else ESAC_COORD_LOSS(false, false, false);
+    } else if (!grad_scale) {
+        if (vec) ESAC_COORD_LOSS(true, true, false);
+        else ESAC_COORD_LOSS(false, true, false);
+    } else if constexpr (!std::is_same_v<T, float>) {   // float32 is never scaled in the kernel
+        if (vec) ESAC_COORD_LOSS(true, true, true);
+        else ESAC_COORD_LOSS(false, true, true);
+    }
+#undef ESAC_COORD_LOSS
+}
+
+void launch_coord_loss(bool vec, int pass, bool grad, int dtype, const CoordImage* recs, int n, int max_blocks, float cut,
+                       const float* grad_scale, unsigned* counts, double* partial, unsigned* tickets, double* losses,
+                       long long* out_counts, cudaStream_t stream) {
     const dim3 grid(max_blocks, n);
-    if (pass == 1) {
+    if (pass == 1) {   // reads the float32 ground truth only: one kernel for every dtype
         if (vec) coord_count_kernel<true><<<grid, kThreads, 0, stream>>>(recs, counts);
         else coord_count_kernel<false><<<grid, kThreads, 0, stream>>>(recs, counts);
-    } else if (grad) {
-        if (vec)
-            coord_loss_kernel<true, true><<<grid, kThreads, 0, stream>>>(recs, cut, counts, partial, tickets, losses, out_counts);
-        else
-            coord_loss_kernel<false, true><<<grid, kThreads, 0, stream>>>(recs, cut, counts, partial, tickets, losses, out_counts);
-    } else if (vec) {
-        coord_loss_kernel<true, false><<<grid, kThreads, 0, stream>>>(recs, cut, counts, partial, tickets, losses, out_counts);
+    } else if (dtype == kLossF32) {
+        launch_coord_pass<float>(vec, grad, grid, recs, cut, nullptr, counts, partial, tickets, losses, out_counts, stream);
+    } else if (dtype == kLossF16) {
+        launch_coord_pass<__half>(vec, grad, grid, recs, cut, grad_scale, counts, partial, tickets, losses, out_counts, stream);
     } else {
-        coord_loss_kernel<false, false><<<grid, kThreads, 0, stream>>>(recs, cut, counts, partial, tickets, losses, out_counts);
+        launch_coord_pass<__nv_bfloat16>(vec, grad, grid, recs, cut, grad_scale, counts, partial, tickets, losses, out_counts,
+                                         stream);
     }
 }
 

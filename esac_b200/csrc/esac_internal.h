@@ -4,6 +4,9 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
 #include "esac_geom.cuh"
 
 namespace esacb200 {
@@ -382,28 +385,71 @@ const void* gate_mark_fn();
 void launch_gate_arm(const GateArm& a, cudaStream_t stream);
 void launch_gate_mark(const GateTag& t, cudaStream_t stream);
 
+// --- the expert losses' element types -------------------------------------------------------
+// The predictions and gradients of one loss call share one element type, the C ABI's dtype code (ESACB200_FLOAT32,
+// _FLOAT16, _BFLOAT16); the ground truth is always float32.  The kernels widen every prediction to fp32 and compute exactly
+// as on a float32 map, and round each gradient to the element type once, after the optional device-side scale s:
+// (g * s) as one fp32 multiply, then round to nearest.
+enum LossDtype : int { kLossF32 = 0, kLossF16 = 1, kLossBF16 = 2 };
+inline int loss_elem_bytes(int dtype) { return dtype == kLossF32 ? 4 : 2; }
+
+#ifdef __CUDACC__
+__device__ __forceinline__ float loss_in(float v) { return v; }
+__device__ __forceinline__ float loss_in(__half v) { return __half2float(v); }
+__device__ __forceinline__ float loss_in(__nv_bfloat16 v) { return __bfloat162float(v); }
+template <class T> __device__ __forceinline__ T loss_out(float v);
+template <> __device__ __forceinline__ float loss_out<float>(float v) { return v; }
+template <> __device__ __forceinline__ __half loss_out<__half>(float v) { return __float2half_rn(v); }
+template <> __device__ __forceinline__ __nv_bfloat16 loss_out<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
+
+// Four consecutive elements, streamed: one 128-bit access for float, one 64-bit access for the 16-bit types (a warp still
+// moves 256 contiguous bytes per plane).
+__device__ __forceinline__ float4 loss_ld4(const float* p) { return __ldcs(reinterpret_cast<const float4*>(p)); }
+template <class T>
+__device__ __forceinline__ float4 loss_ld4(const T* p) {
+    union { uint2 u; T e[4]; } v;
+    v.u = __ldcs(reinterpret_cast<const uint2*>(p));
+    return make_float4(loss_in(v.e[0]), loss_in(v.e[1]), loss_in(v.e[2]), loss_in(v.e[3]));
+}
+__device__ __forceinline__ void loss_st4(float* p, float a, float b, float c, float d) {
+    __stcs(reinterpret_cast<float4*>(p), make_float4(a, b, c, d));
+}
+template <class T>
+__device__ __forceinline__ void loss_st4(T* p, float a, float b, float c, float d) {
+    union { uint2 u; T e[4]; } v;
+    v.e[0] = loss_out<T>(a); v.e[1] = loss_out<T>(b); v.e[2] = loss_out<T>(c); v.e[3] = loss_out<T>(d);
+    __stcs(reinterpret_cast<uint2*>(p), v.u);
+}
+// The gradient's scale: g * s with round to nearest, never contracted into a neighbouring add.
+template <bool SCALE>
+__device__ __forceinline__ float loss_scale(float g, float s) { return SCALE ? __fmul_rn(g, s) : g; }
+#endif
+
 // --- reproj.cu ----------------------------------------------------------------------------
 // Blocks of one image in the loss kernels of reproj.cu and coord_loss.cu: a pure function of its cell count N, so an image
 // is cut into the same blocks, and summed in the same order, whatever else is in the batch.
 int reproj_blocks_per_image(int N);
 // One image of a reprojection-loss launch.  The image's blocks are blockIdx.x < blocks of grid row blockIdx.y; its block
-// partials are partial[part0 .. part0 + blocks).
+// partials are partial[part0 .. part0 + blocks).  The maps hold elements of the call's dtype.
 struct ReprojImage {
-    const float* coords;   // [3, H, W]
-    float* grads;          // [3, H, W] overwritten, or null (loss only)
+    const void* coords;    // [3, H, W]
+    void* grads;           // [3, H, W] overwritten, or null (loss only)
     int N, W;              // cells, row pitch
     int b;                 // index in the batch: img record, ticket, loss
     int blocks;            // reproj_blocks_per_image(N)
     long long part0;
 };
-// 128-bit loads and stores for this image: N % 4 == 0, W >= 4, 16-byte aligned planes.
-bool reproj_vec_ok(const float* coords, const float* grads, int N, int W);
+// Vector loads and stores for this image (4 elements of `esize` bytes per access): N % 4 == 0, W >= 4, planes aligned to
+// 4 * esize bytes.
+bool reproj_vec_ok(const void* coords, const void* grads, int N, int W, int esize);
 // img: per image kReprojImgFloats floats = world->camera 3x4 (row major), padX, padY, f, cx, cy, 3 unused.  recs: n device
 // records, all on the load path `vec`; max_blocks = their largest block count.  tickets: zeroed counters per batch image
-// (left zeroed), losses: a double per batch image.
+// (left zeroed), losses: a double per batch image.  dtype: the maps' LossDtype; grad_scale: a device float that scales
+// every gradient, or null (float32 always null).
 constexpr int kReprojImgFloats = 20;
-void launch_reproj(bool vec, const ReprojImage* recs, int n, int max_blocks, const float* img, float sub, float cut,
-                   float max_err, float min_depth, double* partial, unsigned* tickets, double* losses, cudaStream_t stream);
+void launch_reproj(bool vec, int dtype, const ReprojImage* recs, int n, int max_blocks, const float* img, float sub, float cut,
+                   float max_err, float min_depth, const float* grad_scale, double* partial, unsigned* tickets, double* losses,
+                   cudaStream_t stream);
 
 // fp64 products and sums rounded once each, on both sides: nvcc would contract a*b - c*d into an FMA, the host compiler
 // (no -march) does not, and the reprojection loss's ground-truth inversion must round alike on the host and the device.
@@ -467,11 +513,11 @@ ESAC_HD bool reproj_img_row(const float* T, int padX, int padY, float f, float c
 // --- coord_loss.cu ------------------------------------------------------------------------
 // One image of a coordinate-loss launch: pred [3,Hp,Wp], gt [3,Hg,Wg] (|Hp-Hg|, |Wp-Wg| <= 1, checked by the caller),
 // grads [3,Hp,Wp] overwritten or null (loss only).  blocks = reproj_blocks_per_image(Np), partials part0 .. part0 + blocks
-// (2 doubles each), as for ReprojImage.
+// (2 doubles each), as for ReprojImage.  pred and grads hold elements of the call's dtype, gt float32.
 struct CoordImage {
-    const float* pred;
+    const void* pred;
     const float* gt;
-    float* grads;
+    void* grads;
     int Np, Ng;   // plane sizes of the prediction / the ground truth (Hp*Wp, Hg*Wg)
     int Wp, Wg;   // their row pitches
     int H, W;     // the common top-left window
@@ -481,15 +527,17 @@ struct CoordImage {
     int pad;
     long long part0;
 };
-// Fills the geometry of r from the two sizes and picks the load path: 128-bit when the row pitches are equal (the window is
-// then the first N cells of every plane), N, Np, Ng % 4 == 0 and every plane is 16-byte aligned.
-bool coord_image(CoordImage& r, int Hp, int Wp, int Hg, int Wg);
+// Fills the geometry of r from the two sizes and picks the load path: vector loads when the row pitches are equal (the
+// window is then the first N cells of every plane), N, Np, Ng % 4 == 0, the ground truth's planes are 16-byte aligned and
+// the prediction's and gradient's planes are aligned to 4 * esize bytes.
+bool coord_image(CoordImage& r, int Hp, int Wp, int Hg, int Wg, int esize);
 // Both passes run on a (max_blocks, n) grid of 256-thread blocks, 4 cells per thread, as the reprojection loss; recs: n
 // device records on load path `vec`.  counts: a zeroed counter per batch image (gradient only), tickets: zeroed counters
-// (left zeroed), losses / out_counts: per batch image.  pass 1 = count pass (gradient only), 2 = loss pass.
-void launch_coord_loss(bool vec, int pass, bool grad, const CoordImage* recs, int n, int max_blocks, float cut,
-                       unsigned* counts, double* partial, unsigned* tickets, double* losses, long long* out_counts,
-                       cudaStream_t stream);
+// (left zeroed), losses / out_counts: per batch image.  pass 1 = count pass (gradient only), 2 = loss pass.  dtype and
+// grad_scale as for launch_reproj.
+void launch_coord_loss(bool vec, int pass, bool grad, int dtype, const CoordImage* recs, int n, int max_blocks, float cut,
+                       const float* grad_scale, unsigned* counts, double* partial, unsigned* tickets, double* losses,
+                       long long* out_counts, cudaStream_t stream);
 // The largest reproj_blocks_per_image(n) over n <= N (the count is not monotonic in N): the partials that a workspace for
 // maps of at most N cells must hold per image.
 int reproj_max_blocks(int N);
@@ -504,9 +552,10 @@ template <class Rec> constexpr int loss_chunk() { return (int)(kLossChunkBytes /
 int launch_reproj_prep(const ReprojImage* host_recs, int n, ReprojImage* recs, const float* gt16, const int* shifts,
                        const float* cameras, float* img, int* bad, cudaStream_t st);
 // out_losses[b] = losses[b] (NaN when bad[b]), status[b] = bad[b], and the gradient of a bad image zeroed (grads: the call
-// has gradients).  recs: the B device records.
-void launch_reproj_finish(const ReprojImage* recs, int B, bool grads, const double* losses, const int* bad, double* out_losses,
-                          int* status, cudaStream_t st);
+// has gradients; a zero of the call's dtype, scaled by grad_scale as the loss kernel scales every gradient).  recs: the B
+// device records.
+void launch_reproj_finish(const ReprojImage* recs, int B, bool grads, int dtype, const float* grad_scale, const double* losses,
+                          const int* bad, double* out_losses, int* status, cudaStream_t st);
 // The n host records into recs, in chunks.  Returns the launches.
 int launch_coord_prep(const CoordImage* host_recs, int n, CoordImage* recs, cudaStream_t st);
 // out_losses[b] = losses[b], out_counts[b] = counts[b] (out_counts may be null).

@@ -38,10 +38,11 @@ __global__ void __launch_bounds__(32) reproj_prep_kernel(const RecChunk<ReprojIm
 }
 
 // grid = (gblocks, B), row blockIdx.y = record blockIdx.y of image b: block 0 writes the loss (NaN when bad) and the
-// status; the blocks of a bad image zero its gradient.
+// status; the blocks of a bad image zero its gradient: elements of type T, each the rounded (0 * s) of a scaled call.
+template <class T>
 __global__ void __launch_bounds__(256) reproj_finish_kernel(const ReprojImage* __restrict__ recs, const double* __restrict__ losses,
-                                                            const int* __restrict__ bad, double* __restrict__ out_losses,
-                                                            int* __restrict__ status) {
+                                                            const int* __restrict__ bad, const float* __restrict__ grad_scale,
+                                                            double* __restrict__ out_losses, int* __restrict__ status) {
     const ReprojImage r = recs[blockIdx.y];
     const int b = r.b;
     const bool is_bad = bad[b] != 0;
@@ -51,7 +52,9 @@ __global__ void __launch_bounds__(256) reproj_finish_kernel(const ReprojImage* _
     }
     if (!is_bad || !r.grads) return;
     const size_t n = 3 * (size_t)r.N;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) r.grads[i] = 0.f;
+    const T zero = loss_out<T>(grad_scale ? __fmul_rn(0.f, *grad_scale) : 0.f);
+    T* g = static_cast<T*>(r.grads);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) g[i] = zero;
 }
 
 // One block: records 0 .. n-1 of this chunk into recs.
@@ -85,9 +88,15 @@ int launch_reproj_prep(const ReprojImage* host_recs, int n, ReprojImage* recs, c
     return launches;
 }
 
-void launch_reproj_finish(const ReprojImage* recs, int B, bool grads, const double* losses, const int* bad, double* out_losses,
-                          int* status, cudaStream_t st) {
-    reproj_finish_kernel<<<dim3(grads ? kZeroBlocks : 1, B), 256, 0, st>>>(recs, losses, bad, out_losses, status);
+void launch_reproj_finish(const ReprojImage* recs, int B, bool grads, int dtype, const float* grad_scale, const double* losses,
+                          const int* bad, double* out_losses, int* status, cudaStream_t st) {
+    const dim3 grid(grads ? kZeroBlocks : 1, B);
+    if (dtype == kLossF32)
+        reproj_finish_kernel<float><<<grid, 256, 0, st>>>(recs, losses, bad, nullptr, out_losses, status);
+    else if (dtype == kLossF16)
+        reproj_finish_kernel<__half><<<grid, 256, 0, st>>>(recs, losses, bad, grad_scale, out_losses, status);
+    else
+        reproj_finish_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>(recs, losses, bad, grad_scale, out_losses, status);
 }
 
 int launch_coord_prep(const CoordImage* host_recs, int n, CoordImage* recs, cudaStream_t st) {

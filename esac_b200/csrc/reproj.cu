@@ -137,11 +137,13 @@ __device__ __forceinline__ PairOut reproj_pair(float2 X, float2 Y, float2 Z, con
 
 // grid = (max blocks, images of this load path).  Row blockIdx.y is image recs[blockIdx.y]; its blocks are blockIdx.x <
 // rec.blocks, the others leave at once.  img[b] = kReprojImgFloats floats: 12 matrix entries, padX, padY, f, cx, cy, 3 unused.
-template <bool VEC>
+// T: the maps' element type (float, __half, __nv_bfloat16), widened on load; SCALE: every gradient times *grad_scale
+// (loss_scale) before it is rounded to T.
+template <class T, bool VEC, bool SCALE>
 __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const ReprojImage* __restrict__ recs, const float* __restrict__ img,
                                                           float sub, float cut, float max_err, float min_depth,
-                                                          double* __restrict__ partial, unsigned* __restrict__ tickets,
-                                                          double* __restrict__ losses) {
+                                                          const float* __restrict__ grad_scale, double* __restrict__ partial,
+                                                          unsigned* __restrict__ tickets, double* __restrict__ losses) {
     __shared__ float m[kReprojImgFloats];
     // The image's geometry sits in shared memory and is re-read where it is used (volatile).  Unlike kernel parameters,
     // loaded values cannot be rematerialised: held in registers across the loop they would push the scalar path over the
@@ -173,12 +175,12 @@ __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const ReprojImage* 
         float X[4], Y[4], Z[4];
         int n = min(kCellsPerThread, N - p0);
         if (VEC) {
-            const float* px = vrec.coords;
-            const float* py = px + N;
-            const float* pz = py + N;
-            const float4 a = __ldcs(reinterpret_cast<const float4*>(px + p0));
-            const float4 c = __ldcs(reinterpret_cast<const float4*>(py + p0));
-            const float4 d = __ldcs(reinterpret_cast<const float4*>(pz + p0));
+            const T* px = static_cast<const T*>(vrec.coords);
+            const T* py = px + N;
+            const T* pz = py + N;
+            const float4 a = loss_ld4(px + p0);
+            const float4 c = loss_ld4(py + p0);
+            const float4 d = loss_ld4(pz + p0);
             X[0] = a.x; X[1] = a.y; X[2] = a.z; X[3] = a.w;
             Y[0] = c.x; Y[1] = c.y; Y[2] = c.z; Y[3] = c.w;
             Z[0] = d.x; Z[1] = d.y; Z[2] = d.z; Z[3] = d.w;
@@ -211,33 +213,36 @@ __global__ void __launch_bounds__(kThreads, 5) reproj_kernel(const ReprojImage* 
 #pragma unroll
             for (int i = 0; i < 4; ++i) {
                 // each cell is loaded where it is used: four cells of inputs held at once would not fit the register budget
-                const float* c = vrec.coords;
+                const T* c = static_cast<const T*>(vrec.coords);
                 const bool ok = i < n;
-                X[i] = ok ? c[p0 + i] : 0.f;
-                Y[i] = ok ? c[vrec.N + p0 + i] : 0.f;
-                Z[i] = ok ? c[2 * (size_t)vrec.N + p0 + i] : 1.f;
+                X[i] = ok ? loss_in(c[p0 + i]) : 0.f;
+                Y[i] = ok ? loss_in(c[vrec.N + p0 + i]) : 0.f;
+                Z[i] = ok ? loss_in(c[2 * (size_t)vrec.N + p0 + i]) : 1.f;
                 const float tx = fmaf((float)x, sub, half) - padX;
                 const float ty = fmaf((float)y, sub, half) - padY;
                 const CellOut o = reproj_cell(X[i], Y[i], Z[i], m, m[14], m[15], m[16], tx, ty, cut, max_err, min_depth, inv_n);
                 if (i < n) {
                     four += o.loss;
-                    float* g = vrec.grads;
+                    T* g = static_cast<T*>(vrec.grads);
                     if (g) {   // stored as computed: no gradient array stays live across the four cells
                         const int Nv = vrec.N;
-                        g[p0 + i] = o.gx;
-                        g[Nv + p0 + i] = o.gy;
-                        g[2 * (size_t)Nv + p0 + i] = o.gz;
+                        const float s = SCALE ? *grad_scale : 1.f;
+                        g[p0 + i] = loss_out<T>(loss_scale<SCALE>(o.gx, s));
+                        g[Nv + p0 + i] = loss_out<T>(loss_scale<SCALE>(o.gy, s));
+                        g[2 * (size_t)Nv + p0 + i] = loss_out<T>(loss_scale<SCALE>(o.gz, s));
                     }
                 }
                 if (++x == vrec.W) { x = 0; ++y; }
             }
         }
         acc += (double)four;
-        float* gx = vrec.grads;
+        T* gx = static_cast<T*>(vrec.grads);
         if (VEC && gx) {
-            __stcs(reinterpret_cast<float4*>(gx + p0), make_float4(ox[0], ox[1], ox[2], ox[3]));
-            __stcs(reinterpret_cast<float4*>(gx + N + p0), make_float4(oy[0], oy[1], oy[2], oy[3]));
-            __stcs(reinterpret_cast<float4*>(gx + 2 * (size_t)N + p0), make_float4(oz[0], oz[1], oz[2], oz[3]));
+            const float s = SCALE ? *grad_scale : 1.f;
+            auto sc = [s](float g) { return loss_scale<SCALE>(g, s); };
+            loss_st4(gx + p0, sc(ox[0]), sc(ox[1]), sc(ox[2]), sc(ox[3]));
+            loss_st4(gx + N + p0, sc(oy[0]), sc(oy[1]), sc(oy[2]), sc(oy[3]));
+            loss_st4(gx + 2 * (size_t)N + p0, sc(oz[0]), sc(oz[1]), sc(oz[2]), sc(oz[3]));
         }
     }
     // block sum in a fixed order, then the last block of the image adds the partials, again in a fixed order
@@ -271,17 +276,40 @@ int reproj_max_blocks(int N) {
     return most;
 }
 
-bool reproj_vec_ok(const float* coords, const float* grads, int N, int W) {
-    return (N % 4 == 0) && W >= 4 && ((uintptr_t)coords % 16 == 0) && (!grads || (uintptr_t)grads % 16 == 0);
+bool reproj_vec_ok(const void* coords, const void* grads, int N, int W, int esize) {
+    const uintptr_t align = 4 * (uintptr_t)esize;
+    return (N % 4 == 0) && W >= 4 && ((uintptr_t)coords % align == 0) && (!grads || (uintptr_t)grads % align == 0);
 }
 
-void launch_reproj(bool vec, const ReprojImage* recs, int n, int max_blocks, const float* img, float sub, float cut,
-                   float max_err, float min_depth, double* partial, unsigned* tickets, double* losses, cudaStream_t stream) {
-    const dim3 grid(max_blocks, n);
+template <class T, bool SCALE>
+static void launch_reproj_typed(bool vec, dim3 grid, const ReprojImage* recs, const float* img, float sub, float cut,
+                                float max_err, float min_depth, const float* grad_scale, double* partial, unsigned* tickets,
+                                double* losses, cudaStream_t stream) {
     if (vec)
-        reproj_kernel<true><<<grid, kThreads, 0, stream>>>(recs, img, sub, cut, max_err, min_depth, partial, tickets, losses);
+        reproj_kernel<T, true, SCALE><<<grid, kThreads, 0, stream>>>(recs, img, sub, cut, max_err, min_depth, grad_scale, partial,
+                                                                     tickets, losses);
     else
-        reproj_kernel<false><<<grid, kThreads, 0, stream>>>(recs, img, sub, cut, max_err, min_depth, partial, tickets, losses);
+        reproj_kernel<T, false, SCALE><<<grid, kThreads, 0, stream>>>(recs, img, sub, cut, max_err, min_depth, grad_scale, partial,
+                                                                      tickets, losses);
+}
+
+void launch_reproj(bool vec, int dtype, const ReprojImage* recs, int n, int max_blocks, const float* img, float sub, float cut,
+                   float max_err, float min_depth, const float* grad_scale, double* partial, unsigned* tickets, double* losses,
+                   cudaStream_t stream) {
+    const dim3 grid(max_blocks, n);
+    const bool scale = grad_scale != nullptr;
+    if (dtype == kLossF32)   // float32 is never scaled in the kernel
+        launch_reproj_typed<float, false>(vec, grid, recs, img, sub, cut, max_err, min_depth, nullptr, partial, tickets, losses, stream);
+    else if (dtype == kLossF16 && scale)
+        launch_reproj_typed<__half, true>(vec, grid, recs, img, sub, cut, max_err, min_depth, grad_scale, partial, tickets, losses, stream);
+    else if (dtype == kLossF16)
+        launch_reproj_typed<__half, false>(vec, grid, recs, img, sub, cut, max_err, min_depth, nullptr, partial, tickets, losses, stream);
+    else if (scale)
+        launch_reproj_typed<__nv_bfloat16, true>(vec, grid, recs, img, sub, cut, max_err, min_depth, grad_scale, partial, tickets,
+                                                 losses, stream);
+    else
+        launch_reproj_typed<__nv_bfloat16, false>(vec, grid, recs, img, sub, cut, max_err, min_depth, nullptr, partial, tickets,
+                                                  losses, stream);
 }
 
 }  // namespace esacb200

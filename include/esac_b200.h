@@ -491,6 +491,36 @@ int esacb200_coord_loss_async(esacb200_ctx* ctx, int B, const float* const* pred
                               double* out_losses, int64_t* out_counts);
 int esacb200_reserve_loss_async(esacb200_ctx* ctx, int B, int H, int W);
 
+/* The four loss calls above on predictions of a chosen element type, for experts trained under autocast.  dtype is one
+ * code for the whole call: the predictions and gradients (coords / pred, grads) are B pointers to elements of that type;
+ * the ground truth, poses and cameras stay float32.  Each prediction is widened to fp32 and computed exactly as the float32
+ * call computes it on the widened map, so the losses are bitwise the float32 call's on the same load path (the vector path
+ * needs N % 4 == 0, W >= 4 and planes aligned to 4 elements; the float32 and the 16-bit calls choose it alike for maps
+ * aligned alike).  Each gradient is the float32 call's gradient g, times *grad_scale as one fp32 multiply when grad_scale
+ * is not NULL, rounded to nearest into dtype: bitwise what autograd gives a 16-bit prediction that was cast to float32
+ * before a float32 loss whose upstream gradient is *grad_scale.  grad_scale: a device float, read when the kernels run
+ * (so a capture replays with the current scale), or NULL for 1.  ESACB200_FLOAT16 and ESACB200_BFLOAT16 take device
+ * pointers only.  An unknown code, a host pointer with a 16-bit code, or a grad_scale with ESACB200_FLOAT32 fails with
+ * ESACB200_ERR_ARG before anything is enqueued.  The workspace is the float32 calls' (esacb200_reserve_loss_async covers
+ * both); the untyped calls are these with ESACB200_FLOAT32 and grad_scale NULL. */
+#define ESACB200_FLOAT32 0
+#define ESACB200_FLOAT16 1
+#define ESACB200_BFLOAT16 2
+int esacb200_reproj_loss_ragged_typed(esacb200_ctx* ctx, int B, int dtype, const void* const* coords, void* const* grads,
+                                      const int* H, const int* W, const float* gt_poses, const int* shiftX, const int* shiftY,
+                                      const float* f, const float* ppx, const float* ppy, int subSampling, float cutLoss,
+                                      float maxReproj, float minDepth, const float* grad_scale, double* out_losses);
+int esacb200_coord_loss_ragged_typed(esacb200_ctx* ctx, int B, int dtype, const void* const* pred, const int* Hp, const int* Wp,
+                                     const float* const* gt, const int* Hg, const int* Wg, void* const* grads, float cutLoss,
+                                     const float* grad_scale, double* out_losses, int64_t* out_counts);
+int esacb200_reproj_loss_async_typed(esacb200_ctx* ctx, int B, int dtype, const void* const* coords, void* const* grads,
+                                     const int* H, const int* W, const float* gt_poses, const int32_t* shifts,
+                                     const float* cameras, int subSampling, float cutLoss, float maxReproj, float minDepth,
+                                     const float* grad_scale, double* out_losses, int32_t* out_status);
+int esacb200_coord_loss_async_typed(esacb200_ctx* ctx, int B, int dtype, const void* const* pred, const int* Hp, const int* Wp,
+                                    const float* const* gt, const int* Hg, const int* Wg, void* const* grads, float cutLoss,
+                                    const float* grad_scale, double* out_losses, int64_t* out_counts);
+
 /* Soft-inlier scores of given poses (getReproErrs + getHypScores, esac_util.h:235-363) without
  * sampling/selection/refinement: poses6 = host double [M][6] (rvec, tvec); out_scores host double [M]. */
 int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,

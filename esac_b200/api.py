@@ -190,6 +190,9 @@ def load_library() -> C.CDLL:
     lib.esacb200_reserve_loss_async.argtypes = [vp, i32, i32, i32]
     lib.esacb200_reserve_loss_async.restype = i32
     lib.esacb200_reserve_backward_async.restype = i32
+    for name in ("eval_poses", "eval_poses_async"):
+        getattr(lib, "esacb200_" + name).argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, vp, vp, i64, vp]
+        getattr(lib, "esacb200_" + name).restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
         getattr(lib, "esacb200_" + name).restype = i32
@@ -1686,6 +1689,78 @@ def reserve_loss_async(B: int, H: int, W: int, device: int | None = None):
     """Sizes the workspace of reproj_loss_async and coord_loss_async (and of their _amp forms, which use the same) for B
     images of at most H x W cells (the prediction's); call it before capturing (it allocates)."""
     _reserve_async("reserve_loss_async", device, dict(B=B, H=H, W=W))
+
+
+# The columns of a pose evaluation's record (include/esac_b200.h, esacb200_eval_poses): float64, one row per image.
+EVAL_FIELDS = ("rot_deg", "trans_cm", "correct", "scene", "expert", "status", "active", "qw", "qx", "qy", "qz", "tx", "ty", "tz")
+EVAL_STATE = 4  # int64 words of a record store's device state: rows handed out, overflow flag, launch ticket, unused
+
+
+def _eval_context(call, outPoses, gtPoses, experts, gtScenes, hist, status, outRecords, state):
+    """The checks of evaluate_poses / evaluate_poses_async before any context exists; returns (ctx, B, E, capacity)."""
+    for what, t in (("outPoses", outPoses), ("outRecords", outRecords)):
+        if not _is_torch(t):
+            raise RuntimeError(f"{call} takes torch CUDA tensors only ({what} is a {type(t).__name__})")
+    _check(outPoses, "Float", 3 if outPoses.dim() == 3 else 2, "outPoses")
+    lead = tuple(int(v) for v in outPoses.shape[:-2])
+    if tuple(int(v) for v in outPoses.shape[-2:]) != (4, 4) or (lead and lead[0] < 1):
+        raise RuntimeError(f"outPoses must be [B,4,4] or [4,4], got {list(outPoses.shape)}")
+    B = lead[0] if lead else 1
+    _check(outRecords, "Double", 2, "outRecords")
+    capacity = int(outRecords.shape[0])
+    if capacity < 1:
+        raise RuntimeError("outRecords holds no row")
+    fixed = {"outPoses": (outPoses, "Float", lead + (4, 4)), "gtPoses": (gtPoses, "Float", lead + (4, 4)),
+             "experts": (experts, "Long", lead), "gtScenes": (gtScenes, "Long", lead),
+             "outRecords": (outRecords, "Double", (capacity, len(EVAL_FIELDS))), "state": (state, "Long", (EVAL_STATE,))}
+    E = 0
+    if hist is not None:
+        if not _is_torch(hist) or hist.dim() != len(lead) + 1:
+            raise RuntimeError(f"hist must be a float32 tensor [B,E] or [E], got "
+                               f"{list(hist.shape) if _is_torch(hist) else type(hist).__name__}")
+        E = int(hist.shape[-1])
+        if not 1 <= E <= MAX_EXPERTS:
+            raise RuntimeError(f"{call}: hist holds E={E} experts, outside [1, {MAX_EXPERTS}]")
+        fixed["hist"] = (hist, "Float", lead + (E,))
+    if status is not None:
+        fixed["status"] = (status, "Int", lead)
+    return _async_context(call, fixed, []), B, E, capacity
+
+
+def _eval_call(name, ctx, B, E, capacity, outPoses, gtPoses, experts, gtScenes, hist, status, outRecords, state):
+    ctx.check(getattr(ctx.lib, name)(ctx.handle, B, outPoses.data_ptr(), gtPoses.data_ptr(), experts.data_ptr(),
+                                     gtScenes.data_ptr(), hist.data_ptr() if hist is not None else None, E,
+                                     status.data_ptr() if status is not None else None, outRecords.data_ptr(), capacity,
+                                     state.data_ptr()))
+
+
+def evaluate_poses_async(outPoses, gtPoses, experts, gtScenes, outRecords, state, hist=None, status=None):
+    """test_esac.py's per-image evaluation (pose errors, correct expert, experts active, pose-file entry) enqueued on torch's
+    current stream with no host synchronisation, so that a CUDA graph can capture it.  CUDA tensors only, contiguous:
+    outPoses / gtPoses float32 [B,4,4] (or [4,4]) camera->world, experts / gtScenes int64 [B] (or []), hist float32 [B,E]
+    (or [E]; assign_hypotheses_async's histogram) or None, status int32 [B] (or []; forward_async's) or None.  Image b's
+    record (EVAL_FIELDS, float64) goes to row state[0] + b of outRecords float64 [capacity, 14]; state int64 [4] is the
+    store's device state (zero it to start; state[1] becomes 1 when a row falls past capacity, and that row is dropped)."""
+    ctx, B, E, capacity = _eval_context("evaluate_poses_async", outPoses, gtPoses, experts, gtScenes, hist, status,
+                                        outRecords, state)
+    _eval_call("esacb200_eval_poses_async", ctx, B, E, capacity, outPoses, gtPoses, experts, gtScenes, hist, status,
+               outRecords, state)
+
+
+def evaluate_poses(outPoses, gtPoses, experts, gtScenes, hist=None, status=None):
+    """evaluate_poses_async into a fresh store, synchronised: returns the records, float64 [B,14] (EVAL_FIELDS) for a batch
+    or [14] for one [4,4] pose, on the poses' device."""
+    call = "evaluate_poses"
+    if not _is_torch(outPoses):
+        raise RuntimeError(f"{call} takes torch CUDA tensors only (outPoses is a {type(outPoses).__name__})")
+    import torch
+    B = int(outPoses.shape[0]) if outPoses.dim() == 3 else 1
+    dev = outPoses.device
+    records = torch.empty((max(B, 1), len(EVAL_FIELDS)), dtype=torch.float64, device=dev)
+    state = torch.zeros(EVAL_STATE, dtype=torch.int64, device=dev)
+    ctx, B, E, capacity = _eval_context(call, outPoses, gtPoses, experts, gtScenes, hist, status, records, state)
+    _eval_call("esacb200_eval_poses", ctx, B, E, capacity, outPoses, gtPoses, experts, gtScenes, hist, status, records, state)
+    return records if outPoses.dim() == 3 else records[0]
 
 
 def set_seed(seed: int, device: int | None = None):

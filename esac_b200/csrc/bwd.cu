@@ -36,26 +36,11 @@ int bwd_tiles(int N) { return (N + kBwdTile - 1) / kBwdTile; }
 // trans2pose for the (float) ground truth: general affine inverse like cv::Mat::inv, then Rodrigues.
 __device__ void gt_trans2pose(const float* gt, Pose& p, double T[16]) {
     for (int i = 0; i < 16; ++i) T[i] = (double)gt[i];
-    double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]};
-    double B[9];
-    adj3(R, B);
-    double d = R[0] * B[0] + R[1] * B[3] + R[2] * B[6];
     double Ri[9];
-    for (int i = 0; i < 9; ++i) Ri[i] = B[i] / d;
-    for (int r = 0; r < 3; ++r) p.t[r] = -(Ri[r * 3] * T[3] + Ri[r * 3 + 1] * T[7] + Ri[r * 3 + 2] * T[11]);
-    // polar factor via Newton: X <- (X + X^-T)/2
-    double X[9];
+    affine_inverse(T, Ri, p.t);
+    double X[9];  // a copy of Ri: without it nvcc allocates pose_loss_kernel's registers differently (same arithmetic)
     for (int i = 0; i < 9; ++i) X[i] = Ri[i];
-    for (int it = 0; it < 8; ++it) {
-        double C[9];
-        adj3(X, C);
-        double dd = X[0] * C[0] + X[1] * C[3] + X[2] * C[6];
-        if (!(fabs(dd) > 0)) break;
-        double Y[9];
-        for (int r = 0; r < 3; ++r)
-            for (int c = 0; c < 3; ++c) Y[r * 3 + c] = 0.5 * (X[r * 3 + c] + C[c * 3 + r] / dd);  // X^-T[r][c] = adj[c][r]/det
-        for (int i = 0; i < 9; ++i) X[i] = Y[i];
-    }
+    polar_newton(X);
     rodrigues_m2v(X, p.r);
 }
 

@@ -7,6 +7,7 @@
 //   capi_hypotheses.cu  the hypotheses node and the pose loss
 //   capi_losses.cu      the two expert losses
 //   capi_gate.cu        expert gates and the stream-ordered hypothesis assignment
+//   capi_eval.cu        test-time pose evaluation
 //   capi_testhooks.cu   include/esac_b200_testhooks.h
 #pragma once
 #include <cuda_runtime.h>

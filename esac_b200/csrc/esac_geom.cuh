@@ -267,6 +267,32 @@ ESAC_HD T trace_prod3(const T A[9], const T B[9]) {  // tr(A*B)
            A[7] * B[5] + A[8] * B[8];
 }
 
+// The nearest rotation of X (its orthogonal polar factor, what OpenCV takes as U*V^T of an SVD before Rodrigues), in place:
+// Newton's iteration X <- (X + X^-T) / 2, eight steps, stopping early on a singular X.
+ESAC_HD void polar_newton(double X[9]) {
+    for (int it = 0; it < 8; ++it) {
+        double C[9];
+        adj3(X, C);
+        double dd = X[0] * C[0] + X[1] * C[3] + X[2] * C[6];
+        if (!(fabs(dd) > 0)) break;
+        double Y[9];
+        for (int r = 0; r < 3; ++r)
+            for (int c = 0; c < 3; ++c) Y[r * 3 + c] = 0.5 * (X[r * 3 + c] + C[c * 3 + r] / dd);  // X^-T[r][c] = adj[c][r]/det
+        for (int i = 0; i < 9; ++i) X[i] = Y[i];
+    }
+}
+
+// The inverse of the affine 4x4 T (row major, last row 0 0 0 1) as cv::Mat::inv and torch's .inverse() compute it, not
+// the rigid shortcut: rotation block Ri = adj(R) / det(R), translation t = -Ri * T[:3,3].
+ESAC_HD void affine_inverse(const double T[16], double Ri[9], double t[3]) {
+    double R[9] = {T[0], T[1], T[2], T[4], T[5], T[6], T[8], T[9], T[10]};
+    double B[9];
+    adj3(R, B);
+    double d = R[0] * B[0] + R[1] * B[3] + R[2] * B[6];
+    for (int i = 0; i < 9; ++i) Ri[i] = B[i] / d;
+    for (int r = 0; r < 3; ++r) t[r] = -(Ri[r * 3] * T[3] + Ri[r * 3 + 1] * T[7] + Ri[r * 3 + 2] * T[11]);
+}
+
 ESAC_HD bool solve3(const double A[9], const double b[3], double x[3]) {
     double B[9];
     adj3(A, B);

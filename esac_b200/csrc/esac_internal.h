@@ -668,4 +668,41 @@ void launch_backward_upstream_async(const BwdArgs& a, const void* tape, const do
 void launch_pose_loss(const Pose* poses, int B, int M, const float* gt16, float wRot, float wTrans, float cut, double* losses,
                       double* dloss6, cudaStream_t st);
 
+// --- eval.cu ------------------------------------------------------------------------------
+// One test image's evaluation (test_esac.py:209-247), the row a pose evaluation writes into the caller's record buffer; all
+// fp64 (include/esac_b200.h documents the row).  Integers are stored exactly; `active` is NaN when the call has no histogram.
+struct EvalRecord {
+    double rot_deg;   // rotation error, degrees (exactly 0 in OpenCV's s < 1e-5, c > 0 branch)
+    double trans_cm;  // translation error, centimetres
+    double correct;   // 1 when expert == scene
+    double scene;     // ground-truth scene (expert) index
+    double expert;    // the winning expert
+    double status;    // the forward's status (0 = counted)
+    double active;    // experts that drew a hypothesis
+    double q[4];      // qw qx qy qz of the inverted estimate (q_xyz NaN at angle 0, as the reference writes it)
+    double t[3];      // tx ty tz of the inverted estimate
+};
+constexpr int kEvalRecordDoubles = sizeof(EvalRecord) / sizeof(double);
+static_assert(kEvalRecordDoubles == 14, "EvalRecord is the 14 doubles include/esac_b200.h documents");
+// The record store's device state: rows written so far (slots handed out, including those past the capacity), a flag set
+// when a slot fell past the capacity, and the CTA ticket of the launch in flight (zero between launches).
+struct EvalState {
+    unsigned long long count, overflow, ticket, unused;
+};
+static_assert(sizeof(EvalState) == 4 * sizeof(long long), "EvalState is 4 int64");
+struct EvalArgs {
+    const float* out_poses;       // [B,4,4] camera->world estimates
+    const float* gt_poses;        // [B,4,4] camera->world ground truths
+    const long long* experts;     // [B] winning experts
+    const long long* scenes;      // [B] ground-truth scenes
+    const float* hist;            // [B,E] hypothesis histogram, or null
+    const int* status;            // [B] forward status, or null (0)
+    int B, E;
+    EvalRecord* records;          // [capacity]
+    long long capacity;
+    EvalState* state;
+};
+// Image b of the call goes to slot state->count + b; the launch's last CTA advances count by B.
+void launch_eval_poses(const EvalArgs& a, cudaStream_t st);
+
 }  // namespace esacb200

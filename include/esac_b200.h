@@ -521,6 +521,34 @@ int esacb200_coord_loss_async_typed(esacb200_ctx* ctx, int B, int dtype, const v
                                     const float* const* gt, const int* Hg, const int* Wg, void* const* grads, float cutLoss,
                                     const float* grad_scale, double* out_losses, int64_t* out_counts);
 
+/* Test-time evaluation of estimated poses (test_esac.py:209-247), so that a captured test step evaluates its image on the
+ * device.  Image b of B: its camera->world estimate out_poses[b] and ground truth gt_poses[b] (float32 [B,4,4]), its
+ * winning expert experts[b] and ground-truth scene scenes[b] (int64 [B]), optionally its hypothesis histogram hist[b]
+ * (float32 [B,E], as esacb200_assign_hypotheses_async writes it) and its forward status status[b] (int32 [B]); hist and
+ * status may be NULL.  Every pointer is a device pointer.  Its record, 14 doubles, goes to row state[0] + b of records
+ * (double [capacity][14]):
+ *   0 rotation error in degrees: acos(c) of the nearest rotation (Newton polar factor) to P_R G_R^T, c and s as OpenCV's
+ *     Rodrigues forms them, and exactly 0 where s < 1e-5 and c > 0 (errors below ~5.7e-4 deg read 0, as in the reference)
+ *   1 translation error |G[:3,3] - P[:3,3]| in centimetres
+ *   2 correct (experts[b] == scenes[b]: 1, else 0)   3 scene   4 expert   5 status (0 without a status array)
+ *   6 experts active: hist[b] entries > 0 (NaN without a histogram)
+ *   7-10 qw qx qy qz and 11-13 tx ty tz of the pose-file line: the general 4x4 inverse of P, the axis-angle vector r of
+ *     its rotation's nearest rotation, q = (cos(|r|/2), sin(|r|/2) r/|r|); q_xyz is NaN where |r| = 0, as the reference
+ *     writes it.
+ * All in fp64 from the float32 inputs.  state: int64 [4], zeroed by the caller before the first call: [0] rows handed out so
+ * far (advanced by B by the launch, after every image has read it), [1] set to 1 when a row fell at or past capacity (that
+ * row is not written), [2] a ticket the launch leaves zero, [3] unused.
+ * esacb200_eval_poses_async enqueues on the context's stream: no host synchronisation, read-back or allocation, so it may be
+ * captured.  esacb200_eval_poses is the same followed by a synchronisation of that stream.  Argument errors
+ * (ESACB200_ERR_ARG: a NULL or host pointer, B outside [1, 2^24], capacity <= 0, E outside [1, ESACB200_GATE_MAX] with a
+ * histogram) are reported before anything is enqueued. */
+int esacb200_eval_poses_async(esacb200_ctx* ctx, int B, const float* out_poses, const float* gt_poses, const int64_t* experts,
+                              const int64_t* scenes, const float* hist, int E, const int32_t* status, double* records,
+                              int64_t capacity, int64_t* state);
+int esacb200_eval_poses(esacb200_ctx* ctx, int B, const float* out_poses, const float* gt_poses, const int64_t* experts,
+                        const int64_t* scenes, const float* hist, int E, const int32_t* status, double* records,
+                        int64_t capacity, int64_t* state);
+
 /* Soft-inlier scores of given poses (getReproErrs + getHypScores, esac_util.h:235-363) without
  * sampling/selection/refinement: poses6 = host double [M][6] (rvec, tvec); out_scores host double [M]. */
 int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,

@@ -193,6 +193,12 @@ def load_library() -> C.CDLL:
     for name in ("eval_poses", "eval_poses_async"):
         getattr(lib, "esacb200_" + name).argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, vp, vp, i64, vp]
         getattr(lib, "esacb200_" + name).restype = i32
+    lib.esacb200_cluster_stats_ragged.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, vp]
+    lib.esacb200_cluster_stats_ragged.restype = i32
+    lib.esacb200_kmeans2.argtypes = [vp, i32, vp, C.c_uint64, i32, i32, i32, f64, vp, vp, vp]
+    lib.esacb200_kmeans2.restype = i32
+    lib.esacb200_cluster_targets.argtypes = [vp, i32, vp, vp, i32, f32, vp, vp, vp]
+    lib.esacb200_cluster_targets.restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
         getattr(lib, "esacb200_" + name).restype = i32
@@ -1761,6 +1767,117 @@ def evaluate_poses(outPoses, gtPoses, experts, gtScenes, hist=None, status=None)
     ctx, B, E, capacity = _eval_context(call, outPoses, gtPoses, experts, gtScenes, hist, status, records, state)
     _eval_call("esacb200_eval_poses", ctx, B, E, capacity, outPoses, gtPoses, experts, gtScenes, hist, status, records, state)
     return records if outPoses.dim() == 3 else records[0]
+
+
+# ------------------------------------------------------------------------------------------------
+# clustering a large environment into experts (cluster_dataset.py:19-140, 219-240; esac_b200/cluster.py drives these)
+# ------------------------------------------------------------------------------------------------
+MAX_CLUSTERS = 1024  # clusters one cluster_targets call handles (include/esac_b200.h)
+
+
+def cluster_statistics(init_maps):
+    """Per-image statistics of ground-truth scene-coordinate maps (cluster_dataset.py:52-58, 121-124): init_maps is one
+    stacked float32 tensor [B,3,H,W] or a list / tuple of B float32 tensors [3,H_b,W_b] (all CPU / numpy or all CUDA).  A
+    cell is valid when the float32 sum (x + y) + z is not 0.  Returns (median float32 [B,3]: torch.median(1)[0] over the
+    valid cells, bitwise; mean float32 [B,3]: their fp64 mean rounded once; count int32 [B]: valid cells; status int32
+    [B]: 0 ok, 1 no valid cell, 2 a non-finite median or mean), on the maps' device (CPU for host maps)."""
+    import torch
+    maps = _Images(init_maps, 3, "init_maps")
+    ctx = _pick_ctx(*maps.devices)
+    dev = torch.device("cuda", maps.devices[0]) if maps.devices[0] is not None else torch.device("cpu")
+    median = torch.empty((maps.B, 3), dtype=torch.float32, device=dev)
+    mean = torch.empty((maps.B, 3), dtype=torch.float32, device=dev)
+    count = torch.empty(maps.B, dtype=torch.int32, device=dev)
+    status = torch.empty(maps.B, dtype=torch.int32, device=dev)
+    ctx.check(ctx.lib.esacb200_cluster_stats_ragged(ctx.handle, maps.B, maps.ptrs, maps.hs, maps.ws, median.data_ptr(),
+                                                    mean.data_ptr(), count.data_ptr(), status.data_ptr()))
+    return median, mean, count, status
+
+
+def _cuda_only(call: str, **tensors):
+    """The last check of a CUDA-only call: every tensor lives on the GPU (after the dtype and shape checks, so that those
+    run without one)."""
+    for what, t in tensors.items():
+        if not t.is_cuda:
+            raise RuntimeError(f"{call} takes CUDA tensors only ({what} is on the CPU)")
+
+
+def kmeans2(points, seed: int, attempts: int = 10, max_iter: int = 100, eps: float = 0.1, split: int = 0):
+    """One 2-means split, the replacement of cv2.kmeans(points, 2, None, (EPS + MAX_ITER, max_iter, eps), attempts,
+    KMEANS_PP_CENTERS) (cluster_dataset.py:65-86) with the repository's own random stream: points a CUDA float32 tensor
+    [n,3] (n >= 2); the draws of attempt a are keyed by (seed, split, a), so the splits of one clustering take distinct
+    `split` values.  Stops after max_iter iterations or once no centre moves more than eps (OpenCV squares eps too).
+    Returns (labels int32 [n] of 0 / 1, centres float32 [2,3], compactness float) of the attempt with the lowest
+    compactness; bitwise repeatable.  The numbering of the two clusters is this implementation's, not cv2's."""
+    call = "kmeans2"
+    if not _is_torch(points):
+        raise RuntimeError(f"{call} takes torch CUDA tensors only (points is a {type(points).__name__})")
+    _check(points, "Float", 2, "points")
+    if int(points.shape[1]) != 3 or not points.is_contiguous():
+        raise RuntimeError(f"{call}: points must be a contiguous [n,3], got {list(points.shape)}")
+    n = int(points.shape[0])
+    if n < 2:
+        raise RuntimeError(f"{call}: {n} points, need at least 2")
+    if not 1 <= int(attempts) <= 4096:
+        raise RuntimeError(f"{call}: attempts={attempts} outside [1, 4096]")
+    if int(max_iter) < 1:
+        raise RuntimeError(f"{call}: max_iter={max_iter}, need at least 1")
+    if not float(eps) >= 0:
+        raise RuntimeError(f"{call}: eps={eps}, need eps >= 0")
+    if int(split) < 0:
+        raise RuntimeError(f"{call}: split={split} must not be negative")
+    _cuda_only(call, points=points)
+    import torch
+    ctx = _pick_ctx(points.device.index)
+    labels = torch.empty(n, dtype=torch.int32, device=points.device)
+    centres = torch.empty((2, 3), dtype=torch.float32, device=points.device)
+    compactness = torch.empty(1, dtype=torch.float64, device=points.device)
+    ctx.check(ctx.lib.esacb200_kmeans2(ctx.handle, n, points.data_ptr(), int(seed) & (2**64 - 1), int(split), int(attempts),
+                                       int(max_iter), float(eps), labels.data_ptr(), centres.data_ptr(),
+                                       compactness.data_ptr()))
+    return labels, centres, float(compactness.item())
+
+
+def cluster_targets(means, labels, K: int, softness: float = 5.0):
+    """The cluster centres, sizes and soft gating targets of a clustering (cluster_dataset.py:104-134, 219-240): means a
+    CUDA float32 tensor [N,3] (the images' mean scene coordinates), labels a CUDA int64 tensor [N] with every label in
+    [0, K) and every cluster non-empty.  Returns (cam_centers float32 [K,3]: the mean of each cluster's image means,
+    cam_sizes float32 [K,1]: their mean squared distance to the centre, gating_probs float32 [N,K]:
+    exp(-d^2 / size / 2 * softness) / sqrt(2 pi size) normalised by its sum + 1e-7, in the reference's float32 op order)."""
+    call = "cluster_targets"
+    for what, t in (("means", means), ("labels", labels)):
+        if not _is_torch(t):
+            raise RuntimeError(f"{call} takes torch CUDA tensors only ({what} is a {type(t).__name__})")
+    _check(means, "Float", 2, "means")
+    _check(labels, "Long", 1, "labels")
+    N = int(means.shape[0])
+    if N < 1 or int(means.shape[1]) != 3 or not means.is_contiguous():
+        raise RuntimeError(f"{call}: means must be a contiguous [N,3] with N >= 1, got {list(means.shape)}")
+    if int(labels.shape[0]) != N or not labels.is_contiguous():
+        raise RuntimeError(f"{call}: labels must be a contiguous [{N}], got {list(labels.shape)}")
+    K = int(K)
+    if not 1 <= K <= MAX_CLUSTERS:
+        raise RuntimeError(f"{call}: K={K} outside [1, {MAX_CLUSTERS}]")
+    if not float(softness) > 0:
+        raise RuntimeError(f"{call}: softness={softness}, need softness > 0")
+    import torch
+    if means.device != labels.device:
+        raise RuntimeError(f"{call}: means and labels live on different devices ({means.device}, {labels.device})")
+    lab = labels.cpu().numpy()
+    outside = np.flatnonzero((lab < 0) | (lab >= K))
+    if len(outside):
+        raise RuntimeError(f"{call}: label {int(lab[outside[0]])} of image {int(outside[0])} outside [0, {K})")
+    empty = np.flatnonzero(np.bincount(lab, minlength=K) == 0)
+    if len(empty):
+        raise RuntimeError(f"{call}: cluster {int(empty[0])} has no image")
+    _cuda_only(call, means=means, labels=labels)
+    ctx = _pick_ctx(means.device.index)
+    centres = torch.empty((K, 3), dtype=torch.float32, device=means.device)
+    sizes = torch.empty((K, 1), dtype=torch.float32, device=means.device)
+    probs = torch.empty((N, K), dtype=torch.float32, device=means.device)
+    ctx.check(ctx.lib.esacb200_cluster_targets(ctx.handle, N, means.data_ptr(), labels.data_ptr(), K, float(softness),
+                                               centres.data_ptr(), sizes.data_ptr(), probs.data_ptr()))
+    return centres, sizes, probs
 
 
 def set_seed(seed: int, device: int | None = None):

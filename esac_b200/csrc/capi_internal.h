@@ -8,6 +8,7 @@
 //   capi_losses.cu      the two expert losses
 //   capi_gate.cu        expert gates and the stream-ordered hypothesis assignment
 //   capi_eval.cu        test-time pose evaluation
+//   capi_cluster.cu     clustering a large environment into experts
 //   capi_testhooks.cu   include/esac_b200_testhooks.h
 #pragma once
 #include <cuda_runtime.h>
@@ -326,6 +327,14 @@ int device_args(esacb200_ctx* ctx, const char* what, int n, const void* const* p
 int begin_async(esacb200_ctx* ctx, bool backward, int B, const Problem& P, const float* coords, const int64_t* assign,
                 int64_t assign_stride, const int32_t* shifts, const float* cameras, int32_t* out_status, int n,
                 const void* const* ptrs, const char* const* names, AsyncCall& call, const char* name = nullptr);
+
+// ---- capi_losses.cu: host images of a ragged call ------------------------------------------------------------------
+size_t pack_offsets(const std::vector<size_t>& bytes, std::vector<size_t>& off);
+int copy_packed(esacb200_ctx* ctx, char* const* host, const std::vector<size_t>& bytes, const std::vector<size_t>& off, char* dev,
+                bool to_device, cudaStream_t stream);
+template <class T>
+int stage_images(esacb200_ctx* ctx, T* const* ptrs, const std::vector<size_t>& bytes, bool device, bool upload, DevBuf& buf,
+                 std::vector<T*>& dev, std::vector<size_t>& off);
 
 // ---- capi_pipeline.cu: batches -----------------------------------------------------------------------------------
 int run_batch(esacb200_ctx* ctx, int B, const int* H, const int* W, bool draws, const std::function<int(esacb200_ctx*, int)>& image);

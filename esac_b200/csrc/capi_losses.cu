@@ -12,7 +12,7 @@
 using namespace esacb200;
 using namespace esacb200::capi;
 
-namespace {
+namespace esacb200::capi {
 
 // Offsets of B host images packed into one device buffer, each at a 16-byte aligned offset (so that an image keeps the
 // 128-bit load path a single-image call would give it).  Returns the total.
@@ -57,6 +57,12 @@ int stage_images(esacb200_ctx* ctx, T* const* ptrs, const std::vector<size_t>& b
     if (upload) return copy_packed(ctx, (char* const*)ptrs, bytes, off, (char*)buf.p, true, ctx->stream);
     return 0;
 }
+template int stage_images<const float>(esacb200_ctx*, const float* const*, const std::vector<size_t>&, bool, bool, DevBuf&,
+                                       std::vector<const float*>&, std::vector<size_t>&);
+
+}  // namespace esacb200::capi
+
+namespace {
 
 // Orders a loss call's per-image records by load path (128-bit first) so that each path is one launch over a contiguous
 // slice of the table; returns the bytes of the table.

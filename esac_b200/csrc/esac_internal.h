@@ -705,4 +705,56 @@ struct EvalArgs {
 // Image b of the call goes to slot state->count + b; the launch's last CTA advances count by B.
 void launch_eval_poses(const EvalArgs& a, cudaStream_t st);
 
+// --- cluster.cu ---------------------------------------------------------------------------
+// Clustering a large environment into experts (cluster_dataset.py:19-140, 219-240).
+struct ClusterMap {
+    const float* p;  // [3,H,W] ground-truth scene coordinates, device memory
+    int H, W;
+};
+// One map's statistics over its valid cells ((x + y) + z != 0 in float32): lower median and mean per coordinate.
+struct ClusterStats {
+    float median[3], mean[3];
+    int count;   // valid cells
+    int status;  // 0 ok, 1 no valid cell, 2 a non-finite median or mean
+};
+static_assert(sizeof(ClusterStats) == 32, "ClusterStats is 32 bytes");
+constexpr int kStatsThreads = 256;
+constexpr int kStatsSmemKeys = 8192;  // valid cells per coordinate selected in shared memory; more: from global memory
+// One CTA per map; `cap` keys per coordinate of dynamic shared memory (3 * cap * 4 bytes).
+void launch_cluster_stats(const ClusterMap* maps, int B, int cap, ClusterStats* out, cudaStream_t st);
+
+// One k-means attempt's result: its fp64 centres, the compactness of its final assignment, and the point its final
+// assignment moved into an emptied cluster (-1: none).
+struct KmeansAttempt {
+    double centre[2][3];
+    double compactness;
+    int reseed, reseed_label;
+};
+struct KmeansArgs {
+    const float* points;  // [n,3]
+    int n, attempts, max_iter;
+    double eps2;          // stop when the largest squared centre shift is <= eps2
+    unsigned long long seed;
+    unsigned split;
+    KmeansAttempt* att;   // [attempts] workspace
+    int* labels;          // [n] the best attempt's labels
+    float* centres;       // [2,3]
+    double* compactness;  // [1]
+};
+constexpr int kKmeansThreads = 256;  // the reduction tree of every k-means sum (oracle/cluster_oracle.py restates it)
+// One CTA per attempt, then one pass that picks the best attempt and writes its labels, centres and compactness.
+void launch_kmeans2(const KmeansArgs& a, cudaStream_t st);
+
+struct ClusterTargetsArgs {
+    const float* means;      // [N,3] image means
+    const long long* labels; // [N] in [0, K), every cluster non-empty
+    int N, K;
+    float softness;
+    float* centres;          // [K,3]
+    float* sizes;            // [K]
+    float* probs;            // [N,K]
+};
+constexpr int kTargetsMaxClusters = 1024;
+void launch_cluster_targets(const ClusterTargetsArgs& a, cudaStream_t st);
+
 }  // namespace esacb200

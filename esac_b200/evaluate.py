@@ -15,6 +15,11 @@ format it as the reference prints and writes it.
 An image whose forward status is not 0, or whose scene lies outside [0, num_scenes), keeps its record but is left out of
 the table and counted in table()["excluded"]: the reference cannot produce such images.  The experts-active figures average
 over the counted images.
+
+A clustered environment (test_esac.py with --clusters, a SyntheticClusterDataset or a clustering of esac_b200.cluster) has
+no ground-truth expert: its images carry scene -1.  PoseEvaluator(..., clustered=True) counts every record with status 0
+in scene 0, whatever its scene, as test_esac.py's cluster mode does: one row, whose class accuracy is 0 since -1 matches
+no expert.  Read it with table(average=False), the cluster mode's console.
 """
 from __future__ import annotations
 
@@ -30,12 +35,13 @@ class PoseEvaluator:
     """Records of up to `capacity` test images of `num_scenes` scenes (the ensemble's experts), on `device` (default: the
     current CUDA device)."""
 
-    def __init__(self, num_scenes: int, capacity: int, device=None):
+    def __init__(self, num_scenes: int, capacity: int, device=None, clustered: bool = False):
         import torch
         if int(num_scenes) < 1 or int(capacity) < 1:
             raise RuntimeError(f"PoseEvaluator needs num_scenes >= 1 and capacity >= 1, got {num_scenes} and {capacity}")
         self.num_scenes = int(num_scenes)
         self.capacity = int(capacity)
+        self.clustered = bool(clustered)
         device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         self.state = torch.zeros(api.EVAL_STATE, dtype=torch.int64, device=device)
         self.buffer = torch.empty((self.capacity, len(api.EVAL_FIELDS)), dtype=torch.float64, device=device)
@@ -61,8 +67,8 @@ class PoseEvaluator:
         """The reference's statistics over the counted records: "rows" (scene, class accuracy, pose accuracy, median
         rotation error in degrees, median translation error in cm), "console" (the lines test_esac.py prints, with the
         Average row when `average`, as for clusters < 0), "results" (the results-file lines), "experts" (the experts-active
-        lines) and "excluded" (records left out)."""
-        return _table(self.records(), self.num_scenes, rot_threshold, trans_threshold, average)
+        lines) and "excluded" (records left out).  When clustered: one row, scene 0, over every record with status 0."""
+        return _table(self.records(), self.num_scenes, rot_threshold, trans_threshold, average, self.clustered)
 
     def pose_lines(self, names) -> list[str]:
         """The pose-file lines, one per record, names[i] being record i's already stripped file name."""
@@ -77,9 +83,14 @@ def _upper_median(values: np.ndarray) -> float:
     return float(np.sort(values)[len(values) // 2]) if len(values) else 0
 
 
-def _table(recs: np.ndarray, num_scenes: int, rot_threshold, trans_threshold, average: bool) -> dict:
+def _table(recs: np.ndarray, num_scenes: int, rot_threshold, trans_threshold, average: bool, clustered: bool = False) -> dict:
     scene = recs[:, _SCENE]
-    counted = (recs[:, _STATUS] == 0) & (scene >= 0) & (scene < num_scenes)
+    if clustered:
+        counted = recs[:, _STATUS] == 0
+        scene = np.where(counted, 0.0, scene)
+        num_scenes = 1
+    else:
+        counted = (recs[:, _STATUS] == 0) & (scene >= 0) & (scene < num_scenes)
     rows, console, results = [], ["Scene - Class.Acc. - Pose.Acc. - Median Rot. - Median Trans.", _RULE], []
     for s in range(num_scenes):
         r = recs[counted & (scene == s)]

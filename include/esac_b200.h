@@ -549,6 +549,37 @@ int esacb200_eval_poses(esacb200_ctx* ctx, int B, const float* out_poses, const 
                         const int64_t* scenes, const float* hist, int E, const int32_t* status, double* records,
                         int64_t capacity, int64_t* state);
 
+/* Clustering a large environment into experts (cluster_dataset.py:19-140, 219-240).  Each call checks every argument
+ * before it enqueues anything (ESACB200_ERR_ARG) and returns after its work is done.
+ *
+ * esacb200_cluster_stats_ragged: the statistics of B >= 1 ground-truth maps, map b float32 [3, H[b], W[b]] at maps[b]
+ * (all device or all host pointers; 1 <= H*W <= 2^30).  A cell is valid when the float32 sum (x + y) + z is not 0.  Per map:
+ * out_median[b*3 + c] torch's lower median of coordinate c over the valid cells (sorted[(n-1)/2], the first NaN when there
+ * is one; -0 sorts before +0), out_mean[b*3 + c] the fp64 mean of the valid cells rounded to
+ * float32, out_count[b] the valid cells and out_status[b]: 0 ok, 1 no valid cell (median and mean NaN), 2 a non-finite
+ * median or mean.  Outputs may be host or device memory.
+ *
+ * esacb200_kmeans2: cv2.kmeans(points, 2, None, (EPS + MAX_ITER, max_iter, eps), attempts, KMEANS_PP_CENTERS) on n >= 2
+ * points (device float32 [n,3]), with its own random stream: draw d of attempt a is mix64-keyed by (seed, split, a, d).  Per
+ * attempt (one CTA each, all in one launch): k-means++ seeding with 3 trials, then Lloyd iterations (nearer centre, centre
+ * 0 on a tie; a cluster left empty takes the point farthest from the other centre, lowest index on a tie) until max_iter
+ * >= 1 iterations or the largest squared centre shift <= eps^2 (eps >= 0).  The attempt with the lowest compactness (fp64
+ * sum of squared distances; lowest attempt on a tie) writes out_labels (device int32 [n], 0 / 1), out_centres (device
+ * float32 [2,3]) and out_compactness (device double [1]).  1 <= attempts <= 4096, split >= 0.  Every sum has a fixed
+ * order: two calls with the same arguments agree bitwise.
+ *
+ * esacb200_cluster_targets: for N >= 1 images with means (device float32 [N,3]) and labels (device int64 [N], each in
+ * [0, K), every cluster non-empty; 1 <= K <= 1024): out_centres (device float32 [K,3]) the fp64 mean of each cluster's
+ * image means, out_sizes (device float32 [K]) the fp64 mean squared distance of those means to the float32 centre, and
+ * out_probs (device float32 [N,K]) the soft gating targets in the reference's float32 op order:
+ * exp(-|m_i - c_k|^2 / size_k / 2 * softness) / sqrt(2 pi size_k), normalised by their sum + 1e-7 (softness > 0). */
+int esacb200_cluster_stats_ragged(esacb200_ctx* ctx, int B, const float* const* maps, const int* H, const int* W,
+                                  float* out_median, float* out_mean, int32_t* out_count, int32_t* out_status);
+int esacb200_kmeans2(esacb200_ctx* ctx, int n, const float* points, uint64_t seed, int split, int attempts, int max_iter,
+                     double eps, int32_t* out_labels, float* out_centres, double* out_compactness);
+int esacb200_cluster_targets(esacb200_ctx* ctx, int N, const float* means, const int64_t* labels, int K, float softness,
+                             float* out_centres, float* out_sizes, float* out_probs);
+
 /* Soft-inlier scores of given poses (getReproErrs + getHypScores, esac_util.h:235-363) without
  * sampling/selection/refinement: poses6 = host double [M][6] (rvec, tvec); out_scores host double [M]. */
 int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,

@@ -1,5 +1,6 @@
 // The context of libesac_b200.so's C ABI (include/esac_b200.h): its lifecycle, options and getters, and the frame every entry
 // point shares -- the error message, the stage timers and the last-call record.
+#include <climits>
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdio.h>
@@ -204,10 +205,17 @@ int esacb200_inject_cells(esacb200_ctx* ctx, const int32_t* cells, int M, int T)
     if (!cells) { ctx->inj_M = ctx->inj_T = 0; return ESACB200_OK; }
     if (M <= 0 || T <= 0) return fail(ctx, ESACB200_ERR_ARG, "inject_cells: M and T must be positive");
     size_t bytes = (size_t)M * T * 8 * 4;
+    int lo[2] = {INT_MAX, INT_MAX}, hi[2] = {INT_MIN, INT_MIN};
+    for (size_t i = 0; i < (size_t)M * T * 8; ++i) {
+        const int c = (int)(i & 1);
+        lo[c] = cells[i] < lo[c] ? cells[i] : lo[c];
+        hi[c] = cells[i] > hi[c] ? cells[i] : hi[c];
+    }
     CK(ctx->inject.ensure(bytes));
     CK(cudaMemcpy(ctx->inject.p, cells, bytes, cudaMemcpyHostToDevice));
     ctx->inj_M = M;
     ctx->inj_T = T;
+    for (int c = 0; c < 2; ++c) { ctx->inj_lo[c] = lo[c]; ctx->inj_hi[c] = hi[c]; }
     return ESACB200_OK;
 } ESAC_ABI_CATCH(ctx)
 

@@ -123,6 +123,7 @@ struct esacb200_ctx {
         contrib8, upstream;
     esacb200::capi::Pinned* pin = nullptr;
     int inj_M = 0, inj_T = 0;
+    int inj_lo[2] = {0, 0}, inj_hi[2] = {0, 0};  // smallest and largest injected x, y: checked against each call's map
     cudaEvent_t ev[esacb200::capi::EV_COUNT] = {nullptr};
     bool ev_used[esacb200::capi::EV_COUNT] = {false};
     esacb200_stats st;

@@ -48,6 +48,11 @@ int fill_problem(esacb200_ctx* ctx, Problem& P, int E, int H, int W, int M, int 
         return fail(ctx, ESACB200_ERR_ARG, "map %dx%d too small to draw 4 distinct cells from [0,W-2]x[0,H-2]", W, H);
     if (draw == DRAWS_INJECTED && ctx->inj_M && ctx->inj_M != M)
         return fail(ctx, ESACB200_ERR_ARG, "injected cells are for M=%d, call has M=%d", ctx->inj_M, M);
+    // the sampling kernels gather coords[cy * W + cx] of every injected cell unchecked
+    if (draw == DRAWS_INJECTED && ctx->inj_M &&
+        (ctx->inj_lo[0] < 0 || ctx->inj_lo[1] < 0 || ctx->inj_hi[0] > W - 1 || ctx->inj_hi[1] > H - 1))
+        return fail(ctx, ESACB200_ERR_ARG, "injected cells span x %d..%d, y %d..%d: outside the %dx%d map", ctx->inj_lo[0],
+                    ctx->inj_hi[0], ctx->inj_lo[1], ctx->inj_hi[1], W, H);
     P.E = E; P.H = H; P.W = W; P.N = H * W; P.M = M;
     P.shiftX = shiftX; P.shiftY = shiftY; P.sub = sub;
     P.f = f; P.ppx = ppx; P.ppy = ppy; P.tau = tau; P.alpha = alpha; P.beta = beta; P.max_reproj = maxReproj;

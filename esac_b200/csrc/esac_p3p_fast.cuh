@@ -9,7 +9,9 @@
 // The code is written over a value pack (Pack1: one try per thread; a pack of two tries side by side in a float2 paid
 // on Blackwell's packed fp32x2 pipe and was measured slower on the H100, which has none).  Every decision that is
 // numerically borderline returns "may pass", i.e. hands the try to the exact fp64 path; the invariant "an accepted try
-// is never rejected here" is what tests/test_host_geom.py::test_float_prefilter_never_rejects_an_accepted_try checks.
+// is never rejected here" is what tests/test_host_geom.py::test_float_prefilter_never_rejects_an_accepted_try checks on
+// random draws, and tests/test_host_minimal_sets.py (host compile) and tests/test_gpu_minimal_sets.py (device compile)
+// on crafted ill-conditioned sets.
 #pragma once
 #include "esac_geom.cuh"
 
@@ -97,7 +99,13 @@ ESAC_HD void fast_line_conic(P l0, P l1, P l2, P d00, P d01, P d02, P d11, P d12
     const P C = Djj - two * s * Djk + s * s * Dkk;
     P disc = B * B - A * C;
     const P mag = B * B + abs_(A * C);
-    unc = unc | !lk_ok | (lk_ok & lt_(abs_(disc), bc<P>(N::kUncertain) * mag));
+    // A, B and C themselves come out of cancelling sums (near the danger cylinder C << its terms), and the line carries
+    // the error of the cubic's float root: the sign of disc is only known beyond the error those terms propagate into it
+    const P sA = abs_(Dii) + two * abs_(r * Dik) + r * r * abs_(Dkk);
+    const P sB = abs_(Dij) + abs_(s * Dik) + abs_(r * Djk) + abs_(r * s * Dkk);
+    const P sC = abs_(Djj) + two * abs_(s * Djk) + s * s * abs_(Dkk);
+    const P derr = two * abs_(B) * sB + abs_(A) * sC + abs_(C) * sA;
+    unc = unc | !lk_ok | (lk_ok & lt_(abs_(disc), bc<P>(N::kUncertain) * (mag + derr)));
     const M real = !lt_(disc, -(bc<P>(N::kDiscTol) * mag));
     disc = max_(disc, zero);
     const P sq = sqrt_(disc);
@@ -121,7 +129,11 @@ ESAC_HD void fast_line_conic(P l0, P l1, P l2, P d00, P d01, P d02, P d11, P d12
     }
 }
 
-constexpr float kPrefilterMargin = 2.f;    // 4th-point error band, in units of tau, inside which the exact path decides (MC: no false reject down to 1.5)
+// 4th-point error band, in units of tau, inside which the exact path decides.  It covers the float error of a
+// well-conditioned P3P only: near the danger cylinder a float root can miss the 4th point by many tau (no margin up to
+// 16 tau was enough there), so those tries are sent to the exact path by the uncertainty latches above and below instead
+// (tests/test_host_minimal_sets.py).
+constexpr float kPrefilterMargin = 2.f;
 constexpr float kPrefilterNeedle = 0.02f;  // shortest / longest squared side below which the triangle goes to the exact path
 
 // obj[i][c] / img[i][c]: point i, coordinate c, of the W tries of the pack.  Returns, per try, false only when the try
@@ -204,6 +216,11 @@ ESAC_HD typename MaskOf<P>::type p3p_may_pass_pack(const P obj[4][3], const P im
         g = g - sel(gt_(abs_(dv), zero), fv * rcp_(dv), zero);
     }
     ESAC_LATCH(nan_(g), yes)
+    {   // a near-multiple root (two base points of the pencil close together: the danger cylinder) is only known to
+        // ~sqrt(eps) in float, and so are the lines built from it: exact path
+        const P dv = (three * g + two * a) * g + b, ag = abs_(g);
+        ESAC_LATCH(lt_(abs_(dv), bc<P>(1e-3f) * ((three * ag + two * abs_(a)) * ag + abs_(b))), yes)
+    }
     // ---- degenerate member D0 and the other conic -------------------------------------------------------------
     const M small = le_(abs_(g), one);
     const P w1 = sel(small, one, rcp_(g)), w2 = sel(small, g, one);

@@ -139,6 +139,23 @@ def test_injected_cells_of_another_m(api, sc):
         (ERR_ARG, f"injected cells are for M=3, call has M={M}")
 
 
+@pytest.mark.parametrize("bad", [(W, 0), (0, H), (-1, 0), (0, -1)])
+def test_injected_cells_outside_the_map(api, sc, bad):
+    """The sampling kernels read coords at every injected cell unchecked: a set with one cell outside [0,W-1]x[0,H-1] is
+    refused before anything launches, on every entry point that draws injected cells."""
+    cells = np.zeros((M, 1, 4, 2), np.int32)
+    cells[:, 0] = [[0, 0], [W - 1, 0], [0, H - 1], [W - 1, H - 1]]
+    cells[M // 2, 0, 3] = bad
+    api.context().inject_cells(cells)
+    xs, ys = cells[..., 0], cells[..., 1]
+    msg = f"injected cells span x {xs.min()}..{xs.max()}, y {ys.min()}..{ys.max()}: outside the {W}x{H} map"
+    for name in ("forward", "backward"):
+        assert _call(api, name, *_single(sc, True, E, H, W, M)[name]) == (ERR_ARG, msg), name
+    tape = np.zeros(64, np.uint8)
+    assert _call(api, "hypotheses_forward", _ptr(sc.coords), E, H, W, _ptr(sc.assign), 1, M, *sc.params, _ptr(tape), 64,
+                 _ptr(np.zeros(M)), _ptr(np.zeros((M, 6))), _ptr(np.zeros(M, np.uint8))) == (ERR_ARG, msg)
+
+
 def _ragged(sc, hs, ws, tapes=None, tape_bytes=None):
     """The argument lists of the ragged entry points for len(hs) images (host arrays, never read by a failing check)."""
     B = len(hs)

@@ -199,6 +199,8 @@ def load_library() -> C.CDLL:
     lib.esacb200_kmeans2.restype = i32
     lib.esacb200_cluster_targets.argtypes = [vp, i32, vp, vp, i32, f32, vp, vp, vp]
     lib.esacb200_cluster_targets.restype = i32
+    lib.esacb200_render_init_maps.argtypes = [vp, i32, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.esacb200_render_init_maps.restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
         getattr(lib, "esacb200_" + name).restype = i32
@@ -1878,6 +1880,109 @@ def cluster_targets(means, labels, K: int, softness: float = 5.0):
     ctx.check(ctx.lib.esacb200_cluster_targets(ctx.handle, N, means.data_ptr(), labels.data_ptr(), K, float(softness),
                                                centres.data_ptr(), sizes.data_ptr(), probs.data_ptr()))
     return centres, sizes, probs
+
+
+# ------------------------------------------------------------------------------------------------
+# ground-truth maps from an SfM reconstruction (setup_aachen.py:184-202, setup_dubrovnik.py:171-190; esac_b200/prepare.py
+# reads the reconstructions and writes the files)
+# ------------------------------------------------------------------------------------------------
+RENDER_MAX_SIDE = 8192           # out map side (include/esac_b200.h: ESACB200_RENDER_MAX_SIDE)
+RENDER_MAX_CELLS = 1 << 30       # cells of all maps of one call
+RENDER_MAX_OBS = 2**31 - 256     # observations, and points, of one call
+RENDER_STATUS = {1: "a point index out of range", 2: "a NaN projection"}
+
+
+def _host_values(t) -> np.ndarray:
+    if _is_torch(t):
+        t = t.detach().cpu().numpy()
+    return np.asarray(t)
+
+
+def render_init_maps(points, offsets, indices, poses, focal, out_scale, out_shapes, zbuffer: bool = False):
+    """Renders the ground-truth scene-coordinate maps of C cameras from an SfM reconstruction, as the z-buffer loop of
+    setup_aachen.py / setup_dubrovnik.py does, on the GPU.
+
+    points float32 [P,3]; offsets integer [C+1] (0, non-decreasing, ending at V): camera c's observations are
+    indices[offsets[c]:offsets[c+1]], int32 point indices in reconstruction file order; poses float32 [C,4,4] or [C,3,4]
+    (world -> camera; only rows 0-2 are used); focal and out_scale (out width / image width) C numbers, rounded to float32;
+    out_shapes C pairs (h, w), each side in [1, RENDER_MAX_SIDE].  points and indices may be host (numpy / CPU torch) or
+    CUDA tensors; the other arguments are read on the host.
+
+    Each projection runs in float32 in one stated order (include/esac_b200.h); off-image points and points behind the
+    camera are clamped onto the border and take part in the z-test, as in the reference.  Returns (maps: C float32 views
+    [3,h,w] of one CUDA buffer, counts: int32 CPU tensor [C] of the cells written, zbufs: C float32 views [h,w] or None
+    unless zbuffer).  Raises RuntimeError naming the cameras with an observation whose point index is out of range or
+    whose projection is NaN (cam.z = 0 with cam.x or cam.y = 0: the reference's int(nan)).  Argument errors raise before
+    any context exists."""
+    call = "render_init_maps"
+    _check(points, "Float", 2, "points")
+    if int(points.shape[1]) != 3:
+        raise RuntimeError(f"{call}: points must be [P,3], got {list(points.shape)}")
+    _check(indices, "Int", 1, "indices")
+    _check(poses, "Float", 3, "poses")
+    offs = _host_values(offsets)
+    if offs.ndim != 1 or not np.issubdtype(offs.dtype, np.integer):
+        raise RuntimeError(f"{call}: offsets must be a 1-d integer array, got {offs.dtype} of shape {list(offs.shape)}")
+    C = int(offs.shape[0]) - 1
+    if C < 1:
+        raise RuntimeError(f"{call}: {C} cameras, need at least 1 (offsets holds C+1 values)")
+    offs = offs.astype(np.int64)
+    P, V = int(points.shape[0]), int(indices.shape[0])
+    if offs[0] != 0:
+        raise RuntimeError(f"{call}: offsets[0]={int(offs[0])}, need 0")
+    dec = np.flatnonzero(np.diff(offs) < 0)
+    if len(dec):
+        raise RuntimeError(f"{call}: offsets decrease at camera {int(dec[0])}")
+    if int(offs[-1]) != V:
+        raise RuntimeError(f"{call}: offsets end at {int(offs[-1])}, but indices holds {V} observations")
+    if V > RENDER_MAX_OBS or P > RENDER_MAX_OBS:
+        raise RuntimeError(f"{call}: {V} observations and {P} points, at most {RENDER_MAX_OBS} each")
+    if tuple(int(v) for v in poses.shape[1:]) not in ((4, 4), (3, 4)) or int(poses.shape[0]) != C:
+        raise RuntimeError(f"{call}: poses must be [{C},4,4] or [{C},3,4], got {list(poses.shape)}")
+    f = _per_image(focal, C, np.float32, "focal")
+    s = _per_image(out_scale, C, np.float32, "out_scale")
+    shp = _host_values(out_shapes)
+    if shp.shape != (C, 2) or not np.issubdtype(shp.dtype, np.integer):
+        raise RuntimeError(f"{call}: out_shapes must be {C} integer pairs (h, w), got {shp.dtype} of shape {list(shp.shape)}")
+    shp = shp.astype(np.int64)
+    off_side = np.flatnonzero((shp < 1).any(1) | (shp > RENDER_MAX_SIDE).any(1))
+    if len(off_side):
+        c = int(off_side[0])
+        raise RuntimeError(f"{call}: camera {c} map is {int(shp[c, 0])}x{int(shp[c, 1])}, need sides in [1, {RENDER_MAX_SIDE}]")
+    cells = shp[:, 0] * shp[:, 1]
+    if int(cells.sum()) > RENDER_MAX_CELLS:
+        raise RuntimeError(f"{call}: the maps hold {int(cells.sum())} cells, more than {RENDER_MAX_CELLS}")
+    devs = {t.device.index for t in (points, indices) if _is_torch(t) and t.is_cuda}
+    if len(devs) > 1:
+        raise RuntimeError(f"{call}: points and indices live on different CUDA devices {sorted(devs)}")
+    pose34 = np.ascontiguousarray(_host_values(poses)[:, :3, :], np.float32)
+    pts, idx = _Arg(points), _Arg(indices)
+    import torch
+    # Always on torch's current stream of the target device, also for host inputs: the outputs come from torch's caching
+    # allocator, which may hand out a block that queued torch work on that stream still writes.
+    ctx = _pick_ctx(*devs) if devs else _pick_ctx(torch.cuda.current_device() if torch.cuda.is_available() else None)
+    dev = torch.device("cuda", ctx.device)
+    buf = torch.empty(int(3 * cells.sum()), dtype=torch.float32, device=dev)
+    zb = torch.empty(int(cells.sum()), dtype=torch.float32, device=dev) if zbuffer else None
+    count = np.zeros(C, np.int32)
+    status = np.zeros(C, np.int32)
+    H = np.ascontiguousarray(shp[:, 0], np.int32)
+    W = np.ascontiguousarray(shp[:, 1], np.int32)
+    ctx.check(ctx.lib.esacb200_render_init_maps(
+        ctx.handle, C, pts.ptr if P else None, P, offs.ctypes.data, idx.ptr if V else None, pose34.ctypes.data,
+        f.ctypes.data, s.ctypes.data, H.ctypes.data, W.ctypes.data, buf.data_ptr(),
+        zb.data_ptr() if zb is not None else None, count.ctypes.data, status.ctypes.data))
+    bad = np.flatnonzero(status)
+    if len(bad):
+        listed = ", ".join(f"{int(c)} (" + " and ".join(m for b, m in RENDER_STATUS.items() if status[c] & b) + ")"
+                           for c in bad[:10])
+        raise RuntimeError(f"{call}: {len(bad)} camera(s) cannot be rendered: {listed}" + (", ..." if len(bad) > 10 else ""))
+    starts = np.concatenate([[0], np.cumsum(cells)])
+    maps = [buf[3 * int(starts[c]):3 * int(starts[c + 1])].view(3, int(shp[c, 0]), int(shp[c, 1])) for c in range(C)]
+    zbufs = None
+    if zb is not None:
+        zbufs = [zb[int(starts[c]):int(starts[c + 1])].view(int(shp[c, 0]), int(shp[c, 1])) for c in range(C)]
+    return maps, torch.from_numpy(count), zbufs
 
 
 def set_seed(seed: int, device: int | None = None):

@@ -16,9 +16,9 @@ HERE = Path(__file__).resolve().parent
 CSRC = HERE / "csrc"
 OBJ = HERE / "_obj"
 LIB = HERE / "libesac_b200.so"
-SOURCES = ["score.cu", "hyp.cu", "refine.cu", "bwd.cu", "gating.cu", "gate.cu", "reproj.cu", "coord_loss.cu", "loss_async.cu", "eval.cu", "cluster.cu",
+SOURCES = ["score.cu", "hyp.cu", "refine.cu", "bwd.cu", "gating.cu", "gate.cu", "reproj.cu", "coord_loss.cu", "loss_async.cu", "eval.cu", "cluster.cu", "render.cu",
            "capi.cu", "capi_pipeline.cu", "capi_esac.cu", "capi_hypotheses.cu", "capi_losses.cu", "capi_gate.cu",
-           "capi_eval.cu", "capi_cluster.cu", "capi_testhooks.cu"]
+           "capi_eval.cu", "capi_cluster.cu", "capi_render.cu", "capi_testhooks.cu"]
 HEADERS = ["esac_internal.h", "capi_internal.h", "esac_geom.cuh", "esac_rng.cuh", "esac_p3p_fast.cuh", "refine_body.inc", "bwd_assemble_body.inc",
            "../../include/esac_b200.h", "../../include/esac_b200_testhooks.h"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -9,6 +9,7 @@
 //   capi_gate.cu        expert gates and the stream-ordered hypothesis assignment
 //   capi_eval.cu        test-time pose evaluation
 //   capi_cluster.cu     clustering a large environment into experts
+//   capi_render.cu      rendering ground-truth maps from an SfM reconstruction
 //   capi_testhooks.cu   include/esac_b200_testhooks.h
 #pragma once
 #include <cuda_runtime.h>

@@ -757,4 +757,38 @@ struct ClusterTargetsArgs {
 constexpr int kTargetsMaxClusters = 1024;
 void launch_cluster_targets(const ClusterTargetsArgs& a, cudaStream_t st);
 
+// --- render.cu ----------------------------------------------------------------------------
+// Ground-truth scene-coordinate maps from an SfM reconstruction (setup_aachen.py:184-202, setup_dubrovnik.py:171-190).
+struct RenderCamera {
+    float pose[12];        // world -> camera, rows 0-2 of the 4x4, row-major
+    float f, scale;        // focal length and out_w / image width, as float32
+    float half_w, half_h;  // w / 2, h / 2 of the out map
+    int H, W;
+    int cell0;             // first cell of this camera in the packed cell numbering (cells of camera c: [cell0, cell0 + H*W))
+    int pad;
+};
+static_assert(sizeof(RenderCamera) == 80, "RenderCamera is 80 bytes");
+// Per-camera status bits.
+enum { kRenderBadIndex = 1, kRenderNaN = 2 };
+struct RenderArgs {
+    const float* points;     // [P,3]
+    const int* indices;      // [V] point of each observation; camera c owns [offsets[c], offsets[c+1])
+    const int* offsets;      // [C+1]
+    const RenderCamera* cams;  // [C]
+    int C, P, V, cells;      // cells: the sum of H*W over the cameras
+    // workspace
+    int* obs_cell;           // [V] the cell of each observation, -1 when it takes no part
+    float* obs_z;            // [V] its camera-space depth
+    unsigned* first_neg;     // [cells] first observation with a negative depth (0xFFFFFFFF: none)
+    int* last_zero;          // [cells] last observation with depth +-0 before first_neg (-1: none)
+    unsigned long long* key; // [cells] min of (order-preserving depth << 32 | observation) after last_zero
+    // outputs
+    float* maps;             // camera c: [3,H,W] at 3 * cell0
+    float* zbuf;             // camera c: [H,W] at cell0 (may be null)
+    int* count;              // [C] cells written
+    int* status;             // [C] kRender* bits
+};
+// Clears the per-cell workspace and the counters, then the four passes; the caller synchronises.
+void launch_render(const RenderArgs& a, cudaStream_t st);
+
 }  // namespace esacb200

@@ -135,3 +135,46 @@ def pose_error(T_est: np.ndarray, T_gt: np.ndarray) -> tuple[float, float]:
     sin = 0.5 * np.linalg.norm([Rd[2, 1] - Rd[1, 2], Rd[0, 2] - Rd[2, 0], Rd[1, 0] - Rd[0, 1]])
     cos = (np.trace(Rd) - 1) / 2
     return float(np.degrees(np.arctan2(sin, cos))), float(np.linalg.norm(T_est[:3, 3] - T_gt[:3, 3]))
+
+
+# Image sizes of a synthetic Aachen-like reconstruction, cycled over the cameras: 60x80, 80x60 and 60x107 out maps.
+RECON_IMAGE_SIZES = ((480, 640), (640, 480), (480, 854))
+
+
+def make_reconstruction(seed: int = 0, cameras: int = 4000, points: int = 1_500_000, observers: tuple = (2, 10)) -> dict:
+    """A deterministic SfM-like reconstruction in the form prepare.read_nvm returns (esac_b200.prepare.Reconstruction
+    fields, kind "aachen"): cameras along a wandering path, each point made in front of a home camera (mostly on the image,
+    a few off it or behind) and observed by it and the next observers[0] .. observers[1] - 1 cameras, so that cells fill
+    as in a real reconstruction.  The CSR lists each camera's points in point order.  Also returns the image sizes."""
+    from .prepare import Reconstruction, camera_geometry
+    rng = np.random.default_rng(seed)
+    C, P = int(cameras), int(points)
+    yaw = np.cumsum(rng.normal(0, 0.05, C))
+    centre = np.cumsum(np.stack([np.cos(yaw), np.zeros(C), np.sin(yaw)], 1) * 0.5, 0) + rng.normal(0, 0.05, (C, 3))
+    poses = np.zeros((C, 4, 4))
+    for c in range(C):
+        R = rodrigues([rng.normal(0, 0.05), yaw[c], rng.normal(0, 0.05)])
+        poses[c, :3, :3] = R
+        poses[c, :3, 3] = -R @ centre[c]
+        poses[c, 3, 3] = 1
+    sizes = [RECON_IMAGE_SIZES[c % len(RECON_IMAGE_SIZES)] for c in range(C)]
+    focal = np.array([rng.uniform(0.8, 1.2) * max(s) for s in sizes])
+    geo = [camera_geometry("aachen", h, w) for h, w in sizes]
+    home = rng.integers(0, C, P)
+    hw = np.array(sizes, np.float64)[home]
+    u = rng.uniform(-0.1, 1.1, P) * hw[:, 1] - hw[:, 1] / 2
+    v = rng.uniform(-0.1, 1.1, P) * hw[:, 0] - hw[:, 0] / 2
+    d = rng.uniform(2, 60, P) * np.where(rng.random(P) < 0.01, -1, 1)
+    cam = np.stack([u / focal[home] * d, v / focal[home] * d, d], 1)
+    R, t = poses[home, :3, :3], poses[home, :3, 3]
+    world = np.einsum("pji,pj->pi", R, cam - t).astype(np.float32)
+    k = rng.integers(observers[0], observers[1], P)
+    pt = np.repeat(np.arange(P), k)
+    step = np.arange(len(pt)) - np.repeat(np.cumsum(k) - k, k)
+    cam_of = (home[pt] + step) % C
+    order = np.argsort(cam_of, kind="stable")
+    offsets = np.concatenate([[0], np.cumsum(np.bincount(cam_of, minlength=C))]).astype(np.int64)
+    rec = Reconstruction("aachen", [f"db_{c}.jpg" for c in range(C)], [f"db/{c}.jpg" for c in range(C)], world, offsets,
+                         pt[order].astype(np.int32), poses.astype(np.float32), focal)
+    return {"rec": rec, "sizes": sizes, "out_scale": np.array([g[2] for g in geo]),
+            "shapes": [(g[0], g[1]) for g in geo]}

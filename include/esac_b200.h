@@ -580,6 +580,35 @@ int esacb200_kmeans2(esacb200_ctx* ctx, int n, const float* points, uint64_t see
 int esacb200_cluster_targets(esacb200_ctx* ctx, int N, const float* means, const int64_t* labels, int K, float softness,
                              float* out_centres, float* out_sizes, float* out_probs);
 
+/* Rendering ground-truth scene-coordinate maps from an SfM reconstruction (setup_aachen.py:184-202,
+ * setup_dubrovnik.py:171-190).  The call checks every argument before it enqueues anything (ESACB200_ERR_ARG) and returns
+ * after its work is done.
+ *
+ * esacb200_render_init_maps: C >= 1 cameras; camera c owns the observations offsets[c] .. offsets[c+1] - 1 (host int64
+ * [C+1], offsets[0] = 0, non-decreasing, V = offsets[C] <= ESACB200_RENDER_MAX_OBS), in reconstruction file order;
+ * observation v sees point indices[v] (int32 [V]) of points (float32 [P,3], 0 <= P <= ESACB200_RENDER_MAX_OBS); both host or
+ * device memory; indices may be null when V = 0, points when P = 0.  Per camera (host arrays): poses[c*12 ..] rows 0-2 of the float32 world -> camera
+ * pose, focal[c], out_scale[c] (out width / image width) and the out map's H[c] x W[c], each side in
+ * [1, ESACB200_RENDER_MAX_SIDE], ESACB200_RENDER_MAX_CELLS cells in all.  Each observation projects in float32 with
+ * round-to-nearest and no contraction: cam = ((r0 x + r1 y) + r2 z) + r3 per row, u = ((cam.x f) / cam.z) s + W/2,
+ * v = ((cam.y f) / cam.z) s + H/2, cell (int(clamp(v, 0, H-1)), int(clamp(u, 0, W-1))), so off-image points and points behind
+ * the camera land on the border.  A cell keeps what the serial test `zbuf == 0 or zbuf > cam.z` over its observations in
+ * file order keeps: the nearest depth (the earliest on equal depths) after the cell's last written depth-+-0 point, else that
+ * point, else nothing; a depth-0 point is written unless a negative depth came before it in the cell.  Out: camera c's map float32 [3,H[c],W[c]] at out_maps + 3 * (cells of cameras 0..c-1), all-zero where
+ * nothing was written (device memory); optionally its z-buffer float32 [H[c],W[c]] at out_zbuf + (cells of cameras 0..c-1)
+ * (device memory or null); out_count[c] the cells written and out_status[c] (host or device memory): bit 1 an observation
+ * with a point index outside [0, P), bit 2 a NaN projection (cam.z = 0 with cam.x or cam.y = 0); such observations take no
+ * part.  The result does not depend on the order of the device's atomics: two calls agree bitwise.  The call allocates
+ * its workspace (16 bytes per cell, 8 per observation, plus a device copy of host points and indices) and frees it
+ * before it returns, so the context keeps none of it. */
+#define ESACB200_RENDER_MAX_SIDE 8192
+#define ESACB200_RENDER_MAX_CELLS (1 << 30)
+#define ESACB200_RENDER_MAX_OBS 2147483392 /* 2^31 - 256 */
+int esacb200_render_init_maps(esacb200_ctx* ctx, int C, const float* points, int64_t P, const int64_t* offsets,
+                              const int32_t* indices, const float* poses, const float* focal, const float* out_scale,
+                              const int32_t* H, const int32_t* W, float* out_maps, float* out_zbuf, int32_t* out_count,
+                              int32_t* out_status);
+
 /* Soft-inlier scores of given poses (getReproErrs + getHypScores, esac_util.h:235-363) without
  * sampling/selection/refinement: poses6 = host double [M][6] (rvec, tvec); out_scores host double [M]. */
 int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,

@@ -201,6 +201,9 @@ def load_library() -> C.CDLL:
     lib.esacb200_cluster_targets.restype = i32
     lib.esacb200_render_init_maps.argtypes = [vp, i32, vp, i64, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
     lib.esacb200_render_init_maps.restype = i32
+    lib.esacb200_data_step_async.argtypes = [vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, i32, vp, vp, vp, i64,
+                                             vp, i32, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    lib.esacb200_data_step_async.restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
         getattr(lib, "esacb200_" + name).restype = i32
@@ -1984,6 +1987,121 @@ def render_init_maps(points, offsets, indices, poses, focal, out_scale, out_shap
         zbufs = [zb[int(starts[c]):int(starts[c + 1])].view(int(shp[c, 0]), int(shp[c, 1])) for c in range(C)]
     return maps, torch.from_numpy(count), zbufs
 
+
+
+# ------------------------------------------------------------------------------------------------
+# one step of a device-resident image set (esac_b200/data.py: DeviceImageSet drives this)
+# ------------------------------------------------------------------------------------------------
+# The records include/esac_b200.h names, as numpy dtypes: a plan row, an image of the set, the set's device state.
+DATA_ROW = np.dtype([("image", "<i4"), ("padX", "<i4"), ("padY", "<i4"), ("n_ops", "<i4"), ("ops", "<i4", (3,)),
+                     ("factors", "<f4", (3,))])
+DATA_IMAGE = np.dtype([("pixels", "<i8"), ("gt", "<i8"), ("focal", "<f8"), ("scene", "<i8"), ("pose", "<f4", (16,)),
+                       ("group", "<i4"), ("H", "<i4"), ("W", "<i4"), ("gt_h", "<i4"), ("gt_w", "<i4"), ("unused", "<i4")])
+DATA_STATE = 2   # int64 words: the next plan row, the rows the plan holds
+DATA_BRIGHTNESS, DATA_CONTRAST, DATA_SATURATION = 0, 1, 2
+DATA_MAX_ATTACH, DATA_MAX_SIDE, DATA_MAX_BATCH = 8, 8192, 4096
+assert DATA_ROW.itemsize == 40 and DATA_IMAGE.itemsize == 120
+
+
+def _storage_kind(t, what: str, call: str):
+    """Set storage lives on a CUDA device or in pinned host memory (which the kernels read through its device alias)."""
+    if not (t.is_cuda or t.is_pinned()):
+        raise RuntimeError(f"{call}: {what} must be a CUDA tensor or a pinned CPU tensor")
+
+
+def data_step_async(pixels, images, plan, state, group, mean, std, work, outImage, outShifts, outCameras, outPoses,
+                    outScenes, outIndices, outStatus, gt=None, outCoords=None, attachments=(), outAttachments=()):
+    """One step of B images of shape group `group` of a device-resident image set, enqueued on torch's current stream with
+    no host synchronisation, so that a CUDA graph can capture it (include/esac_b200.h: esacb200_data_step_async).
+    Storage (CUDA or pinned CPU tensors): pixels uint8 [bytes] (RGB [H,W,3] per image), gt float32 [floats] or None,
+    attachments float32 [N, ...] each.  Device tensors: images uint8 [N, 120] (DATA_IMAGE records), plan int32
+    [capacity, 10] (DATA_ROW rows), state int64 [2] (DATA_STATE), work int64 [B].  Outputs (CUDA): outImage float32
+    [B,3,H,W], outShifts int32 [B,2], outCameras float32 [B,3], outPoses float32 [B,4,4], outScenes / outIndices int64
+    [B], outStatus int32 [1] (0 ok, 1 plan exhausted, 2 a row of another group), outCoords float32 [B,3,h,w] (with gt),
+    outAttachments float32 [B, ...] (one per attachment).  mean, std: three numbers each."""
+    call = "data_step_async"
+    named = {"pixels": pixels, "images": images, "plan": plan, "state": state, "work": work, "outImage": outImage,
+             "outShifts": outShifts, "outCameras": outCameras, "outPoses": outPoses, "outScenes": outScenes,
+             "outIndices": outIndices, "outStatus": outStatus}
+    if (gt is None) != (outCoords is None):
+        raise RuntimeError(f"{call}: gt and outCoords must both be given or both be None")
+    if gt is not None:
+        named.update(gt=gt, outCoords=outCoords)
+    for k, (a, o) in enumerate(zip(attachments, outAttachments)):
+        named.update({f"attachments[{k}]": a, f"outAttachments[{k}]": o})
+    for what, t in named.items():
+        if not _is_torch(t):
+            raise RuntimeError(f"{call} takes torch tensors only ({what} is a {type(t).__name__})")
+    if len(attachments) != len(outAttachments) or len(attachments) > DATA_MAX_ATTACH:
+        raise RuntimeError(f"{call}: {len(attachments)} attachments for {len(outAttachments)} outputs "
+                           f"(at most {DATA_MAX_ATTACH})")
+    if isinstance(group, bool) or not isinstance(group, numbers.Integral) or group < 0:
+        raise RuntimeError(f"{call}: group must be a non-negative int, got {group!r}")
+    mean, std = (np.ascontiguousarray(np.resize(np.asarray(v, np.float32).reshape(-1), 3) if np.size(v) == 1 else
+                                      np.asarray(v, np.float32).reshape(-1)) for v in (mean, std))
+    if mean.shape != (3,) or std.shape != (3,) or not np.isfinite(mean).all() or not np.isfinite(std).all() or \
+            (std == 0).any():
+        raise RuntimeError(f"{call}: mean and std must be three finite numbers each, std nonzero")
+    _check(outImage, "Float", 4, "outImage")
+    B, three, H, W = (int(v) for v in outImage.shape)
+    if three != 3 or not 1 <= B <= DATA_MAX_BATCH or not (1 <= H <= DATA_MAX_SIDE and 1 <= W <= DATA_MAX_SIDE):
+        raise RuntimeError(f"outImage must be [B,3,H,W] with B in [1, {DATA_MAX_BATCH}] and sides in [1, {DATA_MAX_SIDE}], "
+                           f"got {list(outImage.shape)}")
+    _check(images, "Byte", 2, "images")
+    N = int(images.shape[0])
+    _check(plan, "Int", 2, "plan")
+    capacity = int(plan.shape[0])
+    if N < 1 or capacity < 1:
+        raise RuntimeError(f"{call}: the set holds {N} images and the plan {capacity} rows; both must be positive")
+    fixed = {"images": (images, "Byte", (N, DATA_IMAGE.itemsize)), "plan": (plan, "Int", (capacity, DATA_ROW.itemsize // 4)),
+             "state": (state, "Long", (DATA_STATE,)), "work": (work, "Long", (B,)), "outImage": (outImage, "Float", (B, 3, H, W)),
+             "outShifts": (outShifts, "Int", (B, 2)), "outCameras": (outCameras, "Float", (B, 3)),
+             "outPoses": (outPoses, "Float", (B, 4, 4)), "outScenes": (outScenes, "Long", (B,)),
+             "outIndices": (outIndices, "Long", (B,)), "outStatus": (outStatus, "Int", (1,))}
+    gt_h = gt_w = 0
+    if gt is not None:
+        _check(gt, "Float", 1, "gt")
+        _check(outCoords, "Float", 4, "outCoords")
+        _, _, gt_h, gt_w = (int(v) for v in outCoords.shape)
+        if not (1 <= gt_h <= DATA_MAX_SIDE and 1 <= gt_w <= DATA_MAX_SIDE):
+            raise RuntimeError(f"outCoords must be [B,3,h,w] with sides in [1, {DATA_MAX_SIDE}], got {list(outCoords.shape)}")
+        fixed["outCoords"] = (outCoords, "Float", (B, 3, gt_h, gt_w))
+    numel = []
+    for k, (a, o) in enumerate(zip(attachments, outAttachments)):
+        _check(a, "Float", a.dim(), f"attachments[{k}]")
+        if a.dim() < 1 or int(a.shape[0]) != N or a.numel() == 0 or not a.is_contiguous():
+            raise RuntimeError(f"attachments[{k}] must be a contiguous float32 [{N}, ...] tensor with elements, "
+                               f"got {list(a.shape)}")
+        fixed[f"outAttachments[{k}]"] = (o, "Float", (B,) + tuple(int(v) for v in a.shape[1:]))
+        numel.append(a.numel() // N)
+    for what, (t, dt, shape) in fixed.items():
+        _check(t, dt, len(shape), what)
+        if tuple(int(v) for v in t.shape) != shape or not t.is_contiguous():
+            raise RuntimeError(f"{what} must be a contiguous {list(shape)} tensor, got {list(t.shape)}")
+    _check(pixels, "Byte", 1, "pixels")
+    storage = [("pixels", pixels)] + ([("gt", gt)] if gt is not None else []) + \
+        [(f"attachments[{k}]", a) for k, a in enumerate(attachments)]
+    for what, t in storage:
+        if not t.is_contiguous():
+            raise RuntimeError(f"{what} must be contiguous")
+        _storage_kind(t, what, call)
+    for what, (t, _, _) in fixed.items():
+        if not t.is_cuda:
+            raise RuntimeError(f"{call} takes CUDA tensors only ({what} is on the CPU)")
+    devs = {t.device.index for _, (t, _, _) in fixed.items()} | {t.device.index for _, t in storage if t.is_cuda}
+    if len(devs) > 1:
+        raise RuntimeError(f"esac_b200: tensors live on different CUDA devices {sorted(devs)}")
+    ctx = _pick_ctx(*devs)
+    n = len(attachments)
+    att = (C.c_void_p * max(n, 1))(*[a.data_ptr() for a in attachments])
+    att_out = (C.c_void_p * max(n, 1))(*[o.data_ptr() for o in outAttachments])
+    att_numel = (C.c_int64 * max(n, 1))(*numel)
+    ctx.check(ctx.lib.esacb200_data_step_async(
+        ctx.handle, pixels.data_ptr(), gt.data_ptr() if gt is not None else None, images.data_ptr(), N, int(group), H, W,
+        gt_h, gt_w, mean.ctypes.data, std.ctypes.data, n, att, att_numel, plan.data_ptr(), capacity, state.data_ptr(), B,
+        work.data_ptr(), outImage.data_ptr(), outShifts.data_ptr(), outCameras.data_ptr(), outPoses.data_ptr(),
+        outCoords.data_ptr() if outCoords is not None else None, outScenes.data_ptr(), outIndices.data_ptr(), att_out,
+        outStatus.data_ptr()))
 
 def set_seed(seed: int, device: int | None = None):
     context(device).set_seed(seed)

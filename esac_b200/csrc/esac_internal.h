@@ -8,6 +8,7 @@
 #include <cuda_fp16.h>
 
 #include "esac_geom.cuh"
+#include "../../include/esac_b200.h"
 
 namespace esacb200 {
 
@@ -790,5 +791,35 @@ struct RenderArgs {
 };
 // Clears the per-cell workspace and the counters, then the four passes; the caller synchronises.
 void launch_render(const RenderArgs& a, cudaStream_t st);
+
+// --- data.cu ------------------------------------------------------------------------------
+// One step of a device-resident image set (include/esac_b200.h: esacb200_data_step_async documents every field).
+struct DataArgs {
+    const unsigned char* pixels;          // RGB uint8 storage (device pointer, or the device alias of mapped pinned memory)
+    const float* gt;                      // ground-truth storage, or null
+    const esacb200_data_image* images;    // [n_images]
+    long long n_images;
+    int group, H, W, gt_h, gt_w;
+    float mean[3], std[3];
+    int n_attach;
+    const float* attach[ESACB200_DATA_MAX_ATTACH];
+    long long attach_numel[ESACB200_DATA_MAX_ATTACH];
+    const esacb200_data_row* plan;        // [capacity]
+    long long capacity;
+    esacb200_data_state* state;
+    int B;
+    unsigned long long* sums;             // [B] per-row L sums of the contrast mean
+    float* image;                         // [B,3,H,W]
+    int* shifts;                          // [B,2]
+    float* cameras;                       // [B,3]
+    float* poses;                         // [B,4,4]
+    float* coords;                        // [B,3,gt_h,gt_w], or null
+    long long* scenes;                    // [B]
+    long long* indices;                   // [B]
+    float* out_attach[ESACB200_DATA_MAX_ATTACH];
+    int* status;                          // [1]
+};
+// head (status, per-image records, clears sums), contrast mean, compose, gather, advance: five launches on st.
+void launch_data_step(const DataArgs& a, cudaStream_t st);
 
 }  // namespace esacb200

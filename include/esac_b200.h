@@ -609,6 +609,76 @@ int esacb200_render_init_maps(esacb200_ctx* ctx, int C, const float* points, int
                               const int32_t* H, const int32_t* W, float* out_maps, float* out_zbuf, int32_t* out_count,
                               int32_t* out_status);
 
+/* A device-resident image set feeding a captured step (esac_b200/data.py: DeviceImageSet): each step's image, colour
+ * jitter, normalisation, shift and ground truth are made on the device from the set's decoded, resized uint8 images, by
+ * the rows of a plan the host drew with the reference loop's random calls (room_dataset.py:134-207,
+ * cluster_dataset.py:245-275, util.py:4-11).
+ *
+ * esacb200_data_row: one image of one step.  image indexes the set's records; (padX, padY) is the shift
+ * nn.ZeroPad2d((padX, -padX, padY, -padY)) applies; ops[0 .. n_ops-1] are the jitter's ops in the order ColorJitter runs
+ * them (ESACB200_DATA_BRIGHTNESS / _CONTRAST / _SATURATION, each at most once, n_ops in [0, 3]) with factors[k] the
+ * factor of ops[k].  40 bytes. */
+#define ESACB200_DATA_BRIGHTNESS 0
+#define ESACB200_DATA_CONTRAST 1
+#define ESACB200_DATA_SATURATION 2
+#define ESACB200_DATA_MAX_ATTACH 8
+#define ESACB200_DATA_MAX_SIDE 8192
+#define ESACB200_DATA_MAX_BATCH 4096
+typedef struct {
+    int32_t image;
+    int32_t padX, padY;
+    int32_t n_ops;
+    int32_t ops[3];
+    float factors[3];
+} esacb200_data_row;
+
+/* esacb200_data_image: one image of the set.  pixels: byte offset of its RGB uint8 [H,W,3] pixels in the set's pixel
+ * storage; gt: float offset of its float32 [3,gt_h,gt_w] ground-truth map in the set's ground-truth storage (-1: none);
+ * focal: its focal length, already scaled to the stored image (the camera holds its float32 rounding); scene: the
+ * ground-truth scene (-1 for a clustered set); pose: float32 [4,4] camera->world, already offset; group: its shape group,
+ * whose image is H x W and whose ground truth is gt_h x gt_w.  120 bytes. */
+typedef struct {
+    int64_t pixels;
+    int64_t gt;
+    double focal;
+    int64_t scene;
+    float pose[16];
+    int32_t group;
+    int32_t H, W, gt_h, gt_w;
+    int32_t unused;
+} esacb200_data_image;
+
+/* esacb200_data_state: device memory.  position: the next plan row; rows: the rows the plan holds (from the last upload). */
+typedef struct {
+    int64_t position;
+    int64_t rows;
+} esacb200_data_state;
+
+/* esacb200_data_step_async: one step of B images of shape group `group` (images H x W, ground truth gt_h x gt_w), enqueued
+ * on the context's stream with no host synchronisation, read-back or allocation, so it may be captured.  It reads plan
+ * rows state->position .. + B - 1 (plan: device esacb200_data_row [capacity]) when the kernels run, and writes out_status
+ * (device int32 [1]): 0 ok; 1 the plan is exhausted (position + B > rows); 2 a row's image is outside [0, n_images) or not
+ * of this group and shape.  On 1 and 2 no other output is written and the position stays; on 0 the position advances by
+ * B.  Per image b: out_indices[b] (int64) the row's image, out_scenes[b] (int64) its scene, out_shifts[b] (int32 [2])
+ * padX, padY, out_cameras[b] (float32 [3]) (float)focal, W/2, H/2, out_poses[b] (float32 [4,4]) its pose, out_image[b]
+ * (float32 [3,H,W]) its pixels through the row's jitter, then (u/255 - mean[c]) / std[c] in float32, shifted by
+ * (padX, padY) with zeros outside; out_coords[b] (float32 [3,gt_h,gt_w]) its ground truth (gt and out_coords both null,
+ * or both given; every image of the group must then have one), and for k < n_attach out_attach[k][b] the
+ * attach_numel[k] floats of attachment k at attach[k] + image * attach_numel[k].
+ * Jitter, bitwise PIL's ImageEnhance: blend(a, b, f) = a + f (b - a) in float32 with no contraction, truncated to uint8
+ * for 0 <= f <= 1, else clipped to [0, 255] and truncated; brightness blends from 0, saturation from L = (19595 R +
+ * 38470 G + 7471 B + 0x8000) >> 16, contrast from int(sum(L) / N + 0.5) (fp64) over the image as the ops before it left it.
+ * pixels, gt and attach may be device memory or mapped pinned host memory; images, plan, state, work (int64 [B]) and the
+ * outputs are device memory; mean / std are host float[3].  Argument errors (ESACB200_ERR_ARG) are reported before
+ * anything is enqueued. */
+int esacb200_data_step_async(esacb200_ctx* ctx, const uint8_t* pixels, const float* gt, const esacb200_data_image* images,
+                             int64_t n_images, int group, int H, int W, int gt_h, int gt_w, const float* mean,
+                             const float* std, int n_attach, const float* const* attach, const int64_t* attach_numel,
+                             const esacb200_data_row* plan, int64_t capacity, esacb200_data_state* state, int B,
+                             int64_t* work, float* out_image, int32_t* out_shifts, float* out_cameras, float* out_poses,
+                             float* out_coords, int64_t* out_scenes, int64_t* out_indices, float* const* out_attach,
+                             int32_t* out_status);
+
 /* Soft-inlier scores of given poses (getReproErrs + getHypScores, esac_util.h:235-363) without
  * sampling/selection/refinement: poses6 = host double [M][6] (rvec, tvec); out_scores host double [M]. */
 int esacb200_score_poses(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,

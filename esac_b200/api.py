@@ -218,6 +218,8 @@ def load_library() -> C.CDLL:
     lib.esacb200_host_p3p_pose.restype = i32
     lib.esacb200_host_try.argtypes = [vp, vp, f32, f32, f32, f32, f32, C.POINTER(i32), C.POINTER(i32)]
     lib.esacb200_host_try.restype = None
+    lib.esacb200_host_tries_hint.argtypes = [i32, vp, vp, f32, f32, f32, f32, f32, vp, vp, vp]
+    lib.esacb200_host_tries_hint.restype = None
     lib.esacb200_host_try_verdict.argtypes = [vp, vp, f32, f32, f32, f32, C.POINTER(i32), vp]
     lib.esacb200_host_try_verdict.restype = None
     lib.esacb200_host_project.argtypes = [vp, f32, f32, f32, vp, vp, vp, vp]
@@ -321,7 +323,8 @@ class Context:
         out = np.zeros(8, np.int64)
         self.check(self.lib.esacb200_get_sample_profile(self.handle, out.ctypes.data))
         d = {"tries_prefiltered": int(out[0]), "survivors_judged": int(out[1]), "waves": int(out[2]),
-             "left_to_tail": int(out[3]), "accepted_staged": int(out[4]), "lanes": int(out[5])}
+             "left_to_tail": int(out[3]), "accepted_staged": int(out[4]), "lanes": int(out[5]),
+             "tries_cut": int(out[6]), "hints_rejected": int(out[7])}
         return d
 
     def sample_trace(self) -> np.ndarray:

@@ -189,6 +189,7 @@ int esacb200_set_option(esacb200_ctx* ctx, const char* key, double v) {
     else if (!strcmp(key, "sample_window")) o.sample_window = v < 0.05 ? 0.05f : (float)v;
     else if (!strcmp(key, "sample_waves")) o.sample_waves = v < 0 ? 0 : (v > 64 ? 64 : (int)v);
     else if (!strcmp(key, "upload_split")) o.upload_split = v != 0;  // host maps in two halves, sampling under the second copy
+    else if (!strcmp(key, "sample_hint")) o.sample_hint = v > 0 ? (v < 1.99 ? (float)v : 1.99f) : 0.f;  // fraction of tau, < kPrefilterMargin
     else if (!strcmp(key, "sample_groups")) o.sample_groups = v >= 4 ? 4 : (v >= 2 ? (int)v : 1);  // interleaved lanes, one stream each
     else if (!strcmp(key, "hyp_offset")) o.hyp_offset = (int)v;  // global index of local hypothesis 0 (sharded runs)
     else if (!strcmp(key, "hyp_stride")) o.hyp_stride = v < 1 ? 1 : (int)v;  // ... of local hypothesis h: offset + h * stride

@@ -66,6 +66,8 @@ struct Options {
     float sample_tail_boost = 1.f;  // window factor once <= 64 hypotheses are left in a lane (x2 more for <= 8)
     int sample_trace = 0;         // 1: prefilter / exact kernels of waves 0-31 stamp first-CTA-start / last-CTA-end times (esacb200_get_sample_trace)
     int sample_groups = 2;        // lanes of the sampling stage (third and fourth lane: no gain measured)
+    float sample_hint = 0.95f;    // prefilter no tries of a window beyond one whose 4th point the float path puts within
+                                  // this fraction of tau (0: off; below the prefilter's 2 tau band)
     int upload_split = 1;
     int hyp_offset = 0, hyp_stride = 1;
     int score_ppt_opt = 0, score_hc_opt = 0;

@@ -224,9 +224,9 @@ SampleSizes sample_layout(int M, int G, int Mg) {
     z.M = M;
     z.G = G;
     z.Mg = Mg;
-    // ints: [best: 2M] [base: M] [ovf: M] then per group [list: 2*Mg] [counters: SC_COUNT]
+    // ints: [best: 2M] [base: M] [ovf: M] [cut: M] then per group [list: 2*Mg] [counters: SC_COUNT]
     z.per_group_ints = (size_t)2 * z.Mg + SC_COUNT;
-    z.int_bytes = ((size_t)M * 4 + G * z.per_group_ints) * 4 + 8;
+    z.int_bytes = ((size_t)M * 5 + G * z.per_group_ints) * 4 + 8;
     z.per_group_bytes = (size_t)kSampleCap * sizeof(int2) + (size_t)kSampleCapAcc * sizeof(Accepted);
     z.surv_bytes = G * z.per_group_bytes;
     return z;
@@ -248,7 +248,8 @@ SampleState lane_state(const esacb200_ctx* ctx, const SampleSizes& z, int g) {
     s.best = ctx->smp_int.as<unsigned long long>();  // 8-byte aligned: first in the buffer
     s.base = b;
     s.ovf = b + z.M;
-    s.list = b + 2 * (size_t)z.M + g * z.per_group_ints;
+    s.cut = b + 2 * (size_t)z.M;
+    s.list = b + 3 * (size_t)z.M + g * z.per_group_ints;
     s.counters = s.list + 2 * (size_t)z.Mg;
     char* sb = (char*)ctx->smp_surv.p + g * z.per_group_bytes;
     s.surv = (int2*)sb;
@@ -295,7 +296,7 @@ int run_sample(esacb200_ctx* ctx, const Plan& pl, uint64_t seed) {
                                              ctx->tries.as<int>(), lane_streams, ctx->ev_fork, lane_joins,
                                              pl.split_e, ctx->perm.as<int>(), ctx->offsets.as<int>(), ctx->ev_copied,
                                              o.sample_span0, o.sample_window, o.sample_waves, trace, o.sample_tail_boost,
-                                             pl.async ? &pl.async->dev : nullptr);
+                                             o.sample_prefilter ? o.sample_hint : 0.f, pl.async ? &pl.async->dev : nullptr);
     CK(cudaGetLastError());
     if (pl.split_e) {
         // both halves have landed (the join orders this stream after lane 1, which waited for the second half): plane centres
@@ -881,6 +882,8 @@ int esacb200_get_sample_profile(esacb200_ctx* ctx, long long* out8) try {
         out8[2] = out8[2] > c[SC_WAVES] ? out8[2] : c[SC_WAVES];
         out8[3] += c[SC_UNRESOLVED];
         out8[4] += c[SC_STAGED];
+        out8[6] += (unsigned)c[SC_CUT];
+        out8[7] += (unsigned)c[SC_HINTS_REJECTED];
     }
     out8[5] = G;
     return ESACB200_OK;

@@ -57,6 +57,23 @@ void esacb200_host_try(const float* obj12, const float* img8, float f, float ppx
     *accept = (ok && minimal_set_gate(obj, img, p, (double)f, (double)ppx, (double)ppy, tau)) ? 1 : 0;
 }
 
+void esacb200_host_tries_hint(int n, const float* obj12n, const float* img8n, float f, float ppx, float ppy, float tau,
+                              float hint_frac, int* may_pass, int* hint, int* accept) {
+    for (int k = 0; k < n; ++k) {
+        float obj[4][3], img[4][2];
+        for (int i = 0; i < 4; ++i) {
+            for (int c = 0; c < 3; ++c) obj[i][c] = obj12n[k * 12 + i * 3 + c];
+            for (int c = 0; c < 2; ++c) img[i][c] = img8n[k * 8 + i * 2 + c];
+        }
+        bool h;
+        may_pass[k] = p3p_may_pass_hint(obj, img, f, ppx, ppy, tau, hint_frac, h) ? 1 : 0;
+        hint[k] = h ? 1 : 0;
+        Pose p;
+        const bool ok = p3p_pose(obj, img, (double)f, (double)ppx, (double)ppy, p);
+        accept[k] = (ok && minimal_set_gate(obj, img, p, (double)f, (double)ppx, (double)ppy, tau)) ? 1 : 0;
+    }
+}
+
 void esacb200_host_try_verdict(const float* obj12, const float* img8, float f, float ppx, float ppy, float tau, int* accept,
                                double* pose6) {
     float obj[4][3], img[4][2];

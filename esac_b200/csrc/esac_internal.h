@@ -269,6 +269,7 @@ struct SampleState {
     int cap_acc;
     int* base;      // [M] first try not judged yet
     int* ovf;       // [M] lowest survivor that did not fit the list in the current wave
+    int* cut;       // [M] 1 + lowest hinted survivor in the list in the current wave: later tries are not prefiltered
     int* list;      // [2M] unresolved hypotheses (second half: scratch for rebuilding)
     int2* surv;     // [cap] (hypothesis, try) pairs that passed the float prefilter
     int cap;
@@ -286,6 +287,8 @@ enum SampleCounter {
     SC_PREFILTERED,     // tries prefiltered
     SC_JUDGED,          // survivors judged
     SC_WAVES,           // waves that had work
+    SC_CUT,             // tries of the windows the prefilter skipped, being beyond a hinted survivor (option sample_hint)
+    SC_HINTS_REJECTED,  // hinted survivors the exact verdict rejected
     SC_COUNT
 };
 // Returns the number of kernel launches it enqueued.
@@ -294,7 +297,7 @@ int launch_sample(const float* coords, float4* coords4, const int* assign32, con
                   int hyp_offset, int hyp_stride, Pose* poses, int* cells, int* tries, const cudaStream_t* lanes,
                   cudaEvent_t ev_fork, const cudaEvent_t* ev_join, int split_e, const int* perm, const int* offsets,
                   const cudaEvent_t* ev_half, int span0, float window, int n_waves,
-                  unsigned long long* trace, float tail_boost, const DevParams* dev = nullptr);
+                  unsigned long long* trace, float tail_boost, float hint, const DevParams* dev = nullptr);
 void launch_trace_init(unsigned long long* trace, int slots, cudaStream_t st);
 
 // --- refine.cu ----------------------------------------------------------------------------

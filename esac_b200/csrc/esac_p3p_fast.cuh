@@ -137,10 +137,13 @@ constexpr float kPrefilterMargin = 2.f;
 constexpr float kPrefilterNeedle = 0.02f;  // shortest / longest squared side below which the triangle goes to the exact path
 
 // obj[i][c] / img[i][c]: point i, coordinate c, of the W tries of the pack.  Returns, per try, false only when the try
-// certainly fails the 4-point gate.
+// certainly fails the 4-point gate.  `hint` is raised, per try, when the try is all but certain to pass: a root that is
+// used and trusted (accurate residual, scale ok, no depth near a sign change) brings the 4th point within hint_frac * tau,
+// and no latch sent the set to the exact path as ill-conditioned.  hint implies the returned mask; it is never a verdict
+// (hint_frac = 0: never raised).
 template <typename P>
 ESAC_HD typename MaskOf<P>::type p3p_may_pass_pack(const P obj[4][3], const P img[4][2], float f, float ppx, float ppy, float tau,
-                                                   float margin = kPrefilterMargin, float needle = kPrefilterNeedle) {
+                                                   float margin, float needle, float hint_frac, typename MaskOf<P>::type& hint) {
     typedef typename MaskOf<P>::type M;
     using N = Num<float>;
     const P zero = bc<P>(0.f), one = bc<P>(1.f), two = bc<P>(2.f);
@@ -276,11 +279,11 @@ ESAC_HD typename MaskOf<P>::type p3p_may_pass_pack(const P obj[4][3], const P im
     const P idet = rcp_(det);
     const P al = (v1 * a13 - v2 * g12) * idet, be = (v2 * a12 - v1 * g12) * idet;
     const P ga = (x3[0] * nrm[0] + x3[1] * nrm[1] + x3[2] * nrm[2]) * rcp_(nn);
-    const float lim = margin * tau;
-    const P lim2 = bc<P>(lim * lim);
+    const float lim = margin * tau, hlim = hint_frac * tau;
+    const P lim2 = bc<P>(lim * lim), hlim2 = bc<P>(hlim * hlim);
     const P sa = sqrt_(amax);
     const P vf = bc<P>(f);
-    M pass = no;
+    M pass = no, near = no;
 #pragma unroll
     for (int s = 0; s < 4; ++s) {
         const M live = s < 2 ? okL : okM;
@@ -303,7 +306,8 @@ ESAC_HD typename MaskOf<P>::type p3p_may_pass_pack(const P obj[4][3], const P im
         l0 = l0 * sc; l1 = l1 * sc; l2 = l2 * sc;
         const P res = abs_(l0 * l0 + l1 * l1 - two * c12 * l0 * l1 - s12) + abs_(l0 * l0 + l2 * l2 - two * c13 * l0 * l2 - s13) +
                       abs_(l1 * l1 + l2 * l2 - two * c23 * l1 * l2 - s23);
-        pass = pass | (use & !lt_(res, bc<P>(1e-4f) * (l0 * l0 + l1 * l1 + l2 * l2 + one)));  // inaccurate candidate: not trusted
+        const M accurate = lt_(res, bc<P>(1e-4f) * (l0 * l0 + l1 * l1 + l2 * l2 + one));
+        pass = pass | (use & !accurate);  // inaccurate candidate: not trusted
         P P0[3], u1[3], u2[3], m[3];
 #pragma unroll
         for (int cc = 0; cc < 3; ++cc) {
@@ -321,13 +325,21 @@ ESAC_HD typename MaskOf<P>::type p3p_may_pass_pack(const P obj[4][3], const P im
         const P du = vppx + vf * xc * iz - img[3][0], dv = vppy + vf * yc * iz - img[3][1];
         const P e = du * du + dv * dv;
         pass = pass | (use & !gt_(e, lim2));  // close enough (or NaN/inf): let the exact path decide
+        near = near | (use & accurate & !near0 & le_(e, hlim2));
     }
+    hint = near & !decided & pass;  // every earlier latch either rejected or forwarded an ill-conditioned set
     ESAC_LATCH(yes, pass)
 #undef ESAC_LATCH
     return verdict;
 }
+template <typename P>
+ESAC_HD typename MaskOf<P>::type p3p_may_pass_pack(const P obj[4][3], const P img[4][2], float f, float ppx, float ppy, float tau,
+                                                   float margin = kPrefilterMargin, float needle = kPrefilterNeedle) {
+    typename MaskOf<P>::type hint;
+    return p3p_may_pass_pack<P>(obj, img, f, ppx, ppy, tau, margin, needle, 0.f, hint);
+}
 
-// one try (prefilter_kernel, tail_kernel, host test hooks)
+// one try (tail_kernel, host test hooks)
 ESAC_HD bool p3p_may_pass_fast(const float obj[4][3], const float img[4][2], float f, float ppx, float ppy, float tau,
                                float margin = kPrefilterMargin, float needle = kPrefilterNeedle) {
     Pack1 o[4][3], im[4][2];
@@ -338,6 +350,21 @@ ESAC_HD bool p3p_may_pass_fast(const float obj[4][3], const float img[4][2], flo
         im[i][0] = bc1(img[i][0]); im[i][1] = bc1(img[i][1]);
     }
     return p3p_may_pass_pack<Pack1>(o, im, f, ppx, ppy, tau, margin, needle).a;
+}
+// ... and its "near-certain" hint (prefilter_kernel, host test hooks): returns may-pass, `hint` implies it
+ESAC_HD bool p3p_may_pass_hint(const float obj[4][3], const float img[4][2], float f, float ppx, float ppy, float tau,
+                               float hint_frac, bool& hint, float margin = kPrefilterMargin, float needle = kPrefilterNeedle) {
+    Pack1 o[4][3], im[4][2];
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) o[i][c] = bc1(obj[i][c]);
+        im[i][0] = bc1(img[i][0]); im[i][1] = bc1(img[i][1]);
+    }
+    Mask1 h;
+    const bool pass = p3p_may_pass_pack<Pack1>(o, im, f, ppx, ppy, tau, margin, needle, hint_frac, h).a;
+    hint = h.a;
+    return pass;
 }
 
 }  // namespace esacb200

@@ -12,12 +12,16 @@
 //     prefilter_kernel   one try per thread, fp32 only, branch-free: discards tries whose
 //                        every P3P root misses the 4th point by > 2 tau (>96% on wrong experts); the gathers of a
 //                        CTA's next 128-try item are in flight under the math of the current one; survivors are
-//                        appended to a global list
+//                        appended to a global list.  A survivor a trusted root puts within sample_hint * tau is all but
+//                        certain to pass: it cuts its hypothesis' window (st.cut), and the items of that window issued
+//                        later (items are chunk-major, so a hypothesis' next chunk comes a grid round later) skip the
+//                        tries beyond it
 //     exact_kernel       one thread per survivor: the fp64 path (p3p_pose + minimal_set_gate) whose verdict is the
 //                        only one that counts (it leaves early when no P3P candidate can pass, and polishes only the
 //                        candidate far ahead on the 4th point); atomicMin keeps the lowest accepted try per hypothesis
-//     (advance)          the last CTA of exact_kernel marks resolved hypotheses, advances the window of the others and
-//                        rebuilds the work list
+//     (advance)          the last CTA of exact_kernel marks resolved hypotheses (an accept at or below the hinted try,
+//                        or the list-overflow point), advances the window of the others -- past a false hint, from the
+//                        try after it -- and rebuilds the work list
 //   tail_kernel          CTA per still-unresolved hypothesis: same two phases inside one CTA up to max_tries
 //   emit_kernel          one thread per hypothesis: re-derives the winning (or, when exhausted, the last) try and
 //                        writes pose / cells / try count
@@ -55,6 +59,7 @@ struct SampleArgs {
     int span0;                // window of the first wave (tries per hypothesis)
     float window;             // later windows: window / (acceptance rate per try seen in the last wave)
     float tail_boost;         // ... times this once <= 64 hypotheses are left (twice this for <= 8)
+    float hint;               // a surviving try whose 4th point the float path puts within hint * tau cuts its window (0: off)
     SampleState st;
     unsigned long long* trace;  // diagnostics (option sample_trace): [slot][2] first CTA start / last CTA end, globaltimer ns
     int trace_slot;
@@ -156,16 +161,18 @@ __global__ void sample_init_kernel(const __grid_constant__ SampleArgs a) {
     const int n = lane_size(a);
     if (k < n) {
         const int h = lane_hyp(a, k);
-        st.best[h] = kNoKey; st.base[h] = 0; st.ovf[h] = kNoTry; st.list[k] = h;
+        st.best[h] = kNoKey; st.base[h] = 0; st.ovf[h] = kNoTry; st.cut[h] = kNoTry; st.list[k] = h;
     }
     if (k == 0) {
         st.counters[SC_UNRESOLVED] = n; st.counters[SC_SURVIVORS] = 0; st.counters[SC_STAGED] = 0; st.counters[SC_SPAN] = a.span0;
         st.counters[SC_TICKET] = 0; st.counters[SC_PREFILTERED] = 0; st.counters[SC_JUDGED] = 0; st.counters[SC_WAVES] = 0;
+        st.counters[SC_CUT] = 0; st.counters[SC_HINTS_REJECTED] = 0;
     }
 }
 
 // ---- wave phase 1: fp32 prefilter, one try per thread ----------------------------------------------------------------
 constexpr int kSpanQuantum = 256;  // windows are multiples of this many tries
+constexpr unsigned kHintBit = 0x80000000u;  // survivor record (h, t): top bit of t = the prefilter's hint
 // One work item of the prefilter: kTryThreads consecutive tries of one hypothesis, one per thread.
 struct PreItem {
     int h, t;               // hypothesis, this thread's try
@@ -176,15 +183,27 @@ __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"((unsigned)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
 }
 // Decodes item -> (hypothesis, try), draws the 4 cells and starts the 4 gathers of 16 bytes straight into shared memory
-// (cp.async: no registers are held while they are in flight).
+// (cp.async: no registers are held while they are in flight).  With the hint on, items are chunk-major (chunk c of every
+// unresolved hypothesis, then chunk c + 1), so a hypothesis' next chunk is issued about one grid round after the current
+// one, by when a hinted survivor among its tries may have cut the window: tries at or beyond st.cut are not drawn, gathered
+// or judged.  The cut is read through L2 (other CTAs lower it with atomicMin); a stale read only means less skipping.  With
+// the hint off, items are hypothesis-major, as the survivor list's overflow schedules were laid out for.
 template <bool DEV>
-__device__ __forceinline__ void prefilter_issue(const SampleArgsT<DEV>& a, long long item, int cph, int span, float4 (*dst)[kTryThreads], PreItem& it) {
-    const int u = (int)(item / cph), c = (int)(item - (long long)u * cph);
+__device__ __forceinline__ void prefilter_issue(const SampleArgsT<DEV>& a, long long item, int n_unres, int cph, int span, float4 (*dst)[kTryThreads], PreItem& it) {
+    int u, c;
+    if (a.hint > 0.f) { c = (int)(item / n_unres); u = (int)(item - (long long)c * n_unres); }
+    else { u = (int)(item / cph); c = (int)(item - (long long)u * cph); }
     it.h = a.st.list[u];
     const int t0 = a.st.base[it.h];
     const int off = c * kTryThreads + threadIdx.x;
     it.t = t0 + off;
     it.valid = off < span && it.t < a.limit;
+    if (a.hint > 0.f) {
+        const bool cut = it.valid && it.t >= __ldcg(&a.st.cut[it.h]);
+        const unsigned m = __ballot_sync(0xffffffffu, cut);
+        if (m && (threadIdx.x & 31) == 0) atomicAdd(&a.st.counters[SC_CUT], __popc(m));
+        it.valid = it.valid && !cut;
+    }
     if (!it.valid) return;
     const Problem& P = a.P;
     const float4* pl = a.coords4 + (size_t)a.assign32[it.h] * P.N;
@@ -219,15 +238,15 @@ __global__ void __launch_bounds__(kTryThreads, 6) prefilter_kernel(const __grid_
     const Problem& P = a.P;
     PreItem cur, nxt;
     long long item = blockIdx.x;
-    if (item < n_items) prefilter_issue<DEV>(a, item, cph, span, s_obj[0], cur);
+    if (item < n_items) prefilter_issue<DEV>(a, item, n_unres, cph, span, s_obj[0], cur);
     asm volatile("cp.async.commit_group;" ::: "memory");
     int buf = 0;
     for (; item < n_items; item += gridDim.x) {
         const long long ni = item + gridDim.x;
-        if (ni < n_items) prefilter_issue<DEV>(a, ni, cph, span, s_obj[buf ^ 1], nxt);
+        if (ni < n_items) prefilter_issue<DEV>(a, ni, n_unres, cph, span, s_obj[buf ^ 1], nxt);
         asm volatile("cp.async.commit_group;" ::: "memory");
         asm volatile("cp.async.wait_group 1;" ::: "memory");  // everything but the group just committed has landed
-        bool pass = false;
+        bool pass = false, hint = false;
         if (cur.valid) {
             float obj[4][3], img[4][2];
 #pragma unroll
@@ -238,7 +257,8 @@ __global__ void __launch_bounds__(kTryThreads, 6) prefilter_kernel(const __grid_
                 img[j][0] = (float)((int)(c & 0xffffu) * P.sub + P.sub / 2 - dev_shift_x<DEV>(P, a));
                 img[j][1] = (float)((int)(c >> 16) * P.sub + P.sub / 2 - dev_shift_y<DEV>(P, a));
             }
-            pass = !a.use_prefilter || p3p_may_pass_fast(obj, img, dev_f<DEV>(P, a), dev_ppx<DEV>(P, a), dev_ppy<DEV>(P, a), P.tau);
+            pass = !a.use_prefilter || p3p_may_pass_hint(obj, img, dev_f<DEV>(P, a), dev_ppx<DEV>(P, a), dev_ppy<DEV>(P, a), P.tau, a.hint, hint);
+            hint = hint && a.use_prefilter;
         }
         // warp-aggregated append of the survivors
         const unsigned m = __ballot_sync(0xffffffffu, pass);
@@ -248,8 +268,13 @@ __global__ void __launch_bounds__(kTryThreads, 6) prefilter_kernel(const __grid_
             basei = __shfl_sync(0xffffffffu, basei, 0);
             if (pass) {
                 const int idx = basei + __popc(m & ((1u << lane) - 1u));
-                if (idx < a.st.cap) a.st.surv[idx] = make_int2(cur.h, cur.t);
-                else atomicMin(&a.st.ovf[cur.h], cur.t);  // list full: this hypothesis resumes from here in the next wave
+                if (idx < a.st.cap) {
+                    a.st.surv[idx] = make_int2(cur.h, hint ? (int)((unsigned)cur.t | kHintBit) : cur.t);
+                    // all but certain to pass: no later try of this window needs prefiltering (every earlier one still is)
+                    if (hint) atomicMin(&a.st.cut[cur.h], cur.t + 1);
+                } else {
+                    atomicMin(&a.st.ovf[cur.h], cur.t);  // list full: this hypothesis resumes from here in the next wave
+                }
             }
         }
         cur = nxt;
@@ -266,12 +291,18 @@ __global__ void __launch_bounds__(128) exact_kernel(const __grid_constant__ Samp
     TraceScope trace(a.trace, a.trace_slot);
     const int n = min(a.st.counters[SC_SURVIVORS], a.st.cap);
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const int2 ht = a.st.surv[i];
+        int2 ht = a.st.surv[i];
+        const bool hinted = (unsigned)ht.y & kHintBit;
+        ht.y = (int)((unsigned)ht.y & ~kHintBit);
         if (ht.y >= a.st.ovf[ht.x]) continue;  // beyond the point where the list overflowed: redone next wave
+        // survivors beyond a hypothesis' cut are judged all the same: the wave's exact kernel lasts as long as its longest
+        // verdict, and advance_wave discounts an accept beyond the cut
         Pose pose;
         int cx[4], cy[4];
         bool solved;
-        if (exact_try<DEV>(a, ht.x, ht.y, pose, cx, cy, solved, true)) {
+        const bool accepted = exact_try<DEV>(a, ht.x, ht.y, pose, cx, cy, solved, true);
+        if (hinted && !accepted) atomicAdd(&a.st.counters[SC_HINTS_REJECTED], 1);
+        if (accepted) {
             // stage the accepted pose so that emit_kernel does not have to solve it again
             unsigned slot = (unsigned)atomicAdd(&a.st.counters[SC_STAGED], 1);
             if (slot < (unsigned)a.st.cap_acc) {
@@ -307,7 +338,7 @@ __device__ void advance_wave(const SampleState& st, int limit, float window, flo
     int* next = st.list + st.M;
     for (int u = threadIdx.x; u < n_unres; u += blockDim.x) {
         const int h = st.list[u];
-        const int ovf = st.ovf[h];
+        const int ovf = min(st.ovf[h], st.cut[h]);
         const int end = min(st.base[h] + span, ovf);  // tries below `end` have all been judged
         const unsigned long long best = __ldcg(&st.best[h]);
         const bool resolved = (long long)(best >> 32) < (long long)end;
@@ -315,6 +346,7 @@ __device__ void advance_wave(const SampleState& st, int limit, float window, flo
             if (best != kNoKey) st.best[h] = kNoKey;  // an accept beyond an overflow hole does not count yet
             st.base[h] = end;
             st.ovf[h] = kNoTry;
+            st.cut[h] = kNoTry;
             if (end < limit) next[atomicAdd(&s_fill, 1)] = h;
         }
     }
@@ -423,7 +455,7 @@ int launch_sample(const float* coords, float4* coords4, const int* assign32, con
                   int hyp_offset, int hyp_stride, Pose* poses, int* cells, int* tries, const cudaStream_t* lanes,
                   cudaEvent_t ev_fork, const cudaEvent_t* ev_join, int split_e, const int* perm, const int* offsets,
                   const cudaEvent_t* ev_half, int span0, float window, int n_waves,
-                  unsigned long long* trace, float tail_boost, const DevParams* dev) {
+                  unsigned long long* trace, float tail_boost, float hint, const DevParams* dev) {
     int launches = 0;
     cudaStream_t stream = lanes[0];
     if (!split_e) { interleave_kernel<<<sm_count * 8, 256, 0, stream>>>(coords, coords4, P.E, P.N); ++launches; }
@@ -436,7 +468,7 @@ int launch_sample(const float* coords, float4* coords4, const int* assign32, con
         a.injected = injected; a.inj_T = inj_T; a.st = st[g]; a.use_prefilter = use_prefilter; a.hyp_offset = hyp_offset; a.hyp_stride = hyp_stride > 0 ? hyp_stride : 1;
         a.h_first = g; a.h_step = n_lanes; a.Mg = (P.M - g + n_lanes - 1) / n_lanes;
         a.perm = nullptr; a.offsets = nullptr; a.e_lo = a.e_hi = 0;
-        a.span0 = span0; a.window = window; a.trace = trace; a.trace_slot = 0; a.tail_boost = tail_boost;
+        a.span0 = span0; a.window = window; a.trace = trace; a.trace_slot = 0; a.tail_boost = tail_boost; a.hint = hint;
         a.dev = dev ? *dev : DevParams{};
         bound[g] = a.Mg;  // host-side bound on the lane size (grid sizing)
         if (split_e) {

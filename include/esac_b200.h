@@ -51,7 +51,9 @@ int esacb200_set_seed(esacb200_ctx* ctx, uint64_t seed);
  * (esac.cpp:45 MAX_REF_STEPS, default 100), "fixed_seed" (1: do not advance the call counter),
  * "refine_group" (CTAs per refinement job, 0 = automatic), "refine_jobs_per_group" (jobs a group
  * works through when many hypotheses are refined), "refine_profile", "sample_prefilter" (default 1; 0 sends every sampling
- * try through the exact fp64 path -- the results must not change, only the time), "hyp_offset" (global index of
+ * try through the exact fp64 path -- the results must not change, only the time), "sample_hint" (default 0.95, 0 = off,
+ * below 2: a try whose 4th point the float prefilter puts within this fraction of tau stops the prefiltering of the later
+ * tries of its window -- the results must not change, only the time), "hyp_offset" (global index of
  * local hypothesis 0 for the minimal-set stream; sharded runs), "score_ppt" / "score_hc" (scoring launch shape). */
 int esacb200_set_option(esacb200_ctx* ctx, const char* key, double value);
 /* Inject minimal sets instead of drawing them: cells int32 [M][T][4][2] (x, y), host pointer,
@@ -718,7 +720,9 @@ int esacb200_get_refine_profile(esacb200_ctx* ctx, long long* out16);
 
 /* Diagnostics of the last call's sampling stage (summed over its lanes): [0] tries that went through the float prefilter,
  * [1] survivors the fp64 path judged, [2] waves that had work (max over lanes), [3] hypotheses left to the tail kernel,
- * [4] accepted tries staged, [5] lanes.  out8: host long long [8].  Valid after a call that drew hypotheses (those listed
+ * [4] accepted tries staged, [5] lanes, [6] tries of the windows the prefilter skipped because an earlier try was hinted
+ * (option "sample_hint"; [0] still counts the whole windows), [7] hinted tries the exact verdict rejected.
+ * out8: host long long [8].  Valid after a call that drew hypotheses (those listed
  * at esacb200_get_hypotheses); after any other call it fails with ESACB200_ERR_ARG. */
 int esacb200_get_sample_profile(esacb200_ctx* ctx, long long* out8);
 /* With option "sample_trace" = 1 the prefilter / exact kernels of the sampling waves stamp %globaltimer: out512 (host uint64

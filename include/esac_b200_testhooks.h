@@ -26,6 +26,11 @@ int esacb200_host_p3p_pose(const float* obj12, const float* img8, float f, float
  * *accept = exact verdict (P3P solved and the 4-point gate passed).  Invariant: accept implies may_pass. */
 void esacb200_host_try(const float* obj12, const float* img8, float f, float ppx, float ppy, float tau, float margin,
                        int* may_pass, int* accept);
+/* n sampling tries (obj float[n][4][3], img float[n][4][2]) as prefilter_kernel sees them: may_pass[i] = float prefilter
+ * verdict at its shipping band, hint[i] = its "near-certain" hint at hint_frac * tau (option sample_hint), accept[i] = exact
+ * verdict (as esacb200_host_try's).  Invariants: hint implies may_pass, accept implies may_pass. */
+void esacb200_host_tries_hint(int n, const float* obj12n, const float* img8n, float f, float ppx, float ppy, float tau,
+                              float hint_frac, int* may_pass, int* hint, int* accept);
 /* The sampling kernels' verdict path: the same exact decision, but a try none of whose P3P candidates brings the 4th point
  * within 1.25 tau + 1 px is rejected before polish / alignment (p3p_solve's early exit).  Only the candidate that is far ahead
  * on the 4th point is polished (p3p_solve's favourite).  Invariants: *accept equals esacb200_host_try's, and for an accepted

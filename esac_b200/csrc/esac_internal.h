@@ -825,4 +825,93 @@ struct DataArgs {
 // head (status, per-image records, clears sums), contrast mean, compose, gather, advance: five launches on st.
 void launch_data_step(const DataArgs& a, cudaStream_t st);
 
+// --- experts.cu ---------------------------------------------------------------------------
+// The reference's Expert (code/expert.py), layer l in state-dict order: conv1 .. conv4, res1_conv1..3, res2_conv1..3,
+// res2_skip, res3_conv1..3, fc1, fc2, fc3.  Packed weights of E experts: per layer, W [E][Cout][k][k][Cin] then
+// b [E][Cout], each segment starting on a 64-float boundary; then mean [E][3].
+constexpr int kExpertLayers = 17;
+struct ExpertLayer {
+    int cin, cout, k, stride;
+    int index;
+    __host__ __device__ static constexpr long long round64(long long n) { return (n + 63) / 64 * 64; }
+    __host__ __device__ constexpr long long w_count() const { return (long long)cout * cin * k * k; }
+    __host__ __device__ constexpr long long w_off(int E) const;
+    __host__ __device__ constexpr long long b_off(int E) const { return w_off(E) + round64(E * w_count()); }
+};
+__host__ __device__ constexpr ExpertLayer expert_layer(int l) {
+    constexpr int t[kExpertLayers][4] = {{3, 32, 3, 1},    {32, 64, 3, 2},    {64, 128, 3, 2},   {128, 256, 3, 2},
+                                         {256, 256, 3, 1}, {256, 256, 1, 1},  {256, 256, 3, 1},  {256, 512, 3, 1},
+                                         {512, 512, 1, 1}, {512, 512, 3, 1},  {256, 512, 1, 1},  {512, 512, 1, 1},
+                                         {512, 512, 1, 1}, {512, 512, 1, 1},  {512, 512, 1, 1},  {512, 512, 1, 1},
+                                         {512, 3, 1, 1}};
+    return ExpertLayer{t[l][0], t[l][1], t[l][2], t[l][3], l};
+}
+__host__ __device__ constexpr long long ExpertLayer::w_off(int E) const {
+    long long off = 0;
+    for (int l = 0; l < index; ++l) {
+        const ExpertLayer d = expert_layer(l);
+        off += round64(E * d.w_count()) + round64((long long)E * d.cout);
+    }
+    return off;
+}
+__host__ __device__ constexpr long long expert_mean_off(int E) {
+    return expert_layer(kExpertLayers - 1).b_off(E) + ExpertLayer::round64(3LL * E);
+}
+__host__ __device__ constexpr long long experts_packed_floats(int E) { return expert_mean_off(E) + ExpertLayer::round64(3LL * E); }
+
+// Sides of the four resolutions (full, /2, /4, /8: stride-2 3x3 convolutions with padding 1 give ceil(n / 2)) and the
+// float offsets of one pair's NHWC activations in its workspace block: a0 (conv1, full resolution) shares its space with
+// a2 (conv3, /4); a1 (conv2); at /8: r (conv4 and the first residual sum), s (the second and third residual sums), x, y.
+struct ExpertsShape {
+    int h[4], w[4];
+    long long a0, a1, a2, r, s, x, y, pair_floats;
+};
+inline ExpertsShape experts_shape(int H, int W) {
+    ExpertsShape s{};
+    s.h[0] = H;
+    s.w[0] = W;
+    for (int i = 1; i < 4; ++i) {
+        s.h[i] = (s.h[i - 1] + 1) / 2;
+        s.w[i] = (s.w[i - 1] + 1) / 2;
+    }
+    auto r64 = ExpertLayer::round64;
+    const long long p0 = (long long)s.h[0] * s.w[0], p1 = (long long)s.h[1] * s.w[1], p2 = (long long)s.h[2] * s.w[2],
+                    p3 = (long long)s.h[3] * s.w[3];
+    s.a0 = s.a2 = 0;
+    s.a1 = r64(32 * p0 > 128 * p2 ? 32 * p0 : 128 * p2);
+    s.r = s.a1 + r64(64 * p1);
+    s.s = s.r + r64(256 * p3);
+    s.x = s.s + r64(512 * p3);
+    s.y = s.x + r64(512 * p3);
+    s.pair_floats = s.y + r64(512 * p3);
+    return s;
+}
+// The workspace: a header of ints -- [0] active pairs, [kExpertsHdrList ..) their pair indices b * E + e in ascending
+// order, then B * E flags (1: active) -- and from byte experts_hdr_bytes(B * E) on, one block of pair_floats per pair.
+constexpr int kExpertsHdrList = 16;
+inline long long experts_hdr_bytes(int pairs) { return ExpertLayer::round64(kExpertsHdrList + 2LL * pairs) * 4; }
+
+struct ExpertsArgs {
+    int B, E, H, W;
+    const float* image;   // [image_batch,3,H,W]
+    int image_batch;      // 1 (every image of the batch) or B
+    const float* hist;    // [B,E], or null: every pair is active
+    const float* packed;  // experts_packed_floats(E)
+    int* ws_hdr;
+    float* ws_pairs;
+    long long pair_floats;
+    float* out;           // [B,E,3,h[3],w[3]]
+};
+struct ExpertsConvLayer {
+    int cin, cout, hin, win, hout, wout;
+    long long in_off, out_off, res_off;  // in a pair's block; res_off -1: no residual
+    long long w_off, b_off;              // in the packed weights
+    bool relu;
+};
+// The active list, conv1, conv2 .. fc2 (15 implicit-GEMM launches), fc3: 18 launches on st.
+void launch_experts_forward(const ExpertsArgs& a, cudaStream_t st);
+// Layer l of E experts from `staged` (W at staged_w, b at staged_b, in torch's layouts, experts back to back) into `packed`.
+void launch_experts_pack(const float* staged, float* packed, int E, int l, long long staged_w, long long staged_b,
+                         cudaStream_t st);
+
 }  // namespace esacb200

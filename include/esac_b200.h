@@ -748,6 +748,34 @@ int esacb200_get_hypotheses(esacb200_ctx* ctx, double* poses6, int32_t* cells, i
  * not the last call's. */
 int esacb200_copy_last_scores(esacb200_ctx* ctx, double* dst, int M);
 
+/* ---- expert stack: inference of the reference's Expert FCN (code/expert.py) for E experts ---------------------------
+ * TF32 tensor-core operands with fp32 accumulation and fp32 activations (the regime of torch's default
+ * cudnn.allow_tf32 = True).  Only (image, expert) pairs with a positive histogram count run; every layer of all of them is
+ * one launch.  Expert e's output for image b does not depend on the other pairs of the call.
+ *
+ * esacb200_experts_pack: params is a host array of E * ESACB200_EXPERT_TENSORS pointers (host or device memory, float32,
+ * contiguous), expert by expert, each in the order conv1.weight, conv1.bias, conv2.weight, ..., res2_skip.weight,
+ * res2_skip.bias, res3_conv1.weight, ..., fc3.weight, fc3.bias, mean -- the layers of Expert.__init__ with torch's shapes.
+ * packed: device, esacb200_experts_packed_floats(E) floats (16-byte aligned).  Synchronous.
+ *
+ * esacb200_experts_forward_async: image float32 [image_batch,3,H,W] (image_batch 1: one image for the whole batch, or B);
+ * hist float32 [B,E] (pair (b, e) runs when hist[b][e] > 0) or NULL (every pair runs); out float32 [B,E,3,ceil(H/8),
+ * ceil(W/8)], zero planes for the pairs that do not run.  Enqueued on the context's stream with no host synchronisation
+ * (capturable).  workspace: device, 256-byte aligned, at least esacb200_experts_workspace_bytes(B, E, H, W) bytes; it is
+ * the caller's, so reserve it before a capture: a call with less fails (ESACB200_ERR_ARG) before enqueuing anything. */
+#define ESACB200_EXPERT_TENSORS 35
+#define ESACB200_EXPERTS_MAX 1024
+#define ESACB200_EXPERTS_MAX_SIDE 8192
+#define ESACB200_EXPERTS_MAX_PAIRS 65535
+/* Floats of the packed weights of E experts (-1: E outside [1, ESACB200_EXPERTS_MAX]). */
+int64_t esacb200_experts_packed_floats(int E);
+/* Workspace bytes of one forward (-1: sizes the forward rejects). */
+int64_t esacb200_experts_workspace_bytes(int B, int E, int H, int W);
+int esacb200_experts_pack(esacb200_ctx* ctx, int E, const float* const* params, float* packed);
+int esacb200_experts_forward_async(esacb200_ctx* ctx, int B, int E, int H, int W, const float* image, int image_batch,
+                                   const float* hist, const float* packed, void* workspace, int64_t workspace_bytes,
+                                   float* out);
+
 /* Device properties the bench needs without importing a CUDA binding: SM count and name. */
 int esacb200_device_info(esacb200_ctx* ctx, int* sm_count, char* name, int name_len);
 

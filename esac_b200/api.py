@@ -212,6 +212,14 @@ def load_library() -> C.CDLL:
     lib.esacb200_experts_pack.restype = i32
     lib.esacb200_experts_forward_async.argtypes = [vp, i32, i32, i32, i32, vp, i32, vp, vp, vp, i64, vp]
     lib.esacb200_experts_forward_async.restype = i32
+    lib.esacb200_gating_packed_floats.argtypes = [i32, i32]
+    lib.esacb200_gating_packed_floats.restype = i64
+    lib.esacb200_gating_workspace_bytes.argtypes = [i32, i32, i32, i32, i32]
+    lib.esacb200_gating_workspace_bytes.restype = i64
+    lib.esacb200_gating_pack.argtypes = [vp, i32, i32, vp, vp]
+    lib.esacb200_gating_pack.restype = i32
+    lib.esacb200_gating_forward_async.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, i64, vp, vp]
+    lib.esacb200_gating_forward_async.restype = i32
     for name in ("set_stream", "set_seed", "set_option", "inject_cells", "forward", "backward", "score_poses",
                  "refine_poses", "get_stats", "get_hypotheses", "device_info"):
         getattr(lib, "esacb200_" + name).restype = i32

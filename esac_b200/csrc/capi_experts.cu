@@ -49,6 +49,8 @@ int esacb200_experts_pack(esacb200_ctx* ctx, int E, const float* const* params, 
     }
     DevBuf staged;
     CK(staged.ensure((size_t)total * sizeof(float)));
+    // the padding between segments is never read, but the packed weights are one well-defined array: zero it
+    CK(cudaMemsetAsync(packed, 0, experts_packed_floats(E) * sizeof(float), ctx->stream));
     for (int l = 0; l < kExpertLayers; ++l) {
         const ExpertLayer d = expert_layer(l);
         for (int e = 0; e < E; ++e) {

@@ -12,6 +12,7 @@
 //   capi_render.cu      rendering ground-truth maps from an SfM reconstruction
 //   capi_data.cu        one step of a device-resident image set
 //   capi_experts.cu     inference of a stack of experts
+//   capi_gating_net.cu  inference of the gating network
 //   capi_testhooks.cu   include/esac_b200_testhooks.h
 #pragma once
 #include <cuda_runtime.h>

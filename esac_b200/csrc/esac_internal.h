@@ -910,8 +910,95 @@ struct ExpertsConvLayer {
 };
 // The active list, conv1, conv2 .. fc2 (15 implicit-GEMM launches), fc3: 18 launches on st.
 void launch_experts_forward(const ExpertsArgs& a, cudaStream_t st);
+// Its parts that the gating network runs too (with E = 1, its images as the pairs): the active list into a.ws_hdr, and one
+// implicit-GEMM convolution (k 1 or 3, stride 1 or 2; Cin a multiple of 32; offsets multiples of 4 floats) of every active
+// pair, reading the weights of expert e at L.w_off + e * Cout * k * k * Cin.
+void launch_experts_active(const ExpertsArgs& a, cudaStream_t st);
+void launch_experts_conv(const ExpertsArgs& a, const ExpertsConvLayer& L, int k, int stride, cudaStream_t st);
 // Layer l of E experts from `staged` (W at staged_w, b at staged_b, in torch's layouts, experts back to back) into `packed`.
 void launch_experts_pack(const float* staged, float* packed, int E, int l, long long staged_w, long long staged_b,
                          cudaStream_t st);
+
+// fp32 to TF32 (10 mantissa bits), to nearest with ties away from zero: how the tensor cores' operands are rounded.
+__device__ __forceinline__ uint32_t to_tf32(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return r;
+}
+
+// --- gating_net.cu ------------------------------------------------------------------------
+// The reference's Gating (code/gating.py) of capacity c (1 or 2) over E experts, layer l in state-dict order: conv1 ..
+// conv4, res1_conv1..3, fc1 .. fc3.  Packed weights, per layer W then b [Cout], each on a 64-float boundary:
+//   conv1 .. conv3        W [k][k][Cin][Cout] fp32 (the front end reads a tap's Cout weights as float4s)
+//   conv4, res1_conv1..3  W [Cout][k][k][Cin] TF32-rounded (experts_conv_kernel's layout)
+//   fc1 .. fc3            W [Cin][Cout] fp32 (the head's threads read one output each)
+constexpr int kGatingLayers = 10;
+struct GatingLayer {
+    int cin, cout, k, stride;
+    long long w_off, b_off;
+};
+inline GatingLayer gating_layer(int l, int E, int c) {
+    const int C = 64 * c, F = 64 * c * c;
+    const int t[kGatingLayers][4] = {{3, 8, 3, 1}, {8, 16, 3, 2}, {16, 32, 3, 2}, {32, C, 3, 2}, {C, C, 3, 1},
+                                     {C, C, 1, 1}, {C, C, 3, 1},  {C, F, 1, 1},   {F, F, 1, 1},  {F, E, 1, 1}};
+    long long off = 0;
+    GatingLayer d{};
+    for (int i = 0; i <= l; ++i) {
+        d = GatingLayer{t[i][0], t[i][1], t[i][2], t[i][3], off, 0};
+        off += ExpertLayer::round64((long long)d.cout * d.cin * d.k * d.k);
+        d.b_off = off;
+        off += ExpertLayer::round64(d.cout);
+    }
+    return d;
+}
+inline long long gating_packed_floats(int E, int c) {
+    const GatingLayer d = gating_layer(kGatingLayers - 1, E, c);
+    return d.b_off + ExpertLayer::round64(d.cout);
+}
+
+// One image's block of the workspace (floats): conv3's output a3 (NHWC, /4), the /8 activations x and y (NHWC, 64c
+// channels; conv4 -> x, res1_conv1 -> y, res1_conv2 -> x, res1_conv3 -> y), then the pool's partial sums, one row of 64c
+// per chunk of kGatingPoolPixels cells.  The header before the blocks is the experts' active list (experts_hdr_bytes(B)).
+constexpr int kGatingPoolPixels = 128;
+struct GatingShape {
+    int h[4], w[4];
+    int chunks;
+    long long a3, x, y, part, image_floats;
+};
+inline GatingShape gating_shape(int H, int W, int c) {
+    GatingShape s{};
+    s.h[0] = H;
+    s.w[0] = W;
+    for (int i = 1; i < 4; ++i) {
+        s.h[i] = (s.h[i - 1] + 1) / 2;
+        s.w[i] = (s.w[i - 1] + 1) / 2;
+    }
+    const long long p2 = (long long)s.h[2] * s.w[2], p3 = (long long)s.h[3] * s.w[3];
+    s.chunks = (int)((p3 + kGatingPoolPixels - 1) / kGatingPoolPixels);
+    auto r64 = ExpertLayer::round64;
+    s.a3 = 0;
+    s.x = r64(32 * p2);
+    s.y = s.x + r64(64LL * c * p3);
+    s.part = s.y + r64(64LL * c * p3);
+    s.image_floats = s.part + r64(64LL * c * s.chunks);
+    return s;
+}
+
+struct GatingArgs {
+    int B, E, c, H, W;
+    const float* image;   // [B,3,H,W]
+    const float* packed;  // gating_packed_floats(E, c)
+    int* ws_hdr;          // experts_hdr_bytes(B)
+    float* ws_images;     // B blocks of gating_shape(H, W, c).image_floats
+    float* out_log;       // [B,E]
+    float* out_prob;      // [B,E] or null
+    long long w_off[kGatingLayers], b_off[kGatingLayers];  // set by launch_gating_forward
+};
+// The active list, the front end (conv1 .. conv3), conv4 and res1_conv1..3 (experts_conv_kernel), the pool, the head:
+// eight launches on st.
+void launch_gating_forward(GatingArgs a, cudaStream_t st);
+// Layer l from `staged` (torch's [Cout][Cin][k][k] at staged_w, b at staged_b) into `packed`.
+void launch_gating_pack(const float* staged, float* packed, int E, int c, int l, long long staged_w, long long staged_b,
+                        cudaStream_t st);
 
 }  // namespace esacb200

@@ -19,12 +19,6 @@ namespace {
 constexpr int kBM = 128, kBN = 128, kBK = 32, kStages = 3, kConvThreads = 256;
 constexpr int kConvSmem = kStages * (kBM + kBN) * kBK * (int)sizeof(float);  // 96 KiB: two CTAs per SM
 
-__device__ __forceinline__ uint32_t to_tf32(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return r;
-}
-
 __device__ __forceinline__ void cp_async16(float* dst, const float* src, bool ok) {
     const uint32_t d = (uint32_t)__cvta_generic_to_shared(dst);
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(d), "l"(src), "r"(ok ? 16 : 0));
@@ -332,9 +326,17 @@ static void conv(const ExpertsArgs& a, const ExpertsConvLayer& L, cudaStream_t s
     experts_conv_kernel<KS, STRIDE><<<dim3(tiles, a.B * a.E), kConvThreads, kConvSmem, st>>>(a, L);
 }
 
+void launch_experts_active(const ExpertsArgs& a, cudaStream_t st) { experts_active_kernel<<<1, 1024, 0, st>>>(a); }
+
+void launch_experts_conv(const ExpertsArgs& a, const ExpertsConvLayer& L, int k, int stride, cudaStream_t st) {
+    if (k == 1) conv<1, 1>(a, L, st);
+    else if (stride == 2) conv<3, 2>(a, L, st);
+    else conv<3, 1>(a, L, st);
+}
+
 void launch_experts_forward(const ExpertsArgs& a, cudaStream_t st) {
     const ExpertsShape s = experts_shape(a.H, a.W);
-    experts_active_kernel<<<1, 1024, 0, st>>>(a);
+    launch_experts_active(a, st);
     experts_conv1_kernel<<<dim3((a.H * a.W + 255) / 256, a.B * a.E), 256, 0, st>>>(a);
     // the layer sequence of Expert.forward: (layer, input, output, residual or -1, ReLU)
     struct Step { int l; long long in, out, res; bool relu; };
@@ -361,9 +363,7 @@ void launch_experts_forward(const ExpertsArgs& a, cudaStream_t st) {
         L.relu = q.relu;
         L.w_off = d.w_off(a.E);
         L.b_off = d.b_off(a.E);
-        if (d.k == 1) conv<1, 1>(a, L, st);
-        else if (d.stride == 2) conv<3, 2>(a, L, st);
-        else conv<3, 1>(a, L, st);
+        launch_experts_conv(a, L, d.k, d.stride, st);
     }
     const ExpertLayer d = expert_layer(kExpertLayers - 1);
     ExpertsConvLayer L{};

@@ -41,23 +41,22 @@ def prediction_size(H: int, W: int) -> tuple:
     return -(-H // OUTPUT_SUBSAMPLE), -(-W // OUTPUT_SUBSAMPLE)
 
 
-def _check_state_dict(i: int, sd) -> list:
-    """The tensors of expert i in ABI order, as contiguous float32: exactly the keys of an Expert's state dict, with its
-    shapes."""
+def _check_state_dict(who: str, sd, want: dict, cls: str) -> list:
+    """The tensors of `who`'s state dict in ABI order, as contiguous float32: exactly the keys of a `cls` state dict with
+    the shapes `want` (key -> shape, in ABI order)."""
     import torch
-    want = state_dict_shapes()
     have = set(sd.keys())
     missing, extra = [k for k in want if k not in have], sorted(have - set(want))
     if missing or extra:
-        raise RuntimeError(f"expert {i}: state dict keys differ from Expert's (missing {missing}, unexpected {extra})")
+        raise RuntimeError(f"{who}: state dict keys differ from {cls}'s (missing {missing}, unexpected {extra})")
     out = []
     for k, shape in want.items():
         t = sd[k]
         if not isinstance(t, torch.Tensor) or not t.is_floating_point():
-            raise RuntimeError(f"expert {i}: {k} must be a floating-point tensor, got "
+            raise RuntimeError(f"{who}: {k} must be a floating-point tensor, got "
                                f"{t.dtype if isinstance(t, torch.Tensor) else type(t).__name__}")
         if tuple(t.shape) != shape:
-            raise RuntimeError(f"expert {i}: {k} must be {list(shape)}, got {list(t.shape)}")
+            raise RuntimeError(f"{who}: {k} must be {list(shape)}, got {list(t.shape)}")
         out.append(t.detach().to(torch.float32).contiguous())
     return out
 
@@ -72,7 +71,8 @@ class ExpertStack:
         E = len(state_dicts)
         if not 1 <= E <= api.MAX_EXPERTS:
             raise RuntimeError(f"ExpertStack: {E} experts, outside [1, {api.MAX_EXPERTS}]")
-        tensors = [t for i, sd in enumerate(state_dicts) for t in _check_state_dict(i, sd)]
+        tensors = [t for i, sd in enumerate(state_dicts)
+                   for t in _check_state_dict(f"expert {i}", sd, state_dict_shapes(), "Expert")]
         self.device = torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError(f"ExpertStack runs on a CUDA device, not {self.device}")

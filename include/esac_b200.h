@@ -776,6 +776,32 @@ int esacb200_experts_forward_async(esacb200_ctx* ctx, int B, int E, int H, int W
                                    const float* hist, const float* packed, void* workspace, int64_t workspace_bytes,
                                    float* out);
 
+/* ---- gating network: inference of the reference's Gating (code/gating.py) of capacity 1 or 2 over E experts ----------
+ * conv1 .. conv3 in fp32; conv4 and res1_conv1..3 on the tensor cores (TF32 operands, fp32 accumulation: the experts'
+ * kernel); tanh (capacity 1), the mean over the /8 map, fc1 .. fc3 and log_softmax in fp32.  No split-K and no atomics:
+ * image b's output is bitwise independent of the batch, of its place in it and of the run.
+ *
+ * esacb200_gating_pack: params is a host array of ESACB200_GATING_TENSORS pointers (host or device memory, float32,
+ * contiguous) in the order conv1.weight, conv1.bias, ..., conv4.bias, res1_conv1.weight, ..., res1_conv3.bias, fc1.weight,
+ * ..., fc3.bias -- the layers of Gating.__init__ with torch's shapes (64 * capacity channels at /8, 64 * capacity^2 in fc1
+ * and fc2, E out of fc3).  packed: device, esacb200_gating_packed_floats(E, capacity) floats (16-byte aligned).
+ * Synchronous.
+ *
+ * esacb200_gating_forward_async: image float32 [B,3,H,W]; out_log_probs float32 [B,E] (Gating.forward's output);
+ * out_probs float32 [B,E] = exp(out_log_probs), what esacb200_assign_hypotheses_async takes, or NULL.  Enqueued on the
+ * context's stream with no host synchronisation (capturable); every argument is checked before anything is enqueued.
+ * workspace: device, 256-byte aligned, at least esacb200_gating_workspace_bytes(B, E, capacity, H, W) bytes, the caller's. */
+#define ESACB200_GATING_TENSORS 20
+/* Floats of the packed weights (-1: E outside [1, ESACB200_EXPERTS_MAX] or capacity not 1 or 2). */
+int64_t esacb200_gating_packed_floats(int E, int capacity);
+/* Workspace bytes of one forward (-1: sizes the forward rejects: B above ESACB200_EXPERTS_MAX_PAIRS, sides above
+ * ESACB200_EXPERTS_MAX_SIDE). */
+int64_t esacb200_gating_workspace_bytes(int B, int E, int capacity, int H, int W);
+int esacb200_gating_pack(esacb200_ctx* ctx, int E, int capacity, const float* const* params, float* packed);
+int esacb200_gating_forward_async(esacb200_ctx* ctx, int B, int E, int capacity, int H, int W, const float* image,
+                                  const float* packed, void* workspace, int64_t workspace_bytes, float* out_log_probs,
+                                  float* out_probs);
+
 /* Device properties the bench needs without importing a CUDA binding: SM count and name. */
 int esacb200_device_info(esacb200_ctx* ctx, int* sm_count, char* name, int name_len);
 

@@ -38,6 +38,7 @@ import esac_b200.api as esac_api  # noqa: E402
 from esac_b200.autograd import esac_loss, esac_loss_async  # noqa: E402
 from esac_b200.compat import OUTPUT_SUBSAMPLE, random_shift  # noqa: E402
 from esac_b200.gate import ExpertGate  # noqa: E402
+from esac_b200.networks import init_adam_state  # noqa: E402
 from test_step_graph_synthetic import PerImageFocalDataset  # noqa: E402
 from train_step_synthetic import TinyExpert, TinyGating  # noqa: E402
 
@@ -60,18 +61,6 @@ def parse(argv=None):
     ap.add_argument("--losscut", type=float, default=100.0)
     ap.add_argument("--check", action="store_true", help="train an eager twin beside the graph and compare, bitwise")
     return ap.parse_args(argv)
-
-
-def init_adam_state(opt):
-    """The state torch.optim.Adam(capturable=True) creates at its first step, created now: zero moments, step 0 on the
-    parameter's device."""
-    for group in opt.param_groups:
-        for p in group["params"]:
-            st = opt.state[p]
-            if not st:
-                st["step"] = torch.zeros((), dtype=torch.float32, device=p.device)
-                st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
-                st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
 
 
 class AlwaysGate:

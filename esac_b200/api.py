@@ -256,6 +256,9 @@ def load_library() -> C.CDLL:
     lib.esacb200_host_draw_cells.restype = None
     lib.esacb200_graph_node_types.argtypes = [vp, vp, i32]
     lib.esacb200_graph_node_types.restype = i32
+    lib.esacb200_test_experts_conv.argtypes = [vp, i32, i32, vp, vp, i64, i64, i32, i32, i32, i32, i32, i32, i32, vp, i64,
+                                               i64, i64, i64, vp]
+    lib.esacb200_test_experts_conv.restype = i32
     _lib = lib
     return lib
 

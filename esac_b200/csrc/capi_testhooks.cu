@@ -1,12 +1,14 @@
-// The host test hooks of include/esac_b200_testhooks.h: single geometry primitives of the kernels, run on the CPU.
+// The test hooks of include/esac_b200_testhooks.h: single geometry primitives of the kernels, run on the CPU, and one
+// layer of the expert stack's convolution on the device.
 #include "../../include/esac_b200_testhooks.h"
-#include "esac_internal.h"
+#include "capi_internal.h"
 #include "esac_p3p_fast.cuh"
 #include "esac_rng.cuh"
 
 #include <vector>
 
 using namespace esacb200;
+using namespace esacb200::capi;
 
 extern "C" {
 
@@ -157,6 +159,66 @@ int esacb200_graph_node_types(void* graph, int* types, int cap) {
         types[i] = t;
     }
     return (int)n;
+}
+
+int esacb200_test_experts_conv(esacb200_ctx* ctx, int B, int E, const float* hist, const float* packed, int64_t w_off,
+                               int64_t b_off, int k, int stride, int cin, int cout, int hin, int win, int relu, float* pairs,
+                               int64_t pair_floats, int64_t in_off, int64_t out_off, int64_t res_off, int* hdr) {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    const char* what = "test_experts_conv";
+    if (B < 1 || E < 1 || E > ESACB200_EXPERTS_MAX || (long long)B * E > ESACB200_EXPERTS_MAX_PAIRS)
+        return fail(ctx, ESACB200_ERR_ARG, "%s: B=%d E=%d: need E <= %d and B * E <= %d", what, B, E, ESACB200_EXPERTS_MAX,
+                    ESACB200_EXPERTS_MAX_PAIRS);
+    if ((k != 1 && k != 3) || (stride != 1 && stride != 2) || (k == 1 && stride == 2))
+        return fail(ctx, ESACB200_ERR_ARG, "%s: k=%d stride=%d: need k 1 or 3, stride 1 or 2, and stride 1 for k 1", what, k,
+                    stride);
+    if (cin < 32 || cin % 32 || cout < 2 || cout % 2 || hin < 1 || win < 1 || hin > ESACB200_EXPERTS_MAX_SIDE ||
+        win > ESACB200_EXPERTS_MAX_SIDE)
+        return fail(ctx, ESACB200_ERR_ARG, "%s: cin=%d cout=%d at %dx%d: need cin a multiple of 32, cout even, sides in [1, %d]",
+                    what, cin, cout, hin, win, ESACB200_EXPERTS_MAX_SIDE);
+    const int hout = (hin + stride - 1) / stride, wout = (win + stride - 1) / stride;
+    const long long in_n = (long long)hin * win * cin, out_n = (long long)hout * wout * cout;
+    if (w_off < 0 || b_off < 0 || in_off < 0 || out_off < 0 || res_off < -1 || pair_floats < 1 || w_off % 4 || b_off % 4 ||
+        in_off % 4 || out_off % 4 || (res_off >= 0 && res_off % 4) || pair_floats % 4)
+        return fail(ctx, ESACB200_ERR_ARG, "%s: offsets and pair_floats must be non-negative multiples of 4 (res_off may be -1)",
+                    what);
+    if (in_off + in_n > pair_floats || out_off + out_n > pair_floats || (res_off >= 0 && res_off + out_n > pair_floats))
+        return fail(ctx, ESACB200_ERR_ARG, "%s: a region runs past the pair's block of %lld floats", what, (long long)pair_floats);
+    const void* ptrs[] = {packed, pairs, hdr, hist};
+    const char* names[] = {"packed", "pairs", "hdr", "hist"};
+    const int rc = device_args(ctx, what, 4, ptrs, names, 1u << 3);
+    if (rc) return rc;
+    if ((uintptr_t)packed % 16 || (uintptr_t)pairs % 16 || (uintptr_t)hdr % 4 || (uintptr_t)hist % 4)
+        return fail(ctx, ESACB200_ERR_ARG, "%s: packed and pairs must be 16-byte, hdr and hist 4-byte aligned", what);
+    ExpertsArgs a{};
+    a.B = B;
+    a.E = E;
+    a.H = hin;
+    a.W = win;
+    a.hist = hist;
+    a.packed = packed;
+    a.ws_hdr = hdr;
+    a.ws_pairs = pairs;
+    a.pair_floats = pair_floats;
+    ExpertsConvLayer L{};
+    L.cin = cin;
+    L.cout = cout;
+    L.hin = hin;
+    L.win = win;
+    L.hout = hout;
+    L.wout = wout;
+    L.in_off = in_off;
+    L.out_off = out_off;
+    L.res_off = res_off;
+    L.w_off = w_off;
+    L.b_off = b_off;
+    L.relu = relu != 0;
+    launch_experts_active(a, ctx->stream);
+    CK(cudaGetLastError());
+    launch_experts_conv(a, L, k, stride, ctx->stream);
+    CK(cudaGetLastError());
+    return ESACB200_OK;
 }
 
 }  // extern "C"

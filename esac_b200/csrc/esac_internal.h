@@ -911,8 +911,9 @@ struct ExpertsConvLayer {
 // The active list, conv1, conv2 .. fc2 (15 implicit-GEMM launches), fc3: 18 launches on st.
 void launch_experts_forward(const ExpertsArgs& a, cudaStream_t st);
 // Its parts that the gating network runs too (with E = 1, its images as the pairs): the active list into a.ws_hdr, and one
-// implicit-GEMM convolution (k 1 or 3, stride 1 or 2; Cin a multiple of 32; offsets multiples of 4 floats) of every active
-// pair, reading the weights of expert e at L.w_off + e * Cout * k * k * Cin.
+// implicit-GEMM convolution (k 1 or 3, stride 1 or 2; Cin a multiple of 32; Cout even, since the epilogue stores and reads
+// the bias and residual as float2 pairs; offsets multiples of 4 floats) of every active pair, reading the weights of expert e
+// at L.w_off + e * Cout * k * k * Cin.
 void launch_experts_active(const ExpertsArgs& a, cudaStream_t st);
 void launch_experts_conv(const ExpertsArgs& a, const ExpertsConvLayer& L, int k, int stride, cudaStream_t st);
 // Layer l of E experts from `staged` (W at staged_w, b at staged_b, in torch's layouts, experts back to back) into `packed`.

@@ -1,8 +1,10 @@
-/* Host-side test hooks of libesac_b200.so.
+/* Test hooks of libesac_b200.so.
  *
- * These run single geometry primitives of esac_b200/csrc/esac_geom.cuh / esac_rng.cuh -- the very
- * functions the CUDA kernels call -- on the CPU, so the `-m "not gpu"` tests can check them against
- * OpenCV without a GPU.  They are NOT a CPU fallback: no forward/backward pipeline exists on the host.
+ * The esacb200_host_* hooks run single geometry primitives of esac_b200/csrc/esac_geom.cuh / esac_rng.cuh -- the very
+ * functions the CUDA kernels call -- on the CPU, so the `-m "not gpu"` tests can check them against OpenCV without a
+ * GPU.  They are NOT a CPU fallback: no forward/backward pipeline exists on the host.  esacb200_test_experts_conv runs
+ * one layer of the expert stack's device kernels on caller-owned device buffers, so a test can hold that layer alone
+ * to a reference.
  */
 #ifndef ESAC_B200_TESTHOOKS_H
 #define ESAC_B200_TESTHOOKS_H
@@ -59,6 +61,20 @@ void esacb200_host_draw_cells(uint64_t seed, uint32_t h, uint32_t t, int W, int 
 /* The node types (cudaGraphNodeType values) of a CUDA graph's top level, through the runtime the library uses: writes up
  * to `cap` of them to `types` and returns the node count, or -1 if the runtime refuses the graph. */
 int esacb200_graph_node_types(void* graph, int* types, int cap);
+
+struct esacb200_ctx;
+/* On the device, on the context's stream, without a host synchronisation: the expert stack's active list of B * E pairs
+ * from hist [B,E] (NULL: every pair) into hdr, then one implicit-GEMM convolution of every active pair p = b * E + e
+ * (experts_conv_kernel, as ExpertStack and GatingNet run it).  Pair p's block is pairs + p * pair_floats: its NHWC input
+ * [hin][win][cin] at in_off, its output [hout][wout][cout] at out_off, and the residual added after the ReLU at res_off
+ * (-1: none; res_off == out_off: in place).  Expert e's weights [cout][k][k][cin] are packed + w_off + e * cout * k * k
+ * * cin, its biases packed + b_off + e * cout.  hout, wout = ceil(hin / stride), ceil(win / stride).  hdr holds
+ * 16 + 2 * B * E ints: the active count, the ascending active list, then B * E flags.  The kernel's contract: k 1 or 3,
+ * stride 1 or 2 (not k 1 with stride 2), cin a multiple of 32, cout even, every offset and pair_floats a multiple of 4,
+ * the regions inside a block, packed and pairs 16-byte aligned.  Anything else is refused with ESACB200_ERR_ARG. */
+int esacb200_test_experts_conv(struct esacb200_ctx* ctx, int B, int E, const float* hist, const float* packed, int64_t w_off,
+                               int64_t b_off, int k, int stride, int cin, int cout, int hin, int win, int relu, float* pairs,
+                               int64_t pair_floats, int64_t in_off, int64_t out_off, int64_t res_off, int* hdr);
 
 #ifdef __cplusplus
 }

@@ -53,6 +53,142 @@ def tf32(a: np.ndarray) -> np.ndarray:
     return ((u + np.uint32(0x1000)) & np.uint32(0xFFFFE000)).view(np.float32)
 
 
+def tf32_rz(a: np.ndarray) -> np.ndarray:
+    """float32 values truncated to TF32 (round toward zero): what the tensor cores read from fp32 bits left unrounded."""
+    u = np.ascontiguousarray(a, np.float32).view(np.uint32)
+    return (u & np.uint32(0xFFFFE000)).view(np.float32)
+
+
+def tf32_rne(a: np.ndarray) -> np.ndarray:
+    """float32 values rounded to TF32 to nearest, ties to even; finite inputs."""
+    u = np.ascontiguousarray(a, np.float32).view(np.uint32)
+    odd = (u >> np.uint32(13)) & np.uint32(1)
+    return ((u + np.uint32(0xFFF) + odd) & np.uint32(0xFFFFE000)).view(np.float32)
+
+
+def tf32_none(a: np.ndarray) -> np.ndarray:
+    """float32 values as they are: full fp32 operands."""
+    return np.ascontiguousarray(a, np.float32).copy()
+
+
+# The operand roundings a tensor-core layer could apply to its fp32 activations; the kernels use "rna".
+ROUNDINGS = {"rna": tf32, "rz": tf32_rz, "rne": tf32_rne, "none": tf32_none}
+
+
+def conv_nhwc(x, w, b, stride: int, relu: bool = True, res=None):
+    """One layer of the stack in float64: res + ReLU(conv(x, w) + b), with zero padding k // 2.  x [..., H, W, Cin]
+    (NHWC, leading axes are images), w [Cout, k, k, Cin] (the packed layout of one expert), b [Cout] or None, res
+    [..., Hout, Wout, Cout] or None.  numpy in, numpy out; torch tensors stay on their device."""
+    import torch
+    import torch.nn.functional as F
+    as_np = not isinstance(x, torch.Tensor)
+    t = lambda v: torch.as_tensor(np.asarray(v) if not isinstance(v, torch.Tensor) else v).to(torch.float64)
+    xt = t(x)
+    dev = xt.device
+    lead = xt.shape[:-3]
+    wt = t(w).to(dev).permute(0, 3, 1, 2)
+    k = int(wt.shape[-1])
+    xin = xt.reshape((-1,) + tuple(xt.shape[-3:])).permute(0, 3, 1, 2)
+    y = F.conv2d(xin, wt, None if b is None else t(b).to(dev), stride=stride, padding=k // 2).permute(0, 2, 3, 1)
+    y = y.reshape(tuple(lead) + tuple(y.shape[1:]))
+    if relu:
+        y = torch.relu(y)
+    if res is not None:
+        y = y + t(res).to(dev)
+    return y.cpu().numpy() if as_np else y
+
+
+def accumulation_bound(absx, absw, absb, stride: int, unit: float, absres=None):
+    """Worst-case error of one layer's fp32 output, elementwise, given exact operands x~ (what the layer multiplies: TF32
+    values for the tensor cores, fp32 ones for the FMA kernels) and float64 arithmetic for the reference:
+
+        |fl(res + ReLU(sum_k w_k x~_k + b)) - (res + ReLU(sum_k w_k x~_k + b))|
+            <= 2 (K + 2) unit (sum_k |w_k| |x~_k| + |b| + |res|).
+
+    Derivation.  A product of two TF32 values has at most 22 significant bits, so the tensor cores form it exactly; an
+    FMA rounds once per step.  Summing K terms in any order (any tree, any grouping into MMA k-steps) with a relative
+    error of at most `unit` per addition is off by at most gamma_K * sum|terms| (Higham, Accuracy and Stability of
+    Numerical Algorithms, eq. 4.4), gamma_K = K unit / (1 - K unit) <= 2 K unit while K unit <= 1/2.  Adding the bias
+    and then the residual are two more roundings, each at most `unit` times |sum| + |b| + |res|.  ReLU is 1-Lipschitz.
+    `unit` is 2^-24 for round-to-nearest fp32 (the FMA kernels) and 2^-23 for the tensor cores, whose adds are allowed
+    to truncate.  The bound holds for any accumulation order, so it cannot fail on a correct kernel; it is loose (a
+    random-sign sum errs about sqrt(K) unit), which makes it a check of wiring -- offsets, operands, residual targets
+    -- not of rounding.  absx |x~| NHWC, absw |w| [Cout, k, k, Cin], absb |b| or None, absres |res| or None."""
+    K = int(np.prod(absw.shape[1:]))
+    assert K * unit <= 0.5
+    return 2 * (K + 2) * unit * conv_nhwc(absx, absw, absb, stride, relu=False, res=absres)
+
+
+def bounded_layer(x, w, b, stride: int, relu: bool = True, res=None, unit: float = 2.0 ** -23, rounding=tf32):
+    """One layer on the device's own input x (fp32 NHWC, numpy or torch): (float64 reference, elementwise bound) of its
+    fp32 output.  The reference multiplies rounding(x) -- the operand the tensor cores read; pass tf32_none and
+    unit 2^-24 for the FMA kernels -- by w [Cout, k, k, Cin] as packed, adds b, applies the ReLU and adds res; the bound is
+    accumulation_bound's."""
+    import torch
+    if isinstance(x, torch.Tensor):
+        xr = _tf32_torch(x, rounding).to(torch.float64)
+        w, b = torch.as_tensor(w).to(x.device), None if b is None else torch.as_tensor(b).to(x.device)
+        res = None if res is None else torch.as_tensor(res).to(x.device)
+    else:
+        xr = rounding(np.asarray(x, np.float32)).astype(np.float64)
+    val = conv_nhwc(xr, w, b, stride, relu=relu, res=res)
+    bnd = accumulation_bound(abs(xr), abs(w), None if b is None else abs(b), stride, unit, None if res is None else abs(res))
+    return val, bnd
+
+
+def _tf32_torch(x, rounding):
+    """rounding (tf32, tf32_rz, tf32_rne or tf32_none) on a float32 torch tensor, on its device."""
+    import torch
+    u = x.to(torch.float32).contiguous().view(torch.int32)
+    mask = torch.tensor(-8192, dtype=torch.int32, device=x.device)  # 0xFFFFE000
+    if rounding is tf32:
+        u = (u + 0x1000) & mask
+    elif rounding is tf32_rz:
+        u = u & mask
+    elif rounding is tf32_rne:
+        u = (u + 0xFFF + ((u >> 13) & 1)) & mask
+    elif rounding is not tf32_none:
+        raise ValueError(rounding)
+    return u.view(torch.float32)
+
+
+def _np(a):
+    return a.detach().cpu().numpy() if hasattr(a, "detach") else np.asarray(a)
+
+
+def lattice_mismatches(got, ref64) -> int:
+    """Elements of a float32 result that are not bitwise the float64 reference cast to float32."""
+    want = np.asarray(_np(ref64), np.float64).astype(np.float32)
+    return int(np.count_nonzero(np.asarray(_np(got), np.float32).view(np.uint32) != want.view(np.uint32)))
+
+
+def bound_violations(got, ref, bound) -> int:
+    """Elements farther from the reference than their bound (a NaN counts)."""
+    d = np.abs(np.asarray(_np(got), np.float64) - np.asarray(_np(ref), np.float64))
+    return int(np.count_nonzero(~(d <= _np(bound))))
+
+
+def workspace_layout(B: int, E: int, H: int, W: int) -> dict:
+    """esacb200_experts_workspace_bytes's layout, restated: the int header's bytes (active count, ascending list of b*E+e,
+    B*E flags), then B*E blocks of pair_floats floats; per block the NHWC activations' float offsets (a0 and a2 share
+    offset 0), the sides h, w of the four resolutions and the total bytes."""
+    h, w = [H], [W]
+    for _ in range(3):
+        h.append((h[-1] + 1) // 2)
+        w.append((w[-1] + 1) // 2)
+    p = [h[i] * w[i] for i in range(4)]
+    r64 = _round
+    a1 = r64(max(32 * p[0], 128 * p[2]))
+    r = a1 + r64(64 * p[1])
+    s_ = r + r64(256 * p[3])
+    x = s_ + r64(512 * p[3])
+    y = x + r64(512 * p[3])
+    pair = y + r64(512 * p[3])
+    hdr = r64(16 + 2 * B * E) * 4
+    return dict(h=h, w=w, hdr_bytes=hdr, a0=0, a1=a1, a2=0, r=r, s=s_, x=x, y=y, pair_floats=pair,
+                total_bytes=hdr + B * E * pair * 4)
+
+
 def _round(n: int) -> int:
     return -(-n // ALIGN) * ALIGN
 

@@ -145,3 +145,81 @@ def unpack(packed: np.ndarray, E: int, capacity: int) -> dict:
         sd[name + ".weight"] = np.ascontiguousarray(w)
         sd[name + ".bias"] = packed[b_off: b_off + cout].copy()
     return sd
+
+
+POOL_CELLS = 128  # cells of the /8 map per pool chunk
+
+
+def workspace_layout(B: int, H: int, W: int, c: int) -> dict:
+    """esacb200_gating_workspace_bytes's layout, restated: the experts' int header for B images (no expert axis), then B
+    blocks of image_floats floats; per block the float offsets of conv3's NHWC output a3 (/4, 32 channels), the /8 maps
+    x and y (64c channels) and the pool's partial sums (one row of 64c per chunk of POOL_CELLS cells), the sides h, w,
+    the chunk count and the total bytes."""
+    h, w = [H], [W]
+    for _ in range(3):
+        h.append((h[-1] + 1) // 2)
+        w.append((w[-1] + 1) // 2)
+    p2, p3 = h[2] * w[2], h[3] * w[3]
+    chunks = -(-p3 // POOL_CELLS)
+    x = _round(32 * p2)
+    y = x + _round(64 * c * p3)
+    part = y + _round(64 * c * p3)
+    image = part + _round(64 * c * chunks)
+    hdr = _round(16 + 2 * B) * 4
+    return dict(h=h, w=w, chunks=chunks, hdr_bytes=hdr, a3=0, x=x, y=y, part=part, image_floats=image,
+                total_bytes=hdr + B * image * 4)
+
+
+def pool_partials(y: np.ndarray, capacity: int, cells=None) -> np.ndarray:
+    """The pool's partial sums in float64: [chunks, 64c] from the /8 map y [P, 64c] (NHWC cells in row order), tanh first
+    at capacity 1.  cells: the chunk boundaries (default: every POOL_CELLS cells)."""
+    t = np.tanh(np.asarray(y, np.float64)) if capacity == 1 else np.asarray(y, np.float64)
+    P = t.shape[0]
+    edges = list(range(0, P, POOL_CELLS)) + [P] if cells is None else list(cells)
+    return np.stack([t[a:b].sum(0) for a, b in zip(edges[:-1], edges[1:])])
+
+
+def pool_bound(y: np.ndarray, capacity: int) -> np.ndarray:
+    """Worst-case error of the fp32 partial sums: a chunk of n cells is a sum of n terms in some order (gamma_n, see
+    expert_oracle.accumulation_bound) of values that tanhf gives to within 2 ulp, so
+    2 (n + 4) 2^-24 sum|t| per channel, with n = POOL_CELLS."""
+    a = np.abs(np.tanh(np.asarray(y, np.float64)) if capacity == 1 else np.asarray(y, np.float64))
+    return 2 * (POOL_CELLS + 4) * 2.0 ** -24 * pool_partials(a, 2)
+
+
+def head(part: np.ndarray, cells: int, sd) -> tuple:
+    """The head in float64 from the partial sums part [chunks, 64c]: (log-probabilities [E], the logits z [E])."""
+    p = {k: np.asarray(v, np.float64) for k, v in sd.items()}
+    v = part.sum(0) / cells
+    v = np.maximum(p["fc1.weight"][:, :, 0, 0] @ v + p["fc1.bias"], 0)
+    v = np.maximum(p["fc2.weight"][:, :, 0, 0] @ v + p["fc2.bias"], 0)
+    z = p["fc3.weight"][:, :, 0, 0] @ v + p["fc3.bias"]
+    m = z.max()
+    return z - m - np.log(np.exp(z - m).sum()), z
+
+
+def head_bound(part: np.ndarray, cells: int, sd) -> tuple:
+    """Worst-case error of the head's fp32 log-probabilities and probabilities, elementwise, from exact partial sums.
+    The mean is a sum of `chunks` terms and a division (gamma_{chunks+1}); fc1 .. fc3 are FMA chains, each bounded as in
+    expert_oracle.accumulation_bound (unit 2^-24) plus |W| times the input's bound.  log_softmax: the logits' errors dz
+    move z_e - lse(z) by at most dz_e + max dz (lse is 1-Lipschitz in the max norm); the kernel's own roundings are z - m
+    (2^-24 |z - m|), expf (2 ulp), the sum of E terms (gamma_E), logf (1 ulp of lse) and the final subtraction, all
+    counted twice.  The probabilities are expf(log p): p (expm1(d) + 2^-22), d the log bound."""
+    u = 2.0 ** -24
+    p = {k: np.asarray(v, np.float64) for k, v in sd.items()}
+    n = part.shape[0]
+    v = part.sum(0) / cells
+    e = 2 * (n + 2) * u * np.abs(part).sum(0) / cells
+    for name in ("fc1", "fc2", "fc3"):
+        Wt, b = p[name + ".weight"][:, :, 0, 0], p[name + ".bias"]
+        K = Wt.shape[1]
+        z = Wt @ v + b
+        e = np.abs(Wt) @ e + 2 * (K + 2) * u * (np.abs(Wt) @ (np.abs(v) + e) + np.abs(b))
+        v = np.maximum(z, 0) if name != "fc3" else z
+    E = v.shape[0]
+    m = v.max()
+    lse = np.log(np.exp(v - m).sum())
+    lp = v - m - lse
+    own = 2 * (u * np.abs(v - m) + 2 * (E + 2) * 2 * u + u * abs(lse) + u * np.abs(v - m).max() + u * np.abs(lp))
+    d = e + e.max() + own
+    return d, np.exp(lp) * (np.expm1(d) + 4 * u)

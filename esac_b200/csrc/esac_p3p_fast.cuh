@@ -132,8 +132,19 @@ ESAC_HD void fast_line_conic(P l0, P l1, P l2, P d00, P d01, P d02, P d11, P d12
 // 4th-point error band, in units of tau, inside which the exact path decides.  It covers the float error of a
 // well-conditioned P3P only: near the danger cylinder a float root can miss the 4th point by many tau (no margin up to
 // 16 tau was enough there), so those tries are sent to the exact path by the uncertainty latches above and below instead
-// (tests/test_host_minimal_sets.py).
+// (tests/test_host_minimal_sets.py).  The float error of the 4th point is in absolute pixels, though, not in units of tau:
+// on make_scene's maps the host compile's float 4th point missed the exact one by up to 0.76 px among accepted tries (at
+// tau = 0.5 a try whose exact 4th point is 0.45 px off needed a band of 1.21 px; at tau = 0.05 on a world-offset map,
+// 0.37 px), so below tau ~ 0.6 px a band of 2 tau threw away tries the exact path accepts.  The device compile (MUFU
+// approximations, its own FMA contraction) errs differently but as much: on an H100, injected sub-pixel tries (about 40k
+// accepted random true-expert draws and 12k accepted crafted sets at tau 0.05 - 1) lost 5 accepted tries with 2 tau
+// alone, 1 with a floor of 1 px and none with 2 px.  The band is therefore max(kPrefilterMargin tau, kPrefilterFloorPx):
+// the floor is twice the smallest one that held on the device and about five times the largest host discrepancy, and it
+// is at or below 2 tau for every tau >= 2 px, so at the default tau = 10 the prefilter's verdicts are unchanged
+// (tests/test_host_thresholds.py, tests/test_gpu_thresholds.py).  Below tau = 2 px the exact path judges the tries within
+// 4 px, as many as at tau = 2.
 constexpr float kPrefilterMargin = 2.f;
+constexpr float kPrefilterFloorPx = 4.f;
 constexpr float kPrefilterNeedle = 0.02f;  // shortest / longest squared side below which the triangle goes to the exact path
 
 // obj[i][c] / img[i][c]: point i, coordinate c, of the W tries of the pack.  Returns, per try, false only when the try
@@ -279,7 +290,7 @@ ESAC_HD typename MaskOf<P>::type p3p_may_pass_pack(const P obj[4][3], const P im
     const P idet = rcp_(det);
     const P al = (v1 * a13 - v2 * g12) * idet, be = (v2 * a12 - v1 * g12) * idet;
     const P ga = (x3[0] * nrm[0] + x3[1] * nrm[1] + x3[2] * nrm[2]) * rcp_(nn);
-    const float lim = margin * tau, hlim = hint_frac * tau;
+    const float lim = fmaxf(margin * tau, kPrefilterFloorPx), hlim = hint_frac * tau;
     const P lim2 = bc<P>(lim * lim), hlim2 = bc<P>(hlim * hlim);
     const P sa = sqrt_(amax);
     const P vf = bc<P>(f);

@@ -10,6 +10,7 @@ the CUDA path and compares; tests/test_oracle.py checks the oracle against them 
 
 Needs a checkout of vislearn/esac named by $ESAC_REFERENCE.  Run:  python tests/golden/make_ref_golden.py [name ...]
 """
+import dataclasses
 import sys
 import time
 from pathlib import Path
@@ -45,6 +46,20 @@ SMALL = {
     "ref_flip_x_30x40": dict(E=2, H=30, W=40, M=32, sub=8, seed=1, rotation=(3.141592653589793, 0.0, 0.0)),
     "ref_near_pi_30x40": dict(E=2, H=30, W=40, M=32, sub=8, seed=1, rotation=NEAR_PI_RVEC),
 }
+# away from the reference's default hyperparameters: (tau, beta, maxReproj) over the scene's and the loss arguments
+PARAMS = {
+    # beta 2 keeps the scoring kernel's per-cell form (tmax > 63), lossCut 5 sends most hypotheses to sqrt(cut * loss)
+    "ref_params_tight_30x40": (dict(E=2, H=30, W=40, M=24, sub=8, seed=81, noise=0.005, alpha=50.0),
+                               dict(tau=2.0, beta=2.0), (0.5, 30.0, 5.0)),
+    # tau above maxReproj: every clamped cell is an inlier of the refinement (few outliers, so that fitting all cells stays
+    # well-conditioned)
+    "ref_params_clamp_30x40": (dict(E=2, H=30, W=40, M=24, sub=8, seed=82, outlier_frac=0.02, alpha=400.0),
+                               dict(tau=40.0, beta=0.1, max_reproj=30.0), (1.0, 100.0, 100.0)),
+    # a sub-pixel threshold on a low-noise map, every hypothesis on the true expert
+    "ref_params_subpx_24x32": (dict(E=2, H=24, W=32, M=24, sub=8, seed=83, noise=5e-4, outlier_frac=0.2, gt_mass=1.0),
+                               dict(tau=0.6), (1.0, 100.0, 100.0)),
+}
+SMALL.update({name: kw for name, (kw, _, _) in PARAMS.items()})
 LARGE = {
     "ref_mid_4x120x160": dict(E=4, H=120, W=160, M=48, sub=4, seed=45),
     "ref_full_7x480x640": dict(E=7, H=480, W=640, M=32, sub=1, seed=46, active_only=False),       # BASELINE configs[1] shape
@@ -86,7 +101,16 @@ def tried_sets(sc, seed=1305):
     return cells, tries
 
 
-def run_reference(R, sc):
+def scene(name, kw):
+    """make_scene(**kw) with the fixture's own tau, beta and maxReproj, and its loss arguments."""
+    sc = make_scene(**kw)
+    if name not in PARAMS:
+        return sc, LOSS_ARGS
+    _, over, loss_args = PARAMS[name]
+    return dataclasses.replace(sc, **over), loss_args
+
+
+def run_reference(R, sc, loss_args):
     co, asg = torch.from_numpy(sc.coords), torch.from_numpy(sc.assign)
     R.force_init(1305)
     pose = torch.zeros(4, 4)
@@ -95,7 +119,7 @@ def run_reference(R, sc):
     t1 = time.time()
     R.force_init(1305)
     g = torch.zeros(sc.coords.shape)
-    loss = R.backward(co, g, asg, torch.from_numpy(sc.gt_pose), *LOSS_ARGS, *sc.params)
+    loss = R.backward(co, g, asg, torch.from_numpy(sc.gt_pose), *loss_args, *sc.params)
     t2 = time.time()
     return e, pose.numpy(), loss, g.numpy(), (t1 - t0, t2 - t1)
 
@@ -110,9 +134,9 @@ if __name__ == "__main__":
     for name, kw in {**SMALL, **LARGE}.items():
         if want and name not in want:
             continue
-        sc = make_scene(**kw)
+        sc, loss_args = scene(name, kw)
         cells, tries = tried_sets(sc)
-        e, pose, loss, g, dt = run_reference(R, sc)
+        e, pose, loss, g, dt = run_reference(R, sc, loss_args)
         # auxiliary: the oracle's per-hypothesis view of the same run (the reference does not expose scores); the
         # generator refuses to write a fixture on which oracle and reference disagree
         o_pose = np.zeros((4, 4), np.float32)
@@ -122,17 +146,17 @@ if __name__ == "__main__":
         assert top[0] - top[1] > 1e-2, f"{name}: near-tie at the top ({top[0] - top[1]:.2e}) -- pick another seed"
         # which hypotheses trip the two clamps, and how far the gradient would move without them (oracle view)
         g_o = np.zeros_like(sc.coords)
-        _, bt = O.backward(sc.coords, g_o, sc.assign, sc.gt_pose, *LOSS_ARGS, *sc.params, mt=O.ThreadRandStream(1305), trace=True)
+        _, bt = O.backward(sc.coords, g_o, sc.assign, sc.gt_pose, *loss_args, *sc.params, mt=O.ThreadRandStream(1305), trace=True)
         extra = {}
         if name.startswith("ref_clamp"):
             g_u = np.zeros_like(sc.coords)
-            O.backward(sc.coords, g_u, sc.assign, sc.gt_pose, *LOSS_ARGS, *sc.params, mt=O.ThreadRandStream(1305),
+            O.backward(sc.coords, g_u, sc.assign, sc.gt_pose, *loss_args, *sc.params, mt=O.ThreadRandStream(1305),
                        clamp_thresh=np.inf)
             extra = dict(clamped_jr=np.array(bt.clamped_jr, np.int32), clamped_dpnp=np.array(bt.clamped_dpnp, np.int32),
                          unclamped_grad_diff=float(np.abs(g_u - g_o).max()))
             print(f"  clamps: J_R {bt.clamped_jr}, dPNP {bt.clamped_dpnp}, |g(no clamp) - g| max {extra['unclamped_grad_diff']:.3g}")
         common = dict(**extra, scene_kw=np.array(repr(kw)), assign=sc.assign, gt_pose=sc.gt_pose, params=np.array(sc.params, np.float64),
-                      loss_args=np.array(LOSS_ARGS), cells=cells, tries=tries, expert=e, pose=pose, loss=loss,
+                      loss_args=np.array(loss_args), cells=cells, tries=tries, expert=e, pose=pose, loss=loss,
                       oracle_scores=np.array(tr.scores), oracle_winner=tr.winner, oracle_rounds=tr.rounds,
                       oracle_inliers=int(tr.inlier_map.sum()) if tr.inlier_map is not None else 0)
         if name in SMALL:

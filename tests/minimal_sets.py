@@ -13,7 +13,8 @@ those rays in the camera frame, then moved to a world frame by a random rigid mo
   flat       the first three points almost collinear: sin^2 of the angle at point 0 just above the 1e-6 latch on det
   spread     depths of one set spread over 1e-3 .. 1e3
   noise      generic sets
-Every try puts its 4th point so that the true pose misses it by e, spread over [0, 1.2 tau), and the first three points
+Every try puts its 4th point so that the true pose misses it by e, spread over [0, 1.2 tau) (tau = TAU unless generate()
+is given another), and the first three points
 off their rays by 0, 0.3 or 2 px (a 3D offset: the pixels are fixed by the cells).  variants() adds, for every try, the
 same set scaled by 2^k (k in +-10, +-20, +-40), by 7000 and 1/7000, and moved by world offsets of 700 m and 1e5 m.
 
@@ -111,10 +112,10 @@ def _world(rng, Pc):
     return ((Pc - t) @ R).astype(np.float32)  # R^T (Pc - t)
 
 
-def _one(rng, family, f):
+def _one(rng, family, f, tau=TAU):
     """One try of `family` (None when this draw has no solution: the caller draws again)."""
     noise = float(rng.choice([0.0, 0.3, 2.0]))
-    e4 = float(rng.uniform(0, 1.2 * TAU))
+    e4 = float(rng.uniform(0, 1.2 * tau))
     cells = _cells(rng)
     par = {"noise_px": noise, "err4_px": e4}
     if family == "parallel":
@@ -172,11 +173,11 @@ def _one(rng, family, f):
     return Try(family, f, cells, _world(rng, P), par)
 
 
-def generate(family: str, n: int, seed: int = 0, f: float = 525.0) -> list:
+def generate(family: str, n: int, seed: int = 0, f: float = 525.0, tau: float = TAU) -> list:
     rng = np.random.default_rng([seed, FAMILIES.index(family), int(f)])
     out = []
     while len(out) < n:
-        t = _one(rng, family, f)
+        t = _one(rng, family, f, tau)
         if t is not None and np.all(np.isfinite(t.obj)):
             out.append(t)
     return out

@@ -49,7 +49,7 @@ def test_forward_and_backward_match_the_compiled_reference(api, path):
     st = api.last_stats()
     assert hy["tries"].tolist() == np.minimum(z["tries"], T).tolist()      # same verdict on every candidate set
     assert hy["cells"].tolist() == cells[:, -1].tolist()                    # the accepted sets
-    assert np.abs(hy["scores"] - z["oracle_scores"]).max() < 1e-4
+    assert np.abs(hy["scores"] - z["oracle_scores"]).max() < 1e-4 * max(1.0, params[6] / 100.0)   # scores scale with alpha
     s = np.sort(z["oracle_scores"])[::-1]
     assert s[0] - s[1] > 1e-3, "fixture has a tie at the top: regenerate with another seed"
     assert e == int(z["expert"]) and st["winner"] == int(z["oracle_winner"])

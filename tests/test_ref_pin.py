@@ -94,6 +94,57 @@ def test_loss_cut_and_weights_equal_the_compiled_reference(gold):
         assert np.abs(g_ref - g_or).max() <= 1e-6 * max(np.abs(g_or).max(), 1e-30)
 
 
+# the fixtures of tests/golden/make_ref_golden.py away from the reference's default hyperparameters: each stores its
+# make_scene arguments, its (shiftX, shiftY, f, ppx, ppy, tau, alpha, beta, maxReproj, sub) and its loss arguments
+PARAM_FIXTURES = ("ref_params_tight_30x40", "ref_params_clamp_30x40", "ref_params_subpx_24x32")
+
+
+def _param_case(name):
+    """(fixture, scene regenerated from its make_scene arguments, parameters, loss arguments)."""
+    import ast
+    from ref_golden_util import params_of
+    z = np.load(GOLD.parents[1] / f"{name}.npz")
+    sc = make_scene(**ast.literal_eval(str(z["scene_kw"])))
+    assert np.array_equal(z["coords"], sc.coords) and np.array_equal(z["assign"], sc.assign)
+    return z, sc, params_of(z), tuple(float(v) for v in z["loss_args"])
+
+
+def test_parameter_fixtures_leave_the_defaults():
+    """tau 2 / beta 2 / alpha 50 with the loss (0.5, 30, 5); tau 40 above maxReproj 30, beta 0.1, alpha 400; tau 0.6 px."""
+    got = {name: (_param_case(name)[2][5:9], _param_case(name)[3]) for name in PARAM_FIXTURES}
+    assert got == {"ref_params_tight_30x40": ((2.0, 50.0, 2.0, 100.0), (0.5, 30.0, 5.0)),
+                   "ref_params_clamp_30x40": ((40.0, 400.0, 0.1, 30.0), (1.0, 100.0, 100.0)),
+                   "ref_params_subpx_24x32": ((0.6, 100.0, 0.5, 100.0), (1.0, 100.0, 100.0))}
+
+
+@pytest.mark.parametrize("name", PARAM_FIXTURES)
+def test_oracle_equals_the_compiled_reference_away_from_the_defaults(name):
+    """What the compiled reference returned is the fixture; the oracle must return it too, on the scene regenerated from the
+    fixture's make_scene arguments."""
+    z, sc, params, loss_args = _param_case(name)
+    mine = np.zeros((4, 4), np.float32)
+    assert O.forward(sc.coords, sc.assign, mine, *params, mt=O.ThreadRandStream(1305)) == int(z["expert"])
+    assert np.abs(z["pose"] - mine).max() <= 1e-6
+    g_or = np.zeros_like(sc.coords)
+    l_or = O.backward(sc.coords, g_or, sc.assign, sc.gt_pose, *loss_args, *params, mt=O.ThreadRandStream(1305))
+    assert abs(float(z["loss"]) - l_or) <= 1e-9 * max(1.0, abs(float(z["loss"])))
+    assert np.abs(z["grads"] - g_or).max() <= 1e-6 * np.abs(g_or).max()
+
+
+@pytest.mark.parametrize("name", PARAM_FIXTURES)
+def test_compiled_reference_away_from_the_defaults_still_gives_the_fixture(ref, name):
+    z, sc, params, loss_args = _param_case(name)
+    co, asg = torch.from_numpy(sc.coords), torch.from_numpy(sc.assign)
+    ref.force_init(1305)
+    pose = torch.zeros(4, 4)
+    assert ref.forward(co, asg, pose, *params) == int(z["expert"])
+    assert np.array_equal(pose.numpy(), z["pose"])
+    ref.force_init(1305)
+    g = torch.zeros(sc.coords.shape)
+    loss = ref.backward(co, g, asg, torch.from_numpy(sc.gt_pose), *loss_args, *params)
+    assert loss == float(z["loss"]) and np.array_equal(g.numpy(), z["grads"])
+
+
 PERSIST_SCENE = dict(E=1, H=24, W=32, M=16, sub=8, seed=11)
 
 

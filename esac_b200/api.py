@@ -259,6 +259,8 @@ def load_library() -> C.CDLL:
     lib.esacb200_test_experts_conv.argtypes = [vp, i32, i32, vp, vp, i64, i64, i32, i32, i32, i32, i32, i32, i32, vp, i64,
                                                i64, i64, i64, vp]
     lib.esacb200_test_experts_conv.restype = i32
+    lib.esacb200_test_gathered.argtypes = [vp, i32, i32, vp, vp, vp, vp, i32, vp, vp, vp, vp]
+    lib.esacb200_test_gathered.restype = i32
     _lib = lib
     return lib
 

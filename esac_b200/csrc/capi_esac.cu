@@ -196,6 +196,8 @@ int esacb200_forward_sharded(esacb200_ctx* ctx, const float* coords, int E, int 
     mark(ctx, EV_END);
     CK(cudaStreamSynchronize(ctx->stream));
     CK(cudaGetLastError());
+    // every rank selects from the same records, so every rank refuses alike (esac.forward refuses M = 0 as well)
+    if (h.fwd.winner < 0.f) return fail(ctx, ESACB200_ERR_ARG, "no shard holds a hypothesis: hypAssignment is empty on every rank");
     if (h.fwd.bad != 0.f) return fail(ctx, ESACB200_ERR_ARG, "a shard's hypAssignment holds an expert index outside its experts");
     if (!is_device_ptr(out_pose)) memcpy(out_pose, h.fwd.pose, sizeof(h.fwd.pose));
     if (out_expert) *out_expert = (int)h.fwd.expert;

@@ -1,5 +1,5 @@
-// The test hooks of include/esac_b200_testhooks.h: single geometry primitives of the kernels, run on the CPU, and one
-// layer of the expert stack's convolution on the device.
+// The test hooks of include/esac_b200_testhooks.h: single geometry primitives of the kernels, run on the CPU, one
+// layer of the expert stack's convolution on the device, and the two kernels that merge the shards of a sharded call.
 #include "../../include/esac_b200_testhooks.h"
 #include "capi_internal.h"
 #include "esac_p3p_fast.cuh"
@@ -218,6 +218,48 @@ int esacb200_test_experts_conv(esacb200_ctx* ctx, int B, int E, const float* his
     CK(cudaGetLastError());
     launch_experts_conv(a, L, k, stride, ctx->stream);
     CK(cudaGetLastError());
+    return ESACB200_OK;
+}
+
+int esacb200_test_gathered(esacb200_ctx* ctx, int world, int M_pad, const double* gathered, float* out_record,
+                           const double* pairs, const double* scores, int M, double* norm_out, double* probs, int* contrib,
+                           int* n_contrib) {
+    if (!ctx) return ESACB200_ERR_ARG;
+    DeviceGuard device_guard(ctx->device);
+    const char* what = "test_gathered";
+    if (!gathered && !pairs) return fail(ctx, ESACB200_ERR_ARG, "%s: neither gathered nor pairs: nothing to run", what);
+    if (world < 1) return fail(ctx, ESACB200_ERR_ARG, "%s: world=%d: need at least one rank", what, world);
+    if (gathered) {
+        if (M_pad < 1 || (long long)world * M_pad > 0x7fffffffll)
+            return fail(ctx, ESACB200_ERR_ARG, "%s: M_pad=%d world=%d: need M_pad >= 1 and world * M_pad < 2^31", what, M_pad, world);
+        const void* ptrs[] = {gathered, out_record};
+        const char* names[] = {"gathered", "out_record"};
+        const int rc = device_args(ctx, what, 2, ptrs, names);
+        if (rc) return rc;
+        if ((uintptr_t)gathered % 8 || (uintptr_t)out_record % 4)
+            return fail(ctx, ESACB200_ERR_ARG, "%s: gathered must be 8-byte and out_record 4-byte aligned", what);
+    }
+    if (pairs) {
+        if (M < 0) return fail(ctx, ESACB200_ERR_ARG, "%s: M=%d: need M >= 0", what, M);
+        const void* ptrs[] = {pairs, norm_out, n_contrib, scores, probs, contrib};
+        const char* names[] = {"pairs", "norm_out", "n_contrib", "scores", "probs", "contrib"};
+        const int rc = device_args(ctx, what, M > 0 ? 6 : 3, ptrs, names);
+        if (rc) return rc;
+        if ((uintptr_t)pairs % 8 || (uintptr_t)norm_out % 8 || (uintptr_t)n_contrib % 4 || (uintptr_t)scores % 8 ||
+            (uintptr_t)probs % 8 || (uintptr_t)contrib % 4)
+            return fail(ctx, ESACB200_ERR_ARG, "%s: the double arrays must be 8-byte and the int arrays 4-byte aligned", what);
+    }
+    if (gathered) {
+        launch_select_gathered(gathered, world, M_pad, (ForwardRecord*)out_record, ctx->stream);
+        CK(cudaGetLastError());
+    }
+    if (pairs) {
+        Problem P{};
+        P.M = M;
+        launch_rescale_probs_gathered(scores, P, pairs, world, norm_out, probs, contrib, n_contrib, kProbThresh, ctx->stream);
+        CK(cudaGetLastError());
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
     return ESACB200_OK;
 }
 

@@ -774,7 +774,7 @@ void launch_pack_forward(const double* scores, const ForwardRecord* fwd, int M, 
 // softMax + draw(training = false) over the gathered records of all shards (esac_util.h:461-530): the first strict maximum in
 // the hypothesis order of the UNSHARDED problem (global index = the record's hyp_offset + k * hyp_stride).  One block.
 // out: the camera pose of the global winner, its expert, 1 if any shard flagged a bad assignment, its global hypothesis index
-// and its owning rank.
+// and its owning rank; winner and rank -1 (and a pose of -1s) when no shard holds a hypothesis.
 __global__ void __launch_bounds__(256) select_gathered_kernel(const double* __restrict__ g, int world, int M_pad, ForwardRecord* out) {
     __shared__ double sbest[8];
     __shared__ long long sidx[8];
@@ -814,7 +814,14 @@ __global__ void __launch_bounds__(256) select_gathered_kernel(const double* __re
         int r = srank[0];
         for (int w = 1; w < 8; ++w)
             if (sbest[w] > b || (sbest[w] == b && sidx[w] < i)) { b = sbest[w]; i = sidx[w]; r = srank[w]; }
-        if (i == 0x7fffffffffffffffll) { i = 0; r = 0; }
+        if (i == 0x7fffffffffffffffll) {  // no shard holds a hypothesis: nothing to select (the host refuses the call)
+            for (int k = 0; k < 16; ++k) out->pose[k] = -1.f;
+            out->expert = -1.f;
+            out->bad = (float)sbad;
+            out->winner = -1.f;
+            out->rank = -1.f;
+            return;
+        }
         const ShardTail& t = *(const ShardTail*)(g + (size_t)r * rec + M_pad);
         for (int k = 0; k < 16; ++k) out->pose[k] = (float)t.pose[k];
         out->expert = (float)t.expert;

@@ -163,6 +163,15 @@ def backward_sharded(coords_local, grads_local, assign_local, gt_pose, w_rot, w_
                                 hyp_offset=hyp_offset)
 
 
+def _check_selected(expert: int, M: int):
+    """The refusals of esacb200_forward_sharded: no shard holds a hypothesis (M of the selected record is 0), or the
+    winner's shard flagged an expert index outside its experts (expert -1)."""
+    if M == 0:
+        raise RuntimeError("no shard holds a hypothesis: hypAssignment is empty on every rank")
+    if expert < 0:
+        raise RuntimeError("hypAssignment holds an expert index outside the shard's experts")
+
+
 def forward_sharded(coords_local, assign_local, out_pose, params, expert_offset: int, group=None, local_forward=None,
                     hyp_offset: int = 0, M_pad: int | None = None, device: int | None = None, hyp_stride: int = 1):
     """esac.forward over experts sharded across the ranks of `group`.  coords_local [E_local,3,H,W] and
@@ -222,20 +231,21 @@ def forward_sharded(coords_local, assign_local, out_pose, params, expert_offset:
         # selection on the device: first maximum = draw(training=false) -- in rank-major order, which is the order of the
         # unsharded problem for contiguous shards (this fallback transport does not support hyp_stride > 1 tie-breaking);
         # ONE read-back of the winner's pose and expert (the only host sync of the step)
+        # (the winner's record holds no hypothesis only when no record does: every real slot beats the -inf padding)
         w = torch.argmax(g[:, :M_pad].reshape(-1))
-        tail = g.reshape(-1)[(w // M_pad) * rec + M_pad + torch.arange(api.TAIL_WINNER, device=g.device)]
+        tail = g.reshape(-1)[(w // M_pad) * rec + M_pad + torch.arange(api.TAIL_M + 1, device=g.device)]
         if hasattr(out_pose, "is_cuda") and out_pose.is_cuda:
             out_pose.copy_(tail[api.TAIL_POSE:api.TAIL_EXPERT].reshape(4, 4))
-            expert = int(tail[api.TAIL_EXPERT].item())
-            if expert < 0:
-                raise RuntimeError("hypAssignment holds an expert index outside the shard's experts")
+            expert, m = (int(v) for v in tail[[api.TAIL_EXPERT, api.TAIL_M]].tolist())
+            _check_selected(expert, m)
             return expert
         small = tail.cpu().numpy()
         gpose, expert = small[api.TAIL_POSE:api.TAIL_EXPERT].reshape(4, 4).astype(np.float32), int(small[api.TAIL_EXPERT])
-        if expert < 0:
-            raise RuntimeError("hypAssignment holds an expert index outside the shard's experts")
+        _check_selected(expert, int(small[api.TAIL_M]))
     else:
-        _, _, gpose, expert, _ = select_global(g.numpy(), M_pad)
+        gn = g.numpy()
+        _, _, gpose, expert, _ = select_global(gn, M_pad)
+        _check_selected(expert, int(gn[:, M_pad + api.TAIL_M].max()))
     if hasattr(out_pose, "copy_"):
         out_pose.copy_(torch.from_numpy(gpose))
     else:

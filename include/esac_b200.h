@@ -196,7 +196,8 @@ int esacb200_comm_init(esacb200_ctx* ctx, int world, int rank, const void* id128
 int esacb200_comm_destroy(esacb200_ctx* ctx);
 /* esac_forward over all shards: local pipeline -> record -> one ncclAllGather -> softMax / draw over the records on the device
  * (first strict maximum in rank-major order) -> one 80-byte read-back.  Every rank receives the global winner's camera pose
- * and (global) expert index.  coords / assign host or device pointers; M may be 0; M_pad = max M over the ranks. */
+ * and (global) expert index.  coords / assign host or device pointers; M may be 0, but not on every rank (esac.forward refuses
+ * M = 0 too: every rank then fails with ESACB200_ERR_ARG); M_pad = max M over the ranks. */
 int esacb200_forward_sharded(esacb200_ctx* ctx, const float* coords, int E, int H, int W, const int64_t* assign,
                              int64_t assign_stride, int M, int M_pad, float* out_pose, int shiftX, int shiftY, float focalLength,
                              float ppointX, float ppointY, float inlierThreshold, float inlierAlpha, float inlierBeta,

@@ -4,7 +4,7 @@
  * functions the CUDA kernels call -- on the CPU, so the `-m "not gpu"` tests can check them against OpenCV without a
  * GPU.  They are NOT a CPU fallback: no forward/backward pipeline exists on the host.  esacb200_test_experts_conv runs
  * one layer of the expert stack's device kernels on caller-owned device buffers, so a test can hold that layer alone
- * to a reference.
+ * to a reference; esacb200_test_gathered does the same for the two kernels that merge the shards of a sharded call.
  */
 #ifndef ESAC_B200_TESTHOOKS_H
 #define ESAC_B200_TESTHOOKS_H
@@ -75,6 +75,20 @@ struct esacb200_ctx;
 int esacb200_test_experts_conv(struct esacb200_ctx* ctx, int B, int E, const float* hist, const float* packed, int64_t w_off,
                                int64_t b_off, int k, int stride, int cin, int cout, int hin, int win, int relu, float* pairs,
                                int64_t pair_floats, int64_t in_off, int64_t out_off, int64_t res_off, int* hdr);
+/* The two kernels that merge the shards of a sharded call, on caller-owned device buffers, on the context's stream; the hook
+ * synchronises that stream before it returns.  At least one of gathered and pairs is non-NULL.
+ * gathered != NULL: select_gathered_kernel (esacb200_forward_sharded's selection) over `world` records of M_pad + 21 doubles
+ * laid out as esacb200_forward_pack writes them; out_record receives 20 floats: the winner's pose [16], its expert, the
+ * bad-assignment flag, the global index of the winner and its rank (winner and rank -1 when no record holds a hypothesis).
+ * pairs != NULL: rescale_probs_gathered_kernel (the NCCL backward's probabilities) over `world` (max, sum exp) pairs [world][2]
+ * and one shard's M scores: norm_out[2] = (global max, global sum exp), probs[M], and contrib[M] the ascending local indices
+ * whose probability is not below ESACB200_PROB_THRESH, *n_contrib of them.  scores, probs and contrib may be NULL when M = 0.
+ * The kernels' contract: world >= 1; M_pad >= 1 with world * M_pad < 2^31; M >= 0; doubles 8-byte and ints 4-byte aligned;
+ * in every record 0 <= M <= M_pad and hyp_stride >= 1.  Arguments outside it are refused with ESACB200_ERR_ARG (the records'
+ * contents are the caller's to keep). */
+int esacb200_test_gathered(struct esacb200_ctx* ctx, int world, int M_pad, const double* gathered, float* out_record,
+                           const double* pairs, const double* scores, int M, double* norm_out, double* probs, int* contrib,
+                           int* n_contrib);
 
 #ifdef __cplusplus
 }

@@ -149,3 +149,18 @@ def test_select_global_breaks_ties_in_the_unsharded_order_with_strided_shards():
         g[r, M_pad + 18:M_pad + 21] = [3, r, 2]
     w, rank, pose, expert, _ = sharded.select_global(g, M_pad)
     assert (w, rank, expert) == (M_pad + 1, 1, 1) and pose[0, 0] == 2.0
+
+
+def test_forward_sharded_refuses_a_call_in_which_no_shard_holds_a_hypothesis(tmp_path):
+    """esac.forward refuses M = 0, and so does the sharded forward when every rank's hypAssignment is empty: the torch route
+    with the library's message (one-rank gloo group in this process)."""
+    def never(coords, assign, params):
+        raise AssertionError("a shard without hypotheses runs no local pipeline")
+
+    dist.init_process_group("gloo", store=dist.FileStore(str(tmp_path / "store"), 1), rank=0, world_size=1)
+    try:
+        with pytest.raises(RuntimeError, match="no shard holds a hypothesis"):
+            sharded.forward_sharded(torch.zeros(1, 3, 2, 2), torch.zeros(0, dtype=torch.int64), torch.zeros(4, 4), (),
+                                    expert_offset=0, local_forward=never, M_pad=4)
+    finally:
+        dist.destroy_process_group()
